@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- headline benchmark of the B200 Hades engine (driver contract).
+"""bench.py -- headline benchmark of the H100 Hades engine (driver contract).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload W]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload W] [--dump-outputs DIR]
 
 Workload (default `merkle4`, BASELINE.json configs[1]): one step = one batch of 2^20 independent
 `Hash::digest(Domain::Merkle4, 4 scalars)` per GPU = 2^20 width-5 Hades permutations per GPU, on
@@ -19,11 +19,15 @@ all-gather per level -- the only path north_star shards with a collective -- wit
 time (full build vs a compute-only build with the gathers skipped), per-level kernel / all-gather device times,
 and an in-run parity verdict against the CPU oracle (outside every timed region).
 
-Other workloads (not the driver's headline; used for profiles/ and DESIGN.md numbers):
+Other workloads (not the driver's headline):
   --workload encrypt|decrypt   2^20 x encrypt/decrypt(L=2)  (configs[2])      --workload permute  raw 2^20 x 5 states
   --workload sweep     Domain::Other, EVERY in_len 1..256 at 2^18 items (configs[4]); per-length table in `sweep`
                        (--sweep-lens 1,2,4 to subsample)
   --workload tree      the tree build alone (--log4-leaves k)                  --workload convert  wire-format kernel
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed (rank 0) as DIR/<name>.npy: every
+255-bit scalar as its sixteen 16-bit words (little-endian, exact in float32), a fixed seeded sample of rows where the
+whole output would exceed 64 MB.  Inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -40,8 +44,8 @@ METRIC = "hades_permutations_per_sec"
 UNIT = "perm/s"
 LOG2_BATCH = 20
 BYTES_PER_PERM = 160          # Merkle4 digest: 4 x 32 B in + 32 B out (SURVEY.md 8d)
-SM_COUNT = 148
 TREE_LOG4 = {1: 11, 2: 12, 4: 13, 8: 14}
+DUMP_BYTES = 60_000_000       # --dump-outputs budget, sample indices included (+ .npy headers: below 64 MB)
 
 
 def env_int(name, default):
@@ -52,10 +56,10 @@ def env_int(name, default):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons streamed (-lms) DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons streamed (-lms) DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-         "clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.index, self.proc = index, None
@@ -81,7 +85,7 @@ class ClockSampler:
                 out = ""
             for ln in out.splitlines():
                 parts = [p.strip() for p in ln.split(",")]
-                if len(parts) >= 7:
+                if len(parts) >= 8:
                     try:
                         float(parts[0])
                         rows.append(parts)
@@ -92,8 +96,13 @@ class ClockSampler:
         sm = [float(r[0]) for r in rows]
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         reasons = [n for k, n in enumerate(names) if any(r[3 + k].lower().startswith("active") for r in rows)]
+        try:
+            limit = float(rows[0][7])
+        except ValueError:
+            limit = None
         return {"sm_mhz": statistics.median(sm), "sm_min_mhz": min(sm), "sm_max_mhz": float(rows[0][1]),
-                "reasons": reasons, "power_w_max": max(float(r[2]) for r in rows), "samples": len(rows)}
+                "reasons": reasons, "power_w_max": max(float(r[2]) for r in rows), "power_limit_w": limit,
+                "samples": len(rows)}
 
 
 def usable_cores():
@@ -114,20 +123,29 @@ def measured_peaks():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s)"
 
 
-def ncu_traffic():
-    """dram bytes per launch of the dominant kernel from the committed `ncu --set full` capture (newest round)."""
-    for name in ("r2_ncu_summary.json", "r1_ncu_summary.json"):
-        try:
-            with open(os.path.join(ROOT, "profiles", name)) as f:
-                v = json.load(f).get("merkle4_2p20", {}).get("dram_bytes_per_launch")
-            if v:
-                return v
-        except Exception:
-            pass
-    return None
+def dump_outputs(path, arrays, seed=0):
+    """arrays: name -> CUDA tensor, one row per item: int64 BlsScalar limbs (written as their 16-bit words) or uint8
+    flags, as float32.  Rows are sampled (fixed seed, sorted; indices in <name>_rows.npy) where the whole set would
+    exceed DUMP_BYTES."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    per_array = DUMP_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        words_per_elem = 4 if t.dtype == torch.int64 else 1
+        row_bytes = t[0].numel() * words_per_elem * 4
+        if t.shape[0] * row_bytes > per_array:
+            keep = per_array // (row_bytes + 8)            # + the row's float64 index
+            rows = np.sort(np.random.default_rng(seed).choice(t.shape[0], keep, replace=False))
+            t = t[torch.from_numpy(rows).to(t.device)]
+            np.save(os.path.join(path, name + "_rows.npy"), rows.astype(np.float64))
+        a = t.contiguous().cpu().numpy()
+        if words_per_elem == 4:
+            a = a.view(np.uint16)
+        np.save(os.path.join(path, name + ".npy"), a.reshape(t.shape[0], -1).astype(np.float32))
 
 
 def workload_config(log2_batch, world):
@@ -342,7 +360,9 @@ def tree_block(eng, torch, dist, rank, world, stream, k, builds=3, paths=64):
             row.update(gather_ms=round(t["gather_ms"], 4), gather_MiB=t["gather_bytes"] >> 20,
                        gather_GBps=round(t["gather_bytes"] * (world - 1) / world / (t["gather_ms"] * 1e-3) / 1e9, 1) if t["gather_ms"] > 0 else None)
         per_level.append(row)
-    small_levels = [r for r in per_level if r["nodes"] < 740 * 128]
+    info = eng.kernel_info()
+    wave = torch.cuda.get_device_properties(stream.device).multi_processor_count * info["min_blocks_per_sm"] * info["threads_per_block"]
+    small_levels = [r for r in per_level if r["nodes"] < wave]
     exposed = max(0.0, ms_full - ms_compute)
     worst = max((r for r in per_level if "gather_ms" in r), key=lambda r: r["gather_ms"], default=None)
     limiting = ("levels with < 1 wave of blocks are latency-bound: %d levels, %.2f ms of kernels" %
@@ -357,7 +377,7 @@ def tree_block(eng, torch, dist, rank, world, stream, k, builds=3, paths=64):
             "compute_only_ms": ms_compute, "exposed_allgather_ms": exposed,
             "gathered_MiB_per_rank": sum(t["gather_bytes"] for t in levels) >> 20,
             "timed_build_ms_rank0": total_timed, "per_level_rank0": per_level, "limiting": limiting,
-            "parity": "ok" if all_ok else "MISMATCH", "parity_checks": parity}
+            "parity": "ok" if all_ok else "MISMATCH", "parity_checks": parity, "nodes": nodes}
 
 
 # ---------------------------------------------------------------------------------------------------------
@@ -375,9 +395,12 @@ def main():
     ap.add_argument("--sweep-lens", default="", help="sweep: comma-separated input lengths (default: every length 1..256)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-tree", action="store_true", help="merkle4: skip the tree block")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs as DIR/*.npy")
     args = ap.parse_args()
     if args.steps is None:
         args.steps = 2 if args.workload == "sweep" else 40
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank, world, local = env_int("RANK", 0), env_int("WORLD_SIZE", 1), env_int("LOCAL_RANK", 0)
 
@@ -446,18 +469,20 @@ def main():
     per_launch_events = False
     # ---- workload set-up: step(i) enqueues one batch on `stream`; returns perms per step ----------------
     if args.workload == "merkle4":
-        nbuf = 4                                          # rotate over 4 x 128 MiB inputs (> 126 MB L2)
+        nbuf = 4                                          # rotate over 4 x 128 MiB inputs (> 50 MB L2)
         with torch.cuda.stream(stream):
             ins = [torch.from_numpy(random_limbs_fast(rng, (n, 4)).view(np.int64)).cuda() for _ in range(nbuf)]
             out = torch.empty((n, 1, 4), dtype=torch.int64, device="cuda")
         perms_per_step, bytes_per_step = n, n * BYTES_PER_PERM
         step = lambda i: pb.Hash.digest_batch(pb.Domain.Merkle4, ins[i % nbuf], engine=eng, out=out, async_=True)
+        outputs = lambda: {"digests": out}
         config = workload_config(args.log2_batch, world)
     elif args.workload == "permute":
         with torch.cuda.stream(stream):
             st = torch.from_numpy(random_limbs_fast(rng, (n, 5)).view(np.int64)).cuda()
         perms_per_step, bytes_per_step = n, n * 320
         step = lambda i: eng.permute_batch_inplace(st, async_=True)
+        outputs = lambda: {"states": st}
         workload, l2_note = "raw permute_batch of 2^%d x 5 states in place" % args.log2_batch, "160 MiB state array > L2"
     elif args.workload == "encrypt":
         with torch.cuda.stream(stream):
@@ -467,6 +492,7 @@ def main():
             cip = torch.empty((n, 3, 4), dtype=torch.int64, device="cuda")
         perms_per_step, bytes_per_step = 2 * n, n * 256
         step = lambda i: pb.encrypt_batch(msg, sec, non, engine=eng, out=cip, async_=True)
+        outputs = lambda: {"cipher": cip}
         workload, l2_note = "encrypt_batch 2^%d messages, L=2 (benches/encrypt.rs:17)" % args.log2_batch, "256 MiB touched per step > L2"
     elif args.workload == "decrypt":
         with torch.cuda.stream(stream):
@@ -480,6 +506,7 @@ def main():
 
         def step(i):
             ok_holder["m"], ok_holder["ok"] = pb.decrypt_batch(cip, sec, non, engine=eng, async_=True)
+        outputs = lambda: {"message": ok_holder["m"], "ok": ok_holder["ok"]}
         workload, l2_note = "decrypt_batch 2^%d ciphers, L=2 (benches/decrypt.rs:17)" % args.log2_batch, "257 MiB touched per step > L2"
     elif args.workload == "sweep":
         n = 1 << 18
@@ -492,6 +519,7 @@ def main():
         perms_per_step = sum(n * ((L + 3) // 4) for L in lens)
         bytes_per_step = sum(n * (32 * L + 32) for L in lens)
         sweep_events = []
+        outputs = lambda: {"digests_in_len_%d" % lens[-1]: out}        # `out` holds the last length of the step
 
         def step(i):
             evs = [torch.cuda.Event(enable_timing=True)]
@@ -513,10 +541,14 @@ def main():
         perms_per_step, bytes_per_step = n, n * 64       # "perms" here = scalars converted (no permutation)
         lib, ctx = eng._lib, eng._ctx
         step = lambda i: eng._check(lib.p252_scalars_to_bytes(ctx, sc.data_ptr(), n, ob.data_ptr(), 3))
+        outputs = lambda: {"bytes": ob}
         workload, l2_note = "to_bytes of 2^25 scalars (wire-format kernel, the one HBM-bound kernel); value = scalars/s", "1 GiB in + 1 GiB out per step"
     else:  # tree alone
         k = args.log4_leaves or TREE_LOG4.get(world, 12)
-        blk = tree_block(eng, torch, dist, rank, world, stream, k, builds=max(3, min(args.steps, 10)))
+        blk = tree_block(eng, torch, dist, rank, world, stream, k, builds=args.steps)
+        nodes = blk.pop("nodes")
+        if rank == 0 and args.dump_outputs:
+            dump_outputs(args.dump_outputs, {"tree_nodes": nodes})
         if rank == 0:
             clocks = {"sm_mhz": None, "sm_max_mhz": None, "reasons": [], "samples": 0}
             line = {"metric": METRIC, "value": blk["value"], "unit": UNIT, "n_gpus": world, "steps": blk["builds_timed"],
@@ -552,6 +584,8 @@ def main():
     barrier()
     clocks = sampler.stop()
     launches = eng.launch_count - launches0
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, outputs())
     total_ms = ev[0].elapsed_time(ev[-1])
     per_step_ms = [ev[i].elapsed_time(ev[i + 1]) for i in range(args.steps)]
     if dist is not None:
@@ -605,6 +639,7 @@ def main():
             del ins
             torch.cuda.empty_cache()
             tree = tree_block(eng, torch, dist, rank, world, stream, args.log4_leaves or TREE_LOG4.get(world, 12))
+            tree.pop("nodes")
         except Exception as exc:  # never hide the headline because of the additional block
             tree = {"error": repr(exc)}
 
@@ -617,20 +652,21 @@ def main():
     launch_ms = statistics.mean(per_step_ms) / launches_per_step
     achieved = bytes_per_step / launches_per_step / (launch_ms * 1e-3) / 1e9
     info = eng.kernel_info()
-    sm_mhz = clocks.get("sm_mhz") or 1965.0
+    props = torch.cuda.get_device_properties(local)
+    sm_mhz = clocks.get("sm_mhz") or props.clock_rate / 1e3
     # Integer-multiplier roofline, computed from THIS run: the multiplier instructions one permutation issues (counted
     # by the PTX generator, exported by the library) x the measured permutation rate, against one IMAD.WIDE per 4
-    # cycles per SM sub-partition (measured: tools/microbench/pipe_table.cu) at the SM clock sampled during the run.
+    # cycles per SM sub-partition (tools/microbench/pipe_table.cu measures it) at the SM clock sampled during the run.
     wide_rate = info["wide_mul_per_permutation"] * (value / world) / 32.0          # warp instructions / s / GPU
-    wide_peak = SM_COUNT * 4 * sm_mhz * 1e6 / 4.0
+    wide_peak = props.multi_processor_count * 4 * sm_mhz * 1e6 / 4.0
     imad = {"bound": "imad", "achieved": wide_rate / 1e9, "peak": wide_peak / 1e9, "unit": "G warp-IMAD.WIDE/s",
             "frac": wide_rate / wide_peak, "wide_mul_per_permutation": info["wide_mul_per_permutation"],
             "dfma_per_permutation": info["dfma_per_permutation"], "sm_mhz": sm_mhz,
-            "peak_source": "148 SMs x 4 sub-partitions x SM clock / 4 cycles per IMAD.WIDE (B200 measurement, "
-                           "profiles/r2_pipe_table.log); clock = median nvidia-smi sample of this run",
+            "peak_source": "%d SMs x 4 sub-partitions x SM clock / 4 cycles per IMAD.WIDE (issue interval assumed; tools/microbench/pipe_table.cu measures it); "
+                           "clock = median nvidia-smi sample of this run, else the device's maximum" % props.multi_processor_count,
             "note": "achieved = multiplier instructions per permutation (library: p252_get_kernel_info) x measured perm/s / 32"}
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": ncu_traffic(), "peak_source": peak_src,
+                "peak_source": peak_src,
                 "kernel": "k_sponge_digest" if args.workload in ("merkle4", "sweep") else
                           ("k_crypt<false>" if args.workload == "encrypt" else "k_crypt<true>" if args.workload == "decrypt" else
                            ("k_convert<false>" if args.workload == "convert" else "k_permute<false>")),
@@ -641,7 +677,8 @@ def main():
     line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": total_ms / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "u32 limbs (255-bit modular integer, IMAD.WIDE carry chains)", "data": "synthetic",
-            "config": config, "clocks": clocks, "gpu_launches": launches, "roofline": roofline, "target_perm_per_s_1gpu": 1e8}
+            "config": config, "clocks": clocks, "gpu_launches": launches, "roofline": roofline, "target_perm_per_s_1gpu": 1e8,
+            "device": props.name}
     line.update(extra)
     if e2e is not None:
         line["e2e"] = e2e

@@ -1,5 +1,5 @@
 //! SOURCE ONLY -- never compiled in this repository's image (no cargo/rustc).  Batch entry points for
-//! `dusk_poseidon` over the B200 engine: `Hash::digest_batch`, `hades::permute_batch`,
+//! `dusk_poseidon` over the H100 engine: `Hash::digest_batch`, `hades::permute_batch`,
 //! `encrypt_batch`, `decrypt_batch`, `merkle4_build`, Merkle openings, bound to include/poseidon252_b200.h.
 //! The `extern "C"` block below is checked mechanically against the header by tests/test_abi.py
 //! (same symbol set, same parameter counts) and its exact call set is exercised by tests/c/abi_smoke.c.

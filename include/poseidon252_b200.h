@@ -1,6 +1,6 @@
-/* poseidon252_b200 -- C ABI of the B200-native batched Poseidon/Hades engine.
+/* poseidon252_b200 -- C ABI of the H100-native batched Poseidon/Hades engine.
  *
- * Drop-in boundary for the hot path of dusk-poseidon (reference = /root/reference, a pure-Rust,
+ * Drop-in boundary for the hot path of dusk-poseidon (reference = dusk-network/Poseidon252, a pure-Rust,
  * one-state-at-a-time CPU crate with no FFI of its own).  The reference's seam for this path is
  * the trait pair dusk_safe::Safe<BlsScalar,5> (impl: src/hades/permutation/scalar.rs:24-36) +
  * Hades<BlsScalar> (src/hades/permutation.rs:34-124) under the public surface src/lib.rs:13-31.
@@ -19,7 +19,7 @@
  *     P252_ASYNC to return right after enqueueing on the context's stream).
  *   - Every function returns a p252_status; nothing unwinds across the boundary.  Positive codes
  *     mirror dusk_poseidon::Error (src/error.rs:11-32); negative codes are engine failures.
- *   - There is NO CPU fallback: without a usable sm_100 device p252_create fails.
+ *   - There is NO CPU fallback: without a usable sm_90 (H100) device p252_create fails.
  *   - A context is bound to one device and one stream; calls on one context serialise (a mutex
  *     inside the context: concurrent callers block, they do not race); separate contexts are
  *     independent (the reference is stateless: ScalarPermutation is a ZST,
@@ -85,7 +85,7 @@ const char* p252_strerror(int status);
 int p252_device_count(int* count);
 
 /* Create a context on CUDA device `device` with its own stream.  Fails with P252_ERR_NO_DEVICE
- * when there is no sm_100 GPU (no CPU fallback). */
+ * when there is no sm_90 (H100) GPU (no CPU fallback). */
 int p252_create(int device, p252_ctx** out);
 /* Same, but enqueue all work on an existing CUDA stream (cudaStream_t passed as void*), e.g. the
  * caller's torch stream, so that the caller's CUDA events bracket the kernels. */
@@ -113,8 +113,8 @@ typedef struct p252_kernel_info {
 int p252_get_kernel_info(p252_kernel_info* out);
 
 /* Digest and raw-permutation batches of at most `max_items` items run the lane-split kernels (five threads per sponge state: lower latency,
- * ~3x lower throughput per state) -- the regime of single digests and of the top levels of a Merkle tree.  Default
- * 3552 = one lane-split warp per SM sub-partition, the measured crossover (environment variable P252_COOP_MAX
+ * ~3x lower throughput per state) -- the regime of single digests and of the top levels of a Merkle tree.  Default:
+ * one lane-split warp (6 items) per SM sub-partition, 3168 on a 132-SM H100 (environment variable P252_COOP_MAX
  * overrides it at context creation); 0 disables the lane-split path.  Both
  * kernels produce bit-identical results. */
 int p252_set_small_batch_max(p252_ctx* ctx, size_t max_items);

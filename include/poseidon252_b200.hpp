@@ -1,5 +1,5 @@
 // poseidon252_b200.hpp -- header-only C++17 host mirror of the dusk_poseidon public surface
-// (/root/reference/src/lib.rs:13-31) above the C ABI of poseidon252_b200.h.  The reference is compiled
+// (src/lib.rs:13-31) above the C ABI of poseidon252_b200.h.  The reference is compiled
 // (Rust) code and no Rust toolchain exists in this image, so the compiled host side is C++; the Rust
 // binding a maintainer would add is shown in INTEGRATION.md / bindings/rust/.
 //
@@ -10,7 +10,7 @@
 //   NEW batch entries: Hash::digest_batch, hades::permute_batch, encrypt_batch, decrypt_batch,
 //   merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
-// single-item calls).  No CPU fallback: Engine's constructor throws without an sm_100 device.
+// single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
 #include <cstdint>
 #include <stdexcept>

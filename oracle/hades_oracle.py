@@ -4,7 +4,7 @@ dusk-poseidon hot path: Hades permutation + SAFE sponge + Hash / encrypt / decry
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline leg may import this module.
 The product path (poseidon252_b200/) never imports it and has no CPU fallback.
 
-Every function cites the reference file:line (relative to /root/reference) it restates.
+Every function cites the reference file:line (relative to the reference repository's root) it restates.
 All values here are *canonical* integers in [0, p); the reference's in-memory form
 (`BlsScalar.0`, 4 x u64 little-endian limbs, Montgomery form x*R mod p) is produced by
 `to_mont_limbs` / consumed by `from_mont_limbs`.
@@ -15,7 +15,7 @@ PINNING STATUS
     (tests/test_oracle.py reproduces all of them with this file).
   * parity unpinned: `hash_to_scalar` (dusk-bls12_381 0.14, BLAKE2b-512 -> from_bytes_wide) and
     the tag-input byte encoding + encrypt/decrypt internals of dusk-safe 0.3. Neither crate is
-    vendored under /root/reference and no reference test fixes their absolute output; they are
+    vendored in the reference and no reference test fixes their absolute output; they are
     restated from the crates' published algorithm (SAFE paper, eprint 2023/522 sec. 2.3) and
     anchored on the reference's call sites and property tests (README doctest,
     tests/encryption.rs). The device never computes a tag: it is a per-batch input.

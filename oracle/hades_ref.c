@@ -11,11 +11,11 @@
  * load this library.  The product (poseidon252_b200/) never links or calls it.
  *
  * Pinned by: tests/test_oracle.py checks this file against hades_oracle.py, which reproduces the
- * 6 known-answer vectors of /root/reference/src/hades.rs:134-162.
+ * 6 known-answer vectors of src/hades.rs:134-162.
  * Parity unpinned: tag derivation (not done here: the tag is an input scalar) -- see
  * hades_oracle.py header.
  *
- * Reference lines restated (relative to /root/reference):
+ * Reference lines restated (relative to the reference repository's root):
  *   src/hades/permutation.rs:63-72,83-92,105-123   round schedule
  *   src/hades/permutation/scalar.rs:39-64          add_round_constants, quintic_s_box, mul_matrix
  *   src/hades/round_constants.rs:40-47, src/hades/mds_matrix.rs:25-32   from_raw of file limbs

@@ -1,6 +1,6 @@
-"""poseidon252_b200 -- B200-native batched Poseidon/Hades engine with the dusk_poseidon API.
+"""poseidon252_b200 -- H100-native batched Poseidon/Hades engine with the dusk_poseidon API.
 
-Public surface mirrors /root/reference/src/lib.rs:13-31:
+Public surface mirrors src/lib.rs:13-31:
     Hash, Domain, Error, HADES_WIDTH, encrypt, decrypt
 plus the batch entry points this engine adds:
     Hash.digest_batch, hades.permute_batch, encrypt_batch, decrypt_batch, merkle4_build.

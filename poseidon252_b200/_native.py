@@ -88,7 +88,7 @@ def lib():
     if _LIB is None:
         if not os.path.exists(LIB_PATH):
             raise ImportError(
-                "poseidon252_b200: %s is missing. Build the sm_100a library first "
+                "poseidon252_b200: %s is missing. Build the sm_90a library first "
                 "(`python -m poseidon252_b200.build` or __graft_entry__.build()). "
                 "There is no CPU fallback for the batch path." % LIB_PATH)
         handle = ctypes.CDLL(LIB_PATH)

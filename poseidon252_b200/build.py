@@ -1,10 +1,10 @@
-"""In-tree build of libposeidon252_b200.so (hand-written sm_100a CUDA + the C ABI).
+"""In-tree build of libposeidon252_b200.so (hand-written sm_90a CUDA + the C ABI).
 
     python -m poseidon252_b200.build            # regenerate tables/PTX header and compile
     python -m poseidon252_b200.build --check    # exit 0 iff the library is up to date
 
-nvcc cross-compiles for sm_100a without a GPU; the .so is built in-tree
-(poseidon252_b200/lib/) so it travels with the repository snapshot to the GPU box.
+nvcc cross-compiles for sm_90a (H100) without a GPU; the .so is built in-tree
+(poseidon252_b200/lib/), so the package imports straight from the repository tree.
 """
 import os
 import subprocess
@@ -19,7 +19,7 @@ DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("hades_device.cuh", "fr_ptx.cu
                                                  "host_field.h")] + [os.path.join(ROOT, "include", "poseidon252_b200.h")]
 GENERATORS = [os.path.join(ROOT, "tools", f) for f in ("gen_tables.py", "gen_field_ptx.py", "hades_model.py")]
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "-Xptxas", "-v"]
 
 

@@ -2,7 +2,7 @@
 // (io-pattern checks, tag derivation), staging for HOST buffers, kernel launches, and the
 // multi-GPU arity-4 tree build (one process per GPU, NCCL all-gather per level).
 //
-// Mirrors, for the batch path, the reference's public surface (/root/reference/src/lib.rs:13-31):
+// Mirrors, for the batch path, the reference's public surface (src/lib.rs:13-31):
 //   Hash / Domain / io_pattern      src/hash.rs:21-155      -> p252_hash_tag, p252_hash_batch
 //   encrypt / decrypt               src/encryption.rs:62-95 -> p252_encrypt_batch, p252_decrypt_batch
 //   Error                           src/error.rs:11-44      -> p252_status
@@ -296,7 +296,7 @@ const uint64_t* limbs(const p252_fr* f) { return f->l; }
 
 extern "C" {
 
-const char* p252_version(void) { return "poseidon252_b200 0.1.0 (sm_100a)"; }
+const char* p252_version(void) { return "poseidon252_b200 0.1.0 (sm_90a)"; }
 
 const char* p252_strerror(int status) {
     switch (status) {
@@ -310,7 +310,7 @@ const char* p252_strerror(int status) {
         case P252_ERR_INVALID_ARGUMENT: return "invalid argument";
         case P252_ERR_CUDA: return "CUDA error";
         case P252_ERR_NCCL: return "NCCL error";
-        case P252_ERR_NO_DEVICE: return "no usable sm_100 CUDA device (there is no CPU fallback)";
+        case P252_ERR_NO_DEVICE: return "no usable sm_90 CUDA device (there is no CPU fallback)";
         case P252_ERR_OUT_OF_MEMORY: return "out of device memory";
     }
     return "unknown status";
@@ -338,10 +338,10 @@ int p252_create_on_stream(int device, void* cuda_stream, p252_ctx** out) {
     if (device < 0 || device >= n) return P252_ERR_INVALID_ARGUMENT;
     cudaDeviceProp prop;
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return P252_ERR_NO_DEVICE;
-    if (prop.major != 10) return P252_ERR_NO_DEVICE;   // kernels are sm_100a SASS only
+    if (prop.major != 9 || prop.minor != 0) return P252_ERR_NO_DEVICE;   // kernels are sm_90a SASS only
     p252_ctx* ctx = new p252_ctx();
     ctx->device = device;
-    ctx->coop_max = p252::coop_max_items();
+    ctx->coop_max = p252::coop_max_items(prop.multiProcessorCount);
     DeviceGuard g(device);
     auto bail = [&](cudaError_t e, const char* w) {
         int rc = fail_cuda(nullptr, e, w);

@@ -1,10 +1,10 @@
-// Device-side Hades permutation for BLS12-381 Fr on sm_100a -- one width-5 state per thread, all
+// Device-side Hades permutation for BLS12-381 Fr on sm_90a -- one width-5 state per thread, all
 // 40 state words in registers.
 //
 // Replaces, on the batch path, the reference's scalar loop
-//   Hades::perm                      /root/reference/src/hades/permutation.rs:105-123
+//   Hades::perm                      src/hades/permutation.rs:105-123
 //   add_round_constants / quintic_s_box / mul_matrix
-//                                    /root/reference/src/hades/permutation/scalar.rs:39-64
+//                                    src/hades/permutation/scalar.rs:39-64
 // with the bit-exact "scaled lazy" formulation derived in tools/hades_model.py:
 //   * 365 unreduced Montgomery products per permutation (IMAD.WIDE carry chains, fr_ptx.cuh)
 //     instead of the reference's 2000 (dense 25-multiply MDS every round);
@@ -108,7 +108,7 @@ __device__ __forceinline__ void montsqr(uint32_t (&r)[8], const uint32_t (&a)[8]
 }
 
 // z = u^5 / R^4 (unreduced): two squarings and one product like quintic_s_box
-// (/root/reference/src/hades/permutation/scalar.rs:50-52).  u < 1.0003 p  =>  z < 1.89 p.
+// (src/hades/permutation/scalar.rs:50-52).  u < 1.0003 p  =>  z < 1.89 p.
 __device__ __forceinline__ void sbox(uint32_t (&z)[8], const uint32_t (&u)[8]) {
     uint32_t a[8], b[8];
     montsqr(a, u);             // < 1.4533 p
@@ -124,11 +124,11 @@ __device__ __forceinline__ void load_const(uint32_t (&d)[8], const uint32_t* c) 
 constexpr double kTwo52 = 4503599627370496.0;
 
 // s <- redc1(C s + A[next_round]) in place -- mul_matrix (+ the next add_round_constants) of the reference,
-// /root/reference/src/hades/permutation/scalar.rs:39-48,54-64.
+// src/hades/permutation/scalar.rs:39-48,54-64.
 //
 // The 25 products per round are (<= 17 bit constant) x (32-bit limb); a column sum over the five lanes is
-// below 268697 * 2^32 < 2^50.1, i.e. EXACT in an IEEE double.  B200 has a full-rate FP64 pipe that the integer
-// S-box leaves idle, so the column sums are formed with DFMA there (concurrently with the IMAD.WIDE carry
+// below 268697 * 2^32 < 2^50.1, i.e. EXACT in an IEEE double.  The FP64 pipe is left idle by the integer
+// S-box, so the column sums are formed with DFMA there (concurrently with the IMAD.WIDE carry
 // chains on the fmaheavy pipe) instead of 40 IMAD.WIDE per lane:
 //   limb -> double      : I2F.F64.U32 (exact)
 //   acc = 2^52 + sum_j c_ij * limb_j   (five DFMA; every partial sum is an integer < 2^53: no rounding)
@@ -234,8 +234,8 @@ __device__ __forceinline__ void hades_permute(uint32_t (&s)[5][8], uint32_t out_
 // ---------------------------------------------------------------------------------------------
 // Lane-split permutation for SMALL batches: five threads per state, thread `li` of a group holds lane `li`.
 //
-// One permutation on one thread is a chain of ~106 k dependent-ish instructions (0.18 ms for a lone warp on B200:
-// a single warp can issue an IMAD.WIDE only every ~6 cycles); a batch that does not fill the machine (the top
+// One permutation on one thread is a chain of ~106 k dependent-ish instructions (a single warp
+// cannot issue its IMAD.WIDEs back to back); a batch that does not fill the machine (the top
 // levels of a Merkle tree, a single Hash::digest) is bound by that latency, not by throughput.  Splitting the
 // state over five threads takes the four idle S-boxes of a full round and four of the five mix rows off the
 // critical path:  full round = 1 S-box + 1 mix row per thread (instead of 5 + 5), partial round = lane 4's
@@ -244,7 +244,7 @@ __device__ __forceinline__ void hades_permute(uint32_t (&s)[5][8], uint32_t out_
 // two paths and the oracle).  Throughput per state is ~3x worse (6 states per warp instead of 32), so the
 // launchers use it only below kCoopMaxItems.
 //   li   : lane of the state this thread owns (0..4; the reference's S-box lane in partial rounds is 4,
-//          /root/reference/src/hades/permutation.rs:68)
+//          src/hades/permutation.rs:68)
 //   g0   : warp lane of the group's thread 0 (groups are 5 consecutive lanes; lanes 30,31 of a warp idle)
 //   crow : this thread's row of the small-integer MDS as doubles, crow[j] = hades_cmat(li, j)
 // ---------------------------------------------------------------------------------------------
@@ -318,7 +318,7 @@ __device__ __forceinline__ void hades_permute_coop(uint32_t (&s)[8], int li, int
 
 // ---------------------------------------------------------------------------------------------
 // Modular add / sub on fully reduced operands (Safe::add, Encryption::subtract,
-// /root/reference/src/hades/permutation/scalar.rs:33-35,69-75)
+// src/hades/permutation/scalar.rs:33-35,69-75)
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ void fr_add_mod(uint32_t (&r)[8], const uint32_t (&a)[8],
                                            const uint32_t (&b)[8]) {

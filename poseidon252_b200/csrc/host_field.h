@@ -1,6 +1,6 @@
 // Host-side helpers of the library: BLAKE2b-512 (RFC 7693) and the little bit of Fr arithmetic
 // needed to derive sponge tags once per batch (BlsScalar::hash_to_scalar ->
-// from_bytes_wide, called at /root/reference/src/hades/permutation/scalar.rs:29-31).
+// from_bytes_wide, called at src/hades/permutation/scalar.rs:29-31).
 // This is per-batch bookkeeping, not a data path: no permutation is ever computed on the host.
 #pragma once
 #include <stddef.h>

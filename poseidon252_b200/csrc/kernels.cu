@@ -1,12 +1,12 @@
-// Batch kernels of the B200 Poseidon/Hades engine (sm_100a).  One sponge state per thread, state in
+// Batch kernels of the Poseidon/Hades engine (sm_90a).  One sponge state per thread, state in
 // registers; global memory is touched only by 128-bit accesses: warp-cooperative, fully coalesced
 // tiles staged through shared memory for the hash/permute kernels (each LDG.128/STG.128 of a warp
 // covers whole 128-byte item chunks), per-thread 2 x 128-bit per scalar for encrypt/decrypt.
 //
 // Sponge schedule = dusk-safe 0.3 `Sponge` as driven by the reference:
-//   Hash::finalize   /root/reference/src/hash.rs:128-155      -> k_sponge_digest
-//   encrypt/decrypt  /root/reference/src/encryption.rs:62-95  -> k_encrypt / k_decrypt
-//   Safe::permute    /root/reference/src/hades/permutation/scalar.rs:25-27 -> k_permute
+//   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest
+//   encrypt/decrypt  src/encryption.rs:62-95  -> k_encrypt / k_decrypt
+//   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
 #include "kernels.h"
@@ -107,12 +107,12 @@ __device__ __forceinline__ void store_fr(uint8_t* p, const uint32_t (&d)[8]) {
 // One permutation call site: step s > 0 is always preceded by a permutation; steps [0, nin) absorb
 // 4-scalar chunks, steps [nin, nin+nout) squeeze 4-scalar chunks.  Permutations = nin + nout - 1
 // = ceil(in_len/4) + ceil(out_len/4) - 1  (Merkle4: exactly 1).
-// kTruncate: Hash::finalize_truncated (/root/reference/src/hash.rs:164-183) -- every squeezed scalar is taken
+// kTruncate: Hash::finalize_truncated (src/hash.rs:164-183) -- every squeezed scalar is taken
 // out of Montgomery form and masked to 250 bits; the 4 x u64 written are the raw limbs the reference hands to
 // JubJubScalar::from_raw.
 // Launch shape: kT threads per block, register allocation held to kMB resident blocks per SM.  128 x 5 (96 registers,
-// 20 warps/SM) is the general shape; 256 x 2 (128 registers, 16 warps/SM) is 0.9 % faster on batches of many waves
-// and much slower below one wave (8-warp blocks pile onto half the SMs), so only launch_digest's large-batch path uses it.
+// 20 warps/SM) is the general shape; 256 x 2 (128 registers, 16 warps/SM) serves only batches of many waves (the
+// large-batch paths of launch_digest / launch_permute): below one wave its 8-warp blocks pile onto half the SMs.
 template <bool kTruncate, int kT = kThreads, int kMB = kMinBlocks>
 __global__ void __launch_bounds__(kT, kMB) k_sponge_digest(FrArg tag, const uint8_t* __restrict__ in, size_t n,
                                                             uint32_t in_len, uint8_t* __restrict__ out,
@@ -374,7 +374,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) k_crypt(FrArg tag, const
     }
 }
 
-// ---- Merkle openings (consumer: poseidon-merkle `Opening`, /root/reference/AGENTS.md:62-66) -------------------
+// ---- Merkle openings (consumer: poseidon-merkle `Opening`, AGENTS.md:62-66) -------------------
 // A tree over n_leaves = arity^depth leaves is stored as `leaves` + `nodes` (internal levels bottom-up, root last:
 // the layout p252_merkle_build writes).  The opening of leaf i holds, for every level l = 0..depth-1 (0 = leaf level),
 // the whole sibling group of the path node: the `arity` items at positions [g*arity, (g+1)*arity) of level l, with
@@ -410,7 +410,7 @@ __global__ void __launch_bounds__(256) k_merkle_open(const uint8_t* __restrict__
 }
 
 // k_merkle_verify: one thread per opening, `depth` chained Merkle digests (Hash::digest(Domain::MerkleA, group),
-// /root/reference/src/hash.rs:22-31,191-195) with the membership check of every level fused in:
+// src/hash.rs:22-31,191-195) with the membership check of every level fused in:
 //   cur = leaf;  for l: require group[l][pos_l] == cur;  cur = digest(group[l]);   finally require cur == root.
 // The sibling groups are read with the same warp-cooperative 128-bit tile as k_sponge_digest.
 template <int kLog2Arity>
@@ -492,17 +492,11 @@ static inline unsigned grid_for(size_t n) { return (unsigned)((n + kThreads - 1)
 constexpr size_t kWideShapeMinItems = P252_WIDE_SHAPE_MIN;
 
 // Default for p252_set_small_batch_max: batches up to this many items take the lane-split kernel (latency-bound
-// regime); the environment variable P252_COOP_MAX overrides it (0 disables the lane-split path).  Measured crossover:
-// profiles/README.md "small batches".
-#ifndef P252_COOP_MAX_DEFAULT
-#define P252_COOP_MAX_DEFAULT 3552   // 148 SMs x 4 sub-partitions x 6 items per warp: one lane-split warp per sub-partition
-#endif
-size_t coop_max_items() {
-    static const size_t v = [] {
-        const char* e = getenv("P252_COOP_MAX");
-        return e ? (size_t)strtoull(e, nullptr, 10) : (size_t)P252_COOP_MAX_DEFAULT;
-    }();
-    return v;
+// regime): one lane-split warp (6 items) per SM sub-partition, i.e. 3168 items on a 132-SM H100.  The environment
+// variable P252_COOP_MAX overrides it (0 disables the lane-split path).
+size_t coop_max_items(int sm_count) {
+    const char* e = getenv("P252_COOP_MAX");
+    return e ? (size_t)strtoull(e, nullptr, 10) : (size_t)sm_count * 4 * kCoopItemsPerWarp;
 }
 
 cudaError_t launch_permute(void* states, size_t n, bool dense, size_t coop_max, cudaStream_t st) {
@@ -543,7 +537,7 @@ cudaError_t launch_digest(const uint64_t tag[4], const void* in, size_t n, uint3
 }
 
 // ---- wire format: canonical 32-byte little-endian <-> BlsScalar.0 (Montgomery limbs) ---------------------
-// BlsScalar::from_bytes / to_bytes (used at /root/reference/src/hades.rs:94-105,131 and
+// BlsScalar::from_bytes / to_bytes (used at src/hades.rs:94-105,131 and
 // src/hades/round_constants.rs:64-68).  Elementwise, 32 B in + 32 B out per scalar: the one HBM-bound kernel.
 template <bool kFromBytes>
 __global__ void __launch_bounds__(256) k_convert(const uint8_t* __restrict__ in, size_t n, uint8_t* __restrict__ out,

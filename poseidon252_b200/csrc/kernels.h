@@ -1,4 +1,4 @@
-// Host-callable launchers of the sm_100a kernels (kernels.cu).  Internal to the library; the public
+// Host-callable launchers of the sm_90a kernels (kernels.cu).  Internal to the library; the public
 // boundary is include/poseidon252_b200.h.  All pointers are DEVICE pointers, 16-byte aligned;
 // scalars are BlsScalar.0 (4 x u64 LE limbs, Montgomery form, < p).
 #pragma once
@@ -25,7 +25,7 @@ cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], 
                                  const uint64_t* leaf_idx, const void* paths, size_t n, int arity, uint32_t depth,
                                  uint8_t* ok, unsigned long long* n_failed, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
-size_t coop_max_items();   // default small-batch threshold (P252_COOP_MAX or the built-in value)
+size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from
 // the generated PTX (fr_ptx.cuh) and the round structure of hades_permute()
 uint32_t wide_mul_per_permutation();

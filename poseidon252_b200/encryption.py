@@ -1,4 +1,4 @@
-"""`encrypt` / `decrypt` -- mirror of /root/reference/src/encryption.rs over the B200 engine.
+"""`encrypt` / `decrypt` -- mirror of src/encryption.rs over the GPU engine.
 The shared secret is the (u, v) coordinate pair of the JubJubAffine point
 (src/encryption.rs:71,92): a (2, 4) uint64 array."""
 import numpy as np

@@ -2,7 +2,7 @@
 
 Buffers are either numpy uint64 arrays (HOST: the library stages H2D/D2H in overlapped chunks) or
 torch CUDA tensors of dtype int64/uint64 (DEVICE: zero-copy, enqueued on the engine's stream).
-There is no CPU fallback: constructing an Engine without a B200-class GPU raises EngineError."""
+There is no CPU fallback: constructing an Engine without an H100 (sm_90) GPU raises EngineError."""
 import ctypes
 
 import numpy as np

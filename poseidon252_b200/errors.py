@@ -1,5 +1,5 @@
 """Error variants of the batch engine -- mirror of dusk_poseidon::Error
-(/root/reference/src/error.rs:11-32) plus engine failures."""
+(src/error.rs:11-32) plus engine failures."""
 
 
 class Error(Exception):
@@ -39,7 +39,7 @@ class InvalidPoint(Error):
 
 
 class EngineError(RuntimeError):
-    """CUDA / NCCL / argument failures of the B200 engine (negative p252_status codes)."""
+    """CUDA / NCCL / argument failures of the engine (negative p252_status codes)."""
 
     def __init__(self, code, message):
         super().__init__("p252 status %d: %s" % (code, message))

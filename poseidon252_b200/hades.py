@@ -1,4 +1,4 @@
-"""`hades` -- the permutation seam (/root/reference/src/hades.rs, src/hades/permutation.rs).
+"""`hades` -- the permutation seam (src/hades.rs, src/hades/permutation.rs).
 `permute` = Safe::permute for one state; `permute_batch` = NEW batch entry."""
 import numpy as np
 

@@ -1,4 +1,4 @@
-"""`Hash` / `Domain` -- host-side mirror of /root/reference/src/hash.rs over the B200 engine.
+"""`Hash` / `Domain` -- host-side mirror of src/hash.rs over the GPU engine.
 
 Same names, argument meaning and error behaviour as the reference; every digest is computed by the
 CUDA sponge kernel (a single `Hash::digest` is a batch of one).  New: `Hash.digest_batch`."""

@@ -1,5 +1,5 @@
 """Arity-4 Merkle trees of Domain::Merkle4 digests (node = Hash::digest(Domain::Merkle4, 4 children),
-/root/reference/src/hash.rs:22-26).  Tree logic itself left the reference crate in 0.29.0
+src/hash.rs:22-26).  Tree logic itself left the reference crate in 0.29.0
 (CHANGELOG.md:164-168); only the node hash is defined there."""
 from .engine import default_engine
 

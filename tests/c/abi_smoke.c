@@ -3,7 +3,7 @@
  * The Rust source cannot be compiled in this image, so this program is the mechanical check that the signatures
  * the binding assumes link and behave: compiled as C (not C++) against the header, linked with the library.
  *   without a GPU : p252_create must fail with P252_ERR_NO_DEVICE (no CPU fallback)       -> prints ABI_SMOKE_NO_DEVICE
- *   with a B200   : every call runs on small host buffers and the results are cross-checked -> prints ABI_SMOKE_OK   */
+ *   with an H100  : every call runs on small host buffers and the results are cross-checked -> prints ABI_SMOKE_OK   */
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>

@@ -12,7 +12,7 @@ for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tools")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run by the driver with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
 
 
 @pytest.fixture(scope="session")
@@ -36,9 +36,10 @@ def coracle():
 
 @pytest.fixture(scope="session", params=["default", "throughput-kernel-only"])
 def engine(request):
-    """The CUDA engine.  No skip-on-failure: a GPU test without the native library or without a
-    B200 must fail loudly.  Every test runs twice: with the default dispatch (digest batches <= 3552 items take the
-    lane-split small-batch kernel) and with that kernel disabled, so that both digest kernels see every shape."""
+    """The CUDA engine.  No skip-on-failure: a GPU test without the native library or without an
+    H100 must fail loudly.  Every test runs twice: with the default dispatch (digest batches up to 24 items per SM,
+    3168 on an H100, take the lane-split small-batch kernel) and with that kernel disabled, so that both digest
+    kernels see every shape."""
     import poseidon252_b200 as pb
     eng = pb.Engine(0)
     if request.param != "default":

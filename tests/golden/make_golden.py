@@ -1,5 +1,5 @@
 """Regenerates tests/golden/hades_golden.json from the Python oracle (oracle/hades_oracle.py), which
-reproduces the 6 known-answer vectors of /root/reference/src/hades.rs:134-162.  The reference is Rust
+reproduces the 6 known-answer vectors of src/hades.rs:134-162.  The reference is Rust
 and cannot be executed here (no cargo/rustc; deps not vendored), so these are ORACLE-derived vectors:
 the KAT block is pinned by the reference, the rest by the oracle that passes those KATs.
 All values are canonical big-endian hex (the `{:?}` format of BlsScalar)."""

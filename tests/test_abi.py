@@ -27,7 +27,7 @@ def test_library_exports_every_declared_symbol():
     for n in names:
         assert hasattr(lib, n), n
     assert sorted(_native.SIGNATURES) == names
-    assert b"sm_100a" in lib.p252_version()
+    assert b"sm_90a" in lib.p252_version()
 
 
 def test_tag_derivation_matches_oracle(oracle):

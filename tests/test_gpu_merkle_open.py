@@ -1,7 +1,7 @@
 """GPU (-m gpu): Merkle openings and batch verification (SURVEY.md 8 row f1, second half) against an oracle
 recomputation -- arity 4 (4^6 leaves) and arity 2 (2^10 leaves), host and device buffers, tampered siblings,
 wrong leaf, wrong index, wrong root.  Node hash = Hash::digest(Domain::Merkle4|Merkle2, children),
-/root/reference/src/hash.rs:22-31; opening semantics = poseidon-merkle `Opening` (AGENTS.md:62-66)."""
+src/hash.rs:22-31; opening semantics = poseidon-merkle `Opening` (AGENTS.md:62-66)."""
 import numpy as np
 import pytest
 

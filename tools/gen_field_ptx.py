@@ -112,7 +112,7 @@ class Prog:
             kind = "sub" if base in ("sub", "subc") else "add"
             if uses_c:
                 # On the GPU a borrow written by sub.cc is NOT a carry for addc/madc (and vice versa) even though
-                # PTX names one flag: measured on B200 (DESIGN.md, rejected experiments).  Never mix flavours.
+                # PTX names one flag: found on the GPU (DESIGN.md, alternatives).  Never mix flavours.
                 assert cf_kind == kind, "carry chain mixes add and sub flavours in %s at %s" % (self.name, opc)
             if sets_cc:
                 cf_kind = kind
@@ -650,7 +650,7 @@ def emu_binary(name: str, a: int, b: int) -> int:
 
 
 HEADER = '''// GENERATED by tools/gen_field_ptx.py -- do not edit by hand.
-// Carry-chain primitives for BLS12-381 Fr on 8 x 32-bit limbs (sm_100a).  Each primitive is ONE asm
+// Carry-chain primitives for BLS12-381 Fr on 8 x 32-bit limbs (sm_90a).  Each primitive is ONE asm
 // statement (the carry flag never crosses a statement); mad.lo.cc/madc.hi.cc pairs become
 // IMAD.WIDE.U32[.X] in SASS.  Verified instruction-by-instruction by the emulator in the generator
 // (tests/test_field_ptx.py) against the integer definitions of tools/hades_model.py.

@@ -1,6 +1,6 @@
-"""Build-time model of the B200 Hades kernel's *scaled lazy* formulation (product tooling; it does
+"""Build-time model of the Hades kernel's *scaled lazy* formulation (product tooling; it does
 not import oracle/).  It (1) regenerates the base constants from the published recipe
-(/root/reference/assets/HOWTO.md:23-41,70-97), (2) derives the per-round tables the CUDA kernel
+(assets/HOWTO.md:23-41,70-97), (2) derives the per-round tables the CUDA kernel
 uses, and (3) provides an integer-exact model of the kernel's arithmetic (same montmul /
 redc1 / cond-sub definitions, same operand bounds) that tests compare with the oracle.
 

@@ -1,11 +1,17 @@
 // Microbenchmark (developer tool): cycles per IMAD.WIDE.U32 on one SM sub-partition, for
 //   A: independent plain mad.wide (no carry; operands vary so that ptxas cannot strength-reduce them)      B: carry chains (mad.lo.cc/madc.hi.cc -> IMAD.WIDE.X)
 //   C: the real interleaved Montgomery row (fr_row) D: A + one DFMA per wide   E: A + two IADD3 per wide
-// as a function of resident warps per sub-partition.  nvcc -gencode arch=compute_100a,code=sm_100a -O3
+// as a function of resident warps per sub-partition.  nvcc -gencode arch=compute_90a,code=sm_90a -O3
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
 #include "../../poseidon252_b200/csrc/fr_ptx.cuh"
+
+static int sm_count() {   // SMs of device 0 (132 on an H100 SXM)
+    static int n = 0;
+    if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
 
 constexpr int REP = 32;
 
@@ -70,9 +76,9 @@ void run(const char* name, int wides_per_rep, uint32_t* d_out) {
         cudaEvent_t a, b;
         cudaEventCreate(&a);
         cudaEventCreate(&b);
-        kern<MODE><<<148, threads>>>(d_out, 12345u, 10);
+        kern<MODE><<<sm_count(), threads>>>(d_out, 12345u, 10);
         cudaEventRecord(a);
-        kern<MODE><<<148, threads>>>(d_out, 12345u, iters);
+        kern<MODE><<<sm_count(), threads>>>(d_out, 12345u, iters);
         cudaEventRecord(b);
         cudaEventSynchronize(b);
         float ms = 0;
@@ -85,7 +91,7 @@ void run(const char* name, int wides_per_rep, uint32_t* d_out) {
 
 int main() {
     uint32_t* d_out;
-    cudaMalloc(&d_out, 148 * 1024 * sizeof(uint32_t));
+    cudaMalloc(&d_out, sm_count() * 1024 * sizeof(uint32_t));
     run<0>("A plain wide, independent", 8, d_out);
     run<1>("B carry chains (2 x 4)", 8, d_out);
     run<2>("C real Montgomery row", 15, d_out);

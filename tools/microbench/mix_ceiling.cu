@@ -6,6 +6,12 @@
 #include <cuda_runtime.h>
 #include "../../poseidon252_b200/csrc/fr_ptx.cuh"
 
+static int sm_count() {   // SMs of device 0 (132 on an H100 SXM)
+    static int n = 0;
+    if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
+
 template <int NALU, int NDFMA>
 __global__ void __launch_bounds__(128, 5) kern(uint32_t* out, uint32_t b, int iters) {
     uint32_t e[8], o[8], x[8];
@@ -36,7 +42,7 @@ void run(uint32_t* d_out) {
     int khz = 0;
     cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
     const int iters = 1000;
-    const int blocks = 148 * 5;      // 5 warps per sub-partition, like the shipped kernels
+    const int blocks = sm_count() * 5;      // 5 warps per sub-partition, like the shipped kernels
     cudaEvent_t a, b;
     cudaEventCreate(&a);
     cudaEventCreate(&b);
@@ -56,7 +62,7 @@ void run(uint32_t* d_out) {
 
 int main() {
     uint32_t* d_out;
-    cudaMalloc(&d_out, 148 * 5 * 128 * sizeof(uint32_t));
+    cudaMalloc(&d_out, sm_count() * 5 * 128 * sizeof(uint32_t));
     run<0, 0>(d_out);
     run<6, 0>(d_out);
     run<12, 0>(d_out);

@@ -5,6 +5,12 @@
 #include "../../poseidon252_b200/csrc/fr_ptx.cuh"
 #include "fr29_proto.cuh"
 
+static int sm_count() {   // SMs of device 0 (132 on an H100 SXM)
+    static int n = 0;
+    if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
+
 __device__ __forceinline__ void montmul32(uint32_t (&r)[8], const uint32_t (&x)[8], const uint32_t (&y)[8]) {
     uint32_t a[8], b[8];
     p252::fr_row_first(a, b, x, y[0]); p252::fr_row(b, a, x, y[1]); p252::fr_row(a, b, x, y[2]); p252::fr_row(b, a, x, y[3]);
@@ -59,7 +65,7 @@ void run(const char* name, uint32_t* d, int blocks) {
 }
 
 int main() {
-    const int blocks = 148 * 5 * 4;
+    const int blocks = sm_count() * 5 * 4;
     uint32_t* d;
     cudaMalloc(&d, (size_t)blocks * 128 * 8 * 4);
     cudaMemset(d, 0x5a, (size_t)blocks * 128 * 8 * 4);

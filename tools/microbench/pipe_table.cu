@@ -1,11 +1,17 @@
 // Microbenchmark (developer tool): issue cost per warp instruction per SM sub-partition for the opcodes the Hades
 // kernel is made of, alone and in pairs, at 5 resident warps per sub-partition (the kernel's occupancy).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o pipe_table pipe_table.cu && ./pipe_table
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o pipe_table pipe_table.cu && ./pipe_table
 // Every test body is REP copies of one asm block over 8 independent accumulators; check the SASS with
 //   cuobjdump -sass pipe_table | grep -A40 'kernILi<k>E'
 #include <cstdint>
 #include <cstdio>
 #include <cuda_runtime.h>
+
+static int sm_count() {   // SMs of device 0 (132 on an H100 SXM)
+    static int n = 0;
+    if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
 
 constexpr int REP = 16;
 
@@ -182,7 +188,7 @@ void run(const char* name, double inst_per_rep, uint32_t* d_out) {
     cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
     const int iters = 4000;
     for (int w : {1, 2, 5, 8}) {
-        const int blocks = 148 * w;     // 128-thread blocks: one warp per sub-partition each
+        const int blocks = sm_count() * w;     // 128-thread blocks: one warp per sub-partition each
         cudaEvent_t a, b;
         cudaEventCreate(&a);
         cudaEventCreate(&b);
@@ -202,7 +208,7 @@ void run(const char* name, double inst_per_rep, uint32_t* d_out) {
 
 int main() {
     uint32_t* d_out;
-    cudaMalloc(&d_out, 148 * 8 * 128 * sizeof(uint32_t));
+    cudaMalloc(&d_out, sm_count() * 8 * 128 * sizeof(uint32_t));
     run<0>("IMAD.WIDE reg,reg", 8, d_out);
     run<1>("IMAD.WIDE reg,imm", 8, d_out);
     run<2>("IMAD.WIDE reg,uniform", 8, d_out);

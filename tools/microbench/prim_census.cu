@@ -1,11 +1,17 @@
 // Developer tool: each arithmetic primitive of the Hades kernel alone in a loop, so that tools/sass_census.py --loops
 // gives the per-primitive SASS instruction mix (and so that variants of one primitive can be compared without a GPU).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -cubin -o /tmp/prim.cubin prim_census.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -cubin -o /tmp/prim.cubin prim_census.cu
 //   python tools/sass_census.py /tmp/prim.cubin --loops
 // Run on a GPU it also times them (modmul/s), one dependent chain per thread at the kernel's occupancy.
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "../../poseidon252_b200/csrc/hades_device.cuh"
+
+static int sm_count() {   // SMs of device 0 (132 on an H100 SXM)
+    static int n = 0;
+    if (!n) cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, 0);
+    return n;
+}
 
 using namespace p252;
 
@@ -60,13 +66,13 @@ void run(const char* name, uint32_t* d, int blocks, int iters, double units) {
     cudaEventElapsedTime(&ms, a, b);
     int khz = 0;
     cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0);
-    const double per_warp_cycles = ms * 1e-3 * khz * 1e3 / ((double)iters * blocks * 4 / (148.0 * 4));
+    const double per_warp_cycles = ms * 1e-3 * khz * 1e3 / ((double)iters * blocks * 4 / ((double)sm_count() * 4));
     printf("%-10s %8.3f ms  %.3e /s   %.0f cycles per warp-op per sub-partition\n", name, ms,
            (double)blocks * 128 * iters * units / (ms * 1e-3), per_warp_cycles);
 }
 
 int main() {
-    const int blocks = 148 * 5 * 4;
+    const int blocks = sm_count() * 5 * 4;
     uint32_t* d;
     cudaMalloc(&d, (size_t)blocks * 128 * 40 * 4);
     cudaMemset(d, 0x5a, (size_t)blocks * 128 * 40 * 4);

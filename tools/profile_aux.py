@@ -21,7 +21,7 @@ if what == "verify":
     ok = eng.merkle_verify_batch(leaves[idx], idx, paths, nodes[-1].cpu().numpy())
     print("verified", int(ok.sum().item()), "of", idx.numel(), "failures", eng.last_verify_failures())
 else:
-    x = torch.from_numpy(random_limbs_fast(rng, (3552, 4)).view(np.int64)).cuda()
+    x = torch.from_numpy(random_limbs_fast(rng, (3168, 4)).view(np.int64)).cuda()
     for _ in range(3):
         out = pb.Hash.digest_batch(pb.Domain.Merkle4, x, engine=eng)
     print(out.shape)

@@ -1,4 +1,4 @@
-"""SASS opcode census of the built library (evidence for profiles/: which instructions the kernels really issue).
+"""SASS opcode census of the built library (which instructions the kernels really issue).
 
     python tools/sass_census.py [path/to/lib.so|cubin] [--kernel SUBSTR] [--loops] [--lines OPC[,OPC...]]
 

@@ -1,6 +1,6 @@
 """Developer timing helper: latency of small Merkle4 digest batches -- lane-split kernel vs throughput kernel vs the
 CPU port (oracle/hades_ref.c, test infrastructure) -- device-resident buffers, CUDA events, median of 20.
-    python tools/small_batch.py > profiles/r2_small_batch.json"""
+    python tools/small_batch.py > small_batch.json"""
 import json
 import os
 import sys
