@@ -1,7 +1,7 @@
 //! SOURCE ONLY -- never compiled in this repository's image (no cargo/rustc).  Batch entry points for
 //! `dusk_poseidon` over the H100 engine: `Hash::digest_batch`, `hades::permute_batch`,
 //! `encrypt_batch`, `decrypt_batch`, `merkle4_build`, Merkle openings, fixed-height trees with batched updates
-//! (`Tree`), bound to include/poseidon252_b200.h.
+//! (`Tree`), variable-length digest batches (`Engine::digest_batch_varlen`), bound to include/poseidon252_b200.h.
 //! The `extern "C"` block below is checked mechanically against the header by tests/test_abi.py
 //! (same symbol set, same parameter counts) and its exact call set is exercised by tests/c/abi_smoke.c.
 //!
@@ -93,6 +93,14 @@ extern "C" {
                              paths_out: *mut Fr, flags: c_int) -> c_int;
 }
 
+// Variable-length digest batches.  A block of its own holding exactly this function: tests/c/varlen_smoke.c calls it
+// (tests/test_varlen_bindings.py checks both against the header).
+extern "C" {
+    fn p252_hash_batch_varlen(ctx: *mut p252_ctx, domain: c_int, input: *const Fr, n_scalars: usize, offsets: *const u64,
+                              n: usize, max_len: usize, out: *mut Fr, out_len: usize, n_rejected: *mut usize,
+                              flags: c_int) -> c_int;
+}
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {
@@ -158,6 +166,25 @@ impl Engine {
             p252_hash_batch(self.0, domain_code(domain), as_fr(inputs), n, in_len, as_fr_mut(&mut out), ol, P252_MEM_HOST)
         })?;
         Ok(out)
+    }
+
+    /// `Hash::digest(domain, inputs[i])` for inputs of any lengths in one call (`output_len` as `Hash::output_len`).
+    pub fn digest_batch_varlen(&self, domain: Domain, inputs: &[&[BlsScalar]], output_len: usize)
+                               -> Result<Vec<Vec<BlsScalar>>, BatchError> {
+        let ol = if domain == Domain::Other && output_len > 0 { output_len } else { 1 };
+        let data: Vec<BlsScalar> = inputs.iter().flat_map(|s| s.iter().copied()).collect();
+        let mut offsets = Vec::with_capacity(inputs.len() + 1);
+        offsets.push(0u64);
+        for s in inputs {
+            offsets.push(offsets[offsets.len() - 1] + s.len() as u64);
+        }
+        let longest = inputs.iter().map(|s| s.len()).max().unwrap_or(1).max(1);
+        let mut out = vec![BlsScalar::zero(); inputs.len() * ol];
+        status(unsafe {
+            p252_hash_batch_varlen(self.0, domain_code(domain), as_fr(&data), data.len(), offsets.as_ptr(), inputs.len(),
+                                   longest, as_fr_mut(&mut out), ol, core::ptr::null_mut(), P252_MEM_HOST)
+        })?;
+        Ok(out.chunks(ol).map(|c| c.to_vec()).collect())
     }
 
     /// `Hash::digest_truncated` batch: raw limbs for `JubJubScalar::from_raw` (src/hash.rs:164-183).

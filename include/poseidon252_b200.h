@@ -163,6 +163,29 @@ int p252_hash_batch(p252_ctx* ctx, int domain, const p252_fr* in, size_t n, size
 int p252_hash_batch_truncated(p252_ctx* ctx, int domain, const p252_fr* in, size_t n, size_t in_len, p252_fr* out_raw,
                               size_t out_len, int flags);
 
+/* Variable-length digest batch: out[i] = Hash::digest(domain, in[offsets[i] .. offsets[i+1])) with
+ * Hash::output_len(out_len) (src/hash.rs:111-115,191-195) for i < n, one call for inputs of any mix of lengths.
+ *   in: n_scalars scalars; offsets: n + 1 entries in the same memory space as in / out (offsets[0] need not be 0, so a
+ *   slice of a larger CSR array works); out: n x out_len, item-major, in input order; n < 2^31.
+ *   Batch checks, before anything runs: out_len == 0 -> INVALID_IO_PATTERN; a Merkle domain with out_len != 1 ->
+ *   IO_PATTERN_VIOLATION; max_len == 0 or > P252_VARLEN_MAX_LEN -> INVALID_ARGUMENT; DEVICE in / out not 16-byte or
+ *   offsets not 8-byte aligned -> INVALID_ARGUMENT.
+ *   Item i is valid iff offsets[i] <= offsets[i+1] <= n_scalars, 1 <= len_i <= max_len (len_i = offsets[i+1] -
+ *   offsets[i]) and p252_hash_tag(domain, len_i, out_len) accepts it (Merkle domains: len_i == arity).
+ *   HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written:
+ *   INVALID_ARGUMENT for a range outside [0, n_scalars] or decreasing offsets, IO_PATTERN_VIOLATION for a Merkle length
+ *   other than the arity, INVALID_IO_PATTERN for length 0, INVALID_ARGUMENT for length > max_len.
+ *   DEVICE: offsets are not inspected on the host; an invalid item is skipped on the device, its out_len output
+ *   scalars are written as zero and it is counted into *n_rejected (optional HOST pointer, 0 for HOST calls; lifetime as
+ *   for p252_mtree_update).  No offset value makes a kernel read outside in[0, n_scalars) or write outside out.
+ *   With P252_ASYNC nothing is synchronised.
+ * The tags of lengths 1..max_len for (domain, out_len) are derived on the host and kept on the device in the context;
+ * the table is rebuilt only when max_len grows or (domain, out_len) changes, so a steady max_len costs nothing.  Items
+ * are sorted by length on the device so that a warp hashes items of (nearly) equal length together. */
+#define P252_VARLEN_MAX_LEN 65536
+int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t n_scalars, const uint64_t* offsets, size_t n,
+                           size_t max_len, p252_fr* out, size_t out_len, size_t* n_rejected, int flags);
+
 /* Wire format (BlsScalar::from_bytes / to_bytes as used at src/hades.rs:94-105,131): n canonical 32-byte
  * little-endian integers <-> BlsScalar.0.  from_bytes: ok[i] = 0 and out[i] = 0 when the value is >= p (the
  * reference returns None); ok may be NULL. */

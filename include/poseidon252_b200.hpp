@@ -7,8 +7,8 @@
 //   dusk_poseidon::Hash{new,output_len,update,finalize,digest}   (src/hash.rs:92-195)  -> p252::Hash
 //   dusk_poseidon::{encrypt, decrypt}        (src/encryption.rs:62-95) -> p252::encrypt / p252::decrypt
 //   dusk_poseidon::Error                     (src/error.rs:11-32)      -> p252::Error (exception)
-//   NEW batch entries: Hash::digest_batch, hades::permute_batch, encrypt_batch, decrypt_batch,
-//   merkle4_build.
+//   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
+//   decrypt_batch, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -134,6 +134,28 @@ public:
         check(p252_hash_batch(eng.get(), static_cast<int>(domain), in, n, in_len, out.data(), ol, P252_MEM_HOST),
               eng.get());
         return out;
+    }
+
+    // NEW: Hash::digest(domain, inputs[i]) for inputs of any lengths, one device call (p252_hash_batch_varlen);
+    // output_len follows src/hash.rs:111-115.  Throws Error like Hash::finalize for an invalid item (nothing computed).
+    static std::vector<std::vector<Scalar>> digest_batch_varlen(Domain domain, const std::vector<std::vector<Scalar>>& inputs,
+                                                                size_t output_len = 1, Engine& e = Engine::default_engine()) {
+        const size_t ol = (domain == Domain::Other && output_len > 0) ? output_len : 1;
+        std::vector<Scalar> data;
+        std::vector<uint64_t> offsets{0};
+        size_t longest = 1;
+        for (auto& in : inputs) {
+            data.insert(data.end(), in.begin(), in.end());
+            offsets.push_back(data.size());
+            longest = in.size() > longest ? in.size() : longest;
+        }
+        std::vector<Scalar> out(inputs.size() * ol);
+        check(p252_hash_batch_varlen(e.get(), static_cast<int>(domain), data.data(), data.size(), offsets.data(), inputs.size(),
+                                     longest, out.data(), ol, nullptr, P252_MEM_HOST),
+              e.get());
+        std::vector<std::vector<Scalar>> res(inputs.size());
+        for (size_t i = 0; i < res.size(); ++i) res[i].assign(out.begin() + i * ol, out.begin() + (i + 1) * ol);
+        return res;
     }
 
 private:

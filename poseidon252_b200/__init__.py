@@ -3,8 +3,8 @@
 Public surface mirrors src/lib.rs:13-31:
     Hash, Domain, Error, HADES_WIDTH, encrypt, decrypt
 plus the batch entry points this engine adds:
-    Hash.digest_batch, hades.permute_batch, encrypt_batch, decrypt_batch, merkle4_build, Tree (fixed-height Merkle
-    tree with batched appends / overwrites).
+    Hash.digest_batch, Hash.digest_batch_varlen (inputs of different lengths in one call), hades.permute_batch,
+    encrypt_batch, decrypt_batch, merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
 from . import hades, merkle, scalar
@@ -12,12 +12,12 @@ from .encryption import decrypt, decrypt_batch, encrypt, encrypt_batch
 from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
-from .hash import Domain, Hash
+from .hash import Domain, Hash, pack_varlen
 from .merkle import Tree, merkle4_build, merkle4_level
 
 HADES_WIDTH = hades.WIDTH
 
-__all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch",
+__all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch", "pack_varlen",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",
            "DecryptionFailed", "InvalidPoint", "EngineError"]

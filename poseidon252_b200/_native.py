@@ -61,9 +61,12 @@ SIGNATURES = {
     "p252_mtree_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
                                   ctypes.POINTER(c_size_t), c_int]),
     "p252_mtree_open_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
+    "p252_hash_batch_varlen": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t,
+                                       ctypes.POINTER(c_size_t), c_int]),
 }
 
 MEM_HOST, MEM_DEVICE, ASYNC, TIMING, NO_GATHER = 0, 1, 2, 4, 8
+VARLEN_MAX_LEN = 65536   # P252_VARLEN_MAX_LEN
 
 
 class KernelInfo(ctypes.Structure):

@@ -1,6 +1,7 @@
 // C ABI of poseidon252_b200 (include/poseidon252_b200.h): context, host-side sponge bookkeeping
 // (io-pattern checks, tag derivation), staging for HOST buffers, kernel launches, fixed-height trees with batched
-// updates (p252_mtree_*), and the multi-GPU arity-4 tree build (one process per GPU, NCCL all-gather per level).
+// updates (p252_mtree_*), variable-length digest batches (p252_hash_batch_varlen), and the multi-GPU arity-4 tree build
+// (one process per GPU, NCCL all-gather per level).
 //
 // Mirrors, for the batch path, the reference's public surface (src/lib.rs:13-31):
 //   Hash / Domain / io_pattern      src/hash.rs:21-155      -> p252_hash_tag, p252_hash_batch
@@ -63,6 +64,15 @@ struct p252_ctx {
     unsigned long long* d_counter = nullptr;
     unsigned long long* h_counter = nullptr;
     size_t coop_max = 0;          // small-batch threshold of the lane-split digest kernel
+    // tag table of p252_hash_batch_varlen: tags[len] for len = 0..vt_len of (vt_domain, vt_out_len) on the device
+    // (stream-ordered allocation), uploaded from a pinned staging buffer whose last upload ev_tags marks; staging
+    // buffers replaced while their upload was still pending wait in vt_retired until the context is destroyed
+    p252_fr* vt_dev = nullptr;
+    p252_fr* vt_host = nullptr;
+    std::vector<p252_fr*> vt_retired;
+    size_t vt_host_cap = 0, vt_len = 0, vt_out_len = 0;
+    int vt_domain = -1;
+    cudaEvent_t ev_tags = nullptr;
     // test hook: index of the staged chunk that fails in the next host-buffer call (-1 = none)
     long long fail_chunk = -1;
     // multi-GPU
@@ -162,6 +172,8 @@ struct Io {
     size_t item_bytes;   // bytes per batch item
 };
 
+int join_slots(p252_ctx* ctx, int rc, bool wipe);
+
 // wipe = true: the staging arenas held secrets (shared secret, nonce, plaintext); they are cleared before
 // returning (the reference's dependencies zeroize sponge state, Cargo.toml:15,17 "zeroize").
 // Whatever happens inside the chunk loop, the common exit below runs: slot streams are joined back into the
@@ -222,9 +234,11 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
         }
         return P252_OK;
     };
-    int rc = body();
+    return join_slots(ctx, body(), wipe);
+}
 
-    // ---- common exit (success and failure): wipe, join, drain --------------------------------------------------
+// Common exit of every HOST call that ran on the slot streams (success and failure): wipe, join, drain.
+int join_slots(p252_ctx* ctx, int rc, bool wipe) {
     const std::string first_error = ctx->last_error;
     cudaError_t ce = cudaSuccess;
     auto keep = [&](cudaError_t e) {
@@ -371,6 +385,8 @@ int p252_create_on_stream(int device, void* cuda_stream, p252_ctx** out) {
     if ((e = cudaEventCreateWithFlags(&ctx->ev_comm, cudaEventDisableTiming)) != cudaSuccess)
         return bail(e, "cudaEventCreate");
     if ((e = cudaEventCreate(&ctx->ev_tree_end)) != cudaSuccess) return bail(e, "cudaEventCreate");
+    if ((e = cudaEventCreateWithFlags(&ctx->ev_tags, cudaEventDisableTiming)) != cudaSuccess)
+        return bail(e, "cudaEventCreate");
     if ((e = cudaMalloc(reinterpret_cast<void**>(&ctx->d_counter), sizeof(unsigned long long))) != cudaSuccess)
         return bail(e, "cudaMalloc");
     if ((e = cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_counter), sizeof(unsigned long long), cudaHostAllocPortable)) != cudaSuccess)
@@ -402,7 +418,11 @@ void p252_destroy(p252_ctx* ctx) {
     for (auto& le : ctx->level_events)
         for (cudaEvent_t ev : {le.k0, le.k1, le.g0, le.g1})
             if (ev) cudaEventDestroy(ev);
+    if (ctx->vt_dev) cudaFreeAsync(ctx->vt_dev, ctx->stream);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);   // pending host functions reference h_counter
+    if (ctx->vt_host) cudaFreeHost(ctx->vt_host);
+    for (p252_fr* h : ctx->vt_retired) cudaFreeHost(h);
+    if (ctx->ev_tags) cudaEventDestroy(ctx->ev_tags);
     if (ctx->d_counter) cudaFree(ctx->d_counter);
     if (ctx->h_counter) cudaFreeHost(ctx->h_counter);
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -1191,6 +1211,185 @@ int p252_mtree_open_batch(p252_ctx* ctx, const p252_mtree* tree, const uint64_t*
         }
     }
     return P252_OK;
+}
+
+}  // extern "C"
+
+// ---- variable-length digest batches (p252_hash_batch_varlen) ----------------------------------------------------
+namespace {
+
+// The device tag table for (domain, out_len) covering lengths 1..max_len: reused while it covers the call, otherwise
+// rebuilt on the host (BLAKE2b stays there) and uploaded on the context stream.  The replaced table is freed in stream
+// order, after every kernel already enqueued that reads it; the pinned staging buffer is rewritten only after its
+// previous upload has completed.  Lengths the domain refuses (a Merkle length other than the arity) get a zero tag:
+// k_varlen_keys rejects them before any kernel reads it.
+int varlen_tags(p252_ctx* ctx, int domain, size_t max_len, size_t out_len, const p252_fr** table) {
+    if (ctx->vt_dev && ctx->vt_domain == domain && ctx->vt_out_len == out_len && ctx->vt_len >= max_len) {
+        *table = ctx->vt_dev;
+        return P252_OK;
+    }
+    if (ctx->vt_host) {
+        const cudaError_t q = cudaEventQuery(ctx->ev_tags);
+        if (q == cudaErrorNotReady) {                      // still being read: retire it instead of waiting
+            ctx->vt_retired.push_back(ctx->vt_host);
+            ctx->vt_host = nullptr;
+            ctx->vt_host_cap = 0;
+        } else if (q != cudaSuccess) {
+            return fail_cuda(ctx, q, "cudaEventQuery");
+        }
+    }
+    if (ctx->vt_host_cap < max_len + 1) {
+        if (ctx->vt_host) CU(cudaFreeHost(ctx->vt_host));
+        ctx->vt_host = nullptr;
+        ctx->vt_host_cap = 0;
+        CU(cudaHostAlloc(reinterpret_cast<void**>(&ctx->vt_host), (max_len + 1) * sizeof(p252_fr), cudaHostAllocPortable));
+        ctx->vt_host_cap = max_len + 1;
+    }
+    memset(&ctx->vt_host[0], 0, sizeof(p252_fr));
+    for (size_t len = 1; len <= max_len; ++len)
+        if (p252_hash_tag(domain, len, out_len, &ctx->vt_host[len]) != P252_OK) memset(&ctx->vt_host[len], 0, sizeof(p252_fr));
+    p252_fr* d = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&d), (max_len + 1) * sizeof(p252_fr), ctx->stream));
+    cudaError_t e = cudaMemcpyAsync(d, ctx->vt_host, (max_len + 1) * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_tags, ctx->stream);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(d, ctx->stream);
+        return fail_cuda(ctx, e, "varlen tag table upload");
+    }
+    if (ctx->vt_dev) CU(cudaFreeAsync(ctx->vt_dev, ctx->stream));
+    ctx->vt_dev = d;
+    ctx->vt_len = max_len;
+    ctx->vt_domain = domain;
+    ctx->vt_out_len = out_len;
+    *table = d;
+    return P252_OK;
+}
+
+// One batch on `st`: keys (length or 0 = rejected) -> radix sort by length -> the varlen digest kernel.  Temporaries are
+// one stream-ordered allocation.
+int varlen_run(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, uint64_t base, uint64_t n_scalars, const uint64_t* offsets,
+               uint32_t n, uint32_t max_len, uint32_t fixed_len, p252_fr* out, uint32_t out_len, unsigned long long* rejected,
+               cudaStream_t st) {
+    int end_bit = 1;
+    while ((max_len >> end_bit) != 0) ++end_bit;            // keys <= max_len
+    size_t sort_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
+                                       (uint32_t*)nullptr, (int)n, 0, end_bit, st));
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    const size_t arr = up((size_t)n * 4);
+    uint8_t* tmp = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&tmp), 4 * arr + up(sort_bytes), st));
+    uint32_t* keys = reinterpret_cast<uint32_t*>(tmp);
+    uint32_t* vals = reinterpret_cast<uint32_t*>(tmp + arr);
+    uint32_t* lens = reinterpret_cast<uint32_t*>(tmp + 2 * arr);
+    uint32_t* perm = reinterpret_cast<uint32_t*>(tmp + 3 * arr);
+    auto body = [&]() -> int {
+        cudaError_t le = p252::launch_varlen_keys(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected, st);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        size_t b = sort_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(tmp + 4 * arr, b, keys, lens, vals, perm, (int)n, 0, end_bit, st));
+        le = p252::launch_digest_varlen(tags, in, base, offsets, lens, perm, n, out, out_len, ctx->coop_max, st);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        return P252_OK;
+    };
+    int rc = body();
+    cudaError_t fe = cudaFreeAsync(tmp, st);
+    if (rc != P252_OK) return rc;
+    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
+    return P252_OK;
+}
+
+// HOST batch (already validated): consecutive item ranges of about kChunkBytesTarget input bytes (a longer item is a
+// chunk by itself, at most chunk_items_max() items) are staged on the slot streams -- input scalars, their offsets and
+// the output rows in one stream-ordered allocation -- hashed by varlen_run with base = the chunk's first offset, and
+// copied back.
+int varlen_host(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n, uint32_t max_len,
+                uint32_t fixed_len, p252_fr* out, uint32_t out_len) {
+    const long long fail_at = ctx->fail_chunk;
+    ctx->fail_chunk = -1;                                  // one shot
+    auto body = [&]() -> int {
+        CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
+        for (int s = 0; s < kSlots; ++s) CU(cudaStreamWaitEvent(ctx->slots[s].stream, ctx->ev_fork, 0));
+        auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+        size_t k = 0;
+        for (size_t lo = 0, hi = 0; lo < n; lo = hi, ++k) {
+            hi = lo + 1;
+            while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * sizeof(p252_fr) <= kChunkBytesTarget) ++hi;
+            const size_t cnt = hi - lo;
+            const uint64_t s0 = offsets[lo], ns = offsets[hi] - s0;
+            cudaStream_t st = ctx->slots[k % kSlots].stream;
+            const size_t in_b = up(ns * sizeof(p252_fr)), off_b = up((cnt + 1) * 8);
+            uint8_t* d = nullptr;
+            CU(cudaMallocAsync(reinterpret_cast<void**>(&d), in_b + off_b + cnt * out_len * sizeof(p252_fr), st));
+            p252_fr* d_in = reinterpret_cast<p252_fr*>(d);
+            uint64_t* d_off = reinterpret_cast<uint64_t*>(d + in_b);
+            p252_fr* d_out = reinterpret_cast<p252_fr*>(d + in_b + off_b);
+            int rc = P252_OK;
+            cudaError_t e = cudaMemcpyAsync(d_in, in + s0, ns * sizeof(p252_fr), cudaMemcpyHostToDevice, st);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, st);
+            if (e != cudaSuccess)
+                rc = fail_cuda(ctx, e, "varlen staging");
+            else if ((long long)k == fail_at)
+                rc = fail_cuda(ctx, cudaErrorLaunchFailure, "kernel launch (injected fault)");
+            else
+                rc = varlen_run(ctx, tags, d_in, s0, ns, d_off, (uint32_t)cnt, max_len, fixed_len, d_out, out_len, nullptr, st);
+            if (rc == P252_OK) {
+                e = cudaMemcpyAsync(out + lo * out_len, d_out, cnt * out_len * sizeof(p252_fr), cudaMemcpyDeviceToHost, st);
+                if (e != cudaSuccess) rc = fail_cuda(ctx, e, "varlen D2H");
+            }
+            cudaError_t fe = cudaFreeAsync(d, st);
+            if (rc != P252_OK) return rc;
+            if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
+        }
+        return P252_OK;
+    };
+    return join_slots(ctx, body(), false);
+}
+
+}  // namespace
+
+extern "C" {
+
+int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t n_scalars, const uint64_t* offsets, size_t n,
+                           size_t max_len, p252_fr* out, size_t out_len, size_t* n_rejected, int flags) {
+    bool known;
+    domain_sep(domain, &known);
+    if (!ctx || !known || ((!in && n_scalars) || ((!offsets || !out) && n))) return P252_ERR_INVALID_ARGUMENT;
+    if (out_len == 0) return P252_ERR_INVALID_IO_PATTERN;
+    const uint32_t fixed_len = domain == P252_DOMAIN_MERKLE4 ? 4u : (domain == P252_DOMAIN_MERKLE2 ? 2u : 0u);
+    if (fixed_len && out_len != 1) return P252_ERR_IO_PATTERN_VIOLATION;
+    if (max_len == 0 || max_len > P252_VARLEN_MAX_LEN) return P252_ERR_INVALID_ARGUMENT;
+    if (n >= 0x80000000ull || out_len > 0x7fffffffull / 32) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_rejected) *n_rejected = 0;
+    const p252_fr* tags = nullptr;
+    int rc;
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(in) || !aligned16(out) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        if ((rc = varlen_tags(ctx, domain, max_len, out_len, &tags)) != P252_OK) return rc;
+        if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        rc = varlen_run(ctx, tags, in, 0, n_scalars, offsets, (uint32_t)n, (uint32_t)max_len, fixed_len, out, (uint32_t)out_len,
+                        n_rejected ? ctx->d_counter : nullptr, ctx->stream);
+        if (rc != P252_OK) return rc;
+        if ((rc = counter_end(ctx, n_rejected)) != P252_OK) return rc;
+        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        return P252_OK;
+    }
+    // HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written
+    for (size_t i = 0; i < n; ++i) {
+        const uint64_t a = offsets[i], b = offsets[i + 1];
+        if (a > b || b > n_scalars) return P252_ERR_INVALID_ARGUMENT;
+        if (fixed_len && b - a != fixed_len) return P252_ERR_IO_PATTERN_VIOLATION;
+        if (b == a) return P252_ERR_INVALID_IO_PATTERN;
+        if (b - a > max_len) return P252_ERR_INVALID_ARGUMENT;
+    }
+    if (n == 0) return P252_OK;
+    if ((rc = varlen_tags(ctx, domain, max_len, out_len, &tags)) != P252_OK) return rc;
+    return varlen_host(ctx, tags, in, offsets, n, (uint32_t)max_len, fixed_len, out, (uint32_t)out_len);
 }
 
 }  // extern "C"

@@ -4,7 +4,7 @@
 // covers whole 128-byte item chunks), per-thread 2 x 128-bit per scalar for encrypt/decrypt.
 //
 // Sponge schedule = dusk-safe 0.3 `Sponge` as driven by the reference:
-//   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest
+//   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest (k_sponge_digest_varlen: inputs of any lengths)
 //   encrypt/decrypt  src/encryption.rs:62-95  -> k_encrypt / k_decrypt
 //   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
@@ -616,6 +616,178 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) k_merkle_verify(FrArg ta
     }
 }
 
+// ---- variable-length digest batches (p252_hash_batch_varlen) ------------------------------------------------------
+// Item i is the input range [offsets[i] - base, offsets[i+1] - base) of `in` (n_scalars scalars); base lets a staged
+// chunk keep the caller's offsets.  tags[len] is the tag of Hash::digest over `len` inputs (tags[0] = 0, unused).
+//
+// k_varlen_keys: one thread per item.  key = len for a valid item, 0 for an invalid one (counted into *rejected, one
+// atomic per warp); value = i.  Valid: offsets[i] - base <= offsets[i+1] - base <= n_scalars, 1 <= len <= max_len and,
+// for a Merkle domain (fixed_len != 0), len == fixed_len.  Every later read of `in` is bounded by this check.
+__global__ void __launch_bounds__(256) k_varlen_keys(const uint64_t* __restrict__ offsets, uint32_t n, uint64_t base,
+                                                     uint64_t n_scalars, uint32_t max_len, uint32_t fixed_len,
+                                                     uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                     unsigned long long* __restrict__ rejected) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t a = offsets[i] - base, b = offsets[i + 1] - base;
+    const uint64_t len = b - a;
+    const bool ok = a <= b && b <= n_scalars && len >= 1 && len <= max_len && (fixed_len == 0 || len == fixed_len);
+    keys[i] = ok ? (uint32_t)len : 0u;
+    vals[i] = i;
+    if (rejected) {
+        const unsigned act = __activemask();
+        const unsigned bad = __ballot_sync(act, !ok);
+        if (bad && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(bad));
+    }
+}
+
+// k_sponge_digest_varlen: k_sponge_digest over the items sorted by length.  Warp item k is item i = perm[k] with
+// len = lens[k]; every lane carries its own tag, step count and last-chunk width, input chunks go through the warp tile
+// with a per-item base address (shuffled, as in k_mtree_digest), outputs are stored per item.  The loop runs to the
+// warp's largest step count; a lane past its own last step neither absorbs nor permutes.  Rejected items (len 0, sorted
+// to the front) write zero rows.  Warps take the sorted segments from the end, so the longest items start first.
+// 4 resident blocks per SM (128 registers): the per-lane sponge bookkeeping does not fit kMinBlocks' 96 without spills.
+__global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint8_t* __restrict__ tags,
+                                                                      const uint8_t* __restrict__ in, uint64_t base,
+                                                                      const uint64_t* __restrict__ offsets,
+                                                                      const uint32_t* __restrict__ lens,
+                                                                      const uint32_t* __restrict__ perm, uint32_t n,
+                                                                      uint8_t* __restrict__ out, uint32_t out_len) {
+    __shared__ uint4 stage[kWarps][32][8];
+    P252_STAGE_TABLES
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const uint32_t nseg = (n + 31) / 32;
+    const uint32_t wg = blockIdx.x * kWarps + warp;
+    if (wg >= nseg) return;
+    const uint32_t item0 = (nseg - 1 - wg) * 32;
+    const int nitems = (n - item0 < 32) ? (int)(n - item0) : 32;
+    uint4(*st)[8] = stage[warp];
+    const bool live = lane < nitems;
+    const uint32_t k = item0 + (live ? lane : 0);
+    const uint32_t len = live ? lens[k] : 0u;
+    const uint32_t i = perm[k];
+    const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
+    uint8_t* dst = out + (size_t)i * out_len * 32;
+    const uint32_t nin = (len + 3) / 4, nout = (out_len + 3) / 4;
+    const uint32_t steps = len ? nin + nout : 0u;
+    const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
+    uint32_t s[5][8];
+    load_fr(s[0], tags + (size_t)len * 32);
+#pragma unroll
+    for (int q = 1; q < 5; ++q)
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s[q][w] = 0;
+    if (live && len == 0)                                  // rejected: a zero row
+        for (uint32_t q = 0; q < out_len; ++q) store_fr(dst + (size_t)q * 32, s[1]);
+    const int part = lane & 7;
+#pragma unroll 1
+    for (uint32_t step = 0; step < wsteps; ++step) {
+        if (step > 0 && step < steps) {
+            uint32_t need = 0x1fu;                         // the last permutation: only the final squeeze's lanes
+            if (step + 1 == steps) {
+                const uint32_t left = out_len - 4 * (nout - 1);
+                need = ((1u << (left < 4 ? left : 4)) - 1u) << 1;
+            }
+            hades_permute(s, need P252_TAB_PASS);
+        }
+        const uint32_t left = step < nin ? len - 4 * step : 0u;
+        const int nscal = left < 4 ? (int)left : 4;
+        if (__any_sync(0xffffffffu, nscal > 0)) {
+            const uint8_t* mine = src + (size_t)step * 128;
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {                  // warp_gather with a per-item base address and width
+                const int item = r * 4 + (lane >> 3);
+                const uint8_t* g = reinterpret_cast<const uint8_t*>(
+                    __shfl_sync(0xffffffffu, reinterpret_cast<unsigned long long>(mine), item));
+                const int ns = __shfl_sync(0xffffffffu, nscal, item);
+                uint4 x = make_uint4(0, 0, 0, 0);
+                if ((part >> 1) < ns) x = ldg128(g + part * 16);
+                st[item][part ^ (item & 7)] = x;
+            }
+            __syncwarp();
+            uint32_t v[4][8];
+#pragma unroll
+            for (int p = 0; p < 8; ++p) {
+                const uint4 x = st[lane][p ^ (lane & 7)];
+                v[p >> 1][(p & 1) * 4 + 0] = x.x;
+                v[p >> 1][(p & 1) * 4 + 1] = x.y;
+                v[p >> 1][(p & 1) * 4 + 2] = x.z;
+                v[p >> 1][(p & 1) * 4 + 3] = x.w;
+            }
+            __syncwarp();
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                if (q < nscal) {
+                    uint32_t t[8];
+                    fr_add_mod(t, s[1 + q], v[q]);
+#pragma unroll
+                    for (int w = 0; w < 8; ++w) s[1 + q][w] = t[w];
+                }
+            }
+        }
+        if (step >= nin && step < steps) {
+            const uint32_t c = step - nin;
+            const uint32_t oleft = out_len - 4 * c;
+#pragma unroll
+            for (int q = 0; q < 4; ++q)
+                if ((uint32_t)q < oleft) store_fr(dst + (size_t)(4 * c + q) * 32, s[1 + q]);
+        }
+    }
+}
+
+// the same for small batches: five threads per item (hades_permute_coop), as k_sponge_digest_coop.  Every thread runs
+// the warp's largest step count (the permutation's shuffles span the warp); a group past its own last step only idles.
+__global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const uint8_t* __restrict__ tags,
+                                                                        const uint8_t* __restrict__ in, uint64_t base,
+                                                                        const uint64_t* __restrict__ offsets,
+                                                                        const uint32_t* __restrict__ lens,
+                                                                        const uint32_t* __restrict__ perm, uint32_t n,
+                                                                        uint8_t* __restrict__ out, uint32_t out_len) {
+    const int lane = threadIdx.x & 31;
+    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
+    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
+    const size_t k = warp_global * kCoopItemsPerWarp + grp;
+    if (warp_global * kCoopItemsPerWarp >= n) return;            // whole warp idle
+    const bool live = (grp < kCoopItemsPerWarp) && (k < n);      // idle threads still take part in the shuffles
+    double crow[5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
+    const uint32_t len = live ? lens[k] : 0u;
+    const uint32_t i = live ? perm[k] : 0u;
+    const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
+    uint8_t* dst = out + (size_t)i * out_len * 32;
+    const uint32_t nin = (len + 3) / 4, nout = (out_len + 3) / 4;
+    const uint32_t steps = len ? nin + nout : 0u;
+    const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
+    uint32_t s[8];
+    if (li == 0) {
+        load_fr(s, tags + (size_t)len * 32);
+    } else {
+#pragma unroll
+        for (int w = 0; w < 8; ++w) s[w] = 0u;
+        if (live && len == 0)                                    // rejected: a zero row
+            for (uint32_t q = (uint32_t)li - 1; q < out_len; q += 4) store_fr(dst + (size_t)q * 32, s);
+    }
+#pragma unroll 1
+    for (uint32_t step = 0; step < wsteps; ++step) {
+        if (step > 0) hades_permute_coop(s, li, g0, crow);
+        if (step < nin) {
+            const uint32_t q = 4 * step + (uint32_t)li - 1;      // li == 0 wraps to a huge value -> no absorb
+            if (li >= 1 && q < len) {
+                uint32_t v[8], t[8];
+                load_fr(v, src + (size_t)q * 32);
+                fr_add_mod(t, s, v);
+#pragma unroll
+                for (int w = 0; w < 8; ++w) s[w] = t[w];
+            }
+        } else if (step < steps) {
+            const uint32_t q = 4 * (step - nin) + (uint32_t)li - 1;
+            if (li >= 1 && q < out_len) store_fr(dst + (size_t)q * 32, s);
+        }
+    }
+}
+
 // ---- host-callable launchers -------------------------------------------------------------------
 static inline FrArg to_arg(const uint64_t tag[4]) {
     FrArg a;
@@ -794,6 +966,29 @@ cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], 
     else
         k_merkle_verify<1><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), to_arg(root), static_cast<const uint8_t*>(leaf_items),
                                                              leaf_idx, static_cast<const uint8_t*>(paths), n, depth, ok, n_failed);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_varlen_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars, uint32_t max_len,
+                               uint32_t fixed_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_varlen_keys<<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_digest_varlen(const void* tags, const void* in, uint64_t base, const uint64_t* offsets, const uint32_t* lens,
+                                 const uint32_t* perm, uint32_t n, void* out, uint32_t out_len, size_t coop_max, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const uint8_t* t = static_cast<const uint8_t*>(tags);
+    const uint8_t* i = static_cast<const uint8_t*>(in);
+    uint8_t* o = static_cast<uint8_t*>(out);
+    if (n <= coop_max) {
+        const size_t warps = (n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
+        k_sponge_digest_varlen_coop<<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(t, i, base, offsets, lens, perm,
+                                                                                                     n, o, out_len);
+    } else {
+        k_sponge_digest_varlen<<<grid_for(n), kThreads, 0, st>>>(t, i, base, offsets, lens, perm, n, o, out_len);
+    }
     return cudaGetLastError();
 }
 

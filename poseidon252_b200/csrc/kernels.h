@@ -45,6 +45,15 @@ cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int ar
 cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], const void* leaf_items,
                                  const uint64_t* leaf_idx, const void* paths, size_t n, int arity, uint32_t depth,
                                  uint8_t* ok, unsigned long long* n_failed, cudaStream_t st);
+// Variable-length digests (p252_hash_batch_varlen).  Item i = in[offsets[i] - base .. offsets[i+1] - base) of n_scalars.
+// keys: len for a valid item (1 <= len <= max_len, len == fixed_len unless fixed_len == 0, range inside in), 0 for an
+// invalid one (counted into *rejected); vals[i] = i
+cudaError_t launch_varlen_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars, uint32_t max_len,
+                               uint32_t fixed_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st);
+// over the keys sorted ascending (lens) with their values (perm): out[perm[k]] = digest with tag tags[lens[k]] of item
+// perm[k] (out_len scalars, a zero row for lens[k] == 0); lane-split kernel when n <= coop_max
+cudaError_t launch_digest_varlen(const void* tags, const void* in, uint64_t base, const uint64_t* offsets, const uint32_t* lens,
+                                 const uint32_t* perm, uint32_t n, void* out, uint32_t out_len, size_t coop_max, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -203,6 +203,40 @@ class Engine:
                                                         int(out_len), flags | (_native.ASYNC if async_ and flags else 0)))
         return res
 
+    def hash_batch_varlen(self, domain, data, offsets, out_len=1, max_len=None, out=None, async_=False):
+        """n x Hash::digest(domain, data[offsets[i]:offsets[i+1]]) with output_len(out_len), inputs of any lengths in one
+        call.  data (n_scalars, 4) and offsets (n + 1,) live in the same memory space (numpy, or CUDA tensors); offsets[0]
+        need not be 0.  Returns (n, out_len, 4) in input order.  max_len bounds the item lengths (at most
+        VARLEN_MAX_LEN); None takes the longest item, which for CUDA tensors costs a device-to-host sync.  Host batches
+        raise on an invalid item and write nothing; device batches give invalid items a zero row and count them
+        (last_varlen_rejected())."""
+        dp, dlead, flags, dk = self._in(data, (4,))
+        op, n1, ok_ = self._idx(offsets, dk, "offsets")
+        if n1 < 1:
+            raise EngineError(-1, "offsets must have n + 1 >= 1 entries")
+        n = n1 - 1
+        if max_len is None:
+            if n == 0:
+                max_len = 1
+            elif _is_torch(ok_):
+                import torch
+                o = ok_.view(torch.int64)
+                max_len = int((o[1:] - o[:-1]).max().item())
+            else:
+                max_len = int((ok_[1:].astype(np.int64) - ok_[:-1].astype(np.int64)).max())
+            max_len = max(max_len, 1)
+        shape = (n, int(out_len), 4)
+        res = self._out_like(dk, shape) if out is None else self._check_out(out, shape, dk)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._vlrej = self._counter(flags)
+        self._check(self._lib.p252_hash_batch_varlen(self._ctx, int(domain), dp, int(dlead[0]), op, n, int(max_len),
+                                                     self._ptr(res), int(out_len), ctypes.byref(self._vlrej), flags))
+        return res
+
+    def last_varlen_rejected(self):
+        """Items of the last hash_batch_varlen skipped as invalid (device buffers; sync() first after async_)."""
+        return int(getattr(self, "_vlrej", ctypes.c_size_t(0)).value)
+
     def scalars_from_bytes(self, data, async_=False):
         """(n, 32) uint8 canonical little-endian (host) or (n, 4) 64-bit device tensor of the same bytes
         -> (scalars (n, 4), ok (n,) uint8); ok == 0 where the value is >= p."""
@@ -321,11 +355,11 @@ class Engine:
         return res
 
     # -- Merkle openings --------------------------------------------------------------------------
-    def _idx(self, leaf_idx, like):
+    def _idx(self, leaf_idx, like, name="leaf_idx"):
         if _is_torch(like):
             if not _is_torch(leaf_idx) or not leaf_idx.is_cuda or leaf_idx.device != like.device or \
                     str(leaf_idx.dtype) not in ("torch.int64", "torch.uint64") or not leaf_idx.is_contiguous() or leaf_idx.dim() != 1:
-                raise EngineError(-1, "leaf_idx must be a contiguous 1-D int64/uint64 tensor on %s" % like.device)
+                raise EngineError(-1, "%s must be a contiguous 1-D int64/uint64 tensor on %s" % (name, like.device))
             return leaf_idx.data_ptr(), int(leaf_idx.shape[0]), leaf_idx
         a = np.ascontiguousarray(leaf_idx, dtype=np.uint64).reshape(-1)
         return a.ctypes.data, int(a.shape[0]), a

@@ -70,6 +70,17 @@ def io_pattern(domain, chunk_lens, output_len):
     return [("absorb", n) for n in chunk_lens] + [("squeeze", output_len)]
 
 
+def pack_varlen(inputs):
+    """A list of (k_i, 4) scalar arrays -> (data (sum k_i, 4) uint64, offsets (n + 1,) uint64, longest k_i), the
+    layout of `Engine.hash_batch_varlen`.  Pure host work."""
+    arrs = [np.ascontiguousarray(a, dtype=np.uint64).reshape(-1, 4) for a in inputs]
+    lens = np.array([a.shape[0] for a in arrs], dtype=np.uint64)
+    offsets = np.zeros(len(arrs) + 1, dtype=np.uint64)
+    np.cumsum(lens, out=offsets[1:])
+    data = np.concatenate(arrs, axis=0) if arrs else np.zeros((0, 4), dtype=np.uint64)
+    return data, offsets, int(lens.max()) if len(arrs) else 0
+
+
 class Hash:
     """src/hash.rs:92-210.  Scalars are (k, 4) uint64 arrays of BlsScalar.0 limbs."""
 
@@ -133,6 +144,21 @@ class Hash:
         ol = int(output_len) if (domain == Domain.Other and output_len > 0) else 1
         eng = engine or default_engine(inputs.device.index if hasattr(inputs, "is_cuda") else 0)
         return eng.hash_batch_truncated(domain, inputs, ol, out=out, async_=async_)
+
+    @staticmethod
+    def digest_batch_varlen(domain, inputs, output_len=1, engine=None, max_len=None, out=None, async_=False):
+        """NEW batch entry: n independent `Hash::digest(domain, inputs[i])` over inputs of different lengths, one call.
+        inputs: a list of (k_i, 4) host arrays (packed by `pack_varlen`), or a `(data, offsets)` pair as taken by
+        `Engine.hash_batch_varlen` (numpy or CUDA tensors).  Returns (n, out_len, 4) in input order."""
+        domain = Domain(domain)
+        ol = int(output_len) if (domain == Domain.Other and output_len > 0) else 1
+        if isinstance(inputs, tuple):
+            data, offsets = inputs
+        else:
+            data, offsets, longest = pack_varlen(inputs)
+            max_len = max(longest, 1) if max_len is None else max_len
+        eng = engine or default_engine(data.device.index if hasattr(data, "is_cuda") else 0)
+        return eng.hash_batch_varlen(domain, data, offsets, ol, max_len=max_len, out=out, async_=async_)
 
     @staticmethod
     def digest_batch(domain, inputs, output_len=1, engine=None, out=None, async_=False):
