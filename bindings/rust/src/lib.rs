@@ -1,7 +1,8 @@
 //! SOURCE ONLY -- never compiled in this repository's image (no cargo/rustc).  Batch entry points for
 //! `dusk_poseidon` over the H100 engine: `Hash::digest_batch`, `hades::permute_batch`,
 //! `encrypt_batch`, `decrypt_batch`, `merkle4_build`, Merkle openings, fixed-height trees with batched updates
-//! (`Tree`), variable-length digest batches (`Engine::digest_batch_varlen`), bound to include/poseidon252_b200.h.
+//! (`Tree`), sparse fixed-height trees with inserts and removals at any position (`SparseTree`, in smtree.rs),
+//! variable-length digest batches (`Engine::digest_batch_varlen`), bound to include/poseidon252_b200.h.
 //! The `extern "C"` block below is checked mechanically against the header by tests/test_abi.py
 //! (same symbol set, same parameter counts) and its exact call set is exercised by tests/c/abi_smoke.c.
 //!
@@ -100,6 +101,10 @@ extern "C" {
                               n: usize, max_len: usize, out: *mut Fr, out_len: usize, n_rejected: *mut usize,
                               flags: c_int) -> c_int;
 }
+
+// Sparse fixed-height trees (inserts and removals at any position): their own `extern "C"` block in smtree.rs.
+mod smtree;
+pub use smtree::{p252_smtree, SparseTree};
 
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]

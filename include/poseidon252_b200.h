@@ -287,6 +287,53 @@ int p252_mtree_update(p252_ctx* ctx, p252_mtree* tree, const uint64_t* idx, cons
 int p252_mtree_open_batch(p252_ctx* ctx, const p252_mtree* tree, const uint64_t* leaf_idx, size_t n, p252_fr* paths_out,
                           int flags);
 
+/* ---- sparse fixed-height trees: inserts and removals at any position (poseidon-merkle `Tree::insert` / `remove`) ----
+ * Arity A (2 or 4), height H (1..64), capacity <= A^H.  Each position in [0, capacity) is present (holds a value) or
+ * absent.  Level-0 slot j holds the leaf value if j is present and 0 otherwise.  A node of level l >= 1 is present iff
+ * one of its A children is present; a present node is Hash::digest(Domain::Merkle{A}, its A children's slots) (absent
+ * children read as 0), an absent node IS 0 and is never hashed (src/hash.rs:24-26).  The root is the single node of
+ * level H, 0 for an empty tree.  A present leaf whose value is zero is not an absent one: its parent is H(0, ..).
+ * Layout: exactly p252_mtree_layout's, plus one presence byte per slot (1 = present) in the same order -- leaf_slots
+ * bytes for the leaves, then node_slots bytes for levels 1..H.  If the present set is [0, n), leaves and nodes are
+ * bit-identical to those of a p252_mtree with n_leaves = n.  The library owns every absent slot (value and presence of
+ * absent leaves, every node and node presence byte, slots at or beyond capacity) and keeps them consistent; the caller
+ * writes leaves and leaf presence only before p252_smtree_build.  Struct and buffers belong to the caller; flags say
+ * where the buffers live.  DEVICE buffers: leaves / nodes 16-byte aligned, present 4-byte aligned, positions 8-byte
+ * aligned. */
+typedef struct p252_smtree {
+    uint32_t struct_size; /* sizeof(p252_smtree)                                                       */
+    int32_t arity;        /* 2 or 4                                                                    */
+    int32_t height;       /* levels above the leaves; capacity <= arity^height                         */
+    int32_t reserved;
+    uint64_t capacity;    /* positions [0, capacity)                                                   */
+    p252_fr* leaves;      /* leaf_slots scalars (p252_mtree_layout)                                    */
+    p252_fr* nodes;       /* node_slots scalars, levels 1..height bottom-up, root last                 */
+    uint8_t* present;     /* leaf_slots + node_slots bytes, leaves then nodes: 1 = present, 0 = absent  */
+} p252_smtree;
+/* Rebuild every node and node presence byte from the leaves and the leaf presence bytes (a non-zero byte below capacity
+ * is present; build stores 1), and zero the value of every absent leaf.  Hashes only present nodes: the work is
+ * proportional to the present nodes, plus a pass over the leaf presence bytes.  HOST trees are staged to the device. */
+int p252_smtree_build(p252_ctx* ctx, p252_smtree* tree, int flags);
+/* One batch of operations (pos[i], op[i], values[i]): op 0 inserts or overwrites, op 1 removes (values[i] is not read);
+ * op = NULL means all inserts.  The result equals applying the operations one after another in batch order: the last
+ * operation on a position wins, removing an absent position does nothing.  Only the nodes on the touched paths are
+ * revisited, each distinct one once; a node whose children all became absent is zeroed without hashing.  pos / op /
+ * values live in the same memory space as the tree (values is required for n > 0); n < 2^31.
+ *   HOST: a position >= capacity or an op other than 0/1 is P252_ERR_INVALID_ARGUMENT and nothing is modified.
+ *   DEVICE: such an item is skipped on the device and counted into *n_rejected (optional HOST pointer, 0 for HOST
+ *   calls; lifetime as for p252_mtree_update).  Temporaries are stream-ordered; with P252_ASYNC nothing is synchronised.
+ * After a CUDA failure the tree's contents are unspecified: rebuild it. */
+int p252_smtree_update(p252_ctx* ctx, p252_smtree* tree, const uint64_t* pos, const uint8_t* op, const p252_fr* values,
+                       size_t n, size_t* n_rejected, int flags);
+/* *n_present (HOST pointer) = number of present positions.  DEVICE trees: counted on the device; with P252_ASYNC the
+ * value is written by a host function on the context's stream (lifetime as *n_rejected). */
+int p252_smtree_len(p252_ctx* ctx, const p252_smtree* tree, uint64_t* n_present, int flags);
+/* Openings of positions pos[0..n) in the format of p252_mtree_open_batch (n x height x arity, absent slots 0); they
+ * verify with p252_merkle_verify_batch, depth = height.  An absent position or one >= capacity is
+ * P252_ERR_INVALID_ARGUMENT for HOST buffers and an all-zero opening for DEVICE buffers. */
+int p252_smtree_open_batch(p252_ctx* ctx, const p252_smtree* tree, const uint64_t* pos, size_t n, p252_fr* paths_out,
+                           int flags);
+
 /* ---- multi-GPU tree build: one process per GPU, one NCCL all-gather per level ---------------- */
 #define P252_NCCL_UNIQUE_ID_BYTES 128
 /* rank 0 creates the id and ships it to the other ranks by any means (torch.distributed / MPI) */

@@ -325,6 +325,77 @@ private:
     std::vector<Scalar> leaves_, nodes_;
 };
 
+// Sparse fixed-height tree over p252_smtree (host buffers): poseidon-merkle's `Tree::insert(pos, item)` and
+// `Tree::remove(pos)` at any position below `capacity` <= arity^height.  Empty leaves and nodes with no value below them
+// are the zero scalar and are never hashed; a present leaf of value zero is not an empty one.  Batches rehash only the
+// touched paths on the device.
+class SparseTree {
+public:
+    SparseTree(int arity, int height, uint64_t capacity, Engine& e = Engine::default_engine()) : e_(&e) {
+        uint64_t leaf_slots = 0, node_slots = 0;
+        check(p252_mtree_layout(arity, height, capacity, &leaf_slots, &node_slots, nullptr));
+        leaves_.assign(leaf_slots, Scalar{});
+        nodes_.assign(node_slots, Scalar{});
+        present_.assign(leaf_slots + node_slots, 0);
+        t_.struct_size = sizeof(p252_smtree);
+        t_.arity = arity;
+        t_.height = height;
+        t_.reserved = 0;
+        t_.capacity = capacity;
+    }
+    // ops[i] == 0 inserts / overwrites values[i] at pos[i], ops[i] == 1 removes pos[i]; as if applied one after another
+    void apply(const std::vector<uint64_t>& pos, const std::vector<uint8_t>& ops, const std::vector<Scalar>& values) {
+        if (pos.size() != ops.size() || pos.size() != values.size())
+            throw Error(P252_ERR_INVALID_ARGUMENT, "pos, ops and values differ in length");
+        run(pos, ops.data(), values.data());
+    }
+    void insert(const std::vector<uint64_t>& pos, const std::vector<Scalar>& values) {
+        if (pos.size() != values.size()) throw Error(P252_ERR_INVALID_ARGUMENT, "pos and values differ in length");
+        run(pos, nullptr, values.data());
+    }
+    void remove(const std::vector<uint64_t>& pos) {
+        apply(pos, std::vector<uint8_t>(pos.size(), 1), std::vector<Scalar>(pos.size()));
+    }
+    // recompute every node from the leaves and their presence
+    void build() { check(p252_smtree_build(e_->get(), bind(), P252_MEM_HOST), e_->get()); }
+    const Scalar& root() const { return nodes_.back(); }
+    bool contains(uint64_t pos) const { return pos < t_.capacity && present_[pos] != 0; }
+    uint64_t size() {
+        uint64_t n = 0;
+        check(p252_smtree_len(e_->get(), bind(), &n, P252_MEM_HOST), e_->get());
+        return n;
+    }
+    const std::vector<Scalar>& leaves() const { return leaves_; }
+    const std::vector<Scalar>& nodes() const { return nodes_; }
+    const std::vector<uint8_t>& present() const { return present_; }
+    // the poseidon-merkle `Opening` of the present position pos
+    Opening opening(uint64_t pos) {
+        Opening o;
+        o.arity = t_.arity;
+        o.root = root();
+        o.leaf_index = pos;
+        o.branch.resize((size_t)t_.height * t_.arity);
+        check(p252_smtree_open_batch(e_->get(), bind(), &pos, 1, o.branch.data(), P252_MEM_HOST), e_->get());
+        for (int l = 0; l < t_.height; ++l, pos /= (uint64_t)t_.arity) o.positions.push_back(pos % t_.arity);
+        return o;
+    }
+
+private:
+    p252_smtree* bind() {
+        t_.leaves = leaves_.data();
+        t_.nodes = nodes_.data();
+        t_.present = present_.data();
+        return &t_;
+    }
+    void run(const std::vector<uint64_t>& pos, const uint8_t* ops, const Scalar* values) {
+        check(p252_smtree_update(e_->get(), bind(), pos.data(), ops, values, pos.size(), nullptr, P252_MEM_HOST), e_->get());
+    }
+    Engine* e_;
+    p252_smtree t_{};
+    std::vector<Scalar> leaves_, nodes_;
+    std::vector<uint8_t> present_;
+};
+
 // n x Opening::verify with all openings in one launch: ok[i] != 0 iff paths[i] proves items[i] under root
 inline std::vector<uint8_t> merkle_verify_batch(int arity, int depth, const Scalar* items, const uint64_t* leaf_idx,
                                                 const Scalar* paths, const Scalar& root, size_t n,

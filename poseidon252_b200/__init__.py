@@ -4,7 +4,8 @@ Public surface mirrors src/lib.rs:13-31:
     Hash, Domain, Error, HADES_WIDTH, encrypt, decrypt
 plus the batch entry points this engine adds:
     Hash.digest_batch, Hash.digest_batch_varlen (inputs of different lengths in one call), hades.permute_batch,
-    encrypt_batch, decrypt_batch, merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites).
+    encrypt_batch, decrypt_batch, merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites),
+    SparseTree (fixed-height Merkle tree with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
 from . import hades, merkle, scalar
@@ -13,11 +14,11 @@ from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
 from .hash import Domain, Hash, pack_varlen
-from .merkle import Tree, merkle4_build, merkle4_level
+from .merkle import SparseTree, Tree, merkle4_build, merkle4_level
 
 HADES_WIDTH = hades.WIDTH
 
 __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch", "pack_varlen",
-           "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree",
+           "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",
            "DecryptionFailed", "InvalidPoint", "EngineError"]

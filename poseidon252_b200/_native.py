@@ -61,7 +61,11 @@ SIGNATURES = {
     "p252_mtree_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
                                   ctypes.POINTER(c_size_t), c_int]),
     "p252_mtree_open_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
-    "p252_hash_batch_varlen": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t,
+    "p252_smtree_build": (c_int, [c_void_p, c_void_p, c_int]),
+    "p252_smtree_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_size_t), c_int]),
+    "p252_smtree_len": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_uint64), c_int]),
+    "p252_smtree_open_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
+    "p252_hash_batch_varlen":(c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t,
                                        ctypes.POINTER(c_size_t), c_int]),
 }
 
@@ -93,6 +97,13 @@ class MTree(ctypes.Structure):
     _fields_ = [("struct_size", ctypes.c_uint32), ("arity", ctypes.c_int32), ("height", ctypes.c_int32),
                 ("reserved", ctypes.c_int32), ("capacity", ctypes.c_uint64), ("n_leaves", ctypes.c_uint64),
                 ("leaves", ctypes.c_void_p), ("nodes", ctypes.c_void_p)]
+
+
+class SMTree(ctypes.Structure):
+    """p252_smtree"""
+    _fields_ = [("struct_size", ctypes.c_uint32), ("arity", ctypes.c_int32), ("height", ctypes.c_int32),
+                ("reserved", ctypes.c_int32), ("capacity", ctypes.c_uint64), ("leaves", ctypes.c_void_p),
+                ("nodes", ctypes.c_void_p), ("present", ctypes.c_void_p)]
 
 
 NCCL_UNIQUE_ID_BYTES = 128

@@ -1,6 +1,7 @@
 // C ABI of poseidon252_b200 (include/poseidon252_b200.h): context, host-side sponge bookkeeping
 // (io-pattern checks, tag derivation), staging for HOST buffers, kernel launches, fixed-height trees with batched
-// updates (p252_mtree_*), variable-length digest batches (p252_hash_batch_varlen), and the multi-GPU arity-4 tree build
+// updates (p252_mtree_*), sparse fixed-height trees with inserts and removals at any position (p252_smtree_*),
+// variable-length digest batches (p252_hash_batch_varlen), and the multi-GPU arity-4 tree build
 // (one process per GPU, NCCL all-gather per level).
 //
 // Mirrors, for the batch path, the reference's public surface (src/lib.rs:13-31):
@@ -1207,6 +1208,342 @@ int p252_mtree_open_batch(p252_ctx* ctx, const p252_mtree* tree, const uint64_t*
                 else
                     memset(&dst[q], 0, sizeof(p252_fr));
             }
+            j = group;
+        }
+    }
+    return P252_OK;
+}
+
+}  // extern "C"
+
+// ---- sparse fixed-height trees (p252_smtree) -------------------------------------------------------------------
+namespace {
+
+static_assert(sizeof(size_t) == sizeof(uint64_t), "p252_smtree_len publishes its count through the size_t counter path");
+
+int smtree_check(const p252_smtree* t, int flags, MLayout* L) {
+    if (!t || t->struct_size < sizeof(p252_smtree) || !t->leaves || !t->nodes || !t->present) return P252_ERR_INVALID_ARGUMENT;
+    int rc = mtree_layout(t->arity, t->height, t->capacity, L);
+    if (rc != P252_OK) return rc;
+    if ((flags & P252_MEM_DEVICE) && (!aligned16(t->leaves) || !aligned16(t->nodes) || (reinterpret_cast<uintptr_t>(t->present) & 3)))
+        return P252_ERR_INVALID_ARGUMENT;
+    return P252_OK;
+}
+
+// The climb shared by build and update (DEVICE pointers): level l's dirty set D_l = DeviceSelect::Flagged over the
+// candidates (parent, flag) of the level below -- bound[l-1] of them, count on the device -- then the presence-aware
+// digest of exactly those groups, then the candidates of the next level.
+int smtree_climb(p252_ctx* ctx, const p252_smtree* t, const MLayout& L, uint8_t* flag, uint64_t* parent, uint64_t* d, int* cnt,
+                 const uint64_t* bound, void* cub_tmp, size_t cub_bytes) {
+    const int A = t->arity, H = t->height;
+    p252_fr tag;
+    p252_hash_tag(merkle_domain(A), (size_t)A, 1, &tag);
+    const p252_fr* below = t->leaves;
+    const uint8_t* below_p = t->present;
+    uint8_t* node_p = t->present + L.slots[0];
+    for (int l = 1; l <= H; ++l) {
+        size_t b = cub_bytes;
+        CU(cub::DeviceSelect::Flagged(cub_tmp, b, parent, flag, d, cnt + l, (int)bound[l - 1], ctx->stream));
+        p252_fr* level = t->nodes + L.off[l];
+        uint8_t* level_p = node_p + L.off[l];
+        cudaError_t le = p252::launch_smtree_digest(limbs(&tag), below, below_p, A, level, level_p, d, cnt + l, bound[l],
+                                                    ctx->coop_max, ctx->stream);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        if (l < H) {
+            le = p252::launch_mtree_parents(d, cnt + l, (uint32_t)bound[l], A, flag, parent, ctx->stream);
+            if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+            ctx->launches++;
+        }
+        below = level;
+        below_p = level_p;
+    }
+    return P252_OK;
+}
+
+// host-side upper bounds of |D_l|: bound[0] candidates, then at most one node per group of the level below
+void smtree_bounds(const MLayout& L, int A, int H, uint64_t n0, uint64_t* bound) {
+    bound[0] = n0;
+    for (int l = 1; l <= H; ++l) bound[l] = std::min<uint64_t>(bound[l - 1], L.slots[l - 1] / (uint64_t)A);
+}
+
+// DEVICE build: clear every node and node presence byte, seed the climb with the leaf groups that hold a present leaf
+// (k_smtree_seed also zeroes absent leaves), climb.  Only present nodes are hashed.  Temporaries: one stream-ordered
+// allocation of about 17 bytes per leaf group.
+int smtree_build_device(p252_ctx* ctx, const p252_smtree* t, const MLayout& L) {
+    const int A = t->arity, H = t->height;
+    const uint64_t G = L.slots[0] / (uint64_t)A;
+    if (G >= 0x80000000ull) return P252_ERR_INVALID_ARGUMENT;
+    CU(cudaMemsetAsync(t->nodes, 0, L.node_slots * sizeof(p252_fr), ctx->stream));
+    CU(cudaMemsetAsync(t->present + L.slots[0], 0, L.node_slots, ctx->stream));
+    uint64_t bound[p252::kMaxDepth + 1];
+    smtree_bounds(L, A, H, G, bound);
+    size_t select_bytes = 0;
+    CU(cub::DeviceSelect::Flagged(nullptr, select_bytes, (const uint64_t*)nullptr, (const uint8_t*)nullptr, (uint64_t*)nullptr,
+                                  (int*)nullptr, (int)G, ctx->stream));
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    uint8_t* base = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), 2 * up(G * 8) + up(G) + up((H + 1) * sizeof(int)) + up(select_bytes),
+                       ctx->stream));
+    uint64_t* parent = reinterpret_cast<uint64_t*>(base);
+    uint64_t* d = reinterpret_cast<uint64_t*>(base + up(G * 8));
+    uint8_t* flag = base + 2 * up(G * 8);
+    int* cnt = reinterpret_cast<int*>(flag + up(G));
+    void* cub_tmp = reinterpret_cast<uint8_t*>(cnt) + up((H + 1) * sizeof(int));
+    auto body = [&]() -> int {
+        cudaError_t le = p252::launch_smtree_seed(t->present, t->leaves, G, t->capacity, A, flag, parent, ctx->stream);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        return smtree_climb(ctx, t, L, flag, parent, d, cnt, bound, cub_tmp, up(select_bytes));
+    };
+    int rc = body();
+    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
+    if (rc != P252_OK) return rc;
+    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
+    return P252_OK;
+}
+
+// DEVICE update: keys (position, or the sentinel capacity) -> stable radix sort of (key, batch position) -> the last op
+// per position is applied -> climb.  Temporaries are one stream-ordered allocation; the dirty-set counts stay on the
+// device.
+int smtree_update_device(p252_ctx* ctx, p252_smtree* t, const MLayout& L, const uint64_t* pos, const uint8_t* op,
+                         const p252_fr* values, uint32_t n, size_t* n_rejected) {
+    const int A = t->arity, H = t->height;
+    uint64_t bound[p252::kMaxDepth + 1];
+    smtree_bounds(L, A, H, n, bound);
+    int end_bit = 1;
+    while (end_bit < 64 && (t->capacity >> end_bit)) ++end_bit;   // keys <= capacity (the sentinel)
+
+    size_t sort_bytes = 0, select_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                       (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, 0, end_bit, ctx->stream));
+    CU(cub::DeviceSelect::Flagged(nullptr, select_bytes, (const uint64_t*)nullptr, (const uint8_t*)nullptr, (uint64_t*)nullptr,
+                                  (int*)nullptr, (int)n, ctx->stream));
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    const size_t cub_bytes = up(std::max(sort_bytes, select_bytes));
+    const size_t total = 3 * up((size_t)n * 8) + 2 * up((size_t)n * 4) + up(n) + up((H + 1) * sizeof(int)) + cub_bytes;
+    uint8_t* base = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), total, ctx->stream));
+    uint8_t* p = base;
+    auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
+    uint64_t* keys = reinterpret_cast<uint64_t*>(take((size_t)n * 8));      // unsorted keys, then the dirty set D_l
+    uint64_t* skeys = reinterpret_cast<uint64_t*>(take((size_t)n * 8));
+    uint64_t* parent = reinterpret_cast<uint64_t*>(take((size_t)n * 8));
+    uint32_t* bpos = reinterpret_cast<uint32_t*>(take((size_t)n * 4));
+    uint32_t* sbpos = reinterpret_cast<uint32_t*>(take((size_t)n * 4));
+    uint8_t* flag = take(n);
+    int* cnt = reinterpret_cast<int*>(take((H + 1) * sizeof(int)));
+    void* cub_tmp = take(cub_bytes);
+
+    auto body = [&]() -> int {
+        int rc;
+        if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        cudaError_t le = p252::launch_smtree_keys(pos, op, n, t->capacity, keys, bpos, n_rejected ? ctx->d_counter : nullptr,
+                                                  ctx->stream);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        size_t b = cub_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, skeys, bpos, sbpos, (int)n, 0, end_bit, ctx->stream));
+        le = p252::launch_smtree_leaf_write(skeys, sbpos, n, t->capacity, A, op, values, t->leaves, t->present, flag, parent,
+                                            ctx->stream);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        if ((rc = smtree_climb(ctx, t, L, flag, parent, keys, cnt, bound, cub_tmp, cub_bytes)) != P252_OK) return rc;
+        return counter_end(ctx, n_rejected);
+    };
+    int rc = body();
+    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
+    if (rc != P252_OK) return rc;
+    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
+    return P252_OK;
+}
+
+// HOST update (already validated): sort and dedupe here, apply the last op per position, then per level: a dirty node
+// whose children are all absent is zeroed (value and presence) without hashing, the others go through the staged
+// pipeline (p252_hash_batch) and become present.
+int smtree_update_host(p252_ctx* ctx, p252_smtree* t, const MLayout& L, const uint64_t* pos, const uint8_t* op,
+                       const p252_fr* values, size_t n) {
+    const uint64_t A = (uint64_t)t->arity;
+    std::vector<uint32_t> ord(n);
+    for (size_t i = 0; i < n; ++i) ord[i] = (uint32_t)i;
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return pos[a] < pos[b]; });
+    std::vector<uint64_t> d;
+    d.reserve(n);
+    for (size_t i = 0; i < n; ++i) {
+        if (i + 1 < n && pos[ord[i + 1]] == pos[ord[i]]) continue;   // a later operation on the same position wins
+        const uint64_t j = pos[ord[i]];
+        const bool insert = !op || op[ord[i]] == 0;
+        if (insert)
+            t->leaves[j] = values[ord[i]];
+        else
+            memset(&t->leaves[j], 0, sizeof(p252_fr));
+        t->present[j] = insert ? 1 : 0;
+        d.push_back(j);
+    }
+    const p252_fr* below = t->leaves;
+    const uint8_t* below_p = t->present;
+    uint8_t* node_p = t->present + L.slots[0];
+    std::vector<p252_fr> groups, out;
+    std::vector<uint64_t> live;
+    for (int l = 1; l <= t->height; ++l) {
+        size_t k = 0;
+        for (size_t i = 0; i < d.size(); ++i) {
+            const uint64_t par = d[i] / A;
+            if (k == 0 || d[k - 1] != par) d[k++] = par;
+        }
+        d.resize(k);
+        p252_fr* level = t->nodes + L.off[l];
+        uint8_t* level_p = node_p + L.off[l];
+        live.clear();
+        groups.clear();
+        for (size_t i = 0; i < k; ++i) {
+            bool any = false;
+            for (uint64_t q = 0; q < A; ++q) any = any || below_p[d[i] * A + q];
+            if (any) {
+                live.push_back(d[i]);
+                groups.insert(groups.end(), below + d[i] * A, below + d[i] * A + A);
+            } else {
+                memset(&level[d[i]], 0, sizeof(p252_fr));
+                level_p[d[i]] = 0;
+            }
+        }
+        out.resize(live.size());
+        if (!live.empty()) {
+            int rc = p252_hash_batch(ctx, merkle_domain(t->arity), groups.data(), live.size(), A, out.data(), 1, P252_MEM_HOST);
+            if (rc != P252_OK) return rc;
+        }
+        for (size_t i = 0; i < live.size(); ++i) {
+            level[live[i]] = out[i];
+            level_p[live[i]] = 1;
+        }
+        below = level;
+        below_p = level_p;
+    }
+    return P252_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int p252_smtree_build(p252_ctx* ctx, p252_smtree* tree, int flags) {
+    MLayout L;
+    if (!ctx) return P252_ERR_INVALID_ARGUMENT;
+    int rc = smtree_check(tree, flags, &L);
+    if (rc != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (flags & P252_MEM_DEVICE) {
+        if ((rc = smtree_build_device(ctx, tree, L)) != P252_OK) return rc;
+        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        return P252_OK;
+    }
+    // HOST: stage the leaves and their presence bytes, build on the device, copy leaves, nodes and presence back
+    const size_t leaf_b = L.slots[0] * sizeof(p252_fr), node_b = L.node_slots * sizeof(p252_fr);
+    const size_t pres_b = L.slots[0] + L.node_slots;
+    uint8_t* base = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), leaf_b + node_b + pres_b, ctx->stream));
+    p252_smtree dt = *tree;
+    dt.leaves = reinterpret_cast<p252_fr*>(base);
+    dt.nodes = reinterpret_cast<p252_fr*>(base + leaf_b);
+    dt.present = base + leaf_b + node_b;
+    cudaError_t e = cudaMemcpyAsync(dt.leaves, tree->leaves, leaf_b, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dt.present, tree->present, L.slots[0], cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) {
+        rc = fail_cuda(ctx, e, "smtree staging");
+    } else {
+        rc = smtree_build_device(ctx, &dt, L);
+        if (rc == P252_OK) {
+            e = cudaMemcpyAsync(tree->leaves, dt.leaves, leaf_b, cudaMemcpyDeviceToHost, ctx->stream);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->nodes, dt.nodes, node_b, cudaMemcpyDeviceToHost, ctx->stream);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->present, dt.present, pres_b, cudaMemcpyDeviceToHost, ctx->stream);
+            if (e != cudaSuccess) rc = fail_cuda(ctx, e, "smtree D2H");
+        }
+    }
+    cudaFreeAsync(base, ctx->stream);
+    e = cudaStreamSynchronize(ctx->stream);
+    if (rc != P252_OK) return rc;
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "smtree build");
+    return P252_OK;
+}
+
+int p252_smtree_update(p252_ctx* ctx, p252_smtree* tree, const uint64_t* pos, const uint8_t* op, const p252_fr* values,
+                       size_t n, size_t* n_rejected, int flags) {
+    MLayout L;
+    if (!ctx || (n && (!pos || !values))) return P252_ERR_INVALID_ARGUMENT;
+    int rc = smtree_check(tree, flags, &L);
+    if (rc != P252_OK) return rc;
+    if (n >= 0x80000000ull) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_rejected) *n_rejected = 0;
+    if (flags & P252_MEM_DEVICE) {
+        if (n && (!aligned16(values) || (reinterpret_cast<uintptr_t>(pos) & 7))) return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        rc = smtree_update_device(ctx, tree, L, pos, op, values, (uint32_t)n, n_rejected);
+        if (rc != P252_OK) return rc;
+        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        return P252_OK;
+    }
+    for (size_t i = 0; i < n; ++i)
+        if (pos[i] >= tree->capacity || (op && op[i] > 1)) return P252_ERR_INVALID_ARGUMENT;
+    if (n == 0) return P252_OK;
+    return smtree_update_host(ctx, tree, L, pos, op, values, n);
+}
+
+int p252_smtree_len(p252_ctx* ctx, const p252_smtree* tree, uint64_t* n_present, int flags) {
+    MLayout L;
+    if (!ctx || !n_present) return P252_ERR_INVALID_ARGUMENT;
+    int rc = smtree_check(tree, flags, &L);
+    if (rc != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    *n_present = 0;
+    if (flags & P252_MEM_DEVICE) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        cudaError_t le = p252::launch_smtree_count(tree->present, tree->capacity, ctx->d_counter, ctx->stream);
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        if ((rc = counter_end(ctx, reinterpret_cast<size_t*>(n_present))) != P252_OK) return rc;
+        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        return P252_OK;
+    }
+    uint64_t c = 0;   // HOST: the bytes are already here
+    for (uint64_t j = 0; j < tree->capacity; ++j) c += tree->present[j] != 0;
+    *n_present = c;
+    return P252_OK;
+}
+
+int p252_smtree_open_batch(p252_ctx* ctx, const p252_smtree* tree, const uint64_t* pos, size_t n, p252_fr* paths_out,
+                           int flags) {
+    MLayout L;
+    if (!ctx || ((!pos || !paths_out) && n)) return P252_ERR_INVALID_ARGUMENT;
+    int rc = smtree_check(tree, flags, &L);
+    if (rc != P252_OK) return rc;
+    const int A = tree->arity, H = tree->height;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(paths_out) || (reinterpret_cast<uintptr_t>(pos) & 7)) return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        p252::OpenLevels lv{};                          // every slot: absent slots are already zero in memory
+        for (int l = 0; l < H; ++l) {
+            lv.off[l] = L.off[l];
+            lv.m[l] = L.slots[l];
+        }
+        lv.m[0] = tree->capacity;
+        return finish_device_call(ctx, p252::launch_merkle_open(tree->leaves, tree->nodes, pos, n, A, (uint32_t)H, lv, paths_out,
+                                                                ctx->stream, tree->present), flags);
+    }
+    for (size_t i = 0; i < n; ++i)
+        if (pos[i] >= tree->capacity || !tree->present[pos[i]]) return P252_ERR_INVALID_ARGUMENT;
+    const size_t Az = (size_t)A;
+    for (size_t i = 0; i < n; ++i) {
+        uint64_t j = pos[i];
+        for (int l = 0; l < H; ++l) {
+            const uint64_t group = j / Az;
+            const p252_fr* src = (l == 0 ? tree->leaves : tree->nodes + L.off[l]) + group * Az;
+            memcpy(paths_out + (i * (size_t)H + (size_t)l) * Az, src, Az * sizeof(p252_fr));
             j = group;
         }
     }

@@ -382,10 +382,13 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) k_crypt(FrArg tag, const
 // whole sibling group of the path node: the `arity` items at positions [g*arity, (g+1)*arity) of level l, with
 // g = i / arity^(l+1); the path node itself sits at offset (i / arity^l) % arity inside its group.  Slots at or beyond
 // m[l] are written as zero (the empty-slot rule, src/hash.rs:24-26).
-// k_merkle_open: pure gather, one thread per (opening, level).
+// k_merkle_open: pure gather, one thread per (opening, level).  kPresence (p252_smtree): the leaf must also be present
+// (present[idx] != 0), otherwise the opening is all zero.
+template <bool kPresence>
 __global__ void __launch_bounds__(256) k_merkle_open(const uint8_t* __restrict__ leaves, const uint8_t* __restrict__ nodes,
                                                      const uint64_t* __restrict__ leaf_idx, size_t n, uint32_t log2_arity,
-                                                     uint32_t depth, OpenLevels lv, uint8_t* __restrict__ paths) {
+                                                     uint32_t depth, OpenLevels lv, uint8_t* __restrict__ paths,
+                                                     const uint8_t* __restrict__ present) {
     const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n * depth) return;
     const size_t item = t / depth;
@@ -393,7 +396,7 @@ __global__ void __launch_bounds__(256) k_merkle_open(const uint8_t* __restrict__
     const uint32_t arity = 1u << log2_arity;
     const uint64_t idx = leaf_idx[item];
     uint4* dst = reinterpret_cast<uint4*>(paths + ((size_t)item * depth + level) * arity * 32);
-    if (idx >= lv.m[0]) {                                 // HOST buffers are rejected on the host; a device index outside
+    if (idx >= lv.m[0] || (kPresence && !present[idx])) { // HOST buffers are rejected on the host; a device index outside
         for (uint32_t q = 0; q < arity * 2; ++q)          // the prefix gets an all-zero opening (it cannot verify)
             dst[q] = make_uint4(0, 0, 0, 0);
         return;
@@ -474,10 +477,21 @@ __global__ void __launch_bounds__(256) k_mtree_parents(const uint64_t* __restric
 // aligned 32*arity-byte segments, so the warp tile still moves complete segments (4 x 128 B per LDG.128 for arity 4).
 // 4 resident blocks per SM (128 registers): a dirty set is rarely more than one wave, and at kMinBlocks' 96 registers
 // the permutation spills.
-template <int kLog2Arity>
+// kSparse (p252_smtree): presence bytes ride along -- below_present / level_present are indexed like below / level.  A
+// group whose arity presence bytes are all zero is empty: its node stores value 0 and presence 0; any other node stores
+// its digest and presence 1.  A warp whose groups are all empty skips the permutation.  Each node's value and presence
+// byte are written only by the lane that owns the node.
+__device__ __forceinline__ bool group_present(const uint8_t* p, uint32_t arity) {
+    // per-level slot counts are multiples of the arity: a group's presence bytes are one aligned 16- or 32-bit word
+    return arity == 4 ? *reinterpret_cast<const uint32_t*>(p) != 0u : *reinterpret_cast<const uint16_t*>(p) != 0u;
+}
+
+template <int kLog2Arity, bool kSparse>
 __global__ void __launch_bounds__(kThreads, 4) k_mtree_digest(FrArg tag, const uint8_t* __restrict__ below,
                                                                        uint8_t* __restrict__ level, const uint64_t* __restrict__ d,
-                                                                       const int* __restrict__ cnt) {
+                                                                       const int* __restrict__ cnt,
+                                                                       const uint8_t* __restrict__ below_present,
+                                                                       uint8_t* __restrict__ level_present) {
     constexpr int kArity = 1 << kLog2Arity;
     __shared__ uint4 stage[kWarps][32][8];
     P252_STAGE_TABLES
@@ -489,6 +503,8 @@ __global__ void __launch_bounds__(kThreads, 4) k_mtree_digest(FrArg tag, const u
     const int nitems = (n - item0 < 32) ? (int)(n - item0) : 32;
     uint4(*st)[8] = stage[warp];
     const uint64_t mine = d[item0 + (lane < nitems ? lane : 0)];
+    bool any = true;
+    if (kSparse) any = group_present(below_present + mine * kArity, kArity);
     const int part = lane & 7;
 #pragma unroll
     for (int r = 0; r < 8; ++r) {                          // warp_gather with a per-item base address
@@ -518,14 +534,27 @@ __global__ void __launch_bounds__(kThreads, 4) k_mtree_digest(FrArg tag, const u
     }
 #pragma unroll
     for (int k = 0; k < 8; ++k) s[0][k] = tag.l[k];
+    if (kSparse) {
+        if (__any_sync(0xffffffffu, any && lane < nitems)) hades_permute(s, 0x2u P252_TAB_PASS);
+        if (lane < nitems) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s[1][k] = any ? s[1][k] : 0u;
+            store_fr(level + mine * 32, s[1]);
+            level_present[mine] = any ? 1 : 0;
+        }
+        return;
+    }
     hades_permute(s, 0x2u P252_TAB_PASS);                  // a Merkle digest reads lane 1 only
     if (lane < nitems) store_fr(level + mine * 32, s[1]);
 }
 
 // the same for small dirty sets: five threads per item (hades_permute_coop), as k_sponge_digest_coop
+template <bool kSparse>
 __global__ void __launch_bounds__(kThreads) k_mtree_digest_coop(FrArg tag, const uint8_t* __restrict__ below, uint32_t arity,
                                                                 uint8_t* __restrict__ level, const uint64_t* __restrict__ d,
-                                                                const int* __restrict__ cnt) {
+                                                                const int* __restrict__ cnt,
+                                                                const uint8_t* __restrict__ below_present,
+                                                                uint8_t* __restrict__ level_present) {
     const int lane = threadIdx.x & 31;
     const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
     const size_t n = (size_t)*cnt;
@@ -547,8 +576,99 @@ __global__ void __launch_bounds__(kThreads) k_mtree_digest_coop(FrArg tag, const
 #pragma unroll
         for (int k = 0; k < 8; ++k) s[k] = t[k];
     }
-    hades_permute_coop(s, li, g0, crow);
+    hades_permute_coop(s, li, g0, crow);                          // collective: every thread of the warp takes part
+    if (kSparse) {
+        if (live && li == 1) {
+            const bool any = group_present(below_present + g * arity, arity);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s[k] = any ? s[k] : 0u;
+            store_fr(level + g * 32, s);
+            level_present[g] = any ? 1 : 0;
+        }
+        return;
+    }
     if (live && li == 1) store_fr(level + g * 32, s);
+}
+
+// ---- sparse fixed-height trees: inserts and removals at any position (p252_smtree) -----------------------------------
+// The climb is the one of p252_mtree_update (k_mtree_parents, DeviceSelect::Flagged) with the kSparse digest; presence
+// bytes are laid out like the scalars (leaves, then nodes).
+//
+// k_smtree_keys: one thread per batch item.  key = pos[i] for a valid item (pos < capacity, op 0 or 1), the sentinel
+// `capacity` otherwise (sorted last, skipped, counted into *rejected with one atomic per warp); bpos[i] = i.
+__global__ void __launch_bounds__(256) k_smtree_keys(const uint64_t* __restrict__ pos, const uint8_t* __restrict__ op,
+                                                     uint32_t n, uint64_t capacity, uint64_t* __restrict__ keys,
+                                                     uint32_t* __restrict__ bpos, unsigned long long* __restrict__ rejected) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t key = pos[i];
+    const bool bad = key >= capacity || (op && op[i] > 1);
+    keys[i] = bad ? capacity : key;
+    bpos[i] = i;
+    if (rejected) {
+        const unsigned act = __activemask();
+        const unsigned b = __ballot_sync(act, bad);
+        if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(b));
+    }
+}
+
+// k_smtree_leaf_write: over the keys sorted stably by position, the last item of every run of equal keys (the last
+// operation in batch order) applies its op: insert (op 0, or no op array) stores its value and presence 1, remove
+// (op 1) stores zero and presence 0.  Emits the level-1 candidates as k_mtree_leaf_write does.
+__global__ void __launch_bounds__(256) k_smtree_leaf_write(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ bpos,
+                                                           uint32_t n, uint64_t sentinel, uint32_t log2_arity,
+                                                           const uint8_t* __restrict__ op, const uint8_t* __restrict__ values,
+                                                           uint8_t* __restrict__ leaves, uint8_t* __restrict__ present,
+                                                           uint8_t* __restrict__ flag, uint64_t* __restrict__ parent) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t key = keys[i];
+    const bool valid = key != sentinel;
+    if (valid && (i + 1 == n || keys[i + 1] != key)) {
+        const uint32_t p = bpos[i];
+        const bool insert = !op || op[p] == 0;
+        uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        if (insert) load_fr(v, values + (size_t)p * 32);
+        store_fr(leaves + key * 32, v);
+        present[key] = insert ? 1 : 0;
+    }
+    const uint64_t par = key >> log2_arity;
+    flag[i] = valid && (i == 0 || (keys[i - 1] >> log2_arity) != par);
+    parent[i] = par;
+}
+
+// k_smtree_seed (build): one thread per leaf group g.  Normalises the group's presence bytes (a slot is present iff its
+// byte is non-zero and it lies below capacity), zeroes the value of every absent leaf, and makes the group a level-1
+// candidate iff one of its leaves is present: flag[g], parent[g] = g.
+__global__ void __launch_bounds__(256) k_smtree_seed(uint8_t* __restrict__ present, uint8_t* __restrict__ leaves, uint64_t groups,
+                                                     uint64_t capacity, uint32_t log2_arity, uint8_t* __restrict__ flag,
+                                                     uint64_t* __restrict__ parent) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= groups) return;
+    const uint32_t arity = 1u << log2_arity;
+    bool any = false;
+    for (uint32_t q = 0; q < arity; ++q) {
+        const uint64_t j = g * arity + q;
+        const bool p = j < capacity && present[j] != 0;
+        present[j] = p ? 1 : 0;
+        any = any || p;
+        if (!p) {
+            const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            store_fr(leaves + j * 32, zero);
+        }
+    }
+    flag[g] = any;
+    parent[g] = g;
+}
+
+// k_smtree_count: *out += number of non-zero bytes in present[0, n) (grid-stride, one atomic per warp)
+__global__ void __launch_bounds__(256) k_smtree_count(const uint8_t* __restrict__ present, uint64_t n,
+                                                      unsigned long long* __restrict__ out) {
+    unsigned c = 0;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+        c += present[i] != 0;
+    c = __reduce_add_sync(0xffffffffu, c);
+    if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
 // k_merkle_verify: one thread per opening, `depth` chained Merkle digests (Hash::digest(Domain::MerkleA, group),
@@ -905,13 +1025,17 @@ cudaError_t launch_decrypt(const uint64_t tag[4], const void* cipher, size_t n, 
 }
 
 cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint64_t* leaf_idx, size_t n, int arity,
-                               uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st) {
+                               uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st, const uint8_t* present) {
     if (n == 0 || depth == 0) return cudaSuccess;
     const size_t total = n * depth;
-    k_merkle_open<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(static_cast<const uint8_t*>(leaves),
-                                                                   static_cast<const uint8_t*>(nodes), leaf_idx, n,
-                                                                   arity == 4 ? 2u : 1u, depth, lv,
-                                                                   static_cast<uint8_t*>(paths));
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    const uint8_t* l = static_cast<const uint8_t*>(leaves);
+    const uint8_t* o = static_cast<const uint8_t*>(nodes);
+    const uint32_t la = arity == 4 ? 2u : 1u;
+    if (present)
+        k_merkle_open<true><<<grid, 256, 0, st>>>(l, o, leaf_idx, n, la, depth, lv, static_cast<uint8_t*>(paths), present);
+    else
+        k_merkle_open<false><<<grid, 256, 0, st>>>(l, o, leaf_idx, n, la, depth, lv, static_cast<uint8_t*>(paths), nullptr);
     return cudaGetLastError();
 }
 
@@ -947,12 +1071,63 @@ cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int ar
     uint8_t* o = static_cast<uint8_t*>(level);
     if (bound <= coop_max) {
         const size_t warps = (bound + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_mtree_digest_coop<<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(to_arg(tag), b, (uint32_t)arity, o, d, cnt);
+        k_mtree_digest_coop<false><<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(to_arg(tag), b, (uint32_t)arity, o,
+                                                                                                  d, cnt, nullptr, nullptr);
     } else if (arity == 4) {
-        k_mtree_digest<2><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt);
+        k_mtree_digest<2, false><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, nullptr, nullptr);
     } else {
-        k_mtree_digest<1><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt);
+        k_mtree_digest<1, false><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, nullptr, nullptr);
     }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_smtree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t capacity, uint64_t* keys,
+                               uint32_t* bpos, unsigned long long* rejected, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_smtree_keys<<<(n + 255) / 256, 256, 0, st>>>(pos, op, n, capacity, keys, bpos, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_smtree_leaf_write(const uint64_t* keys, const uint32_t* bpos, uint32_t n, uint64_t sentinel, int arity,
+                                     const uint8_t* op, const void* values, void* leaves, uint8_t* present, uint8_t* flag,
+                                     uint64_t* parent, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_smtree_leaf_write<<<(n + 255) / 256, 256, 0, st>>>(keys, bpos, n, sentinel, arity == 4 ? 2u : 1u, op,
+                                                         static_cast<const uint8_t*>(values), static_cast<uint8_t*>(leaves),
+                                                         present, flag, parent);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_smtree_seed(uint8_t* present, void* leaves, uint64_t groups, uint64_t capacity, int arity, uint8_t* flag,
+                               uint64_t* parent, cudaStream_t st) {
+    if (groups == 0) return cudaSuccess;
+    k_smtree_seed<<<(unsigned)((groups + 255) / 256), 256, 0, st>>>(present, static_cast<uint8_t*>(leaves), groups, capacity,
+                                                                    arity == 4 ? 2u : 1u, flag, parent);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_smtree_digest(const uint64_t tag[4], const void* below, const uint8_t* below_present, int arity, void* level,
+                                 uint8_t* level_present, const uint64_t* d, const int* cnt, size_t bound, size_t coop_max,
+                                 cudaStream_t st) {
+    if (bound == 0) return cudaSuccess;
+    const uint8_t* b = static_cast<const uint8_t*>(below);
+    uint8_t* o = static_cast<uint8_t*>(level);
+    if (bound <= coop_max) {
+        const size_t warps = (bound + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
+        k_mtree_digest_coop<true><<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(
+            to_arg(tag), b, (uint32_t)arity, o, d, cnt, below_present, level_present);
+    } else if (arity == 4) {
+        k_mtree_digest<2, true><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, below_present, level_present);
+    } else {
+        k_mtree_digest<1, true><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, below_present, level_present);
+    }
+    return cudaGetLastError();
+}
+
+cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned long long* out, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const uint64_t blocks = (n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096;
+    k_smtree_count<<<(unsigned)blocks, 256, 0, st>>>(present, n, out);
     return cudaGetLastError();
 }
 

@@ -25,8 +25,10 @@ struct OpenLevels {
     uint64_t off[kMaxDepth];
     uint64_t m[kMaxDepth];
 };
+// present (optional, p252_smtree): leaf idx must also have present[idx] != 0, otherwise its opening is all zero
 cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint64_t* leaf_idx, size_t n, int arity,
-                               uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st);
+                               uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st,
+                               const uint8_t* present = nullptr);
 // Fixed-height tree updates (p252_mtree_update).  keys: overwrite i -> idx[i] (>= n_old: sentinel n_new, counted into
 // *rejected), append j -> n_old + j; pos[i] = i
 cudaError_t launch_mtree_keys(const uint64_t* idx, uint32_t n_upd, uint64_t n_old, uint32_t total, uint64_t* keys,
@@ -42,6 +44,25 @@ cudaError_t launch_mtree_parents(const uint64_t* d, const int* cnt, uint32_t bou
 // when bound <= coop_max
 cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int arity, void* level, const uint64_t* d,
                                 const int* cnt, size_t bound, size_t coop_max, cudaStream_t st);
+// Sparse fixed-height trees (p252_smtree).  keys: pos[i] for a valid item (pos < capacity, op NULL or 0/1), else the
+// sentinel `capacity` (counted into *rejected); bpos[i] = i
+cudaError_t launch_smtree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t capacity, uint64_t* keys,
+                               uint32_t* bpos, unsigned long long* rejected, cudaStream_t st);
+// over stably sorted (keys, bpos): the last op per key is applied (insert: value + presence 1, remove: zero + presence 0);
+// level-1 candidates flag / parent = key / arity
+cudaError_t launch_smtree_leaf_write(const uint64_t* keys, const uint32_t* bpos, uint32_t n, uint64_t sentinel, int arity,
+                                     const uint8_t* op, const void* values, void* leaves, uint8_t* present, uint8_t* flag,
+                                     uint64_t* parent, cudaStream_t st);
+// build: normalise leaf presence (slots >= capacity absent), zero absent leaves, flag[g] = group g has a present leaf,
+// parent[g] = g, for the `groups` leaf groups
+cudaError_t launch_smtree_seed(uint8_t* present, void* leaves, uint64_t groups, uint64_t capacity, int arity, uint8_t* flag,
+                               uint64_t* parent, cudaStream_t st);
+// launch_mtree_digest with presence: an empty group stores value 0 / presence 0, any other its digest / presence 1
+cudaError_t launch_smtree_digest(const uint64_t tag[4], const void* below, const uint8_t* below_present, int arity, void* level,
+                                 uint8_t* level_present, const uint64_t* d, const int* cnt, size_t bound, size_t coop_max,
+                                 cudaStream_t st);
+// *out += non-zero bytes of present[0, n)
+cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned long long* out, cudaStream_t st);
 cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], const void* leaf_items,
                                  const uint64_t* leaf_idx, const void* paths, size_t n, int arity, uint32_t depth,
                                  uint8_t* ok, unsigned long long* n_failed, cudaStream_t st);

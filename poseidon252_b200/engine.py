@@ -36,7 +36,7 @@ class Engine:
         self._dist = False
         self._stream_handle = None if stream is None else int(stream)
         # failure / rejection counters of async device calls: a host function on the stream writes through them, so
-        # every one stays alive until sync() or close()
+        # every one stays alive until sync() or close() (as do temporaries an async call made for the device to read)
         self._pending_counters = []
 
     def _fence_torch(self):
@@ -479,6 +479,95 @@ class Engine:
         res = self._out_like(keep[0], shape) if out is None else self._check_out(out, shape, keep[0])
         self._check(self._lib.p252_mtree_open_batch(self._ctx, ctypes.byref(t), ip, n, self._ptr(res),
                                                     flags | (_native.ASYNC if async_ and flags else 0)))
+        return res
+
+    # -- sparse fixed-height trees: inserts and removals at any position (p252_smtree) -----------------------------
+    def _bytes(self, x, like, name, n, writable=False):
+        """A 1-D uint8 buffer of n entries in the memory space of `like` -> (pointer, keepalive).  writable: the library
+        writes through it, so a host buffer must be the caller's own C-contiguous array (no copy is made)."""
+        if _is_torch(like):
+            if not _is_torch(x) or not x.is_cuda or x.device != like.device or str(x.dtype) != "torch.uint8" or \
+                    not x.is_contiguous() or tuple(x.shape) != (n,):
+                raise EngineError(-1, "%s must be a contiguous uint8 tensor of shape (%d,) on %s" % (name, n, like.device))
+            return x.data_ptr(), x
+        if writable:
+            if not isinstance(x, np.ndarray) or x.dtype != np.uint8 or tuple(x.shape) != (n,) or not x.flags.c_contiguous \
+                    or not x.flags.writeable:
+                raise EngineError(-1, "%s must be a writable C-contiguous uint8 array of shape (%d,)" % (name, n))
+            return x.ctypes.data, x
+        if _is_torch(x):
+            raise EngineError(-1, "%s must be a host array like the tree's buffers" % name)
+        a = np.ascontiguousarray(x, dtype=np.uint8).reshape(-1)
+        if a.shape != (n,):
+            raise EngineError(-1, "%s must have %d entries" % (name, n))
+        return a.ctypes.data, a
+
+    def _smtree(self, tree):
+        """tree: anything with arity / height / capacity / leaves (leaf_slots, 4) / nodes (node_slots, 4) / present
+        (leaf_slots + node_slots,) uint8 -> (p252_smtree, flags, keepalive)."""
+        leaf_slots, node_slots, _ = self.mtree_layout(tree.arity, tree.height, tree.capacity)
+        lp, llead, flags, lk = self._in(tree.leaves, (4,))
+        np_, nlead, f2, nk = self._in(tree.nodes, (4,))
+        if flags != f2:
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("leaves", llead, leaf_slots)
+        self._same_lead("nodes", nlead, node_slots)
+        if not _is_torch(lk) and (lk is not tree.leaves or nk is not tree.nodes or not lk.flags.writeable or not nk.flags.writeable):
+            raise EngineError(-1, "host tree buffers must be writable C-contiguous uint64 arrays")
+        pp, pk = self._bytes(tree.present, lk, "present", leaf_slots + node_slots, writable=True)
+        t = _native.SMTree(ctypes.sizeof(_native.SMTree), int(tree.arity), int(tree.height), 0, int(tree.capacity), lp, np_, pp)
+        return t, flags, (lk, nk, pk)
+
+    def smtree_build(self, tree, async_=False):
+        """Rebuild every node (and node presence byte) of the sparse tree from its leaves and leaf presence bytes; absent
+        leaves are zeroed.  Only present nodes are hashed."""
+        t, flags, keep = self._smtree(tree)
+        self._check(self._lib.p252_smtree_build(self._ctx, ctypes.byref(t), flags | (_native.ASYNC if async_ and flags else 0)))
+
+    def smtree_update(self, tree, pos, values=None, op=None, async_=False):
+        """One batch of operations on a sparse tree: op[i] = 0 inserts / overwrites values[i] at pos[i], op[i] = 1 removes
+        pos[i] (op None: all inserts; values None: all zeros, for a batch of removals).  Equal to applying them in batch
+        order.  Device items with pos >= capacity or an op other than 0/1 are skipped and counted
+        (last_smtree_rejected()); host ones raise."""
+        t, flags, keep = self._smtree(tree)
+        like = keep[0]
+        ip, n, ik = self._idx(pos, like, "pos")
+        if values is None:
+            values = self._out_like(like, (n, 4))
+            values[:] = 0
+            if async_ and flags:
+                self._pending_counters.append(values)      # read by the device after this call returns
+        vp, vlead, fv, vk = self._in(values, (4,))
+        if fv != flags:
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("values", vlead, n)
+        opp, ok_ = (None, None) if op is None else self._bytes(op, like, "op", n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._smrej = self._counter(flags)
+        self._check(self._lib.p252_smtree_update(self._ctx, ctypes.byref(t), ip if n else None, opp if n else None,
+                                                 vp if n else None, n, ctypes.byref(self._smrej), flags))
+
+    def last_smtree_rejected(self):
+        """Items of the last smtree_update skipped on the device (pos >= capacity or op not 0/1; sync() first after
+        async_)."""
+        return int(getattr(self, "_smrej", ctypes.c_size_t(0)).value)
+
+    def smtree_len(self, tree):
+        """Number of present positions (counted on the device for device buffers)."""
+        t, flags, keep = self._smtree(tree)
+        c = ctypes.c_uint64(0)
+        self._check(self._lib.p252_smtree_len(self._ctx, ctypes.byref(t), ctypes.byref(c), flags))
+        return int(c.value)
+
+    def smtree_open_batch(self, tree, pos, out=None, async_=False):
+        """Openings of the present positions `pos`: (n, height, arity, 4), absent slots zero; they verify with
+        merkle_verify_batch (depth = height).  Host: an absent position raises; device: it gets an all-zero opening."""
+        t, flags, keep = self._smtree(tree)
+        ip, n, ik = self._idx(pos, keep[0], "pos")
+        shape = (n, int(tree.height), int(tree.arity), 4)
+        res = self._out_like(keep[0], shape) if out is None else self._check_out(out, shape, keep[0])
+        self._check(self._lib.p252_smtree_open_batch(self._ctx, ctypes.byref(t), ip, n, self._ptr(res),
+                                                     flags | (_native.ASYNC if async_ and flags else 0)))
         return res
 
     def set_small_batch_max(self, max_items):

@@ -1,7 +1,8 @@
 """Merkle trees of Domain::Merkle4 / Merkle2 digests (node = Hash::digest(Domain::Merkle{A}, A children),
 src/hash.rs:22-31).  Tree logic itself left the reference crate in 0.29.0
-(CHANGELOG.md:164-168); only the node hash is defined there.  Dense builders (n_leaves = arity^k) and `Tree`, a
-fixed-height tree with batched appends and overwrites (p252_mtree)."""
+(CHANGELOG.md:164-168); only the node hash is defined there.  Dense builders (n_leaves = arity^k), `Tree`, a
+fixed-height tree with batched appends and overwrites (p252_mtree), and `SparseTree`, a fixed-height tree with batched
+inserts and removals at any position (p252_smtree)."""
 from .engine import _is_torch, default_engine
 
 
@@ -157,3 +158,81 @@ class Tree:
         else:
             branch, root = self.open(np.array([int(i)], dtype=np.uint64))[0], self.root
         return Opening(root, branch, int(i), arity=self.arity)
+
+
+class SparseTree:
+    """Sparse fixed-height tree of the poseidon-merkle `Tree<T, H, A>` shape with `insert` and `remove` at any position
+    (p252_smtree): each position in [0, capacity) is present or absent; an absent leaf and a node with no present leaf
+    below it are the zero scalar and are never hashed (src/hash.rs:24-26), a present leaf of value zero is not absent.
+    Buffers are numpy arrays (device=None) or CUDA tensors on cuda:`device`: `leaves` / `nodes` (int64 or uint64, laid
+    out as p252_mtree_layout says) and `present` (uint8, one byte per slot, leaves then nodes; `leaf_present` /
+    `node_present` are views).  Every absent slot belongs to the library.  With the present set [0, n) the buffers equal
+    those of a `Tree` holding n leaves."""
+
+    def __init__(self, arity, height, capacity, engine=None, device=None):
+        import numpy as np
+        self.engine = engine or default_engine(0 if device is None else int(device))
+        self.arity, self.height, self.capacity = int(arity), int(height), int(capacity)
+        leaf_slots, node_slots, self.level_offset = self.engine.mtree_layout(self.arity, self.height, self.capacity)
+        if device is None:
+            self.leaves = np.zeros((leaf_slots, 4), dtype=np.uint64)
+            self.nodes = np.zeros((node_slots, 4), dtype=np.uint64)
+            self.present = np.zeros((leaf_slots + node_slots,), dtype=np.uint8)
+        else:
+            import torch
+            dev = torch.device("cuda", int(device))
+            self.leaves = torch.zeros((leaf_slots, 4), dtype=torch.int64, device=dev)
+            self.nodes = torch.zeros((node_slots, 4), dtype=torch.int64, device=dev)
+            self.present = torch.zeros((leaf_slots + node_slots,), dtype=torch.uint8, device=dev)
+        self.leaf_present = self.present[:leaf_slots]
+        self.node_present = self.present[leaf_slots:]
+        # all-zero buffers are the empty tree (root 0)
+
+    def apply(self, pos, op, values, async_=False):
+        """One batch: op[i] = 0 inserts / overwrites values[i] at pos[i], op[i] = 1 removes pos[i]; the result equals
+        applying the operations in batch order."""
+        self.engine.smtree_update(self, pos, values=values, op=op, async_=async_)
+
+    def insert(self, pos, values, async_=False):
+        """leaves[pos[i]] = values[i], present (the last write to a position wins)."""
+        self.engine.smtree_update(self, pos, values=values, async_=async_)
+
+    def remove(self, pos, async_=False):
+        """Make the positions `pos` absent (removing an absent position does nothing)."""
+        if _is_torch(self.leaves):
+            import torch
+            op = torch.ones((len(pos),), dtype=torch.uint8, device=self.leaves.device)
+        else:
+            import numpy as np
+            op = np.ones((len(pos),), dtype=np.uint8)
+        self.engine.smtree_update(self, pos, op=op, async_=async_)
+        if async_ and _is_torch(op):
+            self.engine._pending_counters.append(op)          # read by the device after the call returns
+
+    def build(self, async_=False):
+        """Recompute every node from the leaves and `leaf_present` (e.g. after writing them directly)."""
+        self.engine.smtree_build(self, async_=async_)
+
+    @property
+    def root(self):
+        return self.nodes[-1]
+
+    def len(self):
+        """Number of present positions."""
+        return self.engine.smtree_len(self)
+
+    def __len__(self):
+        return self.len()
+
+    def contains(self, pos):
+        """Whether position `pos` holds a value."""
+        pos = int(pos)
+        if pos < 0 or pos >= self.capacity:
+            return False
+        return bool(int(self.leaf_present[pos]))
+
+    def open(self, pos, async_=False):
+        """Openings of the present positions `pos`: (n, height, arity, 4), absent slots zero."""
+        return self.engine.smtree_open_batch(self, pos, async_=async_)
+
+    opening = Tree.opening     # poseidon-merkle `Opening` of a present position (host arrays)
