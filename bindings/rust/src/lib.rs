@@ -106,6 +106,10 @@ extern "C" {
 mod smtree;
 pub use smtree::{p252_smtree, SparseTree};
 
+// Encrypt / decrypt batches over messages of different lengths: their own `extern "C"` block in crypt_varlen.rs (methods
+// on Engine).
+mod crypt_varlen;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

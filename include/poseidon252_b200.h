@@ -205,6 +205,46 @@ int p252_encrypt_batch(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, co
 int p252_decrypt_batch(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L, const p252_fr* secret_uv,
                        const p252_fr* nonce, p252_fr* msg, uint8_t* ok, size_t* n_failed, int flags);
 
+/* Variable-length encrypt / decrypt batches: one call for messages (ciphers) of any mix of lengths.
+ *   encrypt: cipher item i = encrypt(msg[offsets[i] .. offsets[i+1]), secret_uv[i], nonce[i]) (src/encryption.rs:62-74);
+ *   decrypt: message item i = decrypt(cipher[offsets[i] .. offsets[i+1]), secret_uv[i], nonce[i]) (src/encryption.rs:83-95).
+ *   Input: n_scalars scalars; offsets: n + 1 absolute indices into it (offsets[0] need not be 0, so a slice of a larger
+ *   CSR array works); secret_uv: n x 2 (JubJubAffine::get_u/get_v), nonce: n; n < 2^31; all buffers, offsets included,
+ *   in one memory space.  max_len bounds the message length L: 1 <= L <= max_len <= P252_VARLEN_MAX_LEN; a cipher has
+ *   L + 1 scalars.
+ *   Output: the input CSR with every item one scalar longer (encrypt) or shorter (decrypt), packed from 0.  With
+ *   a0 = offsets[0] and an = offsets[n], encrypt writes cipher item i to cipher[offsets[i] - a0 + i, offsets[i+1] - a0 +
+ *   i + 1) of an - a0 + n scalars; decrypt writes message item i to msg[offsets[i] - a0 - i, offsets[i+1] - a0 - i - 1)
+ *   of an - a0 - n scalars, and ok[i] (n bytes) as p252_decrypt_batch does: ok[i] = 0 <=> the reference returns
+ *   Error::DecryptionFailed, and that item's message is zeroed.  A decrypt output fed straight back into encrypt (and the
+ *   reverse) needs no second offsets array: its offsets are offsets[i] - a0 -+ i.
+ *   Batch checks, before anything runs: max_len == 0 or > P252_VARLEN_MAX_LEN, n >= 2^31, a NULL buffer with n > 0,
+ *   DEVICE data buffers not 16-byte or offsets not 8-byte aligned -> INVALID_ARGUMENT.
+ *   Item i (a = offsets[i], b = offsets[i+1]) is valid iff a0 <= a <= b <= an <= n_scalars and, for encrypt,
+ *   1 <= b - a <= max_len; for decrypt 2 <= b - a <= max_len + 1, a - a0 >= i and an - b >= n - 1 - i (its output range
+ *   lies inside msg; both hold by themselves when every item is valid).
+ *   HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written:
+ *   INVALID_ARGUMENT for a range outside the bounds or decreasing offsets, INVALID_IO_PATTERN for a message length of 0
+ *   or a cipher length below 2 (as p252_encryption_tag(0)), INVALID_ARGUMENT for a length above max_len (+1 for
+ *   decrypt).  The batch is then staged in chunks of about 24 MiB of input on the staging streams; secrets, nonces and
+ *   plaintext live only in the staging arenas, which are zeroed on every exit path.  *n_failed counts the ok[i] == 0.
+ *   DEVICE: offsets are not inspected on the host; an invalid item is skipped on the device and counted into
+ *   *n_rejected; nothing is written for it (its output position is not trustworthy), except ok[i] = 0 for decrypt.  No
+ *   offset value makes a kernel read outside in[0, n_scalars) or write outside the output range above.  *n_failed
+ *   counts authentication failures among valid items only.  With P252_ASYNC nothing is synchronised.
+ *   n_failed / n_rejected: optional HOST pointers for both memory spaces (*n_rejected is 0 for HOST calls), counted on
+ *   the device for DEVICE calls; lifetime as for p252_mtree_update.
+ * The tags of L = 1..max_len are derived on the host and kept on the device in the context (a table of their own, next
+ * to the one of p252_hash_batch_varlen); it is rebuilt only when max_len grows.  Items are sorted by length on the
+ * device so that a warp runs messages of (nearly) equal length together; batches of at most p252_set_small_batch_max
+ * items run the lane-split kernel. */
+int p252_encrypt_batch_varlen(p252_ctx* ctx, const p252_fr* msg, size_t n_scalars, const uint64_t* offsets, size_t n,
+                              size_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* cipher,
+                              size_t* n_rejected, int flags);
+int p252_decrypt_batch_varlen(p252_ctx* ctx, const p252_fr* cipher, size_t n_scalars, const uint64_t* offsets, size_t n,
+                              size_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* msg, uint8_t* ok,
+                              size_t* n_failed, size_t* n_rejected, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

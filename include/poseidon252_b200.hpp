@@ -8,7 +8,7 @@
 //   dusk_poseidon::{encrypt, decrypt}        (src/encryption.rs:62-95) -> p252::encrypt / p252::decrypt
 //   dusk_poseidon::Error                     (src/error.rs:11-32)      -> p252::Error (exception)
 //   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
-//   decrypt_batch, merkle4_build.
+//   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -210,6 +210,54 @@ inline std::vector<Scalar> decrypt_batch(const Scalar* cipher, size_t n, size_t 
     check(p252_decrypt_batch(e.get(), cipher, n, L, secrets_uv, nonces, msg.data(), ok.data(), nullptr, P252_MEM_HOST),
           e.get());
     return msg;
+}
+
+// NEW: encrypt / decrypt of messages of any lengths in one device call (p252_encrypt_batch_varlen /
+// p252_decrypt_batch_varlen); secrets n x 2, nonces n.  Throws Error for an invalid item (nothing computed).
+namespace detail {
+inline size_t pack(const std::vector<std::vector<Scalar>>& items, std::vector<Scalar>& data, std::vector<uint64_t>& offsets) {
+    size_t longest = 0;
+    offsets.assign(1, 0);
+    for (auto& it : items) {
+        data.insert(data.end(), it.begin(), it.end());
+        offsets.push_back(data.size());
+        longest = it.size() > longest ? it.size() : longest;
+    }
+    return longest;
+}
+}  // namespace detail
+
+inline std::vector<std::vector<Scalar>> encrypt_batch_varlen(const std::vector<std::vector<Scalar>>& messages,
+                                                             const Scalar* secrets_uv, const Scalar* nonces,
+                                                             Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> data;
+    std::vector<uint64_t> off;
+    const size_t longest = detail::pack(messages, data, off);
+    const size_t n = messages.size();
+    std::vector<Scalar> cipher(data.size() + n);
+    check(p252_encrypt_batch_varlen(e.get(), data.data(), data.size(), off.data(), n, longest ? longest : 1, secrets_uv, nonces,
+                                    cipher.data(), nullptr, P252_MEM_HOST),
+          e.get());
+    std::vector<std::vector<Scalar>> res(n);
+    for (size_t i = 0; i < n; ++i) res[i].assign(cipher.begin() + off[i] + i, cipher.begin() + off[i + 1] + i + 1);
+    return res;
+}
+// returns the messages; ok[i] == 0 marks items for which the reference returns DecryptionFailed (their message is zero)
+inline std::vector<std::vector<Scalar>> decrypt_batch_varlen(const std::vector<std::vector<Scalar>>& ciphers,
+                                                             const Scalar* secrets_uv, const Scalar* nonces,
+                                                             std::vector<uint8_t>& ok, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> data;
+    std::vector<uint64_t> off;
+    const size_t longest = detail::pack(ciphers, data, off);
+    const size_t n = ciphers.size();
+    std::vector<Scalar> msg(data.size() > n ? data.size() - n : 0);
+    ok.assign(n, 0);
+    check(p252_decrypt_batch_varlen(e.get(), data.data(), data.size(), off.data(), n, longest > 1 ? longest - 1 : 1, secrets_uv,
+                                    nonces, msg.data(), ok.data(), nullptr, nullptr, P252_MEM_HOST),
+          e.get());
+    std::vector<std::vector<Scalar>> res(n);
+    for (size_t i = 0; i < n; ++i) res[i].assign(msg.begin() + (off[i] - i), msg.begin() + (off[i + 1] - i - 1));
+    return res;
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

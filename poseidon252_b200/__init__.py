@@ -4,12 +4,14 @@ Public surface mirrors src/lib.rs:13-31:
     Hash, Domain, Error, HADES_WIDTH, encrypt, decrypt
 plus the batch entry points this engine adds:
     Hash.digest_batch, Hash.digest_batch_varlen (inputs of different lengths in one call), hades.permute_batch,
-    encrypt_batch, decrypt_batch, merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites),
-    SparseTree (fixed-height Merkle tree with batched inserts / removals at any position).
+    encrypt_batch, decrypt_batch, encrypt_batch_varlen / decrypt_batch_varlen (messages of different lengths in one call),
+    merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
+    with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
 from . import hades, merkle, scalar
-from .encryption import decrypt, decrypt_batch, encrypt, encrypt_batch
+from .encryption import (cipher_offsets, decrypt, decrypt_batch, decrypt_batch_varlen, encrypt, encrypt_batch,
+                         encrypt_batch_varlen, message_offsets)
 from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
@@ -19,6 +21,7 @@ from .merkle import SparseTree, Tree, merkle4_build, merkle4_level
 HADES_WIDTH = hades.WIDTH
 
 __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch", "pack_varlen",
+           "encrypt_batch_varlen", "decrypt_batch_varlen", "cipher_offsets", "message_offsets",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",
            "DecryptionFailed", "InvalidPoint", "EngineError"]

@@ -48,6 +48,18 @@ struct Slot {
     size_t arena_bytes = 0;
 };
 
+// A device table of per-length tags, tags[len] for len = 0..len (tags[0] = 0) of what `key` names, in a stream-ordered
+// allocation, uploaded from a pinned staging buffer whose last upload `ev` marks; staging buffers replaced while their
+// upload was still pending wait in `retired` until the context is destroyed.  Rebuilt by tag_table() (below).
+struct TagTable {
+    p252_fr* dev = nullptr;
+    p252_fr* host = nullptr;
+    std::vector<p252_fr*> retired;
+    size_t host_cap = 0, len = 0;
+    uint64_t key = 0;
+    cudaEvent_t ev = nullptr;
+};
+
 }  // namespace
 
 struct p252_ctx {
@@ -61,19 +73,15 @@ struct p252_ctx {
     std::string last_error;
     // calls on one context serialise (recursive: public entry points call each other)
     std::recursive_mutex mu;
-    // device-side failure counter (decrypt / opening verification on DEVICE buffers) + its pinned mirror
+    // device-side counters (decrypt failures / opening verification / rejected items on DEVICE buffers; slot 0 unless a
+    // call counts two things) + their pinned mirror
+    static constexpr int kCounters = 2;
     unsigned long long* d_counter = nullptr;
     unsigned long long* h_counter = nullptr;
     size_t coop_max = 0;          // small-batch threshold of the lane-split digest kernel
-    // tag table of p252_hash_batch_varlen: tags[len] for len = 0..vt_len of (vt_domain, vt_out_len) on the device
-    // (stream-ordered allocation), uploaded from a pinned staging buffer whose last upload ev_tags marks; staging
-    // buffers replaced while their upload was still pending wait in vt_retired until the context is destroyed
-    p252_fr* vt_dev = nullptr;
-    p252_fr* vt_host = nullptr;
-    std::vector<p252_fr*> vt_retired;
-    size_t vt_host_cap = 0, vt_len = 0, vt_out_len = 0;
-    int vt_domain = -1;
-    cudaEvent_t ev_tags = nullptr;
+    // per-length tag tables: p252_hash_batch_varlen (key = domain and out_len) and p252_{en,de}crypt_batch_varlen; two
+    // instances, so that alternating digest and encryption calls rebuild neither
+    TagTable vt, ct;
     // test hook: index of the staged chunk that fails in the next host-buffer call (-1 = none)
     long long fail_chunk = -1;
     // multi-GPU
@@ -175,6 +183,22 @@ struct Io {
 
 int join_slots(p252_ctx* ctx, int rc, bool wipe);
 
+// Grow a slot's arena to at least `need` bytes.  The old arena is released only after the slot stream has drained, and
+// is cleared first when it may hold secrets (wipe).
+int slot_reserve(p252_ctx* ctx, Slot& sl, size_t need, bool wipe) {
+    if (sl.arena_bytes >= need) return P252_OK;
+    CU(cudaStreamSynchronize(sl.stream));
+    if (sl.arena) {
+        if (wipe) CU(cudaMemset(sl.arena, 0, sl.arena_bytes));
+        CU(cudaFree(sl.arena));
+    }
+    sl.arena = nullptr;
+    sl.arena_bytes = 0;
+    CU(cudaMalloc(&sl.arena, need));
+    sl.arena_bytes = need;
+    return P252_OK;
+}
+
 // wipe = true: the staging arenas held secrets (shared secret, nonce, plaintext); they are cleared before
 // returning (the reference's dependencies zeroize sponge state, Cargo.toml:15,17 "zeroize").
 // Whatever happens inside the chunk loop, the common exit below runs: slot streams are joined back into the
@@ -205,17 +229,8 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
             // arena layout: one 256-byte aligned region per buffer
             size_t need = 0;
             for (auto& io : ios) need += (chunk * io.item_bytes + 255) / 256 * 256;
-            if (sl.arena_bytes < need) {
-                CU(cudaStreamSynchronize(sl.stream));
-                if (sl.arena) {
-                    if (wipe) CU(cudaMemset(sl.arena, 0, sl.arena_bytes));
-                    CU(cudaFree(sl.arena));
-                }
-                sl.arena = nullptr;
-                sl.arena_bytes = 0;
-                CU(cudaMalloc(&sl.arena, need));
-                sl.arena_bytes = need;
-            }
+            int rc = slot_reserve(ctx, sl, need, wipe);
+            if (rc != P252_OK) return rc;
             std::vector<void*> d(ios.size());
             size_t pos = 0;
             for (size_t b = 0; b < ios.size(); ++b) {
@@ -270,9 +285,9 @@ int finish_device_call(p252_ctx* ctx, cudaError_t le, int flags) {
     return P252_OK;
 }
 
-// DEVICE-buffer calls that count failures on the device: zero the counter before the launch ...
-int counter_begin(p252_ctx* ctx) {
-    CU(cudaMemsetAsync(ctx->d_counter, 0, sizeof(unsigned long long), ctx->stream));
+// DEVICE-buffer calls that count failures on the device: zero the first `count` counters before the launch ...
+int counter_begin(p252_ctx* ctx, int count = 1) {
+    CU(cudaMemsetAsync(ctx->d_counter, 0, count * sizeof(unsigned long long), ctx->stream));
     return P252_OK;
 }
 void CUDART_CB publish_counter(void* arg) {
@@ -282,10 +297,11 @@ void CUDART_CB publish_counter(void* arg) {
 }
 // ... and after it copy the counter to the pinned mirror and from there to the caller's size_t (a host function on
 // the stream, so that P252_ASYNC callers see it after p252_sync).
-int counter_end(p252_ctx* ctx, size_t* n_failed) {
+int counter_end(p252_ctx* ctx, size_t* n_failed, int slot = 0) {
     if (!n_failed) return P252_OK;
-    CU(cudaMemcpyAsync(ctx->h_counter, ctx->d_counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost, ctx->stream));
-    auto* pr = new std::pair<const unsigned long long*, size_t*>(ctx->h_counter, n_failed);
+    CU(cudaMemcpyAsync(ctx->h_counter + slot, ctx->d_counter + slot, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    auto* pr = new std::pair<const unsigned long long*, size_t*>(ctx->h_counter + slot, n_failed);
     cudaError_t e = cudaLaunchHostFunc(ctx->stream, publish_counter, pr);
     if (e != cudaSuccess) {
         delete pr;
@@ -386,13 +402,14 @@ int p252_create_on_stream(int device, void* cuda_stream, p252_ctx** out) {
     if ((e = cudaEventCreateWithFlags(&ctx->ev_comm, cudaEventDisableTiming)) != cudaSuccess)
         return bail(e, "cudaEventCreate");
     if ((e = cudaEventCreate(&ctx->ev_tree_end)) != cudaSuccess) return bail(e, "cudaEventCreate");
-    if ((e = cudaEventCreateWithFlags(&ctx->ev_tags, cudaEventDisableTiming)) != cudaSuccess)
-        return bail(e, "cudaEventCreate");
-    if ((e = cudaMalloc(reinterpret_cast<void**>(&ctx->d_counter), sizeof(unsigned long long))) != cudaSuccess)
+    for (TagTable* t : {&ctx->vt, &ctx->ct})
+        if ((e = cudaEventCreateWithFlags(&t->ev, cudaEventDisableTiming)) != cudaSuccess) return bail(e, "cudaEventCreate");
+    const size_t counter_bytes = p252_ctx::kCounters * sizeof(unsigned long long);
+    if ((e = cudaMalloc(reinterpret_cast<void**>(&ctx->d_counter), counter_bytes)) != cudaSuccess)
         return bail(e, "cudaMalloc");
-    if ((e = cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_counter), sizeof(unsigned long long), cudaHostAllocPortable)) != cudaSuccess)
+    if ((e = cudaHostAlloc(reinterpret_cast<void**>(&ctx->h_counter), counter_bytes, cudaHostAllocPortable)) != cudaSuccess)
         return bail(e, "cudaHostAlloc");
-    *ctx->h_counter = 0;
+    memset(ctx->h_counter, 0, counter_bytes);
     *out = ctx;
     return P252_OK;
 }
@@ -419,11 +436,14 @@ void p252_destroy(p252_ctx* ctx) {
     for (auto& le : ctx->level_events)
         for (cudaEvent_t ev : {le.k0, le.k1, le.g0, le.g1})
             if (ev) cudaEventDestroy(ev);
-    if (ctx->vt_dev) cudaFreeAsync(ctx->vt_dev, ctx->stream);
+    for (TagTable* t : {&ctx->vt, &ctx->ct})
+        if (t->dev) cudaFreeAsync(t->dev, ctx->stream);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);   // pending host functions reference h_counter
-    if (ctx->vt_host) cudaFreeHost(ctx->vt_host);
-    for (p252_fr* h : ctx->vt_retired) cudaFreeHost(h);
-    if (ctx->ev_tags) cudaEventDestroy(ctx->ev_tags);
+    for (TagTable* t : {&ctx->vt, &ctx->ct}) {
+        if (t->host) cudaFreeHost(t->host);
+        for (p252_fr* h : t->retired) cudaFreeHost(h);
+        if (t->ev) cudaEventDestroy(t->ev);
+    }
     if (ctx->d_counter) cudaFree(ctx->d_counter);
     if (ctx->h_counter) cudaFreeHost(ctx->h_counter);
     if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
@@ -1555,58 +1575,71 @@ int p252_smtree_open_batch(p252_ctx* ctx, const p252_smtree* tree, const uint64_
 // ---- variable-length digest batches (p252_hash_batch_varlen) ----------------------------------------------------
 namespace {
 
-// The device tag table for (domain, out_len) covering lengths 1..max_len: reused while it covers the call, otherwise
-// rebuilt on the host (BLAKE2b stays there) and uploaded on the context stream.  The replaced table is freed in stream
-// order, after every kernel already enqueued that reads it; the pinned staging buffer is rewritten only after its
-// previous upload has completed.  Lengths the domain refuses (a Merkle length other than the arity) get a zero tag:
-// k_varlen_keys rejects them before any kernel reads it.
-int varlen_tags(p252_ctx* ctx, int domain, size_t max_len, size_t out_len, const p252_fr** table) {
-    if (ctx->vt_dev && ctx->vt_domain == domain && ctx->vt_out_len == out_len && ctx->vt_len >= max_len) {
-        *table = ctx->vt_dev;
+// The device tag table of `t` for `key` covering lengths 1..max_len: reused while it covers the call, otherwise rebuilt
+// on the host (BLAKE2b stays there; fill(len, &tag) derives one tag, a failure leaves a zero tag) and uploaded on the
+// context stream.  The replaced table is freed in stream order, after every kernel already enqueued that reads it; the
+// pinned staging buffer is rewritten only after its previous upload has completed.
+template <typename Fill>
+int tag_table(p252_ctx* ctx, TagTable& t, uint64_t key, size_t max_len, Fill fill, const p252_fr** table) {
+    if (t.dev && t.key == key && t.len >= max_len) {
+        *table = t.dev;
         return P252_OK;
     }
-    if (ctx->vt_host) {
-        const cudaError_t q = cudaEventQuery(ctx->ev_tags);
+    if (t.host) {
+        const cudaError_t q = cudaEventQuery(t.ev);
         if (q == cudaErrorNotReady) {                      // still being read: retire it instead of waiting
-            ctx->vt_retired.push_back(ctx->vt_host);
-            ctx->vt_host = nullptr;
-            ctx->vt_host_cap = 0;
+            t.retired.push_back(t.host);
+            t.host = nullptr;
+            t.host_cap = 0;
         } else if (q != cudaSuccess) {
             return fail_cuda(ctx, q, "cudaEventQuery");
         }
     }
-    if (ctx->vt_host_cap < max_len + 1) {
-        if (ctx->vt_host) CU(cudaFreeHost(ctx->vt_host));
-        ctx->vt_host = nullptr;
-        ctx->vt_host_cap = 0;
-        CU(cudaHostAlloc(reinterpret_cast<void**>(&ctx->vt_host), (max_len + 1) * sizeof(p252_fr), cudaHostAllocPortable));
-        ctx->vt_host_cap = max_len + 1;
+    if (t.host_cap < max_len + 1) {
+        if (t.host) CU(cudaFreeHost(t.host));
+        t.host = nullptr;
+        t.host_cap = 0;
+        CU(cudaHostAlloc(reinterpret_cast<void**>(&t.host), (max_len + 1) * sizeof(p252_fr), cudaHostAllocPortable));
+        t.host_cap = max_len + 1;
     }
-    memset(&ctx->vt_host[0], 0, sizeof(p252_fr));
+    memset(&t.host[0], 0, sizeof(p252_fr));
     for (size_t len = 1; len <= max_len; ++len)
-        if (p252_hash_tag(domain, len, out_len, &ctx->vt_host[len]) != P252_OK) memset(&ctx->vt_host[len], 0, sizeof(p252_fr));
+        if (fill(len, &t.host[len]) != P252_OK) memset(&t.host[len], 0, sizeof(p252_fr));
     p252_fr* d = nullptr;
     CU(cudaMallocAsync(reinterpret_cast<void**>(&d), (max_len + 1) * sizeof(p252_fr), ctx->stream));
-    cudaError_t e = cudaMemcpyAsync(d, ctx->vt_host, (max_len + 1) * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaEventRecord(ctx->ev_tags, ctx->stream);
+    cudaError_t e = cudaMemcpyAsync(d, t.host, (max_len + 1) * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaEventRecord(t.ev, ctx->stream);
     if (e != cudaSuccess) {
         cudaFreeAsync(d, ctx->stream);
         return fail_cuda(ctx, e, "varlen tag table upload");
     }
-    if (ctx->vt_dev) CU(cudaFreeAsync(ctx->vt_dev, ctx->stream));
-    ctx->vt_dev = d;
-    ctx->vt_len = max_len;
-    ctx->vt_domain = domain;
-    ctx->vt_out_len = out_len;
+    if (t.dev) CU(cudaFreeAsync(t.dev, ctx->stream));
+    t.dev = d;
+    t.len = max_len;
+    t.key = key;
     *table = d;
     return P252_OK;
 }
 
-// One batch on `st`: keys (length or 0 = rejected) -> radix sort by length -> the varlen digest kernel.  Temporaries are
-// one stream-ordered allocation.
-int varlen_run(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, uint64_t base, uint64_t n_scalars, const uint64_t* offsets,
-               uint32_t n, uint32_t max_len, uint32_t fixed_len, p252_fr* out, uint32_t out_len, unsigned long long* rejected,
-               cudaStream_t st) {
+// Tags of Hash::digest for (domain, out_len), rebuilt only when max_len grows or (domain, out_len) changes.  Lengths the
+// domain refuses (a Merkle length other than the arity) get a zero tag: k_varlen_keys rejects them before any kernel
+// reads it.
+int varlen_tags(p252_ctx* ctx, int domain, size_t max_len, size_t out_len, const p252_fr** table) {
+    const uint64_t key = ((uint64_t)(uint32_t)domain << 32) | (uint64_t)out_len;   // out_len < 2^26
+    return tag_table(ctx, ctx->vt, key, max_len, [&](size_t len, p252_fr* tag) { return p252_hash_tag(domain, len, out_len, tag); },
+                     table);
+}
+
+// Tags of encrypt / decrypt (p252_encryption_tag) for message lengths 1..max_len, rebuilt only when max_len grows.
+int crypt_tags(p252_ctx* ctx, size_t max_len, const p252_fr** table) {
+    return tag_table(ctx, ctx->ct, 0, max_len, [](size_t len, p252_fr* tag) { return p252_encryption_tag(len, tag); }, table);
+}
+
+// One batch of n items on `st`: keys(keys, vals) writes each item's key (a length, or 0 = rejected) -> radix sort by key
+// over bits(max_len) -> run(lens, perm) launches the batch kernel over the sorted order.  Temporaries are one
+// stream-ordered allocation.
+template <typename Keys, typename Run>
+int varlen_sorted(p252_ctx* ctx, uint32_t n, uint32_t max_len, cudaStream_t st, Keys keys_launch, Run run_launch) {
     int end_bit = 1;
     while ((max_len >> end_bit) != 0) ++end_bit;            // keys <= max_len
     size_t sort_bytes = 0;
@@ -1621,12 +1654,12 @@ int varlen_run(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, uint64_t b
     uint32_t* lens = reinterpret_cast<uint32_t*>(tmp + 2 * arr);
     uint32_t* perm = reinterpret_cast<uint32_t*>(tmp + 3 * arr);
     auto body = [&]() -> int {
-        cudaError_t le = p252::launch_varlen_keys(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected, st);
+        cudaError_t le = keys_launch(keys, vals);
         if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
         ctx->launches++;
         size_t b = sort_bytes;
         CU(cub::DeviceRadixSort::SortPairs(tmp + 4 * arr, b, keys, lens, vals, perm, (int)n, 0, end_bit, st));
-        le = p252::launch_digest_varlen(tags, in, base, offsets, lens, perm, n, out, out_len, ctx->coop_max, st);
+        le = run_launch(lens, perm);
         if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
         ctx->launches++;
         return P252_OK;
@@ -1636,6 +1669,36 @@ int varlen_run(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, uint64_t b
     if (rc != P252_OK) return rc;
     if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
     return P252_OK;
+}
+
+// One digest batch on `st`: keys (length or 0 = rejected) -> radix sort by length -> the varlen digest kernel.
+int varlen_run(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, uint64_t base, uint64_t n_scalars, const uint64_t* offsets,
+               uint32_t n, uint32_t max_len, uint32_t fixed_len, p252_fr* out, uint32_t out_len, unsigned long long* rejected,
+               cudaStream_t st) {
+    return varlen_sorted(
+        ctx, n, max_len, st,
+        [&](uint32_t* keys, uint32_t* vals) {
+            return p252::launch_varlen_keys(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected, st);
+        },
+        [&](const uint32_t* lens, const uint32_t* perm) {
+            return p252::launch_digest_varlen(tags, in, base, offsets, lens, perm, n, out, out_len, ctx->coop_max, st);
+        });
+}
+
+// One encrypt / decrypt batch on `st` (see launch_crypt_varlen for the addressing; base = the value subtracted from the
+// offsets to address `in`, whose length is n_scalars).
+int crypt_run(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* in, uint64_t base, uint64_t n_scalars,
+              const uint64_t* offsets, uint32_t n, uint32_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* out,
+              uint8_t* ok, unsigned long long* failed, unsigned long long* rejected, cudaStream_t st) {
+    return varlen_sorted(
+        ctx, n, max_len, st,
+        [&](uint32_t* keys, uint32_t* vals) {
+            return p252::launch_crypt_varlen_keys(decrypt, offsets, n, base, n_scalars, max_len, keys, vals, rejected, st);
+        },
+        [&](const uint32_t* lens, const uint32_t* perm) {
+            return p252::launch_crypt_varlen(decrypt, tags, in, base, offsets, lens, perm, n, secret_uv, nonce, out, ok, failed,
+                                             ctx->coop_max, st);
+        });
 }
 
 // HOST batch (already validated): consecutive item ranges of about kChunkBytesTarget input bytes (a longer item is a
@@ -1685,6 +1748,61 @@ int varlen_host(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, const uin
     return join_slots(ctx, body(), false);
 }
 
+// HOST encrypt / decrypt batch (already validated, n > 0): consecutive item ranges of about kChunkBytesTarget input bytes
+// (a longer item is a chunk by itself, at most chunk_items_max() items) are staged on the slot streams and run by
+// crypt_run with base = the chunk's first offset s0.  Input, offsets, secrets, nonces, output and ok go through the slot
+// arenas -- never through stream-ordered allocations -- so that join_slots(wipe) clears every secret on every exit path.
+// Output of chunk [lo, hi): (ns +- cnt) scalars at out + (s0 - a0 +- lo), the chunk's part of the output CSR.
+int crypt_host(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n,
+               uint32_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* out, uint8_t* ok) {
+    const long long fail_at = ctx->fail_chunk;
+    ctx->fail_chunk = -1;                                  // one shot
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    std::vector<size_t> bounds = {0};                      // chunk k = items [bounds[k], bounds[k+1])
+    size_t need = 0;                                       // arena bytes of the largest chunk
+    for (size_t lo = 0, hi = 0; lo < n; lo = hi) {
+        hi = lo + 1;
+        while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * sizeof(p252_fr) <= kChunkBytesTarget) ++hi;
+        bounds.push_back(hi);
+        const size_t cnt = hi - lo, ns = offsets[hi] - offsets[lo];
+        need = std::max(need, up(ns * 32) + up((cnt + 1) * 8) + up(cnt * 64) + up(cnt * 32) + up((ns + cnt) * 32) + up(cnt));
+    }
+    auto body = [&]() -> int {
+        CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
+        for (int s = 0; s < kSlots; ++s) CU(cudaStreamWaitEvent(ctx->slots[s].stream, ctx->ev_fork, 0));
+        const uint64_t a0 = offsets[0];
+        for (size_t k = 0; k + 1 < bounds.size(); ++k) {
+            const size_t lo = bounds[k], hi = bounds[k + 1], cnt = hi - lo;
+            const uint64_t s0 = offsets[lo], ns = offsets[hi] - s0;
+            const size_t out_ns = decrypt ? ns - cnt : ns + cnt;
+            const size_t out_at = decrypt ? s0 - a0 - lo : s0 - a0 + lo;
+            Slot& sl = ctx->slots[k % kSlots];
+            int rc = slot_reserve(ctx, sl, need, /*wipe=*/true);
+            if (rc != P252_OK) return rc;
+            uint8_t* p = static_cast<uint8_t*>(sl.arena);
+            auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
+            p252_fr* d_in = reinterpret_cast<p252_fr*>(take(ns * 32));
+            uint64_t* d_off = reinterpret_cast<uint64_t*>(take((cnt + 1) * 8));
+            p252_fr* d_uv = reinterpret_cast<p252_fr*>(take(cnt * 64));
+            p252_fr* d_nonce = reinterpret_cast<p252_fr*>(take(cnt * 32));
+            p252_fr* d_out = reinterpret_cast<p252_fr*>(take(out_ns * 32));
+            uint8_t* d_ok = take(cnt);
+            CU(cudaMemcpyAsync(d_in, in + s0, ns * 32, cudaMemcpyHostToDevice, sl.stream));
+            CU(cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, sl.stream));
+            CU(cudaMemcpyAsync(d_uv, secret_uv + 2 * lo, cnt * 64, cudaMemcpyHostToDevice, sl.stream));
+            CU(cudaMemcpyAsync(d_nonce, nonce + lo, cnt * 32, cudaMemcpyHostToDevice, sl.stream));
+            if ((long long)k == fail_at) return fail_cuda(ctx, cudaErrorLaunchFailure, "kernel launch (injected fault)");
+            rc = crypt_run(ctx, decrypt, tags, d_in, s0, ns, d_off, (uint32_t)cnt, max_len, d_uv, d_nonce, d_out,
+                           decrypt ? d_ok : nullptr, nullptr, nullptr, sl.stream);
+            if (rc != P252_OK) return rc;
+            CU(cudaMemcpyAsync(out + out_at, d_out, out_ns * 32, cudaMemcpyDeviceToHost, sl.stream));
+            if (decrypt) CU(cudaMemcpyAsync(ok + lo, d_ok, cnt, cudaMemcpyDeviceToHost, sl.stream));
+        }
+        return P252_OK;
+    };
+    return join_slots(ctx, body(), /*wipe=*/true);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1727,6 +1845,77 @@ int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t 
     if (n == 0) return P252_OK;
     if ((rc = varlen_tags(ctx, domain, max_len, out_len, &tags)) != P252_OK) return rc;
     return varlen_host(ctx, tags, in, offsets, n, (uint32_t)max_len, fixed_len, out, (uint32_t)out_len);
+}
+
+}  // extern "C"
+
+// ---- variable-length encrypt / decrypt batches (p252_encrypt_batch_varlen / p252_decrypt_batch_varlen) ----------------
+namespace {
+
+int crypt_varlen(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n_scalars, const uint64_t* offsets, size_t n,
+                 size_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* out, uint8_t* ok, size_t* n_failed,
+                 size_t* n_rejected, int flags) {
+    if (!ctx || ((!in || !offsets || !secret_uv || !nonce || !out || (decrypt && !ok)) && n)) return P252_ERR_INVALID_ARGUMENT;
+    if (max_len == 0 || max_len > P252_VARLEN_MAX_LEN || n >= 0x80000000ull) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_failed) *n_failed = 0;
+    if (n_rejected) *n_rejected = 0;
+    const p252_fr* tags = nullptr;
+    int rc;
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(in) || !aligned16(secret_uv) || !aligned16(nonce) || !aligned16(out) ||
+            (reinterpret_cast<uintptr_t>(offsets) & 7))
+            return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        if ((rc = crypt_tags(ctx, max_len, &tags)) != P252_OK) return rc;
+        // counter slot 0: authentication failures (decrypt), slot 1: rejected items
+        if ((n_failed || n_rejected) && (rc = counter_begin(ctx, p252_ctx::kCounters)) != P252_OK) return rc;
+        rc = crypt_run(ctx, decrypt, tags, in, 0, n_scalars, offsets, (uint32_t)n, (uint32_t)max_len, secret_uv, nonce, out, ok,
+                       n_failed ? ctx->d_counter : nullptr, n_rejected ? ctx->d_counter + 1 : nullptr, ctx->stream);
+        if (rc != P252_OK) return rc;
+        if ((rc = counter_end(ctx, n_failed, 0)) != P252_OK) return rc;
+        if ((rc = counter_end(ctx, n_rejected, 1)) != P252_OK) return rc;
+        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        return P252_OK;
+    }
+    // HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written.
+    // With every item valid the output ranges are disjoint and inside the output, so the decrypt range conditions of the
+    // device path need no check here.
+    const uint64_t kMin = decrypt ? 2 : 1;
+    for (size_t i = 0; i < n; ++i) {
+        const uint64_t a = offsets[i], b = offsets[i + 1];
+        if (a < offsets[0] || a > b || b > offsets[n] || offsets[n] > n_scalars) return P252_ERR_INVALID_ARGUMENT;
+        if (b - a < kMin) return P252_ERR_INVALID_IO_PATTERN;                 // as p252_encryption_tag(0)
+        if (b - a > max_len + kMin - 1) return P252_ERR_INVALID_ARGUMENT;
+    }
+    if (n == 0) return P252_OK;
+    if ((rc = crypt_tags(ctx, max_len, &tags)) != P252_OK) return rc;
+    rc = crypt_host(ctx, decrypt, tags, in, offsets, n, (uint32_t)max_len, secret_uv, nonce, out, ok);
+    if (rc == P252_OK && n_failed) {
+        size_t bad = 0;
+        for (size_t i = 0; i < n; ++i) bad += ok[i] ? 0 : 1;
+        *n_failed = bad;
+    }
+    return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int p252_encrypt_batch_varlen(p252_ctx* ctx, const p252_fr* msg, size_t n_scalars, const uint64_t* offsets, size_t n,
+                              size_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* cipher,
+                              size_t* n_rejected, int flags) {
+    return crypt_varlen(ctx, false, msg, n_scalars, offsets, n, max_len, secret_uv, nonce, cipher, nullptr, nullptr, n_rejected,
+                        flags);
+}
+
+int p252_decrypt_batch_varlen(p252_ctx* ctx, const p252_fr* cipher, size_t n_scalars, const uint64_t* offsets, size_t n,
+                              size_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* msg, uint8_t* ok,
+                              size_t* n_failed, size_t* n_rejected, int flags) {
+    return crypt_varlen(ctx, true, cipher, n_scalars, offsets, n, max_len, secret_uv, nonce, msg, ok, n_failed, n_rejected,
+                        flags);
 }
 
 }  // extern "C"

@@ -5,7 +5,7 @@
 //
 // Sponge schedule = dusk-safe 0.3 `Sponge` as driven by the reference:
 //   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest (k_sponge_digest_varlen: inputs of any lengths)
-//   encrypt/decrypt  src/encryption.rs:62-95  -> k_encrypt / k_decrypt
+//   encrypt/decrypt  src/encryption.rs:62-95  -> k_crypt (k_crypt_varlen: messages of any lengths)
 //   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
@@ -743,6 +743,21 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) k_merkle_verify(FrArg ta
 // k_varlen_keys: one thread per item.  key = len for a valid item, 0 for an invalid one (counted into *rejected, one
 // atomic per warp); value = i.  Valid: offsets[i] - base <= offsets[i+1] - base <= n_scalars, 1 <= len <= max_len and,
 // for a Merkle domain (fixed_len != 0), len == fixed_len.  Every later read of `in` is bounded by this check.
+// kCrypt (p252_encrypt_batch_varlen = 1, p252_decrypt_batch_varlen = 2; fixed_len unused): with a0 = offsets[0] - base
+// and an = offsets[n] - base, valid iff a0 <= a <= b <= an <= n_scalars and 1 <= len <= max_len (encrypt) or
+// 2 <= len <= max_len + 1 plus a - a0 >= i and an - b >= n - 1 - i (decrypt: the message range [a - a0 - i,
+// b - a0 - i - 1) lies inside an output of an - a0 - n scalars).  key = the message length (len, or len - 1 for decrypt).
+template <int kCrypt>
+__device__ __forceinline__ bool crypt_item_ok(const uint64_t* __restrict__ offsets, uint32_t n, uint64_t base, uint64_t n_scalars,
+                                              uint32_t max_len, uint32_t i, uint64_t a, uint64_t b) {
+    constexpr uint64_t kMin = kCrypt == 2 ? 2u : 1u;              // a cipher carries one authentication scalar more
+    const uint64_t a0 = offsets[0] - base, an = offsets[n] - base, len = b - a;
+    bool ok = a0 <= a && a <= b && b <= an && an <= n_scalars && len >= kMin && len <= (uint64_t)max_len + kMin - 1;
+    if (kCrypt == 2) ok = ok && a - a0 >= i && an - b >= (uint64_t)(n - 1 - i);
+    return ok;
+}
+
+template <int kCrypt>
 __global__ void __launch_bounds__(256) k_varlen_keys(const uint64_t* __restrict__ offsets, uint32_t n, uint64_t base,
                                                      uint64_t n_scalars, uint32_t max_len, uint32_t fixed_len,
                                                      uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
@@ -751,8 +766,10 @@ __global__ void __launch_bounds__(256) k_varlen_keys(const uint64_t* __restrict_
     if (i >= n) return;
     const uint64_t a = offsets[i] - base, b = offsets[i + 1] - base;
     const uint64_t len = b - a;
-    const bool ok = a <= b && b <= n_scalars && len >= 1 && len <= max_len && (fixed_len == 0 || len == fixed_len);
-    keys[i] = ok ? (uint32_t)len : 0u;
+    const bool ok = kCrypt == 0
+                        ? a <= b && b <= n_scalars && len >= 1 && len <= max_len && (fixed_len == 0 || len == fixed_len)
+                        : crypt_item_ok<kCrypt>(offsets, n, base, n_scalars, max_len, i, a, b);
+    keys[i] = ok ? (uint32_t)(len - (kCrypt == 2 ? 1 : 0)) : 0u;
     vals[i] = i;
     if (rejected) {
         const unsigned act = __activemask();
@@ -904,6 +921,209 @@ __global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const ui
         } else if (step < steps) {
             const uint32_t q = 4 * (step - nin) + (uint32_t)li - 1;
             if (li >= 1 && q < out_len) store_fr(dst + (size_t)q * 32, s);
+        }
+    }
+}
+
+// ---- variable-length encrypt / decrypt batches (p252_encrypt_batch_varlen / p252_decrypt_batch_varlen) ---------------
+// Item i reads src[offsets[i] - base, offsets[i+1] - base) and writes its output from dst[offsets[i] - offsets[0] + i]
+// (encrypt: L + 1 cipher scalars) or dst[offsets[i] - offsets[0] - i] (decrypt: L message scalars), i.e. the input CSR
+// with every item one scalar longer / shorter, packed from 0.  tags[L] is the tag of p252_encryption_tag(L) (tags[0] = 0,
+// unused); secret_uv / nonce / ok are indexed by i.  The items come sorted by message length L (lens; 0 = rejected by
+// k_varlen_keys<1|2>, which bounds every address below) with their indices (perm).
+//
+// k_crypt_varlen: k_crypt over the sorted order, one thread per item.  Every lane carries its own tag, step count
+// 2*ceil(L/4), last-chunk widths and base addresses; the loop runs to the warp's largest step count and a lane past its
+// own last step neither permutes nor touches memory.  A rejected item writes nothing (decrypt: ok = 0).  Warps take the
+// sorted segments from the end, so the longest items start first.  4 resident blocks per SM (128 registers): at
+// kMinBlocks' 96 the per-lane bookkeeping spills.
+template <bool kDecrypt>
+__global__ void __launch_bounds__(kThreads, 4) k_crypt_varlen(const uint8_t* __restrict__ tags, const uint8_t* __restrict__ src,
+                                                              uint64_t base, const uint64_t* __restrict__ offsets,
+                                                              const uint32_t* __restrict__ lens, const uint32_t* __restrict__ perm,
+                                                              uint32_t n, const uint8_t* __restrict__ secret_uv,
+                                                              const uint8_t* __restrict__ nonce, uint8_t* dst,
+                                                              uint8_t* __restrict__ ok, unsigned long long* __restrict__ n_failed) {
+    P252_STAGE_TABLES
+    const int lane = threadIdx.x & 31;
+    const uint32_t nseg = (n + 31) / 32;
+    const uint32_t wg = blockIdx.x * kWarps + (threadIdx.x >> 5);
+    if (wg >= nseg) return;
+    const uint32_t k = (nseg - 1 - wg) * 32 + lane;
+    const bool live = k < n;
+    const uint32_t L = live ? lens[k] : 0u;
+    const uint32_t i = live ? perm[k] : 0u;
+    const uint64_t a = L ? offsets[i] : 0;
+    const uint64_t o = L ? (kDecrypt ? a - offsets[0] - i : a - offsets[0] + i) : 0;
+    const uint8_t* srci = src + (L ? (a - base) * 32 : 0);
+    uint8_t* dsti = dst + o * 32;
+    const uint8_t* msgi = kDecrypt ? dsti : srci;        // the plaintext, wherever it lives
+
+    uint32_t s[5][8];
+    load_fr(s[0], tags + (size_t)L * 32);
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s[1][w] = s[2][w] = s[3][w] = s[4][w] = 0;
+    if (L) {
+        load_fr(s[1], secret_uv + (size_t)i * 64);       // Absorb(2): u, v added to zero
+        load_fr(s[2], secret_uv + (size_t)i * 64 + 32);
+        load_fr(s[3], nonce + (size_t)i * 32);           // Absorb(1)
+    }
+    const uint32_t nk = (L + 3) / 4, steps = 2 * nk;
+    const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
+    bool good = true;
+#pragma unroll 1
+    for (uint32_t step = 0; step < wsteps; ++step) {
+        if (step >= steps) continue;
+        hades_permute(s, (step + 1 == steps) ? 0x2u : 0x1fu P252_TAB_PASS);   // last: only the Squeeze(1) lane is read
+        if (step < nk) {
+            // Squeeze chunk `step` of the keystream and emit cipher (or recovered message)
+            const uint32_t left = L - 4 * step;
+            const int nscal = left < 4 ? (int)left : 4;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                if (q < nscal) {
+                    uint32_t x[8], y[8];
+                    load_fr(x, srci + (size_t)(4 * step + q) * 32);
+                    if (kDecrypt)
+                        fr_sub_mod(y, x, s[1 + q]);      // Encryption::subtract
+                    else
+                        fr_add_mod(y, x, s[1 + q]);      // Safe::add
+                    store_fr(dsti + (size_t)(4 * step + q) * 32, y);
+                }
+            }
+        }
+        if (step + 1 >= nk && step + 1 < steps) {
+            // Absorb(L) chunk c of the plaintext: chunk 0 right after the last squeeze, chunk c > 0 one permutation later each
+            const uint32_t c = step + 1 - nk;
+            const uint32_t left = L - 4 * c;
+            const int nscal = left < 4 ? (int)left : 4;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                if (q < nscal) {
+                    uint32_t x[8], t[8];
+                    if (kDecrypt)
+                        load_fr_rw(x, msgi + (size_t)(4 * c + q) * 32);
+                    else
+                        load_fr(x, msgi + (size_t)(4 * c + q) * 32);
+                    fr_add_mod(t, s[1 + q], x);
+#pragma unroll
+                    for (int w = 0; w < 8; ++w) s[1 + q][w] = t[w];
+                }
+            }
+        }
+        if (step + 1 == steps) {
+            // Squeeze(1): authentication element
+            if (kDecrypt) {
+                uint32_t x[8];
+                load_fr(x, srci + (size_t)L * 32);
+#pragma unroll
+                for (int w = 0; w < 8; ++w) good = good && (x[w] == s[1][w]);   // Encryption::is_equal
+            } else {
+                store_fr(dsti + (size_t)L * 32, s[1]);
+            }
+        }
+    }
+    if (kDecrypt) {
+        if (live) ok[i] = (L && good) ? 1 : 0;
+        if (L && !good) {                                 // Error::DecryptionFailed: release nothing
+            const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            for (uint32_t q = 0; q < L; ++q) store_fr(dsti + (size_t)q * 32, zero);
+        }
+        if (n_failed) {                                   // one atomic per warp that saw a failure; rejected items are not
+            const unsigned bad = __ballot_sync(0xffffffffu, L && !good);   // failures (k_varlen_keys counted them)
+            if (bad && lane == 0) atomicAdd(n_failed, (unsigned long long)__popc(bad));
+        }
+    }
+}
+
+// the same for small batches: five threads per item (hades_permute_coop), as k_sponge_digest_varlen_coop.  Thread li of
+// a group owns state lane li: lane 0 the tag, lanes 1..3 u, v, nonce; rate thread li adds / subtracts, stores and absorbs
+// message scalar 4*c + li - 1 of chunk c, and thread 1 holds the Squeeze(1) lane.  Every thread runs the warp's largest
+// step count (the permutation's shuffles span the warp); a group past its own last step only idles.  Decrypt: thread 1's
+// authentication result is shuffled to its group before any thread zeroes its message scalars.
+template <bool kDecrypt>
+__global__ void __launch_bounds__(kThreads) k_crypt_varlen_coop(const uint8_t* __restrict__ tags, const uint8_t* __restrict__ src,
+                                                                uint64_t base, const uint64_t* __restrict__ offsets,
+                                                                const uint32_t* __restrict__ lens,
+                                                                const uint32_t* __restrict__ perm, uint32_t n,
+                                                                const uint8_t* __restrict__ secret_uv,
+                                                                const uint8_t* __restrict__ nonce, uint8_t* dst,
+                                                                uint8_t* __restrict__ ok, unsigned long long* __restrict__ n_failed) {
+    const int lane = threadIdx.x & 31;
+    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
+    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
+    const size_t k = warp_global * kCoopItemsPerWarp + grp;
+    if (warp_global * kCoopItemsPerWarp >= n) return;            // whole warp idle
+    const bool live = (grp < kCoopItemsPerWarp) && (k < n);      // idle threads still take part in the shuffles
+    double crow[5];
+#pragma unroll
+    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
+    const uint32_t L = live ? lens[k] : 0u;
+    const uint32_t i = live ? perm[k] : 0u;
+    const uint64_t a = L ? offsets[i] : 0;
+    const uint64_t o = L ? (kDecrypt ? a - offsets[0] - i : a - offsets[0] + i) : 0;
+    const uint8_t* srci = src + (L ? (a - base) * 32 : 0);
+    uint8_t* dsti = dst + o * 32;
+    const uint8_t* msgi = kDecrypt ? dsti : srci;
+    uint32_t s[8];
+#pragma unroll
+    for (int w = 0; w < 8; ++w) s[w] = 0u;
+    if (li == 0)
+        load_fr(s, tags + (size_t)L * 32);
+    else if (L && li <= 2)
+        load_fr(s, secret_uv + (size_t)i * 64 + (size_t)(li - 1) * 32);
+    else if (L && li == 3)
+        load_fr(s, nonce + (size_t)i * 32);
+    const uint32_t nk = (L + 3) / 4, steps = 2 * nk;
+    const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
+    bool good = true;
+#pragma unroll 1
+    for (uint32_t step = 0; step < wsteps; ++step) {
+        hades_permute_coop(s, li, g0, crow);
+        const uint32_t q = 4 * step + (uint32_t)li - 1;          // li == 0 wraps to a huge value -> no memory access
+        if (step < nk && li >= 1 && q < L) {                     // squeeze chunk `step`: emit cipher / message scalar q
+            uint32_t x[8], y[8];
+            load_fr(x, srci + (size_t)q * 32);
+            if (kDecrypt)
+                fr_sub_mod(y, x, s);
+            else
+                fr_add_mod(y, x, s);
+            store_fr(dsti + (size_t)q * 32, y);
+        }
+        if (step + 1 >= nk && step + 1 < steps) {                // absorb plaintext chunk c (this thread's own stores)
+            const uint32_t qa = 4 * (step + 1 - nk) + (uint32_t)li - 1;
+            if (li >= 1 && qa < L) {
+                uint32_t x[8], t[8];
+                if (kDecrypt)
+                    load_fr_rw(x, msgi + (size_t)qa * 32);
+                else
+                    load_fr(x, msgi + (size_t)qa * 32);
+                fr_add_mod(t, s, x);
+#pragma unroll
+                for (int w = 0; w < 8; ++w) s[w] = t[w];
+            }
+        }
+        if (step + 1 == steps && li == 1) {                      // Squeeze(1): authentication element
+            if (kDecrypt) {
+                uint32_t x[8];
+                load_fr(x, srci + (size_t)L * 32);
+#pragma unroll
+                for (int w = 0; w < 8; ++w) good = good && (x[w] == s[w]);
+            } else {
+                store_fr(dsti + (size_t)L * 32, s);
+            }
+        }
+    }
+    if (kDecrypt) {
+        good = __shfl_sync(0xffffffffu, good, g0 + 1);           // the group's verdict, before anyone zeroes
+        if (live && li == 0) ok[i] = (L && good) ? 1 : 0;
+        if (L && !good && li >= 1) {
+            const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            for (uint32_t q = (uint32_t)li - 1; q < L; q += 4) store_fr(dsti + (size_t)q * 32, zero);
+        }
+        if (n_failed) {
+            const unsigned bad = __ballot_sync(0xffffffffu, li == 0 && L && !good);
+            if (bad && lane == 0) atomicAdd(n_failed, (unsigned long long)__popc(bad));
         }
     }
 }
@@ -1147,7 +1367,42 @@ cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], 
 cudaError_t launch_varlen_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars, uint32_t max_len,
                                uint32_t fixed_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    k_varlen_keys<<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
+    k_varlen_keys<0><<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_crypt_varlen_keys(bool decrypt, const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars,
+                                     uint32_t max_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected,
+                                     cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    if (decrypt)
+        k_varlen_keys<2><<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
+    else
+        k_varlen_keys<1><<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_crypt_varlen(bool decrypt, const void* tags, const void* src, uint64_t base, const uint64_t* offsets,
+                                const uint32_t* lens, const uint32_t* perm, uint32_t n, const void* secret_uv, const void* nonce,
+                                void* dst, uint8_t* ok, unsigned long long* n_failed, size_t coop_max, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const uint8_t* t = static_cast<const uint8_t*>(tags);
+    const uint8_t* s = static_cast<const uint8_t*>(src);
+    const uint8_t* uv = static_cast<const uint8_t*>(secret_uv);
+    const uint8_t* no = static_cast<const uint8_t*>(nonce);
+    uint8_t* d = static_cast<uint8_t*>(dst);
+    if (n <= coop_max) {
+        const size_t warps = (n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
+        const unsigned grid = (unsigned)((warps + kWarps - 1) / kWarps);
+        if (decrypt)
+            k_crypt_varlen_coop<true><<<grid, kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, ok, n_failed);
+        else
+            k_crypt_varlen_coop<false><<<grid, kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, nullptr, nullptr);
+    } else if (decrypt) {
+        k_crypt_varlen<true><<<grid_for(n), kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, ok, n_failed);
+    } else {
+        k_crypt_varlen<false><<<grid_for(n), kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, nullptr, nullptr);
+    }
     return cudaGetLastError();
 }
 

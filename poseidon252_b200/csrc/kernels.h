@@ -75,6 +75,20 @@ cudaError_t launch_varlen_keys(const uint64_t* offsets, uint32_t n, uint64_t bas
 // perm[k] (out_len scalars, a zero row for lens[k] == 0); lane-split kernel when n <= coop_max
 cudaError_t launch_digest_varlen(const void* tags, const void* in, uint64_t base, const uint64_t* offsets, const uint32_t* lens,
                                  const uint32_t* perm, uint32_t n, void* out, uint32_t out_len, size_t coop_max, cudaStream_t st);
+// Variable-length encrypt / decrypt (p252_encrypt_batch_varlen / p252_decrypt_batch_varlen).  keys: the message length L
+// of a valid item (a0 <= a <= b <= an <= n_scalars with a0 / an the first / last offset minus base; encrypt 1 <= b - a <=
+// max_len, decrypt 2 <= b - a <= max_len + 1 and the message range inside the output), 0 for an invalid one (counted into
+// *rejected); vals[i] = i
+cudaError_t launch_crypt_varlen_keys(bool decrypt, const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars,
+                                     uint32_t max_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected,
+                                     cudaStream_t st);
+// over the keys sorted ascending (lens) with their values (perm): item perm[k] reads src[offsets[i] - base ..) and writes
+// dst from offsets[i] - offsets[0] + i (encrypt, L + 1 scalars) or - i (decrypt, L scalars; ok[i], failures counted into
+// *n_failed); tags[L] = p252_encryption_tag(L); a rejected item (L = 0) writes nothing but ok[i] = 0.  Lane-split kernel
+// when n <= coop_max
+cudaError_t launch_crypt_varlen(bool decrypt, const void* tags, const void* src, uint64_t base, const uint64_t* offsets,
+                                const uint32_t* lens, const uint32_t* perm, uint32_t n, const void* secret_uv, const void* nonce,
+                                void* dst, uint8_t* ok, unsigned long long* n_failed, size_t coop_max, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

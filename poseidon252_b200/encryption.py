@@ -3,8 +3,9 @@ The shared secret is the (u, v) coordinate pair of the JubJubAffine point
 (src/encryption.rs:71,92): a (2, 4) uint64 array."""
 import numpy as np
 
-from .engine import default_engine
+from .engine import default_engine, varlen_out_offsets
 from .errors import DecryptionFailed, EncryptionFailed, Error
+from .hash import pack_varlen
 
 
 def encrypt(message, shared_secret, nonce, engine=None):
@@ -45,3 +46,49 @@ def decrypt_batch(ciphers, secrets_uv, nonces, engine=None, async_=False):
     items for which the reference returns Error::DecryptionFailed (their message is zeroed)."""
     eng = engine or default_engine(ciphers.device.index if hasattr(ciphers, "is_cuda") else 0)
     return eng.decrypt_batch(ciphers, secrets_uv, nonces, async_=async_)
+
+
+def cipher_offsets(offsets):
+    """Offsets of the ciphers of messages at `offsets` (each one scalar longer, packed from 0): offsets - offsets[0] + i.
+    Works on numpy arrays and CUDA tensors (no host sync)."""
+    return varlen_out_offsets(offsets, 1)
+
+
+def message_offsets(offsets):
+    """Offsets of the messages of ciphers at `offsets` (each one scalar shorter, packed from 0): offsets - offsets[0] - i."""
+    return varlen_out_offsets(offsets, -1)
+
+
+def _split(flat, offsets):
+    return [flat[int(offsets[i]):int(offsets[i + 1])] for i in range(len(offsets) - 1)]
+
+
+def encrypt_batch_varlen(messages, secrets_uv, nonces, engine=None, max_len=None, out=None, async_=False):
+    """NEW: n independent encrypt() calls over messages of different lengths, one device call.
+    messages: a list of (k_i, 4) host arrays (packed by `pack_varlen`) -> a list of (k_i + 1, 4) ciphers; or a
+    `(data, offsets)` pair as taken by `Engine.encrypt_batch_varlen` (numpy or CUDA tensors) -> (cipher, cipher_offsets)."""
+    if isinstance(messages, tuple):
+        data, offsets = messages
+        eng = engine or default_engine(data.device.index if hasattr(data, "is_cuda") else 0)
+        return eng.encrypt_batch_varlen(data, offsets, secrets_uv, nonces, max_len=max_len, out=out, async_=async_)
+    data, offsets, longest = pack_varlen(messages)
+    eng = engine or default_engine()
+    cipher, coff = eng.encrypt_batch_varlen(data, offsets, secrets_uv, nonces,
+                                            max_len=max(longest, 1) if max_len is None else max_len, out=out)
+    return _split(cipher, coff)
+
+
+def decrypt_batch_varlen(ciphers, secrets_uv, nonces, engine=None, max_len=None, async_=False):
+    """NEW: n independent decrypt() calls over ciphers of different lengths, one device call.
+    ciphers: a list of (k_i + 1, 4) host arrays -> (list of (k_i, 4) messages, ok (n,) uint8); or a `(data, offsets)`
+    pair as taken by `Engine.decrypt_batch_varlen` -> (msg, msg_offsets, ok).  ok[i] == 0 marks the items for which the
+    reference returns Error::DecryptionFailed (their message is zeroed)."""
+    if isinstance(ciphers, tuple):
+        data, offsets = ciphers
+        eng = engine or default_engine(data.device.index if hasattr(data, "is_cuda") else 0)
+        return eng.decrypt_batch_varlen(data, offsets, secrets_uv, nonces, max_len=max_len, async_=async_)
+    data, offsets, longest = pack_varlen(ciphers)
+    eng = engine or default_engine()
+    msg, moff, ok = eng.decrypt_batch_varlen(data, offsets, secrets_uv, nonces,
+                                             max_len=max(longest - 1, 1) if max_len is None else max_len)
+    return _split(msg, moff), ok

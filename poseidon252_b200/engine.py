@@ -313,9 +313,86 @@ class Engine:
         return msg, ok
 
     def last_decrypt_failures(self):
-        """Items of the last decrypt_batch whose authentication failed (counted on the device for device buffers;
-        after an async_ call, sync() first)."""
+        """Items of the last decrypt_batch or decrypt_batch_varlen whose authentication failed (counted on the device for
+        device buffers; after an async_ call, sync() first)."""
         return int(getattr(self, "_nfail", ctypes.c_size_t(0)).value)
+
+    def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
+        """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
+        max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries
+        beyond its message (0 for messages, 1 for ciphers)."""
+        dp, dlead, flags, dk = self._in(data, (4,))
+        if len(dlead) != 1:
+            raise EngineError(-1, "data must have shape (n_scalars, 4), got leading shape %s" % (tuple(dlead),))
+        op, n1, ok_ = self._idx(offsets, dk, "offsets")
+        if n1 < 1:
+            raise EngineError(-1, "offsets must have n + 1 >= 1 entries")
+        n = n1 - 1
+        sp, l2, f2, sk = self._in(secrets_uv, (2, 4))
+        np_, l3, f3, nk = self._in(nonces, (4,))
+        if not (flags == f2 == f3):
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("secrets_uv", l2, n)
+        self._same_lead("nonces", l3, n)
+        if max_len is None:
+            if n == 0:
+                max_len = 1
+            elif _is_torch(ok_):
+                import torch
+                o = ok_.view(torch.int64)
+                max_len = int((o[1:] - o[:-1]).max().item()) - key_extra
+            else:
+                max_len = int((ok_[1:].astype(np.int64) - ok_[:-1].astype(np.int64)).max()) - key_extra
+            max_len = max(max_len, 1)
+        return dp, int(dlead[0]), op, n, int(max_len), sp, np_, flags, dk, ok_
+
+    def encrypt_batch_varlen(self, data, offsets, secrets_uv, nonces, max_len=None, out=None, async_=False):
+        """n x encrypt(data[offsets[i]:offsets[i+1]], secrets_uv[i], nonces[i]) over messages of any lengths, one call.
+        data (n_scalars, 4), offsets (n + 1,), secrets_uv (n, 2, 4) and nonces (n, 4) live in one memory space (numpy, or
+        CUDA tensors); offsets[0] need not be 0.  Returns (cipher, cipher_offsets): cipher item i is
+        cipher[cipher_offsets[i]:cipher_offsets[i+1]] (len + 1 scalars), packed from 0; cipher has n_scalars + n rows, of
+        which those past cipher_offsets[-1] are unused (offsets covering only part of data).  cipher_offsets
+        (= cipher_offsets(offsets)) is computed in the offsets' memory space.  max_len bounds the message lengths (at most
+        VARLEN_MAX_LEN); None takes the longest, which for CUDA tensors costs a device-to-host sync.  Host batches raise on
+        an invalid item and write nothing; device batches skip invalid items, write nothing for them and count them
+        (last_crypt_rejected())."""
+        dp, ns, op, n, max_len, sp, np_, flags, dk, ok_ = self._crypt_varlen_args(data, offsets, secrets_uv, nonces, max_len, 0)
+        rows = ns + n
+        res = self._out_like(dk, (max(rows, 1), 4))[:rows] if out is None else self._check_out(out, (rows, 4), dk)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._crej = self._counter(flags)
+        self._check(self._lib.p252_encrypt_batch_varlen(self._ctx, dp, ns, op, n, max_len, sp, np_, self._ptr(res),
+                                                        ctypes.byref(self._crej), flags))
+        return res, varlen_out_offsets(ok_, 1)
+
+    def decrypt_batch_varlen(self, ciphers, offsets, secrets_uv, nonces, max_len=None, async_=False):
+        """n x decrypt(ciphers[offsets[i]:offsets[i+1]], secrets_uv[i], nonces[i]) over ciphers of any lengths, one call.
+        Buffers as for encrypt_batch_varlen; max_len bounds the message lengths (cipher length - 1).  Returns
+        (msg, msg_offsets, ok): message item i is msg[msg_offsets[i]:msg_offsets[i+1]] (one scalar shorter than its
+        cipher), packed from 0 in max(n_scalars - n, 0) rows; ok[i] == 0 where the reference returns
+        Error::DecryptionFailed (that message is zeroed) or, for device buffers, the item was invalid and skipped.  Failure
+        count: last_decrypt_failures(); invalid device items: last_crypt_rejected()."""
+        cp, ns, op, n, max_len, sp, np_, flags, ck, ok_ = self._crypt_varlen_args(ciphers, offsets, secrets_uv, nonces,
+                                                                                   max_len, 1)
+        rows = max(ns - n, 0)
+        msg = self._out_like(ck, (max(rows, 1), 4))[:rows]          # never a NULL pointer, even for zero rows
+        if _is_torch(ck):
+            import torch
+            ok = torch.empty((n,), dtype=torch.uint8, device=ck.device)
+        else:
+            ok = np.empty((n,), dtype=np.uint8)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nfail = self._counter(flags)
+        self._crej = self._counter(flags)
+        self._check(self._lib.p252_decrypt_batch_varlen(self._ctx, cp, ns, op, n, max_len, sp, np_, self._ptr(msg),
+                                                        self._ptr(ok), ctypes.byref(self._nfail), ctypes.byref(self._crej),
+                                                        flags))
+        return msg, varlen_out_offsets(ok_, -1), ok
+
+    def last_crypt_rejected(self):
+        """Items of the last encrypt_batch_varlen / decrypt_batch_varlen skipped as invalid (device buffers; sync() first
+        after async_)."""
+        return int(getattr(self, "_crej", ctypes.c_size_t(0)).value)
 
     # -- arity-4 Merkle tree ----------------------------------------------------------------------
     def merkle4_level(self, children, out=None, async_=False):
@@ -628,6 +705,22 @@ def mtree_layout(arity, height, capacity):
     offs = (ctypes.c_uint64 * (min(max(int(height), 0), 64) + 1))()
     raise_for_status(lib.p252_mtree_layout(int(arity), int(height), int(capacity), ctypes.byref(ls), ctypes.byref(ns), offs), lib)
     return int(ls.value), int(ns.value), [int(v) for v in offs]
+
+
+def varlen_out_offsets(offsets, delta):
+    """offsets - offsets[0] + delta * i for i = 0..n: the offsets of a CSR batch whose item i is `delta` scalars longer
+    (encrypt: +1) or shorter (decrypt: -1) than input item i, packed from 0.  Computed in the offsets' own memory space
+    (numpy uint64, or a CUDA tensor of the offsets' dtype, without a host sync).  Pure arithmetic."""
+    if _is_torch(offsets):
+        import torch
+        o = offsets.view(torch.int64)
+        r = o - o[:1] + delta * torch.arange(o.shape[0], dtype=torch.int64, device=o.device)
+        return r.view(offsets.dtype)
+    a = np.ascontiguousarray(offsets, dtype=np.uint64).reshape(-1)
+    if a.shape[0] == 0:
+        raise EngineError(-1, "offsets must have n + 1 >= 1 entries")
+    step = np.arange(a.shape[0], dtype=np.uint64)
+    return (a - a[0]) + step if delta > 0 else (a - a[0]) - step     # uint64 arithmetic: wraps like the C ABI's
 
 
 def default_engine(device=0):
