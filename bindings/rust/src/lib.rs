@@ -2,6 +2,7 @@
 //! `dusk_poseidon` over the H100 engine: `Hash::digest_batch`, `hades::permute_batch`,
 //! `encrypt_batch`, `decrypt_batch`, `merkle4_build`, Merkle openings, fixed-height trees with batched updates
 //! (`Tree`), sparse fixed-height trees with inserts and removals at any position (`SparseTree`, in smtree.rs),
+//! compact sparse trees at any height (`CompactTree`, in ctree.rs),
 //! variable-length digest batches (`Engine::digest_batch_varlen`), bound to include/poseidon252_b200.h.
 //! The `extern "C"` block below is checked mechanically against the header by tests/test_abi.py
 //! (same symbol set, same parameter counts) and its exact call set is exercised by tests/c/abi_smoke.c.
@@ -109,6 +110,11 @@ pub use smtree::{p252_smtree, SparseTree};
 // Encrypt / decrypt batches over messages of different lengths: their own `extern "C"` block in crypt_varlen.rs (methods
 // on Engine).
 mod crypt_varlen;
+
+// Compact sparse trees (positions anywhere below arity^height, storage proportional to the present leaves): their own
+// `extern "C"` block in ctree.rs.
+mod ctree;
+pub use ctree::{p252_ctree, CompactTree};
 
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]

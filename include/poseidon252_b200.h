@@ -374,6 +374,49 @@ int p252_smtree_len(p252_ctx* ctx, const p252_smtree* tree, uint64_t* n_present,
 int p252_smtree_open_batch(p252_ctx* ctx, const p252_smtree* tree, const uint64_t* pos, size_t n, p252_fr* paths_out,
                            int flags);
 
+/* ---- compact sparse trees: storage proportional to the present leaves (poseidon-merkle `Tree<T, H, A>` at any height) --
+ * The semantics of p252_smtree at positions [0, arity^height): presence, and the empty-subtree rule (a node is present
+ * iff one of its children is; a present node is Hash::digest(Domain::Merkle{A}, its A child slots) with absent children
+ * read as 0; an absent node is 0 and never hashed).  Heights up to 64 with arity 2 and 32 with arity 4, so that every
+ * u64 can be a position.  Storage is the sorted list of present nodes, level by level: level l holds exactly its
+ * present nodes as (index, value) pairs, indices ascending, packed from the level's first slot; every slot past
+ * count[l] is zero (keys and values).  This canonical form makes buffers comparable bit for bit, and for any present set
+ * a p252_smtree of the same (arity, height) can hold, level l is the list of that tree's present slots of level l.
+ * The root is values[level_offset[height]], 0 for the empty tree.  Struct and buffers belong to the caller; an
+ * all-zero buffer set is the empty tree.  DEVICE buffers: values 16-byte aligned, keys / count / positions 8-byte
+ * aligned.  An update reads and writes every present node of every level (about 80 B per present node per level) and
+ * hashes only the dirty paths; its stream-ordered temporaries take about 48 B per max_leaves plus 250 B per item. */
+typedef struct p252_ctree {
+    uint32_t struct_size; /* sizeof(p252_ctree)                                                          */
+    int32_t arity;        /* 2 or 4                                                                       */
+    int32_t height;       /* 1..64, and arity^height <= 2^64 (arity 4: height <= 32)                      */
+    int32_t reserved;
+    uint64_t max_leaves;  /* bound on present positions the buffers are laid out for, 1 .. 2^31 - 1       */
+    uint64_t* keys;       /* total_slots: per level the sorted node indices, level l at level_offset[l]   */
+    p252_fr* values;      /* total_slots: the matching node values                                        */
+    uint64_t* count;      /* height + 1 entries: present nodes of level l (count[0] = number of leaves)   */
+} p252_ctree;
+/* Level l has min(max_leaves, arity^(height - l)) slots (level height: 1), starting at level_offset[l] (height + 1
+ * entries, optional); *total_slots (optional) is their sum.  Pure host arithmetic. */
+int p252_ctree_layout(int arity, int height, uint64_t max_leaves, uint64_t* total_slots, uint64_t* level_offset);
+/* One batch of operations (pos[i], op[i], values[i]) with the semantics of p252_smtree_update: op 0 inserts or
+ * overwrites, op 1 removes (values[i] not read), op = NULL means all inserts; the result equals applying them in batch
+ * order.  There is no separate build: inserting n leaves into the empty tree is the build (about n x height
+ * permutations).  pos / op / values live in the tree's memory space (values required for n > 0); n < 2^31.
+ *   HOST: a position >= arity^height or an op other than 0/1 is P252_ERR_INVALID_ARGUMENT and nothing is modified; so is a
+ *   batch that would leave more than max_leaves present positions.  HOST trees are staged to the device and copied back.
+ *   DEVICE: an invalid item is skipped on the device and counted into *n_rejected (optional HOST pointer, 0 for HOST
+ *   calls; lifetime as for p252_mtree_update).  A batch that would leave more than max_leaves present positions is
+ *   refused on the device without a host synchronisation: the tree is unchanged and *n_rejected = n.
+ * After a CUDA failure the tree's contents are unspecified. */
+int p252_ctree_update(p252_ctx* ctx, p252_ctree* tree, const uint64_t* pos, const uint8_t* op, const p252_fr* values,
+                      size_t n, size_t* n_rejected, int flags);
+/* Openings of positions pos[0..n) in the format of p252_mtree_open_batch (n x height x arity, absent slots 0); they
+ * verify with p252_merkle_verify_batch, depth = height.  An absent position is P252_ERR_INVALID_ARGUMENT for HOST
+ * buffers and an all-zero opening for DEVICE buffers. */
+int p252_ctree_open_batch(p252_ctx* ctx, const p252_ctree* tree, const uint64_t* pos, size_t n, p252_fr* paths_out,
+                          int flags);
+
 /* ---- multi-GPU tree build: one process per GPU, one NCCL all-gather per level ---------------- */
 #define P252_NCCL_UNIQUE_ID_BYTES 128
 /* rank 0 creates the id and ships it to the other ranks by any means (torch.distributed / MPI) */

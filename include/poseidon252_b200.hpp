@@ -12,6 +12,8 @@
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
+#include <algorithm>
+#include <cstddef>
 #include <cstdint>
 #include <stdexcept>
 #include <string>
@@ -442,6 +444,77 @@ private:
     p252_smtree t_{};
     std::vector<Scalar> leaves_, nodes_;
     std::vector<uint8_t> present_;
+};
+
+// Compact sparse tree over p252_ctree (host buffers): poseidon-merkle's `Tree<T, H, A>` at any height, positions anywhere
+// below arity^height (every u64 at arity 2 / height 64 or arity 4 / height 32), storage proportional to at most
+// `max_leaves` present positions.  Each level is the sorted list of its present nodes; presence and the empty-subtree
+// rule are those of SparseTree.
+class CompactTree {
+public:
+    CompactTree(int arity, int height, uint64_t max_leaves, Engine& e = Engine::default_engine()) : e_(&e) {
+        uint64_t total = 0;
+        offset_.resize((size_t)(height > 0 && height <= 64 ? height : 0) + 1);
+        check(p252_ctree_layout(arity, height, max_leaves, &total, offset_.data()));
+        keys_.assign(total, 0);
+        values_.assign(total, Scalar{});
+        count_.assign((size_t)height + 1, 0);
+        t_.struct_size = sizeof(p252_ctree);
+        t_.arity = arity;
+        t_.height = height;
+        t_.reserved = 0;
+        t_.max_leaves = max_leaves;
+    }
+    // ops[i] == 0 inserts / overwrites values[i] at pos[i], ops[i] == 1 removes pos[i]; as if applied one after another
+    void apply(const std::vector<uint64_t>& pos, const std::vector<uint8_t>& ops, const std::vector<Scalar>& values) {
+        if (pos.size() != ops.size() || pos.size() != values.size())
+            throw Error(P252_ERR_INVALID_ARGUMENT, "pos, ops and values differ in length");
+        run(pos, ops.data(), values.data());
+    }
+    void insert(const std::vector<uint64_t>& pos, const std::vector<Scalar>& values) {
+        if (pos.size() != values.size()) throw Error(P252_ERR_INVALID_ARGUMENT, "pos and values differ in length");
+        run(pos, nullptr, values.data());
+    }
+    void remove(const std::vector<uint64_t>& pos) {
+        apply(pos, std::vector<uint8_t>(pos.size(), 1), std::vector<Scalar>(pos.size()));
+    }
+    const Scalar& root() const { return values_[offset_.back()]; }
+    uint64_t size() const { return count_[0]; }
+    bool contains(uint64_t pos) const {
+        const auto end = keys_.begin() + (std::ptrdiff_t)count_[0];
+        const auto it = std::lower_bound(keys_.begin(), end, pos);
+        return it != end && *it == pos;
+    }
+    const std::vector<uint64_t>& keys() const { return keys_; }
+    const std::vector<Scalar>& values() const { return values_; }
+    const std::vector<uint64_t>& count() const { return count_; }
+    const std::vector<uint64_t>& level_offset() const { return offset_; }
+    // the poseidon-merkle `Opening` of the present position pos
+    Opening opening(uint64_t pos) {
+        Opening o;
+        o.arity = t_.arity;
+        o.root = root();
+        o.leaf_index = pos;
+        o.branch.resize((size_t)t_.height * t_.arity);
+        check(p252_ctree_open_batch(e_->get(), bind(), &pos, 1, o.branch.data(), P252_MEM_HOST), e_->get());
+        for (int l = 0; l < t_.height; ++l, pos /= (uint64_t)t_.arity) o.positions.push_back(pos % t_.arity);
+        return o;
+    }
+
+private:
+    p252_ctree* bind() {
+        t_.keys = keys_.data();
+        t_.values = values_.data();
+        t_.count = count_.data();
+        return &t_;
+    }
+    void run(const std::vector<uint64_t>& pos, const uint8_t* ops, const Scalar* values) {
+        check(p252_ctree_update(e_->get(), bind(), pos.data(), ops, values, pos.size(), nullptr, P252_MEM_HOST), e_->get());
+    }
+    Engine* e_;
+    p252_ctree t_{};
+    std::vector<uint64_t> keys_, count_, offset_;
+    std::vector<Scalar> values_;
 };
 
 // n x Opening::verify with all openings in one launch: ok[i] != 0 iff paths[i] proves items[i] under root

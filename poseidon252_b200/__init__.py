@@ -16,12 +16,13 @@ from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
 from .hash import Domain, Hash, pack_varlen
-from .merkle import SparseTree, Tree, merkle4_build, merkle4_level
+from .merkle import CompactTree, SparseTree, Tree, merkle4_build, merkle4_level
 
 HADES_WIDTH = hades.WIDTH
 
 __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch", "pack_varlen",
            "encrypt_batch_varlen", "decrypt_batch_varlen", "cipher_offsets", "message_offsets",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
+           "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",
            "DecryptionFailed", "InvalidPoint", "EngineError"]

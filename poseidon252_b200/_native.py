@@ -65,6 +65,9 @@ SIGNATURES = {
     "p252_smtree_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_size_t), c_int]),
     "p252_smtree_len": (c_int, [c_void_p, c_void_p, ctypes.POINTER(c_uint64), c_int]),
     "p252_smtree_open_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
+    "p252_ctree_layout": (c_int, [c_int, c_int, c_uint64, ctypes.POINTER(c_uint64), c_void_p]),
+    "p252_ctree_update": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, ctypes.POINTER(c_size_t), c_int]),
+    "p252_ctree_open_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
     "p252_hash_batch_varlen":(c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t,
                                        ctypes.POINTER(c_size_t), c_int]),
     "p252_encrypt_batch_varlen": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p,
@@ -108,6 +111,13 @@ class SMTree(ctypes.Structure):
     _fields_ = [("struct_size", ctypes.c_uint32), ("arity", ctypes.c_int32), ("height", ctypes.c_int32),
                 ("reserved", ctypes.c_int32), ("capacity", ctypes.c_uint64), ("leaves", ctypes.c_void_p),
                 ("nodes", ctypes.c_void_p), ("present", ctypes.c_void_p)]
+
+
+class CTree(ctypes.Structure):
+    """p252_ctree"""
+    _fields_ = [("struct_size", ctypes.c_uint32), ("arity", ctypes.c_int32), ("height", ctypes.c_int32),
+                ("reserved", ctypes.c_int32), ("max_leaves", ctypes.c_uint64), ("keys", ctypes.c_void_p),
+                ("values", ctypes.c_void_p), ("count", ctypes.c_void_p)]
 
 
 NCCL_UNIQUE_ID_BYTES = 128

@@ -1,6 +1,7 @@
 // C ABI of poseidon252_b200 (include/poseidon252_b200.h): context, host-side sponge bookkeeping
 // (io-pattern checks, tag derivation), staging for HOST buffers, kernel launches, fixed-height trees with batched
 // updates (p252_mtree_*), sparse fixed-height trees with inserts and removals at any position (p252_smtree_*),
+// compact sparse trees stored as sorted present nodes per level (p252_ctree_*),
 // variable-length digest batches (p252_hash_batch_varlen), and the multi-GPU arity-4 tree build
 // (one process per GPU, NCCL all-gather per level).
 //
@@ -1565,6 +1566,294 @@ int p252_smtree_open_batch(p252_ctx* ctx, const p252_smtree* tree, const uint64_
             const p252_fr* src = (l == 0 ? tree->leaves : tree->nodes + L.off[l]) + group * Az;
             memcpy(paths_out + (i * (size_t)H + (size_t)l) * Az, src, Az * sizeof(p252_fr));
             j = group;
+        }
+    }
+    return P252_OK;
+}
+
+}  // extern "C"
+
+// ---- compact sparse trees (p252_ctree) --------------------------------------------------------------------------
+namespace {
+
+struct CLayout {
+    uint64_t slots[p252::kMaxDepth + 1];   // slots of level l
+    uint64_t off[p252::kMaxDepth + 1];     // first slot of level l
+    uint64_t total;
+    uint64_t max_pos;                      // arity^height - 1
+};
+
+// slots[l] = min(max_leaves, A^(H-l)): A^(H-l) is computed only while it stays below 2^63, beyond that it exceeds any
+// max_leaves
+int ctree_layout(int arity, int height, uint64_t max_leaves, CLayout* L) {
+    if (merkle_domain(arity) < 0 || height < 1 || height > p252::kMaxDepth) return P252_ERR_INVALID_ARGUMENT;
+    if (max_leaves == 0 || max_leaves >= 0x80000000ull) return P252_ERR_INVALID_ARGUMENT;
+    const int la = arity == 4 ? 2 : 1;
+    if (la * height > 64) return P252_ERR_INVALID_ARGUMENT;                // arity^height > 2^64
+    uint64_t acc = 0;
+    for (int l = 0; l <= height; ++l) {
+        const int bits = la * (height - l);
+        L->slots[l] = bits >= 63 ? max_leaves : std::min<uint64_t>(max_leaves, 1ull << bits);
+        L->off[l] = acc;
+        acc += L->slots[l];
+    }
+    L->total = acc;
+    L->max_pos = la * height == 64 ? ~0ull : (1ull << (la * height)) - 1;
+    return P252_OK;
+}
+
+int ctree_check(const p252_ctree* t, int flags, CLayout* L) {
+    if (!t || t->struct_size < sizeof(p252_ctree) || !t->keys || !t->values || !t->count) return P252_ERR_INVALID_ARGUMENT;
+    int rc = ctree_layout(t->arity, t->height, t->max_leaves, L);
+    if (rc != P252_OK) return rc;
+    if ((flags & P252_MEM_DEVICE) && (!aligned16(t->values) || (reinterpret_cast<uintptr_t>(t->keys) & 7) ||
+                                      (reinterpret_cast<uintptr_t>(t->count) & 7)))
+        return P252_ERR_INVALID_ARGUMENT;
+    return P252_OK;
+}
+
+// DEVICE update, one stream, no host synchronisation, one stream-ordered allocation:
+//   keys (invalid items flagged in bit 31 of the batch position) -> stable radix sort of (position, batch position)
+//   over bits(arity^height) -> DeviceSelect::Flagged drops the invalid items -> the last item per position is level 0's
+//   change list.  Then for l = 0..height: merge the level's change list into the level out of place (mark, two
+//   exclusive scans, scatter), count, commit gated by the device flag `ok` (level 0 decides it: the new count fits
+//   max_leaves), and for l < height form the next change list: the distinct parents (DeviceSelect::Flagged), their
+//   dense groups gathered from the merged level, hashed by the presence-aware digest over an identity index list.
+//   An empty group comes out absent, i.e. a removal.
+int ctree_update_device(p252_ctx* ctx, p252_ctree* t, const CLayout& L, const uint64_t* pos, const uint8_t* op,
+                        const p252_fr* values, uint32_t n, size_t* n_rejected) {
+    const int A = t->arity, H = t->height, la = A == 4 ? 2 : 1;
+    const uint64_t S = L.slots[0];
+    uint32_t nb[p252::kMaxDepth + 1];                     // bound of level l's change list: min(n, A^(H-l))
+    for (int l = 0; l <= H; ++l) nb[l] = la * (H - l) >= 32 ? n : std::min<uint32_t>(n, 1u << (la * (H - l)));
+    const int end_bit = la * H;
+
+    size_t sort_bytes = 0, select_bytes = 0, scan_bytes = 0, scan2_bytes = 0;
+    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                       (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, 0, end_bit, ctx->stream));
+    CU(cub::DeviceSelect::Flagged(nullptr, select_bytes, (const uint64_t*)nullptr, (const uint8_t*)nullptr, (uint64_t*)nullptr,
+                                  (int*)nullptr, (int)n, ctx->stream));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)S, ctx->stream));
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, scan2_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, ctx->stream));
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    const size_t cub_bytes = up(std::max(std::max(sort_bytes, select_bytes), std::max(scan_bytes, scan2_bytes)));
+    const size_t N = n;
+    const size_t total = 6 * up(N * 8) + 3 * up(N * 4) + up(N) + up(N * 32) + up(N) + up(N * A * 32) + up(N * A) + up(N * 8) +
+                         up(S * 8) + up(S * 32) + 2 * up(S * 4) + 2 * up(N * 4) + up((H + 3) * sizeof(int)) + up(16) + up(8) +
+                         cub_bytes;
+    uint8_t* base = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), total, ctx->stream));
+    uint8_t* p = base;
+    auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
+    uint64_t* keys = reinterpret_cast<uint64_t*>(take(N * 8));
+    uint64_t* skeys = reinterpret_cast<uint64_t*>(take(N * 8));
+    uint64_t* vkeys = reinterpret_cast<uint64_t*>(take(N * 8));       // valid items, sorted
+    uint64_t* ck[2] = {reinterpret_cast<uint64_t*>(take(N * 8)), reinterpret_cast<uint64_t*>(take(N * 8))};
+    uint64_t* parent = reinterpret_cast<uint64_t*>(take(N * 8));
+    uint32_t* bpos = reinterpret_cast<uint32_t*>(take(N * 4));
+    uint32_t* sbpos = reinterpret_cast<uint32_t*>(take(N * 4));
+    uint32_t* vbpos = reinterpret_cast<uint32_t*>(take(N * 4));
+    uint8_t* flag = take(N);
+    p252_fr* cval = reinterpret_cast<p252_fr*>(take(N * 32));          // change values (level 0, then the digests)
+    uint8_t* cpres = take(N);
+    p252_fr* groups = reinterpret_cast<p252_fr*>(take(N * A * 32));
+    uint8_t* gpres = take(N * A);
+    uint64_t* iota = reinterpret_cast<uint64_t*>(take(N * 8));
+    uint64_t* okeys = reinterpret_cast<uint64_t*>(take(S * 8));       // the merged level
+    p252_fr* ovals = reinterpret_cast<p252_fr*>(take(S * 32));
+    uint32_t* kept = reinterpret_cast<uint32_t*>(take(S * 4));
+    uint32_t* K = reinterpret_cast<uint32_t*>(take(S * 4));
+    uint32_t* ins = reinterpret_cast<uint32_t*>(take(N * 4));
+    uint32_t* I = reinterpret_cast<uint32_t*>(take(N * 4));
+    int* cnt = reinterpret_cast<int*>(take((H + 3) * sizeof(int)));  // [0] valid items, [1 + l] level l's change list
+    uint64_t* stats = reinterpret_cast<uint64_t*>(take(16));
+    uint32_t* ok = reinterpret_cast<uint32_t*>(take(8));
+    void* cub_tmp = take(cub_bytes);
+
+    auto launched = [&](cudaError_t le) -> int {
+        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+        ctx->launches++;
+        return P252_OK;
+    };
+    auto body = [&]() -> int {
+        int rc;
+        if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        unsigned long long* rej = n_rejected ? ctx->d_counter : nullptr;
+        if ((rc = launched(p252::launch_ctree_keys(pos, op, n, L.max_pos, keys, bpos, rej, ctx->stream))) != P252_OK) return rc;
+        size_t b = cub_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, skeys, bpos, sbpos, (int)n, 0, end_bit, ctx->stream));
+        if ((rc = launched(p252::launch_ctree_valid(sbpos, n, flag, ctx->stream))) != P252_OK) return rc;
+        b = cub_bytes;
+        CU(cub::DeviceSelect::Flagged(cub_tmp, b, skeys, flag, vkeys, cnt, (int)n, ctx->stream));
+        b = cub_bytes;
+        CU(cub::DeviceSelect::Flagged(cub_tmp, b, sbpos, flag, vbpos, cnt, (int)n, ctx->stream));
+        if ((rc = launched(p252::launch_ctree_last(vkeys, cnt, n, flag, ctx->stream))) != P252_OK) return rc;
+        b = cub_bytes;
+        CU(cub::DeviceSelect::Flagged(cub_tmp, b, vkeys, flag, ck[0], cnt + 1, (int)n, ctx->stream));
+        b = cub_bytes;
+        CU(cub::DeviceSelect::Flagged(cub_tmp, b, vbpos, flag, bpos, cnt + 1, (int)n, ctx->stream));
+        if ((rc = launched(p252::launch_ctree_leaf_changes(bpos, cnt + 1, n, op, values, cval, cpres, ctx->stream))) != P252_OK)
+            return rc;
+        if ((rc = launched(p252::launch_ctree_iota(iota, n, ctx->stream))) != P252_OK) return rc;
+        p252_fr tag;
+        p252_hash_tag(merkle_domain(A), (size_t)A, 1, &tag);
+        for (int l = 0; l <= H; ++l) {
+            const uint64_t s = L.slots[l];
+            uint64_t* lk = t->keys + L.off[l];
+            p252_fr* lv = t->values + L.off[l];
+            uint64_t* lc = t->count + l;
+            const uint64_t* c = ck[l & 1];
+            const int* cc = cnt + 1 + l;
+            if ((rc = launched(p252::launch_ctree_mark(lk, lc, s, c, cc, nb[l], cpres, kept, ins, ctx->stream))) != P252_OK)
+                return rc;
+            b = cub_bytes;
+            CU(cub::DeviceScan::ExclusiveSum(cub_tmp, b, kept, K, (int)s, ctx->stream));
+            b = cub_bytes;
+            CU(cub::DeviceScan::ExclusiveSum(cub_tmp, b, ins, I, (int)nb[l], ctx->stream));
+            if ((rc = launched(p252::launch_ctree_scatter(lk, lv, lc, s, c, cval, cc, nb[l], kept, K, ins, I, okeys, ovals,
+                                                          ctx->stream))) != P252_OK)
+                return rc;
+            if ((rc = launched(p252::launch_ctree_count(lc, s, nb[l], kept, K, ins, I, l == 0, n, stats, ok, rej, ctx->stream))) !=
+                P252_OK)
+                return rc;
+            if ((rc = launched(p252::launch_ctree_commit(okeys, ovals, s, stats, ok, lk, lv, lc, ctx->stream))) != P252_OK)
+                return rc;
+            if (l == H) break;
+            // the next level's change list: distinct parents, their groups from the merged level, hashed
+            if ((rc = launched(p252::launch_ctree_parents(c, cc, nb[l], A, flag, parent, ctx->stream))) != P252_OK) return rc;
+            b = cub_bytes;
+            CU(cub::DeviceSelect::Flagged(cub_tmp, b, parent, flag, ck[(l + 1) & 1], cnt + 2 + l, (int)nb[l], ctx->stream));
+            if ((rc = launched(p252::launch_ctree_gather(okeys, ovals, stats, s, ck[(l + 1) & 1], cnt + 2 + l, nb[l + 1], A, groups,
+                                                         gpres, ctx->stream))) != P252_OK)
+                return rc;
+            if ((rc = launched(p252::launch_smtree_digest(limbs(&tag), groups, gpres, A, cval, cpres, iota, cnt + 2 + l, nb[l + 1],
+                                                          ctx->coop_max, ctx->stream))) != P252_OK)
+                return rc;
+        }
+        return counter_end(ctx, n_rejected);
+    };
+    int rc = body();
+    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
+    if (rc != P252_OK) return rc;
+    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
+    return P252_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int p252_ctree_layout(int arity, int height, uint64_t max_leaves, uint64_t* total_slots, uint64_t* level_offset) {
+    CLayout L;
+    int rc = ctree_layout(arity, height, max_leaves, &L);
+    if (rc != P252_OK) return rc;
+    if (total_slots) *total_slots = L.total;
+    if (level_offset)
+        for (int l = 0; l <= height; ++l) level_offset[l] = L.off[l];
+    return P252_OK;
+}
+
+int p252_ctree_update(p252_ctx* ctx, p252_ctree* tree, const uint64_t* pos, const uint8_t* op, const p252_fr* values,
+                      size_t n, size_t* n_rejected, int flags) {
+    CLayout L;
+    if (!ctx || (n && (!pos || !values))) return P252_ERR_INVALID_ARGUMENT;
+    int rc = ctree_check(tree, flags, &L);
+    if (rc != P252_OK) return rc;
+    if (n >= 0x80000000ull) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_rejected) *n_rejected = 0;
+    if (flags & P252_MEM_DEVICE) {
+        if (n && (!aligned16(values) || (reinterpret_cast<uintptr_t>(pos) & 7))) return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        rc = ctree_update_device(ctx, tree, L, pos, op, values, (uint32_t)n, n_rejected);
+        if (rc != P252_OK) return rc;
+        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        return P252_OK;
+    }
+    for (size_t i = 0; i < n; ++i)
+        if (pos[i] > L.max_pos || (op && op[i] > 1)) return P252_ERR_INVALID_ARGUMENT;
+    if (n == 0) return P252_OK;
+    // HOST: stage the tree and the batch, run the device path, copy the tree back unless the batch was refused (every
+    // item is valid here, so a non-zero rejection count means a capacity overflow)
+    const size_t H1 = (size_t)tree->height + 1;
+    const size_t kb = L.total * 8, vb = L.total * sizeof(p252_fr), cb = H1 * 8;
+    const size_t up_kb = (kb + 255) / 256 * 256, up_cb = (cb + 255) / 256 * 256, up_vb = (vb + 255) / 256 * 256;
+    const size_t pb = (n * 8 + 255) / 256 * 256, ob = (n + 255) / 256 * 256;
+    uint8_t* base = nullptr;
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), up_vb + up_kb + up_cb + n * sizeof(p252_fr) + pb + ob, ctx->stream));
+    p252_ctree dt = *tree;
+    dt.values = reinterpret_cast<p252_fr*>(base);
+    dt.keys = reinterpret_cast<uint64_t*>(base + up_vb);
+    dt.count = reinterpret_cast<uint64_t*>(base + up_vb + up_kb);
+    p252_fr* d_vals = reinterpret_cast<p252_fr*>(base + up_vb + up_kb + up_cb);
+    uint64_t* d_pos = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(d_vals) + n * sizeof(p252_fr));
+    uint8_t* d_op = op ? reinterpret_cast<uint8_t*>(d_pos) + pb : nullptr;
+    size_t refused = 0;
+    cudaError_t e = cudaMemcpyAsync(dt.values, tree->values, vb, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dt.keys, tree->keys, kb, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dt.count, tree->count, cb, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_vals, values, n * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(d_pos, pos, n * 8, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess && op) e = cudaMemcpyAsync(d_op, op, n, cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) {
+        rc = fail_cuda(ctx, e, "ctree staging");
+    } else {
+        rc = ctree_update_device(ctx, &dt, L, d_pos, d_op, d_vals, (uint32_t)n, &refused);
+        if (rc == P252_OK) e = cudaStreamSynchronize(ctx->stream);   // publishes `refused`
+        if (rc == P252_OK && e == cudaSuccess && refused == 0) {
+            e = cudaMemcpyAsync(tree->values, dt.values, vb, cudaMemcpyDeviceToHost, ctx->stream);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->keys, dt.keys, kb, cudaMemcpyDeviceToHost, ctx->stream);
+            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->count, dt.count, cb, cudaMemcpyDeviceToHost, ctx->stream);
+        }
+        if (rc == P252_OK && e != cudaSuccess) rc = fail_cuda(ctx, e, "ctree D2H");
+    }
+    cudaFreeAsync(base, ctx->stream);
+    e = cudaStreamSynchronize(ctx->stream);
+    if (rc != P252_OK) return rc;
+    if (e != cudaSuccess) return fail_cuda(ctx, e, "ctree update");
+    return refused ? P252_ERR_INVALID_ARGUMENT : P252_OK;
+}
+
+int p252_ctree_open_batch(p252_ctx* ctx, const p252_ctree* tree, const uint64_t* pos, size_t n, p252_fr* paths_out, int flags) {
+    CLayout L;
+    if (!ctx || ((!pos || !paths_out) && n)) return P252_ERR_INVALID_ARGUMENT;
+    int rc = ctree_check(tree, flags, &L);
+    if (rc != P252_OK) return rc;
+    const int A = tree->arity, H = tree->height, la = A == 4 ? 2 : 1;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(paths_out) || (reinterpret_cast<uintptr_t>(pos) & 7)) return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        p252::OpenLevels lv{};
+        for (int l = 0; l < H; ++l) lv.off[l] = L.off[l];
+        return finish_device_call(ctx, p252::launch_ctree_open(tree->keys, tree->values, tree->count, pos, n, A, (uint32_t)H, lv,
+                                                               paths_out, ctx->stream), flags);
+    }
+    // HOST: binary searches over the sorted levels
+    auto find = [&](int l, uint64_t key) -> uint64_t {   // first entry of level l whose index is >= key
+        const uint64_t* k = tree->keys + L.off[l];
+        return (uint64_t)(std::lower_bound(k, k + std::min(tree->count[l], L.slots[l]), key) - k);
+    };
+    for (size_t i = 0; i < n; ++i) {
+        const uint64_t j = find(0, pos[i]);
+        if (j >= std::min(tree->count[0], L.slots[0]) || tree->keys[j] != pos[i]) return P252_ERR_INVALID_ARGUMENT;
+    }
+    const uint64_t Az = (uint64_t)A;
+    for (size_t i = 0; i < n; ++i) {
+        for (int l = 0; l < H; ++l) {
+            const uint64_t first = (pos[i] >> (la * l)) >> la << la;
+            const uint64_t c = std::min(tree->count[l], L.slots[l]);
+            const uint64_t* k = tree->keys + L.off[l];
+            uint64_t j = find(l, first);
+            p252_fr* dst = paths_out + (i * (size_t)H + (size_t)l) * Az;
+            for (uint64_t q = 0; q < Az; ++q) {
+                if (j < c && k[j] == first + q)
+                    dst[q] = tree->values[L.off[l] + j++];
+                else
+                    memset(&dst[q], 0, sizeof(p252_fr));
+            }
         }
     }
     return P252_OK;

@@ -671,6 +671,231 @@ __global__ void __launch_bounds__(256) k_smtree_count(const uint8_t* __restrict_
     if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
+// ---- compact sparse trees: sorted (index, value) lists per level (p252_ctree) -----------------------------------------
+// A change list is (key, value, present) sorted by key with distinct keys: present 1 inserts or overwrites, 0 removes.
+// Level l's merge takes its sorted list (keys / values, count on the device) and its change list to a new sorted list
+// out of place; the dirty parents of level l + 1 are gathered from the new list and hashed by launch_smtree_digest.
+
+// first index in a[0, n) whose key is >= k
+__device__ __forceinline__ uint64_t ctree_lower_bound(const uint64_t* __restrict__ a, uint64_t n, uint64_t k) {
+    uint64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi) >> 1;
+        if (a[mid] < k)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    return lo;
+}
+
+// exclusive prefix sum at x of flags f[0, s) with scan e: x == s is the total
+__device__ __forceinline__ uint64_t ctree_excl(const uint32_t* __restrict__ e, const uint32_t* __restrict__ f, uint64_t s,
+                                               uint64_t x) {
+    return x < s ? e[x] : (uint64_t)e[s - 1] + f[s - 1];
+}
+
+// k_ctree_keys: one thread per batch item.  keys[i] = pos[i]; bpos[i] = i, with bit 31 set for an invalid item (pos >
+// max_pos, or op not 0/1), which is counted into *rejected.  No key value is free to act as a sentinel.
+__global__ void __launch_bounds__(256) k_ctree_keys(const uint64_t* __restrict__ pos, const uint8_t* __restrict__ op, uint32_t n,
+                                                    uint64_t max_pos, uint64_t* __restrict__ keys, uint32_t* __restrict__ bpos,
+                                                    unsigned long long* __restrict__ rejected) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t key = pos[i];
+    const bool bad = key > max_pos || (op && op[i] > 1);
+    keys[i] = key;
+    bpos[i] = i | (bad ? 0x80000000u : 0u);
+    if (rejected) {
+        const unsigned act = __activemask();
+        const unsigned b = __ballot_sync(act, bad);
+        if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(b));
+    }
+}
+
+// k_ctree_valid: flag[k] = the sorted item k is valid (bit 31 of its batch position clear)
+__global__ void __launch_bounds__(256) k_ctree_valid(const uint32_t* __restrict__ bpos, uint32_t n, uint8_t* __restrict__ flag) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) flag[i] = (bpos[i] >> 31) == 0;
+}
+
+// k_ctree_last: over the valid items sorted stably by position (count *cnt <= n), flag the last of every run of equal
+// positions: the last operation in batch order
+__global__ void __launch_bounds__(256) k_ctree_last(const uint64_t* __restrict__ keys, const int* __restrict__ cnt, uint32_t n,
+                                                    uint8_t* __restrict__ flag) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t c = (uint32_t)*cnt;
+    flag[i] = i < c && (i + 1 == c || keys[i + 1] != keys[i]);
+}
+
+// k_ctree_leaf_changes: level 0's change list from the last operation per position: value and present = insert
+__global__ void __launch_bounds__(256) k_ctree_leaf_changes(const uint32_t* __restrict__ bpos, const int* __restrict__ cnt,
+                                                            uint32_t n, const uint8_t* __restrict__ op,
+                                                            const uint8_t* __restrict__ values, uint8_t* __restrict__ cval,
+                                                            uint8_t* __restrict__ cpres) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n || i >= (uint32_t)*cnt) return;
+    const uint32_t p = bpos[i];
+    const bool insert = !op || op[p] == 0;
+    uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (insert) load_fr(v, values + (size_t)p * 32);
+    store_fr(cval + (size_t)i * 32, v);
+    cpres[i] = insert ? 1 : 0;
+}
+
+// k_ctree_mark: kept[t] (t < s) = old entry t exists and no change has its key; ins[t] (t < nb) = change t inserts
+__global__ void __launch_bounds__(256) k_ctree_mark(const uint64_t* __restrict__ lkeys, const uint64_t* __restrict__ lcount,
+                                                    uint64_t s, const uint64_t* __restrict__ ckeys, const int* __restrict__ ccnt,
+                                                    uint32_t nb, const uint8_t* __restrict__ cpres, uint32_t* __restrict__ kept,
+                                                    uint32_t* __restrict__ ins) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t cn = (uint64_t)*ccnt;
+    if (t < s) {
+        bool k = t < *lcount;
+        if (k) {
+            const uint64_t key = lkeys[t];
+            const uint64_t j = ctree_lower_bound(ckeys, cn, key);
+            k = j == cn || ckeys[j] != key;
+        }
+        kept[t] = k;
+    }
+    if (t < nb) ins[t] = t < cn && cpres[t];
+}
+
+// k_ctree_scatter: the merge.  A kept old entry t goes to K(t) + I(changes below its key), an inserting change t to
+// I(t) + K(old entries below its key) (K / I: exclusive scans of kept / ins).  Writes at or past s are dropped: only a
+// level-0 overflow produces them, and then nothing is committed.
+__global__ void __launch_bounds__(256) k_ctree_scatter(const uint64_t* __restrict__ lkeys, const uint8_t* __restrict__ lvals,
+                                                       const uint64_t* __restrict__ lcount, uint64_t s,
+                                                       const uint64_t* __restrict__ ckeys, const uint8_t* __restrict__ cvals,
+                                                       const int* __restrict__ ccnt, uint32_t nb, const uint32_t* __restrict__ kept,
+                                                       const uint32_t* __restrict__ K, const uint32_t* __restrict__ ins,
+                                                       const uint32_t* __restrict__ I, uint64_t* __restrict__ okeys,
+                                                       uint8_t* __restrict__ ovals) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint64_t cn = (uint64_t)*ccnt;
+    if (t < s && kept[t]) {
+        const uint64_t key = lkeys[t];
+        const uint64_t p = K[t] + (nb ? ctree_excl(I, ins, nb, ctree_lower_bound(ckeys, cn, key)) : 0);
+        if (p < s) {
+            uint32_t v[8];
+            load_fr(v, lvals + t * 32);
+            okeys[p] = key;
+            store_fr(ovals + p * 32, v);
+        }
+    }
+    if (t < nb && ins[t]) {
+        const uint64_t key = ckeys[t];
+        const uint64_t p = I[t] + ctree_excl(K, kept, s, ctree_lower_bound(lkeys, *lcount, key));
+        if (p < s) {
+            uint32_t v[8];
+            load_fr(v, cvals + t * 32);
+            okeys[p] = key;
+            store_fr(ovals + p * 32, v);
+        }
+    }
+}
+
+// k_ctree_count (one thread): st = {old count, new count}.  Level 0 decides the commit flag: the new count fits the
+// level's s slots; a refused batch reports every item as rejected.
+__global__ void k_ctree_count(const uint64_t* __restrict__ lcount, uint64_t s, uint32_t nb, const uint32_t* __restrict__ kept,
+                              const uint32_t* __restrict__ K, const uint32_t* __restrict__ ins, const uint32_t* __restrict__ I,
+                              bool level0, uint32_t n, uint64_t* __restrict__ st, uint32_t* __restrict__ ok,
+                              unsigned long long* __restrict__ rejected) {
+    const uint64_t c = ctree_excl(K, kept, s, s) + (nb ? ctree_excl(I, ins, nb, nb) : 0);
+    st[0] = *lcount;
+    st[1] = c;
+    if (level0) {
+        *ok = c <= s;
+        if (c > s && rejected) *rejected = n;
+    }
+}
+
+// k_ctree_commit: if *ok, level := the merged list; slots past the new count that held entries are zeroed (every slot
+// past the old count is already zero)
+__global__ void __launch_bounds__(256) k_ctree_commit(const uint64_t* __restrict__ okeys, const uint8_t* __restrict__ ovals,
+                                                      uint64_t s, const uint64_t* __restrict__ st, const uint32_t* __restrict__ ok,
+                                                      uint64_t* __restrict__ lkeys, uint8_t* __restrict__ lvals,
+                                                      uint64_t* __restrict__ lcount) {
+    const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= s || !*ok) return;
+    const uint64_t old = st[0], c = st[1];
+    if (t == 0) *lcount = c;
+    uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (t < c) {
+        load_fr(v, ovals + t * 32);
+        lkeys[t] = okeys[t];
+        store_fr(lvals + t * 32, v);
+    } else if (t < old) {
+        lkeys[t] = 0;
+        store_fr(lvals + t * 32, v);
+    }
+}
+
+// k_ctree_parents: candidates of the next level's change list, key / arity of a sorted change list (first of each run)
+__global__ void __launch_bounds__(256) k_ctree_parents(const uint64_t* __restrict__ ckeys, const int* __restrict__ ccnt, uint32_t nb,
+                                                       uint32_t log2_arity, uint8_t* __restrict__ flag, uint64_t* __restrict__ parent) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nb) return;
+    const uint64_t par = ckeys[t] >> log2_arity;
+    flag[t] = t < (uint32_t)*ccnt && (t == 0 || (ckeys[t - 1] >> log2_arity) != par);
+    parent[t] = par;
+}
+
+// k_ctree_gather: one thread per dirty parent g: its arity children in the merged level (binary search for g * arity,
+// then at most arity consecutive entries) as a dense group, absent slots 0, and their presence bytes
+__global__ void __launch_bounds__(256) k_ctree_gather(const uint64_t* __restrict__ okeys, const uint8_t* __restrict__ ovals,
+                                                      const uint64_t* __restrict__ st, uint64_t s, const uint64_t* __restrict__ pkeys,
+                                                      const int* __restrict__ pcnt, uint32_t nb, uint32_t log2_arity,
+                                                      uint8_t* __restrict__ groups, uint8_t* __restrict__ gpres) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= nb || t >= (uint32_t)*pcnt) return;
+    const uint32_t arity = 1u << log2_arity;
+    const uint64_t c = st[1] < s ? st[1] : s;
+    const uint64_t base = pkeys[t] << log2_arity;
+    uint64_t p = ctree_lower_bound(okeys, c, base);
+    for (uint32_t q = 0; q < arity; ++q) {
+        uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        const bool here = p < c && okeys[p] == base + q;
+        if (here) load_fr(v, ovals + (p++) * 32);
+        store_fr(groups + ((size_t)t * arity + q) * 32, v);
+        gpres[(size_t)t * arity + q] = here ? 1 : 0;
+    }
+}
+
+__global__ void __launch_bounds__(256) k_ctree_iota(uint64_t* __restrict__ d, uint32_t n) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n) d[t] = t;
+}
+
+// k_ctree_open: one thread per (opening, level) as k_merkle_open.  The leaf must be present in level 0 (binary search),
+// otherwise the opening is all zero; the sibling group of level l is found by a binary search for its first index.
+__global__ void __launch_bounds__(256) k_ctree_open(const uint64_t* __restrict__ keys, const uint8_t* __restrict__ vals,
+                                                    const uint64_t* __restrict__ count, const uint64_t* __restrict__ pos, size_t n,
+                                                    uint32_t log2_arity, uint32_t depth, OpenLevels lv, uint8_t* __restrict__ paths) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n * depth) return;
+    const size_t item = t / depth;
+    const uint32_t level = (uint32_t)(t - item * depth);
+    const uint32_t arity = 1u << log2_arity;
+    const uint64_t idx = pos[item];
+    uint8_t* dst = paths + ((size_t)item * depth + level) * arity * 32;
+    const uint64_t c0 = count[0];
+    const uint64_t j0 = ctree_lower_bound(keys, c0, idx);
+    const bool present = j0 < c0 && keys[j0] == idx;
+    const uint64_t* lk = keys + lv.off[level];
+    const uint8_t* lvv = vals + lv.off[level] * 32;
+    const uint64_t c = present ? count[level] : 0;
+    const uint64_t base = (idx >> (log2_arity * level)) >> log2_arity << log2_arity;
+    uint64_t p = ctree_lower_bound(lk, c, base);
+    for (uint32_t q = 0; q < arity; ++q) {
+        uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        if (p < c && lk[p] == base + q) load_fr(v, lvv + (p++) * 32);
+        store_fr(dst + q * 32, v);
+    }
+}
+
 // k_merkle_verify: one thread per opening, `depth` chained Merkle digests (Hash::digest(Domain::MerkleA, group),
 // src/hash.rs:22-31,191-195) with the membership check of every level fused in:
 //   cur = leaf;  for l: require group[l][pos_l] == cur;  cur = digest(group[l]);   finally require cur == root.
@@ -1348,6 +1573,92 @@ cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned lon
     if (n == 0) return cudaSuccess;
     const uint64_t blocks = (n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096;
     k_smtree_count<<<(unsigned)blocks, 256, 0, st>>>(present, n, out);
+    return cudaGetLastError();
+}
+
+static unsigned blocks256(uint64_t n) { return (unsigned)((n + 255) / 256); }
+
+cudaError_t launch_ctree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t max_pos, uint64_t* keys, uint32_t* bpos,
+                              unsigned long long* rejected, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_ctree_keys<<<blocks256(n), 256, 0, st>>>(pos, op, n, max_pos, keys, bpos, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_valid(const uint32_t* bpos, uint32_t n, uint8_t* flag, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_ctree_valid<<<blocks256(n), 256, 0, st>>>(bpos, n, flag);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_last(const uint64_t* keys, const int* cnt, uint32_t n, uint8_t* flag, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_ctree_last<<<blocks256(n), 256, 0, st>>>(keys, cnt, n, flag);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_leaf_changes(const uint32_t* bpos, const int* cnt, uint32_t n, const uint8_t* op, const void* values,
+                                      void* cval, uint8_t* cpres, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_ctree_leaf_changes<<<blocks256(n), 256, 0, st>>>(bpos, cnt, n, op, static_cast<const uint8_t*>(values),
+                                                      static_cast<uint8_t*>(cval), cpres);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_mark(const uint64_t* lkeys, const uint64_t* lcount, uint64_t s, const uint64_t* ckeys, const int* ccnt,
+                              uint32_t nb, const uint8_t* cpres, uint32_t* kept, uint32_t* ins, cudaStream_t st) {
+    k_ctree_mark<<<blocks256(s > nb ? s : nb), 256, 0, st>>>(lkeys, lcount, s, ckeys, ccnt, nb, cpres, kept, ins);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_scatter(const uint64_t* lkeys, const void* lvals, const uint64_t* lcount, uint64_t s,
+                                 const uint64_t* ckeys, const void* cvals, const int* ccnt, uint32_t nb, const uint32_t* kept,
+                                 const uint32_t* K, const uint32_t* ins, const uint32_t* I, uint64_t* okeys, void* ovals,
+                                 cudaStream_t st) {
+    k_ctree_scatter<<<blocks256(s > nb ? s : nb), 256, 0, st>>>(lkeys, static_cast<const uint8_t*>(lvals), lcount, s, ckeys,
+                                                               static_cast<const uint8_t*>(cvals), ccnt, nb, kept, K, ins, I,
+                                                               okeys, static_cast<uint8_t*>(ovals));
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_count(const uint64_t* lcount, uint64_t s, uint32_t nb, const uint32_t* kept, const uint32_t* K,
+                               const uint32_t* ins, const uint32_t* I, bool level0, uint32_t n, uint64_t* stats, uint32_t* ok,
+                               unsigned long long* rejected, cudaStream_t st) {
+    k_ctree_count<<<1, 1, 0, st>>>(lcount, s, nb, kept, K, ins, I, level0, n, stats, ok, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_commit(const uint64_t* okeys, const void* ovals, uint64_t s, const uint64_t* stats, const uint32_t* ok,
+                                uint64_t* lkeys, void* lvals, uint64_t* lcount, cudaStream_t st) {
+    k_ctree_commit<<<blocks256(s), 256, 0, st>>>(okeys, static_cast<const uint8_t*>(ovals), s, stats, ok, lkeys,
+                                                 static_cast<uint8_t*>(lvals), lcount);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_parents(const uint64_t* ckeys, const int* ccnt, uint32_t nb, int arity, uint8_t* flag, uint64_t* parent,
+                                 cudaStream_t st) {
+    k_ctree_parents<<<blocks256(nb), 256, 0, st>>>(ckeys, ccnt, nb, arity == 4 ? 2u : 1u, flag, parent);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_gather(const uint64_t* okeys, const void* ovals, const uint64_t* stats, uint64_t s, const uint64_t* pkeys,
+                                const int* pcnt, uint32_t nb, int arity, void* groups, uint8_t* gpres, cudaStream_t st) {
+    k_ctree_gather<<<blocks256(nb), 256, 0, st>>>(okeys, static_cast<const uint8_t*>(ovals), stats, s, pkeys, pcnt, nb,
+                                                  arity == 4 ? 2u : 1u, static_cast<uint8_t*>(groups), gpres);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_iota(uint64_t* d, uint32_t n, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_ctree_iota<<<blocks256(n), 256, 0, st>>>(d, n);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ctree_open(const uint64_t* keys, const void* values, const uint64_t* count, const uint64_t* pos, size_t n,
+                              int arity, uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st) {
+    if (n == 0 || depth == 0) return cudaSuccess;
+    k_ctree_open<<<(unsigned)((n * depth + 255) / 256), 256, 0, st>>>(keys, static_cast<const uint8_t*>(values), count, pos, n,
+                                                                     arity == 4 ? 2u : 1u, depth, lv, static_cast<uint8_t*>(paths));
     return cudaGetLastError();
 }
 

@@ -63,6 +63,44 @@ cudaError_t launch_smtree_digest(const uint64_t tag[4], const void* below, const
                                  cudaStream_t st);
 // *out += non-zero bytes of present[0, n)
 cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned long long* out, cudaStream_t st);
+// Compact sparse trees (p252_ctree).  A change list is (keys, values, present) sorted by distinct key, count on the device;
+// a level is (keys, values) sorted, count on the device, s slots.  keys: keys[i] = pos[i], bpos[i] = i | (invalid << 31)
+// (invalid: pos > max_pos or op not NULL / 0 / 1, counted into *rejected)
+cudaError_t launch_ctree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t max_pos, uint64_t* keys, uint32_t* bpos,
+                              unsigned long long* rejected, cudaStream_t st);
+// flag[k] = bit 31 of bpos[k] is clear
+cudaError_t launch_ctree_valid(const uint32_t* bpos, uint32_t n, uint8_t* flag, cudaStream_t st);
+// flag[i] = i < *cnt and i is the last of its run of equal keys
+cudaError_t launch_ctree_last(const uint64_t* keys, const int* cnt, uint32_t n, uint8_t* flag, cudaStream_t st);
+// level 0's change values / presence from the batch positions of the last operation per position
+cudaError_t launch_ctree_leaf_changes(const uint32_t* bpos, const int* cnt, uint32_t n, const uint8_t* op, const void* values,
+                                      void* cval, uint8_t* cpres, cudaStream_t st);
+// kept[t < s]: old entry t survives (present, no change with its key); ins[t < nb]: change t inserts
+cudaError_t launch_ctree_mark(const uint64_t* lkeys, const uint64_t* lcount, uint64_t s, const uint64_t* ckeys, const int* ccnt,
+                              uint32_t nb, const uint8_t* cpres, uint32_t* kept, uint32_t* ins, cudaStream_t st);
+// merge into (okeys, ovals) with K / I the exclusive scans of kept / ins; writes at or past s are dropped
+cudaError_t launch_ctree_scatter(const uint64_t* lkeys, const void* lvals, const uint64_t* lcount, uint64_t s,
+                                 const uint64_t* ckeys, const void* cvals, const int* ccnt, uint32_t nb, const uint32_t* kept,
+                                 const uint32_t* K, const uint32_t* ins, const uint32_t* I, uint64_t* okeys, void* ovals,
+                                 cudaStream_t st);
+// stats = {old count, new count}; level0: *ok = new count <= s, and a refusal sets *rejected = n
+cudaError_t launch_ctree_count(const uint64_t* lcount, uint64_t s, uint32_t nb, const uint32_t* kept, const uint32_t* K,
+                               const uint32_t* ins, const uint32_t* I, bool level0, uint32_t n, uint64_t* stats, uint32_t* ok,
+                               unsigned long long* rejected, cudaStream_t st);
+// if *ok: the level and its count become the merged list, vacated slots zeroed
+cudaError_t launch_ctree_commit(const uint64_t* okeys, const void* ovals, uint64_t s, const uint64_t* stats, const uint32_t* ok,
+                                uint64_t* lkeys, void* lvals, uint64_t* lcount, cudaStream_t st);
+// next-level candidates: parent[t] = ckeys[t] / arity, flag = first of its run (t < *ccnt)
+cudaError_t launch_ctree_parents(const uint64_t* ckeys, const int* ccnt, uint32_t nb, int arity, uint8_t* flag, uint64_t* parent,
+                                 cudaStream_t st);
+// dense groups (arity scalars, absent 0) and presence bytes of the dirty parents pkeys[0..*pcnt) from the merged level
+cudaError_t launch_ctree_gather(const uint64_t* okeys, const void* ovals, const uint64_t* stats, uint64_t s, const uint64_t* pkeys,
+                                const int* pcnt, uint32_t nb, int arity, void* groups, uint8_t* gpres, cudaStream_t st);
+// d[t] = t
+cudaError_t launch_ctree_iota(uint64_t* d, uint32_t n, cudaStream_t st);
+// openings in the format of launch_merkle_open; lv.off[l] = first slot of level l; an absent leaf gets an all-zero opening
+cudaError_t launch_ctree_open(const uint64_t* keys, const void* values, const uint64_t* count, const uint64_t* pos, size_t n,
+                              int arity, uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st);
 cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], const void* leaf_items,
                                  const uint64_t* leaf_idx, const void* paths, size_t n, int arity, uint32_t depth,
                                  uint8_t* ok, unsigned long long* n_failed, cudaStream_t st);

@@ -647,6 +647,75 @@ class Engine:
                                                      flags | (_native.ASYNC if async_ and flags else 0)))
         return res
 
+    # -- compact sparse trees: sorted present nodes per level (p252_ctree) --------------------------------------------
+    def ctree_layout(self, arity, height, max_leaves):
+        return ctree_layout(arity, height, max_leaves)
+
+    def _words(self, x, like, name, n):
+        """The caller's own writable 1-D buffer of n 64-bit words in the memory space of `like` -> pointer (no copy)."""
+        if _is_torch(like):
+            if not _is_torch(x) or not x.is_cuda or x.device != like.device or \
+                    str(x.dtype) not in ("torch.int64", "torch.uint64") or not x.is_contiguous() or tuple(x.shape) != (n,):
+                raise EngineError(-1, "%s must be a contiguous int64/uint64 tensor of shape (%d,) on %s" % (name, n, like.device))
+            return x.data_ptr()
+        if not isinstance(x, np.ndarray) or x.dtype != np.uint64 or tuple(x.shape) != (n,) or not x.flags.c_contiguous \
+                or not x.flags.writeable:
+            raise EngineError(-1, "%s must be a writable C-contiguous uint64 array of shape (%d,)" % (name, n))
+        return x.ctypes.data
+
+    def _ctree(self, tree):
+        """tree: anything with arity / height / max_leaves / keys (total_slots,) / values (total_slots, 4) / count
+        (height + 1,) -> (p252_ctree, flags, keepalive)."""
+        total, _ = self.ctree_layout(tree.arity, tree.height, tree.max_leaves)
+        vp, vlead, flags, vk = self._in(tree.values, (4,))
+        self._same_lead("values", vlead, total)
+        if not _is_torch(vk) and (vk is not tree.values or not vk.flags.writeable):
+            raise EngineError(-1, "host tree buffers must be writable C-contiguous uint64 arrays")
+        kp = self._words(tree.keys, vk, "keys", total)
+        cp = self._words(tree.count, vk, "count", int(tree.height) + 1)
+        t = _native.CTree(ctypes.sizeof(_native.CTree), int(tree.arity), int(tree.height), 0, int(tree.max_leaves), kp, vp, cp)
+        return t, flags, (vk, tree.keys, tree.count)
+
+    def ctree_update(self, tree, pos, values=None, op=None, async_=False):
+        """One batch of operations on a compact sparse tree: op[i] = 0 inserts / overwrites values[i] at pos[i], op[i] = 1
+        removes pos[i] (op None: all inserts; values None: all zeros, for a batch of removals).  Equal to applying them
+        in batch order.  Device items with pos >= arity^height or an op other than 0/1 are skipped and counted
+        (last_ctree_rejected()); a device batch that would leave more than max_leaves present positions changes nothing
+        and counts every item as rejected.  Host: either raises and changes nothing."""
+        t, flags, keep = self._ctree(tree)
+        like = keep[0]
+        ip, n, ik = self._idx(pos, like, "pos")
+        if values is None:
+            values = self._out_like(like, (n, 4))
+            values[:] = 0
+            if async_ and flags:
+                self._pending_counters.append(values)      # read by the device after this call returns
+        vp, vlead, fv, vk = self._in(values, (4,))
+        if fv != flags:
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("values", vlead, n)
+        opp, ok_ = (None, None) if op is None else self._bytes(op, like, "op", n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._ctrej = self._counter(flags)
+        self._check(self._lib.p252_ctree_update(self._ctx, ctypes.byref(t), ip if n else None, opp if n else None,
+                                                vp if n else None, n, ctypes.byref(self._ctrej), flags))
+
+    def last_ctree_rejected(self):
+        """Items of the last ctree_update skipped on the device (pos >= arity^height or op not 0/1; all of them when the
+        batch would exceed max_leaves; sync() first after async_)."""
+        return int(getattr(self, "_ctrej", ctypes.c_size_t(0)).value)
+
+    def ctree_open_batch(self, tree, pos, out=None, async_=False):
+        """Openings of the present positions `pos`: (n, height, arity, 4), absent slots zero; they verify with
+        merkle_verify_batch (depth = height).  Host: an absent position raises; device: it gets an all-zero opening."""
+        t, flags, keep = self._ctree(tree)
+        ip, n, ik = self._idx(pos, keep[0], "pos")
+        shape = (n, int(tree.height), int(tree.arity), 4)
+        res = self._out_like(keep[0], shape) if out is None else self._check_out(out, shape, keep[0])
+        self._check(self._lib.p252_ctree_open_batch(self._ctx, ctypes.byref(t), ip, n, self._ptr(res),
+                                                    flags | (_native.ASYNC if async_ and flags else 0)))
+        return res
+
     def set_small_batch_max(self, max_items):
         """Digest batches up to `max_items` items use the lane-split (5 threads per state) kernel; 0 disables it."""
         self._check(self._lib.p252_set_small_batch_max(self._ctx, int(max_items)))
@@ -705,6 +774,16 @@ def mtree_layout(arity, height, capacity):
     offs = (ctypes.c_uint64 * (min(max(int(height), 0), 64) + 1))()
     raise_for_status(lib.p252_mtree_layout(int(arity), int(height), int(capacity), ctypes.byref(ls), ctypes.byref(ns), offs), lib)
     return int(ls.value), int(ns.value), [int(v) for v in offs]
+
+
+def ctree_layout(arity, height, max_leaves):
+    """p252_ctree_layout (host arithmetic, no GPU): -> (total_slots, level_offset) with level_offset[l] the first slot of
+    level l, l = 0..height; level l has min(max_leaves, arity^(height - l)) slots."""
+    lib = _native.lib()
+    total = ctypes.c_uint64(0)
+    offs = (ctypes.c_uint64 * (min(max(int(height), 0), 64) + 1))()
+    raise_for_status(lib.p252_ctree_layout(int(arity), int(height), int(max_leaves), ctypes.byref(total), offs), lib)
+    return int(total.value), [int(v) for v in offs]
 
 
 def varlen_out_offsets(offsets, delta):

@@ -1,8 +1,9 @@
 """Merkle trees of Domain::Merkle4 / Merkle2 digests (node = Hash::digest(Domain::Merkle{A}, A children),
 src/hash.rs:22-31).  Tree logic itself left the reference crate in 0.29.0
 (CHANGELOG.md:164-168); only the node hash is defined there.  Dense builders (n_leaves = arity^k), `Tree`, a
-fixed-height tree with batched appends and overwrites (p252_mtree), and `SparseTree`, a fixed-height tree with batched
-inserts and removals at any position (p252_smtree)."""
+fixed-height tree with batched appends and overwrites (p252_mtree), `SparseTree`, a fixed-height tree with batched
+inserts and removals at any position (p252_smtree), and `CompactTree`, the same at any height with storage
+proportional to the present leaves (p252_ctree)."""
 from .engine import _is_torch, default_engine
 
 
@@ -236,3 +237,98 @@ class SparseTree:
         return self.engine.smtree_open_batch(self, pos, async_=async_)
 
     opening = Tree.opening     # poseidon-merkle `Opening` of a present position (host arrays)
+
+
+class CompactTree:
+    """Compact sparse tree of the poseidon-merkle `Tree<T, H, A>` shape at any height (p252_ctree): positions are any
+    integers below arity^height (every u64 at arity 2 / height 64 or arity 4 / height 32), and storage is proportional
+    to the present leaves, at most `max_leaves` of them.  Presence and the empty-subtree rule are those of `SparseTree`.
+    Level l is the sorted list of its present nodes: `keys` (node indices) and `values` (scalars) from slot
+    level_offset[l], `count[l]` entries, every later slot zero.  Buffers are numpy arrays (device=None) or CUDA tensors
+    on cuda:`device` (int64 tensors hold the indices' bits).  All-zero buffers are the empty tree."""
+
+    def __init__(self, arity, height, max_leaves, engine=None, device=None):
+        import numpy as np
+        self.engine = engine or default_engine(0 if device is None else int(device))
+        self.arity, self.height, self.max_leaves = int(arity), int(height), int(max_leaves)
+        total, self.level_offset = self.engine.ctree_layout(self.arity, self.height, self.max_leaves)
+        if device is None:
+            self.keys = np.zeros((total,), dtype=np.uint64)
+            self.values = np.zeros((total, 4), dtype=np.uint64)
+            self.count = np.zeros((self.height + 1,), dtype=np.uint64)
+        else:
+            import torch
+            dev = torch.device("cuda", int(device))
+            self.keys = torch.zeros((total,), dtype=torch.int64, device=dev)
+            self.values = torch.zeros((total, 4), dtype=torch.int64, device=dev)
+            self.count = torch.zeros((self.height + 1,), dtype=torch.int64, device=dev)
+
+    def apply(self, pos, op, values, async_=False):
+        """One batch: op[i] = 0 inserts / overwrites values[i] at pos[i], op[i] = 1 removes pos[i]; the result equals
+        applying the operations in batch order."""
+        self.engine.ctree_update(self, pos, values=values, op=op, async_=async_)
+
+    def insert(self, pos, values, async_=False):
+        """Position pos[i] holds values[i] (the last write to a position wins)."""
+        self.engine.ctree_update(self, pos, values=values, async_=async_)
+
+    def remove(self, pos, async_=False):
+        """Make the positions `pos` absent (removing an absent position does nothing)."""
+        if _is_torch(self.values):
+            import torch
+            op = torch.ones((len(pos),), dtype=torch.uint8, device=self.values.device)
+        else:
+            import numpy as np
+            op = np.ones((len(pos),), dtype=np.uint8)
+        self.engine.ctree_update(self, pos, op=op, async_=async_)
+        if async_ and _is_torch(op):
+            self.engine._pending_counters.append(op)          # read by the device after the call returns
+
+    @property
+    def root(self):
+        return self.values[self.level_offset[self.height]]
+
+    def len(self):
+        """Number of present positions (count[0])."""
+        return int(self.count[0])
+
+    def __len__(self):
+        return self.len()
+
+    def level(self, l):
+        """(keys, values) views of the present nodes of level l."""
+        c, o = int(self.count[l]), self.level_offset[l]
+        return self.keys[o:o + c], self.values[o:o + c]
+
+    def contains(self, pos):
+        """Whether position `pos` holds a value: a binary search over level 0's keys."""
+        pos = int(pos)
+        if pos < 0 or pos >= self.arity ** self.height:
+            return False
+        keys, _ = self.level(0)
+        if _is_torch(keys):
+            import torch
+            # int64 tensors hold u64 bits: flipping the sign bit turns u64 order into int64 order
+            lo = -(1 << 63)
+            k = torch.tensor([pos + lo], dtype=torch.int64, device=keys.device)
+            j = int(torch.searchsorted(keys ^ lo, k))
+            return j < keys.shape[0] and int(keys[j]) ^ lo == int(k)
+        import numpy as np
+        j = int(np.searchsorted(keys, np.uint64(pos)))
+        return j < keys.shape[0] and int(keys[j]) == pos
+
+    def open(self, pos, async_=False):
+        """Openings of the present positions `pos`: (n, height, arity, 4), absent slots zero."""
+        return self.engine.ctree_open_batch(self, pos, async_=async_)
+
+    def opening(self, i):
+        """poseidon-merkle `Opening` of present position i (host arrays)."""
+        import numpy as np
+        if _is_torch(self.values):
+            import torch
+            j = int(i) - (1 << 64) if int(i) >= 1 << 63 else int(i)
+            branch = self.open(torch.tensor([j], dtype=torch.int64, device=self.values.device))[0]
+            branch, root = branch.cpu().numpy().view(np.uint64), self.root.cpu().numpy().view(np.uint64)
+        else:
+            branch, root = self.open(np.array([int(i)], dtype=np.uint64))[0], self.root
+        return Opening(root, branch, int(i), arity=self.arity)
