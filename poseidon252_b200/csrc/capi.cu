@@ -184,6 +184,56 @@ struct Io {
 
 int join_slots(p252_ctx* ctx, int rc, bool wipe);
 
+// Every kernel launch of the library goes through here: a failed launch is reported, a successful one counted.
+int launched(p252_ctx* ctx, cudaError_t le) {
+    if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
+    ctx->launches++;
+    return P252_OK;
+}
+
+// Tail of every DEVICE-buffer call: the status of its work, then synchronous unless P252_ASYNC.
+int device_done(p252_ctx* ctx, int rc, int flags) {
+    if (rc != P252_OK) return rc;
+    if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+    return P252_OK;
+}
+
+// number of zero bytes of ok[0, n): failures counted on the host
+size_t count_zero(const uint8_t* ok, size_t n) {
+    size_t bad = 0;
+    for (size_t i = 0; i < n; ++i) bad += ok[i] ? 0 : 1;
+    return bad;
+}
+
+// The layout of a set of device temporaries: 256-byte aligned pieces, taken in order.  Over a null base it only adds up
+// the size, so that one layout function both sizes and carves a buffer.
+struct Carve {
+    uint8_t* base = nullptr;
+    size_t used = 0;
+    template <typename T>
+    T* take(size_t count) {
+        T* r = base ? reinterpret_cast<T*>(base + used) : nullptr;
+        used += (count * sizeof(T) + 255) / 256 * 256;
+        return r;
+    }
+};
+
+// Temporaries of one call: layout(Carve&) places them in one stream-ordered allocation on `st`, body() runs, and the
+// allocation is freed in stream order whatever body() returned; the free's error is reported only when body() succeeded.
+template <typename Layout, typename Body>
+int with_scratch(p252_ctx* ctx, cudaStream_t st, Layout layout, Body body) {
+    Carve c;
+    layout(c);
+    CU(cudaMallocAsync(reinterpret_cast<void**>(&c.base), c.used, st));
+    c.used = 0;
+    layout(c);
+    const int rc = body();
+    const cudaError_t fe = cudaFreeAsync(c.base, st);
+    if (rc != P252_OK) return rc;
+    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
+    return P252_OK;
+}
+
 // Grow a slot's arena to at least `need` bytes.  The old arena is released only after the slot stream has drained, and
 // is cleared first when it may hold secrets (wipe).
 int slot_reserve(p252_ctx* ctx, Slot& sl, size_t need, bool wipe) {
@@ -200,11 +250,29 @@ int slot_reserve(p252_ctx* ctx, Slot& sl, size_t need, bool wipe) {
     return P252_OK;
 }
 
+// A HOST call on the slot streams: they first wait for everything already enqueued on the context stream, then
+// body(fail_at) stages its chunks (fail_at: the chunk p252_debug_fail_chunk makes fail, taken one shot).
 // wipe = true: the staging arenas held secrets (shared secret, nonce, plaintext); they are cleared before
 // returning (the reference's dependencies zeroize sponge state, Cargo.toml:15,17 "zeroize").
-// Whatever happens inside the chunk loop, the common exit below runs: slot streams are joined back into the
-// context stream, the arenas are wiped if asked, and the call returns only after everything enqueued has
-// finished -- so on an error no copy into the caller's buffers is still in flight and no secret is left staged.
+// Whatever body returns, the common exit join_slots runs: slot streams are joined back into the context stream, the
+// arenas are wiped if asked, and the call returns only after everything enqueued has finished -- so on an error no copy
+// into the caller's buffers is still in flight and no secret is left staged.
+template <typename Body>
+int on_slots(p252_ctx* ctx, bool wipe, Body body) {
+    const long long fail_at = ctx->fail_chunk;
+    ctx->fail_chunk = -1;
+    auto run = [&]() -> int {
+        CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
+        for (int s = 0; s < kSlots; ++s) CU(cudaStreamWaitEvent(ctx->slots[s].stream, ctx->ev_fork, 0));
+        return body(fail_at);
+    };
+    return join_slots(ctx, run(), wipe);
+}
+
+int injected_fault(p252_ctx* ctx) { return fail_cuda(ctx, cudaErrorLaunchFailure, "kernel launch (injected fault)"); }
+
+// Fixed-size HOST batches: the items stream through the slot arenas in chunks, each buffer of `ios` staged in its own
+// region, one launch per chunk.
 template <typename Launch>
 int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
     if (n == 0) return P252_OK;
@@ -213,13 +281,14 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
     size_t chunk = std::max<size_t>(1024, std::min(chunk_items_max(), kChunkBytesTarget / std::max<size_t>(per_item, 1)));
     chunk = (chunk + 127) / 128 * 128;
     if (chunk > n) chunk = n;
-    const long long fail_at = ctx->fail_chunk;
-    ctx->fail_chunk = -1;                                  // one shot
-
-    auto body = [&]() -> int {
-        // fork: slots wait for everything already enqueued on the context stream
-        CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        for (int s = 0; s < kSlots; ++s) CU(cudaStreamWaitEvent(ctx->slots[s].stream, ctx->ev_fork, 0));
+    std::vector<void*> d(ios.size());
+    auto carve = [&](void* arena) {
+        Carve c{static_cast<uint8_t*>(arena)};
+        for (size_t b = 0; b < ios.size(); ++b) d[b] = c.take<uint8_t>(chunk * ios[b].item_bytes);
+        return c.used;
+    };
+    const size_t need = carve(nullptr);
+    return on_slots(ctx, wipe, [&](long long fail_at) -> int {
         // Ramp-up (batches of several chunks only): the first chunks are small (chunk/8, /4, /2) so that the first
         // kernel starts after a ~1 MiB copy instead of a full chunk's; from the fourth chunk on every chunk has the
         // full size.  A batch that fits one chunk is one launch.
@@ -227,31 +296,22 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
         for (size_t off = 0, cnt = 0; off < n; off += cnt, ++k, cur = std::min(chunk, cur * 2)) {
             cnt = std::min(cur, n - off);
             Slot& sl = ctx->slots[k % kSlots];
-            // arena layout: one 256-byte aligned region per buffer
-            size_t need = 0;
-            for (auto& io : ios) need += (chunk * io.item_bytes + 255) / 256 * 256;
             int rc = slot_reserve(ctx, sl, need, wipe);
             if (rc != P252_OK) return rc;
-            std::vector<void*> d(ios.size());
-            size_t pos = 0;
-            for (size_t b = 0; b < ios.size(); ++b) {
-                d[b] = static_cast<uint8_t*>(sl.arena) + pos;
-                pos += (chunk * ios[b].item_bytes + 255) / 256 * 256;
+            carve(sl.arena);
+            for (size_t b = 0; b < ios.size(); ++b)
                 if (ios[b].h_in)
                     CU(cudaMemcpyAsync(d[b], static_cast<const uint8_t*>(ios[b].h_in) + off * ios[b].item_bytes,
                                        cnt * ios[b].item_bytes, cudaMemcpyHostToDevice, sl.stream));
-            }
-            cudaError_t le = ((long long)k == fail_at) ? cudaErrorLaunchFailure : launch(d.data(), cnt, sl.stream);
-            if (le != cudaSuccess) return fail_cuda(ctx, le, (long long)k == fail_at ? "kernel launch (injected fault)" : "kernel launch");
-            ctx->launches++;
+            if ((long long)k == fail_at) return injected_fault(ctx);
+            if ((rc = launched(ctx, launch(d.data(), cnt, sl.stream))) != P252_OK) return rc;
             for (size_t b = 0; b < ios.size(); ++b)
                 if (ios[b].h_out)
                     CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + off * ios[b].item_bytes, d[b],
                                        cnt * ios[b].item_bytes, cudaMemcpyDeviceToHost, sl.stream));
         }
         return P252_OK;
-    };
-    return join_slots(ctx, body(), wipe);
+    });
 }
 
 // Common exit of every HOST call that ran on the slot streams (success and failure): wipe, join, drain.
@@ -276,13 +336,6 @@ int join_slots(p252_ctx* ctx, int rc, bool wipe) {
         return rc;
     }
     if (ce != cudaSuccess) return fail_cuda(ctx, ce, "host pipeline join");
-    return P252_OK;
-}
-
-int finish_device_call(p252_ctx* ctx, cudaError_t le, int flags) {
-    if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-    ctx->launches++;
-    if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
     return P252_OK;
 }
 
@@ -324,6 +377,28 @@ uint64_t domain_sep(int domain, bool* ok) {
 }
 
 const uint64_t* limbs(const p252_fr* f) { return f->l; }
+
+// HOST openings in the format of k_merkle_open (kernels.h): for leaf idx[i] and level l < depth the sibling group of level
+// l, slots at or beyond lv.m[l] read as zero.  The indices are validated by the caller.
+void open_host(const p252_fr* leaves, const p252_fr* nodes, const uint64_t* idx, size_t n, int arity, int depth,
+               const p252::OpenLevels& lv, p252_fr* paths) {
+    const uint64_t A = (uint64_t)arity;
+    for (size_t i = 0; i < n; ++i) {
+        uint64_t j = idx[i];
+        for (int l = 0; l < depth; ++l) {
+            const uint64_t group = j / A;
+            const p252_fr* src = (l == 0 ? leaves : nodes + lv.off[l]) + group * A;
+            p252_fr* dst = paths + (i * (size_t)depth + (size_t)l) * A;
+            for (uint64_t q = 0; q < A; ++q) {
+                if (group * A + q < lv.m[l])
+                    dst[q] = src[q];
+                else
+                    memset(&dst[q], 0, sizeof(p252_fr));
+            }
+            j = group;
+        }
+    }
+}
 
 }  // namespace
 
@@ -601,7 +676,7 @@ static int permute_impl(p252_ctx* ctx, p252_fr* states, size_t n, int flags, boo
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(states)) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        return finish_device_call(ctx, p252::launch_permute(states, n, dense, ctx->coop_max, ctx->stream), flags);
+        return device_done(ctx, launched(ctx, p252::launch_permute(states, n, dense, ctx->coop_max, ctx->stream)), flags);
     }
     std::vector<Io> ios = {{states, states, 160}};
     return run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
@@ -627,7 +702,8 @@ static int digest_impl(p252_ctx* ctx, const p252_fr* tag, const p252_fr* in, siz
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(in) || !aligned16(out)) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        return finish_device_call(ctx, p252::launch_digest(limbs(tag), in, n, il, out, ol, truncate, ctx->coop_max, ctx->stream), flags);
+        return device_done(
+            ctx, launched(ctx, p252::launch_digest(limbs(tag), in, n, il, out, ol, truncate, ctx->coop_max, ctx->stream)), flags);
     }
     std::vector<Io> ios = {{in, nullptr, in_len * 32}, {nullptr, out, out_len * 32}};
     return run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
@@ -663,7 +739,7 @@ static int convert_impl(p252_ctx* ctx, const void* in, size_t n, void* out, uint
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(in) || !aligned16(out)) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        return finish_device_call(ctx, p252::launch_convert(in, n, out, ok, from_bytes, ctx->stream), flags);
+        return device_done(ctx, launched(ctx, p252::launch_convert(in, n, out, ok, from_bytes, ctx->stream)), flags);
     }
     std::vector<Io> ios = {{in, nullptr, 32}, {nullptr, out, 32}};
     if (from_bytes && ok) ios.push_back({nullptr, ok, 1});
@@ -693,8 +769,8 @@ int p252_encrypt_batch(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, co
         if (!aligned16(msg) || !aligned16(secret_uv) || !aligned16(nonce) || !aligned16(cipher))
             return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        return finish_device_call(
-            ctx, p252::launch_encrypt(limbs(&tag), msg, n, l32, secret_uv, nonce, cipher, ctx->stream), flags);
+        return device_done(
+            ctx, launched(ctx, p252::launch_encrypt(limbs(&tag), msg, n, l32, secret_uv, nonce, cipher, ctx->stream)), flags);
     }
     std::vector<Io> ios = {{msg, nullptr, L * 32}, {secret_uv, nullptr, 64}, {nonce, nullptr, 32},
                            {nullptr, cipher, (L + 1) * 32}};
@@ -718,24 +794,17 @@ int p252_decrypt_batch(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L,
         if (n_failed) *n_failed = 0;
         if (n == 0) return P252_OK;
         if (n_failed && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        cudaError_t le = p252::launch_decrypt(limbs(&tag), cipher, n, l32, secret_uv, nonce, msg, ok,
-                                              n_failed ? ctx->d_counter : nullptr, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        if ((rc = counter_end(ctx, n_failed)) != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        rc = launched(ctx, p252::launch_decrypt(limbs(&tag), cipher, n, l32, secret_uv, nonce, msg, ok,
+                                                n_failed ? ctx->d_counter : nullptr, ctx->stream));
+        if (rc == P252_OK) rc = counter_end(ctx, n_failed);
+        return device_done(ctx, rc, flags);
     }
     std::vector<Io> ios = {{cipher, nullptr, (L + 1) * 32}, {secret_uv, nullptr, 64}, {nonce, nullptr, 32},
                            {nullptr, msg, L * 32}, {nullptr, ok, 1}};
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         return p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], static_cast<uint8_t*>(d[4]), nullptr, st);
     }, /*wipe=*/true);
-    if (rc == P252_OK && n_failed) {
-        size_t bad = 0;
-        for (size_t i = 0; i < n; ++i) bad += ok[i] ? 0 : 1;
-        *n_failed = bad;
-    }
+    if (rc == P252_OK && n_failed) *n_failed = count_zero(ok, n);
     return rc;
 }
 
@@ -777,9 +846,8 @@ static int merkle_build_device(p252_ctx* ctx, int arity, const p252_fr* leaves, 
     const p252_fr* src = leaves;
     p252_fr* dst = nodes;
     for (size_t m = n_leaves / arity; m >= 1; m /= arity) {
-        cudaError_t le = p252::launch_digest(limbs(&tag), src, m, (uint32_t)arity, dst, 1, false, ctx->coop_max, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
+        rc = launched(ctx, p252::launch_digest(limbs(&tag), src, m, (uint32_t)arity, dst, 1, false, ctx->coop_max, ctx->stream));
+        if (rc != P252_OK) return rc;
         src = dst;
         dst += m;
         if (m == 1) break;
@@ -796,10 +864,7 @@ int p252_merkle_build(p252_ctx* ctx, int arity, const p252_fr* leaves, size_t n_
     DeviceGuard g(ctx->device);
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(leaves) || !aligned16(nodes_out)) return P252_ERR_INVALID_ARGUMENT;
-        rc = merkle_build_device(ctx, arity, leaves, n_leaves, nodes_out);
-        if (rc != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        return device_done(ctx, merkle_build_device(ctx, arity, leaves, n_leaves, nodes_out), flags);
     }
     // HOST: the first (largest) level streams through the chunked pipeline straight from the host
     // leaves; the remaining levels run on the device-resident level.
@@ -851,43 +916,26 @@ int p252_merkle_open_batch(p252_ctx* ctx, int arity, const p252_fr* leaves, size
     int depth = 0;
     int rc = tree_depth(arity, n_leaves, &depth);
     if (rc != P252_OK) return rc;
+    p252::OpenLevels lv{};                              // the dense layout: full levels, packed bottom-up
+    lv.m[0] = n_leaves;
+    for (int l = 1; l < depth; ++l) {
+        lv.m[l] = lv.m[l - 1] / (uint64_t)arity;
+        lv.off[l] = (l == 1) ? 0 : lv.off[l - 1] + lv.m[l - 1];
+    }
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(leaves) || !aligned16(nodes) || !aligned16(paths_out) || (reinterpret_cast<uintptr_t>(leaf_idx) & 7))
             return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        p252::OpenLevels lv{};                          // the dense layout: full levels, packed bottom-up
-        lv.m[0] = n_leaves;
-        for (int l = 1; l < depth; ++l) {
-            lv.m[l] = lv.m[l - 1] / (uint64_t)arity;
-            lv.off[l] = (l == 1) ? 0 : lv.off[l - 1] + lv.m[l - 1];
-        }
-        return finish_device_call(ctx, p252::launch_merkle_open(leaves, nodes, leaf_idx, n, arity, (uint32_t)depth,
-                                                                lv, paths_out, ctx->stream), flags);
+        return device_done(ctx, launched(ctx, p252::launch_merkle_open(leaves, nodes, leaf_idx, n, arity, (uint32_t)depth, lv,
+                                                                       paths_out, ctx->stream)), flags);
     }
     // HOST tree: an opening is a pure gather of 32-byte items the caller already holds in host memory -- shipping
     // the whole tree to the GPU to copy depth*arity scalars back would only add PCIe traffic.  No hashing happens here.
-    std::vector<size_t> off((size_t)depth, 0);       // offset of internal level l-1 inside nodes, for l >= 1
-    {
-        size_t m = n_leaves / (size_t)arity, acc = 0;
-        for (int l = 1; l < depth; ++l, m /= (size_t)arity) {
-            off[(size_t)l] = acc;
-            acc += m;
-        }
-    }
     for (size_t i = 0; i < n; ++i)
         if (leaf_idx[i] >= n_leaves) return P252_ERR_INVALID_ARGUMENT;
-    const size_t A = (size_t)arity;
-    for (size_t i = 0; i < n; ++i) {
-        uint64_t idx = leaf_idx[i];
-        for (int l = 0; l < depth; ++l) {
-            const uint64_t group = idx / A;
-            const p252_fr* src = (l == 0) ? leaves + group * A : nodes + off[(size_t)l] + group * A;
-            memcpy(paths_out + (i * (size_t)depth + (size_t)l) * A, src, A * sizeof(p252_fr));
-            idx = group;
-        }
-    }
+    open_host(leaves, nodes, leaf_idx, n, arity, depth, lv, paths_out);
     return P252_OK;
 }
 
@@ -907,13 +955,10 @@ int p252_merkle_verify_batch(p252_ctx* ctx, int arity, int depth, const p252_fr*
             return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
         if (n_failed && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        cudaError_t le = p252::launch_merkle_verify(limbs(&tag), limbs(root), leaf_items, leaf_idx, paths, n, arity,
-                                                    (uint32_t)depth, ok, n_failed ? ctx->d_counter : nullptr, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        if ((rc = counter_end(ctx, n_failed)) != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        rc = launched(ctx, p252::launch_merkle_verify(limbs(&tag), limbs(root), leaf_items, leaf_idx, paths, n, arity,
+                                                      (uint32_t)depth, ok, n_failed ? ctx->d_counter : nullptr, ctx->stream));
+        if (rc == P252_OK) rc = counter_end(ctx, n_failed);
+        return device_done(ctx, rc, flags);
     }
     const size_t path_bytes = (size_t)depth * (size_t)arity * 32;
     std::vector<Io> ios = {{leaf_items, nullptr, 32}, {leaf_idx, nullptr, 8}, {paths, nullptr, path_bytes}, {nullptr, ok, 1}};
@@ -921,11 +966,7 @@ int p252_merkle_verify_batch(p252_ctx* ctx, int arity, int depth, const p252_fr*
         return p252::launch_merkle_verify(limbs(&tag), limbs(root), d[0], static_cast<const uint64_t*>(d[1]), d[2], cnt, arity,
                                           (uint32_t)depth, static_cast<uint8_t*>(d[3]), nullptr, st);
     });
-    if (rc == P252_OK && n_failed) {
-        size_t bad = 0;
-        for (size_t i = 0; i < n; ++i) bad += ok[i] ? 0 : 1;
-        *n_failed = bad;
-    }
+    if (rc == P252_OK && n_failed) *n_failed = count_zero(ok, n);
     return rc;
 }
 
@@ -984,90 +1025,108 @@ int mtree_build_device(p252_ctx* ctx, const MLayout& L, int arity, int height, u
     const p252_fr* below = leaves;
     for (int l = 1; l <= height; ++l) {
         p252_fr* level = nodes + L.off[l];
-        if (m[l]) {
-            cudaError_t le = p252::launch_digest(limbs(&tag), below, m[l], (uint32_t)arity, level, 1, false, ctx->coop_max, ctx->stream);
-            if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-            ctx->launches++;
-        }
+        int rc;
+        if (m[l] && (rc = launched(ctx, p252::launch_digest(limbs(&tag), below, m[l], (uint32_t)arity, level, 1, false,
+                                                             ctx->coop_max, ctx->stream))) != P252_OK)
+            return rc;
         CU(cudaMemsetAsync(level + m[l], 0, (L.slots[l] - m[l]) * sizeof(p252_fr), ctx->stream));
         below = level;
     }
     return P252_OK;
 }
 
-// DEVICE update: sort (key, batch position), write the last value per key, then climb: D_l = distinct(D_{l-1} / A)
-// by candidate flags + DeviceSelect::Flagged (count stays on the device), and rehash exactly the groups in D_l.
-// Temporaries are one stream-ordered allocation.
-int mtree_update_device(p252_ctx* ctx, p252_mtree* t, const MLayout& L, const uint64_t* idx, const p252_fr* values,
-                        uint32_t n_upd, const p252_fr* append, uint32_t n_append, size_t* n_rejected) {
-    const int A = t->arity, H = t->height;
-    const uint32_t T = n_upd + n_append;
-    const uint64_t n_old = t->n_leaves, n_new = n_old + n_append;
-    uint64_t m[p252::kMaxDepth + 1];
-    mtree_prefix(A, H, n_new, m);
-    uint64_t bound[p252::kMaxDepth + 1];                  // host-side upper bound of |D_l|
-    bound[0] = T;
-    for (int l = 1; l <= H; ++l) bound[l] = std::min<uint64_t>(bound[l - 1], m[l]);
-    int end_bit = 1;
-    while (end_bit < 64 && (n_new >> end_bit)) ++end_bit; // keys <= n_new (the sentinel)
+// The climb of every fixed-height tree (DEVICE pointers): level l's dirty set D_l = DeviceSelect::Flagged over the
+// candidates (parent, flag) of the level below -- bound[l-1] of them, count cnt[l] on the device -- then the digest of
+// exactly those groups, then the candidates of the next level.  present (p252_smtree, null for p252_mtree): presence bytes
+// laid out like the scalars (leaves, then nodes), kept by the presence-aware digest.
+int tree_climb(p252_ctx* ctx, int A, int H, const MLayout& L, const p252_fr* leaves, p252_fr* nodes, uint8_t* present,
+               uint8_t* flag, uint64_t* parent, uint64_t* d, int* cnt, const uint64_t* bound, void* cub_tmp, size_t cub_bytes) {
+    p252_fr tag;
+    p252_hash_tag(merkle_domain(A), (size_t)A, 1, &tag);
+    const p252_fr* below = leaves;
+    const uint8_t* below_p = present;
+    for (int l = 1; l <= H; ++l) {
+        size_t b = cub_bytes;
+        CU(cub::DeviceSelect::Flagged(cub_tmp, b, parent, flag, d, cnt + l, (int)bound[l - 1], ctx->stream));
+        p252_fr* level = nodes + L.off[l];
+        uint8_t* level_p = present ? present + L.slots[0] + L.off[l] : nullptr;
+        int rc = launched(ctx, p252::launch_mtree_digest(limbs(&tag), below, A, level, d, cnt + l, bound[l], ctx->coop_max,
+                                                         ctx->stream, below_p, level_p));
+        if (rc == P252_OK && l < H)
+            rc = launched(ctx, p252::launch_mtree_parents(d, cnt + l, (uint32_t)bound[l], A, flag, parent, ctx->stream));
+        if (rc != P252_OK) return rc;
+        below = level;
+        below_p = level_p;
+    }
+    return P252_OK;
+}
 
+// DEVICE update of a fixed-height tree: keys_launch(keys, bpos, rejected) writes each item's key (its position, or a
+// sentinel below 2^end_bit that sorts last) -> stable radix sort of (key, batch position) -> write_launch(skeys, sbpos,
+// flag, parent) applies the last item per position and emits the level-1 candidates -> climb, bound[l] >= |D_l|.
+// Temporaries are one stream-ordered allocation; the dirty-set counts stay on the device.
+template <typename Keys, typename Write>
+int tree_update_device(p252_ctx* ctx, int A, int H, const MLayout& L, const p252_fr* leaves, p252_fr* nodes, uint8_t* present,
+                       uint32_t n, int end_bit, const uint64_t* bound, size_t* n_rejected, Keys keys_launch, Write write_launch) {
     size_t sort_bytes = 0, select_bytes = 0;
     CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                       (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)T, 0, end_bit, ctx->stream));
+                                       (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, 0, end_bit, ctx->stream));
     CU(cub::DeviceSelect::Flagged(nullptr, select_bytes, (const uint64_t*)nullptr, (const uint8_t*)nullptr, (uint64_t*)nullptr,
-                                  (int*)nullptr, (int)T, ctx->stream));
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    const size_t cub_bytes = up(std::max(sort_bytes, select_bytes));
-    const size_t total = 3 * up((size_t)T * 8) + 2 * up((size_t)T * 4) + up(T) + up((H + 1) * sizeof(int)) + cub_bytes;
-    uint8_t* base = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), total, ctx->stream));
-    uint8_t* p = base;
-    auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
-    uint64_t* keys = reinterpret_cast<uint64_t*>(take((size_t)T * 8));      // unsorted keys, then the dirty set D_l
-    uint64_t* skeys = reinterpret_cast<uint64_t*>(take((size_t)T * 8));
-    uint64_t* parent = reinterpret_cast<uint64_t*>(take((size_t)T * 8));
-    uint32_t* pos = reinterpret_cast<uint32_t*>(take((size_t)T * 4));
-    uint32_t* spos = reinterpret_cast<uint32_t*>(take((size_t)T * 4));
-    uint8_t* flag = take(T);
-    int* cnt = reinterpret_cast<int*>(take((H + 1) * sizeof(int)));
-    void* cub_tmp = take(cub_bytes);
-    uint64_t* d = keys;
-
-    auto body = [&]() -> int {
+                                  (int*)nullptr, (int)n, ctx->stream));
+    const size_t cub_bytes = std::max(sort_bytes, select_bytes);
+    uint64_t *keys = nullptr, *skeys = nullptr, *parent = nullptr;
+    uint32_t *bpos = nullptr, *sbpos = nullptr;
+    uint8_t* flag = nullptr;
+    int* cnt = nullptr;
+    void* cub_tmp = nullptr;
+    auto layout = [&](Carve& c) {
+        keys = c.take<uint64_t>(n);                        // unsorted keys, then the dirty set D_l
+        skeys = c.take<uint64_t>(n);
+        parent = c.take<uint64_t>(n);
+        bpos = c.take<uint32_t>(n);
+        sbpos = c.take<uint32_t>(n);
+        flag = c.take<uint8_t>(n);
+        cnt = c.take<int>(H + 1);
+        cub_tmp = c.take<uint8_t>(cub_bytes);
+    };
+    return with_scratch(ctx, ctx->stream, layout, [&]() -> int {
         int rc;
         if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        cudaError_t le = p252::launch_mtree_keys(idx, n_upd, n_old, T, keys, pos, n_rejected ? ctx->d_counter : nullptr, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
+        if ((rc = launched(ctx, keys_launch(keys, bpos, n_rejected ? ctx->d_counter : nullptr))) != P252_OK) return rc;
         size_t b = cub_bytes;
-        CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, skeys, pos, spos, (int)T, 0, end_bit, ctx->stream));
-        le = p252::launch_mtree_leaf_write(skeys, spos, T, n_new, A, values, n_upd, append, t->leaves, flag, parent, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        p252_fr tag;
-        p252_hash_tag(merkle_domain(A), (size_t)A, 1, &tag);
-        const p252_fr* below = t->leaves;
-        for (int l = 1; l <= H; ++l) {
-            b = cub_bytes;
-            CU(cub::DeviceSelect::Flagged(cub_tmp, b, parent, flag, d, cnt + l, (int)bound[l - 1], ctx->stream));
-            p252_fr* level = t->nodes + L.off[l];
-            le = p252::launch_mtree_digest(limbs(&tag), below, A, level, d, cnt + l, bound[l], ctx->coop_max, ctx->stream);
-            if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-            ctx->launches++;
-            if (l < H) {
-                le = p252::launch_mtree_parents(d, cnt + l, (uint32_t)bound[l], A, flag, parent, ctx->stream);
-                if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-                ctx->launches++;
-            }
-            below = level;
-        }
-        return counter_end(ctx, n_rejected);
-    };
-    int rc = body();
-    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
-    if (rc != P252_OK) return rc;
-    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
-    return P252_OK;
+        CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, skeys, bpos, sbpos, (int)n, 0, end_bit, ctx->stream));
+        if ((rc = launched(ctx, write_launch(skeys, sbpos, flag, parent))) != P252_OK) return rc;
+        rc = tree_climb(ctx, A, H, L, leaves, nodes, present, flag, parent, keys, cnt, bound, cub_tmp, cub_bytes);
+        return rc != P252_OK ? rc : counter_end(ctx, n_rejected);
+    });
+}
+
+// smallest end_bit with key >> end_bit == 0 (at least 1): the radix sort's bit range for keys <= key
+int sort_bits(uint64_t key) {
+    int end_bit = 1;
+    while (end_bit < 64 && (key >> end_bit)) ++end_bit;
+    return end_bit;
+}
+
+// HOST updates: the batch positions of the last item per distinct index, in ascending index order (a later item on the
+// same index wins) ...
+std::vector<uint32_t> last_per_index(const uint64_t* idx, size_t n) {
+    std::vector<uint32_t> ord(n);
+    for (size_t i = 0; i < n; ++i) ord[i] = (uint32_t)i;
+    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return idx[a] < idx[b]; });
+    size_t k = 0;
+    for (size_t i = 0; i < n; ++i)
+        if (i + 1 == n || idx[ord[i + 1]] != idx[ord[i]]) ord[k++] = ord[i];
+    ord.resize(k);
+    return ord;
+}
+
+// ... and one level up: the sorted dirty set d becomes its distinct parents d / A
+void parents_host(std::vector<uint64_t>& d, uint64_t A) {
+    size_t k = 0;
+    for (size_t i = 0; i < d.size(); ++i)
+        if (k == 0 || d[k - 1] != d[i] / A) d[k++] = d[i] / A;
+    d.resize(k);
 }
 
 // HOST update: sort and dedupe here, then per level gather the dirty groups into staging, hash them through the
@@ -1075,15 +1134,11 @@ int mtree_update_device(p252_ctx* ctx, p252_mtree* t, const MLayout& L, const ui
 int mtree_update_host(p252_ctx* ctx, p252_mtree* t, const MLayout& L, const uint64_t* idx, const p252_fr* values,
                       size_t n_upd, const p252_fr* append, size_t n_append) {
     const uint64_t A = (uint64_t)t->arity, n_old = t->n_leaves;
-    std::vector<uint32_t> ord(n_upd);
-    for (size_t i = 0; i < n_upd; ++i) ord[i] = (uint32_t)i;
-    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return idx[a] < idx[b]; });
     std::vector<uint64_t> d;
     d.reserve(n_upd + n_append);
-    for (size_t i = 0; i < n_upd; ++i) {
-        if (i + 1 < n_upd && idx[ord[i + 1]] == idx[ord[i]]) continue;   // a later write to the same leaf wins
-        t->leaves[idx[ord[i]]] = values[ord[i]];
-        d.push_back(idx[ord[i]]);
+    for (uint32_t i : last_per_index(idx, n_upd)) {
+        t->leaves[idx[i]] = values[i];
+        d.push_back(idx[i]);
     }
     for (size_t j = 0; j < n_append; ++j) {
         t->leaves[n_old + j] = append[j];
@@ -1092,12 +1147,8 @@ int mtree_update_host(p252_ctx* ctx, p252_mtree* t, const MLayout& L, const uint
     const p252_fr* below = t->leaves;
     std::vector<p252_fr> groups, out;
     for (int l = 1; l <= t->height; ++l) {
-        size_t k = 0;
-        for (size_t i = 0; i < d.size(); ++i) {
-            const uint64_t par = d[i] / A;
-            if (k == 0 || d[k - 1] != par) d[k++] = par;
-        }
-        d.resize(k);
+        parents_host(d, A);
+        const size_t k = d.size();
         groups.resize(k * A);
         out.resize(k);
         for (size_t i = 0; i < k; ++i) memcpy(&groups[i * A], below + d[i] * A, A * sizeof(p252_fr));
@@ -1134,29 +1185,22 @@ int p252_mtree_build(p252_ctx* ctx, p252_mtree* tree, int flags) {
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const uint64_t n = tree->n_leaves;
-    if (flags & P252_MEM_DEVICE) {
-        rc = mtree_build_device(ctx, L, tree->arity, tree->height, n, tree->leaves, tree->nodes);
-        if (rc != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
-    }
+    if (flags & P252_MEM_DEVICE)
+        return device_done(ctx, mtree_build_device(ctx, L, tree->arity, tree->height, n, tree->leaves, tree->nodes), flags);
     // HOST: stage the leaf prefix, build on the device, copy the node slots back
     p252_fr *d_leaves = nullptr, *d_nodes = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&d_leaves), L.slots[0] * sizeof(p252_fr), ctx->stream));
-    cudaError_t e = cudaMallocAsync(reinterpret_cast<void**>(&d_nodes), L.node_slots * sizeof(p252_fr), ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_leaves, tree->leaves, n * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) {
-        rc = fail_cuda(ctx, e, "mtree staging");
-    } else {
-        rc = mtree_build_device(ctx, L, tree->arity, tree->height, n, d_leaves, d_nodes);
-        if (rc == P252_OK) {
-            e = cudaMemcpyAsync(tree->nodes, d_nodes, L.node_slots * sizeof(p252_fr), cudaMemcpyDeviceToHost, ctx->stream);
-            if (e != cudaSuccess) rc = fail_cuda(ctx, e, "mtree D2H");
-        }
-    }
-    if (d_nodes) cudaFreeAsync(d_nodes, ctx->stream);
-    cudaFreeAsync(d_leaves, ctx->stream);
-    e = cudaStreamSynchronize(ctx->stream);
+    auto layout = [&](Carve& c) {
+        d_leaves = c.take<p252_fr>(L.slots[0]);
+        d_nodes = c.take<p252_fr>(L.node_slots);
+    };
+    rc = with_scratch(ctx, ctx->stream, layout, [&]() -> int {
+        CU(cudaMemcpyAsync(d_leaves, tree->leaves, n * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream));
+        const int r = mtree_build_device(ctx, L, tree->arity, tree->height, n, d_leaves, d_nodes);
+        if (r != P252_OK) return r;
+        CU(cudaMemcpyAsync(tree->nodes, d_nodes, L.node_slots * sizeof(p252_fr), cudaMemcpyDeviceToHost, ctx->stream));
+        return P252_OK;
+    });
+    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (rc != P252_OK) return rc;
     if (e != cudaSuccess) return fail_cuda(ctx, e, "mtree build");
     memset(tree->leaves + n, 0, (L.slots[0] - n) * sizeof(p252_fr));
@@ -1178,9 +1222,24 @@ int p252_mtree_update(p252_ctx* ctx, p252_mtree* tree, const uint64_t* idx, cons
         if ((n_upd && (!aligned16(values) || (reinterpret_cast<uintptr_t>(idx) & 7))) || (n_append && !aligned16(append)))
             return P252_ERR_INVALID_ARGUMENT;
         if (n_upd + n_append == 0) return P252_OK;
-        rc = mtree_update_device(ctx, tree, L, idx, values, (uint32_t)n_upd, append, (uint32_t)n_append, n_rejected);
-        if (rc != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
+        // keys: the leaf index, the sentinel n_new for a rejected overwrite; |D_l| <= min(batch, occupied nodes of level l)
+        const int A = tree->arity, H = tree->height;
+        const uint32_t T = (uint32_t)(n_upd + n_append);
+        const uint64_t n_old = tree->n_leaves, n_new = n_old + n_append;
+        uint64_t m[p252::kMaxDepth + 1], bound[p252::kMaxDepth + 1];
+        mtree_prefix(A, H, n_new, m);
+        bound[0] = T;
+        for (int l = 1; l <= H; ++l) bound[l] = std::min<uint64_t>(bound[l - 1], m[l]);
+        rc = tree_update_device(
+            ctx, A, H, L, tree->leaves, tree->nodes, nullptr, T, sort_bits(n_new), bound, n_rejected,
+            [&](uint64_t* keys, uint32_t* pos, unsigned long long* rej) {
+                return p252::launch_mtree_keys(idx, (uint32_t)n_upd, n_old, T, keys, pos, rej, ctx->stream);
+            },
+            [&](const uint64_t* skeys, const uint32_t* spos, uint8_t* flag, uint64_t* parent) {
+                return p252::launch_mtree_leaf_write(skeys, spos, T, n_new, A, values, (uint32_t)n_upd, append, tree->leaves, flag,
+                                                     parent, ctx->stream);
+            });
+        if ((rc = device_done(ctx, rc, flags)) != P252_OK) return rc;
     } else {
         for (size_t i = 0; i < n_upd; ++i)
             if (idx[i] >= tree->n_leaves) return P252_ERR_INVALID_ARGUMENT;
@@ -1201,37 +1260,22 @@ int p252_mtree_open_batch(p252_ctx* ctx, const p252_mtree* tree, const uint64_t*
     const int A = tree->arity, H = tree->height;
     uint64_t m[p252::kMaxDepth + 1];
     mtree_prefix(A, H, tree->n_leaves, m);
+    p252::OpenLevels lv{};
+    for (int l = 0; l < H; ++l) {
+        lv.off[l] = L.off[l];
+        lv.m[l] = m[l];
+    }
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(paths_out) || (reinterpret_cast<uintptr_t>(leaf_idx) & 7)) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        p252::OpenLevels lv{};
-        for (int l = 0; l < H; ++l) {
-            lv.off[l] = L.off[l];
-            lv.m[l] = m[l];
-        }
-        return finish_device_call(ctx, p252::launch_merkle_open(tree->leaves, tree->nodes, leaf_idx, n, A, (uint32_t)H, lv,
-                                                                paths_out, ctx->stream), flags);
+        return device_done(ctx, launched(ctx, p252::launch_merkle_open(tree->leaves, tree->nodes, leaf_idx, n, A, (uint32_t)H, lv,
+                                                                       paths_out, ctx->stream)), flags);
     }
     for (size_t i = 0; i < n; ++i)
         if (leaf_idx[i] >= tree->n_leaves) return P252_ERR_INVALID_ARGUMENT;
-    const size_t Az = (size_t)A;
-    for (size_t i = 0; i < n; ++i) {
-        uint64_t j = leaf_idx[i];
-        for (int l = 0; l < H; ++l) {
-            const uint64_t group = j / Az;
-            const p252_fr* src = (l == 0 ? tree->leaves : tree->nodes + L.off[l]) + group * Az;
-            p252_fr* dst = paths_out + (i * (size_t)H + (size_t)l) * Az;
-            for (size_t q = 0; q < Az; ++q) {
-                if (group * Az + q < m[l])
-                    dst[q] = src[q];
-                else
-                    memset(&dst[q], 0, sizeof(p252_fr));
-            }
-            j = group;
-        }
-    }
+    open_host(tree->leaves, tree->nodes, leaf_idx, n, A, H, lv, paths_out);
     return P252_OK;
 }
 
@@ -1248,37 +1292,6 @@ int smtree_check(const p252_smtree* t, int flags, MLayout* L) {
     if (rc != P252_OK) return rc;
     if ((flags & P252_MEM_DEVICE) && (!aligned16(t->leaves) || !aligned16(t->nodes) || (reinterpret_cast<uintptr_t>(t->present) & 3)))
         return P252_ERR_INVALID_ARGUMENT;
-    return P252_OK;
-}
-
-// The climb shared by build and update (DEVICE pointers): level l's dirty set D_l = DeviceSelect::Flagged over the
-// candidates (parent, flag) of the level below -- bound[l-1] of them, count on the device -- then the presence-aware
-// digest of exactly those groups, then the candidates of the next level.
-int smtree_climb(p252_ctx* ctx, const p252_smtree* t, const MLayout& L, uint8_t* flag, uint64_t* parent, uint64_t* d, int* cnt,
-                 const uint64_t* bound, void* cub_tmp, size_t cub_bytes) {
-    const int A = t->arity, H = t->height;
-    p252_fr tag;
-    p252_hash_tag(merkle_domain(A), (size_t)A, 1, &tag);
-    const p252_fr* below = t->leaves;
-    const uint8_t* below_p = t->present;
-    uint8_t* node_p = t->present + L.slots[0];
-    for (int l = 1; l <= H; ++l) {
-        size_t b = cub_bytes;
-        CU(cub::DeviceSelect::Flagged(cub_tmp, b, parent, flag, d, cnt + l, (int)bound[l - 1], ctx->stream));
-        p252_fr* level = t->nodes + L.off[l];
-        uint8_t* level_p = node_p + L.off[l];
-        cudaError_t le = p252::launch_smtree_digest(limbs(&tag), below, below_p, A, level, level_p, d, cnt + l, bound[l],
-                                                    ctx->coop_max, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        if (l < H) {
-            le = p252::launch_mtree_parents(d, cnt + l, (uint32_t)bound[l], A, flag, parent, ctx->stream);
-            if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-            ctx->launches++;
-        }
-        below = level;
-        below_p = level_p;
-    }
     return P252_OK;
 }
 
@@ -1302,81 +1315,22 @@ int smtree_build_device(p252_ctx* ctx, const p252_smtree* t, const MLayout& L) {
     size_t select_bytes = 0;
     CU(cub::DeviceSelect::Flagged(nullptr, select_bytes, (const uint64_t*)nullptr, (const uint8_t*)nullptr, (uint64_t*)nullptr,
                                   (int*)nullptr, (int)G, ctx->stream));
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    uint8_t* base = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), 2 * up(G * 8) + up(G) + up((H + 1) * sizeof(int)) + up(select_bytes),
-                       ctx->stream));
-    uint64_t* parent = reinterpret_cast<uint64_t*>(base);
-    uint64_t* d = reinterpret_cast<uint64_t*>(base + up(G * 8));
-    uint8_t* flag = base + 2 * up(G * 8);
-    int* cnt = reinterpret_cast<int*>(flag + up(G));
-    void* cub_tmp = reinterpret_cast<uint8_t*>(cnt) + up((H + 1) * sizeof(int));
-    auto body = [&]() -> int {
-        cudaError_t le = p252::launch_smtree_seed(t->present, t->leaves, G, t->capacity, A, flag, parent, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        return smtree_climb(ctx, t, L, flag, parent, d, cnt, bound, cub_tmp, up(select_bytes));
+    uint64_t *parent = nullptr, *d = nullptr;
+    uint8_t* flag = nullptr;
+    int* cnt = nullptr;
+    void* cub_tmp = nullptr;
+    auto layout = [&](Carve& c) {
+        parent = c.take<uint64_t>(G);
+        d = c.take<uint64_t>(G);
+        flag = c.take<uint8_t>(G);
+        cnt = c.take<int>(H + 1);
+        cub_tmp = c.take<uint8_t>(select_bytes);
     };
-    int rc = body();
-    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
-    if (rc != P252_OK) return rc;
-    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
-    return P252_OK;
-}
-
-// DEVICE update: keys (position, or the sentinel capacity) -> stable radix sort of (key, batch position) -> the last op
-// per position is applied -> climb.  Temporaries are one stream-ordered allocation; the dirty-set counts stay on the
-// device.
-int smtree_update_device(p252_ctx* ctx, p252_smtree* t, const MLayout& L, const uint64_t* pos, const uint8_t* op,
-                         const p252_fr* values, uint32_t n, size_t* n_rejected) {
-    const int A = t->arity, H = t->height;
-    uint64_t bound[p252::kMaxDepth + 1];
-    smtree_bounds(L, A, H, n, bound);
-    int end_bit = 1;
-    while (end_bit < 64 && (t->capacity >> end_bit)) ++end_bit;   // keys <= capacity (the sentinel)
-
-    size_t sort_bytes = 0, select_bytes = 0;
-    CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint64_t*)nullptr, (uint64_t*)nullptr,
-                                       (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, 0, end_bit, ctx->stream));
-    CU(cub::DeviceSelect::Flagged(nullptr, select_bytes, (const uint64_t*)nullptr, (const uint8_t*)nullptr, (uint64_t*)nullptr,
-                                  (int*)nullptr, (int)n, ctx->stream));
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    const size_t cub_bytes = up(std::max(sort_bytes, select_bytes));
-    const size_t total = 3 * up((size_t)n * 8) + 2 * up((size_t)n * 4) + up(n) + up((H + 1) * sizeof(int)) + cub_bytes;
-    uint8_t* base = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), total, ctx->stream));
-    uint8_t* p = base;
-    auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
-    uint64_t* keys = reinterpret_cast<uint64_t*>(take((size_t)n * 8));      // unsorted keys, then the dirty set D_l
-    uint64_t* skeys = reinterpret_cast<uint64_t*>(take((size_t)n * 8));
-    uint64_t* parent = reinterpret_cast<uint64_t*>(take((size_t)n * 8));
-    uint32_t* bpos = reinterpret_cast<uint32_t*>(take((size_t)n * 4));
-    uint32_t* sbpos = reinterpret_cast<uint32_t*>(take((size_t)n * 4));
-    uint8_t* flag = take(n);
-    int* cnt = reinterpret_cast<int*>(take((H + 1) * sizeof(int)));
-    void* cub_tmp = take(cub_bytes);
-
-    auto body = [&]() -> int {
-        int rc;
-        if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        cudaError_t le = p252::launch_smtree_keys(pos, op, n, t->capacity, keys, bpos, n_rejected ? ctx->d_counter : nullptr,
-                                                  ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        size_t b = cub_bytes;
-        CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, skeys, bpos, sbpos, (int)n, 0, end_bit, ctx->stream));
-        le = p252::launch_smtree_leaf_write(skeys, sbpos, n, t->capacity, A, op, values, t->leaves, t->present, flag, parent,
-                                            ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        if ((rc = smtree_climb(ctx, t, L, flag, parent, keys, cnt, bound, cub_tmp, cub_bytes)) != P252_OK) return rc;
-        return counter_end(ctx, n_rejected);
-    };
-    int rc = body();
-    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
-    if (rc != P252_OK) return rc;
-    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
-    return P252_OK;
+    return with_scratch(ctx, ctx->stream, layout, [&]() -> int {
+        const int rc = launched(ctx, p252::launch_smtree_seed(t->present, t->leaves, G, t->capacity, A, flag, parent, ctx->stream));
+        if (rc != P252_OK) return rc;
+        return tree_climb(ctx, A, H, L, t->leaves, t->nodes, t->present, flag, parent, d, cnt, bound, cub_tmp, select_bytes);
+    });
 }
 
 // HOST update (already validated): sort and dedupe here, apply the last op per position, then per level: a dirty node
@@ -1385,17 +1339,13 @@ int smtree_update_device(p252_ctx* ctx, p252_smtree* t, const MLayout& L, const 
 int smtree_update_host(p252_ctx* ctx, p252_smtree* t, const MLayout& L, const uint64_t* pos, const uint8_t* op,
                        const p252_fr* values, size_t n) {
     const uint64_t A = (uint64_t)t->arity;
-    std::vector<uint32_t> ord(n);
-    for (size_t i = 0; i < n; ++i) ord[i] = (uint32_t)i;
-    std::stable_sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return pos[a] < pos[b]; });
     std::vector<uint64_t> d;
     d.reserve(n);
-    for (size_t i = 0; i < n; ++i) {
-        if (i + 1 < n && pos[ord[i + 1]] == pos[ord[i]]) continue;   // a later operation on the same position wins
-        const uint64_t j = pos[ord[i]];
-        const bool insert = !op || op[ord[i]] == 0;
+    for (uint32_t i : last_per_index(pos, n)) {
+        const uint64_t j = pos[i];
+        const bool insert = !op || op[i] == 0;
         if (insert)
-            t->leaves[j] = values[ord[i]];
+            t->leaves[j] = values[i];
         else
             memset(&t->leaves[j], 0, sizeof(p252_fr));
         t->present[j] = insert ? 1 : 0;
@@ -1407,25 +1357,20 @@ int smtree_update_host(p252_ctx* ctx, p252_smtree* t, const MLayout& L, const ui
     std::vector<p252_fr> groups, out;
     std::vector<uint64_t> live;
     for (int l = 1; l <= t->height; ++l) {
-        size_t k = 0;
-        for (size_t i = 0; i < d.size(); ++i) {
-            const uint64_t par = d[i] / A;
-            if (k == 0 || d[k - 1] != par) d[k++] = par;
-        }
-        d.resize(k);
+        parents_host(d, A);
         p252_fr* level = t->nodes + L.off[l];
         uint8_t* level_p = node_p + L.off[l];
         live.clear();
         groups.clear();
-        for (size_t i = 0; i < k; ++i) {
+        for (uint64_t g : d) {
             bool any = false;
-            for (uint64_t q = 0; q < A; ++q) any = any || below_p[d[i] * A + q];
+            for (uint64_t q = 0; q < A; ++q) any = any || below_p[g * A + q];
             if (any) {
-                live.push_back(d[i]);
-                groups.insert(groups.end(), below + d[i] * A, below + d[i] * A + A);
+                live.push_back(g);
+                groups.insert(groups.end(), below + g * A, below + g * A + A);
             } else {
-                memset(&level[d[i]], 0, sizeof(p252_fr));
-                level_p[d[i]] = 0;
+                memset(&level[g], 0, sizeof(p252_fr));
+                level_p[g] = 0;
             }
         }
         out.resize(live.size());
@@ -1454,35 +1399,27 @@ int p252_smtree_build(p252_ctx* ctx, p252_smtree* tree, int flags) {
     if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (flags & P252_MEM_DEVICE) {
-        if ((rc = smtree_build_device(ctx, tree, L)) != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
-    }
+    if (flags & P252_MEM_DEVICE) return device_done(ctx, smtree_build_device(ctx, tree, L), flags);
     // HOST: stage the leaves and their presence bytes, build on the device, copy leaves, nodes and presence back
     const size_t leaf_b = L.slots[0] * sizeof(p252_fr), node_b = L.node_slots * sizeof(p252_fr);
     const size_t pres_b = L.slots[0] + L.node_slots;
-    uint8_t* base = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), leaf_b + node_b + pres_b, ctx->stream));
     p252_smtree dt = *tree;
-    dt.leaves = reinterpret_cast<p252_fr*>(base);
-    dt.nodes = reinterpret_cast<p252_fr*>(base + leaf_b);
-    dt.present = base + leaf_b + node_b;
-    cudaError_t e = cudaMemcpyAsync(dt.leaves, tree->leaves, leaf_b, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dt.present, tree->present, L.slots[0], cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) {
-        rc = fail_cuda(ctx, e, "smtree staging");
-    } else {
-        rc = smtree_build_device(ctx, &dt, L);
-        if (rc == P252_OK) {
-            e = cudaMemcpyAsync(tree->leaves, dt.leaves, leaf_b, cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->nodes, dt.nodes, node_b, cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->present, dt.present, pres_b, cudaMemcpyDeviceToHost, ctx->stream);
-            if (e != cudaSuccess) rc = fail_cuda(ctx, e, "smtree D2H");
-        }
-    }
-    cudaFreeAsync(base, ctx->stream);
-    e = cudaStreamSynchronize(ctx->stream);
+    auto layout = [&](Carve& c) {
+        dt.leaves = c.take<p252_fr>(L.slots[0]);
+        dt.nodes = c.take<p252_fr>(L.node_slots);
+        dt.present = c.take<uint8_t>(pres_b);
+    };
+    rc = with_scratch(ctx, ctx->stream, layout, [&]() -> int {
+        CU(cudaMemcpyAsync(dt.leaves, tree->leaves, leaf_b, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dt.present, tree->present, L.slots[0], cudaMemcpyHostToDevice, ctx->stream));
+        const int r = smtree_build_device(ctx, &dt, L);
+        if (r != P252_OK) return r;
+        CU(cudaMemcpyAsync(tree->leaves, dt.leaves, leaf_b, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(tree->nodes, dt.nodes, node_b, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(tree->present, dt.present, pres_b, cudaMemcpyDeviceToHost, ctx->stream));
+        return P252_OK;
+    });
+    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (rc != P252_OK) return rc;
     if (e != cudaSuccess) return fail_cuda(ctx, e, "smtree build");
     return P252_OK;
@@ -1501,10 +1438,21 @@ int p252_smtree_update(p252_ctx* ctx, p252_smtree* tree, const uint64_t* pos, co
     if (flags & P252_MEM_DEVICE) {
         if (n && (!aligned16(values) || (reinterpret_cast<uintptr_t>(pos) & 7))) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        rc = smtree_update_device(ctx, tree, L, pos, op, values, (uint32_t)n, n_rejected);
-        if (rc != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        // keys: the position, the sentinel capacity for a rejected item
+        const int A = tree->arity, H = tree->height;
+        const uint32_t n32 = (uint32_t)n;
+        uint64_t bound[p252::kMaxDepth + 1];
+        smtree_bounds(L, A, H, n, bound);
+        rc = tree_update_device(
+            ctx, A, H, L, tree->leaves, tree->nodes, tree->present, n32, sort_bits(tree->capacity), bound, n_rejected,
+            [&](uint64_t* keys, uint32_t* bpos, unsigned long long* rej) {
+                return p252::launch_smtree_keys(pos, op, n32, tree->capacity, keys, bpos, rej, ctx->stream);
+            },
+            [&](const uint64_t* skeys, const uint32_t* sbpos, uint8_t* flag, uint64_t* parent) {
+                return p252::launch_smtree_leaf_write(skeys, sbpos, n32, tree->capacity, A, op, values, tree->leaves, tree->present,
+                                                      flag, parent, ctx->stream);
+            });
+        return device_done(ctx, rc, flags);
     }
     for (size_t i = 0; i < n; ++i)
         if (pos[i] >= tree->capacity || (op && op[i] > 1)) return P252_ERR_INVALID_ARGUMENT;
@@ -1522,12 +1470,9 @@ int p252_smtree_len(p252_ctx* ctx, const p252_smtree* tree, uint64_t* n_present,
     *n_present = 0;
     if (flags & P252_MEM_DEVICE) {
         if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        cudaError_t le = p252::launch_smtree_count(tree->present, tree->capacity, ctx->d_counter, ctx->stream);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        if ((rc = counter_end(ctx, reinterpret_cast<size_t*>(n_present))) != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        rc = launched(ctx, p252::launch_smtree_count(tree->present, tree->capacity, ctx->d_counter, ctx->stream));
+        if (rc == P252_OK) rc = counter_end(ctx, reinterpret_cast<size_t*>(n_present));
+        return device_done(ctx, rc, flags);
     }
     uint64_t c = 0;   // HOST: the bytes are already here
     for (uint64_t j = 0; j < tree->capacity; ++j) c += tree->present[j] != 0;
@@ -1542,32 +1487,24 @@ int p252_smtree_open_batch(p252_ctx* ctx, const p252_smtree* tree, const uint64_
     int rc = smtree_check(tree, flags, &L);
     if (rc != P252_OK) return rc;
     const int A = tree->arity, H = tree->height;
+    // every slot: absent slots are already zero in memory, and so are leaf slots at or past the capacity
+    p252::OpenLevels lv{};
+    for (int l = 0; l < H; ++l) {
+        lv.off[l] = L.off[l];
+        lv.m[l] = L.slots[l];
+    }
+    lv.m[0] = tree->capacity;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     if (flags & P252_MEM_DEVICE) {
         if (!aligned16(paths_out) || (reinterpret_cast<uintptr_t>(pos) & 7)) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        p252::OpenLevels lv{};                          // every slot: absent slots are already zero in memory
-        for (int l = 0; l < H; ++l) {
-            lv.off[l] = L.off[l];
-            lv.m[l] = L.slots[l];
-        }
-        lv.m[0] = tree->capacity;
-        return finish_device_call(ctx, p252::launch_merkle_open(tree->leaves, tree->nodes, pos, n, A, (uint32_t)H, lv, paths_out,
-                                                                ctx->stream, tree->present), flags);
+        return device_done(ctx, launched(ctx, p252::launch_merkle_open(tree->leaves, tree->nodes, pos, n, A, (uint32_t)H, lv,
+                                                                       paths_out, ctx->stream, tree->present)), flags);
     }
     for (size_t i = 0; i < n; ++i)
         if (pos[i] >= tree->capacity || !tree->present[pos[i]]) return P252_ERR_INVALID_ARGUMENT;
-    const size_t Az = (size_t)A;
-    for (size_t i = 0; i < n; ++i) {
-        uint64_t j = pos[i];
-        for (int l = 0; l < H; ++l) {
-            const uint64_t group = j / Az;
-            const p252_fr* src = (l == 0 ? tree->leaves : tree->nodes + L.off[l]) + group * Az;
-            memcpy(paths_out + (i * (size_t)H + (size_t)l) * Az, src, Az * sizeof(p252_fr));
-            j = group;
-        }
-    }
+    open_host(tree->leaves, tree->nodes, pos, n, A, H, lv, paths_out);
     return P252_OK;
 }
 
@@ -1635,66 +1572,60 @@ int ctree_update_device(p252_ctx* ctx, p252_ctree* t, const CLayout& L, const ui
                                   (int*)nullptr, (int)n, ctx->stream));
     CU(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)S, ctx->stream));
     CU(cub::DeviceScan::ExclusiveSum(nullptr, scan2_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)n, ctx->stream));
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    const size_t cub_bytes = up(std::max(std::max(sort_bytes, select_bytes), std::max(scan_bytes, scan2_bytes)));
-    const size_t N = n;
-    const size_t total = 6 * up(N * 8) + 3 * up(N * 4) + up(N) + up(N * 32) + up(N) + up(N * A * 32) + up(N * A) + up(N * 8) +
-                         up(S * 8) + up(S * 32) + 2 * up(S * 4) + 2 * up(N * 4) + up((H + 3) * sizeof(int)) + up(16) + up(8) +
-                         cub_bytes;
-    uint8_t* base = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), total, ctx->stream));
-    uint8_t* p = base;
-    auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
-    uint64_t* keys = reinterpret_cast<uint64_t*>(take(N * 8));
-    uint64_t* skeys = reinterpret_cast<uint64_t*>(take(N * 8));
-    uint64_t* vkeys = reinterpret_cast<uint64_t*>(take(N * 8));       // valid items, sorted
-    uint64_t* ck[2] = {reinterpret_cast<uint64_t*>(take(N * 8)), reinterpret_cast<uint64_t*>(take(N * 8))};
-    uint64_t* parent = reinterpret_cast<uint64_t*>(take(N * 8));
-    uint32_t* bpos = reinterpret_cast<uint32_t*>(take(N * 4));
-    uint32_t* sbpos = reinterpret_cast<uint32_t*>(take(N * 4));
-    uint32_t* vbpos = reinterpret_cast<uint32_t*>(take(N * 4));
-    uint8_t* flag = take(N);
-    p252_fr* cval = reinterpret_cast<p252_fr*>(take(N * 32));          // change values (level 0, then the digests)
-    uint8_t* cpres = take(N);
-    p252_fr* groups = reinterpret_cast<p252_fr*>(take(N * A * 32));
-    uint8_t* gpres = take(N * A);
-    uint64_t* iota = reinterpret_cast<uint64_t*>(take(N * 8));
-    uint64_t* okeys = reinterpret_cast<uint64_t*>(take(S * 8));       // the merged level
-    p252_fr* ovals = reinterpret_cast<p252_fr*>(take(S * 32));
-    uint32_t* kept = reinterpret_cast<uint32_t*>(take(S * 4));
-    uint32_t* K = reinterpret_cast<uint32_t*>(take(S * 4));
-    uint32_t* ins = reinterpret_cast<uint32_t*>(take(N * 4));
-    uint32_t* I = reinterpret_cast<uint32_t*>(take(N * 4));
-    int* cnt = reinterpret_cast<int*>(take((H + 3) * sizeof(int)));  // [0] valid items, [1 + l] level l's change list
-    uint64_t* stats = reinterpret_cast<uint64_t*>(take(16));
-    uint32_t* ok = reinterpret_cast<uint32_t*>(take(8));
-    void* cub_tmp = take(cub_bytes);
-
-    auto launched = [&](cudaError_t le) -> int {
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        return P252_OK;
+    const size_t cub_bytes = std::max(std::max(sort_bytes, select_bytes), std::max(scan_bytes, scan2_bytes));
+    uint64_t *keys, *skeys, *vkeys, *ck[2], *parent, *iota, *okeys, *stats;
+    uint32_t *bpos, *sbpos, *vbpos, *kept, *K, *ins, *I, *ok;
+    uint8_t *flag, *cpres, *gpres;
+    p252_fr *cval, *groups, *ovals;
+    int* cnt;
+    void* cub_tmp;
+    auto layout = [&](Carve& c) {
+        keys = c.take<uint64_t>(n);
+        skeys = c.take<uint64_t>(n);
+        vkeys = c.take<uint64_t>(n);                       // valid items, sorted
+        ck[0] = c.take<uint64_t>(n);
+        ck[1] = c.take<uint64_t>(n);
+        parent = c.take<uint64_t>(n);
+        bpos = c.take<uint32_t>(n);
+        sbpos = c.take<uint32_t>(n);
+        vbpos = c.take<uint32_t>(n);
+        flag = c.take<uint8_t>(n);
+        cval = c.take<p252_fr>(n);                         // change values (level 0, then the digests)
+        cpres = c.take<uint8_t>(n);
+        groups = c.take<p252_fr>((size_t)n * A);
+        gpres = c.take<uint8_t>((size_t)n * A);
+        iota = c.take<uint64_t>(n);
+        okeys = c.take<uint64_t>(S);                       // the merged level
+        ovals = c.take<p252_fr>(S);
+        kept = c.take<uint32_t>(S);
+        K = c.take<uint32_t>(S);
+        ins = c.take<uint32_t>(n);
+        I = c.take<uint32_t>(n);
+        cnt = c.take<int>(H + 3);                          // [0] valid items, [1 + l] level l's change list
+        stats = c.take<uint64_t>(2);
+        ok = c.take<uint32_t>(2);
+        cub_tmp = c.take<uint8_t>(cub_bytes);
     };
-    auto body = [&]() -> int {
+    return with_scratch(ctx, ctx->stream, layout, [&]() -> int {
         int rc;
         if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
         unsigned long long* rej = n_rejected ? ctx->d_counter : nullptr;
-        if ((rc = launched(p252::launch_ctree_keys(pos, op, n, L.max_pos, keys, bpos, rej, ctx->stream))) != P252_OK) return rc;
+        if ((rc = launched(ctx, p252::launch_ctree_keys(pos, op, n, L.max_pos, keys, bpos, rej, ctx->stream))) != P252_OK) return rc;
         size_t b = cub_bytes;
         CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, skeys, bpos, sbpos, (int)n, 0, end_bit, ctx->stream));
-        if ((rc = launched(p252::launch_ctree_valid(sbpos, n, flag, ctx->stream))) != P252_OK) return rc;
+        if ((rc = launched(ctx, p252::launch_ctree_valid(sbpos, n, flag, ctx->stream))) != P252_OK) return rc;
         b = cub_bytes;
         CU(cub::DeviceSelect::Flagged(cub_tmp, b, skeys, flag, vkeys, cnt, (int)n, ctx->stream));
         b = cub_bytes;
         CU(cub::DeviceSelect::Flagged(cub_tmp, b, sbpos, flag, vbpos, cnt, (int)n, ctx->stream));
-        if ((rc = launched(p252::launch_ctree_last(vkeys, cnt, n, flag, ctx->stream))) != P252_OK) return rc;
+        if ((rc = launched(ctx, p252::launch_ctree_last(vkeys, cnt, n, flag, ctx->stream))) != P252_OK) return rc;
         b = cub_bytes;
         CU(cub::DeviceSelect::Flagged(cub_tmp, b, vkeys, flag, ck[0], cnt + 1, (int)n, ctx->stream));
         b = cub_bytes;
         CU(cub::DeviceSelect::Flagged(cub_tmp, b, vbpos, flag, bpos, cnt + 1, (int)n, ctx->stream));
-        if ((rc = launched(p252::launch_ctree_leaf_changes(bpos, cnt + 1, n, op, values, cval, cpres, ctx->stream))) != P252_OK)
+        if ((rc = launched(ctx, p252::launch_ctree_leaf_changes(bpos, cnt + 1, n, op, values, cval, cpres, ctx->stream))) != P252_OK)
             return rc;
-        if ((rc = launched(p252::launch_ctree_iota(iota, n, ctx->stream))) != P252_OK) return rc;
+        if ((rc = launched(ctx, p252::launch_ctree_iota(iota, n, ctx->stream))) != P252_OK) return rc;
         p252_fr tag;
         p252_hash_tag(merkle_domain(A), (size_t)A, 1, &tag);
         for (int l = 0; l <= H; ++l) {
@@ -1704,39 +1635,34 @@ int ctree_update_device(p252_ctx* ctx, p252_ctree* t, const CLayout& L, const ui
             uint64_t* lc = t->count + l;
             const uint64_t* c = ck[l & 1];
             const int* cc = cnt + 1 + l;
-            if ((rc = launched(p252::launch_ctree_mark(lk, lc, s, c, cc, nb[l], cpres, kept, ins, ctx->stream))) != P252_OK)
+            if ((rc = launched(ctx, p252::launch_ctree_mark(lk, lc, s, c, cc, nb[l], cpres, kept, ins, ctx->stream))) != P252_OK)
                 return rc;
             b = cub_bytes;
             CU(cub::DeviceScan::ExclusiveSum(cub_tmp, b, kept, K, (int)s, ctx->stream));
             b = cub_bytes;
             CU(cub::DeviceScan::ExclusiveSum(cub_tmp, b, ins, I, (int)nb[l], ctx->stream));
-            if ((rc = launched(p252::launch_ctree_scatter(lk, lv, lc, s, c, cval, cc, nb[l], kept, K, ins, I, okeys, ovals,
-                                                          ctx->stream))) != P252_OK)
+            if ((rc = launched(ctx, p252::launch_ctree_scatter(lk, lv, lc, s, c, cval, cc, nb[l], kept, K, ins, I, okeys, ovals,
+                                                               ctx->stream))) != P252_OK)
                 return rc;
-            if ((rc = launched(p252::launch_ctree_count(lc, s, nb[l], kept, K, ins, I, l == 0, n, stats, ok, rej, ctx->stream))) !=
-                P252_OK)
+            if ((rc = launched(ctx, p252::launch_ctree_count(lc, s, nb[l], kept, K, ins, I, l == 0, n, stats, ok, rej,
+                                                             ctx->stream))) != P252_OK)
                 return rc;
-            if ((rc = launched(p252::launch_ctree_commit(okeys, ovals, s, stats, ok, lk, lv, lc, ctx->stream))) != P252_OK)
+            if ((rc = launched(ctx, p252::launch_ctree_commit(okeys, ovals, s, stats, ok, lk, lv, lc, ctx->stream))) != P252_OK)
                 return rc;
             if (l == H) break;
             // the next level's change list: distinct parents, their groups from the merged level, hashed
-            if ((rc = launched(p252::launch_ctree_parents(c, cc, nb[l], A, flag, parent, ctx->stream))) != P252_OK) return rc;
+            if ((rc = launched(ctx, p252::launch_mtree_parents(c, cc, nb[l], A, flag, parent, ctx->stream))) != P252_OK) return rc;
             b = cub_bytes;
             CU(cub::DeviceSelect::Flagged(cub_tmp, b, parent, flag, ck[(l + 1) & 1], cnt + 2 + l, (int)nb[l], ctx->stream));
-            if ((rc = launched(p252::launch_ctree_gather(okeys, ovals, stats, s, ck[(l + 1) & 1], cnt + 2 + l, nb[l + 1], A, groups,
-                                                         gpres, ctx->stream))) != P252_OK)
+            if ((rc = launched(ctx, p252::launch_ctree_gather(okeys, ovals, stats, s, ck[(l + 1) & 1], cnt + 2 + l, nb[l + 1], A,
+                                                              groups, gpres, ctx->stream))) != P252_OK)
                 return rc;
-            if ((rc = launched(p252::launch_smtree_digest(limbs(&tag), groups, gpres, A, cval, cpres, iota, cnt + 2 + l, nb[l + 1],
-                                                          ctx->coop_max, ctx->stream))) != P252_OK)
+            if ((rc = launched(ctx, p252::launch_mtree_digest(limbs(&tag), groups, A, cval, iota, cnt + 2 + l, nb[l + 1],
+                                                              ctx->coop_max, ctx->stream, gpres, cpres))) != P252_OK)
                 return rc;
         }
         return counter_end(ctx, n_rejected);
-    };
-    int rc = body();
-    cudaError_t fe = cudaFreeAsync(base, ctx->stream);
-    if (rc != P252_OK) return rc;
-    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
-    return P252_OK;
+    });
 }
 
 }  // namespace
@@ -1766,10 +1692,7 @@ int p252_ctree_update(p252_ctx* ctx, p252_ctree* tree, const uint64_t* pos, cons
     if (flags & P252_MEM_DEVICE) {
         if (n && (!aligned16(values) || (reinterpret_cast<uintptr_t>(pos) & 7))) return P252_ERR_INVALID_ARGUMENT;
         if (n == 0) return P252_OK;
-        rc = ctree_update_device(ctx, tree, L, pos, op, values, (uint32_t)n, n_rejected);
-        if (rc != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        return device_done(ctx, ctree_update_device(ctx, tree, L, pos, op, values, (uint32_t)n, n_rejected), flags);
     }
     for (size_t i = 0; i < n; ++i)
         if (pos[i] > L.max_pos || (op && op[i] > 1)) return P252_ERR_INVALID_ARGUMENT;
@@ -1778,38 +1701,36 @@ int p252_ctree_update(p252_ctx* ctx, p252_ctree* tree, const uint64_t* pos, cons
     // item is valid here, so a non-zero rejection count means a capacity overflow)
     const size_t H1 = (size_t)tree->height + 1;
     const size_t kb = L.total * 8, vb = L.total * sizeof(p252_fr), cb = H1 * 8;
-    const size_t up_kb = (kb + 255) / 256 * 256, up_cb = (cb + 255) / 256 * 256, up_vb = (vb + 255) / 256 * 256;
-    const size_t pb = (n * 8 + 255) / 256 * 256, ob = (n + 255) / 256 * 256;
-    uint8_t* base = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&base), up_vb + up_kb + up_cb + n * sizeof(p252_fr) + pb + ob, ctx->stream));
     p252_ctree dt = *tree;
-    dt.values = reinterpret_cast<p252_fr*>(base);
-    dt.keys = reinterpret_cast<uint64_t*>(base + up_vb);
-    dt.count = reinterpret_cast<uint64_t*>(base + up_vb + up_kb);
-    p252_fr* d_vals = reinterpret_cast<p252_fr*>(base + up_vb + up_kb + up_cb);
-    uint64_t* d_pos = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(d_vals) + n * sizeof(p252_fr));
-    uint8_t* d_op = op ? reinterpret_cast<uint8_t*>(d_pos) + pb : nullptr;
+    p252_fr* d_vals = nullptr;
+    uint64_t* d_pos = nullptr;
+    uint8_t* d_op = nullptr;
+    auto layout = [&](Carve& c) {
+        dt.values = c.take<p252_fr>(L.total);
+        dt.keys = c.take<uint64_t>(L.total);
+        dt.count = c.take<uint64_t>(H1);
+        d_vals = c.take<p252_fr>(n);
+        d_pos = c.take<uint64_t>(n);
+        d_op = op ? c.take<uint8_t>(n) : nullptr;
+    };
     size_t refused = 0;
-    cudaError_t e = cudaMemcpyAsync(dt.values, tree->values, vb, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dt.keys, tree->keys, kb, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dt.count, tree->count, cb, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_vals, values, n * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_pos, pos, n * 8, cudaMemcpyHostToDevice, ctx->stream);
-    if (e == cudaSuccess && op) e = cudaMemcpyAsync(d_op, op, n, cudaMemcpyHostToDevice, ctx->stream);
-    if (e != cudaSuccess) {
-        rc = fail_cuda(ctx, e, "ctree staging");
-    } else {
-        rc = ctree_update_device(ctx, &dt, L, d_pos, d_op, d_vals, (uint32_t)n, &refused);
-        if (rc == P252_OK) e = cudaStreamSynchronize(ctx->stream);   // publishes `refused`
-        if (rc == P252_OK && e == cudaSuccess && refused == 0) {
-            e = cudaMemcpyAsync(tree->values, dt.values, vb, cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->keys, dt.keys, kb, cudaMemcpyDeviceToHost, ctx->stream);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(tree->count, dt.count, cb, cudaMemcpyDeviceToHost, ctx->stream);
-        }
-        if (rc == P252_OK && e != cudaSuccess) rc = fail_cuda(ctx, e, "ctree D2H");
-    }
-    cudaFreeAsync(base, ctx->stream);
-    e = cudaStreamSynchronize(ctx->stream);
+    rc = with_scratch(ctx, ctx->stream, layout, [&]() -> int {
+        CU(cudaMemcpyAsync(dt.values, tree->values, vb, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dt.keys, tree->keys, kb, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(dt.count, tree->count, cb, cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(d_vals, values, n * sizeof(p252_fr), cudaMemcpyHostToDevice, ctx->stream));
+        CU(cudaMemcpyAsync(d_pos, pos, n * 8, cudaMemcpyHostToDevice, ctx->stream));
+        if (op) CU(cudaMemcpyAsync(d_op, op, n, cudaMemcpyHostToDevice, ctx->stream));
+        const int r = ctree_update_device(ctx, &dt, L, d_pos, d_op, d_vals, (uint32_t)n, &refused);
+        if (r != P252_OK) return r;
+        CU(cudaStreamSynchronize(ctx->stream));   // publishes `refused`
+        if (refused) return P252_OK;
+        CU(cudaMemcpyAsync(tree->values, dt.values, vb, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(tree->keys, dt.keys, kb, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaMemcpyAsync(tree->count, dt.count, cb, cudaMemcpyDeviceToHost, ctx->stream));
+        return P252_OK;
+    });
+    const cudaError_t e = cudaStreamSynchronize(ctx->stream);
     if (rc != P252_OK) return rc;
     if (e != cudaSuccess) return fail_cuda(ctx, e, "ctree update");
     return refused ? P252_ERR_INVALID_ARGUMENT : P252_OK;
@@ -1828,8 +1749,8 @@ int p252_ctree_open_batch(p252_ctx* ctx, const p252_ctree* tree, const uint64_t*
         if (n == 0) return P252_OK;
         p252::OpenLevels lv{};
         for (int l = 0; l < H; ++l) lv.off[l] = L.off[l];
-        return finish_device_call(ctx, p252::launch_ctree_open(tree->keys, tree->values, tree->count, pos, n, A, (uint32_t)H, lv,
-                                                               paths_out, ctx->stream), flags);
+        return device_done(ctx, launched(ctx, p252::launch_ctree_open(tree->keys, tree->values, tree->count, pos, n, A,
+                                                                      (uint32_t)H, lv, paths_out, ctx->stream)), flags);
     }
     // HOST: binary searches over the sorted levels
     auto find = [&](int l, uint64_t key) -> uint64_t {   // first entry of level l whose index is >= key
@@ -1929,35 +1850,26 @@ int crypt_tags(p252_ctx* ctx, size_t max_len, const p252_fr** table) {
 // stream-ordered allocation.
 template <typename Keys, typename Run>
 int varlen_sorted(p252_ctx* ctx, uint32_t n, uint32_t max_len, cudaStream_t st, Keys keys_launch, Run run_launch) {
-    int end_bit = 1;
-    while ((max_len >> end_bit) != 0) ++end_bit;            // keys <= max_len
+    const int end_bit = sort_bits(max_len);                // keys <= max_len
     size_t sort_bytes = 0;
     CU(cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const uint32_t*)nullptr,
                                        (uint32_t*)nullptr, (int)n, 0, end_bit, st));
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    const size_t arr = up((size_t)n * 4);
-    uint8_t* tmp = nullptr;
-    CU(cudaMallocAsync(reinterpret_cast<void**>(&tmp), 4 * arr + up(sort_bytes), st));
-    uint32_t* keys = reinterpret_cast<uint32_t*>(tmp);
-    uint32_t* vals = reinterpret_cast<uint32_t*>(tmp + arr);
-    uint32_t* lens = reinterpret_cast<uint32_t*>(tmp + 2 * arr);
-    uint32_t* perm = reinterpret_cast<uint32_t*>(tmp + 3 * arr);
-    auto body = [&]() -> int {
-        cudaError_t le = keys_launch(keys, vals);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        size_t b = sort_bytes;
-        CU(cub::DeviceRadixSort::SortPairs(tmp + 4 * arr, b, keys, lens, vals, perm, (int)n, 0, end_bit, st));
-        le = run_launch(lens, perm);
-        if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-        ctx->launches++;
-        return P252_OK;
+    uint32_t *keys = nullptr, *vals = nullptr, *lens = nullptr, *perm = nullptr;
+    void* cub_tmp = nullptr;
+    auto layout = [&](Carve& c) {
+        keys = c.take<uint32_t>(n);
+        vals = c.take<uint32_t>(n);
+        lens = c.take<uint32_t>(n);
+        perm = c.take<uint32_t>(n);
+        cub_tmp = c.take<uint8_t>(sort_bytes);
     };
-    int rc = body();
-    cudaError_t fe = cudaFreeAsync(tmp, st);
-    if (rc != P252_OK) return rc;
-    if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
-    return P252_OK;
+    return with_scratch(ctx, st, layout, [&]() -> int {
+        const int rc = launched(ctx, keys_launch(keys, vals));
+        if (rc != P252_OK) return rc;
+        size_t b = sort_bytes;
+        CU(cub::DeviceRadixSort::SortPairs(cub_tmp, b, keys, lens, vals, perm, (int)n, 0, end_bit, st));
+        return launched(ctx, run_launch(lens, perm));
+    });
 }
 
 // One digest batch on `st`: keys (length or 0 = rejected) -> radix sort by length -> the varlen digest kernel.
@@ -1990,75 +1902,74 @@ int crypt_run(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* i
         });
 }
 
-// HOST batch (already validated): consecutive item ranges of about kChunkBytesTarget input bytes (a longer item is a
-// chunk by itself, at most chunk_items_max() items) are staged on the slot streams -- input scalars, their offsets and
-// the output rows in one stream-ordered allocation -- hashed by varlen_run with base = the chunk's first offset, and
-// copied back.
-int varlen_host(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n, uint32_t max_len,
-                uint32_t fixed_len, p252_fr* out, uint32_t out_len) {
-    const long long fail_at = ctx->fail_chunk;
-    ctx->fail_chunk = -1;                                  // one shot
-    auto body = [&]() -> int {
-        CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        for (int s = 0; s < kSlots; ++s) CU(cudaStreamWaitEvent(ctx->slots[s].stream, ctx->ev_fork, 0));
-        auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-        size_t k = 0;
-        for (size_t lo = 0, hi = 0; lo < n; lo = hi, ++k) {
-            hi = lo + 1;
-            while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * sizeof(p252_fr) <= kChunkBytesTarget) ++hi;
-            const size_t cnt = hi - lo;
-            const uint64_t s0 = offsets[lo], ns = offsets[hi] - s0;
-            cudaStream_t st = ctx->slots[k % kSlots].stream;
-            const size_t in_b = up(ns * sizeof(p252_fr)), off_b = up((cnt + 1) * 8);
-            uint8_t* d = nullptr;
-            CU(cudaMallocAsync(reinterpret_cast<void**>(&d), in_b + off_b + cnt * out_len * sizeof(p252_fr), st));
-            p252_fr* d_in = reinterpret_cast<p252_fr*>(d);
-            uint64_t* d_off = reinterpret_cast<uint64_t*>(d + in_b);
-            p252_fr* d_out = reinterpret_cast<p252_fr*>(d + in_b + off_b);
-            int rc = P252_OK;
-            cudaError_t e = cudaMemcpyAsync(d_in, in + s0, ns * sizeof(p252_fr), cudaMemcpyHostToDevice, st);
-            if (e == cudaSuccess) e = cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, st);
-            if (e != cudaSuccess)
-                rc = fail_cuda(ctx, e, "varlen staging");
-            else if ((long long)k == fail_at)
-                rc = fail_cuda(ctx, cudaErrorLaunchFailure, "kernel launch (injected fault)");
-            else
-                rc = varlen_run(ctx, tags, d_in, s0, ns, d_off, (uint32_t)cnt, max_len, fixed_len, d_out, out_len, nullptr, st);
-            if (rc == P252_OK) {
-                e = cudaMemcpyAsync(out + lo * out_len, d_out, cnt * out_len * sizeof(p252_fr), cudaMemcpyDeviceToHost, st);
-                if (e != cudaSuccess) rc = fail_cuda(ctx, e, "varlen D2H");
-            }
-            cudaError_t fe = cudaFreeAsync(d, st);
-            if (rc != P252_OK) return rc;
-            if (fe != cudaSuccess) return fail_cuda(ctx, fe, "cudaFreeAsync");
-        }
-        return P252_OK;
-    };
-    return join_slots(ctx, body(), false);
-}
-
-// HOST encrypt / decrypt batch (already validated, n > 0): consecutive item ranges of about kChunkBytesTarget input bytes
-// (a longer item is a chunk by itself, at most chunk_items_max() items) are staged on the slot streams and run by
-// crypt_run with base = the chunk's first offset s0.  Input, offsets, secrets, nonces, output and ok go through the slot
-// arenas -- never through stream-ordered allocations -- so that join_slots(wipe) clears every secret on every exit path.
-// Output of chunk [lo, hi): (ns +- cnt) scalars at out + (s0 - a0 +- lo), the chunk's part of the output CSR.
-int crypt_host(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n,
-               uint32_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* out, uint8_t* ok) {
-    const long long fail_at = ctx->fail_chunk;
-    ctx->fail_chunk = -1;                                  // one shot
-    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
-    std::vector<size_t> bounds = {0};                      // chunk k = items [bounds[k], bounds[k+1])
-    size_t need = 0;                                       // arena bytes of the largest chunk
+// The chunks of a variable-length HOST batch: consecutive item ranges of about kChunkBytesTarget input bytes (a longer
+// item is a chunk by itself), at most chunk_items_max() items each; chunk k = items [bounds[k], bounds[k+1]).
+std::vector<size_t> chunk_bounds(const uint64_t* offsets, size_t n) {
+    std::vector<size_t> bounds = {0};
     for (size_t lo = 0, hi = 0; lo < n; lo = hi) {
         hi = lo + 1;
         while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * sizeof(p252_fr) <= kChunkBytesTarget) ++hi;
         bounds.push_back(hi);
-        const size_t cnt = hi - lo, ns = offsets[hi] - offsets[lo];
-        need = std::max(need, up(ns * 32) + up((cnt + 1) * 8) + up(cnt * 64) + up(cnt * 32) + up((ns + cnt) * 32) + up(cnt));
     }
-    auto body = [&]() -> int {
-        CU(cudaEventRecord(ctx->ev_fork, ctx->stream));
-        for (int s = 0; s < kSlots; ++s) CU(cudaStreamWaitEvent(ctx->slots[s].stream, ctx->ev_fork, 0));
+    return bounds;
+}
+
+// HOST batch (already validated): each chunk is staged on a slot stream -- input scalars, their offsets and the output
+// rows in one stream-ordered allocation -- hashed by varlen_run with base = the chunk's first offset, and copied back.
+int varlen_host(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n, uint32_t max_len,
+                uint32_t fixed_len, p252_fr* out, uint32_t out_len) {
+    const std::vector<size_t> bounds = chunk_bounds(offsets, n);
+    return on_slots(ctx, false, [&](long long fail_at) -> int {
+        for (size_t k = 0; k + 1 < bounds.size(); ++k) {
+            const size_t lo = bounds[k], hi = bounds[k + 1], cnt = hi - lo;
+            const uint64_t s0 = offsets[lo], ns = offsets[hi] - s0;
+            cudaStream_t st = ctx->slots[k % kSlots].stream;
+            p252_fr *d_in = nullptr, *d_out = nullptr;
+            uint64_t* d_off = nullptr;
+            auto layout = [&](Carve& c) {
+                d_in = c.take<p252_fr>(ns);
+                d_off = c.take<uint64_t>(cnt + 1);
+                d_out = c.take<p252_fr>(cnt * out_len);
+            };
+            const int rc = with_scratch(ctx, st, layout, [&]() -> int {
+                CU(cudaMemcpyAsync(d_in, in + s0, ns * sizeof(p252_fr), cudaMemcpyHostToDevice, st));
+                CU(cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
+                if ((long long)k == fail_at) return injected_fault(ctx);
+                const int r = varlen_run(ctx, tags, d_in, s0, ns, d_off, (uint32_t)cnt, max_len, fixed_len, d_out, out_len, nullptr, st);
+                if (r != P252_OK) return r;
+                CU(cudaMemcpyAsync(out + lo * out_len, d_out, cnt * out_len * sizeof(p252_fr), cudaMemcpyDeviceToHost, st));
+                return P252_OK;
+            });
+            if (rc != P252_OK) return rc;
+        }
+        return P252_OK;
+    });
+}
+
+// HOST encrypt / decrypt batch (already validated, n > 0): each chunk is staged on a slot stream and run by crypt_run with
+// base = the chunk's first offset s0.  Input, offsets, secrets, nonces, output and ok go through the slot arenas -- never
+// through stream-ordered allocations -- so that join_slots(wipe) clears every secret on every exit path.
+// Output of chunk [lo, hi): (ns +- cnt) scalars at out + (s0 - a0 +- lo), the chunk's part of the output CSR.
+int crypt_host(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n,
+               uint32_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* out, uint8_t* ok) {
+    const std::vector<size_t> bounds = chunk_bounds(offsets, n);
+    p252_fr *d_in = nullptr, *d_uv = nullptr, *d_nonce = nullptr, *d_out = nullptr;
+    uint64_t* d_off = nullptr;
+    uint8_t* d_ok = nullptr;
+    auto carve = [&](size_t k, void* arena) {              // chunk k's staging in `arena` (null: its size only)
+        const size_t cnt = bounds[k + 1] - bounds[k], ns = offsets[bounds[k + 1]] - offsets[bounds[k]];
+        Carve c{static_cast<uint8_t*>(arena)};
+        d_in = c.take<p252_fr>(ns);
+        d_off = c.take<uint64_t>(cnt + 1);
+        d_uv = c.take<p252_fr>(2 * cnt);
+        d_nonce = c.take<p252_fr>(cnt);
+        d_out = c.take<p252_fr>(ns + cnt);                 // room for either direction
+        d_ok = c.take<uint8_t>(cnt);
+        return c.used;
+    };
+    size_t need = 0;                                       // arena bytes of the largest chunk
+    for (size_t k = 0; k + 1 < bounds.size(); ++k) need = std::max(need, carve(k, nullptr));
+    return on_slots(ctx, /*wipe=*/true, [&](long long fail_at) -> int {
         const uint64_t a0 = offsets[0];
         for (size_t k = 0; k + 1 < bounds.size(); ++k) {
             const size_t lo = bounds[k], hi = bounds[k + 1], cnt = hi - lo;
@@ -2068,19 +1979,12 @@ int crypt_host(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* 
             Slot& sl = ctx->slots[k % kSlots];
             int rc = slot_reserve(ctx, sl, need, /*wipe=*/true);
             if (rc != P252_OK) return rc;
-            uint8_t* p = static_cast<uint8_t*>(sl.arena);
-            auto take = [&](size_t b) { uint8_t* r = p; p += up(b); return r; };
-            p252_fr* d_in = reinterpret_cast<p252_fr*>(take(ns * 32));
-            uint64_t* d_off = reinterpret_cast<uint64_t*>(take((cnt + 1) * 8));
-            p252_fr* d_uv = reinterpret_cast<p252_fr*>(take(cnt * 64));
-            p252_fr* d_nonce = reinterpret_cast<p252_fr*>(take(cnt * 32));
-            p252_fr* d_out = reinterpret_cast<p252_fr*>(take(out_ns * 32));
-            uint8_t* d_ok = take(cnt);
+            carve(k, sl.arena);
             CU(cudaMemcpyAsync(d_in, in + s0, ns * 32, cudaMemcpyHostToDevice, sl.stream));
             CU(cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, sl.stream));
             CU(cudaMemcpyAsync(d_uv, secret_uv + 2 * lo, cnt * 64, cudaMemcpyHostToDevice, sl.stream));
             CU(cudaMemcpyAsync(d_nonce, nonce + lo, cnt * 32, cudaMemcpyHostToDevice, sl.stream));
-            if ((long long)k == fail_at) return fail_cuda(ctx, cudaErrorLaunchFailure, "kernel launch (injected fault)");
+            if ((long long)k == fail_at) return injected_fault(ctx);
             rc = crypt_run(ctx, decrypt, tags, d_in, s0, ns, d_off, (uint32_t)cnt, max_len, d_uv, d_nonce, d_out,
                            decrypt ? d_ok : nullptr, nullptr, nullptr, sl.stream);
             if (rc != P252_OK) return rc;
@@ -2088,8 +1992,7 @@ int crypt_host(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* 
             if (decrypt) CU(cudaMemcpyAsync(ok + lo, d_ok, cnt, cudaMemcpyDeviceToHost, sl.stream));
         }
         return P252_OK;
-    };
-    return join_slots(ctx, body(), /*wipe=*/true);
+    });
 }
 
 }  // namespace
@@ -2118,10 +2021,8 @@ int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t 
         if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
         rc = varlen_run(ctx, tags, in, 0, n_scalars, offsets, (uint32_t)n, (uint32_t)max_len, fixed_len, out, (uint32_t)out_len,
                         n_rejected ? ctx->d_counter : nullptr, ctx->stream);
-        if (rc != P252_OK) return rc;
-        if ((rc = counter_end(ctx, n_rejected)) != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        if (rc == P252_OK) rc = counter_end(ctx, n_rejected);
+        return device_done(ctx, rc, flags);
     }
     // HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written
     for (size_t i = 0; i < n; ++i) {
@@ -2162,11 +2063,9 @@ int crypt_varlen(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n_scalar
         if ((n_failed || n_rejected) && (rc = counter_begin(ctx, p252_ctx::kCounters)) != P252_OK) return rc;
         rc = crypt_run(ctx, decrypt, tags, in, 0, n_scalars, offsets, (uint32_t)n, (uint32_t)max_len, secret_uv, nonce, out, ok,
                        n_failed ? ctx->d_counter : nullptr, n_rejected ? ctx->d_counter + 1 : nullptr, ctx->stream);
-        if (rc != P252_OK) return rc;
-        if ((rc = counter_end(ctx, n_failed, 0)) != P252_OK) return rc;
-        if ((rc = counter_end(ctx, n_rejected, 1)) != P252_OK) return rc;
-        if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-        return P252_OK;
+        if (rc == P252_OK) rc = counter_end(ctx, n_failed, 0);
+        if (rc == P252_OK) rc = counter_end(ctx, n_rejected, 1);
+        return device_done(ctx, rc, flags);
     }
     // HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written.
     // With every item valid the output ranges are disjoint and inside the output, so the decrypt range conditions of the
@@ -2181,11 +2080,7 @@ int crypt_varlen(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n_scalar
     if (n == 0) return P252_OK;
     if ((rc = crypt_tags(ctx, max_len, &tags)) != P252_OK) return rc;
     rc = crypt_host(ctx, decrypt, tags, in, offsets, n, (uint32_t)max_len, secret_uv, nonce, out, ok);
-    if (rc == P252_OK && n_failed) {
-        size_t bad = 0;
-        for (size_t i = 0; i < n; ++i) bad += ok[i] ? 0 : 1;
-        *n_failed = bad;
-    }
+    if (rc == P252_OK && n_failed) *n_failed = count_zero(ok, n);
     return rc;
 }
 
@@ -2330,9 +2225,9 @@ int p252_merkle4_build_dist(p252_ctx* ctx, const p252_fr* leaves_shard, size_t n
         if (p.sharded) {
             // the first level is always sharded (n_leaves_total / G is a multiple of 4)
             if (timing) CU(cudaEventRecord(ctx->level_events[(size_t)l].k0, ctx->stream));
-            cudaError_t le = p252::launch_digest(limbs(&tag), below_mine, p.my_count, 4, level + p.my_offset, 1, false, ctx->coop_max, ctx->stream);
-            if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-            ctx->launches++;
+            rc = launched(ctx, p252::launch_digest(limbs(&tag), below_mine, p.my_count, 4, level + p.my_offset, 1, false,
+                                                   ctx->coop_max, ctx->stream));
+            if (rc != P252_OK) return rc;
             if (timing) CU(cudaEventRecord(ctx->level_events[(size_t)l].k1, ctx->stream));
             if (G > 1 && !no_gather) {
                 CU(cudaEventRecord(ctx->ev_level, ctx->stream));
@@ -2354,9 +2249,9 @@ int p252_merkle4_build_dist(p252_ctx* ctx, const p252_fr* leaves_shard, size_t n
                 gather_in_flight = false;
             }
             if (timing) CU(cudaEventRecord(ctx->level_events[(size_t)l].k0, ctx->stream));
-            cudaError_t le = p252::launch_digest(limbs(&tag), below_full, p.level_size, 4, level, 1, false, ctx->coop_max, ctx->stream);
-            if (le != cudaSuccess) return fail_cuda(ctx, le, "kernel launch");
-            ctx->launches++;
+            rc = launched(ctx, p252::launch_digest(limbs(&tag), below_full, p.level_size, 4, level, 1, false, ctx->coop_max,
+                                                   ctx->stream));
+            if (rc != P252_OK) return rc;
             if (timing) CU(cudaEventRecord(ctx->level_events[(size_t)l].k1, ctx->stream));
         }
         below_full = level;
@@ -2364,8 +2259,7 @@ int p252_merkle4_build_dist(p252_ctx* ctx, const p252_fr* leaves_shard, size_t n
     // every level must be complete on every rank before the call is considered done
     CU(cudaStreamWaitEvent(ctx->stream, ctx->ev_comm, 0));
     if (timing) CU(cudaEventRecord(ctx->ev_tree_end, ctx->stream));
-    if (!(flags & P252_ASYNC)) CU(cudaStreamSynchronize(ctx->stream));
-    return P252_OK;
+    return device_done(ctx, P252_OK, flags);
 }
 
 int p252_tree_level_timings(p252_ctx* ctx, p252_level_timing* levels, int capacity, int* n_levels, float* total_ms) {

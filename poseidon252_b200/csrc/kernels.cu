@@ -284,6 +284,13 @@ __global__ void __launch_bounds__(kT, kDense ? 1 : kMB) k_permute(uint8_t* __res
     }
 }
 
+// *counter += the number of active lanes of the warp with `hit`, one atomic per warp that has any
+__device__ __forceinline__ void warp_count(unsigned long long* counter, bool hit) {
+    const unsigned act = __activemask();
+    const unsigned b = __ballot_sync(act, hit);
+    if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(counter, (unsigned long long)__popc(b));
+}
+
 // ---- encrypt / decrypt (dusk_safe::encrypt / decrypt with Domain::Encryption) -------------------
 // pattern [Absorb(2), Absorb(1), Squeeze(L), Absorb(L), Squeeze(1)]; 2*ceil(L/4) permutations.
 template <bool kDecrypt>
@@ -366,11 +373,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) k_crypt(FrArg tag, const
             const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
             for (uint32_t k = 0; k < L; ++k) store_fr(dsti + (size_t)k * 32, zero);
         }
-        if (n_failed) {                                   // one atomic per warp that saw a failure
-            const unsigned act = __activemask();
-            const unsigned bad = __ballot_sync(act, !good);
-            if (bad && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(n_failed, (unsigned long long)__popc(bad));
-        }
+        if (n_failed) warp_count(n_failed, !good);
     }
 }
 
@@ -429,11 +432,7 @@ __global__ void __launch_bounds__(256) k_mtree_keys(const uint64_t* __restrict__
     }
     keys[i] = key;
     pos[i] = i;
-    if (rejected) {
-        const unsigned act = __activemask();
-        const unsigned b = __ballot_sync(act, bad);
-        if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(b));
-    }
+    if (rejected) warp_count(rejected, bad);
 }
 
 // k_mtree_leaf_write: over the keys sorted stably by leaf index, the last item of every run of equal keys (the last
@@ -605,11 +604,7 @@ __global__ void __launch_bounds__(256) k_smtree_keys(const uint64_t* __restrict_
     const bool bad = key >= capacity || (op && op[i] > 1);
     keys[i] = bad ? capacity : key;
     bpos[i] = i;
-    if (rejected) {
-        const unsigned act = __activemask();
-        const unsigned b = __ballot_sync(act, bad);
-        if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(b));
-    }
+    if (rejected) warp_count(rejected, bad);
 }
 
 // k_smtree_leaf_write: over the keys sorted stably by position, the last item of every run of equal keys (the last
@@ -674,7 +669,8 @@ __global__ void __launch_bounds__(256) k_smtree_count(const uint8_t* __restrict_
 // ---- compact sparse trees: sorted (index, value) lists per level (p252_ctree) -----------------------------------------
 // A change list is (key, value, present) sorted by key with distinct keys: present 1 inserts or overwrites, 0 removes.
 // Level l's merge takes its sorted list (keys / values, count on the device) and its change list to a new sorted list
-// out of place; the dirty parents of level l + 1 are gathered from the new list and hashed by launch_smtree_digest.
+// out of place; the dirty parents of level l + 1 (k_mtree_parents over the change list) are gathered from the new list and
+// hashed by the presence-aware launch_mtree_digest.
 
 // first index in a[0, n) whose key is >= k
 __device__ __forceinline__ uint64_t ctree_lower_bound(const uint64_t* __restrict__ a, uint64_t n, uint64_t k) {
@@ -706,11 +702,7 @@ __global__ void __launch_bounds__(256) k_ctree_keys(const uint64_t* __restrict__
     const bool bad = key > max_pos || (op && op[i] > 1);
     keys[i] = key;
     bpos[i] = i | (bad ? 0x80000000u : 0u);
-    if (rejected) {
-        const unsigned act = __activemask();
-        const unsigned b = __ballot_sync(act, bad);
-        if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(b));
-    }
+    if (rejected) warp_count(rejected, bad);
 }
 
 // k_ctree_valid: flag[k] = the sorted item k is valid (bit 31 of its batch position clear)
@@ -831,16 +823,6 @@ __global__ void __launch_bounds__(256) k_ctree_commit(const uint64_t* __restrict
         lkeys[t] = 0;
         store_fr(lvals + t * 32, v);
     }
-}
-
-// k_ctree_parents: candidates of the next level's change list, key / arity of a sorted change list (first of each run)
-__global__ void __launch_bounds__(256) k_ctree_parents(const uint64_t* __restrict__ ckeys, const int* __restrict__ ccnt, uint32_t nb,
-                                                       uint32_t log2_arity, uint8_t* __restrict__ flag, uint64_t* __restrict__ parent) {
-    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= nb) return;
-    const uint64_t par = ckeys[t] >> log2_arity;
-    flag[t] = t < (uint32_t)*ccnt && (t == 0 || (ckeys[t - 1] >> log2_arity) != par);
-    parent[t] = par;
 }
 
 // k_ctree_gather: one thread per dirty parent g: its arity children in the merged level (binary search for g * arity,
@@ -996,11 +978,7 @@ __global__ void __launch_bounds__(256) k_varlen_keys(const uint64_t* __restrict_
                         : crypt_item_ok<kCrypt>(offsets, n, base, n_scalars, max_len, i, a, b);
     keys[i] = ok ? (uint32_t)(len - (kCrypt == 2 ? 1 : 0)) : 0u;
     vals[i] = i;
-    if (rejected) {
-        const unsigned act = __activemask();
-        const unsigned bad = __ballot_sync(act, !ok);
-        if (bad && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(rejected, (unsigned long long)__popc(bad));
-    }
+    if (rejected) warp_count(rejected, !ok);
 }
 
 // k_sponge_digest_varlen: k_sponge_digest over the items sorted by length.  Warp item k is item i = perm[k] with
@@ -1509,20 +1487,30 @@ cudaError_t launch_mtree_parents(const uint64_t* d, const int* cnt, uint32_t bou
     return cudaGetLastError();
 }
 
+template <bool kSparse>
+static void mtree_digest(FrArg tag, const uint8_t* b, int arity, uint8_t* o, const uint64_t* d, const int* cnt, size_t bound,
+                         size_t coop_max, cudaStream_t st, const uint8_t* bp, uint8_t* lp) {
+    if (bound <= coop_max) {
+        const size_t warps = (bound + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
+        k_mtree_digest_coop<kSparse><<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(tag, b, (uint32_t)arity, o, d,
+                                                                                                    cnt, bp, lp);
+    } else if (arity == 4) {
+        k_mtree_digest<2, kSparse><<<grid_for(bound), kThreads, 0, st>>>(tag, b, o, d, cnt, bp, lp);
+    } else {
+        k_mtree_digest<1, kSparse><<<grid_for(bound), kThreads, 0, st>>>(tag, b, o, d, cnt, bp, lp);
+    }
+}
+
 cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int arity, void* level, const uint64_t* d,
-                                const int* cnt, size_t bound, size_t coop_max, cudaStream_t st) {
+                                const int* cnt, size_t bound, size_t coop_max, cudaStream_t st, const uint8_t* below_present,
+                                uint8_t* level_present) {
     if (bound == 0) return cudaSuccess;
     const uint8_t* b = static_cast<const uint8_t*>(below);
     uint8_t* o = static_cast<uint8_t*>(level);
-    if (bound <= coop_max) {
-        const size_t warps = (bound + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_mtree_digest_coop<false><<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(to_arg(tag), b, (uint32_t)arity, o,
-                                                                                                  d, cnt, nullptr, nullptr);
-    } else if (arity == 4) {
-        k_mtree_digest<2, false><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, nullptr, nullptr);
-    } else {
-        k_mtree_digest<1, false><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, nullptr, nullptr);
-    }
+    if (below_present)
+        mtree_digest<true>(to_arg(tag), b, arity, o, d, cnt, bound, coop_max, st, below_present, level_present);
+    else
+        mtree_digest<false>(to_arg(tag), b, arity, o, d, cnt, bound, coop_max, st, nullptr, nullptr);
     return cudaGetLastError();
 }
 
@@ -1548,24 +1536,6 @@ cudaError_t launch_smtree_seed(uint8_t* present, void* leaves, uint64_t groups, 
     if (groups == 0) return cudaSuccess;
     k_smtree_seed<<<(unsigned)((groups + 255) / 256), 256, 0, st>>>(present, static_cast<uint8_t*>(leaves), groups, capacity,
                                                                     arity == 4 ? 2u : 1u, flag, parent);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_smtree_digest(const uint64_t tag[4], const void* below, const uint8_t* below_present, int arity, void* level,
-                                 uint8_t* level_present, const uint64_t* d, const int* cnt, size_t bound, size_t coop_max,
-                                 cudaStream_t st) {
-    if (bound == 0) return cudaSuccess;
-    const uint8_t* b = static_cast<const uint8_t*>(below);
-    uint8_t* o = static_cast<uint8_t*>(level);
-    if (bound <= coop_max) {
-        const size_t warps = (bound + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_mtree_digest_coop<true><<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(
-            to_arg(tag), b, (uint32_t)arity, o, d, cnt, below_present, level_present);
-    } else if (arity == 4) {
-        k_mtree_digest<2, true><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, below_present, level_present);
-    } else {
-        k_mtree_digest<1, true><<<grid_for(bound), kThreads, 0, st>>>(to_arg(tag), b, o, d, cnt, below_present, level_present);
-    }
     return cudaGetLastError();
 }
 
@@ -1632,12 +1602,6 @@ cudaError_t launch_ctree_commit(const uint64_t* okeys, const void* ovals, uint64
                                 uint64_t* lkeys, void* lvals, uint64_t* lcount, cudaStream_t st) {
     k_ctree_commit<<<blocks256(s), 256, 0, st>>>(okeys, static_cast<const uint8_t*>(ovals), s, stats, ok, lkeys,
                                                  static_cast<uint8_t*>(lvals), lcount);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_ctree_parents(const uint64_t* ckeys, const int* ccnt, uint32_t nb, int arity, uint8_t* flag, uint64_t* parent,
-                                 cudaStream_t st) {
-    k_ctree_parents<<<blocks256(nb), 256, 0, st>>>(ckeys, ccnt, nb, arity == 4 ? 2u : 1u, flag, parent);
     return cudaGetLastError();
 }
 

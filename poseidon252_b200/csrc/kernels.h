@@ -41,9 +41,11 @@ cudaError_t launch_mtree_leaf_write(const uint64_t* keys, const uint32_t* pos, u
 cudaError_t launch_mtree_parents(const uint64_t* d, const int* cnt, uint32_t bound, int arity, uint8_t* flag, uint64_t* parent,
                                  cudaStream_t st);
 // level[d[k]] = Hash::digest(Domain::Merkle{arity}, below[d[k]*arity .. +arity]) for k < *cnt <= bound; lane-split kernel
-// when bound <= coop_max
+// when bound <= coop_max.  With presence bytes (p252_smtree / p252_ctree, indexed like below / level): an empty group
+// stores value 0 / presence 0, any other its digest / presence 1
 cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int arity, void* level, const uint64_t* d,
-                                const int* cnt, size_t bound, size_t coop_max, cudaStream_t st);
+                                const int* cnt, size_t bound, size_t coop_max, cudaStream_t st,
+                                const uint8_t* below_present = nullptr, uint8_t* level_present = nullptr);
 // Sparse fixed-height trees (p252_smtree).  keys: pos[i] for a valid item (pos < capacity, op NULL or 0/1), else the
 // sentinel `capacity` (counted into *rejected); bpos[i] = i
 cudaError_t launch_smtree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t capacity, uint64_t* keys,
@@ -57,10 +59,6 @@ cudaError_t launch_smtree_leaf_write(const uint64_t* keys, const uint32_t* bpos,
 // parent[g] = g, for the `groups` leaf groups
 cudaError_t launch_smtree_seed(uint8_t* present, void* leaves, uint64_t groups, uint64_t capacity, int arity, uint8_t* flag,
                                uint64_t* parent, cudaStream_t st);
-// launch_mtree_digest with presence: an empty group stores value 0 / presence 0, any other its digest / presence 1
-cudaError_t launch_smtree_digest(const uint64_t tag[4], const void* below, const uint8_t* below_present, int arity, void* level,
-                                 uint8_t* level_present, const uint64_t* d, const int* cnt, size_t bound, size_t coop_max,
-                                 cudaStream_t st);
 // *out += non-zero bytes of present[0, n)
 cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned long long* out, cudaStream_t st);
 // Compact sparse trees (p252_ctree).  A change list is (keys, values, present) sorted by distinct key, count on the device;
@@ -90,9 +88,6 @@ cudaError_t launch_ctree_count(const uint64_t* lcount, uint64_t s, uint32_t nb, 
 // if *ok: the level and its count become the merged list, vacated slots zeroed
 cudaError_t launch_ctree_commit(const uint64_t* okeys, const void* ovals, uint64_t s, const uint64_t* stats, const uint32_t* ok,
                                 uint64_t* lkeys, void* lvals, uint64_t* lcount, cudaStream_t st);
-// next-level candidates: parent[t] = ckeys[t] / arity, flag = first of its run (t < *ccnt)
-cudaError_t launch_ctree_parents(const uint64_t* ckeys, const int* ccnt, uint32_t nb, int arity, uint8_t* flag, uint64_t* parent,
-                                 cudaStream_t st);
 // dense groups (arity scalars, absent 0) and presence bytes of the dirty parents pkeys[0..*pcnt) from the merged level
 cudaError_t launch_ctree_gather(const uint64_t* okeys, const void* ovals, const uint64_t* stats, uint64_t s, const uint64_t* pkeys,
                                 const int* pcnt, uint32_t nb, int arity, void* groups, uint8_t* gpres, cudaStream_t st);
