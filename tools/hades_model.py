@@ -41,6 +41,7 @@ LAMBDA = lcm(*range(WIDTH, 3 * WIDTH - 1))          # lcm(5..13) = 360360
 CMAT = [[LAMBDA // (i + j + WIDTH) for j in range(WIDTH)] for i in range(WIDTH)]
 M32 = (1 << 32) - 1
 TWO256 = 1 << 256
+PINV = pow(P, -1, TWO256)
 # exponent words (0x433 << 20) of the eight IEEE-double column sums the FP64 mix folds into 9 limbs
 K_OFF = 0x43300000 * sum(1 << (32 * k) for k in range(1, 9))
 
@@ -122,7 +123,7 @@ def montmul(x: int, y: int, site: str = "montmul") -> int:
     assert 0 <= x and x + P <= TWO256, "row operand too large for the 9-limb window"
     assert 0 <= y < TWO256
     t = x * y
-    m = (-t * pow(P, -1, TWO256)) % TWO256
+    m = (-t * PINV) % TWO256
     r = (t + m * P) >> 256
     assert (t + m * P) & (TWO256 - 1) == 0
     assert r < TWO256, "montmul result overflows 8 limbs"
@@ -161,20 +162,26 @@ def montsqr(a: int, site: str = "montsqr") -> int:
     plus the high half.  No row-operand constraint; only the result must fit 8 limbs."""
     assert 0 <= a < TWO256
     t = a * a
-    m = (-t * pow(P, -1, TWO256)) % TWO256
+    m = (-t * PINV) % TWO256
     r = (t + m * P) >> 256
     assert r < TWO256, "montsqr result overflows 8 limbs"
     Bounds.note(site, r)
     return r
 
 
-def sbox(u: int) -> int:
+def sbox(u: int, trace=None) -> int:
     a = montsqr(u, "sqr1")
     b = montsqr(a, "sqr2")
-    return montmul(u, b, "x5")
+    x5 = montmul(u, b, "x5")
+    if trace is not None:
+        trace("sqr1", a)
+        trace("sqr2", b)
+        trace("x5", x5)
+    return x5
 
 
-def mix(z: Sequence[int], arc_next: Sequence[int] | None) -> List[int]:
+def mix(z: Sequence[int], arc_next: Sequence[int] | None, trace=None) -> List[int]:
+    """trace(lane, T): called with each lane's 9-limb total before the Montgomery row."""
     out = []
     zl = [limbs32(v) for v in z]
     for i in range(WIDTH):
@@ -185,25 +192,45 @@ def mix(z: Sequence[int], arc_next: Sequence[int] | None) -> List[int]:
         t = sum(CMAT[i][j] * z[j] for j in range(WIDTH))
         if arc_next is not None:
             t += arc_next[i]
+        if trace is not None:
+            trace(i, t)
         out.append(redc1(t))
     return out
 
 
-def permute_model(state_mont: Sequence[int]) -> List[int]:
+def permute_model(state_mont: Sequence[int], trace=None) -> List[int]:
     """state_mont: 5 integers < p in standard Montgomery form (BlsScalar.0 as an integer).
-    Returns the permuted state in the same form -- must equal the reference bit for bit."""
+    Returns the permuted state in the same form -- must equal the reference bit for bit.
+
+    trace(r, site, lane, value), if given, sees every intermediate integer: per round r the S-box
+    input or linear lane `u`, the S-box's `sqr1`, `sqr2`, `x5`, the partial rounds' `gmul`, and the
+    mix total `T` that produces round r+1's `u` (round 67: the final mix); then, under r = ROUNDS,
+    each lane's `final` value before the last conditional subtraction."""
     T = TABLES
     u = [condsub(s + a) for s, a in zip(state_mont, T.A[0])]
     for r in range(ROUNDS):
+        def lane_trace(lane):
+            return None if trace is None else (lambda name, v: trace(r, name, lane, v))
+        if trace is not None:
+            for i, x in enumerate(u):
+                trace(r, "u", i, x)
         if is_full(r):
-            z = [sbox(x) for x in u]
+            z = [sbox(x, lane_trace(i)) for i, x in enumerate(u)]
         else:
-            z = list(u[:4]) + [montmul(T.G[r], sbox(u[4]), "gmul")]
+            g = montmul(T.G[r], sbox(u[4], lane_trace(4)), "gmul")
+            if trace is not None:
+                trace(r, "gmul", 4, g)
+            z = list(u[:4]) + [g]
+        mix_trace = None if trace is None else (lambda i, t: trace(r, "T", i, t))
         if r + 1 < ROUNDS:
-            u = mix(z, T.A[r + 1])
+            u = mix(z, T.A[r + 1], mix_trace)
         else:
-            v = mix(z, None)
-            return [condsub(montmul(T.F, x, "final")) for x in v]
+            v = mix(z, None, mix_trace)
+            w = [montmul(T.F, x, "final") for x in v]
+            if trace is not None:
+                for i, x in enumerate(w):
+                    trace(ROUNDS, "final", i, x)
+            return [condsub(x) for x in w]
     raise AssertionError
 
 
