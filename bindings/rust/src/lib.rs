@@ -116,6 +116,10 @@ mod crypt_varlen;
 mod ctree;
 pub use ctree::{p252_ctree, CompactTree};
 
+// JubJub key exchange and encrypt / decrypt with the shared secret derived on the device: their own `extern "C"` block in
+// dhke.rs (methods on Engine).
+mod dhke;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

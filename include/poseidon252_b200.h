@@ -245,6 +245,49 @@ int p252_decrypt_batch_varlen(p252_ctx* ctx, const p252_fr* cipher, size_t n_sca
                               size_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* msg, uint8_t* ok,
                               size_t* n_failed, size_t* n_rejected, int flags);
 
+/* ---- JubJub key exchange ------------------------------------------------------------------------
+ * dhke(secret, public) = [secret] public as JubJubAffine (u, v): the shared secret that encrypt / decrypt take
+ * (src/encryption.rs:11-43, "Poseidon + JubJub DHKE + SAFE").  JubJub: -u^2 + v^2 = 1 + d u^2 v^2 over the same field
+ * as p252_fr, d = -10240/10241; prime subgroup order r_J (252 bits), cofactor 8.
+ *
+ * A secret scalar is p252_jscalar: the CANONICAL integer s < r_J as 4 x u64 little-endian limbs, i.e. the 32 bytes of
+ * JubJubScalar::to_bytes().  Unlike p252_fr it is NOT a Montgomery image (the limbs of dusk-jubjub's Fr are not public
+ * API, to_bytes is).  Points are (u, v) as two p252_fr (JubJubAffine::get_u / get_v, i.e. BlsScalar.0): the layout of
+ * secret_uv of p252_{en,de}crypt_batch[_varlen], so a p252_dhke_batch output feeds those calls unchanged.
+ *
+ * Shapes: item i uses secret[n_secret == 1 ? 0 : i] and public_uv[n_public == 1 ? 0 : i] (n_public points of 2
+ * scalars); n_secret and n_public are each 1 or n.  (1, n) is a receiver's scan (one view key, the notes' keys), (n, 1) a
+ * sender's R_i = [r_i] G or [r_i] pk.
+ * Item validity: s < r_J, u, v < p and (u, v) on the curve.  There is no subgroup check (the reference does none): a
+ * torsion component passes through.  Validity is a per-item data condition checked on the device for both memory spaces;
+ * the call returns P252_OK and marks an invalid item with ok[i] = 0 and
+ *   p252_dhke_batch:           output (0, 0), which is not a curve point (the identity is (0, 1));
+ *   p252_encrypt_batch_dhke:   a zeroed cipher row;
+ *   p252_decrypt_batch_dhke:   a zeroed message, counted into *n_failed together with the authentication failures (an
+ *                              item counts once).
+ * n_invalid / n_failed: optional HOST pointers for both memory spaces (lifetime as for p252_decrypt_batch).
+ * P252_ERR_INVALID_POINT is returned by the single-item front ends (Python dhke(), p252::dhke), not by these calls.
+ * Batch checks, before anything runs: n_secret or n_public not 1 or n, a NULL buffer with n > 0, DEVICE buffers other
+ * than ok not 16-byte aligned -> INVALID_ARGUMENT; L == 0 -> INVALID_IO_PATTERN (as p252_encryption_tag).
+ * The fused calls run the key exchange and then the kernels of p252_encrypt_batch / p252_decrypt_batch (same shapes:
+ * msg n x L, cipher n x (L + 1), nonce n).  Their intermediate shared secrets never leave the context's staging arenas,
+ * for DEVICE buffers too, and the arenas are zeroed on every exit path; so these calls are synchronous for both memory
+ * spaces (P252_ASYNC only defers the publication of the count to p252_sync).  HOST calls stage secrets, points, nonces and
+ * plaintext through the same zeroed arenas; a broadcast operand is staged once per chunk.
+ * Each item is one scalar multiplication in constant time (no branch and no address depends on secret bits); see
+ * DESIGN.md section 4. */
+typedef struct p252_jscalar {
+    uint64_t l[4];
+} p252_jscalar;
+int p252_dhke_batch(p252_ctx* ctx, const p252_jscalar* secret, size_t n_secret, const p252_fr* public_uv, size_t n_public,
+                    size_t n, p252_fr* shared_uv, uint8_t* ok, size_t* n_invalid, int flags);
+int p252_encrypt_batch_dhke(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* secret, size_t n_secret,
+                            const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* cipher, uint8_t* ok,
+                            size_t* n_invalid, int flags);
+int p252_decrypt_batch_dhke(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L, const p252_jscalar* secret,
+                            size_t n_secret, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* msg,
+                            uint8_t* ok, size_t* n_failed, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

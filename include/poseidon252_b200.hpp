@@ -8,7 +8,8 @@
 //   dusk_poseidon::{encrypt, decrypt}        (src/encryption.rs:62-95) -> p252::encrypt / p252::decrypt
 //   dusk_poseidon::Error                     (src/error.rs:11-32)      -> p252::Error (exception)
 //   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
-//   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, merkle4_build.
+//   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
+//   decrypt_batch_dhke, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -260,6 +261,52 @@ inline std::vector<std::vector<Scalar>> decrypt_batch_varlen(const std::vector<s
     std::vector<std::vector<Scalar>> res(n);
     for (size_t i = 0; i < n; ++i) res[i].assign(msg.begin() + (off[i] - i), msg.begin() + (off[i + 1] - i - 1));
     return res;
+}
+
+// NEW: JubJub key exchange (p252_dhke_batch) and encrypt / decrypt with the shared secret derived on the device
+// (p252_{en,de}crypt_batch_dhke).  Secrets are canonical p252_jscalar (JubJubScalar::to_bytes), points (u, v) pairs;
+// n_secret and n_public are each 1 (broadcast) or n.  ok[i] == 0 marks an invalid item (secret >= r_J or a point off the
+// curve; for decrypt also an authentication failure) with a zeroed output row.
+using JubJubScalar = p252_jscalar;
+// returns n x 2 scalars: (u, v) of [secret] public per item
+inline std::vector<Scalar> dhke_batch(const JubJubScalar* secrets, size_t n_secret, const Scalar* publics_uv, size_t n_public,
+                                      size_t n, std::vector<uint8_t>& ok, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> shared(2 * n);
+    ok.assign(n, 0);
+    check(p252_dhke_batch(e.get(), secrets, n_secret, publics_uv, n_public, n, shared.data(), ok.data(), nullptr, P252_MEM_HOST),
+          e.get());
+    return shared;
+}
+// dhke(secret, public) for one item; throws Error(P252_ERR_INVALID_POINT) like the reference's Error::InvalidPoint
+inline void dhke(const JubJubScalar& secret, const Scalar (&public_uv)[2], Scalar (&shared_uv)[2],
+                 Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok;
+    const auto r = dhke_batch(&secret, 1, public_uv, 1, 1, ok, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    shared_uv[0] = r[0];
+    shared_uv[1] = r[1];
+}
+// msg n x L -> cipher n x (L+1)
+inline std::vector<Scalar> encrypt_batch_dhke(const Scalar* msg, size_t n, size_t L, const JubJubScalar* secrets, size_t n_secret,
+                                              const Scalar* publics_uv, size_t n_public, const Scalar* nonces,
+                                              std::vector<uint8_t>& ok, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> cipher(n * (L + 1));
+    ok.assign(n, 0);
+    check(p252_encrypt_batch_dhke(e.get(), msg, n, L, secrets, n_secret, publics_uv, n_public, nonces, cipher.data(), ok.data(),
+                                  nullptr, P252_MEM_HOST),
+          e.get());
+    return cipher;
+}
+// cipher n x (L+1) -> msg n x L
+inline std::vector<Scalar> decrypt_batch_dhke(const Scalar* cipher, size_t n, size_t L, const JubJubScalar* secrets,
+                                              size_t n_secret, const Scalar* publics_uv, size_t n_public, const Scalar* nonces,
+                                              std::vector<uint8_t>& ok, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> msg(n * L);
+    ok.assign(n, 0);
+    check(p252_decrypt_batch_dhke(e.get(), cipher, n, L, secrets, n_secret, publics_uv, n_public, nonces, msg.data(), ok.data(),
+                                  nullptr, P252_MEM_HOST),
+          e.get());
+    return msg;
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

@@ -74,6 +74,12 @@ SIGNATURES = {
                                           c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_decrypt_batch_varlen": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p,
                                           c_void_p, c_void_p, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t), c_int]),
+    "p252_dhke_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p,
+                                ctypes.POINTER(c_size_t), c_int]),
+    "p252_encrypt_batch_dhke": (c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t,
+                                        c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_decrypt_batch_dhke": (c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_void_p, c_size_t,
+                                        c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
 }
 
 MEM_HOST, MEM_DEVICE, ASYNC, TIMING, NO_GATHER = 0, 1, 2, 4, 8

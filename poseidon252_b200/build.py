@@ -16,7 +16,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "lib", "libposeidon252_b200.so")
 SOURCES = [os.path.join(CSRC, f) for f in ("kernels.cu", "capi.cu")]
 DEPS = SOURCES + [os.path.join(CSRC, f) for f in ("hades_device.cuh", "fr_ptx.cuh", "hades_tables.inc", "kernels.h",
-                                                 "host_field.h")] + [os.path.join(ROOT, "include", "poseidon252_b200.h")]
+                                                 "host_field.h", "jubjub_device.cuh")] + [os.path.join(ROOT, "include", "poseidon252_b200.h")]
 GENERATORS = [os.path.join(ROOT, "tools", f) for f in ("gen_tables.py", "gen_field_ptx.py", "hades_model.py")]
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -8,6 +8,7 @@
 // Mirrors, for the batch path, the reference's public surface (src/lib.rs:13-31):
 //   Hash / Domain / io_pattern      src/hash.rs:21-155      -> p252_hash_tag, p252_hash_batch
 //   encrypt / decrypt               src/encryption.rs:62-95 -> p252_encrypt_batch, p252_decrypt_batch
+//   dhke + encrypt / decrypt        src/encryption.rs:11-43 -> p252_dhke_batch, p252_{en,de}crypt_batch_dhke
 //   Error                           src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -19,6 +20,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <initializer_list>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -180,6 +182,8 @@ struct Io {
     const void* h_in;    // copied to the device before the launch (may be null)
     void* h_out;         // copied back after the launch (may be null)
     size_t item_bytes;   // bytes per batch item
+    bool once = false;   // h_in is ONE item read by every item of the batch: staged once per chunk, never offset
+    bool device = false; // h_in / h_out is a device buffer: the launch uses it in place at the chunk's offset, nothing staged
 };
 
 int join_slots(p252_ctx* ctx, int rc, bool wipe);
@@ -277,14 +281,16 @@ template <typename Launch>
 int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
     if (n == 0) return P252_OK;
     size_t per_item = 0;
-    for (auto& io : ios) per_item += (io.item_bytes + 15) / 16 * 16;
+    for (auto& io : ios)
+        if (!io.once && !io.device) per_item += (io.item_bytes + 15) / 16 * 16;
     size_t chunk = std::max<size_t>(1024, std::min(chunk_items_max(), kChunkBytesTarget / std::max<size_t>(per_item, 1)));
     chunk = (chunk + 127) / 128 * 128;
     if (chunk > n) chunk = n;
     std::vector<void*> d(ios.size());
     auto carve = [&](void* arena) {
         Carve c{static_cast<uint8_t*>(arena)};
-        for (size_t b = 0; b < ios.size(); ++b) d[b] = c.take<uint8_t>(chunk * ios[b].item_bytes);
+        for (size_t b = 0; b < ios.size(); ++b)
+            if (!ios[b].device) d[b] = c.take<uint8_t>((ios[b].once ? 1 : chunk) * ios[b].item_bytes);
         return c.used;
     };
     const size_t need = carve(nullptr);
@@ -299,14 +305,20 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
             int rc = slot_reserve(ctx, sl, need, wipe);
             if (rc != P252_OK) return rc;
             carve(sl.arena);
-            for (size_t b = 0; b < ios.size(); ++b)
-                if (ios[b].h_in)
-                    CU(cudaMemcpyAsync(d[b], static_cast<const uint8_t*>(ios[b].h_in) + off * ios[b].item_bytes,
-                                       cnt * ios[b].item_bytes, cudaMemcpyHostToDevice, sl.stream));
+            for (size_t b = 0; b < ios.size(); ++b) {
+                const Io& io = ios[b];
+                const size_t at = io.once ? 0 : off * io.item_bytes;
+                if (io.device)
+                    d[b] = io.h_out ? static_cast<uint8_t*>(io.h_out) + at
+                                    : const_cast<uint8_t*>(static_cast<const uint8_t*>(io.h_in) + at);
+                else if (io.h_in)
+                    CU(cudaMemcpyAsync(d[b], static_cast<const uint8_t*>(io.h_in) + at, (io.once ? 1 : cnt) * io.item_bytes,
+                                       cudaMemcpyHostToDevice, sl.stream));
+            }
             if ((long long)k == fail_at) return injected_fault(ctx);
             if ((rc = launched(ctx, launch(d.data(), cnt, sl.stream))) != P252_OK) return rc;
             for (size_t b = 0; b < ios.size(); ++b)
-                if (ios[b].h_out)
+                if (ios[b].h_out && !ios[b].device)
                     CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + off * ios[b].item_bytes, d[b],
                                        cnt * ios[b].item_bytes, cudaMemcpyDeviceToHost, sl.stream));
         }
@@ -806,6 +818,107 @@ int p252_decrypt_batch(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L,
     }, /*wipe=*/true);
     if (rc == P252_OK && n_failed) *n_failed = count_zero(ok, n);
     return rc;
+}
+
+// ---- JubJub key exchange (dhke) and the encrypt / decrypt batches that derive their shared secret with it -------------
+// Batch checks shared by the three calls: the broadcast shapes (1 or n), NULL buffers with n > 0 (ok is a byte array and
+// needs no alignment), 16-byte alignment of DEVICE buffers.
+static int dhke_args(size_t n, const void* secret, size_t n_secret, const void* pub, size_t n_public,
+                     std::initializer_list<const void*> bufs, const uint8_t* ok, int flags) {
+    if ((n_secret != 1 && n_secret != n) || (n_public != 1 && n_public != n)) return P252_ERR_INVALID_ARGUMENT;
+    if (n && (!secret || !pub || !ok)) return P252_ERR_INVALID_ARGUMENT;
+    for (const void* b : bufs)
+        if (n && !b) return P252_ERR_INVALID_ARGUMENT;
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(secret) || !aligned16(pub)) return P252_ERR_INVALID_ARGUMENT;
+        for (const void* b : bufs)
+            if (!aligned16(b)) return P252_ERR_INVALID_ARGUMENT;
+    }
+    return P252_OK;
+}
+
+int p252_dhke_batch(p252_ctx* ctx, const p252_jscalar* secret, size_t n_secret, const p252_fr* public_uv, size_t n_public,
+                    size_t n, p252_fr* shared_uv, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, secret, n_secret, public_uv, n_public, {shared_uv}, ok, flags);
+    if (rc != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool sb = n_secret == 1, pb = n_public == 1;
+    if (flags & P252_MEM_DEVICE) {
+        if (n_invalid) *n_invalid = 0;
+        if (n == 0) return P252_OK;
+        if (n_invalid && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        rc = launched(ctx, p252::launch_dhke(secret, sb, public_uv, pb, n, shared_uv, ok, n_invalid ? ctx->d_counter : nullptr,
+                                             ctx->stream));
+        if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+        return device_done(ctx, rc, flags);
+    }
+    std::vector<Io> ios = {{secret, nullptr, 32, sb}, {public_uv, nullptr, 64, pb}, {nullptr, shared_uv, 64}, {nullptr, ok, 1}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return p252::launch_dhke(d[0], sb, d[1], pb, cnt, d[2], static_cast<uint8_t*>(d[3]), nullptr, st);
+    }, /*wipe=*/true);
+    if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+    return rc;
+}
+
+// launch_dhke into a slot arena, then the unchanged launch_encrypt / launch_decrypt on those shared secrets, then
+// launch_dhke_fix.  The shared secrets live only in the slot arenas for BOTH memory spaces (DEVICE buffers are used in
+// place, chunk by chunk), so the common exit join_slots(wipe) clears them on every path.  count: *n_invalid (encrypt) or
+// *n_failed (decrypt: authentication failures and invalid items, each once).
+static int crypt_dhke(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n, size_t L, const p252_jscalar* secret,
+                      size_t n_secret, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* out,
+                      uint8_t* ok, size_t* count, int flags) {
+    if (!ctx) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, secret, n_secret, public_uv, n_public, {in, nonce, out}, ok, flags);
+    if (rc != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = p252_encryption_tag(L, &tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1, pb = n_public == 1;
+    const uint32_t l32 = (uint32_t)L, out_row = decrypt ? l32 : l32 + 1;
+    if (count) *count = 0;
+    if (n == 0) return P252_OK;
+    unsigned long long* counter = nullptr;
+    if (dev && count) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    // 0 input, 1 secret, 2 public, 3 nonce, 4 output, 5 ok; 6 shared secrets and 7 validity live in the arena only
+    std::vector<Io> ios = {{in, nullptr, (decrypt ? L + 1 : L) * 32, false, dev}, {secret, nullptr, 32, sb, dev},
+                           {public_uv, nullptr, 64, pb, dev}, {nonce, nullptr, 32, false, dev},
+                           {nullptr, out, (size_t)out_row * 32, false, dev}, {nullptr, ok, 1, false, dev},
+                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[5]);
+        uint8_t* valid = static_cast<uint8_t*>(d[7]);
+        cudaError_t e = p252::launch_dhke(d[1], sb, d[2], pb, cnt, d[6], valid, nullptr, st);
+        if (e == cudaSuccess)
+            e = decrypt ? p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], okc, counter, st)
+                        : p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], st);
+        if (e == cudaSuccess) e = p252::launch_dhke_fix(decrypt, valid, cnt, d[4], out_row, okc, counter, st);
+        if (e == cudaSuccess) ctx->launches += 2;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    }, /*wipe=*/true);
+    if (!dev) {
+        if (rc == P252_OK && count) *count = count_zero(ok, n);
+        return rc;
+    }
+    if (rc == P252_OK) rc = counter_end(ctx, count);
+    return device_done(ctx, rc, flags);
+}
+
+int p252_encrypt_batch_dhke(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* secret, size_t n_secret,
+                            const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* cipher, uint8_t* ok,
+                            size_t* n_invalid, int flags) {
+    return crypt_dhke(ctx, false, msg, n, L, secret, n_secret, public_uv, n_public, nonce, cipher, ok, n_invalid, flags);
+}
+
+int p252_decrypt_batch_dhke(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L, const p252_jscalar* secret,
+                            size_t n_secret, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* msg,
+                            uint8_t* ok, size_t* n_failed, int flags) {
+    return crypt_dhke(ctx, true, cipher, n, L, secret, n_secret, public_uv, n_public, nonce, msg, ok, n_failed, flags);
 }
 
 // ---- arity-4 Merkle tree ------------------------------------------------------------------------------

@@ -1,0 +1,272 @@
+// Device-side JubJub arithmetic on the BLS12-381 Fr primitives of fr_ptx.cuh / hades_device.cuh: one scalar
+// multiplication per thread, for the key exchange dhke(secret, public) = [s] public (p252_dhke_batch).
+//
+// The curve: a u^2 + v^2 = 1 + d u^2 v^2 over Fr (the same p as the permutation), a = -1,
+// d = -10240/10241.  d is a non-square and -1 a square, so the unified addition law is complete: no identity,
+// doubling or small-order exceptions.  Points are kept in extended twisted-Edwards coordinates (X : Y : Z : T) with
+// u = X/Z, v = Y/Z, uv = T/Z (Hisil-Wong-Carter-Dawson 2008, a = -1).
+//
+// Operand bounds: every value this file produces is FULLY reduced (< p).  fr_add_mod / fr_sub_mod take and give [0, p);
+// fmul / fsqr take operands < p, so the row operand satisfies x + p < 2p < 2^256 (the precondition of montmul in
+// hades_device.cuh), the Montgomery product is < (p^2 + (2^256 - 1) p) / 2^256 < 2p (square: < 1.46 p), and one
+// fr_condsub brings it below p.  No lazy reduction: the condsub costs ~17 instructions next to ~130 per product.
+//
+// Secret independence: the scalar only ever reaches a 4-bit digit that drives masked selects over the whole table
+// (every entry is read, at addresses fixed by the loop counters), so neither a branch nor a memory address depends
+// on a secret bit.  The inversion's chain is the fixed bit pattern of p - 2.
+#pragma once
+#include <stdint.h>
+
+#include "hades_device.cuh"
+
+namespace p252 {
+namespace jj {
+
+// Montgomery images (x R mod p, 8 x u32 LE) of the constants
+__device__ __forceinline__ void set_one(uint32_t (&r)[8]) {
+    const uint32_t c[8] = {0xfffffffeu, 0x00000001u, 0x00034802u, 0x5884b7fau,
+                           0xecbc4ff5u, 0x998c4fefu, 0xacc5056fu, 0x1824b159u};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = c[k];
+}
+__device__ __forceinline__ void set_d(uint32_t (&r)[8]) {     // d = -10240/10241
+    const uint32_t c[8] = {0xb974f6b0u, 0x2a522455u, 0x0d9acab3u, 0xfc6cc9efu,
+                           0xc27628d1u, 0x7a08fb94u, 0xfe0e262eu, 0x57f8f6a8u};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = c[k];
+}
+__device__ __forceinline__ void set_2d(uint32_t (&r)[8]) {
+    const uint32_t c[8] = {0x72e9ed5fu, 0x54a448acu, 0x1b373967u, 0xa51befdbu,
+                           0x7b4a799eu, 0xc0d81f21u, 0xd27ecf14u, 0x3c0445feu};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = c[k];
+}
+// Order of the prime subgroup r_J (canonical, not Montgomery: 252 bits) and p - 2, the Fermat exponent of the inversion
+// (255 bits, 164 of them set).  Immediates, not __constant__ data: indexed only by unrolled or public loop counters.
+#define P252_JJ_ORDER {0xd6f72cb7u, 0xd0970e5eu, 0xccc81082u, 0xa6682093u, 0x01343b00u, 0x06673b01u, 0x6533afa9u, 0x0e7db4eau}
+#define P252_JJ_PM2 {0xffffffffu, 0xfffffffeu, 0xfffe5bfeu, 0x53bda402u, 0x09a1d805u, 0x3339d808u, 0x299d7d48u, 0x73eda753u}
+constexpr int kPm2Bits = 255, kPm2Ones = 164;
+
+// Products per scalar multiplication (montmul + montsqr), following the schedule below:
+//   on-curve check 4, T and 2d T of the input 2, table entries 2..15 14 x (8 + 1), 63 windows x (3 doublings without T
+//   x 7 + 1 doubling with T x 8 + 1 addition without T x 7), inversion (kPm2Bits - 1) squarings + (kPm2Ones - 1)
+//   products, affine conversion 2.
+constexpr int kWindows = 63;
+constexpr int kProductsPerDhke = 4 + 2 + 14 * 9 + kWindows * (3 * 7 + 8 + 7) + (kPm2Bits - 1) + (kPm2Ones - 1) + 2;
+static_assert(kProductsPerDhke == 2819, "product count of DESIGN.md section 4");
+
+__device__ __forceinline__ void fmul(uint32_t (&r)[8], const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    montmul(r, a, b);          // a < p  =>  a + p < 2^256; result < 2p
+    fr_condsub(r);
+}
+__device__ __forceinline__ void fsqr(uint32_t (&r)[8], const uint32_t (&a)[8]) {
+    montsqr(r, a);             // a < p  =>  result < 1.46 p
+    fr_condsub(r);
+}
+__device__ __forceinline__ void fcopy(uint32_t (&r)[8], const uint32_t (&a)[8]) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = a[k];
+}
+// a == b for fully reduced a, b
+__device__ __forceinline__ bool feq(const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    uint32_t x = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) x |= a[k] ^ b[k];
+    return x == 0;
+}
+// c < r_J for 256-bit little-endian words (borrow of c - r_J)
+__device__ __forceinline__ bool below_order(const uint32_t (&c)[8]) {
+    const uint32_t m[8] = P252_JJ_ORDER;
+    uint32_t borrow = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint64_t t = (uint64_t)c[k] - m[k] - borrow;
+        borrow = (uint32_t)(t >> 63);
+    }
+    return borrow != 0;
+}
+
+struct Ext {                    // extended coordinates, every coordinate < p
+    uint32_t X[8], Y[8], Z[8], T[8];
+};
+struct Cached {                 // an addend prepared for add(): (Y - X, Y + X, 2d T, 2 Z)
+    uint32_t ymx[8], ypx[8], kt[8], z2[8];
+};
+
+// on-curve check of an affine (u, v), u, v < p: -u^2 + v^2 == 1 + d u^2 v^2   (4 products)
+__device__ __forceinline__ bool on_curve(const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+    uint32_t uu[8], vv[8], w[8], c[8], lhs[8], rhs[8];
+    fsqr(uu, u);
+    fsqr(vv, v);
+    fr_sub_mod(lhs, vv, uu);
+    fmul(w, uu, vv);
+    set_d(c);
+    fmul(rhs, w, c);
+    set_one(c);
+    fr_add_mod(w, rhs, c);
+    return feq(lhs, w);
+}
+
+__device__ __forceinline__ void to_cached(Cached& c, const Ext& p) {   // 1 product
+    uint32_t k[8];
+    fr_sub_mod(c.ymx, p.Y, p.X);
+    fr_add_mod(c.ypx, p.Y, p.X);
+    set_2d(k);
+    fmul(c.kt, p.T, k);
+    fr_add_mod(c.z2, p.Z, p.Z);
+}
+
+// r = p + q, unified and complete (add-2008-hwcd-3): 8 products, 7 without T3
+template <bool kWantT>
+__device__ __forceinline__ void add(Ext& r, const Ext& p, const Cached& q) {
+    uint32_t a[8], b[8], c[8], d[8], e[8], f[8], g[8], h[8];
+    fr_sub_mod(e, p.Y, p.X);
+    fmul(a, e, q.ymx);          // A = (Y1 - X1)(Y2 - X2)
+    fr_add_mod(e, p.Y, p.X);
+    fmul(b, e, q.ypx);          // B = (Y1 + X1)(Y2 + X2)
+    fmul(c, p.T, q.kt);         // C = T1 2d T2
+    fmul(d, p.Z, q.z2);         // D = Z1 2 Z2
+    fr_sub_mod(e, b, a);        // E = B - A
+    fr_sub_mod(f, d, c);        // F = D - C
+    fr_add_mod(g, d, c);        // G = D + C
+    fr_add_mod(h, b, a);        // H = B + A
+    fmul(r.X, e, f);
+    fmul(r.Y, g, h);
+    fmul(r.Z, f, g);
+    if (kWantT) fmul(r.T, e, h);
+}
+
+// r = 2 p (dbl-2008-hwcd, a = -1): 4 squarings + 4 products, 3 without T3.  T of the input is not read.
+template <bool kWantT>
+__device__ __forceinline__ void dbl(Ext& r, const Ext& p) {
+    uint32_t a[8], b[8], c[8], e[8], f[8], g[8], h[8];
+    fsqr(a, p.X);               // A = X^2
+    fsqr(b, p.Y);               // B = Y^2
+    fsqr(c, p.Z);
+    fr_add_mod(c, c, c);        // C = 2 Z^2
+    fr_add_mod(e, p.X, p.Y);
+    fsqr(h, e);
+    fr_sub_mod(e, h, a);
+    fr_sub_mod(e, e, b);        // E = (X + Y)^2 - A - B
+    fr_sub_mod(g, b, a);        // G = D + B = B - A   (D = a A = -A)
+    fr_sub_mod(f, g, c);        // F = G - C
+    fr_add_mod(h, a, b);
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    fr_sub_mod(h, zero, h);     // H = D - B = -(A + B)
+    fmul(r.X, e, f);
+    fmul(r.Y, g, h);
+    fmul(r.Z, f, g);
+    if (kWantT) fmul(r.T, e, h);
+}
+
+// One cached table entry as 8 x 16 bytes (ymx, ypx, kt, z2), in thread-local memory.
+struct Entry {
+    uint4 w[8];
+};
+__device__ __forceinline__ void store_entry(Entry& e, const Cached& c) {
+    const uint32_t* src[4] = {c.ymx, c.ypx, c.kt, c.z2};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        e.w[2 * q] = make_uint4(src[q][0], src[q][1], src[q][2], src[q][3]);
+        e.w[2 * q + 1] = make_uint4(src[q][4], src[q][5], src[q][6], src[q][7]);
+    }
+}
+
+// c = tab[digit], digit in [0, 16): every entry is read and masked in, so the access pattern is the same for all digits
+__device__ __forceinline__ void select_entry(Cached& c, const Entry (&tab)[16], uint32_t digit) {
+    uint32_t acc[32];
+#pragma unroll
+    for (int k = 0; k < 32; ++k) acc[k] = 0;
+#pragma unroll 1
+    for (int j = 0; j < 16; ++j) {             // j is the public loop counter: the same 16 addresses for every digit
+        const uint32_t m = 0u - (uint32_t)(digit == (uint32_t)j);
+#pragma unroll
+        for (int w = 0; w < 8; ++w) {
+            const uint4 x = tab[j].w[w];
+            acc[4 * w + 0] |= x.x & m;
+            acc[4 * w + 1] |= x.y & m;
+            acc[4 * w + 2] |= x.z & m;
+            acc[4 * w + 3] |= x.w & m;
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) c.ymx[k] = acc[k], c.ypx[k] = acc[8 + k], c.kt[k] = acc[16 + k], c.z2[k] = acc[24 + k];
+}
+
+// r = z^(p-2) = 1/z for z != 0 (Fermat), left to right over the public bits of p - 2
+__device__ __forceinline__ void inverse(uint32_t (&r)[8], const uint32_t (&z)[8]) {
+    fcopy(r, z);                // the top bit
+#pragma unroll 1
+    for (int i = kPm2Bits - 2; i >= 0; --i) {
+        uint32_t t[8];
+        fsqr(t, r);
+        const uint32_t e[8] = P252_JJ_PM2;
+        uint32_t word = 0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) word = (k == (i >> 5)) ? e[k] : word;
+        if ((word >> (i & 31)) & 1u)
+            fmul(r, t, z);
+        else
+            fcopy(r, t);
+    }
+}
+
+// (ou, ov) = [s] (u, v) for s < 2^252 (canonical words) and an on-curve (u, v) with u, v < p (Montgomery).
+// Fixed 4-bit window, most significant first: 63 x (4 doublings + 1 addition of tab[digit]), then one inversion.
+__device__ __forceinline__ void scalar_mul(uint32_t (&ou)[8], uint32_t (&ov)[8], const uint32_t (&s)[8],
+                                           const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+    Entry tab[16];
+    Ext acc;
+    Cached c;
+    // tab[0] = identity (0 : 1 : 1 : 0) cached = (1, 1, 0, 2)
+    set_one(c.ymx);
+    set_one(c.ypx);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) c.kt[k] = 0;
+    fr_add_mod(c.z2, c.ymx, c.ymx);
+    store_entry(tab[0], c);
+    // tab[1] = P = (u : v : 1 : uv)
+    Cached pc;
+    fcopy(acc.X, u);
+    fcopy(acc.Y, v);
+    set_one(acc.Z);
+    fmul(acc.T, u, v);
+    to_cached(pc, acc);
+    store_entry(tab[1], pc);
+    // tab[j] = tab[j - 1] + P
+#pragma unroll 1
+    for (int j = 2; j < 16; ++j) {
+        Ext t;
+        add<true>(t, acc, pc);
+        acc = t;
+        to_cached(c, acc);
+        store_entry(tab[j], c);
+    }
+    // acc = identity
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc.X[k] = 0, acc.T[k] = 0;
+    set_one(acc.Y);
+    set_one(acc.Z);
+#pragma unroll 1
+    for (int w = kWindows - 1; w >= 0; --w) {
+        uint32_t limb = 0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) limb = (k == (w >> 3)) ? s[k] : limb;   // w is the public loop counter
+        const uint32_t digit = (limb >> ((w & 7) * 4)) & 15u;
+        Ext t;
+        dbl<false>(t, acc);
+        dbl<false>(acc, t);
+        dbl<false>(t, acc);
+        dbl<true>(acc, t);
+        select_entry(c, tab, digit);
+        add<false>(t, acc, c);
+        acc = t;
+    }
+    uint32_t zi[8];
+    inverse(zi, acc.Z);
+    fmul(ou, acc.X, zi);
+    fmul(ov, acc.Y, zi);
+}
+
+}  // namespace jj
+}  // namespace p252

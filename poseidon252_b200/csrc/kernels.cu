@@ -7,6 +7,7 @@
 //   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest (k_sponge_digest_varlen: inputs of any lengths)
 //   encrypt/decrypt  src/encryption.rs:62-95  -> k_crypt (k_crypt_varlen: messages of any lengths)
 //   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
+//   dhke             src/encryption.rs:11-43  -> k_dhke (JubJub scalar multiplication, jubjub_device.cuh)
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
 #include "kernels.h"
@@ -14,6 +15,7 @@
 #include <cstdlib>
 
 #include "hades_device.cuh"
+#include "jubjub_device.cuh"
 
 namespace p252 {
 
@@ -1444,6 +1446,70 @@ cudaError_t launch_decrypt(const uint64_t tag[4], const void* cipher, size_t n, 
                                                     static_cast<const uint8_t*>(secret_uv),
                                                     static_cast<const uint8_t*>(nonce), static_cast<uint8_t*>(msg),
                                                     ok, n_failed);
+    return cudaGetLastError();
+}
+
+// ---- JubJub key exchange (dhke(secret, public) = [s] public, JubJubAffine out) -------------------------------------
+// One thread per item, 2819 products (jubjub_device.cuh).  Item i reads secret[sb ? 0 : i] (canonical 4 x u64) and
+// pub[pb ? 0 : i] ((u, v), Montgomery); valid iff s < r_J, u, v < p and (u, v) on the curve.  An invalid item runs the
+// same schedule on (0, identity), so the instruction stream is the same for every item, and writes (0, 0), ok = 0.
+__global__ void __launch_bounds__(kThreads, 3) k_dhke(const uint8_t* __restrict__ secret, bool sb, const uint8_t* __restrict__ pub,
+                                                   bool pb, size_t n, uint8_t* __restrict__ out, uint8_t* __restrict__ ok,
+                                                   unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t s[8], u[8], v[8];
+    load_fr(s, secret + (sb ? 0 : i) * 32);
+    load_fr(u, pub + (pb ? 0 : i) * 64);
+    load_fr(v, pub + (pb ? 0 : i) * 64 + 32);
+    const bool valid = jj::below_order(s) & fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
+    const uint32_t m = 0u - (uint32_t)valid;
+    uint32_t one[8];
+    jj::set_one(one);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s[k] &= m, u[k] &= m, v[k] = (v[k] & m) | (one[k] & ~m);
+    uint32_t ou[8], ov[8];
+    jj::scalar_mul(ou, ov, s, u, v);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m;
+    store_fr(out + i * 64, ou);
+    store_fr(out + i * 64 + 32, ov);
+    ok[i] = valid ? 1 : 0;
+    if (n_invalid) warp_count(n_invalid, !valid);
+}
+
+// After a fused crypt: every item whose key exchange was invalid (valid[i] == 0) gets ok[i] = 0 and a zeroed output row
+// of `row` scalars.  count (may be null): encrypt adds the invalid items; decrypt adds those k_crypt did not already
+// count as authentication failures, so that each failed item is counted once.
+__global__ void __launch_bounds__(256) k_dhke_fix(bool decrypt, const uint8_t* __restrict__ valid, size_t n, uint8_t* out,
+                                                  uint32_t row, uint8_t* ok, unsigned long long* __restrict__ count) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const bool bad = valid[i] == 0;
+    bool hit = bad;
+    if (decrypt) hit = bad && ok[i] != 0;
+    if (bad) {
+        ok[i] = 0;
+        const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        for (uint32_t k = 0; k < row; ++k) store_fr(out + (i * row + k) * 32, zero);
+    } else if (!decrypt) {
+        ok[i] = 1;
+    }
+    if (count) warp_count(count, hit);
+}
+
+cudaError_t launch_dhke(const void* secret, bool secret_bcast, const void* pub, bool pub_bcast, size_t n, void* shared_uv,
+                        uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_dhke<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(secret), secret_bcast, static_cast<const uint8_t*>(pub),
+                                             pub_bcast, n, static_cast<uint8_t*>(shared_uv), ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_dhke_fix(bool decrypt, const uint8_t* valid, size_t n, void* out, uint32_t row, uint8_t* ok,
+                            unsigned long long* count, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_dhke_fix<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(decrypt, valid, n, static_cast<uint8_t*>(out), row, ok, count);
     return cudaGetLastError();
 }
 

@@ -122,6 +122,16 @@ cudaError_t launch_crypt_varlen_keys(bool decrypt, const uint64_t* offsets, uint
 cudaError_t launch_crypt_varlen(bool decrypt, const void* tags, const void* src, uint64_t base, const uint64_t* offsets,
                                 const uint32_t* lens, const uint32_t* perm, uint32_t n, const void* secret_uv, const void* nonce,
                                 void* dst, uint8_t* ok, unsigned long long* n_failed, size_t coop_max, cudaStream_t st);
+// JubJub key exchange (p252_dhke_batch): shared_uv[i] = [secret[i]] pub[i] as (u, v), one thread per item; *_bcast: the
+// operand is one item read by all.  ok[i] = item valid (secret < r_J, u, v < p, on the curve); an invalid item writes
+// (0, 0) and is counted into *n_invalid (device pointer, may be null)
+cudaError_t launch_dhke(const void* secret, bool secret_bcast, const void* pub, bool pub_bcast, size_t n, void* shared_uv,
+                        uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st);
+// after a fused encrypt / decrypt: items with valid[i] == 0 get ok[i] = 0 and a zeroed row of `row` scalars of out (encrypt
+// also sets ok[i] = 1 for the valid ones); count (device, may be null) += invalid items (encrypt) or invalid items
+// launch_decrypt had not already counted as failures (decrypt)
+cudaError_t launch_dhke_fix(bool decrypt, const uint8_t* valid, size_t n, void* out, uint32_t row, uint8_t* ok,
+                            unsigned long long* count, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -4,8 +4,9 @@ The shared secret is the (u, v) coordinate pair of the JubJubAffine point
 import numpy as np
 
 from .engine import default_engine, varlen_out_offsets
-from .errors import DecryptionFailed, EncryptionFailed, Error
+from .errors import DecryptionFailed, EncryptionFailed, Error, InvalidPoint
 from .hash import pack_varlen
+from .scalar import jubjub_limbs
 
 
 def encrypt(message, shared_secret, nonce, engine=None):
@@ -46,6 +47,43 @@ def decrypt_batch(ciphers, secrets_uv, nonces, engine=None, async_=False):
     items for which the reference returns Error::DecryptionFailed (their message is zeroed)."""
     eng = engine or default_engine(ciphers.device.index if hasattr(ciphers, "is_cuda") else 0)
     return eng.decrypt_batch(ciphers, secrets_uv, nonces, async_=async_)
+
+
+def dhke(secret, public, engine=None):
+    """dhke(secret, public) = [secret] public, the shared secret encrypt / decrypt take (src/encryption.rs:11-43).
+    secret: a canonical int < r_J or one p252_jscalar row (4,) uint64; public: the point's (u, v) as a (2, 4) array of
+    BlsScalar.0 limbs -> (2, 4) uint64.  Raises InvalidPoint for a secret >= r_J or a point off the curve."""
+    if isinstance(secret, (int, np.integer)):
+        sec = jubjub_limbs([secret])
+    else:
+        sec = np.ascontiguousarray(secret, dtype=np.uint64).reshape(1, 4)
+    pub = np.ascontiguousarray(public, dtype=np.uint64).reshape(1, 2, 4)
+    eng = engine or default_engine()
+    shared, ok = eng.dhke_batch(sec, pub)
+    if not ok[0]:
+        raise InvalidPoint()
+    return shared[0]
+
+
+def dhke_batch(secrets, publics, engine=None, out=None, async_=False):
+    """NEW: n x dhke(secret, public).  secrets (1 or n, 4) p252_jscalar rows (scalar.jubjub_limbs), publics (1 or n, 2, 4)
+    -> (shared (n, 2, 4), ok (n,) uint8); ok == 0 marks an invalid item, whose output is (0, 0)."""
+    eng = engine or default_engine(publics.device.index if hasattr(publics, "is_cuda") else 0)
+    return eng.dhke_batch(secrets, publics, out=out, async_=async_)
+
+
+def encrypt_batch_dhke(messages, secrets, publics, nonces, engine=None, out=None, async_=False):
+    """NEW: n x encrypt(messages[i], dhke(secret, public), nonces[i]), the shared secret derived on the device
+    -> (ciphers (n, L+1, 4), ok (n,) uint8)."""
+    eng = engine or default_engine(messages.device.index if hasattr(messages, "is_cuda") else 0)
+    return eng.encrypt_batch_dhke(messages, secrets, publics, nonces, out=out, async_=async_)
+
+
+def decrypt_batch_dhke(ciphers, secrets, publics, nonces, engine=None, out=None, async_=False):
+    """NEW: n x decrypt(ciphers[i], dhke(secret, public), nonces[i]) -> (messages (n, L, 4), ok (n,) uint8); ok == 0 for
+    an authentication failure or an invalid key-exchange item (message zeroed).  A wallet scan passes one view key."""
+    eng = engine or default_engine(ciphers.device.index if hasattr(ciphers, "is_cuda") else 0)
+    return eng.decrypt_batch_dhke(ciphers, secrets, publics, nonces, out=out, async_=async_)
 
 
 def cipher_offsets(offsets):

@@ -317,6 +317,93 @@ class Engine:
         device buffers; after an async_ call, sync() first)."""
         return int(getattr(self, "_nfail", ctypes.c_size_t(0)).value)
 
+    # -- JubJub key exchange ----------------------------------------------------------------------
+    def _dhke_args(self, secrets, publics, n=None):
+        """Shared validation of the dhke calls -> (secret ptr, n_secret, public ptr, n_public, n, flags, keepalives).
+        secrets (n_secret, 4) p252_jscalar rows (scalar.jubjub_limbs), publics (n_public, 2, 4); each leading dimension
+        is 1 (broadcast) or n.  n: the batch size the other buffers fix, or None to take it from these two."""
+        sp, sl, fs, sk = self._in(secrets, (4,))
+        pp, pl, fp, pk = self._in(publics, (2, 4))
+        if fs != fp:
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        if len(sl) != 1 or len(pl) != 1:
+            raise EngineError(-1, "secrets must have shape (n_secret, 4) and publics (n_public, 2, 4)")
+        ns, npub = int(sl[0]), int(pl[0])
+        if n is None:
+            n = npub if ns == 1 else ns
+        for name, k in (("secrets", ns), ("publics", npub)):
+            if k not in (1, n):
+                raise EngineError(-1, "%s must have 1 or %d rows, got %d" % (name, n, k))
+        return sp, ns, pp, npub, n, fs, (sk, pk)
+
+    def dhke_batch(self, secrets, publics, out=None, async_=False):
+        """n x dhke(secret, public) = [secret] public as (u, v): secrets (n_secret, 4) canonical p252_jscalar rows,
+        publics (n_public, 2, 4); n_secret and n_public are each 1 or n -> (shared (n, 2, 4), ok (n,) uint8).  ok[i] == 0
+        marks an invalid item (secret >= r_J, or the point not on the curve with u, v < p); its output is (0, 0) and it is
+        counted in last_dhke_invalid()."""
+        sp, ns, pp, npub, n, flags, keep = self._dhke_args(secrets, publics)
+        like = keep[1]
+        res = self._out_like(like, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), like)
+        if _is_torch(like):
+            import torch
+            ok = torch.empty((n,), dtype=torch.uint8, device=like.device)
+        else:
+            ok = np.empty((n,), dtype=np.uint8)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._ninv = self._counter(flags)
+        self._check(self._lib.p252_dhke_batch(self._ctx, sp, ns, pp, npub, n, self._ptr(res), self._ptr(ok),
+                                              ctypes.byref(self._ninv), flags))
+        return res, ok
+
+    def last_dhke_invalid(self):
+        """Invalid items of the last dhke_batch or encrypt_batch_dhke (sync() first after async_)."""
+        return int(getattr(self, "_ninv", ctypes.c_size_t(0)).value)
+
+    def _crypt_dhke(self, decrypt, data, secrets, publics, nonces, out, async_):
+        L = int(data.shape[1]) - (1 if decrypt else 0)
+        if L < 1:
+            raise EngineError(-1, "ciphers must hold at least one message scalar plus the authentication scalar" if decrypt
+                              else "messages must hold at least one scalar")
+        dp, lead, flags, dk = self._in(data, (int(data.shape[1]), 4))
+        if len(lead) != 1:
+            raise EngineError(-1, "expected shape (n, %s, 4)" % ("L + 1" if decrypt else "L"))
+        n = lead[0]
+        sp, ns, pp, npub, _, f2, keep = self._dhke_args(secrets, publics, n)
+        np_, l3, f3, nk = self._in(nonces, (4,))
+        if not (flags == f2 == f3):
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("nonces", l3, n)
+        shape = (n, L if decrypt else L + 1, 4)
+        res = self._out_like(dk, shape) if out is None else self._check_out(out, shape, dk)
+        if _is_torch(dk):
+            import torch
+            ok = torch.empty((n,), dtype=torch.uint8, device=dk.device)
+        else:
+            ok = np.empty((n,), dtype=np.uint8)
+        flags |= _native.ASYNC if async_ and flags else 0
+        cnt = self._counter(flags)
+        if decrypt:
+            self._nfail = cnt
+            fn = self._lib.p252_decrypt_batch_dhke
+        else:
+            self._ninv = cnt
+            fn = self._lib.p252_encrypt_batch_dhke
+        self._check(fn(self._ctx, dp, n, L, sp, ns, pp, npub, np_, self._ptr(res), self._ptr(ok), ctypes.byref(cnt), flags))
+        return res, ok
+
+    def encrypt_batch_dhke(self, messages, secrets, publics, nonces, out=None, async_=False):
+        """n x encrypt(messages[i], dhke(secret, public), nonces[i]) with the shared secret derived on the device and never
+        returned: messages (n, L, 4), secrets (1 or n, 4) p252_jscalar rows, publics (1 or n, 2, 4), nonces (n, 4) ->
+        (ciphers (n, L+1, 4), ok (n,) uint8).  An invalid key-exchange item has ok == 0 and a zeroed cipher row (count:
+        last_dhke_invalid())."""
+        return self._crypt_dhke(False, messages, secrets, publics, nonces, out, async_)
+
+    def decrypt_batch_dhke(self, ciphers, secrets, publics, nonces, out=None, async_=False):
+        """n x decrypt(ciphers[i], dhke(secret, public), nonces[i]) -> (messages (n, L, 4), ok (n,) uint8).  ok == 0 for an
+        authentication failure or an invalid key-exchange item (message zeroed); their count: last_decrypt_failures().
+        The wallet-scan shape is one view key (secrets of 1 row) against every note's public key."""
+        return self._crypt_dhke(True, ciphers, secrets, publics, nonces, out, async_)
+
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
         max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries

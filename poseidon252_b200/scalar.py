@@ -51,3 +51,17 @@ def random_limbs_fast(rng, shape):
         rng.integers(0, 2, size=shape + (4,), dtype=np.uint64)
     a[..., 3] %= np.uint64(0x73EDA753299D7D48)
     return a
+
+
+def jubjub_limbs(values):
+    """canonical integers -> (n, 4) uint64 rows of p252_jscalar: the little-endian u64 limbs of each value, i.e. the 32
+    bytes of JubJubScalar::to_bytes().  NOT a Montgomery image; values >= r_J are passed through (the device marks such an
+    item invalid)."""
+    vals = [int(v) for v in values]
+    out = np.empty((len(vals), 4), dtype=np.uint64)
+    for i, v in enumerate(vals):
+        if not 0 <= v < 1 << 256:
+            raise ValueError("a JubJub scalar must be in [0, 2^256), got %d" % v)
+        for k in range(4):
+            out[i, k] = (v >> (64 * k)) & _M64
+    return out
