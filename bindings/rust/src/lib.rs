@@ -120,6 +120,10 @@ pub use ctree::{p252_ctree, CompactTree};
 // dhke.rs (methods on Engine).
 mod dhke;
 
+// Fixed-base scalar multiplication ([s] G for public and ephemeral keys) and the sender's encrypt batch: their own
+// `extern "C"` block in fixed_base.rs (methods on Engine).
+mod fixed_base;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

@@ -288,6 +288,32 @@ int p252_decrypt_batch_dhke(p252_ctx* ctx, const p252_fr* cipher, size_t n, size
                             size_t n_secret, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* msg,
                             uint8_t* ok, size_t* n_failed, int flags);
 
+/* ---- Fixed-base JubJub scalar multiplication and the sender's encrypt batch ----------------------------------------
+ * [secret] base for ONE base shared by the batch: a public key GENERATOR_EXTENDED * secret, or a note's ephemeral key
+ * R = GENERATOR_EXTENDED * r (src/encryption.rs:22-42).  There is no built-in generator: the caller passes the base, e.g.
+ * dusk_jubjub::GENERATOR's (u, v).  base_uv is a HOST pointer to (u, v) (two p252_fr) for every memory space; any point on
+ * the curve is a valid base, small-order points included.  A base with a coordinate >= p or off the curve is refused
+ * with P252_ERR_INVALID_POINT before anything runs, for every memory space and for n == 0.  The context keeps the table
+ * of its last base (48 KB of device memory, built on the device on the first call with that base, then reused).
+ * Secrets and points are laid out as for p252_dhke_batch.  Item validity: secret / r < r_J and, in the fused call,
+ * public_uv a curve point with u, v < p.  An invalid item gets ok[i] = 0, a zeroed output (and, in the fused call, a
+ * zeroed cipher row and R row) and is counted once into *n_invalid (optional HOST pointer, lifetime as for
+ * p252_decrypt_batch); the call returns P252_OK.
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_public not 1 or n, DEVICE buffers other than ok not
+ * 16-byte aligned -> INVALID_ARGUMENT; L == 0 -> INVALID_IO_PATTERN.
+ * p252_encrypt_batch_ephemeral derives the shared secret dhke(r[i], public_uv[...]) on the device, with the kernels of
+ * p252_encrypt_batch_dhke, and never returns it: like that call it is synchronous for both memory spaces.  HOST calls
+ * stage secrets, points, nonces and plaintext through the context's zeroed staging arenas.  Each item is constant time
+ * (no branch and no address depends on secret bits); see DESIGN.md section 4. */
+/* out_uv[i] = [secret[i]] base (JubJubAffine), n items; base_uv is a HOST pointer to (u, v). */
+int p252_fixed_base_batch(p252_ctx* ctx, const p252_fr* base_uv, const p252_jscalar* secret, size_t n, p252_fr* out_uv,
+                          uint8_t* ok, size_t* n_invalid, int flags);
+/* The reference's sender (src/encryption.rs:22-42) as a batch: R_uv[i] = [r[i]] base,
+ * cipher[i] = encrypt(msg[i], dhke(r[i], public_uv[n_public == 1 ? 0 : i]), nonce[i]); msg n x L, cipher n x (L + 1). */
+int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* r,
+                                 const p252_fr* base_uv, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce,
+                                 p252_fr* cipher, p252_fr* R_uv, uint8_t* ok, size_t* n_invalid, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

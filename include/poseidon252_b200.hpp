@@ -9,7 +9,7 @@
 //   dusk_poseidon::Error                     (src/error.rs:11-32)      -> p252::Error (exception)
 //   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
 //   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
-//   decrypt_batch_dhke, merkle4_build.
+//   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -307,6 +307,41 @@ inline std::vector<Scalar> decrypt_batch_dhke(const Scalar* cipher, size_t n, si
                                   nullptr, P252_MEM_HOST),
           e.get());
     return msg;
+}
+
+// NEW: fixed-base scalar multiplication (p252_fixed_base_batch) and the sender's encrypt batch
+// (p252_encrypt_batch_ephemeral).  base_uv is the caller's base point (u, v), e.g. dusk_jubjub::GENERATOR's; there is no
+// built-in generator.  A base off the curve throws Error(P252_ERR_INVALID_POINT); ok[i] == 0 marks an invalid item (secret
+// >= r_J, or in the fused call a public key off the curve) with zeroed output rows.
+// returns n x 2 scalars: (u, v) of [secrets[i]] base
+inline std::vector<Scalar> fixed_base_batch(const JubJubScalar* secrets, size_t n, const Scalar (&base_uv)[2],
+                                            std::vector<uint8_t>& ok, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> out(2 * n);
+    ok.assign(n, 0);
+    check(p252_fixed_base_batch(e.get(), base_uv, secrets, n, out.data(), ok.data(), nullptr, P252_MEM_HOST), e.get());
+    return out;
+}
+// [secret] base for one item, e.g. a public key; throws Error(P252_ERR_INVALID_POINT) for a secret >= r_J
+inline void fixed_base(const JubJubScalar& secret, const Scalar (&base_uv)[2], Scalar (&out_uv)[2],
+                       Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok;
+    const auto r = fixed_base_batch(&secret, 1, base_uv, ok, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    out_uv[0] = r[0];
+    out_uv[1] = r[1];
+}
+// msg n x L -> cipher n x (L+1); R receives n x 2 scalars, the ephemeral keys [r_i] base
+inline std::vector<Scalar> encrypt_batch_ephemeral(const Scalar* msg, size_t n, size_t L, const JubJubScalar* r,
+                                                   const Scalar (&base_uv)[2], const Scalar* publics_uv, size_t n_public,
+                                                   const Scalar* nonces, std::vector<Scalar>& R, std::vector<uint8_t>& ok,
+                                                   Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> cipher(n * (L + 1));
+    R.assign(2 * n, Scalar{});
+    ok.assign(n, 0);
+    check(p252_encrypt_batch_ephemeral(e.get(), msg, n, L, r, base_uv, publics_uv, n_public, nonces, cipher.data(), R.data(),
+                                       ok.data(), nullptr, P252_MEM_HOST),
+          e.get());
+    return cipher;
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

@@ -9,6 +9,7 @@
 //   Hash / Domain / io_pattern      src/hash.rs:21-155      -> p252_hash_tag, p252_hash_batch
 //   encrypt / decrypt               src/encryption.rs:62-95 -> p252_encrypt_batch, p252_decrypt_batch
 //   dhke + encrypt / decrypt        src/encryption.rs:11-43 -> p252_dhke_batch, p252_{en,de}crypt_batch_dhke
+//   GENERATOR * r, the sender       src/encryption.rs:22-42 -> p252_fixed_base_batch, p252_encrypt_batch_ephemeral
 //   Error                           src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -63,6 +64,13 @@ struct TagTable {
     cudaEvent_t ev = nullptr;
 };
 
+// The device table of p252_fixed_base_batch / p252_encrypt_batch_ephemeral for ONE base, keyed by the base's 64 bytes:
+// reused while calls pass that base, rebuilt on the device for another (base_table(), below).
+struct BaseTable {
+    void* dev = nullptr;
+    p252_fr key[2] = {};
+};
+
 }  // namespace
 
 struct p252_ctx {
@@ -85,6 +93,7 @@ struct p252_ctx {
     // per-length tag tables: p252_hash_batch_varlen (key = domain and out_len) and p252_{en,de}crypt_batch_varlen; two
     // instances, so that alternating digest and encryption calls rebuild neither
     TagTable vt, ct;
+    BaseTable bt;   // fixed-base JubJub table
     // test hook: index of the staged chunk that fails in the next host-buffer call (-1 = none)
     long long fail_chunk = -1;
     // multi-GPU
@@ -526,6 +535,7 @@ void p252_destroy(p252_ctx* ctx) {
             if (ev) cudaEventDestroy(ev);
     for (TagTable* t : {&ctx->vt, &ctx->ct})
         if (t->dev) cudaFreeAsync(t->dev, ctx->stream);
+    if (ctx->bt.dev) cudaFreeAsync(ctx->bt.dev, ctx->stream);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);   // pending host functions reference h_counter
     for (TagTable* t : {&ctx->vt, &ctx->ct}) {
         if (t->host) cudaFreeHost(t->host);
@@ -919,6 +929,117 @@ int p252_decrypt_batch_dhke(p252_ctx* ctx, const p252_fr* cipher, size_t n, size
                             size_t n_secret, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* msg,
                             uint8_t* ok, size_t* n_failed, int flags) {
     return crypt_dhke(ctx, true, cipher, n, L, secret, n_secret, public_uv, n_public, nonce, msg, ok, n_failed, flags);
+}
+
+// ---- fixed-base JubJub scalar multiplication and the sender's encrypt batch ------------------------------------------
+// The base is public and arrives as a HOST pointer for every memory space: checked here before anything runs.
+static int base_check(const p252_fr* base_uv) {
+    return p252::host::jubjub_on_curve(base_uv[0].l, base_uv[1].l) ? P252_OK : P252_ERR_INVALID_POINT;
+}
+
+// The device table of base_uv: the cached one when the base is the same 64 bytes, otherwise built on the context stream
+// (k_fixed_base_table) into a new stream-ordered allocation.  The replaced table is freed in stream order, after every
+// kernel already enqueued that reads it (DEVICE calls run on the context stream, HOST and fused calls join back into it),
+// so P252_ASYNC calls with different bases may follow each other.
+static int base_table(p252_ctx* ctx, const p252_fr* base_uv, const void** table) {
+    BaseTable& t = ctx->bt;
+    if (t.dev && memcmp(t.key, base_uv, sizeof t.key) == 0) {
+        *table = t.dev;
+        return P252_OK;
+    }
+    void* d = nullptr;
+    CU(cudaMallocAsync(&d, p252::kFixedBaseTableBytes, ctx->stream));
+    uint64_t b[8];
+    memcpy(b, base_uv, sizeof b);
+    const int rc = launched(ctx, p252::launch_fixed_base_table(b, d, ctx->stream));
+    if (rc != P252_OK) {
+        cudaFreeAsync(d, ctx->stream);
+        return rc;
+    }
+    void* old = t.dev;
+    t.dev = d;
+    memcpy(t.key, base_uv, sizeof t.key);
+    *table = d;
+    if (old) CU(cudaFreeAsync(old, ctx->stream));
+    return P252_OK;
+}
+
+int p252_fixed_base_batch(p252_ctx* ctx, const p252_fr* base_uv, const p252_jscalar* secret, size_t n, p252_fr* out_uv,
+                          uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
+    if (n && (!secret || !out_uv || !ok)) return P252_ERR_INVALID_ARGUMENT;
+    if ((flags & P252_MEM_DEVICE) && (!aligned16(secret) || !aligned16(out_uv))) return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(base_uv);
+    if (rc != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    if (flags & P252_MEM_DEVICE) {
+        if (n_invalid && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        rc = launched(ctx, p252::launch_fixed_base(secret, n, table, out_uv, ok, n_invalid ? ctx->d_counter : nullptr,
+                                                   ctx->stream));
+        if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+        return device_done(ctx, rc, flags);
+    }
+    std::vector<Io> ios = {{secret, nullptr, 32}, {nullptr, out_uv, 64}, {nullptr, ok, 1}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return p252::launch_fixed_base(d[0], cnt, table, d[1], static_cast<uint8_t*>(d[2]), nullptr, st);
+    }, /*wipe=*/true);
+    if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+    return rc;
+}
+
+// The sender: launch_fixed_base (R), launch_dhke into a slot arena (the shared secrets), the unchanged launch_encrypt,
+// then launch_dhke_fix on the cipher rows and again on the R rows, so that an item with an invalid r or public key has
+// ok = 0 and both rows zeroed.  As in crypt_dhke the shared secrets live only in the slot arenas, for both memory spaces,
+// and the common exit join_slots(wipe) clears them on every path.
+int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* r,
+                                 const p252_fr* base_uv, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce,
+                                 p252_fr* cipher, p252_fr* R_uv, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, r, n, public_uv, n_public, {msg, nonce, cipher, R_uv}, ok, flags);
+    if (rc != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = p252_encryption_tag(L, &tag)) != P252_OK) return rc;
+    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const uint32_t l32 = (uint32_t)L;
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    unsigned long long* counter = nullptr;
+    if (dev && n_invalid) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    // 0 message, 1 r, 2 public, 3 nonce, 4 cipher, 5 R, 6 ok; 7 shared secrets and 8 validity live in the arena only
+    std::vector<Io> ios = {{msg, nullptr, L * 32, false, dev}, {r, nullptr, 32, false, dev}, {public_uv, nullptr, 64, pb, dev},
+                           {nonce, nullptr, 32, false, dev}, {nullptr, cipher, (size_t)(l32 + 1) * 32, false, dev},
+                           {nullptr, R_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64},
+                           {nullptr, nullptr, 1}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[6]);
+        uint8_t* valid = static_cast<uint8_t*>(d[8]);
+        cudaError_t e = p252::launch_fixed_base(d[1], cnt, table, d[5], okc, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_dhke(d[1], false, d[2], pb, cnt, d[7], valid, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[7], d[3], d[4], st);
+        if (e == cudaSuccess) e = p252::launch_dhke_fix(false, valid, cnt, d[4], l32 + 1, okc, counter, st);
+        if (e == cudaSuccess) e = p252::launch_dhke_fix(false, valid, cnt, d[5], 2, okc, nullptr, st);
+        if (e == cudaSuccess) ctx->launches += 4;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    }, /*wipe=*/true);
+    if (!dev) {
+        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+        return rc;
+    }
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+    return device_done(ctx, rc, flags);
 }
 
 // ---- arity-4 Merkle tree ------------------------------------------------------------------------------

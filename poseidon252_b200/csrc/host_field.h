@@ -173,6 +173,50 @@ inline void add_mod(uint64_t r[4], const uint64_t a[4], const uint64_t b[4]) {
     memcpy(r, t, sizeof t);
 }
 
+// r = a - b mod p for a, b < p
+inline void sub_mod(uint64_t r[4], const uint64_t a[4], const uint64_t b[4]) {
+    u128 bw = 0;
+    uint64_t t[4];
+    for (int i = 0; i < 4; ++i) {
+        u128 d = (u128)a[i] - b[i] - (uint64_t)bw;
+        t[i] = (uint64_t)d;
+        bw = (d >> 64) & 1;
+    }
+    if (bw) {
+        u128 c = 0;
+        for (int i = 0; i < 4; ++i) {
+            c += (u128)t[i] + kMod[i];
+            t[i] = (uint64_t)c;
+            c >>= 64;
+        }
+    }
+    memcpy(r, t, sizeof t);
+}
+
+// a < p
+inline bool is_canonical(const uint64_t a[4]) {
+    u128 bw = 0;
+    for (int i = 0; i < 4; ++i) bw = (((u128)a[i] - kMod[i] - (uint64_t)bw) >> 64) & 1;
+    return bw != 0;
+}
+
+// (u, v) (Montgomery limbs) is a JubJub point: u, v < p and -u^2 + v^2 == 1 + d u^2 v^2, d = -10240/10241
+inline bool jubjub_on_curve(const uint64_t u[4], const uint64_t v[4]) {
+    static const uint64_t kOne[4] = {0x00000001fffffffeULL, 0x5884b7fa00034802ULL, 0x998c4fefecbc4ff5ULL,
+                                     0x1824b159acc5056fULL};
+    static const uint64_t kD[4] = {0x2a522455b974f6b0ULL, 0xfc6cc9ef0d9acab3ULL, 0x7a08fb94c27628d1ULL,
+                                   0x57f8f6a8fe0e262eULL};
+    if (!is_canonical(u) || !is_canonical(v)) return false;
+    uint64_t uu[4], vv[4], lhs[4], w[4], rhs[4];
+    mont_mul(uu, u, u);
+    mont_mul(vv, v, v);
+    sub_mod(lhs, vv, uu);
+    mont_mul(w, uu, vv);
+    mont_mul(rhs, w, kD);
+    add_mod(rhs, rhs, kOne);
+    return memcmp(lhs, rhs, sizeof lhs) == 0;
+}
+
 // BlsScalar::from_bytes_wide: 64 LE bytes -> (lo + hi*2^256) mod p, Montgomery form
 inline void from_bytes_wide(uint64_t r[4], const uint8_t b[64]) {
     uint64_t lo[4], hi[4], a[4], c[4];

@@ -268,5 +268,156 @@ __device__ __forceinline__ void scalar_mul(uint32_t (&ou)[8], uint32_t (&ov)[8],
     fmul(ov, acc.Y, zi);
 }
 
+// ---- fixed base: [s] B for one public base B shared by a batch (p252_fixed_base_batch) -------------------------------
+// s < 2^252 is recoded into 64 signed digits e_w in [-8, 8), s = sum e_w 16^w, so [s] B = sum_w [e_w] (16^w B): one
+// mixed addition per window from a precomputed table, no doublings.  The table holds, for w = 0..63 and j = 1..8, the
+// affine point j 16^w B in "Niels" form (v - u, v + u, 2d u v), 6 x 16 bytes per entry, 48 KB in all; the digit's sign is
+// applied by the negation -(u, v) = (-u, v), i.e. swap the first two coordinates and negate the third.
+constexpr int kFbWindows = 64, kFbEntries = 8, kFbEntryWords = 6;   // uint4 per entry
+constexpr int kFbTableWords = kFbWindows * kFbEntries * kFbEntryWords;
+// Products per item: 63 mixed additions with T3 x 7, the last without x 6, the inversion, the affine conversion 2.
+constexpr int kProductsPerFixedBase = (kFbWindows - 1) * 7 + 6 + (kPm2Bits - 1) + (kPm2Ones - 1) + 2;
+static_assert(kProductsPerFixedBase == 866, "product count of DESIGN.md section 4");
+
+struct Niels {                  // an affine addend (v - u, v + u, 2d u v), every coordinate < p
+    uint32_t ymx[8], ypx[8], kt[8];
+};
+
+// r = p + q for an affine q (Z2 = 1): add() with D = 2 Z1 instead of a product, 7 products, 6 without T3
+template <bool kWantT>
+__device__ __forceinline__ void madd(Ext& r, const Ext& p, const Niels& q) {
+    uint32_t a[8], b[8], c[8], d[8], e[8], f[8], g[8], h[8];
+    fr_sub_mod(e, p.Y, p.X);
+    fmul(a, e, q.ymx);          // A = (Y1 - X1)(v2 - u2)
+    fr_add_mod(e, p.Y, p.X);
+    fmul(b, e, q.ypx);          // B = (Y1 + X1)(v2 + u2)
+    fmul(c, p.T, q.kt);         // C = T1 2d u2 v2
+    fr_add_mod(d, p.Z, p.Z);    // D = 2 Z1
+    fr_sub_mod(e, b, a);
+    fr_sub_mod(f, d, c);
+    fr_add_mod(g, d, c);
+    fr_add_mod(h, b, a);
+    fmul(r.X, e, f);
+    fmul(r.Y, g, h);
+    fmul(r.Z, f, g);
+    if (kWantT) fmul(r.T, e, h);
+}
+
+// Signed 4-bit recoding, least significant window first: the low nibble of s plus the carry, in [0, 16] -> a digit in
+// [-8, 8) and the next carry; s is shifted down by 4 (consumed).  Arithmetic only, no indexing by the window.  The last
+// window (bits 252..255, zero for s < 2^252) takes the final carry, a digit in {0, 1}.
+__device__ __forceinline__ int32_t recode_digit(uint32_t (&s)[8], uint32_t& carry) {
+    const uint32_t x = (s[0] & 15u) + carry;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) s[k] = __funnelshift_r(s[k], s[k + 1], 4);
+    s[7] >>= 4;
+    carry = (x + 8u) >> 4;
+    return (int32_t)x - (int32_t)(carry << 4);
+}
+
+// q = sign(e) (|e| 16^w B) from window w of the table: every entry of the window is read, at addresses fixed by w and the
+// entry counter, and masked in (|e| = 0 selects the identity (1, 1, 0)); the sign is a masked swap and negation.
+template <bool kLdg>
+__device__ __forceinline__ void select_niels(Niels& q, const uint4* tab, int w, int32_t e) {
+    const uint32_t neg = (uint32_t)e >> 31;
+    const uint32_t mag = (uint32_t)((e ^ -(int32_t)neg) + (int32_t)neg);
+    uint32_t acc[24], one[8];
+    set_one(one);
+    const uint32_t m0 = 0u - (uint32_t)(mag == 0);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc[k] = one[k] & m0, acc[8 + k] = one[k] & m0, acc[16 + k] = 0;
+    const uint4* win = tab + w * (kFbEntries * kFbEntryWords);
+#pragma unroll 1
+    for (int j = 0; j < kFbEntries; ++j) {          // j is the public loop counter: the same 8 entries for every digit
+        const uint32_t m = 0u - (uint32_t)(mag == (uint32_t)(j + 1));
+#pragma unroll
+        for (int q4 = 0; q4 < kFbEntryWords; ++q4) {
+            const uint4 x = kLdg ? __ldg(win + j * kFbEntryWords + q4) : win[j * kFbEntryWords + q4];
+            acc[4 * q4 + 0] |= x.x & m;
+            acc[4 * q4 + 1] |= x.y & m;
+            acc[4 * q4 + 2] |= x.z & m;
+            acc[4 * q4 + 3] |= x.w & m;
+        }
+    }
+    const uint32_t mn = 0u - neg;
+    uint32_t nk[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint32_t t = (acc[k] ^ acc[8 + k]) & mn;
+        q.ymx[k] = acc[k] ^ t;
+        q.ypx[k] = acc[8 + k] ^ t;
+        q.kt[k] = acc[16 + k];
+    }
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    fr_sub_mod(nk, zero, q.kt);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) q.kt[k] = (q.kt[k] & ~mn) | (nk[k] & mn);
+}
+
+// (ou, ov) = [s] B for s < 2^252 (canonical words) and the table of B (kFbTableWords uint4, built by fixed_base_entry).
+// kLdg: read the table through the read-only data path (a global table); otherwise plain loads (e.g. shared memory).
+template <bool kLdg>
+__device__ __forceinline__ void fixed_base_mul(uint32_t (&ou)[8], uint32_t (&ov)[8], const uint32_t (&s)[8],
+                                               const uint4* tab) {
+    Ext acc;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc.X[k] = 0, acc.T[k] = 0;
+    set_one(acc.Y);
+    set_one(acc.Z);
+    uint32_t d[8], carry = 0;
+    fcopy(d, s);
+    Niels q;
+    Ext t;
+#pragma unroll 1
+    for (int w = 0; w < kFbWindows - 1; ++w) {
+        select_niels<kLdg>(q, tab, w, recode_digit(d, carry));
+        madd<true>(t, acc, q);
+        acc = t;
+    }
+    select_niels<kLdg>(q, tab, kFbWindows - 1, recode_digit(d, carry));
+    madd<false>(t, acc, q);
+    uint32_t zi[8];
+    inverse(zi, t.Z);
+    fmul(ou, t.X, zi);
+    fmul(ov, t.Y, zi);
+}
+
+// Table entry (w, j), j in 1..8, of the base (u, v) (on the curve, u, v < p): j 16^w (u, v) by 4w doublings and j - 1
+// additions, then affine and Niels form.  The base is public, so these loops branch on w and j.
+__device__ __forceinline__ void fixed_base_entry(uint4* out, const uint32_t (&u)[8], const uint32_t (&v)[8], int w, int j) {
+    Ext p, t;
+    fcopy(p.X, u);
+    fcopy(p.Y, v);
+    set_one(p.Z);
+    fmul(p.T, u, v);
+    for (int i = 0; i < 4 * w; ++i) {
+        dbl<true>(t, p);
+        p = t;
+    }
+    Cached c;
+    to_cached(c, p);
+    Ext q = p;
+    for (int i = 1; i < j; ++i) {
+        add<true>(t, q, c);
+        q = t;
+    }
+    uint32_t zi[8], au[8], av[8], uv[8], k[8];
+    inverse(zi, q.Z);
+    fmul(au, q.X, zi);
+    fmul(av, q.Y, zi);
+    Niels n;
+    fr_sub_mod(n.ymx, av, au);
+    fr_add_mod(n.ypx, av, au);
+    fmul(uv, au, av);
+    set_2d(k);
+    fmul(n.kt, uv, k);
+    const uint32_t* src[3] = {n.ymx, n.ypx, n.kt};
+#pragma unroll
+    for (int q3 = 0; q3 < 3; ++q3) {
+        out[2 * q3] = make_uint4(src[q3][0], src[q3][1], src[q3][2], src[q3][3]);
+        out[2 * q3 + 1] = make_uint4(src[q3][4], src[q3][5], src[q3][6], src[q3][7]);
+    }
+}
+
 }  // namespace jj
 }  // namespace p252

@@ -1513,6 +1513,61 @@ cudaError_t launch_dhke_fix(bool decrypt, const uint8_t* valid, size_t n, void* 
     return cudaGetLastError();
 }
 
+// ---- fixed-base JubJub scalar multiplication (out = [s] B for one base B of the whole batch) -------------------------
+static_assert(kFixedBaseTableBytes == jj::kFbTableWords * sizeof(uint4), "fixed-base table size of kernels.h");
+struct FixedBase {               // the base (u, v), Montgomery, passed by value: the table build reads no host memory
+    uint32_t uv[16];
+};
+
+// One thread per table entry (w, j): 512 threads, entry e = 8 w + j - 1 at table + 6 e (jubjub_device.cuh).
+__global__ void __launch_bounds__(128) k_fixed_base_table(FixedBase b, uint4* __restrict__ table) {
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= jj::kFbWindows * jj::kFbEntries) return;
+    uint32_t u[8], v[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] = b.uv[k], v[k] = b.uv[8 + k];
+    jj::fixed_base_entry(table + e * jj::kFbEntryWords, u, v, e / jj::kFbEntries, e % jj::kFbEntries + 1);
+}
+
+// One thread per item, 866 products.  Item i reads secret[i] (canonical 4 x u64); valid iff s < r_J.  An invalid item runs
+// the same schedule on s = 0 and writes (0, 0), ok = 0.  Every lane of a warp reads the same table address at the same
+// time (the window and entry counters are public), so the read-only path serves each load as one broadcast.
+__global__ void __launch_bounds__(kThreads, 3) k_fixed_base(const uint8_t* __restrict__ secret, size_t n,
+                                                         const uint4* __restrict__ table, uint8_t* __restrict__ out,
+                                                         uint8_t* __restrict__ ok, unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t s[8];
+    load_fr(s, secret + i * 32);
+    const bool valid = jj::below_order(s);
+    const uint32_t m = 0u - (uint32_t)valid;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s[k] &= m;
+    uint32_t ou[8], ov[8];
+    jj::fixed_base_mul<true>(ou, ov, s, table);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m;
+    store_fr(out + i * 64, ou);
+    store_fr(out + i * 64 + 32, ov);
+    ok[i] = valid ? 1 : 0;
+    if (n_invalid) warp_count(n_invalid, !valid);
+}
+
+cudaError_t launch_fixed_base_table(const uint64_t base_uv[8], void* table, cudaStream_t st) {
+    FixedBase b;
+    for (int k = 0; k < 8; ++k) b.uv[2 * k] = (uint32_t)base_uv[k], b.uv[2 * k + 1] = (uint32_t)(base_uv[k] >> 32);
+    k_fixed_base_table<<<jj::kFbWindows * jj::kFbEntries / 128, 128, 0, st>>>(b, static_cast<uint4*>(table));
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fixed_base(const void* secret, size_t n, const void* table, void* out_uv, uint8_t* ok,
+                              unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_fixed_base<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(secret), n, static_cast<const uint4*>(table),
+                                                   static_cast<uint8_t*>(out_uv), ok, n_invalid);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint64_t* leaf_idx, size_t n, int arity,
                                uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st, const uint8_t* present) {
     if (n == 0 || depth == 0) return cudaSuccess;

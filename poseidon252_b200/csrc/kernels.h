@@ -132,6 +132,13 @@ cudaError_t launch_dhke(const void* secret, bool secret_bcast, const void* pub, 
 // launch_decrypt had not already counted as failures (decrypt)
 cudaError_t launch_dhke_fix(bool decrypt, const uint8_t* valid, size_t n, void* out, uint32_t row, uint8_t* ok,
                             unsigned long long* count, cudaStream_t st);
+// Fixed-base JubJub scalar multiplication (p252_fixed_base_batch): a table of kFixedBaseTableBytes built once per base
+// (base_uv: (u, v) Montgomery limbs, on the curve, read on the host at launch), then out_uv[i] = [secret[i]] base, one
+// thread per item; ok[i] = secret < r_J, an invalid item writes (0, 0) and is counted into *n_invalid (device, may be null)
+constexpr size_t kFixedBaseTableBytes = 64 * 8 * 96;
+cudaError_t launch_fixed_base_table(const uint64_t base_uv[8], void* table, cudaStream_t st);
+cudaError_t launch_fixed_base(const void* secret, size_t n, const void* table, void* out_uv, uint8_t* ok,
+                              unsigned long long* n_invalid, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

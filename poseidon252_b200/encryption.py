@@ -86,6 +86,36 @@ def decrypt_batch_dhke(ciphers, secrets, publics, nonces, engine=None, out=None,
     return eng.decrypt_batch_dhke(ciphers, secrets, publics, nonces, out=out, async_=async_)
 
 
+def fixed_base(secret, base, engine=None):
+    """[secret] base for one item: a public key GENERATOR_EXTENDED * secret when base is the generator's (u, v).
+    secret: a canonical int < r_J or one p252_jscalar row (4,) uint64; base: (2, 4) BlsScalar.0 limbs -> (2, 4) uint64.
+    Raises InvalidPoint for a secret >= r_J or a base off the curve.  There is no built-in generator: pass it."""
+    if isinstance(secret, (int, np.integer)):
+        sec = jubjub_limbs([secret])
+    else:
+        sec = np.ascontiguousarray(secret, dtype=np.uint64).reshape(1, 4)
+    eng = engine or default_engine()
+    out, ok = eng.fixed_base_batch(sec, base)
+    if not ok[0]:
+        raise InvalidPoint()
+    return out[0]
+
+
+def fixed_base_batch(secrets, base, engine=None, out=None, async_=False):
+    """NEW: n x [secret] base for one base point.  secrets (n, 4) p252_jscalar rows (scalar.jubjub_limbs), base (2, 4)
+    -> (points (n, 2, 4), ok (n,) uint8); ok == 0 marks a secret >= r_J, whose output is (0, 0)."""
+    eng = engine or default_engine(secrets.device.index if hasattr(secrets, "is_cuda") else 0)
+    return eng.fixed_base_batch(secrets, base, out=out, async_=async_)
+
+
+def encrypt_batch_ephemeral(messages, r, base, publics, nonces, engine=None, out=None, async_=False):
+    """NEW: the sender (src/encryption.rs:22-42) as a batch: R_i = [r_i] base and
+    cipher_i = encrypt(messages[i], dhke(r_i, publics[i]), nonces[i]), the shared secret derived on the device
+    -> (ciphers (n, L+1, 4), R (n, 2, 4), ok (n,) uint8).  publics holds 1 or n receiver keys."""
+    eng = engine or default_engine(messages.device.index if hasattr(messages, "is_cuda") else 0)
+    return eng.encrypt_batch_ephemeral(messages, r, base, publics, nonces, out=out, async_=async_)
+
+
 def cipher_offsets(offsets):
     """Offsets of the ciphers of messages at `offsets` (each one scalar longer, packed from 0): offsets - offsets[0] + i.
     Works on numpy arrays and CUDA tensors (no host sync)."""

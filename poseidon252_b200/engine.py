@@ -404,6 +404,73 @@ class Engine:
         The wallet-scan shape is one view key (secrets of 1 row) against every note's public key."""
         return self._crypt_dhke(True, ciphers, secrets, publics, nonces, out, async_)
 
+    # -- fixed-base JubJub scalar multiplication --------------------------------------------------
+    @staticmethod
+    def _base(base):
+        """The base point (u, v) as a host (2, 4) uint64 array: the library reads it on the host for every memory space
+        (a CUDA tensor is copied; the base is public)."""
+        a = np.ascontiguousarray(base.detach().cpu().numpy() if _is_torch(base) else base)
+        b = a.view(np.uint64) if a.dtype == np.int64 else np.ascontiguousarray(a, dtype=np.uint64)
+        if b.size != 8:
+            raise EngineError(-1, "base must be one point (u, v) of shape (2, 4), got %s" % (b.shape,))
+        return b.reshape(2, 4)
+
+    def _ok_like(self, like, n):
+        if _is_torch(like):
+            import torch
+            return torch.empty((n,), dtype=torch.uint8, device=like.device)
+        return np.empty((n,), dtype=np.uint8)
+
+    def fixed_base_batch(self, secrets, base, out=None, async_=False):
+        """n x [secret] base for one base point: secrets (n, 4) canonical p252_jscalar rows (scalar.jubjub_limbs), base
+        (2, 4) -- e.g. the generator, for public keys or ephemeral keys R = [r] G -> (points (n, 2, 4), ok (n,) uint8).
+        ok[i] == 0 marks a secret >= r_J; its output is (0, 0) and it is counted in last_dhke_invalid().  The base is
+        read on the host (a CUDA tensor is copied there); a base off the curve raises InvalidPoint.  The engine keeps
+        the table of its last base, so repeated calls with one base build it once."""
+        sp, sl, flags, sk = self._in(secrets, (4,))
+        if len(sl) != 1:
+            raise EngineError(-1, "secrets must have shape (n, 4)")
+        n = int(sl[0])
+        b = self._base(base)
+        res = self._out_like(sk, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), sk)
+        ok = self._ok_like(sk, n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._ninv = self._counter(flags)
+        self._check(self._lib.p252_fixed_base_batch(self._ctx, b.ctypes.data, sp, n, self._ptr(res), self._ptr(ok),
+                                                    ctypes.byref(self._ninv), flags))
+        return res, ok
+
+    def encrypt_batch_ephemeral(self, messages, r, base, publics, nonces, out=None, R_out=None, async_=False):
+        """The sender's side of the reference's key exchange as one call: R_i = [r_i] base and
+        cipher_i = encrypt(messages[i], dhke(r_i, publics[i]), nonces[i]) with the shared secret derived on the device and
+        never returned.  messages (n, L, 4), r (n, 4) p252_jscalar rows, base (2, 4) (host-read, as in fixed_base_batch),
+        publics (1 or n, 2, 4), nonces (n, 4) -> (ciphers (n, L+1, 4), R (n, 2, 4), ok (n,) uint8).  An item with
+        r >= r_J or a public key off the curve has ok == 0 and zeroed cipher and R rows (count: last_dhke_invalid())."""
+        L = int(messages.shape[1])
+        if L < 1:
+            raise EngineError(-1, "messages must hold at least one scalar")
+        dp, lead, flags, dk = self._in(messages, (L, 4))
+        if len(lead) != 1:
+            raise EngineError(-1, "expected shape (n, L, 4)")
+        n = lead[0]
+        sp, ns, pp, npub, _, f2, keep = self._dhke_args(r, publics, n)
+        if ns != n:
+            raise EngineError(-1, "r must have %d rows, got %d" % (n, ns))
+        np_, l3, f3, nk = self._in(nonces, (4,))
+        if not (flags == f2 == f3):
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("nonces", l3, n)
+        b = self._base(base)
+        res = self._out_like(dk, (n, L + 1, 4)) if out is None else self._check_out(out, (n, L + 1, 4), dk)
+        R = self._out_like(dk, (n, 2, 4)) if R_out is None else self._check_out(R_out, (n, 2, 4), dk)
+        ok = self._ok_like(dk, n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._ninv = self._counter(flags)
+        self._check(self._lib.p252_encrypt_batch_ephemeral(self._ctx, dp, n, L, sp, b.ctypes.data, pp, npub, np_,
+                                                           self._ptr(res), self._ptr(R), self._ptr(ok),
+                                                           ctypes.byref(self._ninv), flags))
+        return res, R, ok
+
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
         max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries
