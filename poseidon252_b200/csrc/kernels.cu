@@ -50,6 +50,19 @@ __device__ __forceinline__ uint4 ldg128(const void* p) { return __ldg(reinterpre
 // LDG.128 / STG.128 of the warp touches 4 complete 128-byte segments.  Shared side: XOR swizzle on
 // the 16-byte column keeps both the row-wise (global side) and the item-per-lane (register side)
 // accesses bank-conflict free.
+//
+// tile_row: the register side of a gather, the lane's own item (row `lane` of the tile) into four scalars v[0..3].
+__device__ __forceinline__ void tile_row(uint4 (*st)[8], int lane, uint32_t (*v)[8]) {
+#pragma unroll
+    for (int p = 0; p < 8; ++p) {
+        const uint4 x = st[lane][p ^ (lane & 7)];
+        v[p >> 1][(p & 1) * 4 + 0] = x.x;
+        v[p >> 1][(p & 1) * 4 + 1] = x.y;
+        v[p >> 1][(p & 1) * 4 + 2] = x.z;
+        v[p >> 1][(p & 1) * 4 + 3] = x.w;
+    }
+}
+
 __device__ __forceinline__ void warp_gather(uint4 (*st)[8], const uint8_t* base, size_t stride, int nitems,
                                             int nscal, int lane, uint32_t (&v)[4][8]) {
     const int part = lane & 7;
@@ -61,14 +74,7 @@ __device__ __forceinline__ void warp_gather(uint4 (*st)[8], const uint8_t* base,
         st[item][part ^ (item & 7)] = x;
     }
     __syncwarp();
-#pragma unroll
-    for (int p = 0; p < 8; ++p) {
-        const uint4 x = st[lane][p ^ (lane & 7)];
-        v[p >> 1][(p & 1) * 4 + 0] = x.x;
-        v[p >> 1][(p & 1) * 4 + 1] = x.y;
-        v[p >> 1][(p & 1) * 4 + 2] = x.z;
-        v[p >> 1][(p & 1) * 4 + 3] = x.w;
-    }
+    tile_row(st, lane, v);
     __syncwarp();
 }
 
@@ -103,6 +109,13 @@ __device__ __forceinline__ void load_fr_rw(uint32_t (&d)[8], const uint8_t* p) {
 __device__ __forceinline__ void store_fr(uint8_t* p, const uint32_t (&d)[8]) {
     *reinterpret_cast<uint4*>(p) = make_uint4(d[0], d[1], d[2], d[3]);
     *reinterpret_cast<uint4*>(p + 16) = make_uint4(d[4], d[5], d[6], d[7]);
+}
+
+// the lanes the last permutation of a digest must produce: only the rate lanes of the final squeeze chunk are read
+__device__ __forceinline__ uint32_t last_squeeze_lanes(uint32_t out_len) {
+    const uint32_t nout = (out_len + 3) / 4;
+    const uint32_t left = out_len - 4 * (nout - 1);
+    return ((1u << (left < 4 ? left : 4)) - 1u) << 1;
 }
 
 // ---- Hash::digest-shaped sponge: Absorb(in_len) -> Squeeze(out_len), item-major AoS ------------
@@ -141,12 +154,8 @@ __global__ void __launch_bounds__(kT, kMB) k_sponge_digest(FrArg tag, const uint
 #pragma unroll 1
     for (uint32_t step = 0; step < nin + nout; ++step) {
         if (step > 0) {
-            // the last permutation is read only through the rate lanes of the final squeeze chunk
             uint32_t need = 0x1fu;
-            if (step + 1 == nin + nout) {
-                const uint32_t left = out_len - 4 * (nout - 1);
-                need = ((1u << (left < 4 ? left : 4)) - 1u) << 1;
-            }
+            if (step + 1 == nin + nout) need = last_squeeze_lanes(out_len);
             hades_permute(s, need P252_TAB_PASS);
         }
         if (step < nin) {
@@ -188,30 +197,48 @@ __global__ void __launch_bounds__(kT, kMB) k_sponge_digest(FrArg tag, const uint
 // capacity (tag), lanes 1..4 the rate, so rate thread li absorbs input scalar 4*step + li - 1 and squeezes output
 // scalar 4*c + li - 1.  Loads/stores are 2 x 128-bit per scalar per thread (tiny batches: coalescing is irrelevant).
 constexpr int kCoopItemsPerWarp = 6;
+
+// Where a thread of a lane-split kernel sits: thread li (state lane li) of group grp, which owns warp item `item`.
+// mds_row fills lane li's MDS row for hades_permute_coop; the row stays a kernel-local array (held in the struct, it
+// changes the kernels' SASS).
+struct LaneSplit {
+    int grp, li, g0;
+    size_t first, item;                                          // first: the warp's first item
+    __device__ __forceinline__ LaneSplit() {
+        const int lane = threadIdx.x & 31;
+        grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
+        first = ((size_t)blockIdx.x * kWarps + (threadIdx.x >> 5)) * kCoopItemsPerWarp;
+        item = first + grp;
+    }
+    __device__ __forceinline__ bool idle(size_t n) const { return first >= n; }   // the whole warp
+    // idle threads (lanes 30, 31 and items past n) still take part in the shuffles
+    __device__ __forceinline__ bool live(size_t n) const { return grp < kCoopItemsPerWarp && item < n; }
+    __device__ __forceinline__ void mds_row(double (&crow)[5]) const {
+#pragma unroll
+        for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
+    }
+};
+
 __global__ void __launch_bounds__(kThreads) k_sponge_digest_coop(FrArg tag, const uint8_t* __restrict__ in, size_t n,
                                                                  uint32_t in_len, uint8_t* __restrict__ out, uint32_t out_len) {
-    const int lane = threadIdx.x & 31;
-    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
-    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const size_t item = warp_global * kCoopItemsPerWarp + grp;
-    if (warp_global * kCoopItemsPerWarp >= n) return;            // whole warp idle
-    const bool live = (grp < kCoopItemsPerWarp) && (item < n);   // idle threads still take part in the shuffles
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
     double crow[5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
+    ls.mds_row(crow);
 
     uint32_t s[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) s[k] = (li == 0) ? tag.l[k] : 0u;
+    for (int k = 0; k < 8; ++k) s[k] = (ls.li == 0) ? tag.l[k] : 0u;
     const uint32_t nin = (in_len + 3) / 4, nout = (out_len + 3) / 4;
-    const uint8_t* in_i = in + (live ? item : 0) * (size_t)in_len * 32;
-    uint8_t* out_i = out + (live ? item : 0) * (size_t)out_len * 32;
+    const uint8_t* in_i = in + (live ? ls.item : 0) * (size_t)in_len * 32;
+    uint8_t* out_i = out + (live ? ls.item : 0) * (size_t)out_len * 32;
 #pragma unroll 1
     for (uint32_t step = 0; step < nin + nout; ++step) {
-        if (step > 0) hades_permute_coop(s, li, g0, crow);
+        if (step > 0) hades_permute_coop(s, ls.li, ls.g0, crow);
         if (step < nin) {
-            const uint32_t q = 4 * step + (uint32_t)li - 1;      // li == 0 wraps to a huge value -> no absorb
-            if (li >= 1 && q < in_len) {
+            const uint32_t q = 4 * step + (uint32_t)ls.li - 1;   // li == 0 wraps to a huge value -> no absorb
+            if (ls.li >= 1 && q < in_len) {
                 uint32_t v[8], t[8];
                 load_fr(v, in_i + (size_t)q * 32);
                 fr_add_mod(t, s, v);
@@ -219,27 +246,23 @@ __global__ void __launch_bounds__(kThreads) k_sponge_digest_coop(FrArg tag, cons
                 for (int k = 0; k < 8; ++k) s[k] = t[k];
             }
         } else {
-            const uint32_t q = 4 * (step - nin) + (uint32_t)li - 1;
-            if (live && li >= 1 && q < out_len) store_fr(out_i + (size_t)q * 32, s);
+            const uint32_t q = 4 * (step - nin) + (uint32_t)ls.li - 1;
+            if (live && ls.li >= 1 && q < out_len) store_fr(out_i + (size_t)q * 32, s);
         }
     }
 }
 
 // raw permutation, small batches: thread li of a group loads / stores lane li of its state (32 B)
 __global__ void __launch_bounds__(kThreads) k_permute_coop(uint8_t* __restrict__ states, size_t n) {
-    const int lane = threadIdx.x & 31;
-    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
-    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const size_t item = warp_global * kCoopItemsPerWarp + grp;
-    if (warp_global * kCoopItemsPerWarp >= n) return;
-    const bool live = (grp < kCoopItemsPerWarp) && (item < n);
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
     double crow[5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
-    uint8_t* p = states + (live ? item : 0) * 160 + (size_t)li * 32;
+    ls.mds_row(crow);
+    uint8_t* p = states + (live ? ls.item : 0) * 160 + (size_t)ls.li * 32;
     uint32_t s[8];
     load_fr_rw(s, p);
-    hades_permute_coop(s, li, g0, crow);
+    hades_permute_coop(s, ls.li, ls.g0, crow);
     if (live) store_fr(p, s);
 }
 
@@ -291,6 +314,12 @@ __device__ __forceinline__ void warp_count(unsigned long long* counter, bool hit
     const unsigned act = __activemask();
     const unsigned b = __ballot_sync(act, hit);
     if (b && (threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(counter, (unsigned long long)__popc(b));
+}
+
+// the same where every lane of the warp is still running: lane 0 adds
+__device__ __forceinline__ void warp_count_full(unsigned long long* counter, bool hit) {
+    const unsigned b = __ballot_sync(0xffffffffu, hit);
+    if (b && (threadIdx.x & 31) == 0) atomicAdd(counter, (unsigned long long)__popc(b));
 }
 
 // ---- encrypt / decrypt (dusk_safe::encrypt / decrypt with Domain::Encryption) -------------------
@@ -517,14 +546,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_mtree_digest(FrArg tag, const u
     }
     __syncwarp();
     uint32_t s[5][8];
-#pragma unroll
-    for (int p = 0; p < 8; ++p) {
-        const uint4 x = st[lane][p ^ (lane & 7)];
-        s[1 + (p >> 1)][(p & 1) * 4 + 0] = x.x;
-        s[1 + (p >> 1)][(p & 1) * 4 + 1] = x.y;
-        s[1 + (p >> 1)][(p & 1) * 4 + 2] = x.z;
-        s[1 + (p >> 1)][(p & 1) * 4 + 3] = x.w;
-    }
+    tile_row(st, lane, s + 1);
 #pragma unroll
     for (int q = 0; q < 4; ++q) {                          // absorb into the zero rate lanes, as k_sponge_digest does
         uint32_t t[8];
@@ -556,30 +578,26 @@ __global__ void __launch_bounds__(kThreads) k_mtree_digest_coop(FrArg tag, const
                                                                 const int* __restrict__ cnt,
                                                                 const uint8_t* __restrict__ below_present,
                                                                 uint8_t* __restrict__ level_present) {
-    const int lane = threadIdx.x & 31;
-    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
     const size_t n = (size_t)*cnt;
-    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const size_t item = warp_global * kCoopItemsPerWarp + grp;
-    if (warp_global * kCoopItemsPerWarp >= n) return;            // whole warp idle
-    const bool live = (grp < kCoopItemsPerWarp) && (item < n);   // idle threads still take part in the shuffles
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
     double crow[5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
-    const uint64_t g = live ? d[item] : 0;
+    ls.mds_row(crow);
+    const uint64_t g = live ? d[ls.item] : 0;
     uint32_t s[8];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) s[k] = (li == 0) ? tag.l[k] : 0u;
-    if (live && li >= 1 && (uint32_t)li <= arity) {
+    for (int k = 0; k < 8; ++k) s[k] = (ls.li == 0) ? tag.l[k] : 0u;
+    if (live && ls.li >= 1 && (uint32_t)ls.li <= arity) {
         uint32_t v[8], t[8];
-        load_fr(v, below + (g * arity + (uint32_t)li - 1) * 32);
+        load_fr(v, below + (g * arity + (uint32_t)ls.li - 1) * 32);
         fr_add_mod(t, s, v);
 #pragma unroll
         for (int k = 0; k < 8; ++k) s[k] = t[k];
     }
-    hades_permute_coop(s, li, g0, crow);                          // collective: every thread of the warp takes part
+    hades_permute_coop(s, ls.li, ls.g0, crow);                    // collective: every thread of the warp takes part
     if (kSparse) {
-        if (live && li == 1) {
+        if (live && ls.li == 1) {
             const bool any = group_present(below_present + g * arity, arity);
 #pragma unroll
             for (int k = 0; k < 8; ++k) s[k] = any ? s[k] : 0u;
@@ -588,7 +606,7 @@ __global__ void __launch_bounds__(kThreads) k_mtree_digest_coop(FrArg tag, const
         }
         return;
     }
-    if (live && li == 1) store_fr(level + g * 32, s);
+    if (live && ls.li == 1) store_fr(level + g * 32, s);
 }
 
 // ---- sparse fixed-height trees: inserts and removals at any position (p252_smtree) -----------------------------------
@@ -939,10 +957,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) k_merkle_verify(FrArg ta
     for (int k = 0; k < 8; ++k) diff |= cur[k] ^ root.l[k];
     good = good && (diff == 0) && (idx == 0);             // idx != 0: leaf index beyond arity^depth
     if (live) ok[me] = good ? 1 : 0;
-    if (n_failed) {
-        const unsigned bad = __ballot_sync(0xffffffffu, live && !good);
-        if (bad && lane == 0) atomicAdd(n_failed, (unsigned long long)__popc(bad));
-    }
+    if (n_failed) warp_count_full(n_failed, live && !good);
 }
 
 // ---- variable-length digest batches (p252_hash_batch_varlen) ------------------------------------------------------
@@ -1026,11 +1041,8 @@ __global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint
 #pragma unroll 1
     for (uint32_t step = 0; step < wsteps; ++step) {
         if (step > 0 && step < steps) {
-            uint32_t need = 0x1fu;                         // the last permutation: only the final squeeze's lanes
-            if (step + 1 == steps) {
-                const uint32_t left = out_len - 4 * (nout - 1);
-                need = ((1u << (left < 4 ? left : 4)) - 1u) << 1;
-            }
+            uint32_t need = 0x1fu;
+            if (step + 1 == steps) need = last_squeeze_lanes(out_len);
             hades_permute(s, need P252_TAB_PASS);
         }
         const uint32_t left = step < nin ? len - 4 * step : 0u;
@@ -1049,14 +1061,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint
             }
             __syncwarp();
             uint32_t v[4][8];
-#pragma unroll
-            for (int p = 0; p < 8; ++p) {
-                const uint4 x = st[lane][p ^ (lane & 7)];
-                v[p >> 1][(p & 1) * 4 + 0] = x.x;
-                v[p >> 1][(p & 1) * 4 + 1] = x.y;
-                v[p >> 1][(p & 1) * 4 + 2] = x.z;
-                v[p >> 1][(p & 1) * 4 + 3] = x.w;
-            }
+            tile_row(st, lane, v);
             __syncwarp();
 #pragma unroll
             for (int q = 0; q < 4; ++q) {
@@ -1086,37 +1091,33 @@ __global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const ui
                                                                         const uint32_t* __restrict__ lens,
                                                                         const uint32_t* __restrict__ perm, uint32_t n,
                                                                         uint8_t* __restrict__ out, uint32_t out_len) {
-    const int lane = threadIdx.x & 31;
-    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
-    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const size_t k = warp_global * kCoopItemsPerWarp + grp;
-    if (warp_global * kCoopItemsPerWarp >= n) return;            // whole warp idle
-    const bool live = (grp < kCoopItemsPerWarp) && (k < n);      // idle threads still take part in the shuffles
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
     double crow[5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
-    const uint32_t len = live ? lens[k] : 0u;
-    const uint32_t i = live ? perm[k] : 0u;
+    ls.mds_row(crow);
+    const uint32_t len = live ? lens[ls.item] : 0u;
+    const uint32_t i = live ? perm[ls.item] : 0u;
     const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
     uint8_t* dst = out + (size_t)i * out_len * 32;
     const uint32_t nin = (len + 3) / 4, nout = (out_len + 3) / 4;
     const uint32_t steps = len ? nin + nout : 0u;
     const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
     uint32_t s[8];
-    if (li == 0) {
+    if (ls.li == 0) {
         load_fr(s, tags + (size_t)len * 32);
     } else {
 #pragma unroll
         for (int w = 0; w < 8; ++w) s[w] = 0u;
         if (live && len == 0)                                    // rejected: a zero row
-            for (uint32_t q = (uint32_t)li - 1; q < out_len; q += 4) store_fr(dst + (size_t)q * 32, s);
+            for (uint32_t q = (uint32_t)ls.li - 1; q < out_len; q += 4) store_fr(dst + (size_t)q * 32, s);
     }
 #pragma unroll 1
     for (uint32_t step = 0; step < wsteps; ++step) {
-        if (step > 0) hades_permute_coop(s, li, g0, crow);
+        if (step > 0) hades_permute_coop(s, ls.li, ls.g0, crow);
         if (step < nin) {
-            const uint32_t q = 4 * step + (uint32_t)li - 1;      // li == 0 wraps to a huge value -> no absorb
-            if (li >= 1 && q < len) {
+            const uint32_t q = 4 * step + (uint32_t)ls.li - 1;   // li == 0 wraps to a huge value -> no absorb
+            if (ls.li >= 1 && q < len) {
                 uint32_t v[8], t[8];
                 load_fr(v, src + (size_t)q * 32);
                 fr_add_mod(t, s, v);
@@ -1124,8 +1125,8 @@ __global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const ui
                 for (int w = 0; w < 8; ++w) s[w] = t[w];
             }
         } else if (step < steps) {
-            const uint32_t q = 4 * (step - nin) + (uint32_t)li - 1;
-            if (li >= 1 && q < out_len) store_fr(dst + (size_t)q * 32, s);
+            const uint32_t q = 4 * (step - nin) + (uint32_t)ls.li - 1;
+            if (ls.li >= 1 && q < out_len) store_fr(dst + (size_t)q * 32, s);
         }
     }
 }
@@ -1234,10 +1235,8 @@ __global__ void __launch_bounds__(kThreads, 4) k_crypt_varlen(const uint8_t* __r
             const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
             for (uint32_t q = 0; q < L; ++q) store_fr(dsti + (size_t)q * 32, zero);
         }
-        if (n_failed) {                                   // one atomic per warp that saw a failure; rejected items are not
-            const unsigned bad = __ballot_sync(0xffffffffu, L && !good);   // failures (k_varlen_keys counted them)
-            if (bad && lane == 0) atomicAdd(n_failed, (unsigned long long)__popc(bad));
-        }
+        // rejected items are not failures (k_varlen_keys counted them)
+        if (n_failed) warp_count_full(n_failed, L && !good);
     }
 }
 
@@ -1254,17 +1253,13 @@ __global__ void __launch_bounds__(kThreads) k_crypt_varlen_coop(const uint8_t* _
                                                                 const uint8_t* __restrict__ secret_uv,
                                                                 const uint8_t* __restrict__ nonce, uint8_t* dst,
                                                                 uint8_t* __restrict__ ok, unsigned long long* __restrict__ n_failed) {
-    const int lane = threadIdx.x & 31;
-    const int grp = lane / 5, li = lane - grp * 5, g0 = grp * 5;
-    const size_t warp_global = (size_t)blockIdx.x * kWarps + (threadIdx.x >> 5);
-    const size_t k = warp_global * kCoopItemsPerWarp + grp;
-    if (warp_global * kCoopItemsPerWarp >= n) return;            // whole warp idle
-    const bool live = (grp < kCoopItemsPerWarp) && (k < n);      // idle threads still take part in the shuffles
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
     double crow[5];
-#pragma unroll
-    for (int j = 0; j < 5; ++j) crow[j] = (double)(HADES_LAMBDA / (uint32_t)(li + j + 5));
-    const uint32_t L = live ? lens[k] : 0u;
-    const uint32_t i = live ? perm[k] : 0u;
+    ls.mds_row(crow);
+    const uint32_t L = live ? lens[ls.item] : 0u;
+    const uint32_t i = live ? perm[ls.item] : 0u;
     const uint64_t a = L ? offsets[i] : 0;
     const uint64_t o = L ? (kDecrypt ? a - offsets[0] - i : a - offsets[0] + i) : 0;
     const uint8_t* srci = src + (L ? (a - base) * 32 : 0);
@@ -1273,20 +1268,20 @@ __global__ void __launch_bounds__(kThreads) k_crypt_varlen_coop(const uint8_t* _
     uint32_t s[8];
 #pragma unroll
     for (int w = 0; w < 8; ++w) s[w] = 0u;
-    if (li == 0)
+    if (ls.li == 0)
         load_fr(s, tags + (size_t)L * 32);
-    else if (L && li <= 2)
-        load_fr(s, secret_uv + (size_t)i * 64 + (size_t)(li - 1) * 32);
-    else if (L && li == 3)
+    else if (L && ls.li <= 2)
+        load_fr(s, secret_uv + (size_t)i * 64 + (size_t)(ls.li - 1) * 32);
+    else if (L && ls.li == 3)
         load_fr(s, nonce + (size_t)i * 32);
     const uint32_t nk = (L + 3) / 4, steps = 2 * nk;
     const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
     bool good = true;
 #pragma unroll 1
     for (uint32_t step = 0; step < wsteps; ++step) {
-        hades_permute_coop(s, li, g0, crow);
-        const uint32_t q = 4 * step + (uint32_t)li - 1;          // li == 0 wraps to a huge value -> no memory access
-        if (step < nk && li >= 1 && q < L) {                     // squeeze chunk `step`: emit cipher / message scalar q
+        hades_permute_coop(s, ls.li, ls.g0, crow);
+        const uint32_t q = 4 * step + (uint32_t)ls.li - 1;       // li == 0 wraps to a huge value -> no memory access
+        if (step < nk && ls.li >= 1 && q < L) {                  // squeeze chunk `step`: emit cipher / message scalar q
             uint32_t x[8], y[8];
             load_fr(x, srci + (size_t)q * 32);
             if (kDecrypt)
@@ -1296,8 +1291,8 @@ __global__ void __launch_bounds__(kThreads) k_crypt_varlen_coop(const uint8_t* _
             store_fr(dsti + (size_t)q * 32, y);
         }
         if (step + 1 >= nk && step + 1 < steps) {                // absorb plaintext chunk c (this thread's own stores)
-            const uint32_t qa = 4 * (step + 1 - nk) + (uint32_t)li - 1;
-            if (li >= 1 && qa < L) {
+            const uint32_t qa = 4 * (step + 1 - nk) + (uint32_t)ls.li - 1;
+            if (ls.li >= 1 && qa < L) {
                 uint32_t x[8], t[8];
                 if (kDecrypt)
                     load_fr_rw(x, msgi + (size_t)qa * 32);
@@ -1308,7 +1303,7 @@ __global__ void __launch_bounds__(kThreads) k_crypt_varlen_coop(const uint8_t* _
                 for (int w = 0; w < 8; ++w) s[w] = t[w];
             }
         }
-        if (step + 1 == steps && li == 1) {                      // Squeeze(1): authentication element
+        if (step + 1 == steps && ls.li == 1) {                   // Squeeze(1): authentication element
             if (kDecrypt) {
                 uint32_t x[8];
                 load_fr(x, srci + (size_t)L * 32);
@@ -1320,16 +1315,13 @@ __global__ void __launch_bounds__(kThreads) k_crypt_varlen_coop(const uint8_t* _
         }
     }
     if (kDecrypt) {
-        good = __shfl_sync(0xffffffffu, good, g0 + 1);           // the group's verdict, before anyone zeroes
-        if (live && li == 0) ok[i] = (L && good) ? 1 : 0;
-        if (L && !good && li >= 1) {
+        good = __shfl_sync(0xffffffffu, good, ls.g0 + 1);        // the group's verdict, before anyone zeroes
+        if (live && ls.li == 0) ok[i] = (L && good) ? 1 : 0;
+        if (L && !good && ls.li >= 1) {
             const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-            for (uint32_t q = (uint32_t)li - 1; q < L; q += 4) store_fr(dsti + (size_t)q * 32, zero);
+            for (uint32_t q = (uint32_t)ls.li - 1; q < L; q += 4) store_fr(dsti + (size_t)q * 32, zero);
         }
-        if (n_failed) {
-            const unsigned bad = __ballot_sync(0xffffffffu, li == 0 && L && !good);
-            if (bad && lane == 0) atomicAdd(n_failed, (unsigned long long)__popc(bad));
-        }
+        if (n_failed) warp_count_full(n_failed, ls.li == 0 && L && !good);
     }
 }
 
@@ -1344,6 +1336,12 @@ static inline FrArg to_arg(const uint64_t tag[4]) {
 }
 
 static inline unsigned grid_for(size_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
+static inline unsigned blocks256(uint64_t n) { return (unsigned)((n + 255) / 256); }
+// lane-split kernels: kCoopItemsPerWarp items per warp
+static inline unsigned coop_grid(size_t n) {
+    return (unsigned)(((n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp + kWarps - 1) / kWarps);
+}
+static inline uint32_t log2_arity(int arity) { return arity == 4 ? 2u : 1u; }
 // digest batches from this size on (>= 7 waves of 256-thread blocks) take the 256 x 2 launch shape
 #ifndef P252_WIDE_SHAPE_MIN
 #define P252_WIDE_SHAPE_MIN (1u << 19)
@@ -1361,14 +1359,13 @@ size_t coop_max_items(int sm_count) {
 cudaError_t launch_permute(void* states, size_t n, bool dense, size_t coop_max, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!dense && n <= coop_max) {
-        const size_t warps = (n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_permute_coop<<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
+        k_permute_coop<<<coop_grid(n), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
         return cudaGetLastError();
     }
     if (dense)
         k_permute<true><<<grid_for(n), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
     else if (n >= kWideShapeMinItems)
-        k_permute<false, 256, 2><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<uint8_t*>(states), n);
+        k_permute<false, 256, 2><<<blocks256(n), 256, 0, st>>>(static_cast<uint8_t*>(states), n);
     else
         k_permute<false><<<grid_for(n), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
     return cudaGetLastError();
@@ -1378,8 +1375,7 @@ cudaError_t launch_digest(const uint64_t tag[4], const void* in, size_t n, uint3
                           uint32_t out_len, bool truncate, size_t coop_max, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (!truncate && n <= coop_max) {
-        const size_t warps = (n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_sponge_digest_coop<<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(
+        k_sponge_digest_coop<<<coop_grid(n), kThreads, 0, st>>>(
             to_arg(tag), static_cast<const uint8_t*>(in), n, in_len, static_cast<uint8_t*>(out), out_len);
         return cudaGetLastError();
     }
@@ -1387,7 +1383,7 @@ cudaError_t launch_digest(const uint64_t tag[4], const void* in, size_t n, uint3
         k_sponge_digest<true><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), static_cast<const uint8_t*>(in), n, in_len,
                                                                 static_cast<uint8_t*>(out), out_len);
     else if (n >= kWideShapeMinItems)
-        k_sponge_digest<false, 256, 2><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(
+        k_sponge_digest<false, 256, 2><<<blocks256(n), 256, 0, st>>>(
             to_arg(tag), static_cast<const uint8_t*>(in), n, in_len, static_cast<uint8_t*>(out), out_len);
     else
         k_sponge_digest<false><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), static_cast<const uint8_t*>(in), n, in_len,
@@ -1421,7 +1417,7 @@ __global__ void __launch_bounds__(256) k_convert(const uint8_t* __restrict__ in,
 
 cudaError_t launch_convert(const void* in, size_t n, void* out, uint8_t* ok, bool from_bytes, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    const unsigned grid = (unsigned)((n + 255) / 256);
+    const unsigned grid = blocks256(n);
     if (from_bytes)
         k_convert<true><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(in), n, static_cast<uint8_t*>(out), ok);
     else
@@ -1509,7 +1505,7 @@ cudaError_t launch_dhke(const void* secret, bool secret_bcast, const void* pub, 
 cudaError_t launch_dhke_fix(bool decrypt, const uint8_t* valid, size_t n, void* out, uint32_t row, uint8_t* ok,
                             unsigned long long* count, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    k_dhke_fix<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(decrypt, valid, n, static_cast<uint8_t*>(out), row, ok, count);
+    k_dhke_fix<<<blocks256(n), 256, 0, st>>>(decrypt, valid, n, static_cast<uint8_t*>(out), row, ok, count);
     return cudaGetLastError();
 }
 
@@ -1571,11 +1567,10 @@ cudaError_t launch_fixed_base(const void* secret, size_t n, const void* table, v
 cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint64_t* leaf_idx, size_t n, int arity,
                                uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st, const uint8_t* present) {
     if (n == 0 || depth == 0) return cudaSuccess;
-    const size_t total = n * depth;
-    const unsigned grid = (unsigned)((total + 255) / 256);
+    const unsigned grid = blocks256(n * depth);
     const uint8_t* l = static_cast<const uint8_t*>(leaves);
     const uint8_t* o = static_cast<const uint8_t*>(nodes);
-    const uint32_t la = arity == 4 ? 2u : 1u;
+    const uint32_t la = log2_arity(arity);
     if (present)
         k_merkle_open<true><<<grid, 256, 0, st>>>(l, o, leaf_idx, n, la, depth, lv, static_cast<uint8_t*>(paths), present);
     else
@@ -1586,7 +1581,7 @@ cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint
 cudaError_t launch_mtree_keys(const uint64_t* idx, uint32_t n_upd, uint64_t n_old, uint32_t total, uint64_t* keys,
                               uint32_t* pos, unsigned long long* rejected, cudaStream_t st) {
     if (total == 0) return cudaSuccess;
-    k_mtree_keys<<<(total + 255) / 256, 256, 0, st>>>(idx, n_upd, n_old, total, keys, pos, rejected);
+    k_mtree_keys<<<blocks256(total), 256, 0, st>>>(idx, n_upd, n_old, total, keys, pos, rejected);
     return cudaGetLastError();
 }
 
@@ -1594,7 +1589,7 @@ cudaError_t launch_mtree_leaf_write(const uint64_t* keys, const uint32_t* pos, u
                                     const void* values, uint32_t n_upd, const void* append, void* leaves, uint8_t* flag,
                                     uint64_t* parent, cudaStream_t st) {
     if (total == 0) return cudaSuccess;
-    k_mtree_leaf_write<<<(total + 255) / 256, 256, 0, st>>>(keys, pos, total, sentinel, arity == 4 ? 2u : 1u,
+    k_mtree_leaf_write<<<blocks256(total), 256, 0, st>>>(keys, pos, total, sentinel, log2_arity(arity),
                                                             static_cast<const uint8_t*>(values), n_upd,
                                                             static_cast<const uint8_t*>(append), static_cast<uint8_t*>(leaves),
                                                             flag, parent);
@@ -1604,7 +1599,7 @@ cudaError_t launch_mtree_leaf_write(const uint64_t* keys, const uint32_t* pos, u
 cudaError_t launch_mtree_parents(const uint64_t* d, const int* cnt, uint32_t bound, int arity, uint8_t* flag, uint64_t* parent,
                                  cudaStream_t st) {
     if (bound == 0) return cudaSuccess;
-    k_mtree_parents<<<(bound + 255) / 256, 256, 0, st>>>(d, cnt, bound, arity == 4 ? 2u : 1u, flag, parent);
+    k_mtree_parents<<<blocks256(bound), 256, 0, st>>>(d, cnt, bound, log2_arity(arity), flag, parent);
     return cudaGetLastError();
 }
 
@@ -1612,9 +1607,7 @@ template <bool kSparse>
 static void mtree_digest(FrArg tag, const uint8_t* b, int arity, uint8_t* o, const uint64_t* d, const int* cnt, size_t bound,
                          size_t coop_max, cudaStream_t st, const uint8_t* bp, uint8_t* lp) {
     if (bound <= coop_max) {
-        const size_t warps = (bound + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_mtree_digest_coop<kSparse><<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(tag, b, (uint32_t)arity, o, d,
-                                                                                                    cnt, bp, lp);
+        k_mtree_digest_coop<kSparse><<<coop_grid(bound), kThreads, 0, st>>>(tag, b, (uint32_t)arity, o, d, cnt, bp, lp);
     } else if (arity == 4) {
         k_mtree_digest<2, kSparse><<<grid_for(bound), kThreads, 0, st>>>(tag, b, o, d, cnt, bp, lp);
     } else {
@@ -1638,7 +1631,7 @@ cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int ar
 cudaError_t launch_smtree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t capacity, uint64_t* keys,
                                uint32_t* bpos, unsigned long long* rejected, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    k_smtree_keys<<<(n + 255) / 256, 256, 0, st>>>(pos, op, n, capacity, keys, bpos, rejected);
+    k_smtree_keys<<<blocks256(n), 256, 0, st>>>(pos, op, n, capacity, keys, bpos, rejected);
     return cudaGetLastError();
 }
 
@@ -1646,7 +1639,7 @@ cudaError_t launch_smtree_leaf_write(const uint64_t* keys, const uint32_t* bpos,
                                      const uint8_t* op, const void* values, void* leaves, uint8_t* present, uint8_t* flag,
                                      uint64_t* parent, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    k_smtree_leaf_write<<<(n + 255) / 256, 256, 0, st>>>(keys, bpos, n, sentinel, arity == 4 ? 2u : 1u, op,
+    k_smtree_leaf_write<<<blocks256(n), 256, 0, st>>>(keys, bpos, n, sentinel, log2_arity(arity), op,
                                                          static_cast<const uint8_t*>(values), static_cast<uint8_t*>(leaves),
                                                          present, flag, parent);
     return cudaGetLastError();
@@ -1655,19 +1648,16 @@ cudaError_t launch_smtree_leaf_write(const uint64_t* keys, const uint32_t* bpos,
 cudaError_t launch_smtree_seed(uint8_t* present, void* leaves, uint64_t groups, uint64_t capacity, int arity, uint8_t* flag,
                                uint64_t* parent, cudaStream_t st) {
     if (groups == 0) return cudaSuccess;
-    k_smtree_seed<<<(unsigned)((groups + 255) / 256), 256, 0, st>>>(present, static_cast<uint8_t*>(leaves), groups, capacity,
-                                                                    arity == 4 ? 2u : 1u, flag, parent);
+    k_smtree_seed<<<blocks256(groups), 256, 0, st>>>(present, static_cast<uint8_t*>(leaves), groups, capacity, log2_arity(arity),
+                                                     flag, parent);
     return cudaGetLastError();
 }
 
 cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned long long* out, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    const uint64_t blocks = (n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096;
-    k_smtree_count<<<(unsigned)blocks, 256, 0, st>>>(present, n, out);
+    k_smtree_count<<<n < 4096 * 256 ? blocks256(n) : 4096u, 256, 0, st>>>(present, n, out);
     return cudaGetLastError();
 }
-
-static unsigned blocks256(uint64_t n) { return (unsigned)((n + 255) / 256); }
 
 cudaError_t launch_ctree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t max_pos, uint64_t* keys, uint32_t* bpos,
                               unsigned long long* rejected, cudaStream_t st) {
@@ -1729,7 +1719,7 @@ cudaError_t launch_ctree_commit(const uint64_t* okeys, const void* ovals, uint64
 cudaError_t launch_ctree_gather(const uint64_t* okeys, const void* ovals, const uint64_t* stats, uint64_t s, const uint64_t* pkeys,
                                 const int* pcnt, uint32_t nb, int arity, void* groups, uint8_t* gpres, cudaStream_t st) {
     k_ctree_gather<<<blocks256(nb), 256, 0, st>>>(okeys, static_cast<const uint8_t*>(ovals), stats, s, pkeys, pcnt, nb,
-                                                  arity == 4 ? 2u : 1u, static_cast<uint8_t*>(groups), gpres);
+                                                  log2_arity(arity), static_cast<uint8_t*>(groups), gpres);
     return cudaGetLastError();
 }
 
@@ -1742,8 +1732,8 @@ cudaError_t launch_ctree_iota(uint64_t* d, uint32_t n, cudaStream_t st) {
 cudaError_t launch_ctree_open(const uint64_t* keys, const void* values, const uint64_t* count, const uint64_t* pos, size_t n,
                               int arity, uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st) {
     if (n == 0 || depth == 0) return cudaSuccess;
-    k_ctree_open<<<(unsigned)((n * depth + 255) / 256), 256, 0, st>>>(keys, static_cast<const uint8_t*>(values), count, pos, n,
-                                                                     arity == 4 ? 2u : 1u, depth, lv, static_cast<uint8_t*>(paths));
+    k_ctree_open<<<blocks256(n * depth), 256, 0, st>>>(keys, static_cast<const uint8_t*>(values), count, pos, n, log2_arity(arity),
+                                                       depth, lv, static_cast<uint8_t*>(paths));
     return cudaGetLastError();
 }
 
@@ -1763,7 +1753,7 @@ cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], 
 cudaError_t launch_varlen_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars, uint32_t max_len,
                                uint32_t fixed_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st) {
     if (n == 0) return cudaSuccess;
-    k_varlen_keys<0><<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
+    k_varlen_keys<0><<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
     return cudaGetLastError();
 }
 
@@ -1772,9 +1762,9 @@ cudaError_t launch_crypt_varlen_keys(bool decrypt, const uint64_t* offsets, uint
                                      cudaStream_t st) {
     if (n == 0) return cudaSuccess;
     if (decrypt)
-        k_varlen_keys<2><<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
+        k_varlen_keys<2><<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
     else
-        k_varlen_keys<1><<<(n + 255) / 256, 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
+        k_varlen_keys<1><<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
     return cudaGetLastError();
 }
 
@@ -1788,8 +1778,7 @@ cudaError_t launch_crypt_varlen(bool decrypt, const void* tags, const void* src,
     const uint8_t* no = static_cast<const uint8_t*>(nonce);
     uint8_t* d = static_cast<uint8_t*>(dst);
     if (n <= coop_max) {
-        const size_t warps = (n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        const unsigned grid = (unsigned)((warps + kWarps - 1) / kWarps);
+        const unsigned grid = coop_grid(n);
         if (decrypt)
             k_crypt_varlen_coop<true><<<grid, kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, ok, n_failed);
         else
@@ -1809,9 +1798,7 @@ cudaError_t launch_digest_varlen(const void* tags, const void* in, uint64_t base
     const uint8_t* i = static_cast<const uint8_t*>(in);
     uint8_t* o = static_cast<uint8_t*>(out);
     if (n <= coop_max) {
-        const size_t warps = (n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp;
-        k_sponge_digest_varlen_coop<<<(unsigned)((warps + kWarps - 1) / kWarps), kThreads, 0, st>>>(t, i, base, offsets, lens, perm,
-                                                                                                     n, o, out_len);
+        k_sponge_digest_varlen_coop<<<coop_grid(n), kThreads, 0, st>>>(t, i, base, offsets, lens, perm, n, o, out_len);
     } else {
         k_sponge_digest_varlen<<<grid_for(n), kThreads, 0, st>>>(t, i, base, offsets, lens, perm, n, o, out_len);
     }

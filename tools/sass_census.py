@@ -1,11 +1,14 @@
 """SASS opcode census of the built library (which instructions the kernels really issue).
 
     python tools/sass_census.py [path/to/lib.so|cubin] [--kernel SUBSTR] [--loops] [--lines OPC[,OPC...]]
+    python tools/sass_census.py [path/to/lib.so|cubin] --same-as OTHER.so
 
 For every kernel: static instruction count, opcode histogram, pipe summary (IMAD.WIDE-class on the fmaheavy pipe,
 narrow IMAD, ALU, FP64, memory).  --loops also prints one census per natural loop (backward branch -> its target),
 innermost first, which is what the round loop / S-box loop of the Hades kernel execute dynamically.
 --lines prints the first SASS lines of the given opcodes (e.g. LDG.E.128.CONSTANT,STG.E.128,DFMA) per kernel.
+--same-as OTHER.so compares every kernel's instruction text with OTHER's (addresses and encodings stripped), prints the
+kernels that differ or exist on one side only, and exits 1 if there are any.
 """
 import collections
 import os
@@ -83,9 +86,29 @@ def loops(ins):
     return sorted(found, key=lambda lo_hi: lo_hi[1] - lo_hi[0])
 
 
+def text(ins):
+    # instruction text only: the /*addr*/ prefix and the /* 0x... */ encoding comment removed
+    return [" ".join(re.sub(r"/\*[^*]*\*/", " ", ln).split()) for _, _, _, ln in ins]
+
+
+def same_as(path, other):
+    a, b = parse(path), parse(other)
+    names = list(a) + [k for k in b if k not in a]
+    bad = 0
+    for name in names:
+        if name not in a or name not in b:
+            print("only in %s: %s" % (path if name in a else other, demangle(name)))
+            bad += 1
+        elif text(a[name]) != text(b[name]):
+            print("differs: %s" % demangle(name))
+            bad += 1
+    print("%d kernels, %d identical" % (len(names), len(names) - bad))
+    return 1 if bad else 0
+
+
 def main():
     args = sys.argv[1:]
-    path, want, show_loops, lines = DEFAULT, None, False, []
+    path, want, show_loops, lines, other = DEFAULT, None, False, [], None
     while args:
         a = args.pop(0)
         if a == "--kernel":
@@ -94,8 +117,12 @@ def main():
             show_loops = True
         elif a == "--lines":
             lines = args.pop(0).split(",")
+        elif a == "--same-as":
+            other = args.pop(0)
         else:
             path = a
+    if other:
+        sys.exit(same_as(path, other))
     for name, ins in parse(path).items():
         dn = demangle(name)
         if want and want not in dn and want not in name:
