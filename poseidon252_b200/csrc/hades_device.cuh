@@ -6,8 +6,9 @@
 //   add_round_constants / quintic_s_box / mul_matrix
 //                                    src/hades/permutation/scalar.rs:39-64
 // with the bit-exact "scaled lazy" formulation derived in tools/hades_model.py:
-//   * 365 unreduced Montgomery products per permutation (IMAD.WIDE carry chains, fr_ptx.cuh)
-//     instead of the reference's 2000 (dense 25-multiply MDS every round);
+//   * 300 unreduced Montgomery products + 65 products by a table constant ("constant folds", 78 instead of 120
+//     IMAD.WIDE each) per permutation (carry chains, fr_ptx.cuh) instead of the reference's 2000 (dense 25-multiply
+//     MDS every round);
 //   * the MDS layer is 25 small-integer (<= 17 bit) multiply-adds per round, computed EXACTLY in FP64
 //     (DFMA on the otherwise idle FP64 pipe; column sums < 2^52) followed by ONE Montgomery row per
 //     lane; round constants ride inside that same accumulation;
@@ -28,7 +29,7 @@ namespace p252 {
 #include "hades_tables.inc"
 
 #if P252_CONST_SMEM
-// Experiment (north_star's suggestion): stage kA|kG into shared memory once per block with cp.async.bulk
+// Experiment (north_star's suggestion): stage kA|kGT into shared memory once per block with cp.async.bulk
 // (TMA, completion on an mbarrier) and read them with broadcast LDS instead of LDCU from the constant bank.
 __device__ __forceinline__ const uint32_t* stage_round_tables(uint32_t* s_tab, uint64_t* mbar) {
     const uint32_t bar = (uint32_t)__cvta_generic_to_shared(mbar);
@@ -57,17 +58,17 @@ __device__ __forceinline__ const uint32_t* stage_round_tables(uint32_t* s_tab, u
 #define P252_TAB_ARG , const uint32_t* tab
 #define P252_TAB_PASS , tab
 #define P252_A_ROW(round, lane) (tab + ((round) * 5 + (lane)) * 12)
-#define P252_G_ROW(idx) (tab + P252_TAB_A_WORDS + (idx) * 8)
+#define P252_G_ROW(idx) (tab + P252_TAB_A_WORDS + (idx) * 64)
 #else
 #define P252_TAB_ARG
 #define P252_TAB_PASS
 #define P252_A_ROW(round, lane) (kA[round][lane])
-#define P252_G_ROW(idx) (kG[idx])
+#define P252_G_ROW(idx) (&kGT[idx][0][0])
 #endif
 
 // hades_tables.inc defines, in the constant bank (statically initialised at module load):
-//   kA0[5][8], kA[69][5][12]  per-round additive constants (scaled)   kG[60][8]  lane-4 correction
-//   kF[8]         final multiplier                           kDenseArc / kDenseMds  dense tables
+//   kA0[5][8], kA[69][5][12]  per-round additive constants (scaled)   kGT[60][8][8]  lane-4 correction (fold table)
+//   kFT[8][8]     final multiplier (fold table)             kDenseArc / kDenseMds  dense tables
 // Every thread of a warp reads the same word in the same instruction (the round index is
 // warp-uniform), which the constant cache serves as a broadcast operand.
 
@@ -76,13 +77,15 @@ constexpr int kHalfFull = 4;
 constexpr int kPartial = 60;
 
 // Work per permutation in this formulation (see hades_permute below): 100 S-boxes (5 per full round, 1 per partial
-// round) = 200 squarings + 100 products, 60 lane-4 corrections, 5 final products; 68 mixes of 5 Montgomery rows.
+// round) = 200 squarings + 100 products; 60 lane-4 corrections and 5 final products as constant folds; 68 mixes of 5
+// Montgomery rows.
 constexpr int kSboxPerPerm = 2 * kHalfFull * 5 + kPartial;
 constexpr int kMontSqrPerPerm = 2 * kSboxPerPerm;
-constexpr int kMontMulPerPerm = kSboxPerPerm + kPartial + 5;
+constexpr int kMontMulPerPerm = kSboxPerPerm;
+constexpr int kFoldPerPerm = kPartial + 5;
 constexpr int kWideMulPerPerm = kMontSqrPerPerm * (kWideOps_fr_sqr_wide + kWideOps_fr_redc_wide) +
                                 kMontMulPerPerm * (kWideOps_fr_row_first + 7 * kWideOps_fr_row) +
-                                kRounds * 5 * kWideOps_fr_arc_redc1;
+                                kFoldPerPerm * kWideOps_fr_cfold + kRounds * 5 * kWideOps_fr_arc_redc1;
 constexpr int kDfmaPerPerm = kRounds * 5 * 5 * 8;
 
 // r = (x*y + m p) / 2^256.  Row operand x must satisfy x + p <= 2^256; y < 2^256.
@@ -119,6 +122,37 @@ __device__ __forceinline__ void sbox(uint32_t (&z)[8], const uint32_t (&u)[8]) {
 __device__ __forceinline__ void load_const(uint32_t (&d)[8], const uint32_t* c) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) d[k] = c[k];
+}
+
+// r = C w / R (mod p) for a constant C given by its fold table tab[8 j + k] = limb k of C 2^(32j - 192) mod p
+// (gen_tables.py): S = sum_j w_j T_j < 8 * 2^32 p < 2^290 over the 32-bit limbs w_j of w, then two Montgomery rows,
+// r = (S + m0 p + m1 p 2^32) / 2^64 < p + 2^226.  The same residue as montmul(C, w) (so the scale bookkeeping is
+// unchanged) for 64 + 2 * 7 multiplier instructions instead of 8 * 15.  w < 2^256, any value.  The table index is
+// warp-uniform, so every limb is a broadcast constant operand.
+__device__ __forceinline__ void cfold(uint32_t (&r)[8], const uint32_t* tab, const uint32_t (&w)[8]) {
+    uint32_t ev[9], od[9], t[8];
+    load_const(t, tab);
+    fr_fold_row_first(ev, od, t, w[0]);
+#pragma unroll
+    for (int j = 1; j < 8; ++j) {
+        load_const(t, tab + 8 * j);
+        fr_fold_row(ev, od, t, w[j]);
+    }
+    uint32_t s[10], u[9];
+    fr_fold_merge(s, ev, od);
+    fr_redc1_10(u, s);
+    fr_redc1(r, u);
+}
+
+// Partial-round S-box of lane 4 with its correction: z = G u^5 / R^5 = montmul(cfold(G, u), u^4 / R^3).  The fold
+// g = G u / R depends on u alone, so it runs alongside the two squarings instead of after the S-box; g < p + 2^226
+// keeps the row-operand condition g + p <= 2^256 of the last product.  z < 1.887 p.
+__device__ __forceinline__ void sbox_partial(uint32_t (&z)[8], const uint32_t (&u)[8], const uint32_t* gtab) {
+    uint32_t g[8], a[8], b[8];
+    cfold(g, gtab, u);
+    montsqr(a, u);             // < 1.4533 p
+    montsqr(b, a);             // < 1.9564 p
+    montmul(z, g, b);
 }
 
 constexpr double kTwo52 = 4503599627370496.0;
@@ -185,14 +219,12 @@ __device__ __forceinline__ void hades_permute(uint32_t (&s)[5][8], uint32_t out_
 #pragma unroll 1
     for (int r = 0; r < kRounds; ++r) {
         const bool full = (r < kHalfFull) || (r >= kHalfFull + kPartial);
-        // One S-box code instance serves both round kinds: it always works on slot 4.  Full rounds run it five
-        // times, rotating the lanes through slot 4; partial rounds run it once and apply the lane-4 correction.
-        const int n_sbox = full ? 5 : 1;
+        if (full) {
+            // one S-box code instance on slot 4, run five times, rotating the lanes through slot 4
 #pragma unroll 1
-        for (int it = 0; it < n_sbox; ++it) {
-            uint32_t w[8];
-            sbox(w, s[4]);
-            if (full) {
+            for (int it = 0; it < 5; ++it) {
+                uint32_t w[8];
+                sbox(w, s[4]);
 #pragma unroll
                 for (int k = 0; k < 8; ++k) {
                     s[4][k] = s[3][k];
@@ -201,20 +233,18 @@ __device__ __forceinline__ void hades_permute(uint32_t (&s)[5][8], uint32_t out_
                     s[1][k] = s[0][k];
                     s[0][k] = w[k];
                 }
-            } else {
-                load_const(c, P252_G_ROW(r - kHalfFull));
-                montmul(s[4], c, w);
             }
+        } else {
+            sbox_partial(s[4], s[4], P252_G_ROW(r - kHalfFull));
         }
         mix(s, r + 1 P252_TAB_PASS);      // r + 1 == kRounds: row 68 of kA carries no round constants
     }
-    // leave the scaled domain: out = montmul(F, v) fully reduced
-    load_const(c, kF);
+    // leave the scaled domain: out = F v / R (constant fold) fully reduced
 #pragma unroll 1
     for (int it = 0; it < 5; ++it) {
         uint32_t w[8];
         if ((out_lanes >> (4 - it)) & 1u) {            // slot 4 holds lane 4 - it
-            montmul(w, c, s[4]);
+            cfold(w, &kFT[0][0], s[4]);
             fr_condsub(w);
         } else {
 #pragma unroll
@@ -294,23 +324,22 @@ __device__ __forceinline__ void hades_permute_coop(uint32_t (&s)[8], int li, int
 #pragma unroll 1
     for (int r = 0; r < kRounds; ++r) {
         const bool full = (r < kHalfFull) || (r >= kHalfFull + kPartial);
-        uint32_t w[8];
-        sbox(w, s);                                   // every thread runs it; in partial rounds only lane 4 keeps it
+        // every thread runs the S-box; in partial rounds only lane 4 keeps it
         if (full) {
+            uint32_t w[8];
+            sbox(w, s);
 #pragma unroll
             for (int k = 0; k < 8; ++k) s[k] = w[k];
         } else {
-            uint32_t c[8], z[8];
-            load_const(c, kG[r - kHalfFull]);         // always the constant bank (warp-uniform index)
-            montmul(z, c, w);
+            uint32_t z[8];
+            sbox_partial(z, s, &kGT[r - kHalfFull][0][0]);   // always the constant bank (warp-uniform index)
 #pragma unroll
             for (int k = 0; k < 8; ++k) s[k] = (li == 4) ? z[k] : s[k];
         }
         coop_mix(s, r + 1, li, g0, crow);
     }
-    uint32_t c[8], w[8];
-    load_const(c, kF);
-    montmul(w, c, s);
+    uint32_t w[8];
+    cfold(w, &kFT[0][0], s);
     fr_condsub(w);
 #pragma unroll
     for (int k = 0; k < 8; ++k) s[k] = w[k];

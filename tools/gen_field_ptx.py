@@ -289,16 +289,19 @@ def gen_mix_sum() -> Prog:
     return pg
 
 
-def gen_redc1(with_arc: bool) -> Prog:
+def gen_redc1(with_arc: bool, n: int = 9) -> Prog:
     """t (9 limbs) holds the folded FP64 column sums INCLUDING the double-exponent offsets
     K_off = 0x43300000 * sum_{k=1..8} 2^(32k); a (9 limbs) = (A - K_off) mod 2^288, so that t + a wraps to the
     true T + A < 2^288.  Then one Montgomery row, kept in even/odd form so that every IMAD.WIDE accumulator is
     one fixed (even, odd) register pair: the even products m*p2, m*p4, m*p6 chain into t itself, the odd
-    products m*p1..p7 go to a fresh odd-aligned array (plain mul.wide), and one add chain merges them."""
-    name = "fr_arc_redc1" if with_arc else "fr_redc1"
-    pg = Prog(name, "u = (t + a (mod 2^288) + m p) >> 32 with m = -(t+a) mod 2^32; t, a are 9 limbs")
-    u = pg.out(*arr("u", 8))
-    t = pg.inout(*arr("t", 9))
+    products m*p1..p7 go to a fresh odd-aligned array (plain mul.wide), and one add chain merges them.
+    n = 10 (no constant): the same row on a 10-limb t, giving 9 limbs (first row of the constant fold)."""
+    assert n == 9 or not with_arc
+    name = "fr_arc_redc1" if with_arc else ("fr_redc1" if n == 9 else "fr_redc1_%d" % n)
+    pg = Prog(name, "u = (t + a (mod 2^288) + m p) >> 32 with m = -(t+a) mod 2^32; t, a are 9 limbs" if with_arc else
+              "u = (t + m p) >> 32 with m = -t mod 2^32; t is %d limbs, u %d" % (n, n - 1))
+    u = pg.out(*arr("u", n - 1))
+    t = pg.inout(*arr("t", n))
     if with_arc:
         a = pg.inp(*arr("a", 9))
         pg.op("add.cc.u32", t[0], t[0], a[0])
@@ -320,11 +323,64 @@ def gen_redc1(with_arc: bool) -> Prog:
     for k in (2, 4, 6):                               # even columns (2,3),(4,5),(6,7)
         pg.op("madc.lo.cc.u32", t[k], m, PL[k], t[k])
         pg.op("madc.hi.cc.u32", t[k + 1], m, PL[k], t[k + 1])
-    pg.op("addc.u32", t[8], t[8], 0, nocarry=True)
+    for k in range(8, n - 1):
+        pg.op("addc.cc.u32", t[k], t[k], 0)
+    pg.op("addc.u32", t[n - 1], t[n - 1], 0, nocarry=True)
     pg.op("add.cc.u32", u[0], t[1], o[0])
     for k in range(1, 7):
         pg.op("addc.cc.u32", u[k], t[k + 1], o[k])
-    pg.op("addc.u32", u[7], t[8], o[7], nocarry=True)
+    if n == 9:
+        pg.op("addc.u32", u[7], t[8], o[7], nocarry=True)
+    else:
+        pg.op("addc.cc.u32", u[7], t[8], o[7])
+        for k in range(8, n - 2):
+            pg.op("addc.cc.u32", u[k], t[k + 1], 0)
+        pg.op("addc.u32", u[n - 2], t[n - 1], 0, nocarry=True)
+    return pg
+
+
+# ------------------------------------------------------------------------------------------------
+# Product by a table constant C:  S = sum_j w_j T_j  with  T_j = C 2^(32j - 192) mod p  (eight 32 x 256-bit rows, all
+# at the same alignment, S < 8 * 2^32 p < 2^290), then two Montgomery rows (fr_redc1_10, fr_redc1):
+#   z = (S + m0 p + m1 p 2^32) / 2^64  ==  C w / R  (mod p),  z < p + 2^226.
+# Same residue as montmul(C, w) with 64 + 2 * 7 multiplier instructions instead of 8 * 15.
+# Window: ev[k] = limb k (0..8) takes the products with T_j's even limbs, od[k] = limb k + 1 (1..9) the odd ones; each
+# row's carry stops in the top limb (< 8 after eight rows).
+# ------------------------------------------------------------------------------------------------
+def gen_fold_row(first: bool) -> Prog:
+    name = "fr_fold_row_first" if first else "fr_fold_row"
+    pg = Prog(name, "ev/od = t * wj (first row)" if first else "ev/od += t * wj  (t: 8 limbs, wj: one 32-bit limb)")
+    ev = (pg.out if first else pg.inout)(*arr("ev", 9))
+    od = (pg.out if first else pg.inout)(*arr("od", 9))
+    t = pg.inp(*arr("t", 8))
+    wj = pg.inp("wj")
+    if first:
+        for k in (0, 2, 4, 6):
+            pg.op("mul.lo.u32", ev[k], t[k], wj)
+            pg.op("mul.hi.u32", ev[k + 1], t[k], wj)
+            pg.op("mul.lo.u32", od[k], t[k + 1], wj)
+            pg.op("mul.hi.u32", od[k + 1], t[k + 1], wj)
+        pg.op("mov.u32", ev[8], 0)
+        pg.op("mov.u32", od[8], 0)
+        return pg
+    for acc, off in ((ev, 0), (od, 1)):
+        for k in (0, 2, 4, 6):
+            pg.op("mad.lo.cc.u32" if k == 0 else "madc.lo.cc.u32", acc[k], t[k + off], wj, acc[k])
+            pg.op("madc.hi.cc.u32", acc[k + 1], t[k + off], wj, acc[k + 1])
+        pg.op("addc.u32", acc[8], acc[8], 0, nocarry=True)
+    return pg
+
+
+def gen_fold_merge() -> Prog:
+    pg = Prog("fr_fold_merge", "s[0..9] = ev[0..8] + (od[0..8] << 32)")
+    s = pg.out(*arr("s", 10))
+    ev = pg.inp(*arr("ev", 9))
+    od = pg.inp(*arr("od", 9))
+    pg.op("mov.u32", s[0], ev[0])
+    pg.op("add.cc.u32", s[1], ev[1], od[0])
+    for k in range(2, 9):
+        pg.op("addc.cc.u32", s[k], ev[k], od[k - 1])
+    pg.op("addc.u32", s[9], od[8], 0, nocarry=True)
     return pg
 
 
@@ -564,7 +620,8 @@ def gen_redc_wide() -> Prog:
 
 ALL = [gen_row_first(), gen_row(), gen_merge(), gen_redc1(True),
        gen_condsub255(), gen_condsub(), gen_add(), gen_submod(),
-       gen_sqr_product(), gen_redc_wide()]
+       gen_sqr_product(), gen_redc_wide(),
+       gen_fold_row(True), gen_fold_row(False), gen_fold_merge(), gen_redc1(False, 10), gen_redc1(False)]
 BY_NAME = {p.name: p for p in ALL}
 
 SIGS = {
@@ -578,6 +635,11 @@ SIGS = {
     "fr_sub_mod": "uint32_t (&r)[8], const uint32_t (&a)[8], const uint32_t (&b)[8]",
     "fr_sqr_wide": "uint32_t (&t)[16], const uint32_t (&a)[8]",
     "fr_redc_wide": "uint32_t (&r)[8], const uint32_t (&t)[16]",
+    "fr_fold_row_first": "uint32_t (&ev)[9], uint32_t (&od)[9], const uint32_t (&t)[8], uint32_t wj",
+    "fr_fold_row": "uint32_t (&ev)[9], uint32_t (&od)[9], const uint32_t (&t)[8], uint32_t wj",
+    "fr_fold_merge": "uint32_t (&s)[10], const uint32_t (&ev)[9], const uint32_t (&od)[9]",
+    "fr_redc1_10": "uint32_t (&u)[9], uint32_t (&t)[10]",
+    "fr_redc1": "uint32_t (&u)[8], uint32_t (&t)[9]",
 }
 
 
@@ -638,6 +700,23 @@ def emu_mix_lane(cols: Sequence[int], arc: int | None) -> int:
     return sum(v << (32 * i) for i, v in enumerate(_get(reg, "u", 8)))
 
 
+def emu_cfold(tab: Sequence[int], w: int) -> int:
+    """The constant fold as hades_device.cuh's cfold() composes it: eight rows, the merge, two Montgomery rows."""
+    wl = hm_limbs(w)
+    reg = BY_NAME["fr_fold_row_first"].run({**_put("t", hm_limbs(tab[0])), "wj": wl[0]})
+    for j in range(1, 8):
+        env = {**_put("t", hm_limbs(tab[j])), "wj": wl[j], **_put("ev", _get(reg, "ev", 9)), **_put("od", _get(reg, "od", 9))}
+        reg = BY_NAME["fr_fold_row"].run(env)
+    reg = BY_NAME["fr_fold_merge"].run({**_put("ev", _get(reg, "ev", 9)), **_put("od", _get(reg, "od", 9))})
+    reg = BY_NAME["fr_redc1_10"].run(_put("t", _get(reg, "s", 10)))
+    reg = BY_NAME["fr_redc1"].run(_put("t", _get(reg, "u", 9)))
+    return sum(v << (32 * i) for i, v in enumerate(_get(reg, "u", 8)))
+
+
+def hm_limbs(v: int) -> List[int]:
+    return [(v >> (32 * i)) & M32 for i in range(8)]
+
+
 def emu_unary(name: str, a: int) -> int:
     reg = BY_NAME[name].run(_put("a", [(a >> (32 * i)) & M32 for i in range(8)]))
     return sum(v << (32 * i) for i, v in enumerate(_get(reg, "a", 8)))
@@ -668,12 +747,19 @@ def wide_ops(pg: Prog) -> int:
     return sum(1 for opc, *_ in pg.ops if opc == "mulwide" or ".hi" in opc)
 
 
+def cfold_wide_ops() -> int:
+    return sum(wide_ops(BY_NAME[n]) * k for n, k in (("fr_fold_row_first", 1), ("fr_fold_row", 7), ("fr_redc1_10", 1),
+                                                      ("fr_redc1", 1)))
+
+
 def emit_header() -> str:
     s = HEADER
     s += "// multiplier instructions (IMAD.WIDE / IMAD.HI class) per primitive, counted by the generator\n"
     for pg in ALL:
         if wide_ops(pg):
             s += "constexpr int kWideOps_%s = %d;\n" % (pg.name, wide_ops(pg))
+    s += "// the whole constant fold: eight rows + two Montgomery rows (cfold in hades_device.cuh)\n"
+    s += "constexpr int kWideOps_fr_cfold = %d;\n" % cfold_wide_ops()
     s += "\n"
     for pg in ALL:
         s += "// %s\n" % pg.doc

@@ -14,15 +14,19 @@ round-dependent, data-independent scale kappa_r:
 
   * montmul(a,b) = (a*b + m*p)/2^256 (m = -a*b/p mod 2^256)  -- unreduced Montgomery product
   * full round   : z = montmul(u, montsqr(montsqr(u)))            (scale kappa^5 R^4)
-  * partial round: lane 4 gets one extra montmul by G_r = kappa_r^4 R^5 so that its scale equals
-                   the scale kappa_r of the four linear lanes
+  * partial round: lane 4 is multiplied by G_r = kappa_r^4 R^5 (result scale G_r / R, as a montmul) so that its
+                   scale equals the scale kappa_r of the four linear lanes: z = montmul(cfold(G_r, u), montsqr^2(u)),
+                   the fold taken on the S-box input so that it does not wait for the squarings
+  * constant fold: a product C w / R by a table constant C (G_r, F) is  S = sum_j w_j T_j  over w's 32-bit
+                   limbs with T_j = C 2^(32j-192) mod p, then two Montgomery rows (S + m0 p + m1 p 2^32)/2^64:
+                   64 + 14 limb products instead of a montmul's 120, result < p + 2^226
   * mix          : T_i = A_{r+1,i} + sum_j c_ij z_j  (plain small-integer MADs, 9 limbs), then one
                    Montgomery row  u_i = (T_i + m p)/2^32  (m = -T_i mod 2^32)
                    => kappa_{r+1} = K * sigma_r * 2^32,  A_{r+1,i} = arc_{r+1,i} / (K sigma_r)
-  * last round   : out_i = montmul(redc1(T_i), F),  F = K sigma R^2 2^32, then one conditional
+  * last round   : out_i = fold of redc1(T_i) by F,  F = K sigma R^2 2^32, then one conditional
                    subtraction -> standard Montgomery form in [0,p), i.e. BlsScalar.0 bit-exact.
 
-Per permutation: 365 Montgomery products + 340 small mixes instead of the reference's
+Per permutation: 300 Montgomery products + 65 constant folds + 340 small mixes instead of the reference's
 2000 products (src/hades/permutation/scalar.rs:54-64 does 25 per round).
 """
 from __future__ import annotations
@@ -79,7 +83,7 @@ def is_full(r: int) -> bool:
 class Tables:
     """kappa[r]: scale at the S-box input of round r.  A[r][i]: ARC term added inside the mix that
     *produces* round r's input (r >= 1); A[0] is the explicit first add.  G[r]: lane-4 correction
-    (partial rounds).  F: final output multiplier."""
+    (partial rounds).  F: final output multiplier.  GT[r], FT: their constant-fold tables (fold_table)."""
 
     def __init__(self):
         self.kappa = [0] * ROUNDS
@@ -100,6 +104,14 @@ class Tables:
                 kappa = ks * (1 << 32) % P
             else:
                 self.F = ks * pow(R, 2, P) * (1 << 32) % P
+        self.GT = [fold_table(g) if g else None for g in self.G]
+        self.FT = fold_table(self.F)
+
+
+def fold_table(c: int) -> List[int]:
+    """T_j = c 2^(32j - 192) mod p, j = 0..7: sum_j w_j T_j = c w 2^-192 (mod p) for w = sum_j w_j 2^(32j)."""
+    i192 = inv(1 << 192)
+    return [c * pow(2, 32 * j, P) * i192 % P for j in range(8)]
 
 
 TABLES = Tables()
@@ -139,6 +151,20 @@ def redc1(t: int, site: str = "redc1") -> int:
     assert r < TWO256
     Bounds.note(site, r)
     return r
+
+
+def cfold(tab: Sequence[int], w: int, site: str = "cfold") -> int:
+    """Constant fold (hades_device.cuh cfold): S = sum_j w_j tab[j] over the 32-bit limbs of w, then two Montgomery
+    rows.  Equals C w / R (mod p) for tab = fold_table(C), like montmul(C, w), with a different representative."""
+    assert 0 <= w < TWO256
+    s = sum(((w >> (32 * j)) & M32) * t for j, t in enumerate(tab))
+    assert s < 1 << 290, "fold sum overflows the 10-limb window"
+    for _ in range(2):
+        m = (-s) & M32
+        s = (s + m * P) >> 32
+    assert s < TWO256
+    Bounds.note(site, s)
+    return s
 
 
 def condsub255(a: int) -> int:
@@ -203,7 +229,8 @@ def permute_model(state_mont: Sequence[int], trace=None) -> List[int]:
     Returns the permuted state in the same form -- must equal the reference bit for bit.
 
     trace(r, site, lane, value), if given, sees every intermediate integer: per round r the S-box
-    input or linear lane `u`, the S-box's `sqr1`, `sqr2`, `x5`, the partial rounds' `gmul`, and the
+    input or linear lane `u`, the S-box's `sqr1`, `sqr2`, `x5` (full rounds; in partial rounds lane 4's `gfold` =
+    cfold(G, u) and the corrected S-box output `gmul` = montmul(gfold, sqr2) instead of `x5`), and the
     mix total `T` that produces round r+1's `u` (round 67: the final mix); then, under r = ROUNDS,
     each lane's `final` value before the last conditional subtraction."""
     T = TABLES
@@ -217,16 +244,21 @@ def permute_model(state_mont: Sequence[int], trace=None) -> List[int]:
         if is_full(r):
             z = [sbox(x, lane_trace(i)) for i, x in enumerate(u)]
         else:
-            g = montmul(T.G[r], sbox(u[4], lane_trace(4)), "gmul")
+            # lane 4: G u^5 / R^5 = montmul(cfold(G, u), u^4 / R^3); the fold of u runs beside the squarings
+            gu = cfold(T.GT[r], u[4], "gfold")
+            a = montsqr(u[4], "sqr1")
+            b = montsqr(a, "sqr2")
+            g = montmul(gu, b, "gmul")
             if trace is not None:
-                trace(r, "gmul", 4, g)
+                for name, v in (("gfold", gu), ("sqr1", a), ("sqr2", b), ("gmul", g)):
+                    trace(r, name, 4, v)
             z = list(u[:4]) + [g]
         mix_trace = None if trace is None else (lambda i, t: trace(r, "T", i, t))
         if r + 1 < ROUNDS:
             u = mix(z, T.A[r + 1], mix_trace)
         else:
             v = mix(z, None, mix_trace)
-            w = [montmul(T.F, x, "final") for x in v]
+            w = [cfold(T.FT, x, "final") for x in v]
             if trace is not None:
                 for i, x in enumerate(w):
                     trace(ROUNDS, "final", i, x)
