@@ -124,6 +124,10 @@ mod dhke;
 // `extern "C"` block in fixed_base.rs (methods on Engine).
 mod fixed_base;
 
+// Stealth addresses (the sender's note keys and a view key's ownership scan): their own `extern "C"` block in stealth.rs
+// (methods on Engine).
+mod stealth;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

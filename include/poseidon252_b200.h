@@ -314,6 +314,38 @@ int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, si
                                  const p252_fr* base_uv, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce,
                                  p252_fr* cipher, p252_fr* R_uv, uint8_t* ok, size_t* n_invalid, int flags);
 
+/* ---- Stealth addresses: the sender's (R, note_pk) and the receiver's ownership scan (Phoenix notes) ----------------
+ *   hash(P)                       = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0]   (P affine, < 2^250 < r_J)
+ *   sender   (r; A, B):             R = [r] G,  note_pk = [hash([r] A)] G + B
+ *   receiver (a, B; R, note_pk):    owns  <=>  note_pk == [hash([a] R)] G + B
+ * (A, B) = ([a] G, [b] G) is the receiver's public key and a its view key; [r] A = [a] R, so a note is owned by its
+ * receiver.  Scalars and points are laid out as for p252_dhke_batch.  base_uv (G) is a HOST pointer for every memory space,
+ * as in p252_fixed_base_batch, and so is spend_B_uv in the scan.  Either one with a coordinate >= p or off the curve is
+ * refused with P252_ERR_INVALID_POINT before anything runs, for every memory space and for n == 0.
+ * Item validity:
+ *   sender:   r < r_J, and A and B curve points with u, v < p (checked on the device per item, also for n_public == 1).  An
+ *             invalid item gets ok[i] = 0, a zeroed R row and a zeroed note_pk row, and is counted once into *n_invalid.
+ *   receiver: view_a < r_J (one scalar; if it is out of range every item is invalid), R a curve point with u, v < p, and
+ *             both note_pk coordinates < p.  An invalid item gets owned[i] = 0 and is counted into *n_invalid, not
+ *             *n_owned.  A note_pk with canonical coordinates off the curve is simply not owned.
+ * *n_owned = number of owned[i] == 1.  n_owned / n_invalid: optional HOST pointers for both memory spaces (lifetime as for
+ * p252_decrypt_batch).
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_public not 1 or n, DEVICE buffers other than ok / owned
+ * not 16-byte aligned -> INVALID_ARGUMENT.
+ * r, view_a, the shared points [r] A = [a] R and their hashes live only in the context's staging arenas, for both memory
+ * spaces, and the arenas are zeroed on every exit path: both calls are synchronous (P252_ASYNC only defers the
+ * publication of the counts to p252_sync).  Each item is constant time (no branch and no address depends on secret bits);
+ * see DESIGN.md section 4. */
+/* Sender: R_uv[i] = [r[i]] base, note_pk_uv[i] = [hash([r[i]] A)] base + B, with (A, B) =
+ * (A_uv, B_uv)[n_public == 1 ? 0 : i]. */
+int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, const p252_fr* base_uv, const p252_fr* A_uv,
+                               const p252_fr* B_uv, size_t n_public, p252_fr* R_uv, p252_fr* note_pk_uv, uint8_t* ok,
+                               size_t* n_invalid, int flags);
+/* Receiver: owned[i] = note_pk_uv[i] == [hash([view_a] R_uv[i])] base + spend_B. */
+int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p252_fr* spend_B_uv, const p252_fr* base_uv,
+                            const p252_fr* R_uv, const p252_fr* note_pk_uv, size_t n, uint8_t* owned, size_t* n_owned,
+                            size_t* n_invalid, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

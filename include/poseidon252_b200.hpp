@@ -9,7 +9,8 @@
 //   dusk_poseidon::Error                     (src/error.rs:11-32)      -> p252::Error (exception)
 //   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
 //   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
-//   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, merkle4_build.
+//   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
+//   stealth_address_batch, owns / stealth_owns_batch, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -342,6 +343,54 @@ inline std::vector<Scalar> encrypt_batch_ephemeral(const Scalar* msg, size_t n, 
                                        ok.data(), nullptr, P252_MEM_HOST),
           e.get());
     return cipher;
+}
+
+// NEW: stealth addresses (p252_stealth_address_batch / p252_stealth_owns_batch).  The sender makes R = [r] G and
+// note_pk = [hash([r] A)] G + B for the receiver's key (A, B); the receiver with view key a and spend key B owns a note iff
+// note_pk == [hash([a] R)] G + B.  base_uv is the caller's G (no built-in generator); a G or receiver B off the curve
+// throws Error(P252_ERR_INVALID_POINT).  publics_A / publics_B hold 1 or n points each (n_public).
+// returns n x 2 scalars, the note keys; R receives n x 2 scalars; ok[i] == 0 marks an invalid item (zeroed rows)
+inline std::vector<Scalar> stealth_address_batch(const JubJubScalar* r, size_t n, const Scalar (&base_uv)[2],
+                                                 const Scalar* publics_A, const Scalar* publics_B, size_t n_public,
+                                                 std::vector<Scalar>& R, std::vector<uint8_t>& ok,
+                                                 Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> note_pk(2 * n);
+    R.assign(2 * n, Scalar{});
+    ok.assign(n, 0);
+    check(p252_stealth_address_batch(e.get(), r, n, base_uv, publics_A, publics_B, n_public, R.data(), note_pk.data(),
+                                     ok.data(), nullptr, P252_MEM_HOST),
+          e.get());
+    return note_pk;
+}
+// one note; throws Error(P252_ERR_INVALID_POINT) for r >= r_J or a receiver key off the curve
+inline void stealth_address(const JubJubScalar& r, const Scalar (&base_uv)[2], const Scalar (&A_uv)[2], const Scalar (&B_uv)[2],
+                            Scalar (&R_uv)[2], Scalar (&note_pk_uv)[2], Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> R;
+    std::vector<uint8_t> ok;
+    const auto pk = stealth_address_batch(&r, 1, base_uv, A_uv, B_uv, 1, R, ok, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    R_uv[0] = R[0], R_uv[1] = R[1];
+    note_pk_uv[0] = pk[0], note_pk_uv[1] = pk[1];
+}
+// R and note_pk n x 2 scalars each; returns owned[i] (0 also for an invalid item); n_owned / n_invalid may be null
+inline std::vector<uint8_t> stealth_owns_batch(const JubJubScalar& view_a, const Scalar (&spend_B_uv)[2],
+                                               const Scalar (&base_uv)[2], const Scalar* R, const Scalar* note_pk, size_t n,
+                                               size_t* n_owned = nullptr, size_t* n_invalid = nullptr,
+                                               Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> owned(n, 0);
+    check(p252_stealth_owns_batch(e.get(), &view_a, spend_B_uv, base_uv, R, note_pk, n, owned.data(), n_owned, n_invalid,
+                                  P252_MEM_HOST),
+          e.get());
+    return owned;
+}
+// ViewKey::owns for one note; throws Error(P252_ERR_INVALID_POINT) for a view key >= r_J, an R off the curve or a
+// note_pk coordinate >= p
+inline bool owns(const JubJubScalar& view_a, const Scalar (&spend_B_uv)[2], const Scalar (&base_uv)[2], const Scalar (&R_uv)[2],
+                 const Scalar (&note_pk_uv)[2], Engine& e = Engine::default_engine()) {
+    size_t invalid = 0;
+    const auto owned = stealth_owns_batch(view_a, spend_B_uv, base_uv, R_uv, note_pk_uv, 1, nullptr, &invalid, e);
+    if (invalid) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    return owned[0] != 0;
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

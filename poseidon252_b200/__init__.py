@@ -7,7 +7,8 @@ plus the batch entry points this engine adds:
     encrypt_batch, decrypt_batch, encrypt_batch_varlen / decrypt_batch_varlen (messages of different lengths in one call),
     dhke / dhke_batch (JubJub key exchange), encrypt_batch_dhke / decrypt_batch_dhke (shared secret derived on the device),
     fixed_base / fixed_base_batch ([s] B for one base, e.g. public and ephemeral keys), encrypt_batch_ephemeral (the
-    sender: ephemeral keys and ciphers in one call),
+    sender: ephemeral keys and ciphers in one call), stealth_address / stealth_address_batch and owns /
+    stealth_owns_batch (stealth addresses: the sender's note keys and a view key's ownership scan),
     merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
     with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
@@ -15,7 +16,8 @@ All computation runs in hand-written sm_90a CUDA behind the C ABI in include/pos
 from . import hades, merkle, scalar
 from .encryption import (cipher_offsets, decrypt, decrypt_batch, decrypt_batch_dhke, decrypt_batch_varlen, dhke, dhke_batch,
                          encrypt, encrypt_batch, encrypt_batch_dhke, encrypt_batch_ephemeral, encrypt_batch_varlen,
-                         fixed_base, fixed_base_batch, message_offsets)
+                         fixed_base, fixed_base_batch, message_offsets, owns, stealth_address, stealth_address_batch,
+                         stealth_owns_batch)
 from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
@@ -27,7 +29,7 @@ HADES_WIDTH = hades.WIDTH
 __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch", "pack_varlen",
            "encrypt_batch_varlen", "decrypt_batch_varlen", "cipher_offsets", "message_offsets",
            "dhke", "dhke_batch", "encrypt_batch_dhke", "decrypt_batch_dhke", "fixed_base", "fixed_base_batch",
-           "encrypt_batch_ephemeral",
+           "encrypt_batch_ephemeral", "stealth_address", "stealth_address_batch", "owns", "stealth_owns_batch",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",

@@ -10,6 +10,7 @@
 //   encrypt / decrypt               src/encryption.rs:62-95 -> p252_encrypt_batch, p252_decrypt_batch
 //   dhke + encrypt / decrypt        src/encryption.rs:11-43 -> p252_dhke_batch, p252_{en,de}crypt_batch_dhke
 //   GENERATOR * r, the sender       src/encryption.rs:22-42 -> p252_fixed_base_batch, p252_encrypt_batch_ephemeral
+//   Phoenix stealth addresses (consumer, not the reference) -> p252_stealth_address_batch, p252_stealth_owns_batch
 //   Error                           src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -1040,6 +1041,102 @@ int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, si
     }
     if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
     return device_done(ctx, rc, flags);
+}
+
+// ---- stealth addresses: the sender's (R, note_pk) and the receiver's ownership scan ----------------------------------
+// hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0].  Sender: R = [r] G, note_pk = [hash([r] A)] G + B;
+// receiver (view key a, spend key B): owns <=> note_pk == [hash([a] R)] G + B.  Per chunk: launch_dhke into a slot arena
+// (the shared points and their validity), the truncated launch_digest of them into the arena (h), then launch_stealth_*
+// (the sender runs launch_fixed_base for R first).  r, view_a, the shared points and h live only in the slot arenas for
+// both memory spaces, so both calls are synchronous and the common exit join_slots(wipe) clears them on every path.
+static int stealth_tag(p252_fr* tag) { return p252_hash_tag(P252_DOMAIN_OTHER, 2, 1, tag); }
+
+int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, const p252_fr* base_uv, const p252_fr* A_uv,
+                               const p252_fr* B_uv, size_t n_public, p252_fr* R_uv, p252_fr* note_pk_uv, uint8_t* ok,
+                               size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, r, n, A_uv, n_public, {B_uv, R_uv, note_pk_uv}, ok, flags);
+    if (rc != P252_OK) return rc;
+    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = stealth_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    unsigned long long* counter = nullptr;
+    if (dev && n_invalid) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    // 0 r, 1 A, 2 B, 3 R, 4 note_pk, 5 ok; 6 shared points, 7 validity and 8 h live in the arena only
+    std::vector<Io> ios = {{r, nullptr, 32, false, dev}, {A_uv, nullptr, 64, pb, dev}, {B_uv, nullptr, 64, pb, dev},
+                           {nullptr, R_uv, 64, false, dev}, {nullptr, note_pk_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
+                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[5]);
+        uint8_t* valid = static_cast<uint8_t*>(d[7]);
+        cudaError_t e = p252::launch_fixed_base(d[0], cnt, table, d[3], okc, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_dhke(d[0], false, d[1], pb, cnt, d[6], valid, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st);
+        if (e == cudaSuccess) e = p252::launch_stealth_derive(d[8], cnt, table, d[2], pb, valid, d[3], d[4], okc, counter, st);
+        if (e == cudaSuccess) ctx->launches += 3;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    }, /*wipe=*/true);
+    if (!dev) {
+        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+        return rc;
+    }
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+    return device_done(ctx, rc, flags);
+}
+
+// The receiver's B is public and a HOST pointer, like the base: checked here, and its Niels form computed once on the host
+// and passed to the kernel by value.  An item's owned flag does not tell an invalid item from a note of someone else, so
+// both counts come from the device counters (0: owned, 1: invalid) for both memory spaces.
+int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p252_fr* spend_B_uv, const p252_fr* base_uv,
+                            const p252_fr* R_uv, const p252_fr* note_pk_uv, size_t n, uint8_t* owned, size_t* n_owned,
+                            size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv || !spend_B_uv) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, view_a, 1, R_uv, n, {note_pk_uv}, owned, flags);
+    if (rc != P252_OK) return rc;
+    if ((rc = base_check(base_uv)) != P252_OK || (rc = base_check(spend_B_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = stealth_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0;
+    if (n_owned) *n_owned = 0;
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    uint64_t nb[12];
+    p252::host::jubjub_niels(nb, spend_B_uv[0].l, spend_B_uv[1].l);
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    unsigned long long *c_owned = nullptr, *c_invalid = nullptr;
+    if (n_owned || n_invalid) {
+        if ((rc = counter_begin(ctx, 2)) != P252_OK) return rc;
+        c_owned = n_owned ? ctx->d_counter : nullptr;
+        c_invalid = n_invalid ? ctx->d_counter + 1 : nullptr;
+    }
+    // 0 view_a, 1 R, 2 note_pk, 3 owned; 4 shared points, 5 validity and 6 h live in the arena only
+    std::vector<Io> ios = {{view_a, nullptr, 32, true, dev}, {R_uv, nullptr, 64, false, dev}, {note_pk_uv, nullptr, 64, false, dev},
+                           {nullptr, owned, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* valid = static_cast<uint8_t*>(d[5]);
+        cudaError_t e = p252::launch_dhke(d[0], true, d[1], false, cnt, d[4], valid, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[4], cnt, 2, d[6], 1, true, ctx->coop_max, st);
+        if (e == cudaSuccess)
+            e = p252::launch_stealth_owns(d[6], cnt, table, nb, d[2], valid, static_cast<uint8_t*>(d[3]), c_owned, c_invalid, st);
+        if (e == cudaSuccess) ctx->launches += 2;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    }, /*wipe=*/true);
+    if (rc == P252_OK) rc = counter_end(ctx, n_owned, 0);
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
+    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
 }
 
 // ---- arity-4 Merkle tree ------------------------------------------------------------------------------

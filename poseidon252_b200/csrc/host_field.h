@@ -200,12 +200,13 @@ inline bool is_canonical(const uint64_t a[4]) {
     return bw != 0;
 }
 
+// d = -10240/10241 of JubJub, Montgomery
+static const uint64_t kD[4] = {0x2a522455b974f6b0ULL, 0xfc6cc9ef0d9acab3ULL, 0x7a08fb94c27628d1ULL, 0x57f8f6a8fe0e262eULL};
+
 // (u, v) (Montgomery limbs) is a JubJub point: u, v < p and -u^2 + v^2 == 1 + d u^2 v^2, d = -10240/10241
 inline bool jubjub_on_curve(const uint64_t u[4], const uint64_t v[4]) {
     static const uint64_t kOne[4] = {0x00000001fffffffeULL, 0x5884b7fa00034802ULL, 0x998c4fefecbc4ff5ULL,
                                      0x1824b159acc5056fULL};
-    static const uint64_t kD[4] = {0x2a522455b974f6b0ULL, 0xfc6cc9ef0d9acab3ULL, 0x7a08fb94c27628d1ULL,
-                                   0x57f8f6a8fe0e262eULL};
     if (!is_canonical(u) || !is_canonical(v)) return false;
     uint64_t uu[4], vv[4], lhs[4], w[4], rhs[4];
     mont_mul(uu, u, u);
@@ -215,6 +216,17 @@ inline bool jubjub_on_curve(const uint64_t u[4], const uint64_t v[4]) {
     mont_mul(rhs, w, kD);
     add_mod(rhs, rhs, kOne);
     return memcmp(lhs, rhs, sizeof lhs) == 0;
+}
+
+// The Niels form (v - u, v + u, 2d u v) of a JubJub point (u, v < p, Montgomery limbs): the addend of the device's
+// mixed addition (jubjub_device.cuh, madd), as out[0..4), out[4..8), out[8..12)
+inline void jubjub_niels(uint64_t out[12], const uint64_t u[4], const uint64_t v[4]) {
+    uint64_t d2[4], uv[4];
+    add_mod(d2, kD, kD);
+    sub_mod(out, v, u);
+    add_mod(out + 4, v, u);
+    mont_mul(uv, u, v);
+    mont_mul(out + 8, uv, d2);
 }
 
 // BlsScalar::from_bytes_wide: 64 LE bytes -> (lo + hi*2^256) mod p, Montgomery form

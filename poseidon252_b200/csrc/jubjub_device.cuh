@@ -354,11 +354,13 @@ __device__ __forceinline__ void select_niels(Niels& q, const uint4* tab, int w, 
     for (int k = 0; k < 8; ++k) q.kt[k] = (q.kt[k] & ~mn) | (nk[k] & mn);
 }
 
-// (ou, ov) = [s] B for s < 2^252 (canonical words) and the table of B (kFbTableWords uint4, built by fixed_base_entry).
-// kLdg: read the table through the read-only data path (a global table); otherwise plain loads (e.g. shared memory).
-template <bool kLdg>
-__device__ __forceinline__ void fixed_base_mul(uint32_t (&ou)[8], uint32_t (&ov)[8], const uint32_t (&s)[8],
-                                               const uint4* tab) {
+// t = [s] B in extended coordinates for s < 2^252 (canonical words) and the table of B (kFbTableWords uint4, built by
+// fixed_base_entry).  kLdg: read the table through the read-only data path (a global table); otherwise plain loads (e.g.
+// shared memory).  kLastT: the last window also computes T (64 x 7 products instead of 63 x 7 + 6), for a caller that
+// adds another point to the result; without it t.T is not the result's.  t is also the windows' temporary, as it was in
+// fixed_base_mul before the split, which keeps k_fixed_base's code unchanged.
+template <bool kLdg, bool kLastT>
+__device__ __forceinline__ void fixed_base_ext(Ext& t, const uint32_t (&s)[8], const uint4* tab) {
     Ext acc;
 #pragma unroll
     for (int k = 0; k < 8; ++k) acc.X[k] = 0, acc.T[k] = 0;
@@ -367,7 +369,6 @@ __device__ __forceinline__ void fixed_base_mul(uint32_t (&ou)[8], uint32_t (&ov)
     uint32_t d[8], carry = 0;
     fcopy(d, s);
     Niels q;
-    Ext t;
 #pragma unroll 1
     for (int w = 0; w < kFbWindows - 1; ++w) {
         select_niels<kLdg>(q, tab, w, recode_digit(d, carry));
@@ -375,11 +376,41 @@ __device__ __forceinline__ void fixed_base_mul(uint32_t (&ou)[8], uint32_t (&ov)
         acc = t;
     }
     select_niels<kLdg>(q, tab, kFbWindows - 1, recode_digit(d, carry));
-    madd<false>(t, acc, q);
+    madd<kLastT>(t, acc, q);
+}
+
+// (ou, ov) = [s] B, affine: fixed_base_ext without the last T, one inversion
+template <bool kLdg>
+__device__ __forceinline__ void fixed_base_mul(uint32_t (&ou)[8], uint32_t (&ov)[8], const uint32_t (&s)[8],
+                                               const uint4* tab) {
+    Ext t;
+    fixed_base_ext<kLdg, false>(t, s, tab);
     uint32_t zi[8];
     inverse(zi, t.Z);
     fmul(ou, t.X, zi);
     fmul(ov, t.Y, zi);
+}
+
+// ---- stealth addresses: note_pk = [h] G + B (p252_stealth_address_batch / p252_stealth_owns_batch) -------------------
+// h = hash([r] A) = hash([a] R) < 2^250 comes from the truncated digest; [h] G is fixed_base_ext with T in every window,
+// then one mixed addition of B in Niels form.
+//   owns:   B's Niels form is precomputed on the host; the result is compared projectively with note_pk, X == u Z and
+//           Y == v Z (no inversion).
+//   derive: B is read per item: on-curve check 4, Niels form 2 (u v, 2d u v); then the inversion and the affine
+//           conversion.
+constexpr int kProductsPerStealthOwns = kFbWindows * 7 + 6 + 2;
+constexpr int kProductsPerStealthDerive = kFbWindows * 7 + 4 + 2 + 6 + (kPm2Bits - 1) + (kPm2Ones - 1) + 2;
+static_assert(kProductsPerStealthOwns == 456, "product count of DESIGN.md section 4");
+static_assert(kProductsPerStealthDerive == 879, "product count of DESIGN.md section 4");
+
+// The Niels form (v - u, v + u, 2d u v) of an affine (u, v), u, v < p: 2 products
+__device__ __forceinline__ void to_niels(Niels& q, const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+    uint32_t uv[8], k[8];
+    fr_sub_mod(q.ymx, v, u);
+    fr_add_mod(q.ypx, v, u);
+    fmul(uv, u, v);
+    set_2d(k);
+    fmul(q.kt, uv, k);
 }
 
 // Table entry (w, j), j in 1..8, of the base (u, v) (on the curve, u, v < p): j 16^w (u, v) by 4w doublings and j - 1

@@ -8,6 +8,7 @@
 //   encrypt/decrypt  src/encryption.rs:62-95  -> k_crypt (k_crypt_varlen: messages of any lengths)
 //   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
 //   dhke             src/encryption.rs:11-43  -> k_dhke (JubJub scalar multiplication, jubjub_device.cuh)
+//   stealth addresses (note_pk = [hash(shared)] G + B) -> k_stealth
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
 #include "kernels.h"
@@ -1561,6 +1562,125 @@ cudaError_t launch_fixed_base(const void* secret, size_t n, const void* table, v
     if (n == 0) return cudaSuccess;
     k_fixed_base<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(secret), n, static_cast<const uint4*>(table),
                                                    static_cast<uint8_t*>(out_uv), ok, n_invalid);
+    return cudaGetLastError();
+}
+
+// ---- stealth addresses: note_pk = [h] G + B, h = hash([r] A) = hash([a] R) (jubjub_device.cuh) ------------------------
+struct NielsArg {                // the receiver's B in Niels form (v - u, v + u, 2d u v), Montgomery, passed by value
+    uint32_t w[24];
+};
+
+// *counter += the lanes of the warp with `hit`: one atomic per warp whatever the flags, so that not even the count's
+// bookkeeping branches on an item's result
+__device__ __forceinline__ void warp_count_every(unsigned long long* counter, bool hit) {
+    const unsigned act = __activemask();
+    const unsigned b = __ballot_sync(act, hit);
+    if ((threadIdx.x & 31) == (unsigned)(__ffs(act) - 1)) atomicAdd(counter, (unsigned long long)__popc(b));
+}
+
+// One thread per item.  h[i]: the truncated digest of the item's shared point (raw limbs < 2^250); valid[i]: the validity
+// k_dhke gave that point.  Every item runs the same schedule: invalid operands are replaced by the identity or zero.
+//   kOwns (the receiver, 456 products): pk = the note keys (read); flag[i] = owned = valid[i], both note_pk coordinates
+//     < p and note_pk == [h] G + nb, compared projectively.  cnt_a += owned, cnt_b += invalid.
+//   derive (the sender, 879 products): B_uv[bb ? 0 : i] is B (read); pk = the note keys (written); flag[i] = ok = valid[i]
+//     and B a curve point with u, v < p.  An item with ok = 0 gets a zeroed note_pk row and a zeroed R row (R as written
+//     by k_fixed_base).  cnt_a += invalid.
+template <bool kOwns>
+__global__ void __launch_bounds__(kThreads, 3) k_stealth(const uint8_t* __restrict__ h, size_t n, const uint4* __restrict__ table,
+                                                      NielsArg nb, const uint8_t* __restrict__ B_uv, bool bb,
+                                                      const uint8_t* __restrict__ valid, uint8_t* pk, uint8_t* R_uv,
+                                                      uint8_t* __restrict__ flag, unsigned long long* __restrict__ cnt_a,
+                                                      unsigned long long* __restrict__ cnt_b) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    // The point operand is loaded twice (derive: its check runs before [h] G, its Niels form after) so that during the
+    // 64 windows of [h] G nothing but the scalar and a flag is live.  Coordinates >= p enter no product: they are
+    // replaced first (derive: by the identity (0, 1)).
+    uint32_t u[8], v[8], one[8];
+    jj::set_one(one);
+    const uint8_t* pt = kOwns ? pk + i * 64 : B_uv + (bb ? 0 : i) * 64;
+    auto load_point = [&](bool& canon) {
+        load_fr(u, pt);
+        load_fr(v, pt + 32);
+        canon = fr_is_canonical(u) & fr_is_canonical(v);
+        const uint32_t mc = 0u - (uint32_t)canon;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] = (v[k] & mc) | (kOwns ? 0u : one[k] & ~mc);
+    };
+    bool good = valid[i] != 0, canon;
+    if (!kOwns) {
+        load_point(canon);
+        good &= canon & jj::on_curve(u, v);
+    }
+    jj::Ext t, r;
+    {
+        uint32_t s[8];
+        load_fr(s, h + i * 32);
+        jj::fixed_base_ext<true, true>(t, s, table);
+    }
+    load_point(canon);
+    jj::Niels q;
+    if (kOwns) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) q.ymx[k] = nb.w[k], q.ypx[k] = nb.w[8 + k], q.kt[k] = nb.w[16 + k];
+        good &= canon;
+    } else {
+        const uint32_t mo = 0u - (uint32_t)good;   // an item that is not valid adds the identity: B is on the curve
+#pragma unroll
+        for (int k = 0; k < 8; ++k) u[k] &= mo, v[k] = (v[k] & mo) | (one[k] & ~mo);
+        jj::to_niels(q, u, v);
+    }
+    jj::madd<false>(r, t, q);
+    if (kOwns) {
+        uint32_t x[8], y[8];
+        jj::fmul(x, u, r.Z);
+        jj::fmul(y, v, r.Z);
+        const bool owned = good & jj::feq(x, r.X) & jj::feq(y, r.Y);
+        flag[i] = owned ? 1 : 0;
+        if (cnt_a) warp_count_every(cnt_a, owned);
+        if (cnt_b) warp_count_every(cnt_b, !good);
+    } else {
+        uint32_t zi[8], ou[8], ov[8];
+        jj::inverse(zi, r.Z);
+        jj::fmul(ou, r.X, zi);
+        jj::fmul(ov, r.Y, zi);
+        const uint32_t m = 0u - (uint32_t)good;
+        uint32_t ru[8], rv[8];
+        load_fr_rw(ru, R_uv + i * 64);
+        load_fr_rw(rv, R_uv + i * 64 + 32);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m, ru[k] &= m, rv[k] &= m;
+        store_fr(pk + i * 64, ou);
+        store_fr(pk + i * 64 + 32, ov);
+        store_fr(R_uv + i * 64, ru);
+        store_fr(R_uv + i * 64 + 32, rv);
+        flag[i] = good ? 1 : 0;
+        if (cnt_a) warp_count_every(cnt_a, !good);
+    }
+}
+
+cudaError_t launch_stealth_owns(const void* h, size_t n, const void* table, const uint64_t b_niels[12], const void* note_pk,
+                                const uint8_t* valid, uint8_t* owned, unsigned long long* n_owned,
+                                unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    NielsArg nb;
+    for (int k = 0; k < 12; ++k) nb.w[2 * k] = (uint32_t)b_niels[k], nb.w[2 * k + 1] = (uint32_t)(b_niels[k] >> 32);
+    k_stealth<true><<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), n, static_cast<const uint4*>(table), nb,
+                                                      nullptr, false, valid,
+                                                      const_cast<uint8_t*>(static_cast<const uint8_t*>(note_pk)), nullptr,
+                                                      owned, n_owned, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, const void* B_uv, bool B_bcast,
+                                  const uint8_t* valid, void* R_uv, void* note_pk, uint8_t* ok, unsigned long long* n_invalid,
+                                  cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    NielsArg nb = {};
+    k_stealth<false><<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), n, static_cast<const uint4*>(table), nb,
+                                                       static_cast<const uint8_t*>(B_uv), B_bcast, valid,
+                                                       static_cast<uint8_t*>(note_pk), static_cast<uint8_t*>(R_uv), ok,
+                                                       n_invalid, nullptr);
     return cudaGetLastError();
 }
 

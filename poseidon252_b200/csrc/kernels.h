@@ -139,6 +139,19 @@ constexpr size_t kFixedBaseTableBytes = 64 * 8 * 96;
 cudaError_t launch_fixed_base_table(const uint64_t base_uv[8], void* table, cudaStream_t st);
 cudaError_t launch_fixed_base(const void* secret, size_t n, const void* table, void* out_uv, uint8_t* ok,
                               unsigned long long* n_invalid, cudaStream_t st);
+// Stealth addresses (p252_stealth_address_batch / p252_stealth_owns_batch), one thread per item: h[i] is the truncated
+// digest of the item's shared point (4 x u64 < 2^250), valid[i] its validity from launch_dhke, table the fixed-base table
+// of G.  Counters are device pointers and may be null.
+// owns: owned[i] = valid[i], both coordinates of note_pk[i] < p and note_pk[i] == [h[i]] G + B, with B given in Niels
+// form b_niels = (v - u, v + u, 2d u v), 3 x 4 u64 Montgomery limbs; *n_owned += owned items, *n_invalid += invalid ones
+cudaError_t launch_stealth_owns(const void* h, size_t n, const void* table, const uint64_t b_niels[12], const void* note_pk,
+                                const uint8_t* valid, uint8_t* owned, unsigned long long* n_owned,
+                                unsigned long long* n_invalid, cudaStream_t st);
+// derive: note_pk[i] = [h[i]] G + B_uv[B_bcast ? 0 : i]; ok[i] = valid[i] and B a curve point with u, v < p.  An item
+// with ok = 0 gets a zeroed note_pk row and a zeroed R_uv row and is counted into *n_invalid
+cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, const void* B_uv, bool B_bcast,
+                                  const uint8_t* valid, void* R_uv, void* note_pk, uint8_t* ok, unsigned long long* n_invalid,
+                                  cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -116,6 +116,51 @@ def encrypt_batch_ephemeral(messages, r, base, publics, nonces, engine=None, out
     return eng.encrypt_batch_ephemeral(messages, r, base, publics, nonces, out=out, async_=async_)
 
 
+def _jscalar_row(secret):
+    if isinstance(secret, (int, np.integer)):
+        return jubjub_limbs([secret])
+    return np.ascontiguousarray(secret, dtype=np.uint64).reshape(1, 4)
+
+
+def stealth_address(r, base, A, B, engine=None):
+    """NEW: one stealth address, the sender's PublicKey::gen_stealth_address: R = [r] base and
+    note_pk = [hash([r] A)] base + B, hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0].  r: a canonical int
+    < r_J or one p252_jscalar row; base, A, B: (2, 4) BlsScalar.0 limbs -> (R (2, 4), note_pk (2, 4)).  Raises
+    InvalidPoint for r >= r_J or a point off the curve."""
+    eng = engine or default_engine()
+    pt = lambda x: np.ascontiguousarray(x, dtype=np.uint64).reshape(1, 2, 4)   # noqa: E731
+    R, pk, ok = eng.stealth_address_batch(_jscalar_row(r), base, pt(A), pt(B))
+    if not ok[0]:
+        raise InvalidPoint()
+    return R[0], pk[0]
+
+
+def stealth_address_batch(r, base, publics_A, publics_B, engine=None, async_=False):
+    """NEW: n stealth addresses.  r (n, 4) p252_jscalar rows, base (2, 4), publics_A / publics_B (1 or n, 2, 4)
+    -> (R (n, 2, 4), note_pk (n, 2, 4), ok (n,) uint8); ok == 0 marks an invalid item, whose rows are zeroed."""
+    eng = engine or default_engine(r.device.index if hasattr(r, "is_cuda") else 0)
+    return eng.stealth_address_batch(r, base, publics_A, publics_B, async_=async_)
+
+
+def owns(view_a, spend_B, base, R, note_pk, engine=None):
+    """NEW: ViewKey::owns for one note: note_pk == [hash([view_a] R)] base + spend_B -> bool.  view_a: a canonical int
+    < r_J or one p252_jscalar row; spend_B, base, R, note_pk: (2, 4) BlsScalar.0 limbs.  Raises InvalidPoint for
+    view_a >= r_J, R off the curve, a note_pk coordinate >= p, or spend_B or base off the curve."""
+    eng = engine or default_engine()
+    pt = lambda x: np.ascontiguousarray(x, dtype=np.uint64).reshape(1, 2, 4)   # noqa: E731
+    owned = eng.stealth_owns_batch(_jscalar_row(view_a), spend_B, base, pt(R), pt(note_pk))
+    if eng.last_stealth_invalid():
+        raise InvalidPoint()
+    return bool(owned[0])
+
+
+def stealth_owns_batch(view_a, spend_B, base, R, note_pk, engine=None, async_=False):
+    """NEW: a wallet's scan with one view key: owned[i] = note_pk[i] == [hash([view_a] R[i])] base + spend_B.
+    view_a (1, 4), R and note_pk (n, 2, 4), spend_B and base (2, 4) -> owned (n,) uint8 (0 also for an invalid item)."""
+    eng = engine or default_engine(R.device.index if hasattr(R, "is_cuda") else 0)
+    return eng.stealth_owns_batch(view_a, spend_B, base, R, note_pk, async_=async_)
+
+
 def cipher_offsets(offsets):
     """Offsets of the ciphers of messages at `offsets` (each one scalar longer, packed from 0): offsets - offsets[0] + i.
     Works on numpy arrays and CUDA tensors (no host sync)."""

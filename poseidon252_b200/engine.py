@@ -471,6 +471,67 @@ class Engine:
                                                            ctypes.byref(self._ninv), flags))
         return res, R, ok
 
+    # -- stealth addresses ------------------------------------------------------------------------
+    def stealth_address_batch(self, r, base, publics_A, publics_B, R_out=None, out=None, async_=False):
+        """The sender's stealth addresses: R_i = [r_i] base and note_pk_i = [hash([r_i] A_i)] base + B_i, where
+        hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0].  r (n, 4) p252_jscalar rows, base (2, 4)
+        (host-read, as in fixed_base_batch), publics_A and publics_B (1 or n, 2, 4) with the same number of rows: the
+        receiver's public key (A, B) -> (R (n, 2, 4), note_pk (n, 2, 4), ok (n,) uint8).  An item with r >= r_J or A or B
+        not a curve point has ok == 0 and zeroed R and note_pk rows (count: last_stealth_invalid())."""
+        if len(tuple(r.shape)) != 2:
+            raise EngineError(-1, "r must have shape (n, 4)")
+        n = int(r.shape[0])
+        sp, _, ap, na, _, flags, keep = self._dhke_args(r, publics_A, n)
+        bp, bl, fb, bk = self._in(publics_B, (2, 4))
+        if fb != flags:
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        if tuple(bl) != (na,):
+            raise EngineError(-1, "publics_B must have %d rows like publics_A, got leading shape %s" % (na, tuple(bl)))
+        b = self._base(base)
+        like = keep[0]
+        R = self._out_like(like, (n, 2, 4)) if R_out is None else self._check_out(R_out, (n, 2, 4), like)
+        pk = self._out_like(like, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), like)
+        ok = self._ok_like(like, n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nsinv = self._counter(flags)
+        self._check(self._lib.p252_stealth_address_batch(self._ctx, sp, n, b.ctypes.data, ap, bp, na, self._ptr(R),
+                                                         self._ptr(pk), self._ptr(ok), ctypes.byref(self._nsinv), flags))
+        return R, pk, ok
+
+    def stealth_owns_batch(self, view_a, spend_B, base, R, note_pk, out=None, async_=False):
+        """The receiver's scan, ViewKey::owns over a batch of notes: owned[i] = note_pk[i] == [hash([view_a] R[i])] base +
+        spend_B.  view_a: one p252_jscalar row (1, 4) in the memory space of R and note_pk (n, 2, 4); spend_B and base
+        (2, 4) are host-read, as the base of fixed_base_batch -> owned (n,) uint8.  An item with view_a >= r_J, R not a
+        curve point or a note_pk coordinate >= p is invalid: owned == 0, counted in last_stealth_invalid(), not in
+        last_stealth_owned().  A spend_B or base off the curve raises InvalidPoint."""
+        rp, rl, flags, rk = self._in(R, (2, 4))
+        if len(rl) != 1:
+            raise EngineError(-1, "R must have shape (n, 2, 4)")
+        n = rl[0]
+        pp, pl, fp, pk = self._in(note_pk, (2, 4))
+        vp, vl, fv, vk = self._in(view_a, (4,))
+        if not (flags == fp == fv):
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_lead("note_pk", pl, n)
+        if tuple(vl) not in ((), (1,)):
+            raise EngineError(-1, "view_a must be one p252_jscalar row, got leading shape %s" % (tuple(vl),))
+        b, g = self._base(spend_B), self._base(base)
+        owned = self._ok_like(rk, n) if out is None else self._check_out(out, (n,), rk, itemsize=1)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nowned, self._nsinv = self._counter(flags), self._counter(flags)
+        self._check(self._lib.p252_stealth_owns_batch(self._ctx, vp, b.ctypes.data, g.ctypes.data, rp, pp, n,
+                                                      self._ptr(owned), ctypes.byref(self._nowned),
+                                                      ctypes.byref(self._nsinv), flags))
+        return owned
+
+    def last_stealth_owned(self):
+        """Owned notes of the last stealth_owns_batch (sync() first after async_)."""
+        return int(getattr(self, "_nowned", ctypes.c_size_t(0)).value)
+
+    def last_stealth_invalid(self):
+        """Invalid items of the last stealth_address_batch or stealth_owns_batch (sync() first after async_)."""
+        return int(getattr(self, "_nsinv", ctypes.c_size_t(0)).value)
+
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
         max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries
