@@ -128,6 +128,10 @@ mod fixed_base;
 // (methods on Engine).
 mod stealth;
 
+// Schnorr signatures over JubJub (signing and verification with the Poseidon challenge): their own `extern "C"` block in
+// schnorr.rs (methods on Engine).
+mod schnorr;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

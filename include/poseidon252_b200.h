@@ -346,6 +346,39 @@ int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p25
                             const p252_fr* R_uv, const p252_fr* note_pk_uv, size_t n, uint8_t* owned, size_t* n_owned,
                             size_t* n_invalid, int flags);
 
+/* ---- Schnorr signatures over JubJub (jubjub-schnorr's SecretKey::sign / PublicKey::verify) -------------------------
+ *   challenge(R, m) = Hash::digest_truncated(Domain::Other, [R.u, R.v, m])[0]          (R affine; c < 2^250 < r_J)
+ *   sign   (sk, r; m):        R = [r] G,  c = challenge(R, m),  u = (r - c sk) mod r_J,  signature = (u, R)
+ *   verify (PK; (u, R), m):   ok  <=>  [u] G + [c] PK == R,  c = challenge(R, m)
+ * PK = [sk] G.  Both scalar multiplications multiply by the canonical integer; there is no subgroup check (a torsion
+ * component of PK passes through, as in p252_dhke_batch).  Scalars (sk, r, u) are p252_jscalar, points (u, v) pairs of
+ * p252_fr, messages p252_fr, all laid out as for p252_dhke_batch.  base_uv (G) is a HOST pointer for every memory space,
+ * as in p252_fixed_base_batch: a coordinate >= p or a point off the curve is refused with P252_ERR_INVALID_POINT before
+ * anything runs, for every memory space and for n == 0.
+ * r is one nonce per item; there is no broadcast on purpose.  The nonce must be secret, uniformly random and never used
+ * twice: two signatures with the same sk and r on different messages reveal sk = (u1 - u2) / (c2 - c1) mod r_J.
+ * Item validity (checked on the device, for both memory spaces):
+ *   sign:   sk < r_J, r < r_J, msg < p.  An invalid item gets ok[i] = 0, a zeroed u row and a zeroed R row, and is counted
+ *           once into *n_invalid.
+ *   verify: u < r_J, msg < p, both coordinates of R < p, and PK a curve point with u, v < p (per item, also for
+ *           n_public == 1).  An invalid item gets verified[i] = 0 and is counted into *n_invalid, not *n_verified.  An R
+ *           with canonical coordinates off the curve is simply not verified (the projective equality implies R on the curve).
+ * n_verified / n_invalid: optional HOST pointers for both memory spaces (lifetime as for p252_decrypt_batch).
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_secret / n_public not 1 or n, DEVICE buffers other than
+ * ok / verified not 16-byte aligned -> INVALID_ARGUMENT.
+ * Signing: sk and r live only in the context's staging arenas, for both memory spaces, and the arenas are zeroed on every
+ * exit path: the call is synchronous (P252_ASYNC only defers the publication of *n_invalid to p252_sync).  Each item is
+ * constant time (no branch and no address depends on sk or r); see DESIGN.md section 4.  Verification reads public data
+ * only; as for p252_stealth_owns_batch, P252_ASYNC defers the publication of the counts to p252_sync. */
+/* u[i], R_uv[i] = sign(sk[n_secret == 1 ? 0 : i], r[i]; msg[i]) */
+int p252_schnorr_sign_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_jscalar* r,
+                            const p252_fr* msg, size_t n, const p252_fr* base_uv, p252_jscalar* u_out, p252_fr* R_uv,
+                            uint8_t* ok, size_t* n_invalid, int flags);
+/* verified[i] = verify(pk_uv[n_public == 1 ? 0 : i]; (u[i], R_uv[i]), msg[i]) */
+int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_jscalar* u,
+                              const p252_fr* R_uv, const p252_fr* msg, size_t n, const p252_fr* base_uv,
+                              uint8_t* verified, size_t* n_verified, size_t* n_invalid, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

@@ -10,7 +10,8 @@
 //   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
 //   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
 //   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
-//   stealth_address_batch, owns / stealth_owns_batch, merkle4_build.
+//   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
+//   schnorr_verify_batch, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -391,6 +392,55 @@ inline bool owns(const JubJubScalar& view_a, const Scalar (&spend_B_uv)[2], cons
     const auto owned = stealth_owns_batch(view_a, spend_B_uv, base_uv, R_uv, note_pk_uv, 1, nullptr, &invalid, e);
     if (invalid) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
     return owned[0] != 0;
+}
+
+// NEW: Schnorr signatures over JubJub (p252_schnorr_sign_batch / p252_schnorr_verify_batch), jubjub-schnorr's
+// SecretKey::sign / PublicKey::verify: R = [r] G, u = (r - c sk) mod r_J with c = challenge(R, m) =
+// Hash::digest_truncated(Domain::Other, [R.u, R.v, m])[0]; verified iff [u] G + [c] PK == R.  base_uv is the caller's G;
+// a G off the curve throws Error(P252_ERR_INVALID_POINT).  r is one fresh secret nonce per message (never reused).
+// sk holds 1 or n keys (n_secret); returns the n scalars u; R receives n x 2 scalars; ok[i] == 0 marks an invalid item
+inline std::vector<JubJubScalar> schnorr_sign_batch(const JubJubScalar* sk, size_t n_secret, const JubJubScalar* r,
+                                                    const Scalar* msg, size_t n, const Scalar (&base_uv)[2],
+                                                    std::vector<Scalar>& R, std::vector<uint8_t>& ok,
+                                                    Engine& e = Engine::default_engine()) {
+    std::vector<JubJubScalar> u(n);
+    R.assign(2 * n, Scalar{});
+    ok.assign(n, 0);
+    check(p252_schnorr_sign_batch(e.get(), sk, n_secret, r, msg, n, base_uv, u.data(), R.data(), ok.data(), nullptr,
+                                  P252_MEM_HOST),
+          e.get());
+    return u;
+}
+// one signature (u, R); throws Error(P252_ERR_INVALID_POINT) for sk or r >= r_J or msg >= p
+inline void schnorr_sign(const JubJubScalar& sk, const JubJubScalar& r, const Scalar& msg, const Scalar (&base_uv)[2],
+                         JubJubScalar& u, Scalar (&R_uv)[2], Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> R;
+    std::vector<uint8_t> ok;
+    const auto us = schnorr_sign_batch(&sk, 1, &r, &msg, 1, base_uv, R, ok, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    u = us[0];
+    R_uv[0] = R[0], R_uv[1] = R[1];
+}
+// pk holds 1 or n points (n_public), R n x 2 scalars; returns verified[i] (0 also for an invalid item); n_verified /
+// n_invalid may be null
+inline std::vector<uint8_t> schnorr_verify_batch(const Scalar* pk, size_t n_public, const JubJubScalar* u, const Scalar* R,
+                                                 const Scalar* msg, size_t n, const Scalar (&base_uv)[2],
+                                                 size_t* n_verified = nullptr, size_t* n_invalid = nullptr,
+                                                 Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> verified(n, 0);
+    check(p252_schnorr_verify_batch(e.get(), pk, n_public, u, R, msg, n, base_uv, verified.data(), n_verified, n_invalid,
+                                    P252_MEM_HOST),
+          e.get());
+    return verified;
+}
+// PublicKey::verify for one signature; throws Error(P252_ERR_INVALID_POINT) for u >= r_J, msg >= p, an R coordinate
+// >= p or a key off the curve
+inline bool schnorr_verify(const Scalar (&pk_uv)[2], const JubJubScalar& u, const Scalar (&R_uv)[2], const Scalar& msg,
+                           const Scalar (&base_uv)[2], Engine& e = Engine::default_engine()) {
+    size_t invalid = 0;
+    const auto verified = schnorr_verify_batch(pk_uv, 1, &u, R_uv, &msg, 1, base_uv, nullptr, &invalid, e);
+    if (invalid) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    return verified[0] != 0;
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

@@ -88,6 +88,10 @@ SIGNATURES = {
                                            c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_stealth_owns_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
                                         ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t), c_int]),
+    "p252_schnorr_sign_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p,
+                                        c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_schnorr_verify_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p,
+                                          c_void_p, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t), c_int]),
 }
 
 MEM_HOST, MEM_DEVICE, ASYNC, TIMING, NO_GATHER = 0, 1, 2, 4, 8

@@ -11,7 +11,8 @@
 //   dhke + encrypt / decrypt        src/encryption.rs:11-43 -> p252_dhke_batch, p252_{en,de}crypt_batch_dhke
 //   GENERATOR * r, the sender       src/encryption.rs:22-42 -> p252_fixed_base_batch, p252_encrypt_batch_ephemeral
 //   Phoenix stealth addresses (consumer, not the reference) -> p252_stealth_address_batch, p252_stealth_owns_batch
-//   Error                           src/error.rs:11-44      -> p252_status
+//   jubjub-schnorr sign / verify (consumer, not the reference) -> p252_schnorr_sign_batch, p252_schnorr_verify_batch
+//   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
@@ -1135,6 +1136,100 @@ int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p25
         return e;
     }, /*wipe=*/true);
     if (rc == P252_OK) rc = counter_end(ctx, n_owned, 0);
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
+    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
+}
+
+// ---- Schnorr signatures over JubJub: signing and verification ----------------------------------------------------------
+// challenge(R, m) = Hash::digest_truncated(Domain::Other, [R.u, R.v, m])[0].  Sign: R = [r] G, u = (r - c sk) mod r_J;
+// verify: [u] G + [c] PK == R.  Per chunk: launch_schnorr_pack writes the rows [R.u, R.v, m] into a slot arena, the
+// truncated launch_digest of them gives c into the arena, then launch_schnorr_sign / launch_schnorr_verify (the signer runs
+// launch_fixed_base for R first).  Signing stages sk and r only in the slot arenas (DEVICE buffers are used in place), so
+// it is synchronous and the common exit join_slots(wipe) clears them on every path; verification reads public data only.
+static int schnorr_tag(p252_fr* tag) { return p252_hash_tag(P252_DOMAIN_OTHER, 3, 1, tag); }
+
+int p252_schnorr_sign_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_jscalar* r, const p252_fr* msg,
+                            size_t n, const p252_fr* base_uv, p252_jscalar* u_out, p252_fr* R_uv, uint8_t* ok, size_t* n_invalid,
+                            int flags) {
+    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, r, n, sk, n_secret, {msg, u_out, R_uv}, ok, flags);
+    if (rc != P252_OK) return rc;
+    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = schnorr_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    unsigned long long* counter = nullptr;
+    if (dev && n_invalid) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    // 0 sk, 1 r, 2 msg, 3 u, 4 R, 5 ok; 6 the digest rows and 7 c live in the arena only
+    std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev},
+                           {nullptr, u_out, 32, false, dev}, {nullptr, R_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
+                           {nullptr, nullptr, 96}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[5]);
+        cudaError_t e = p252::launch_fixed_base(d[1], cnt, table, d[4], okc, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_schnorr_pack(d[4], d[2], cnt, d[6], okc, true, st);
+        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[6], cnt, 3, d[7], 1, true, ctx->coop_max, st);
+        if (e == cudaSuccess) e = p252::launch_schnorr_sign(d[0], sb, d[1], d[7], cnt, d[3], d[4], okc, counter, st);
+        if (e == cudaSuccess) ctx->launches += 3;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    }, /*wipe=*/true);
+    if (!dev) {
+        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+        return rc;
+    }
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+    return device_done(ctx, rc, flags);
+}
+
+// An item's verified flag does not tell an invalid item from a signature that does not verify, so both counts come from
+// the device counters (0: verified, 1: invalid) for both memory spaces.  Nothing here is secret: no wipe.
+int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_jscalar* u, const p252_fr* R_uv,
+                              const p252_fr* msg, size_t n, const p252_fr* base_uv, uint8_t* verified, size_t* n_verified,
+                              size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, u, n, pk_uv, n_public, {R_uv, msg}, verified, flags);
+    if (rc != P252_OK) return rc;
+    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = schnorr_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    if (n_verified) *n_verified = 0;
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    unsigned long long *c_ok = nullptr, *c_bad = nullptr;
+    if (n_verified || n_invalid) {
+        if ((rc = counter_begin(ctx, 2)) != P252_OK) return rc;
+        c_ok = n_verified ? ctx->d_counter : nullptr;
+        c_bad = n_invalid ? ctx->d_counter + 1 : nullptr;
+    }
+    // 0 PK, 1 u, 2 R, 3 msg, 4 verified; 5 the digest rows, 6 validity and 7 c live in the arena only
+    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev}, {R_uv, nullptr, 64, false, dev},
+                           {msg, nullptr, 32, false, dev}, {nullptr, verified, 1, false, dev}, {nullptr, nullptr, 96},
+                           {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* valid = static_cast<uint8_t*>(d[6]);
+        cudaError_t e = p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st);
+        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st);
+        if (e == cudaSuccess)
+            e = p252::launch_schnorr_verify(d[0], pb, d[1], d[2], d[7], valid, cnt, table, static_cast<uint8_t*>(d[4]), c_ok,
+                                            c_bad, st);
+        if (e == cudaSuccess) ctx->launches += 2;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    });
+    if (rc == P252_OK) rc = counter_end(ctx, n_verified, 0);
     if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
     return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
 }

@@ -211,12 +211,45 @@ __device__ __forceinline__ void inverse(uint32_t (&r)[8], const uint32_t (&z)[8]
     }
 }
 
-// (ou, ov) = [s] (u, v) for s < 2^252 (canonical words) and an on-curve (u, v) with u, v < p (Montgomery).
-// Fixed 4-bit window, most significant first: 63 x (4 doublings + 1 addition of tab[digit]), then one inversion.
-__device__ __forceinline__ void scalar_mul(uint32_t (&ou)[8], uint32_t (&ov)[8], const uint32_t (&s)[8],
-                                           const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+// c = tab[digit] for a PUBLIC digit: one entry read at the digit's address (8 loads instead of 16 x 8 masked ones)
+__device__ __forceinline__ void load_entry(Cached& c, const Entry& e) {
+    uint32_t* dst[4] = {c.ymx, c.ypx, c.kt, c.z2};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const uint4 a = e.w[2 * q], b = e.w[2 * q + 1];
+        dst[q][0] = a.x, dst[q][1] = a.y, dst[q][2] = a.z, dst[q][3] = a.w;
+        dst[q][4] = b.x, dst[q][5] = b.y, dst[q][6] = b.z, dst[q][7] = b.w;
+    }
+}
+
+// One window of the walk, most significant first: acc = 16 acc + tab[digit w of s], 3 x 7 + 8 + 7 products (8 with
+// kWantT).  kPublic: the digit indexes the table directly (load_entry); otherwise every entry is read (select_entry).
+template <bool kPublic, bool kWantT>
+__device__ __forceinline__ void window_step(Ext& acc, Cached& c, const Entry (&tab)[16], const uint32_t (&s)[8], int w) {
+    uint32_t limb = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) limb = (k == (w >> 3)) ? s[k] : limb;   // w is the public loop counter
+    const uint32_t digit = (limb >> ((w & 7) * 4)) & 15u;
+    Ext t;
+    dbl<false>(t, acc);
+    dbl<false>(acc, t);
+    dbl<false>(t, acc);
+    dbl<true>(acc, t);
+    if (kPublic)
+        load_entry(c, tab[digit]);
+    else
+        select_entry(c, tab, digit);
+    add<kWantT>(t, acc, c);
+    acc = t;
+}
+
+// acc = [s] (u, v) in extended coordinates for s < 2^252 (canonical words) and an on-curve (u, v) with u, v < p
+// (Montgomery).  Fixed 4-bit window: the 16-entry table of (u, v) in thread-local memory, then 63 window_steps.
+// kPublic: s is public (signature verification), so each window reads only its entry; a secret s (the key exchange)
+// must not, and reads all 16.  kLastT: the last window also computes T, for a caller that adds another point to acc.
+template <bool kPublic, bool kLastT>
+__device__ __forceinline__ void scalar_mul_ext(Ext& acc, const uint32_t (&s)[8], const uint32_t (&u)[8], const uint32_t (&v)[8]) {
     Entry tab[16];
-    Ext acc;
     Cached c;
     // tab[0] = identity (0 : 1 : 1 : 0) cached = (1, 1, 0, 2)
     set_one(c.ymx);
@@ -248,20 +281,15 @@ __device__ __forceinline__ void scalar_mul(uint32_t (&ou)[8], uint32_t (&ov)[8],
     set_one(acc.Y);
     set_one(acc.Z);
 #pragma unroll 1
-    for (int w = kWindows - 1; w >= 0; --w) {
-        uint32_t limb = 0;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) limb = (k == (w >> 3)) ? s[k] : limb;   // w is the public loop counter
-        const uint32_t digit = (limb >> ((w & 7) * 4)) & 15u;
-        Ext t;
-        dbl<false>(t, acc);
-        dbl<false>(acc, t);
-        dbl<false>(t, acc);
-        dbl<true>(acc, t);
-        select_entry(c, tab, digit);
-        add<false>(t, acc, c);
-        acc = t;
-    }
+    for (int w = kWindows - 1; w >= (kLastT ? 1 : 0); --w) window_step<kPublic, false>(acc, c, tab, s, w);
+    if (kLastT) window_step<kPublic, true>(acc, c, tab, s, 0);
+}
+
+// (ou, ov) = [s] (u, v), affine, for a secret s: scalar_mul_ext with masked table reads, then one inversion.
+__device__ __forceinline__ void scalar_mul(uint32_t (&ou)[8], uint32_t (&ov)[8], const uint32_t (&s)[8],
+                                           const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+    Ext acc;
+    scalar_mul_ext<false, false>(acc, s, u, v);
     uint32_t zi[8];
     inverse(zi, acc.Z);
     fmul(ou, acc.X, zi);
@@ -359,13 +387,10 @@ __device__ __forceinline__ void select_niels(Niels& q, const uint4* tab, int w, 
 // shared memory).  kLastT: the last window also computes T (64 x 7 products instead of 63 x 7 + 6), for a caller that
 // adds another point to the result; without it t.T is not the result's.  t is also the windows' temporary, as it was in
 // fixed_base_mul before the split, which keeps k_fixed_base's code unchanged.
+// fixed_base_from: the same walk from acc (with T) instead of the identity, t = acc + [s] B; acc is the walk's
+// accumulator and is overwritten.
 template <bool kLdg, bool kLastT>
-__device__ __forceinline__ void fixed_base_ext(Ext& t, const uint32_t (&s)[8], const uint4* tab) {
-    Ext acc;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) acc.X[k] = 0, acc.T[k] = 0;
-    set_one(acc.Y);
-    set_one(acc.Z);
+__device__ __forceinline__ void fixed_base_from(Ext& t, Ext& acc, const uint32_t (&s)[8], const uint4* tab) {
     uint32_t d[8], carry = 0;
     fcopy(d, s);
     Niels q;
@@ -377,6 +402,16 @@ __device__ __forceinline__ void fixed_base_ext(Ext& t, const uint32_t (&s)[8], c
     }
     select_niels<kLdg>(q, tab, kFbWindows - 1, recode_digit(d, carry));
     madd<kLastT>(t, acc, q);
+}
+
+template <bool kLdg, bool kLastT>
+__device__ __forceinline__ void fixed_base_ext(Ext& t, const uint32_t (&s)[8], const uint4* tab) {
+    Ext acc;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) acc.X[k] = 0, acc.T[k] = 0;
+    set_one(acc.Y);
+    set_one(acc.Z);
+    fixed_base_from<kLdg, kLastT>(t, acc, s, tab);
 }
 
 // (ou, ov) = [s] B, affine: fixed_base_ext without the last T, one inversion
@@ -411,6 +446,91 @@ __device__ __forceinline__ void to_niels(Niels& q, const uint32_t (&u)[8], const
     fmul(uv, u, v);
     set_2d(k);
     fmul(q.kt, uv, k);
+}
+
+// ---- Schnorr signatures (p252_schnorr_sign_batch / p252_schnorr_verify_batch) ------------------------------------------
+// c = challenge(R, m) < 2^250 comes from the truncated digest.
+//   sign:   u = (r - c sk) mod r_J, no field product: two Montgomery products modulo r_J (order_mul) and one subtraction.
+//   verify: [c] PK + [u] G == R.  PK is checked on the curve (4), [c] PK is scalar_mul_ext with public table reads and T
+//           in the last window (table 2 + 14 x 9, 62 windows x 36, the last 37), then the fixed-base walk of [u] G starts
+//           from it (63 x 7 + 6), and the result is compared projectively with R (2): no inversion.
+constexpr int kOrderProductsPerSchnorrSign = 2;
+constexpr int kProductsPerSchnorrVerify =
+    4 + 2 + 14 * 9 + (kWindows - 1) * (3 * 7 + 8 + 7) + (3 * 7 + 8 + 8) + (kFbWindows - 1) * 7 + 6 + 2;
+static_assert(kOrderProductsPerSchnorrSign == 2, "product count of DESIGN.md section 4");
+static_assert(kProductsPerSchnorrVerify == 2850, "product count of DESIGN.md section 4");
+
+// Arithmetic modulo r_J on 8 x 32-bit little-endian words, Montgomery form with R = 2^256.  Constants (immediates, as
+// P252_JJ_ORDER): R^2 mod r_J and kOrderInv = -r_J^-1 mod 2^32.  Constant time: no branch and no address depends on an
+// operand; each final correction is a masked subtraction or addition of r_J.
+#define P252_JJ_ORDER_R2 {0x95e57731u, 0x67719aa4u, 0x9ce3fc26u, 0x51b0cef0u, 0xc026e9a5u, 0x69dab7fau, 0x8d127688u, 0x04f6547bu}
+constexpr uint32_t kOrderInv = 0xef788ef9u;
+
+// r = a b / 2^256 mod r_J for a, b < r_J (word-serial Montgomery, CIOS).  After row i the accumulator is < a + r_J <
+// 2 r_J < 2^253, so it fits 8 words between rows and one masked subtraction of r_J makes it < r_J.
+__device__ __forceinline__ void order_mont(uint32_t (&r)[8], const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    const uint32_t n[8] = P252_JJ_ORDER;
+    uint32_t t[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) t[k] = 0;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+        uint64_t c = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {                  // t += a b_i
+            c += (uint64_t)a[j] * b[i] + t[j];
+            t[j] = (uint32_t)c;
+            c >>= 32;
+        }
+        const uint32_t hi = (uint32_t)c;
+        const uint32_t m = t[0] * kOrderInv;          // t + m r_J = 0 mod 2^32
+        c = ((uint64_t)m * n[0] + t[0]) >> 32;
+#pragma unroll
+        for (int j = 1; j < 8; ++j) {                  // t = (t + m r_J) / 2^32
+            c += (uint64_t)m * n[j] + t[j];
+            t[j - 1] = (uint32_t)c;
+            c >>= 32;
+        }
+        t[7] = (uint32_t)(c + hi);                      // < 2^32 by the bound above
+    }
+    uint32_t d[8], borrow = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint64_t x = (uint64_t)t[k] - n[k] - borrow;
+        d[k] = (uint32_t)x;
+        borrow = (uint32_t)(x >> 63);
+    }
+    const uint32_t keep = 0u - borrow;                  // t < r_J: keep t, otherwise t - r_J
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = (t[k] & keep) | (d[k] & ~keep);
+}
+
+// r = a b mod r_J for a, b < r_J: (a b / 2^256) (2^512 mod r_J) / 2^256, two Montgomery products
+__device__ __forceinline__ void order_mul(uint32_t (&r)[8], const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    const uint32_t r2[8] = P252_JJ_ORDER_R2;
+    uint32_t x[8];
+    order_mont(x, a, b);
+    order_mont(r, x, r2);
+}
+
+// r = a - b mod r_J for a, b < r_J: the borrow of a - b selects a masked addition of r_J
+__device__ __forceinline__ void order_sub(uint32_t (&r)[8], const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    const uint32_t n[8] = P252_JJ_ORDER;
+    uint32_t borrow = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint64_t x = (uint64_t)a[k] - b[k] - borrow;
+        r[k] = (uint32_t)x;
+        borrow = (uint32_t)(x >> 63);
+    }
+    const uint32_t m = 0u - borrow;
+    uint32_t carry = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint64_t y = (uint64_t)r[k] + (n[k] & m) + carry;
+        r[k] = (uint32_t)y;
+        carry = (uint32_t)(y >> 32);
+    }
 }
 
 // Table entry (w, j), j in 1..8, of the base (u, v) (on the curve, u, v < p): j 16^w (u, v) by 4w doublings and j - 1

@@ -9,6 +9,7 @@
 //   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
 //   dhke             src/encryption.rs:11-43  -> k_dhke (JubJub scalar multiplication, jubjub_device.cuh)
 //   stealth addresses (note_pk = [hash(shared)] G + B) -> k_stealth
+//   Schnorr signatures (u = r - c sk, [u] G + [c] PK == R) -> k_schnorr_pack, k_schnorr_sign, k_schnorr_verify
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
 #include "kernels.h"
@@ -1681,6 +1682,148 @@ cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, co
                                                        static_cast<const uint8_t*>(B_uv), B_bcast, valid,
                                                        static_cast<uint8_t*>(note_pk), static_cast<uint8_t*>(R_uv), ok,
                                                        n_invalid, nullptr);
+    return cudaGetLastError();
+}
+
+// ---- Schnorr signatures: u = r - c sk mod r_J; [u] G + [c] PK == R, c = challenge(R, m) (jubjub_device.cuh) -----------
+// The digest's input rows [R.u, R.v, m]: a value >= p is written as 0, and flag[i] = (and_flag ? flag[i] : 1) and all three
+// values < p.  Sign: flag is ok (r < r_J from k_fixed_base), R as k_fixed_base wrote it; verify: flag is the item's
+// validity, R the caller's.  Public data only.
+__global__ void __launch_bounds__(256) k_schnorr_pack(const uint8_t* R_uv, const uint8_t* __restrict__ msg, size_t n,
+                                                      uint8_t* __restrict__ rows, uint8_t* flag, bool and_flag) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t x[3][8];
+    load_fr_rw(x[0], R_uv + i * 64);
+    load_fr_rw(x[1], R_uv + i * 64 + 32);
+    load_fr(x[2], msg + i * 32);
+    bool good = !and_flag || flag[i] != 0;
+#pragma unroll
+    for (int q = 0; q < 3; ++q) {
+        const bool canon = fr_is_canonical(x[q]);
+        const uint32_t m = 0u - (uint32_t)canon;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) x[q][k] &= m;
+        good &= canon;
+        store_fr(rows + i * 96 + q * 32, x[q]);
+    }
+    flag[i] = good ? 1 : 0;
+}
+
+// Sign, one thread per item, after k_fixed_base (R rows, ok = r < r_J), k_schnorr_pack (ok &= m < p) and the truncated
+// digest (c[i] < 2^250): ok[i] = ok[i] and sk < r_J; u[i] = (r - c sk) mod r_J (kOrderProductsPerSchnorrSign Montgomery
+// products modulo r_J).  An item with ok = 0 runs the same code on r = sk = 0 and gets zeroed u and R rows; *n_invalid
+// += invalid items.  sk and r are secret: every validity is a mask, and no branch or address depends on them.
+__global__ void __launch_bounds__(kThreads, 3) k_schnorr_sign(const uint8_t* __restrict__ sk, bool sb, const uint8_t* __restrict__ r,
+                                                           const uint8_t* __restrict__ c, size_t n, uint8_t* __restrict__ u_out,
+                                                           uint8_t* R_uv, uint8_t* ok, unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t s[8], k[8], e[8];
+    load_fr(s, sk + (sb ? 0 : i) * 32);
+    load_fr(k, r + i * 32);
+    load_fr(e, c + i * 32);
+    const bool good = (ok[i] != 0) & jj::below_order(s);
+    const uint32_t m = 0u - (uint32_t)good;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) s[q] &= m, k[q] &= m;
+    uint32_t x[8], u[8];
+    jj::order_mul(x, e, s);
+    jj::order_sub(u, k, x);
+    uint32_t ru[8], rv[8];
+    load_fr_rw(ru, R_uv + i * 64);
+    load_fr_rw(rv, R_uv + i * 64 + 32);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) u[q] &= m, ru[q] &= m, rv[q] &= m;
+    store_fr(u_out + i * 32, u);
+    store_fr(R_uv + i * 64, ru);
+    store_fr(R_uv + i * 64 + 32, rv);
+    ok[i] = good ? 1 : 0;
+    if (n_invalid) warp_count_every(n_invalid, !good);
+}
+
+// Verify, one thread per item, after k_schnorr_pack (valid[i]: R and m canonical) and the truncated digest (c[i]):
+// verified[i] = valid[i], u < r_J, PK = pk[pb ? 0 : i] a curve point with u, v < p, and [c] PK + [u] G == R, compared
+// projectively (kProductsPerSchnorrVerify products).  Every operand is public, so the variable-base walk of [c] PK reads
+// one table entry per window at the digit's address (jj::scalar_mul_ext<true, ...>); k_dhke keeps the masked reads.
+// PK, then u, then R are loaded, each just before its use, so that across each walk little else is live.  An invalid
+// item runs the same code on the identity and zero.  cnt_ok += verified items, cnt_bad += invalid ones.
+__global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify(const uint8_t* __restrict__ pk, bool pb, const uint8_t* __restrict__ u,
+                                                             const uint8_t* __restrict__ R_uv, const uint8_t* __restrict__ c,
+                                                             const uint8_t* __restrict__ valid, size_t n,
+                                                             const uint4* __restrict__ table, uint8_t* __restrict__ verified,
+                                                             unsigned long long* __restrict__ cnt_ok,
+                                                             unsigned long long* __restrict__ cnt_bad) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    jj::Ext acc;
+    bool good = valid[i] != 0;
+    {
+        uint32_t x[8], y[8], one[8], e[8];
+        load_fr(x, pk + (pb ? 0 : i) * 64);
+        load_fr(y, pk + (pb ? 0 : i) * 64 + 32);
+        const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
+        jj::set_one(one);
+        uint32_t mc = 0u - (uint32_t)canon;            // coordinates >= p enter no product
+#pragma unroll
+        for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+        const bool on = canon & jj::on_curve(x, y);
+        good &= on;
+        mc = 0u - (uint32_t)on;                         // an off-curve PK is replaced by the identity
+#pragma unroll
+        for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+        load_fr(e, c + i * 32);
+        jj::scalar_mul_ext<true, true>(acc, e, x, y);
+    }
+    jj::Ext t;
+    {
+        uint32_t s[8];
+        load_fr(s, u + i * 32);
+        const bool in_range = jj::below_order(s);
+        good &= in_range;
+        const uint32_t m = 0u - (uint32_t)in_range;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] &= m;
+        jj::fixed_base_from<true, false>(t, acc, s, table);
+    }
+    uint32_t ru[8], rv[8], x[8], y[8];
+    load_fr(ru, R_uv + i * 64);
+    load_fr(rv, R_uv + i * 64 + 32);
+    const uint32_t m = 0u - (uint32_t)good;             // an invalid item's R may be >= p: it enters no product
+#pragma unroll
+    for (int k = 0; k < 8; ++k) ru[k] &= m, rv[k] &= m;
+    jj::fmul(x, ru, t.Z);
+    jj::fmul(y, rv, t.Z);
+    const bool ok = good & jj::feq(x, t.X) & jj::feq(y, t.Y);
+    verified[i] = ok ? 1 : 0;
+    if (cnt_ok) warp_count_every(cnt_ok, ok);
+    if (cnt_bad) warp_count_every(cnt_bad, !good);
+}
+
+cudaError_t launch_schnorr_pack(const void* R_uv, const void* msg, size_t n, void* rows, uint8_t* flag, bool and_flag,
+                                cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_pack<<<blocks256(n), 256, 0, st>>>(static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(msg), n,
+                                                 static_cast<uint8_t*>(rows), flag, and_flag);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_schnorr_sign(const void* sk, bool sk_bcast, const void* r, const void* c, size_t n, void* u_out, void* R_uv,
+                                uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_sign<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(sk), sk_bcast, static_cast<const uint8_t*>(r),
+                                                     static_cast<const uint8_t*>(c), n, static_cast<uint8_t*>(u_out),
+                                                     static_cast<uint8_t*>(R_uv), ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c,
+                                  const uint8_t* valid, size_t n, const void* table, uint8_t* verified,
+                                  unsigned long long* n_verified, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_verify<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u),
+                                                       static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(c), valid,
+                                                       n, static_cast<const uint4*>(table), verified, n_verified, n_invalid);
     return cudaGetLastError();
 }
 

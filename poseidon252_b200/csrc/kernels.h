@@ -152,6 +152,20 @@ cudaError_t launch_stealth_owns(const void* h, size_t n, const void* table, cons
 cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, const void* B_uv, bool B_bcast,
                                   const uint8_t* valid, void* R_uv, void* note_pk, uint8_t* ok, unsigned long long* n_invalid,
                                   cudaStream_t st);
+// Schnorr signatures (p252_schnorr_sign_batch / p252_schnorr_verify_batch), challenge c = the truncated digest of the row
+// [R.u, R.v, m] (4 x u64 < 2^250).  Counters are device pointers and may be null.
+// pack: rows[i] = [R.u, R.v, m] (96 bytes, a value >= p written as 0); flag[i] = (and_flag ? flag[i] : 1) and all three < p
+cudaError_t launch_schnorr_pack(const void* R_uv, const void* msg, size_t n, void* rows, uint8_t* flag, bool and_flag,
+                                cudaStream_t st);
+// sign: ok[i] &= sk[sk_bcast ? 0 : i] < r_J; u_out[i] = (r[i] - c[i] sk) mod r_J.  An item with ok = 0 gets a zeroed u row
+// and a zeroed R_uv row and is counted into *n_invalid
+cudaError_t launch_schnorr_sign(const void* sk, bool sk_bcast, const void* r, const void* c, size_t n, void* u_out, void* R_uv,
+                                uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st);
+// verify: verified[i] = valid[i], u[i] < r_J, pk[pk_bcast ? 0 : i] a curve point with u, v < p, and [u[i]] G + [c[i]] pk ==
+// R_uv[i] (table: the fixed-base table of G); *n_verified += verified items, *n_invalid += invalid ones
+cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c,
+                                  const uint8_t* valid, size_t n, const void* table, uint8_t* verified,
+                                  unsigned long long* n_verified, unsigned long long* n_invalid, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

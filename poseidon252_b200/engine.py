@@ -532,6 +532,70 @@ class Engine:
         """Invalid items of the last stealth_address_batch or stealth_owns_batch (sync() first after async_)."""
         return int(getattr(self, "_nsinv", ctypes.c_size_t(0)).value)
 
+    # -- Schnorr signatures -----------------------------------------------------------------------
+    def schnorr_sign_batch(self, sk, r, msg, base, u_out=None, R_out=None, async_=False):
+        """jubjub-schnorr's SecretKey::sign over a batch: R_i = [r_i] base, c_i = challenge(R_i, msg_i) =
+        Hash::digest_truncated(Domain::Other, [R.u, R.v, m])[0] and u_i = (r_i - c_i sk_i) mod r_J.  sk (1 or n, 4) and
+        r (n, 4) p252_jscalar rows (one nonce per message, never reused), msg (n, 4) BlsScalar.0 limbs, base (2, 4)
+        (host-read, as in fixed_base_batch) -> (u (n, 4), R (n, 2, 4), ok (n,) uint8).  An item with sk or r >= r_J or
+        msg >= p has ok == 0 and zeroed u and R rows (count: last_schnorr_invalid())."""
+        rp, rl, flags, rk = self._in(r, (4,))
+        if len(rl) != 1:
+            raise EngineError(-1, "r must have shape (n, 4)")
+        n = int(rl[0])
+        sp, sl, fs, skk = self._in(sk, (4,))
+        mp, ml, fm, mk = self._in(msg, (4,))
+        if not (flags == fs == fm):
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        if len(sl) != 1 or int(sl[0]) not in (1, n):
+            raise EngineError(-1, "sk must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(sl)))
+        self._same_lead("msg", ml, n)
+        b = self._base(base)
+        u = self._out_like(rk, (n, 4)) if u_out is None else self._check_out(u_out, (n, 4), rk)
+        R = self._out_like(rk, (n, 2, 4)) if R_out is None else self._check_out(R_out, (n, 2, 4), rk)
+        ok = self._ok_like(rk, n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nschinv = self._counter(flags)
+        self._check(self._lib.p252_schnorr_sign_batch(self._ctx, sp, int(sl[0]), rp, mp, n, b.ctypes.data, self._ptr(u),
+                                                      self._ptr(R), self._ptr(ok), ctypes.byref(self._nschinv), flags))
+        return u, R, ok
+
+    def schnorr_verify_batch(self, pk, u, R, msg, base, out=None, async_=False):
+        """jubjub-schnorr's PublicKey::verify over a batch: verified[i] = [u_i] base + [c_i] PK_i == R_i with
+        c_i = challenge(R_i, msg_i).  pk (1 or n, 2, 4), u (n, 4) p252_jscalar rows, R (n, 2, 4), msg (n, 4), base (2, 4)
+        (host-read) -> verified (n,) uint8.  An item with u >= r_J, msg >= p, an R coordinate >= p or PK not a curve point
+        is invalid: verified == 0, counted in last_schnorr_invalid(), not in last_schnorr_verified().  A base off the
+        curve raises InvalidPoint."""
+        up, ul, flags, uk = self._in(u, (4,))
+        if len(ul) != 1:
+            raise EngineError(-1, "u must have shape (n, 4)")
+        n = int(ul[0])
+        pp, pl, fp, pkk = self._in(pk, (2, 4))
+        Rp, Rl, fR, Rk = self._in(R, (2, 4))
+        mp, ml, fm, mk = self._in(msg, (4,))
+        if not (flags == fp == fR == fm):
+            raise EngineError(-1, "all buffers must live in the same memory space")
+        if len(pl) != 1 or int(pl[0]) not in (1, n):
+            raise EngineError(-1, "pk must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(pl)))
+        self._same_lead("R", Rl, n)
+        self._same_lead("msg", ml, n)
+        b = self._base(base)
+        verified = self._ok_like(uk, n) if out is None else self._check_out(out, (n,), uk, itemsize=1)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nschok, self._nschinv = self._counter(flags), self._counter(flags)
+        self._check(self._lib.p252_schnorr_verify_batch(self._ctx, pp, int(pl[0]), up, Rp, mp, n, b.ctypes.data,
+                                                        self._ptr(verified), ctypes.byref(self._nschok),
+                                                        ctypes.byref(self._nschinv), flags))
+        return verified
+
+    def last_schnorr_verified(self):
+        """Verified signatures of the last schnorr_verify_batch (sync() first after async_)."""
+        return int(getattr(self, "_nschok", ctypes.c_size_t(0)).value)
+
+    def last_schnorr_invalid(self):
+        """Invalid items of the last schnorr_sign_batch or schnorr_verify_batch (sync() first after async_)."""
+        return int(getattr(self, "_nschinv", ctypes.c_size_t(0)).value)
+
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
         max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries
