@@ -132,6 +132,10 @@ mod stealth;
 // schnorr.rs (methods on Engine).
 mod schnorr;
 
+// JubJub point compression (JubJubAffine::from_bytes / to_bytes over a batch): their own `extern "C"` block in points.rs
+// (methods on Engine).
+mod points;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

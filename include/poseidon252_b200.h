@@ -379,6 +379,28 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
                               const p252_fr* R_uv, const p252_fr* msg, size_t n, const p252_fr* base_uv,
                               uint8_t* verified, size_t* n_verified, size_t* n_invalid, int flags);
 
+/* ---- JubJub point compression (dusk-jubjub's JubJubAffine::to_bytes / from_bytes) -----------------------------------
+ *   encoding:  the 32 little-endian bytes of canonical v, with bit 255 (bytes[31] >> 7) = the low bit of canonical u
+ *   decoding:  sign = bit 255, cleared; the remaining 255-bit value is v (rejected if >= p); u^2 = (v^2 - 1) / (1 + d v^2)
+ *              (rejected if not a square); u is the root whose canonical low bit is sign.
+ * A set sign bit with u = 0 (v = +-1) is accepted and decodes to the same point, as pre-ZIP-216 jubjub does; 32 zero
+ * bytes decode to (sqrt(-1), 0), a point of order 4.  There is no subgroup check.  Points are (u, v) pairs of p252_fr
+ * (Montgomery limbs), laid out as for p252_dhke_batch; bytes are n x 32.
+ * Item validity (checked on the device, for both memory spaces):
+ *   from_bytes: v < p and u^2 a square.  An invalid item gets ok[i] = 0 and the row (0, 0), which is not a curve point.
+ *   to_bytes:   u, v < p and (u, v) on the curve.  An invalid item gets ok[i] = 0 and 32 bytes of 0xff (v = 2^255 - 1 >= p,
+ *               so from_bytes rejects it; zero bytes would decode).
+ * Invalid items are counted into *n_invalid (optional HOST pointer, lifetime as for p252_decrypt_batch); the call still
+ * returns P252_OK.  Batch checks, before anything runs: a NULL buffer (ok included) with n > 0, DEVICE buffers other than
+ * ok not 16-byte aligned -> INVALID_ARGUMENT.  Public data only: with P252_ASYNC, DEVICE calls defer the publication of
+ * *n_invalid to p252_sync. */
+/* out_uv[i] = JubJubAffine::from_bytes(bytes[32 i .. 32 i + 32]) */
+int p252_points_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out_uv, uint8_t* ok,
+                           size_t* n_invalid, int flags);
+/* bytes[32 i ..] = JubJubAffine::to_bytes(uv[i]) */
+int p252_points_to_bytes(p252_ctx* ctx, const p252_fr* uv, size_t n, uint8_t* bytes, uint8_t* ok,
+                         size_t* n_invalid, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

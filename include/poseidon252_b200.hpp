@@ -11,7 +11,8 @@
 //   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
 //   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
 //   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
-//   schnorr_verify_batch, merkle4_build.
+//   schnorr_verify_batch, point_from_bytes / points_from_bytes_batch, point_to_bytes / points_to_bytes_batch,
+//   merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -441,6 +442,41 @@ inline bool schnorr_verify(const Scalar (&pk_uv)[2], const JubJubScalar& u, cons
     const auto verified = schnorr_verify_batch(pk_uv, 1, &u, R_uv, &msg, 1, base_uv, nullptr, &invalid, e);
     if (invalid) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
     return verified[0] != 0;
+}
+
+// NEW: JubJub point compression (p252_points_from_bytes / p252_points_to_bytes), dusk-jubjub's JubJubAffine::from_bytes /
+// to_bytes: the 32 little-endian bytes of canonical v with the low bit of canonical u in bit 255.
+// bytes holds n x 32 bytes; returns n x 2 scalars (u, v); ok[i] == 0 marks an encoding with v >= p or u^2 not a square,
+// whose row is (0, 0).  n_invalid may be null.
+inline std::vector<Scalar> points_from_bytes_batch(const uint8_t* bytes, size_t n, std::vector<uint8_t>& ok,
+                                                   size_t* n_invalid = nullptr, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> uv(2 * n);
+    ok.assign(n, 0);
+    check(p252_points_from_bytes(e.get(), bytes, n, uv.data(), ok.data(), n_invalid, P252_MEM_HOST), e.get());
+    return uv;
+}
+// uv holds n x 2 scalars; returns n x 32 bytes; ok[i] == 0 marks a coordinate >= p or a point off the curve, whose
+// encoding is 32 bytes of 0xff.  n_invalid may be null.
+inline std::vector<uint8_t> points_to_bytes_batch(const Scalar* uv, size_t n, std::vector<uint8_t>& ok,
+                                                  size_t* n_invalid = nullptr, Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> bytes(32 * n);
+    ok.assign(n, 0);
+    check(p252_points_to_bytes(e.get(), uv, n, bytes.data(), ok.data(), n_invalid, P252_MEM_HOST), e.get());
+    return bytes;
+}
+// JubJubAffine::from_bytes for one encoding; throws Error(P252_ERR_INVALID_POINT) for an invalid one
+inline void point_from_bytes(const uint8_t (&bytes)[32], Scalar (&uv)[2], Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok;
+    const auto r = points_from_bytes_batch(bytes, 1, ok, nullptr, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    uv[0] = r[0], uv[1] = r[1];
+}
+// JubJubAffine::to_bytes for one point; throws Error(P252_ERR_INVALID_POINT) for a coordinate >= p or a point off the curve
+inline void point_to_bytes(const Scalar (&uv)[2], uint8_t (&bytes)[32], Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok;
+    const auto r = points_to_bytes_batch(uv, 1, ok, nullptr, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    std::copy(r.begin(), r.end(), bytes);
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

@@ -12,6 +12,7 @@
 //   GENERATOR * r, the sender       src/encryption.rs:22-42 -> p252_fixed_base_batch, p252_encrypt_batch_ephemeral
 //   Phoenix stealth addresses (consumer, not the reference) -> p252_stealth_address_batch, p252_stealth_owns_batch
 //   jubjub-schnorr sign / verify (consumer, not the reference) -> p252_schnorr_sign_batch, p252_schnorr_verify_batch
+//   JubJubAffine::from_bytes / to_bytes (dusk-jubjub, not the reference) -> p252_points_from_bytes, p252_points_to_bytes
 //   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -1232,6 +1233,51 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
     if (rc == P252_OK) rc = counter_end(ctx, n_verified, 0);
     if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
     return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
+}
+
+// ---- JubJub point compression: JubJubAffine::from_bytes / to_bytes -----------------------------------------------------
+// One launch per chunk (launch_points_from_bytes / launch_points_to_bytes).  HOST batches stream through the slot arenas;
+// DEVICE buffers are used in place.  Nothing here is secret: no wipe.  HOST calls count the invalid items from ok on the
+// host, DEVICE calls on the device counter.
+static int points_impl(p252_ctx* ctx, bool from_bytes, const void* in, size_t n, void* out, uint8_t* ok, size_t* n_invalid,
+                       int flags) {
+    if (!ctx || (n && (!in || !out || !ok))) return P252_ERR_INVALID_ARGUMENT;
+    const bool dev = (flags & P252_MEM_DEVICE) != 0;
+    if (dev && (!aligned16(in) || !aligned16(out))) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    int rc = P252_OK;
+    unsigned long long* counter = nullptr;
+    if (dev && n_invalid) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    const size_t in_bytes = from_bytes ? 32 : 64, out_bytes = from_bytes ? 64 : 32;
+    // 0 input, 1 output, 2 ok
+    std::vector<Io> ios = {{in, nullptr, in_bytes, false, dev}, {nullptr, out, out_bytes, false, dev}, {nullptr, ok, 1, false, dev}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[2]);
+        return from_bytes ? p252::launch_points_from_bytes(d[0], cnt, d[1], okc, counter, st)
+                          : p252::launch_points_to_bytes(d[0], cnt, d[1], okc, counter, st);
+    });
+    if (!dev) {
+        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+        return rc;
+    }
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+    return device_done(ctx, rc, flags);
+}
+
+int p252_points_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out_uv, uint8_t* ok, size_t* n_invalid,
+                           int flags) {
+    return points_impl(ctx, true, bytes, n, out_uv, ok, n_invalid, flags);
+}
+
+int p252_points_to_bytes(p252_ctx* ctx, const p252_fr* uv, size_t n, uint8_t* bytes, uint8_t* ok, size_t* n_invalid,
+                         int flags) {
+    return points_impl(ctx, false, uv, n, bytes, ok, n_invalid, flags);
 }
 
 // ---- arity-4 Merkle tree ------------------------------------------------------------------------------

@@ -570,5 +570,143 @@ __device__ __forceinline__ void fixed_base_entry(uint4* out, const uint32_t (&u)
     }
 }
 
+// ---- point compression: JubJubAffine::to_bytes / from_bytes (p252_points_to_bytes / p252_points_from_bytes) ------------
+// Encoding: the 32 little-endian bytes of canonical v, bit 255 = the low bit of canonical u (v < p < 2^255 leaves it free).
+// Decoding solves the curve equation for u: u^2 = (v^2 - 1) / (1 + d v^2).  The denominator is never 0 (d is a
+// non-square, -1 a square), so the root is RFC 9380 Appendix F.2.1.1 sqrt_ratio(num, den): no inversion, and a trip count
+// fixed by p alone, so every lane of a warp runs the same instructions.  With p - 1 = 2^c1 t, t odd, c1 = 32 and Z = 5 (a
+// non-residue mod p), its constants are c3 = (t - 1) / 2 (222 bits, 132 set; canonical words), c6 = Z^t and
+// c7 = Z^((t + 1) / 2) (Montgomery images).  Immediates, as P252_JJ_PM2.
+#define P252_JJ_SQRT_C3 {0x7fffffffu, 0x7fff2dffu, 0xa9ded201u, 0x04d0ec02u, 0x199cec04u, 0x94cebea4u, 0x39f6d3a9u, 0x00000000u}
+#define P252_JJ_SQRT_C6 {0x0c17f47cu, 0x9cab6d5cu, 0xfd4b71e5u, 0x1ce1e93du, 0x471dd505u, 0x0d6db230u, 0x743a3b6au, 0x3f0ee990u}
+#define P252_JJ_SQRT_C7 {0xbb7b07a1u, 0xba8e19e4u, 0x92112747u, 0x0dc42383u, 0x26b941a1u, 0xdfd3d081u, 0x7a45cec5u, 0x6bb1a261u}
+constexpr int kSqrtC1 = 32, kSqrtC3Bits = 222, kSqrtC3Ones = 132;
+
+// Products of sqrt_ratio, step by step (RFC numbering): 2. den^(2^32 - 1) by the chain 2^(2k) - 1 = (2^k - 1) 2^k +
+// (2^k - 1), 31 squarings + 5 products; 3.-5. 3; 6. the exponent c3, (bits - 1) squarings + (ones - 1) products; 7.-10. 4;
+// 11. 31 squarings; 13.-14. 2; the loop k = 32..2, (k - 2) squarings + 3 products per round.
+constexpr int kProductsPerSqrtRatio = (31 + 5) + 3 + (kSqrtC3Bits - 1) + (kSqrtC3Ones - 1) + 4 + (kSqrtC1 - 1) + 2 +
+                                      (kSqrtC1 - 2) * (kSqrtC1 - 1) / 2 + 3 * (kSqrtC1 - 1);
+// Decompression: v into Montgomery form 1, v^2 and d v^2 2, sqrt_ratio; the sign needs one canonical conversion (a
+// reduction, no product).  Compression: the on-curve check 4 and two canonical conversions.
+constexpr int kProductsPerDecompress = 1 + 2 + kProductsPerSqrtRatio;
+constexpr int kProductsPerCompress = 4;
+static_assert(kProductsPerSqrtRatio == 986, "product count of DESIGN.md section 4");
+static_assert(kProductsPerDecompress == 989, "product count of DESIGN.md section 4");
+static_assert(kProductsPerCompress == 4, "product count of DESIGN.md section 4");
+
+// r = a^(2^k): k squarings (k public)
+__device__ __forceinline__ void fsqr_n(uint32_t (&r)[8], const uint32_t (&a)[8], int k) {
+    fcopy(r, a);
+#pragma unroll 1
+    for (int i = 0; i < k; ++i) {
+        uint32_t t[8];
+        fsqr(t, r);
+        fcopy(r, t);
+    }
+}
+
+// r = c ? a : b, masked
+__device__ __forceinline__ void fsel(uint32_t (&r)[8], bool c, const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    const uint32_t m = 0u - (uint32_t)c;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = (a[k] & m) | (b[k] & ~m);
+}
+
+// Returns whether num / den is a square; y = sqrt(num / den) if it is, sqrt(Z num / den) otherwise.  num, den < p,
+// den != 0.  The RFC's is_square is false for num = 0 (tv4 = 0 never powers to 1); num = 0 is a square here, and y is 0
+// on both paths.
+__device__ __forceinline__ bool sqrt_ratio(uint32_t (&y)[8], const uint32_t (&num)[8], const uint32_t (&den)[8]) {
+    uint32_t tv1[8] = P252_JJ_SQRT_C6, tv2[8], tv3[8], tv4[8], tv5[8], t[8], one[8];
+    set_one(one);
+    // 2. tv2 = den^(2^32 - 1)
+    fcopy(tv2, den);
+#pragma unroll 1
+    for (int k = 1; k < kSqrtC1; k *= 2) {
+        fsqr_n(t, tv2, k);
+        fmul(tv3, t, tv2);
+        fcopy(tv2, tv3);
+    }
+    fsqr(t, tv2);                   // 3. tv3 = tv2^2
+    fmul(tv3, t, den);              // 4. tv3 = tv3 den
+    fmul(t, num, tv3);              // 5. tv5 = num tv3
+    fcopy(tv5, t);                  // 6. tv5 = tv5^c3, left to right over the public bits of c3
+#pragma unroll 1
+    for (int i = kSqrtC3Bits - 2; i >= 0; --i) {
+        uint32_t s[8];
+        fsqr(s, tv5);
+        const uint32_t e[8] = P252_JJ_SQRT_C3;
+        uint32_t word = 0;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) word = (k == (i >> 5)) ? e[k] : word;
+        if ((word >> (i & 31)) & 1u)
+            fmul(tv5, s, t);
+        else
+            fcopy(tv5, s);
+    }
+    fmul(t, tv5, tv2);              // 7. tv5 = tv5 tv2
+    fmul(tv2, t, den);              // 8. tv2 = tv5 den
+    fmul(tv3, t, num);              // 9. tv3 = tv5 num
+    fmul(tv4, tv3, tv2);            // 10. tv4 = tv3 tv2
+    fsqr_n(tv5, tv4, kSqrtC1 - 1);  // 11. tv5 = tv4^(2^31)
+    const bool is_qr = feq(tv5, one);                       // 12.
+    const uint32_t c7[8] = P252_JJ_SQRT_C7;
+    fmul(tv2, tv3, c7);             // 13. tv2 = tv3 c7
+    fmul(tv5, tv4, tv1);            // 14. tv5 = tv4 tv1
+    fsel(tv3, is_qr, tv3, tv2);     // 15.
+    fsel(tv4, is_qr, tv4, tv5);     // 16.
+#pragma unroll 1
+    for (int k = kSqrtC1; k >= 2; --k) {                    // 17.
+        fsqr_n(tv5, tv4, k - 2);    // 18.-20. tv5 = tv4^(2^(k - 2))
+        const bool e1 = feq(tv5, one);                      // 21.
+        fmul(tv2, tv3, tv1);        // 22.
+        fsqr(t, tv1);               // 23.
+        fcopy(tv1, t);
+        fmul(tv5, tv4, tv1);        // 24.
+        fsel(tv3, e1, tv3, tv2);    // 25.
+        fsel(tv4, e1, tv4, tv5);    // 26.
+    }
+    fcopy(y, tv3);
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    return is_qr | feq(num, zero);
+}
+
+// (u, v) = JubJubAffine::from_bytes(b) (Montgomery), b the 8 little-endian words of the encoding.  Returns validity: the
+// 255-bit v < p and u^2 a square.  kProductsPerDecompress products.  An invalid encoding runs the same schedule on v = 0
+// and its (u, v) is not a point; the caller discards it.
+__device__ __forceinline__ bool decompress(uint32_t (&u)[8], uint32_t (&v)[8], const uint32_t (&b)[8]) {
+    uint32_t c[8], vv[8], dvv[8], num[8], den[8], r[8], one[8], k[8];
+    const uint32_t sign = b[7] >> 31;
+    fcopy(c, b);
+    c[7] &= 0x7fffffffu;
+    const bool canon = fr_is_canonical(c);
+    const uint32_t mc = 0u - (uint32_t)canon;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) c[q] &= mc;
+    fr_from_canonical(v, c);
+    fsqr(vv, v);
+    set_d(k);
+    fmul(dvv, vv, k);
+    set_one(one);
+    fr_sub_mod(num, vv, one);       // v^2 - 1
+    fr_add_mod(den, dvv, one);      // 1 + d v^2
+    const bool square = sqrt_ratio(r, num, den);
+    uint32_t rc[8], nr[8];
+    fr_to_canonical(rc, r);
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    fr_sub_mod(nr, zero, r);        // p - r (0 for r = 0: a set sign bit with u = 0 decodes to the same point)
+    fsel(u, (rc[0] & 1u) == sign, r, nr);
+    return canon & square;
+}
+
+// b = JubJubAffine::to_bytes(u, v) as 8 little-endian words, for u, v < p (Montgomery) on the curve: canonical v with the
+// low bit of canonical u in bit 255
+__device__ __forceinline__ void compress(uint32_t (&b)[8], const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+    uint32_t uc[8];
+    fr_to_canonical(uc, u);
+    fr_to_canonical(b, v);
+    b[7] |= uc[0] << 31;
+}
+
 }  // namespace jj
 }  // namespace p252

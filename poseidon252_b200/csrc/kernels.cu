@@ -10,6 +10,7 @@
 //   dhke             src/encryption.rs:11-43  -> k_dhke (JubJub scalar multiplication, jubjub_device.cuh)
 //   stealth addresses (note_pk = [hash(shared)] G + B) -> k_stealth
 //   Schnorr signatures (u = r - c sk, [u] G + [c] PK == R) -> k_schnorr_pack, k_schnorr_sign, k_schnorr_verify
+//   JubJubAffine::from_bytes / to_bytes (point compression) -> k_points_from_bytes, k_points_to_bytes
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
 #include "kernels.h"
@@ -1824,6 +1825,67 @@ cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, 
     k_schnorr_verify<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u),
                                                        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(c), valid,
                                                        n, static_cast<const uint4*>(table), verified, n_verified, n_invalid);
+    return cudaGetLastError();
+}
+
+// ---- point compression: JubJubAffine::from_bytes / to_bytes (jubjub_device.cuh) ---------------------------------------
+// One thread per point.  Public data only.
+// from_bytes (kProductsPerDecompress products): bytes[i] -> (u, v) Montgomery; ok[i] = v < p and u^2 a square.  An
+// invalid item writes (0, 0), which is not a curve point.
+__global__ void __launch_bounds__(kThreads, 3) k_points_from_bytes(const uint8_t* __restrict__ bytes, size_t n,
+                                                                uint8_t* __restrict__ uv, uint8_t* __restrict__ ok,
+                                                                unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t b[8], u[8], v[8];
+    load_fr(b, bytes + i * 32);
+    const bool good = jj::decompress(u, v, b);
+    const uint32_t m = 0u - (uint32_t)good;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= m, v[k] &= m;
+    store_fr(uv + i * 64, u);
+    store_fr(uv + i * 64 + 32, v);
+    ok[i] = good ? 1 : 0;
+    if (n_invalid) warp_count_every(n_invalid, !good);
+}
+
+// to_bytes (kProductsPerCompress products): (u, v) Montgomery -> bytes[i]; ok[i] = u, v < p and (u, v) on the curve.  An
+// invalid item writes 32 bytes of 0xff: v = 2^255 - 1 >= p, which from_bytes rejects (zero bytes would decode).
+__global__ void __launch_bounds__(kThreads, 3) k_points_to_bytes(const uint8_t* __restrict__ uv, size_t n,
+                                                              uint8_t* __restrict__ bytes, uint8_t* __restrict__ ok,
+                                                              unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t u[8], v[8], b[8];
+    load_fr(u, uv + i * 64);
+    load_fr(v, uv + i * 64 + 32);
+    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
+    const uint32_t mc = 0u - (uint32_t)canon;           // coordinates >= p enter no product
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] &= mc;
+    const bool good = canon & jj::on_curve(u, v);
+    jj::compress(b, u, v);
+    const uint32_t m = 0u - (uint32_t)good;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) b[k] |= ~m;
+    store_fr(bytes + i * 32, b);
+    ok[i] = good ? 1 : 0;
+    if (n_invalid) warp_count_every(n_invalid, !good);
+}
+
+cudaError_t launch_points_from_bytes(const void* bytes, size_t n, void* uv, uint8_t* ok, unsigned long long* n_invalid,
+                                     cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_points_from_bytes<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(bytes), n, static_cast<uint8_t*>(uv), ok,
+                                                          n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_points_to_bytes(const void* uv, size_t n, void* bytes, uint8_t* ok, unsigned long long* n_invalid,
+                                   cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_points_to_bytes<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(uv), n, static_cast<uint8_t*>(bytes), ok,
+                                                        n_invalid);
     return cudaGetLastError();
 }
 

@@ -166,6 +166,13 @@ cudaError_t launch_schnorr_sign(const void* sk, bool sk_bcast, const void* r, co
 cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c,
                                   const uint8_t* valid, size_t n, const void* table, uint8_t* verified,
                                   unsigned long long* n_verified, unsigned long long* n_invalid, cudaStream_t st);
+// Point compression (p252_points_from_bytes / p252_points_to_bytes): 32-byte encodings <-> (u, v) Montgomery pairs (64
+// bytes).  from: ok[i] = v < p and u^2 a square, an invalid item gets (0, 0); to: ok[i] = u, v < p and on the curve, an
+// invalid item gets 32 bytes of 0xff.  *n_invalid (a device counter, may be null) += invalid items.
+cudaError_t launch_points_from_bytes(const void* bytes, size_t n, void* uv, uint8_t* ok, unsigned long long* n_invalid,
+                                     cudaStream_t st);
+cudaError_t launch_points_to_bytes(const void* uv, size_t n, void* bytes, uint8_t* ok, unsigned long long* n_invalid,
+                                   cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -596,6 +596,49 @@ class Engine:
         """Invalid items of the last schnorr_sign_batch or schnorr_verify_batch (sync() first after async_)."""
         return int(getattr(self, "_nschinv", ctypes.c_size_t(0)).value)
 
+    # -- point compression ------------------------------------------------------------------------
+    def points_from_bytes(self, data, out=None, async_=False):
+        """JubJubAffine::from_bytes over a batch: (n, 32) uint8 encodings (host) or (n, 4) 64-bit device tensor of the
+        same bytes -> (points (n, 2, 4) BlsScalar.0 limbs, ok (n,) uint8).  An encoding whose v is >= p or whose u^2 is
+        not a square has ok == 0 and the row (0, 0) (count: last_points_invalid())."""
+        if _is_torch(data):
+            ptr, lead, flags, keep = self._in(data, (4,))
+            if len(lead) != 1:
+                raise EngineError(-1, "device bytes must have shape (n, 4)")
+            n = int(lead[0])
+        else:
+            keep = np.ascontiguousarray(data, dtype=np.uint8)
+            if keep.ndim != 2 or keep.shape[1] != 32:
+                raise EngineError(-1, "host bytes must have shape (n, 32), got %s" % (keep.shape,))
+            ptr, n, flags = keep.ctypes.data, int(keep.shape[0]), _native.MEM_HOST
+        res = self._out_like(keep, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), keep)
+        ok = self._ok_like(keep, n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nptinv = self._counter(flags)
+        self._check(self._lib.p252_points_from_bytes(self._ctx, ptr, n, self._ptr(res), self._ptr(ok),
+                                                     ctypes.byref(self._nptinv), flags))
+        return res, ok
+
+    def points_to_bytes(self, points, async_=False):
+        """JubJubAffine::to_bytes over a batch: points (n, 2, 4) BlsScalar.0 limbs -> (bytes, ok (n,) uint8), bytes
+        (n, 32) uint8 (host) or an (n, 4) device tensor of the same bytes.  A point with a coordinate >= p or off the curve
+        has ok == 0 and 32 bytes of 0xff, which from_bytes rejects (count: last_points_invalid())."""
+        pp, pl, flags, pk = self._in(points, (2, 4))
+        if len(pl) != 1:
+            raise EngineError(-1, "points must have shape (n, 2, 4)")
+        n = int(pl[0])
+        res = self._out_like(pk, (n, 4)) if _is_torch(pk) else np.empty((n, 32), dtype=np.uint8)
+        ok = self._ok_like(pk, n)
+        flags |= _native.ASYNC if async_ and flags else 0
+        self._nptinv = self._counter(flags)
+        self._check(self._lib.p252_points_to_bytes(self._ctx, pp, n, self._ptr(res), self._ptr(ok),
+                                                   ctypes.byref(self._nptinv), flags))
+        return res, ok
+
+    def last_points_invalid(self):
+        """Invalid items of the last points_from_bytes or points_to_bytes (sync() first after async_)."""
+        return int(getattr(self, "_nptinv", ctypes.c_size_t(0)).value)
+
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
         max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries
