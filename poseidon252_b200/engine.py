@@ -35,9 +35,11 @@ class Engine:
             raise EngineError(rc, self._lib.p252_strerror(rc).decode())
         self._dist = False
         self._stream_handle = None if stream is None else int(stream)
-        # failure / rejection counters of async device calls: a host function on the stream writes through them, so
-        # every one stays alive until sync() or close() (as do temporaries an async call made for the device to read)
-        self._pending_counters = []
+        # name -> the c_size_t the last call that publishes that count was given (read by the last_*() methods)
+        self._counters = {}
+        # what an async device call left for the stream to use after it returned: a host function writes through its
+        # counters, the device reads the temporaries made for it; all of it stays alive until sync() or close()
+        self._kept_until_sync = []
 
     def _fence_torch(self):
         """Device tensors are produced on torch's current stream; unless the engine was bound to that
@@ -52,7 +54,7 @@ class Engine:
         if getattr(self, "_ctx", None) and self._ctx.value:
             self._lib.p252_destroy(self._ctx)          # drains the stream: pending counter writes are done
             self._ctx = ctypes.c_void_p()
-        self._pending_counters = []
+        self._kept_until_sync = []
 
     def __del__(self):
         try:
@@ -68,14 +70,23 @@ class Engine:
 
     def sync(self):
         self._check(self._lib.p252_sync(self._ctx))
-        self._pending_counters = []
+        self._kept_until_sync = []
 
-    def _counter(self, flags):
-        """A c_size_t for a count the library publishes; kept alive until sync() when the call is asynchronous."""
-        c = ctypes.c_size_t(0)
+    def _keep_until_sync(self, obj):
+        """Keep `obj` alive until sync() or close(): the stream still reads or writes it after the call returned."""
+        self._kept_until_sync.append(obj)
+
+    def _counter(self, name, flags):
+        """A fresh c_size_t for the count the library publishes as `name`, installed before the call so that a call
+        that raises leaves 0 behind; kept alive until sync() when the call is asynchronous."""
+        c = self._counters[name] = ctypes.c_size_t(0)
         if flags & _native.ASYNC:
-            self._pending_counters.append(c)
+            self._keep_until_sync(c)
         return c
+
+    def _last(self, name):
+        """The count `name` of the last call that publishes it; 0 before any such call."""
+        return int(self._counters[name].value) if name in self._counters else 0
 
     @property
     def launch_count(self):
@@ -101,6 +112,17 @@ class Engine:
             raise EngineError(-1, "expected trailing shape %s, got %s" % (shape_tail, a.shape))
         return a.ctypes.data, tuple(a.shape[:-len(shape_tail)]), _native.MEM_HOST, a
 
+    @staticmethod
+    def _flags(flags, async_):
+        """The flags of a call on buffers of memory space `flags`: ASYNC only when asked for and only for DEVICE buffers
+        (MEM_HOST is 0); a HOST call is always synchronous."""
+        return flags | (_native.ASYNC if async_ and flags else 0)
+
+    @staticmethod
+    def _same_space(*flags):
+        if len(set(flags)) > 1:
+            raise EngineError(-1, "all buffers must live in the same memory space")
+
     def _check_out(self, out, shape, like, itemsize=8):
         """A caller-supplied result buffer goes to native code as a raw pointer: refuse anything whose shape,
         element type, contiguity or memory space differs from what the call will write."""
@@ -123,15 +145,38 @@ class Engine:
         if tuple(lead) != (n,):
             raise EngineError(-1, "%s must have %d rows, got leading shape %s" % (name, n, tuple(lead)))
 
-    def _out_like(self, ref, shape, dtype=None):
-        if _is_torch(ref):
+    def _out_like(self, like, shape, itemsize=8):
+        """An uninitialised result buffer in the memory space of `like`: 64-bit words (a tensor takes the dtype of
+        `like`) or, with itemsize 1, bytes."""
+        if _is_torch(like):
             import torch
-            return torch.empty(shape, dtype=ref.dtype if dtype is None else dtype, device=ref.device)
-        return np.empty(shape, dtype=np.uint64 if dtype is None else dtype)
+            return torch.empty(shape, dtype=like.dtype if itemsize == 8 else torch.uint8, device=like.device)
+        return np.empty(shape, dtype=np.uint64 if itemsize == 8 else np.uint8)
+
+    def _ok_like(self, like, n):
+        return self._out_like(like, (n,), itemsize=1)
+
+    def _result(self, out, shape, like, itemsize=8):
+        """The buffer a call writes its result to: a new one like `like`, or the caller's `out` once it is validated."""
+        return self._out_like(like, shape, itemsize) if out is None else self._check_out(out, shape, like, itemsize)
+
+    def _rows_like(self, like, rows):
+        """A new (rows, 4) result buffer whose pointer is never NULL, even for zero rows."""
+        return self._out_like(like, (max(rows, 1), 4))[:rows]
 
     @staticmethod
     def _ptr(x):
         return x.data_ptr() if _is_torch(x) else x.ctypes.data
+
+    @staticmethod
+    def _host_limbs(x, shape, what):
+        """A public value the library reads on the host for every memory space, as a host uint64 array of `shape`: a CUDA
+        tensor is copied there, and int64 (a tensor's dtype) is reinterpreted, not converted."""
+        a = np.ascontiguousarray(x.detach().cpu().numpy() if _is_torch(x) else x)
+        b = a.view(np.uint64) if a.dtype == np.int64 else np.ascontiguousarray(a, dtype=np.uint64)
+        if b.size != int(np.prod(shape)):
+            raise EngineError(-1, "%s of shape %s, got %s" % (what, shape, b.shape))
+        return b.reshape(shape)
 
     # -- hades::permute_batch ---------------------------------------------------------------------
     def permute_batch(self, states, dense=False, out=None, async_=False):
@@ -145,7 +190,7 @@ class Engine:
                 res = self._check_out(out, keep.shape, keep)
                 if out is not keep:
                     out.copy_(keep)
-            self._fence_torch()
+            self._fence_torch()                   # that copy was enqueued on torch's stream
         elif out is not None:
             res = self._check_out(out, keep.shape, keep)
             if res is not states:
@@ -153,7 +198,7 @@ class Engine:
         else:
             res = keep.copy() if keep is states else keep   # `keep` is already a private copy otherwise
         fn = self._lib.p252_permute_batch_dense if dense else self._lib.p252_permute_batch
-        self._check(fn(self._ctx, self._ptr(res), n, flags | (_native.ASYNC if async_ and flags else 0)))
+        self._check(fn(self._ctx, self._ptr(res), n, self._flags(flags, async_)))
         return res
 
     def permute_batch_inplace(self, states, async_=False):
@@ -161,47 +206,48 @@ class Engine:
         n = int(np.prod(lead)) if lead else 1
         if not _is_torch(keep) and keep is not states:
             raise EngineError(-1, "in-place permute needs a contiguous uint64 array")
-        self._check(self._lib.p252_permute_batch(self._ctx, ptr, n,
-                                                 flags | (_native.ASYNC if async_ and flags else 0)))
+        self._check(self._lib.p252_permute_batch(self._ctx, ptr, n, self._flags(flags, async_)))
         return states
 
     # -- sponges ------------------------------------------------------------------------------------
+    def _sponge_batch(self, fn, first, inputs, out_len, out, async_):
+        """The fixed-length digest calls: fn(ctx, first, inputs, n, in_len, out, out_len, flags); `first` is the tag
+        pointer or the domain."""
+        if inputs.ndim != 3:
+            raise EngineError(-1, "inputs must have shape (n, in_len, 4)")
+        in_len = int(inputs.shape[1])
+        ptr, lead, flags, keep = self._in(inputs, (in_len, 4))
+        n = lead[0]
+        res = self._result(out, (n, int(out_len), 4), keep)
+        self._check(fn(self._ctx, first, ptr, n, in_len, self._ptr(res), int(out_len), self._flags(flags, async_)))
+        return res
+
     def digest_batch_with_tag(self, tag, inputs, out_len=1, out=None, async_=False):
         """start(tag) -> absorb(in_len) -> squeeze(out_len) for every item.  inputs: (n, in_len, 4)."""
         tag = np.ascontiguousarray(tag, dtype=np.uint64).reshape(4)
-        if inputs.ndim != 3:
-            raise EngineError(-1, "inputs must have shape (n, in_len, 4)")
-        in_len = int(inputs.shape[1])
-        ptr, lead, flags, keep = self._in(inputs, (in_len, 4))
-        n = lead[0]
-        res = self._out_like(keep, (n, int(out_len), 4)) if out is None else self._check_out(out, (n, int(out_len), 4), keep)
-        self._check(self._lib.p252_digest_batch(self._ctx, tag.ctypes.data, ptr, n, in_len, self._ptr(res),
-                                                int(out_len), flags | (_native.ASYNC if async_ and flags else 0)))
-        return res
+        return self._sponge_batch(self._lib.p252_digest_batch, tag.ctypes.data, inputs, out_len, out, async_)
 
     def hash_batch(self, domain, inputs, out_len=1, out=None, async_=False):
         """n x Hash::digest(domain, inputs[i]) with output_len(out_len)."""
-        if inputs.ndim != 3:
-            raise EngineError(-1, "inputs must have shape (n, in_len, 4)")
-        in_len = int(inputs.shape[1])
-        ptr, lead, flags, keep = self._in(inputs, (in_len, 4))
-        n = lead[0]
-        res = self._out_like(keep, (n, int(out_len), 4)) if out is None else self._check_out(out, (n, int(out_len), 4), keep)
-        self._check(self._lib.p252_hash_batch(self._ctx, int(domain), ptr, n, in_len, self._ptr(res), int(out_len),
-                                              flags | (_native.ASYNC if async_ and flags else 0)))
-        return res
+        return self._sponge_batch(self._lib.p252_hash_batch, int(domain), inputs, out_len, out, async_)
 
     def hash_batch_truncated(self, domain, inputs, out_len=1, out=None, async_=False):
         """n x Hash::digest_truncated: raw (canonical, 250-bit masked) limbs for JubJubScalar::from_raw."""
-        if inputs.ndim != 3:
-            raise EngineError(-1, "inputs must have shape (n, in_len, 4)")
-        in_len = int(inputs.shape[1])
-        ptr, lead, flags, keep = self._in(inputs, (in_len, 4))
-        n = lead[0]
-        res = self._out_like(keep, (n, int(out_len), 4)) if out is None else self._check_out(out, (n, int(out_len), 4), keep)
-        self._check(self._lib.p252_hash_batch_truncated(self._ctx, int(domain), ptr, n, in_len, self._ptr(res),
-                                                        int(out_len), flags | (_native.ASYNC if async_ and flags else 0)))
-        return res
+        return self._sponge_batch(self._lib.p252_hash_batch_truncated, int(domain), inputs, out_len, out, async_)
+
+    @staticmethod
+    def _longest_item(offsets, n, extra=0):
+        """max_len of a varlen call that was given none: the longest of the n items at `offsets`, less the `extra`
+        scalars an item carries beyond its message, at least 1.  CUDA offsets cost one device-to-host read."""
+        if n == 0:
+            return 1
+        if _is_torch(offsets):
+            import torch
+            o = offsets.view(torch.int64)
+            longest = int((o[1:] - o[:-1]).max().item())
+        else:
+            longest = int((offsets[1:].astype(np.int64) - offsets[:-1].astype(np.int64)).max())
+        return max(longest - extra, 1)
 
     def hash_batch_varlen(self, domain, data, offsets, out_len=1, max_len=None, out=None, async_=False):
         """n x Hash::digest(domain, data[offsets[i]:offsets[i+1]]) with output_len(out_len), inputs of any lengths in one
@@ -216,56 +262,39 @@ class Engine:
             raise EngineError(-1, "offsets must have n + 1 >= 1 entries")
         n = n1 - 1
         if max_len is None:
-            if n == 0:
-                max_len = 1
-            elif _is_torch(ok_):
-                import torch
-                o = ok_.view(torch.int64)
-                max_len = int((o[1:] - o[:-1]).max().item())
-            else:
-                max_len = int((ok_[1:].astype(np.int64) - ok_[:-1].astype(np.int64)).max())
-            max_len = max(max_len, 1)
-        shape = (n, int(out_len), 4)
-        res = self._out_like(dk, shape) if out is None else self._check_out(out, shape, dk)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._vlrej = self._counter(flags)
+            max_len = self._longest_item(ok_, n)
+        res = self._result(out, (n, int(out_len), 4), dk)
+        flags = self._flags(flags, async_)
+        rejected = self._counter("varlen_rejected", flags)
         self._check(self._lib.p252_hash_batch_varlen(self._ctx, int(domain), dp, int(dlead[0]), op, n, int(max_len),
-                                                     self._ptr(res), int(out_len), ctypes.byref(self._vlrej), flags))
+                                                     self._ptr(res), int(out_len), ctypes.byref(rejected), flags))
         return res
 
     def last_varlen_rejected(self):
         """Items of the last hash_batch_varlen skipped as invalid (device buffers; sync() first after async_)."""
-        return int(getattr(self, "_vlrej", ctypes.c_size_t(0)).value)
+        return self._last("varlen_rejected")
 
     def scalars_from_bytes(self, data, async_=False):
         """(n, 32) uint8 canonical little-endian (host) or (n, 4) 64-bit device tensor of the same bytes
         -> (scalars (n, 4), ok (n,) uint8); ok == 0 where the value is >= p."""
         if _is_torch(data):
-            import torch
             ptr, lead, flags, keep = self._in(data, (4,))
             n = lead[0]
-            out = torch.empty((n, 4), dtype=keep.dtype, device=keep.device)
-            ok = torch.empty((n,), dtype=torch.uint8, device=keep.device)
         else:
             keep = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1, 32)
             ptr, n, flags = keep.ctypes.data, keep.shape[0], _native.MEM_HOST
-            out = np.empty((n, 4), dtype=np.uint64)
-            ok = np.empty((n,), dtype=np.uint8)
+        out = self._out_like(keep, (n, 4))
+        ok = self._ok_like(keep, n)
         self._check(self._lib.p252_scalars_from_bytes(self._ctx, ptr, n, self._ptr(out), self._ptr(ok),
-                                                      flags | (_native.ASYNC if async_ and flags else 0)))
+                                                      self._flags(flags, async_)))
         return out, ok
 
     def scalars_to_bytes(self, scalars, async_=False):
         """(n, 4) scalars -> canonical little-endian bytes: (n, 32) uint8 (host) or (n, 4) device tensor."""
         ptr, lead, flags, keep = self._in(scalars, (4,))
         n = lead[0]
-        if _is_torch(keep):
-            import torch
-            out = torch.empty((n, 4), dtype=keep.dtype, device=keep.device)
-        else:
-            out = np.empty((n, 32), dtype=np.uint8)
-        self._check(self._lib.p252_scalars_to_bytes(self._ctx, ptr, n, self._ptr(out),
-                                                    flags | (_native.ASYNC if async_ and flags else 0)))
+        out = self._out_like(keep, (n, 4)) if _is_torch(keep) else np.empty((n, 32), dtype=np.uint8)
+        self._check(self._lib.p252_scalars_to_bytes(self._ctx, ptr, n, self._ptr(out), self._flags(flags, async_)))
         return out
 
     def encrypt_batch(self, messages, secrets_uv, nonces, out=None, async_=False):
@@ -275,13 +304,11 @@ class Engine:
         n = lead[0]
         sp, l2, f2, sk = self._in(secrets_uv, (2, 4))
         np_, l3, f3, nk = self._in(nonces, (4,))
-        if not (flags == f2 == f3):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2, f3)
         self._same_lead("secrets_uv", l2, n)
         self._same_lead("nonces", l3, n)
-        res = self._out_like(mk, (n, L + 1, 4)) if out is None else self._check_out(out, (n, L + 1, 4), mk)
-        self._check(self._lib.p252_encrypt_batch(self._ctx, mp, n, L, sp, np_, self._ptr(res),
-                                                 flags | (_native.ASYNC if async_ and flags else 0)))
+        res = self._result(out, (n, L + 1, 4), mk)
+        self._check(self._lib.p252_encrypt_batch(self._ctx, mp, n, L, sp, np_, self._ptr(res), self._flags(flags, async_)))
         return res
 
     def decrypt_batch(self, ciphers, secrets_uv, nonces, async_=False):
@@ -291,31 +318,23 @@ class Engine:
         n = lead[0]
         sp, l2, f2, sk = self._in(secrets_uv, (2, 4))
         np_, l3, f3, nk = self._in(nonces, (4,))
-        if not (flags == f2 == f3):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2, f3)
         self._same_lead("secrets_uv", l2, n)
         self._same_lead("nonces", l3, n)
         if L < 1:
             raise EngineError(-1, "ciphers must hold at least one message scalar plus the authentication scalar")
-        if _is_torch(ck):
-            import torch
-            msg = torch.empty((n, max(L, 0), 4), dtype=ck.dtype, device=ck.device)
-            ok = torch.empty((n,), dtype=torch.uint8, device=ck.device)
-        else:
-            msg = np.empty((n, max(L, 0), 4), dtype=np.uint64)
-            ok = np.empty((n,), dtype=np.uint8)
-        # the failure count is written through this pointer after the stream reaches it (immediately for
-        # synchronous calls): keep it alive on the engine, read it with last_decrypt_failures()
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nfail = self._counter(flags)
-        self._check(self._lib.p252_decrypt_batch(self._ctx, cp, n, max(L, 0), sp, np_, self._ptr(msg), self._ptr(ok),
-                                                 ctypes.byref(self._nfail), flags))
+        msg = self._out_like(ck, (n, L, 4))
+        ok = self._ok_like(ck, n)
+        flags = self._flags(flags, async_)
+        failed = self._counter("decrypt_failures", flags)
+        self._check(self._lib.p252_decrypt_batch(self._ctx, cp, n, L, sp, np_, self._ptr(msg), self._ptr(ok),
+                                                 ctypes.byref(failed), flags))
         return msg, ok
 
     def last_decrypt_failures(self):
         """Items of the last decrypt_batch or decrypt_batch_varlen whose authentication failed (counted on the device for
         device buffers; after an async_ call, sync() first)."""
-        return int(getattr(self, "_nfail", ctypes.c_size_t(0)).value)
+        return self._last("decrypt_failures")
 
     # -- JubJub key exchange ----------------------------------------------------------------------
     def _dhke_args(self, secrets, publics, n=None):
@@ -324,8 +343,7 @@ class Engine:
         is 1 (broadcast) or n.  n: the batch size the other buffers fix, or None to take it from these two."""
         sp, sl, fs, sk = self._in(secrets, (4,))
         pp, pl, fp, pk = self._in(publics, (2, 4))
-        if fs != fp:
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(fs, fp)
         if len(sl) != 1 or len(pl) != 1:
             raise EngineError(-1, "secrets must have shape (n_secret, 4) and publics (n_public, 2, 4)")
         ns, npub = int(sl[0]), int(pl[0])
@@ -343,21 +361,17 @@ class Engine:
         counted in last_dhke_invalid()."""
         sp, ns, pp, npub, n, flags, keep = self._dhke_args(secrets, publics)
         like = keep[1]
-        res = self._out_like(like, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), like)
-        if _is_torch(like):
-            import torch
-            ok = torch.empty((n,), dtype=torch.uint8, device=like.device)
-        else:
-            ok = np.empty((n,), dtype=np.uint8)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._ninv = self._counter(flags)
+        res = self._result(out, (n, 2, 4), like)
+        ok = self._ok_like(like, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("dhke_invalid", flags)
         self._check(self._lib.p252_dhke_batch(self._ctx, sp, ns, pp, npub, n, self._ptr(res), self._ptr(ok),
-                                              ctypes.byref(self._ninv), flags))
+                                              ctypes.byref(invalid), flags))
         return res, ok
 
     def last_dhke_invalid(self):
         """Invalid items of the last dhke_batch or encrypt_batch_dhke (sync() first after async_)."""
-        return int(getattr(self, "_ninv", ctypes.c_size_t(0)).value)
+        return self._last("dhke_invalid")
 
     def _crypt_dhke(self, decrypt, data, secrets, publics, nonces, out, async_):
         L = int(data.shape[1]) - (1 if decrypt else 0)
@@ -370,24 +384,13 @@ class Engine:
         n = lead[0]
         sp, ns, pp, npub, _, f2, keep = self._dhke_args(secrets, publics, n)
         np_, l3, f3, nk = self._in(nonces, (4,))
-        if not (flags == f2 == f3):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2, f3)
         self._same_lead("nonces", l3, n)
-        shape = (n, L if decrypt else L + 1, 4)
-        res = self._out_like(dk, shape) if out is None else self._check_out(out, shape, dk)
-        if _is_torch(dk):
-            import torch
-            ok = torch.empty((n,), dtype=torch.uint8, device=dk.device)
-        else:
-            ok = np.empty((n,), dtype=np.uint8)
-        flags |= _native.ASYNC if async_ and flags else 0
-        cnt = self._counter(flags)
-        if decrypt:
-            self._nfail = cnt
-            fn = self._lib.p252_decrypt_batch_dhke
-        else:
-            self._ninv = cnt
-            fn = self._lib.p252_encrypt_batch_dhke
+        res = self._result(out, (n, L if decrypt else L + 1, 4), dk)
+        ok = self._ok_like(dk, n)
+        flags = self._flags(flags, async_)
+        cnt = self._counter("decrypt_failures" if decrypt else "dhke_invalid", flags)
+        fn = self._lib.p252_decrypt_batch_dhke if decrypt else self._lib.p252_encrypt_batch_dhke
         self._check(fn(self._ctx, dp, n, L, sp, ns, pp, npub, np_, self._ptr(res), self._ptr(ok), ctypes.byref(cnt), flags))
         return res, ok
 
@@ -405,21 +408,11 @@ class Engine:
         return self._crypt_dhke(True, ciphers, secrets, publics, nonces, out, async_)
 
     # -- fixed-base JubJub scalar multiplication --------------------------------------------------
-    @staticmethod
-    def _base(base):
+    @classmethod
+    def _base(cls, base):
         """The base point (u, v) as a host (2, 4) uint64 array: the library reads it on the host for every memory space
         (a CUDA tensor is copied; the base is public)."""
-        a = np.ascontiguousarray(base.detach().cpu().numpy() if _is_torch(base) else base)
-        b = a.view(np.uint64) if a.dtype == np.int64 else np.ascontiguousarray(a, dtype=np.uint64)
-        if b.size != 8:
-            raise EngineError(-1, "base must be one point (u, v) of shape (2, 4), got %s" % (b.shape,))
-        return b.reshape(2, 4)
-
-    def _ok_like(self, like, n):
-        if _is_torch(like):
-            import torch
-            return torch.empty((n,), dtype=torch.uint8, device=like.device)
-        return np.empty((n,), dtype=np.uint8)
+        return cls._host_limbs(base, (2, 4), "base must be one point (u, v)")
 
     def fixed_base_batch(self, secrets, base, out=None, async_=False):
         """n x [secret] base for one base point: secrets (n, 4) canonical p252_jscalar rows (scalar.jubjub_limbs), base
@@ -432,12 +425,12 @@ class Engine:
             raise EngineError(-1, "secrets must have shape (n, 4)")
         n = int(sl[0])
         b = self._base(base)
-        res = self._out_like(sk, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), sk)
+        res = self._result(out, (n, 2, 4), sk)
         ok = self._ok_like(sk, n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._ninv = self._counter(flags)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("dhke_invalid", flags)
         self._check(self._lib.p252_fixed_base_batch(self._ctx, b.ctypes.data, sp, n, self._ptr(res), self._ptr(ok),
-                                                    ctypes.byref(self._ninv), flags))
+                                                    ctypes.byref(invalid), flags))
         return res, ok
 
     def encrypt_batch_ephemeral(self, messages, r, base, publics, nonces, out=None, R_out=None, async_=False):
@@ -457,18 +450,17 @@ class Engine:
         if ns != n:
             raise EngineError(-1, "r must have %d rows, got %d" % (n, ns))
         np_, l3, f3, nk = self._in(nonces, (4,))
-        if not (flags == f2 == f3):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2, f3)
         self._same_lead("nonces", l3, n)
         b = self._base(base)
-        res = self._out_like(dk, (n, L + 1, 4)) if out is None else self._check_out(out, (n, L + 1, 4), dk)
-        R = self._out_like(dk, (n, 2, 4)) if R_out is None else self._check_out(R_out, (n, 2, 4), dk)
+        res = self._result(out, (n, L + 1, 4), dk)
+        R = self._result(R_out, (n, 2, 4), dk)
         ok = self._ok_like(dk, n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._ninv = self._counter(flags)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("dhke_invalid", flags)
         self._check(self._lib.p252_encrypt_batch_ephemeral(self._ctx, dp, n, L, sp, b.ctypes.data, pp, npub, np_,
                                                            self._ptr(res), self._ptr(R), self._ptr(ok),
-                                                           ctypes.byref(self._ninv), flags))
+                                                           ctypes.byref(invalid), flags))
         return res, R, ok
 
     # -- stealth addresses ------------------------------------------------------------------------
@@ -483,19 +475,18 @@ class Engine:
         n = int(r.shape[0])
         sp, _, ap, na, _, flags, keep = self._dhke_args(r, publics_A, n)
         bp, bl, fb, bk = self._in(publics_B, (2, 4))
-        if fb != flags:
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, fb)
         if tuple(bl) != (na,):
             raise EngineError(-1, "publics_B must have %d rows like publics_A, got leading shape %s" % (na, tuple(bl)))
         b = self._base(base)
         like = keep[0]
-        R = self._out_like(like, (n, 2, 4)) if R_out is None else self._check_out(R_out, (n, 2, 4), like)
-        pk = self._out_like(like, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), like)
+        R = self._result(R_out, (n, 2, 4), like)
+        pk = self._result(out, (n, 2, 4), like)
         ok = self._ok_like(like, n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nsinv = self._counter(flags)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("stealth_invalid", flags)
         self._check(self._lib.p252_stealth_address_batch(self._ctx, sp, n, b.ctypes.data, ap, bp, na, self._ptr(R),
-                                                         self._ptr(pk), self._ptr(ok), ctypes.byref(self._nsinv), flags))
+                                                         self._ptr(pk), self._ptr(ok), ctypes.byref(invalid), flags))
         return R, pk, ok
 
     def stealth_owns_batch(self, view_a, spend_B, base, R, note_pk, out=None, async_=False):
@@ -510,27 +501,26 @@ class Engine:
         n = rl[0]
         pp, pl, fp, pk = self._in(note_pk, (2, 4))
         vp, vl, fv, vk = self._in(view_a, (4,))
-        if not (flags == fp == fv):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, fp, fv)
         self._same_lead("note_pk", pl, n)
         if tuple(vl) not in ((), (1,)):
             raise EngineError(-1, "view_a must be one p252_jscalar row, got leading shape %s" % (tuple(vl),))
         b, g = self._base(spend_B), self._base(base)
-        owned = self._ok_like(rk, n) if out is None else self._check_out(out, (n,), rk, itemsize=1)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nowned, self._nsinv = self._counter(flags), self._counter(flags)
+        owned = self._result(out, (n,), rk, itemsize=1)
+        flags = self._flags(flags, async_)
+        n_owned, invalid = self._counter("stealth_owned", flags), self._counter("stealth_invalid", flags)
         self._check(self._lib.p252_stealth_owns_batch(self._ctx, vp, b.ctypes.data, g.ctypes.data, rp, pp, n,
-                                                      self._ptr(owned), ctypes.byref(self._nowned),
-                                                      ctypes.byref(self._nsinv), flags))
+                                                      self._ptr(owned), ctypes.byref(n_owned), ctypes.byref(invalid),
+                                                      flags))
         return owned
 
     def last_stealth_owned(self):
         """Owned notes of the last stealth_owns_batch (sync() first after async_)."""
-        return int(getattr(self, "_nowned", ctypes.c_size_t(0)).value)
+        return self._last("stealth_owned")
 
     def last_stealth_invalid(self):
         """Invalid items of the last stealth_address_batch or stealth_owns_batch (sync() first after async_)."""
-        return int(getattr(self, "_nsinv", ctypes.c_size_t(0)).value)
+        return self._last("stealth_invalid")
 
     # -- Schnorr signatures -----------------------------------------------------------------------
     def schnorr_sign_batch(self, sk, r, msg, base, u_out=None, R_out=None, async_=False):
@@ -545,19 +535,18 @@ class Engine:
         n = int(rl[0])
         sp, sl, fs, skk = self._in(sk, (4,))
         mp, ml, fm, mk = self._in(msg, (4,))
-        if not (flags == fs == fm):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, fs, fm)
         if len(sl) != 1 or int(sl[0]) not in (1, n):
             raise EngineError(-1, "sk must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(sl)))
         self._same_lead("msg", ml, n)
         b = self._base(base)
-        u = self._out_like(rk, (n, 4)) if u_out is None else self._check_out(u_out, (n, 4), rk)
-        R = self._out_like(rk, (n, 2, 4)) if R_out is None else self._check_out(R_out, (n, 2, 4), rk)
+        u = self._result(u_out, (n, 4), rk)
+        R = self._result(R_out, (n, 2, 4), rk)
         ok = self._ok_like(rk, n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nschinv = self._counter(flags)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("schnorr_invalid", flags)
         self._check(self._lib.p252_schnorr_sign_batch(self._ctx, sp, int(sl[0]), rp, mp, n, b.ctypes.data, self._ptr(u),
-                                                      self._ptr(R), self._ptr(ok), ctypes.byref(self._nschinv), flags))
+                                                      self._ptr(R), self._ptr(ok), ctypes.byref(invalid), flags))
         return u, R, ok
 
     def schnorr_verify_batch(self, pk, u, R, msg, base, out=None, async_=False):
@@ -573,28 +562,27 @@ class Engine:
         pp, pl, fp, pkk = self._in(pk, (2, 4))
         Rp, Rl, fR, Rk = self._in(R, (2, 4))
         mp, ml, fm, mk = self._in(msg, (4,))
-        if not (flags == fp == fR == fm):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, fp, fR, fm)
         if len(pl) != 1 or int(pl[0]) not in (1, n):
             raise EngineError(-1, "pk must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(pl)))
         self._same_lead("R", Rl, n)
         self._same_lead("msg", ml, n)
         b = self._base(base)
-        verified = self._ok_like(uk, n) if out is None else self._check_out(out, (n,), uk, itemsize=1)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nschok, self._nschinv = self._counter(flags), self._counter(flags)
+        verified = self._result(out, (n,), uk, itemsize=1)
+        flags = self._flags(flags, async_)
+        n_verified, invalid = self._counter("schnorr_verified", flags), self._counter("schnorr_invalid", flags)
         self._check(self._lib.p252_schnorr_verify_batch(self._ctx, pp, int(pl[0]), up, Rp, mp, n, b.ctypes.data,
-                                                        self._ptr(verified), ctypes.byref(self._nschok),
-                                                        ctypes.byref(self._nschinv), flags))
+                                                        self._ptr(verified), ctypes.byref(n_verified),
+                                                        ctypes.byref(invalid), flags))
         return verified
 
     def last_schnorr_verified(self):
         """Verified signatures of the last schnorr_verify_batch (sync() first after async_)."""
-        return int(getattr(self, "_nschok", ctypes.c_size_t(0)).value)
+        return self._last("schnorr_verified")
 
     def last_schnorr_invalid(self):
         """Invalid items of the last schnorr_sign_batch or schnorr_verify_batch (sync() first after async_)."""
-        return int(getattr(self, "_nschinv", ctypes.c_size_t(0)).value)
+        return self._last("schnorr_invalid")
 
     # -- point compression ------------------------------------------------------------------------
     def points_from_bytes(self, data, out=None, async_=False):
@@ -611,12 +599,12 @@ class Engine:
             if keep.ndim != 2 or keep.shape[1] != 32:
                 raise EngineError(-1, "host bytes must have shape (n, 32), got %s" % (keep.shape,))
             ptr, n, flags = keep.ctypes.data, int(keep.shape[0]), _native.MEM_HOST
-        res = self._out_like(keep, (n, 2, 4)) if out is None else self._check_out(out, (n, 2, 4), keep)
+        res = self._result(out, (n, 2, 4), keep)
         ok = self._ok_like(keep, n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nptinv = self._counter(flags)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("points_invalid", flags)
         self._check(self._lib.p252_points_from_bytes(self._ctx, ptr, n, self._ptr(res), self._ptr(ok),
-                                                     ctypes.byref(self._nptinv), flags))
+                                                     ctypes.byref(invalid), flags))
         return res, ok
 
     def points_to_bytes(self, points, async_=False):
@@ -629,20 +617,20 @@ class Engine:
         n = int(pl[0])
         res = self._out_like(pk, (n, 4)) if _is_torch(pk) else np.empty((n, 32), dtype=np.uint8)
         ok = self._ok_like(pk, n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nptinv = self._counter(flags)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("points_invalid", flags)
         self._check(self._lib.p252_points_to_bytes(self._ctx, pp, n, self._ptr(res), self._ptr(ok),
-                                                   ctypes.byref(self._nptinv), flags))
+                                                   ctypes.byref(invalid), flags))
         return res, ok
 
     def last_points_invalid(self):
         """Invalid items of the last points_from_bytes or points_to_bytes (sync() first after async_)."""
-        return int(getattr(self, "_nptinv", ctypes.c_size_t(0)).value)
+        return self._last("points_invalid")
 
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
-        max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive).  key_extra: scalars an item carries
-        beyond its message (0 for messages, 1 for ciphers)."""
+        max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive, secrets and nonces keepalives).
+        key_extra: scalars an item carries beyond its message (0 for messages, 1 for ciphers)."""
         dp, dlead, flags, dk = self._in(data, (4,))
         if len(dlead) != 1:
             raise EngineError(-1, "data must have shape (n_scalars, 4), got leading shape %s" % (tuple(dlead),))
@@ -652,21 +640,12 @@ class Engine:
         n = n1 - 1
         sp, l2, f2, sk = self._in(secrets_uv, (2, 4))
         np_, l3, f3, nk = self._in(nonces, (4,))
-        if not (flags == f2 == f3):
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2, f3)
         self._same_lead("secrets_uv", l2, n)
         self._same_lead("nonces", l3, n)
         if max_len is None:
-            if n == 0:
-                max_len = 1
-            elif _is_torch(ok_):
-                import torch
-                o = ok_.view(torch.int64)
-                max_len = int((o[1:] - o[:-1]).max().item()) - key_extra
-            else:
-                max_len = int((ok_[1:].astype(np.int64) - ok_[:-1].astype(np.int64)).max()) - key_extra
-            max_len = max(max_len, 1)
-        return dp, int(dlead[0]), op, n, int(max_len), sp, np_, flags, dk, ok_
+            max_len = self._longest_item(ok_, n, key_extra)
+        return dp, int(dlead[0]), op, n, int(max_len), sp, np_, flags, dk, ok_, (sk, nk)
 
     def encrypt_batch_varlen(self, data, offsets, secrets_uv, nonces, max_len=None, out=None, async_=False):
         """n x encrypt(data[offsets[i]:offsets[i+1]], secrets_uv[i], nonces[i]) over messages of any lengths, one call.
@@ -678,13 +657,14 @@ class Engine:
         VARLEN_MAX_LEN); None takes the longest, which for CUDA tensors costs a device-to-host sync.  Host batches raise on
         an invalid item and write nothing; device batches skip invalid items, write nothing for them and count them
         (last_crypt_rejected())."""
-        dp, ns, op, n, max_len, sp, np_, flags, dk, ok_ = self._crypt_varlen_args(data, offsets, secrets_uv, nonces, max_len, 0)
+        dp, ns, op, n, max_len, sp, np_, flags, dk, ok_, keep = self._crypt_varlen_args(data, offsets, secrets_uv, nonces,
+                                                                                         max_len, 0)
         rows = ns + n
-        res = self._out_like(dk, (max(rows, 1), 4))[:rows] if out is None else self._check_out(out, (rows, 4), dk)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._crej = self._counter(flags)
+        res = self._rows_like(dk, rows) if out is None else self._check_out(out, (rows, 4), dk)
+        flags = self._flags(flags, async_)
+        rejected = self._counter("crypt_rejected", flags)
         self._check(self._lib.p252_encrypt_batch_varlen(self._ctx, dp, ns, op, n, max_len, sp, np_, self._ptr(res),
-                                                        ctypes.byref(self._crej), flags))
+                                                        ctypes.byref(rejected), flags))
         return res, varlen_out_offsets(ok_, 1)
 
     def decrypt_batch_varlen(self, ciphers, offsets, secrets_uv, nonces, max_len=None, async_=False):
@@ -694,27 +674,20 @@ class Engine:
         cipher), packed from 0 in max(n_scalars - n, 0) rows; ok[i] == 0 where the reference returns
         Error::DecryptionFailed (that message is zeroed) or, for device buffers, the item was invalid and skipped.  Failure
         count: last_decrypt_failures(); invalid device items: last_crypt_rejected()."""
-        cp, ns, op, n, max_len, sp, np_, flags, ck, ok_ = self._crypt_varlen_args(ciphers, offsets, secrets_uv, nonces,
-                                                                                   max_len, 1)
-        rows = max(ns - n, 0)
-        msg = self._out_like(ck, (max(rows, 1), 4))[:rows]          # never a NULL pointer, even for zero rows
-        if _is_torch(ck):
-            import torch
-            ok = torch.empty((n,), dtype=torch.uint8, device=ck.device)
-        else:
-            ok = np.empty((n,), dtype=np.uint8)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._nfail = self._counter(flags)
-        self._crej = self._counter(flags)
+        cp, ns, op, n, max_len, sp, np_, flags, ck, ok_, keep = self._crypt_varlen_args(ciphers, offsets, secrets_uv,
+                                                                                         nonces, max_len, 1)
+        msg = self._rows_like(ck, max(ns - n, 0))
+        ok = self._ok_like(ck, n)
+        flags = self._flags(flags, async_)
+        failed, rejected = self._counter("decrypt_failures", flags), self._counter("crypt_rejected", flags)
         self._check(self._lib.p252_decrypt_batch_varlen(self._ctx, cp, ns, op, n, max_len, sp, np_, self._ptr(msg),
-                                                        self._ptr(ok), ctypes.byref(self._nfail), ctypes.byref(self._crej),
-                                                        flags))
+                                                        self._ptr(ok), ctypes.byref(failed), ctypes.byref(rejected), flags))
         return msg, varlen_out_offsets(ok_, -1), ok
 
     def last_crypt_rejected(self):
         """Items of the last encrypt_batch_varlen / decrypt_batch_varlen skipped as invalid (device buffers; sync() first
         after async_)."""
-        return int(getattr(self, "_crej", ctypes.c_size_t(0)).value)
+        return self._last("crypt_rejected")
 
     # -- arity-4 Merkle tree ----------------------------------------------------------------------
     def merkle4_level(self, children, out=None, async_=False):
@@ -724,9 +697,8 @@ class Engine:
         if lead[0] % 4:
             from .errors import IOPatternViolation
             raise IOPatternViolation()
-        res = self._out_like(ck, (m, 4)) if out is None else self._check_out(out, (m, 4), ck)
-        self._check(self._lib.p252_merkle4_level(self._ctx, cp, m, self._ptr(res),
-                                                 flags | (_native.ASYNC if async_ and flags else 0)))
+        res = self._result(out, (m, 4), ck)
+        self._check(self._lib.p252_merkle4_level(self._ctx, cp, m, self._ptr(res), self._flags(flags, async_)))
         return res
 
     def tree_nodes(self, n_leaves):
@@ -738,9 +710,8 @@ class Engine:
         """leaves (4^k, 4) -> all internal nodes bottom-up ((4^k-1)/3, 4); root = last row."""
         lp, lead, flags, lk = self._in(leaves, (4,))
         n_internal, _ = self.tree_nodes(lead[0])
-        res = self._out_like(lk, (n_internal, 4)) if out is None else self._check_out(out, (n_internal, 4), lk)
-        self._check(self._lib.p252_merkle4_build(self._ctx, lp, lead[0], self._ptr(res),
-                                                 flags | (_native.ASYNC if async_ and flags else 0)))
+        res = self._result(out, (n_internal, 4), lk)
+        self._check(self._lib.p252_merkle4_build(self._ctx, lp, lead[0], self._ptr(res), self._flags(flags, async_)))
         return res
 
     def merkle_build(self, leaves, arity=4, out=None, async_=False):
@@ -748,9 +719,9 @@ class Engine:
         lp, lead, flags, lk = self._in(leaves, (4,))
         ni = ctypes.c_size_t(0)
         self._check(self._lib.p252_merkle_tree_nodes(int(arity), lead[0], ctypes.byref(ni), None))
-        res = self._out_like(lk, (int(ni.value), 4)) if out is None else self._check_out(out, (int(ni.value), 4), lk)
+        res = self._result(out, (int(ni.value), 4), lk)
         self._check(self._lib.p252_merkle_build(self._ctx, int(arity), lp, lead[0], self._ptr(res),
-                                                flags | (_native.ASYNC if async_ and flags else 0)))
+                                                self._flags(flags, async_)))
         return res
 
     # -- Merkle openings --------------------------------------------------------------------------
@@ -768,17 +739,14 @@ class Engine:
         (n, d, arity, 4) -- for every level the whole sibling group of the path node (poseidon-merkle `Opening`)."""
         lp, lead, flags, lk = self._in(leaves, (4,))
         np_, nlead, f2, nk = self._in(nodes, (4,))
-        if flags != f2:
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2)
         ni, nl = ctypes.c_size_t(0), ctypes.c_int(0)
         self._check(self._lib.p252_merkle_tree_nodes(int(arity), lead[0], ctypes.byref(ni), ctypes.byref(nl)))
         self._same_lead("nodes", nlead, int(ni.value))
         ip, n, ik = self._idx(leaf_idx, lk)
-        depth = int(nl.value)
-        shape = (n, depth, int(arity), 4)
-        res = self._out_like(lk, shape) if out is None else self._check_out(out, shape, lk)
+        res = self._result(out, (n, int(nl.value), int(arity), 4), lk)
         self._check(self._lib.p252_merkle_open_batch(self._ctx, int(arity), lp, lead[0], np_, ip, n, self._ptr(res),
-                                                     flags | (_native.ASYNC if async_ and flags else 0)))
+                                                     self._flags(flags, async_)))
         return res
 
     def merkle_verify_batch(self, leaf_items, leaf_idx, paths, root, arity=4, async_=False):
@@ -790,46 +758,52 @@ class Engine:
         pp, plead, flags, pk = self._in(paths, (depth, int(arity), 4))
         n = plead[0]
         lp, llead, f2, lk = self._in(leaf_items, (4,))
-        if flags != f2:
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2)
         self._same_lead("leaf_items", llead, n)
         ip, ni, ik = self._idx(leaf_idx, pk)
         if ni != n:
             raise EngineError(-1, "leaf_idx must have %d entries" % n)
-        if _is_torch(root):
-            root = root.detach().cpu().numpy()
-        root = np.ascontiguousarray(root)
-        root = (root.view(np.uint64) if root.dtype == np.int64 else root.astype(np.uint64)).reshape(4)
-        if _is_torch(pk):
-            import torch
-            ok = torch.empty((n,), dtype=torch.uint8, device=pk.device)
-        else:
-            ok = np.empty((n,), dtype=np.uint8)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._vfail = self._counter(flags)
+        root = self._host_limbs(root, (4,), "root must be one scalar")
+        ok = self._ok_like(pk, n)
+        flags = self._flags(flags, async_)
+        failed = self._counter("verify_failures", flags)
         self._check(self._lib.p252_merkle_verify_batch(self._ctx, int(arity), depth, lp, ip, pp, root.ctypes.data, n,
-                                                       self._ptr(ok), ctypes.byref(self._vfail), flags))
+                                                       self._ptr(ok), ctypes.byref(failed), flags))
         return ok
 
     def last_verify_failures(self):
-        return int(getattr(self, "_vfail", ctypes.c_size_t(0)).value)
+        return self._last("verify_failures")
+
+    def _open_batch(self, describe, fn, tree, idx, name, out, async_):
+        """The openings of a tree with a descriptor: `describe` is _mtree, _smtree or _ctree, fn its open_batch call."""
+        t, flags, keep = describe(tree)
+        ip, n, ik = self._idx(idx, keep[0], name)
+        res = self._result(out, (n, int(tree.height), int(tree.arity), 4), keep[0])
+        self._check(fn(self._ctx, ctypes.byref(t), ip, n, self._ptr(res), self._flags(flags, async_)))
+        return res
 
     # -- fixed-height trees with batched updates (p252_mtree) ------------------------------------------
     def mtree_layout(self, arity, height, capacity):
         return mtree_layout(arity, height, capacity)
 
-    def _mtree(self, tree):
-        """tree: anything with arity / height / capacity / n_leaves / leaves (leaf_slots, 4) / nodes (node_slots, 4)
-        -> (p252_mtree, flags, keepalive)."""
+    def _tree_buffers(self, tree):
+        """The leaves (leaf_slots, 4) and nodes (node_slots, 4) of a p252_mtree / p252_smtree -> (leaf pointer, node
+        pointer, flags, leaves, nodes, leaf_slots + node_slots).  The library writes through them, so host buffers must
+        be the caller's own arrays: a converted copy would take the update and be dropped."""
         leaf_slots, node_slots, _ = self.mtree_layout(tree.arity, tree.height, tree.capacity)
         lp, llead, flags, lk = self._in(tree.leaves, (4,))
         np_, nlead, f2, nk = self._in(tree.nodes, (4,))
-        if flags != f2:
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, f2)
         self._same_lead("leaves", llead, leaf_slots)
         self._same_lead("nodes", nlead, node_slots)
         if not _is_torch(lk) and (lk is not tree.leaves or nk is not tree.nodes or not lk.flags.writeable or not nk.flags.writeable):
             raise EngineError(-1, "host tree buffers must be writable C-contiguous uint64 arrays")
+        return lp, np_, flags, lk, nk, leaf_slots + node_slots
+
+    def _mtree(self, tree):
+        """tree: anything with arity / height / capacity / n_leaves / leaves (leaf_slots, 4) / nodes (node_slots, 4)
+        -> (p252_mtree, flags, keepalive)."""
+        lp, np_, flags, lk, nk, _ = self._tree_buffers(tree)
         t = _native.MTree(ctypes.sizeof(_native.MTree), int(tree.arity), int(tree.height), 0, int(tree.capacity),
                           int(tree.n_leaves), lp, np_)
         return t, flags, (lk, nk)
@@ -837,7 +811,7 @@ class Engine:
     def mtree_build(self, tree, async_=False):
         """Rebuild every node of `tree` from its occupied leaf prefix."""
         t, flags, keep = self._mtree(tree)
-        self._check(self._lib.p252_mtree_build(self._ctx, ctypes.byref(t), flags | (_native.ASYNC if async_ and flags else 0)))
+        self._check(self._lib.p252_mtree_build(self._ctx, ctypes.byref(t), self._flags(flags, async_)))
 
     def mtree_update(self, tree, idx=None, values=None, append=None, async_=False):
         """Overwrite leaves idx[i] with values[i] (n, 4) -- the last write to a leaf wins -- and append the rows of
@@ -850,35 +824,27 @@ class Engine:
         if idx is not None or values is not None:
             ip, n_upd, ik = self._idx(idx, like)
             vp, vlead, fv, vk = self._in(values, (4,))
-            if fv != flags:
-                raise EngineError(-1, "all buffers must live in the same memory space")
+            self._same_space(flags, fv)
             self._same_lead("values", vlead, n_upd)
         if append is not None:
             ap, alead, fa, ak = self._in(append, (4,))
-            if fa != flags:
-                raise EngineError(-1, "all buffers must live in the same memory space")
+            self._same_space(flags, fa)
             n_app = int(alead[0])
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._ufail = self._counter(flags)
+        flags = self._flags(flags, async_)
+        rejected = self._counter("update_rejected", flags)
         self._check(self._lib.p252_mtree_update(self._ctx, ctypes.byref(t), ip if n_upd else None, vp if n_upd else None,
-                                                n_upd, ap if n_app else None, n_app, ctypes.byref(self._ufail), flags))
+                                                n_upd, ap if n_app else None, n_app, ctypes.byref(rejected), flags))
         tree.n_leaves = int(t.n_leaves)
         return tree.n_leaves
 
     def last_update_rejected(self):
         """Updates of the last mtree_update skipped for an index >= n_leaves (device buffers; sync() first after async_)."""
-        return int(getattr(self, "_ufail", ctypes.c_size_t(0)).value)
+        return self._last("update_rejected")
 
     def mtree_open_batch(self, tree, leaf_idx, out=None, async_=False):
         """Openings of leaves `leaf_idx`: (n, height, arity, 4), zero slots beyond each level's prefix; they verify with
         merkle_verify_batch (depth = height)."""
-        t, flags, keep = self._mtree(tree)
-        ip, n, ik = self._idx(leaf_idx, keep[0])
-        shape = (n, int(tree.height), int(tree.arity), 4)
-        res = self._out_like(keep[0], shape) if out is None else self._check_out(out, shape, keep[0])
-        self._check(self._lib.p252_mtree_open_batch(self._ctx, ctypes.byref(t), ip, n, self._ptr(res),
-                                                    flags | (_native.ASYNC if async_ and flags else 0)))
-        return res
+        return self._open_batch(self._mtree, self._lib.p252_mtree_open_batch, tree, leaf_idx, "leaf_idx", out, async_)
 
     # -- sparse fixed-height trees: inserts and removals at any position (p252_smtree) -----------------------------
     def _bytes(self, x, like, name, n, writable=False):
@@ -904,16 +870,8 @@ class Engine:
     def _smtree(self, tree):
         """tree: anything with arity / height / capacity / leaves (leaf_slots, 4) / nodes (node_slots, 4) / present
         (leaf_slots + node_slots,) uint8 -> (p252_smtree, flags, keepalive)."""
-        leaf_slots, node_slots, _ = self.mtree_layout(tree.arity, tree.height, tree.capacity)
-        lp, llead, flags, lk = self._in(tree.leaves, (4,))
-        np_, nlead, f2, nk = self._in(tree.nodes, (4,))
-        if flags != f2:
-            raise EngineError(-1, "all buffers must live in the same memory space")
-        self._same_lead("leaves", llead, leaf_slots)
-        self._same_lead("nodes", nlead, node_slots)
-        if not _is_torch(lk) and (lk is not tree.leaves or nk is not tree.nodes or not lk.flags.writeable or not nk.flags.writeable):
-            raise EngineError(-1, "host tree buffers must be writable C-contiguous uint64 arrays")
-        pp, pk = self._bytes(tree.present, lk, "present", leaf_slots + node_slots, writable=True)
+        lp, np_, flags, lk, nk, slots = self._tree_buffers(tree)
+        pp, pk = self._bytes(tree.present, lk, "present", slots, writable=True)
         t = _native.SMTree(ctypes.sizeof(_native.SMTree), int(tree.arity), int(tree.height), 0, int(tree.capacity), lp, np_, pp)
         return t, flags, (lk, nk, pk)
 
@@ -921,35 +879,39 @@ class Engine:
         """Rebuild every node (and node presence byte) of the sparse tree from its leaves and leaf presence bytes; absent
         leaves are zeroed.  Only present nodes are hashed."""
         t, flags, keep = self._smtree(tree)
-        self._check(self._lib.p252_smtree_build(self._ctx, ctypes.byref(t), flags | (_native.ASYNC if async_ and flags else 0)))
+        self._check(self._lib.p252_smtree_build(self._ctx, ctypes.byref(t), self._flags(flags, async_)))
 
-    def smtree_update(self, tree, pos, values=None, op=None, async_=False):
-        """One batch of operations on a sparse tree: op[i] = 0 inserts / overwrites values[i] at pos[i], op[i] = 1 removes
-        pos[i] (op None: all inserts; values None: all zeros, for a batch of removals).  Equal to applying them in batch
-        order.  Device items with pos >= capacity or an op other than 0/1 are skipped and counted
-        (last_smtree_rejected()); host ones raise."""
-        t, flags, keep = self._smtree(tree)
+    def _sparse_update(self, describe, fn, counter, tree, pos, values, op, async_):
+        """One batch of inserts and removals on a sparse tree: `describe` is _smtree or _ctree, fn its update call and
+        `counter` the name its rejected items are counted under."""
+        t, flags, keep = describe(tree)
         like = keep[0]
         ip, n, ik = self._idx(pos, like, "pos")
         if values is None:
             values = self._out_like(like, (n, 4))
             values[:] = 0
             if async_ and flags:
-                self._pending_counters.append(values)      # read by the device after this call returns
+                self._keep_until_sync(values)      # read by the device after this call returns
         vp, vlead, fv, vk = self._in(values, (4,))
-        if fv != flags:
-            raise EngineError(-1, "all buffers must live in the same memory space")
+        self._same_space(flags, fv)
         self._same_lead("values", vlead, n)
         opp, ok_ = (None, None) if op is None else self._bytes(op, like, "op", n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._smrej = self._counter(flags)
-        self._check(self._lib.p252_smtree_update(self._ctx, ctypes.byref(t), ip if n else None, opp if n else None,
-                                                 vp if n else None, n, ctypes.byref(self._smrej), flags))
+        flags = self._flags(flags, async_)
+        rejected = self._counter(counter, flags)
+        self._check(fn(self._ctx, ctypes.byref(t), ip if n else None, opp if n else None, vp if n else None, n,
+                       ctypes.byref(rejected), flags))
+
+    def smtree_update(self, tree, pos, values=None, op=None, async_=False):
+        """One batch of operations on a sparse tree: op[i] = 0 inserts / overwrites values[i] at pos[i], op[i] = 1 removes
+        pos[i] (op None: all inserts; values None: all zeros, for a batch of removals).  Equal to applying them in batch
+        order.  Device items with pos >= capacity or an op other than 0/1 are skipped and counted
+        (last_smtree_rejected()); host ones raise."""
+        self._sparse_update(self._smtree, self._lib.p252_smtree_update, "smtree_rejected", tree, pos, values, op, async_)
 
     def last_smtree_rejected(self):
         """Items of the last smtree_update skipped on the device (pos >= capacity or op not 0/1; sync() first after
         async_)."""
-        return int(getattr(self, "_smrej", ctypes.c_size_t(0)).value)
+        return self._last("smtree_rejected")
 
     def smtree_len(self, tree):
         """Number of present positions (counted on the device for device buffers)."""
@@ -961,13 +923,7 @@ class Engine:
     def smtree_open_batch(self, tree, pos, out=None, async_=False):
         """Openings of the present positions `pos`: (n, height, arity, 4), absent slots zero; they verify with
         merkle_verify_batch (depth = height).  Host: an absent position raises; device: it gets an all-zero opening."""
-        t, flags, keep = self._smtree(tree)
-        ip, n, ik = self._idx(pos, keep[0], "pos")
-        shape = (n, int(tree.height), int(tree.arity), 4)
-        res = self._out_like(keep[0], shape) if out is None else self._check_out(out, shape, keep[0])
-        self._check(self._lib.p252_smtree_open_batch(self._ctx, ctypes.byref(t), ip, n, self._ptr(res),
-                                                     flags | (_native.ASYNC if async_ and flags else 0)))
-        return res
+        return self._open_batch(self._smtree, self._lib.p252_smtree_open_batch, tree, pos, "pos", out, async_)
 
     # -- compact sparse trees: sorted present nodes per level (p252_ctree) --------------------------------------------
     def ctree_layout(self, arity, height, max_leaves):
@@ -1004,39 +960,17 @@ class Engine:
         in batch order.  Device items with pos >= arity^height or an op other than 0/1 are skipped and counted
         (last_ctree_rejected()); a device batch that would leave more than max_leaves present positions changes nothing
         and counts every item as rejected.  Host: either raises and changes nothing."""
-        t, flags, keep = self._ctree(tree)
-        like = keep[0]
-        ip, n, ik = self._idx(pos, like, "pos")
-        if values is None:
-            values = self._out_like(like, (n, 4))
-            values[:] = 0
-            if async_ and flags:
-                self._pending_counters.append(values)      # read by the device after this call returns
-        vp, vlead, fv, vk = self._in(values, (4,))
-        if fv != flags:
-            raise EngineError(-1, "all buffers must live in the same memory space")
-        self._same_lead("values", vlead, n)
-        opp, ok_ = (None, None) if op is None else self._bytes(op, like, "op", n)
-        flags |= _native.ASYNC if async_ and flags else 0
-        self._ctrej = self._counter(flags)
-        self._check(self._lib.p252_ctree_update(self._ctx, ctypes.byref(t), ip if n else None, opp if n else None,
-                                                vp if n else None, n, ctypes.byref(self._ctrej), flags))
+        self._sparse_update(self._ctree, self._lib.p252_ctree_update, "ctree_rejected", tree, pos, values, op, async_)
 
     def last_ctree_rejected(self):
         """Items of the last ctree_update skipped on the device (pos >= arity^height or op not 0/1; all of them when the
         batch would exceed max_leaves; sync() first after async_)."""
-        return int(getattr(self, "_ctrej", ctypes.c_size_t(0)).value)
+        return self._last("ctree_rejected")
 
     def ctree_open_batch(self, tree, pos, out=None, async_=False):
         """Openings of the present positions `pos`: (n, height, arity, 4), absent slots zero; they verify with
         merkle_verify_batch (depth = height).  Host: an absent position raises; device: it gets an all-zero opening."""
-        t, flags, keep = self._ctree(tree)
-        ip, n, ik = self._idx(pos, keep[0], "pos")
-        shape = (n, int(tree.height), int(tree.arity), 4)
-        res = self._out_like(keep[0], shape) if out is None else self._check_out(out, shape, keep[0])
-        self._check(self._lib.p252_ctree_open_batch(self._ctx, ctypes.byref(t), ip, n, self._ptr(res),
-                                                    flags | (_native.ASYNC if async_ and flags else 0)))
-        return res
+        return self._open_batch(self._ctree, self._lib.p252_ctree_open_batch, tree, pos, "pos", out, async_)
 
     def set_small_batch_max(self, max_items):
         """Digest batches up to `max_items` items use the lane-split (5 threads per state) kernel; 0 disables it."""
@@ -1081,9 +1015,9 @@ class Engine:
         if flags != _native.MEM_DEVICE:
             raise EngineError(-1, "merkle4_build_dist takes device tensors")
         n_internal, _ = self.tree_nodes(n_leaves_total)
-        res = self._out_like(lk, (n_internal, 4)) if out is None else self._check_out(out, (n_internal, 4), lk)
+        res = self._result(out, (n_internal, 4), lk)
         self._check(self._lib.p252_merkle4_build_dist(self._ctx, lp, int(n_leaves_total), self._ptr(res),
-                                                      flags | (_native.ASYNC if async_ else 0) |
+                                                      self._flags(flags, async_) |
                                                       (_native.TIMING if timing else 0) | (_native.NO_GATHER if no_gather else 0)))
         return res
 
@@ -1129,3 +1063,9 @@ def default_engine(device=0):
     if device not in _DEFAULT:
         _DEFAULT[device] = Engine(device)
     return _DEFAULT[device]
+
+
+def _engine_for(engine, like=None):
+    """The engine a module-level call runs on: the caller's, else the process-wide one of the device the CUDA tensor
+    `like` lives on (device 0 for host arrays and for no buffer at all)."""
+    return engine or default_engine(like.device.index if hasattr(like, "is_cuda") else 0)

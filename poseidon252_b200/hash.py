@@ -8,7 +8,7 @@ import enum
 import numpy as np
 
 from . import _native
-from .engine import default_engine
+from .engine import _engine_for
 from .errors import raise_for_status
 from .scalar import P, from_mont
 
@@ -105,7 +105,7 @@ class Hash:
         lens = [int(c.shape[0]) for c in self.input]
         pattern = io_pattern(self.domain, lens, self._output_len)
         t = tag(pattern, domain_separator(self.domain))
-        eng = self._engine or default_engine()
+        eng = _engine_for(self._engine)
         data = np.concatenate(self.input, axis=0) if self.input else np.zeros((0, 4), dtype=np.uint64)
         out = eng.digest_batch_with_tag(t, data.reshape(1, -1, 4), self._output_len)
         return out[0]
@@ -120,7 +120,7 @@ class Hash:
             vals = [int(v) & mask for v in from_mont(self.finalize())]
             return np.array([[(v >> (64 * k)) & ((1 << 64) - 1) for k in range(4)] for v in vals], dtype=np.uint64)
         io_pattern(self.domain, lens, self._output_len)
-        eng = self._engine or default_engine()
+        eng = _engine_for(self._engine)
         return eng.hash_batch_truncated(self.domain, self.input[0].reshape(1, -1, 4), self._output_len)[0]
 
     @staticmethod
@@ -142,7 +142,7 @@ class Hash:
         """NEW batch entry: n x Hash::digest_truncated -> (n, out_len, 4) raw limbs (< 2^250)."""
         domain = Domain(domain)
         ol = int(output_len) if (domain == Domain.Other and output_len > 0) else 1
-        eng = engine or default_engine(inputs.device.index if hasattr(inputs, "is_cuda") else 0)
+        eng = _engine_for(engine, inputs)
         return eng.hash_batch_truncated(domain, inputs, ol, out=out, async_=async_)
 
     @staticmethod
@@ -157,7 +157,7 @@ class Hash:
         else:
             data, offsets, longest = pack_varlen(inputs)
             max_len = max(longest, 1) if max_len is None else max_len
-        eng = engine or default_engine(data.device.index if hasattr(data, "is_cuda") else 0)
+        eng = _engine_for(engine, data)
         return eng.hash_batch_varlen(domain, data, offsets, ol, max_len=max_len, out=out, async_=async_)
 
     @staticmethod
@@ -167,5 +167,5 @@ class Hash:
         array (host) or torch CUDA tensor (device).  Returns (n, out_len, 4)."""
         domain = Domain(domain)
         ol = int(output_len) if (domain == Domain.Other and output_len > 0) else 1
-        eng = engine or default_engine(inputs.device.index if hasattr(inputs, "is_cuda") else 0)
+        eng = _engine_for(engine, inputs)
         return eng.hash_batch(domain, inputs, ol, out=out, async_=async_)

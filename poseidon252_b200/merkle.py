@@ -4,36 +4,36 @@ src/hash.rs:22-31).  Tree logic itself left the reference crate in 0.29.0
 fixed-height tree with batched appends and overwrites (p252_mtree), `SparseTree`, a fixed-height tree with batched
 inserts and removals at any position (p252_smtree), and `CompactTree`, the same at any height with storage
 proportional to the present leaves (p252_ctree)."""
-from .engine import _is_torch, default_engine
+from .engine import _engine_for, _is_torch, default_engine
 
 
 def merkle4_level(children, engine=None, out=None, async_=False):
-    eng = engine or default_engine(children.device.index if hasattr(children, "is_cuda") else 0)
+    eng = _engine_for(engine, children)
     return eng.merkle4_level(children, out=out, async_=async_)
 
 
 def merkle4_build(leaves, engine=None, out=None, async_=False):
     """leaves (4^k, 4) -> internal nodes bottom-up, root last."""
-    eng = engine or default_engine(leaves.device.index if hasattr(leaves, "is_cuda") else 0)
+    eng = _engine_for(engine, leaves)
     return eng.merkle4_build(leaves, out=out, async_=async_)
 
 
 def merkle2_build(leaves, engine=None, out=None, async_=False):
     """Binary tree of Domain::Merkle2 digests (src/hash.rs:27-31): leaves (2^k, 4) -> internal nodes, root last."""
-    eng = engine or default_engine(leaves.device.index if hasattr(leaves, "is_cuda") else 0)
+    eng = _engine_for(engine, leaves)
     return eng.merkle_build(leaves, arity=2, out=out, async_=async_)
 
 
 def open_batch(leaves, nodes, leaf_idx, arity=4, engine=None, out=None, async_=False):
     """Openings of the leaves `leaf_idx`: (n, depth, arity, 4) -- per level the whole sibling group of the path
     node, level 0 = the leaf's own group (the `branch` of a poseidon-merkle `Opening`, AGENTS.md:62-66)."""
-    eng = engine or default_engine(leaves.device.index if hasattr(leaves, "is_cuda") else 0)
+    eng = _engine_for(engine, leaves)
     return eng.merkle_open_batch(leaves, nodes, leaf_idx, arity=arity, out=out, async_=async_)
 
 
 def verify_batch(leaf_items, leaf_idx, paths, root, arity=4, engine=None, async_=False):
     """n x Opening::verify on the device (depth chained Merkle digests per item) -> ok (n,) uint8."""
-    eng = engine or default_engine(paths.device.index if hasattr(paths, "is_cuda") else 0)
+    eng = _engine_for(engine, paths)
     return eng.merkle_verify_batch(leaf_items, leaf_idx, paths, root, arity=arity, async_=async_)
 
 
@@ -161,6 +161,20 @@ class Tree:
         return Opening(root, branch, int(i), arity=self.arity)
 
 
+def _remove(update, tree, like, pos, async_):
+    """A batch of removals through the engine's `update` call: an op vector of ones in the memory space of `like`, one
+    of the tree's buffers."""
+    if _is_torch(like):
+        import torch
+        op = torch.ones((len(pos),), dtype=torch.uint8, device=like.device)
+    else:
+        import numpy as np
+        op = np.ones((len(pos),), dtype=np.uint8)
+    update(tree, pos, op=op, async_=async_)
+    if async_ and _is_torch(op):
+        tree.engine._keep_until_sync(op)          # read by the device after the call returns
+
+
 class SparseTree:
     """Sparse fixed-height tree of the poseidon-merkle `Tree<T, H, A>` shape with `insert` and `remove` at any position
     (p252_smtree): each position in [0, capacity) is present or absent; an absent leaf and a node with no present leaf
@@ -200,15 +214,7 @@ class SparseTree:
 
     def remove(self, pos, async_=False):
         """Make the positions `pos` absent (removing an absent position does nothing)."""
-        if _is_torch(self.leaves):
-            import torch
-            op = torch.ones((len(pos),), dtype=torch.uint8, device=self.leaves.device)
-        else:
-            import numpy as np
-            op = np.ones((len(pos),), dtype=np.uint8)
-        self.engine.smtree_update(self, pos, op=op, async_=async_)
-        if async_ and _is_torch(op):
-            self.engine._pending_counters.append(op)          # read by the device after the call returns
+        _remove(self.engine.smtree_update, self, self.leaves, pos, async_)
 
     def build(self, async_=False):
         """Recompute every node from the leaves and `leaf_present` (e.g. after writing them directly)."""
@@ -274,15 +280,7 @@ class CompactTree:
 
     def remove(self, pos, async_=False):
         """Make the positions `pos` absent (removing an absent position does nothing)."""
-        if _is_torch(self.values):
-            import torch
-            op = torch.ones((len(pos),), dtype=torch.uint8, device=self.values.device)
-        else:
-            import numpy as np
-            op = np.ones((len(pos),), dtype=np.uint8)
-        self.engine.ctree_update(self, pos, op=op, async_=async_)
-        if async_ and _is_torch(op):
-            self.engine._pending_counters.append(op)          # read by the device after the call returns
+        _remove(self.engine.ctree_update, self, self.values, pos, async_)
 
     @property
     def root(self):

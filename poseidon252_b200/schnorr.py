@@ -9,7 +9,7 @@ nonce r must be secret, uniformly random and used once: two signatures with one 
 import numpy as np
 
 from .encryption import _jscalar_row
-from .engine import default_engine
+from .engine import _engine_for
 from .errors import InvalidPoint
 
 
@@ -25,7 +25,7 @@ def schnorr_sign(sk, r, msg, base, engine=None):
     """NEW: one signature (u, R) of msg with secret key sk and nonce r.  sk, r: canonical ints < r_J or one p252_jscalar
     row; msg: (4,) BlsScalar.0 limbs; base: (2, 4) -> (u (4,) p252_jscalar, R (2, 4)).  Raises InvalidPoint for sk or
     r >= r_J or msg >= p."""
-    eng = engine or default_engine()
+    eng = _engine_for(engine)
     u, R, ok = eng.schnorr_sign_batch(_jscalar_row(sk), _jscalar_row(r), _fr(msg), base)
     if not ok[0]:
         raise InvalidPoint()
@@ -35,7 +35,7 @@ def schnorr_sign(sk, r, msg, base, engine=None):
 def schnorr_sign_batch(sk, r, msg, base, engine=None, async_=False):
     """NEW: n signatures.  sk (1 or n, 4) and r (n, 4) p252_jscalar rows, msg (n, 4), base (2, 4)
     -> (u (n, 4), R (n, 2, 4), ok (n,) uint8); ok == 0 marks an invalid item, whose rows are zeroed."""
-    eng = engine or default_engine(r.device.index if hasattr(r, "is_cuda") else 0)
+    eng = _engine_for(engine, r)
     return eng.schnorr_sign_batch(sk, r, msg, base, async_=async_)
 
 
@@ -43,7 +43,7 @@ def schnorr_verify(pk, u, R, msg, base, engine=None):
     """NEW: PublicKey::verify for one signature (u, R) of msg -> bool.  pk, R, base: (2, 4) BlsScalar.0 limbs; u: a
     canonical int < r_J or one p252_jscalar row; msg: (4,).  Raises InvalidPoint for u >= r_J, msg >= p, an R coordinate
     >= p, PK not a curve point, or a base off the curve."""
-    eng = engine or default_engine()
+    eng = _engine_for(engine)
     verified = eng.schnorr_verify_batch(_pt(pk), _jscalar_row(u), _pt(R), _fr(msg), base)
     if eng.last_schnorr_invalid():
         raise InvalidPoint()
@@ -53,5 +53,5 @@ def schnorr_verify(pk, u, R, msg, base, engine=None):
 def schnorr_verify_batch(pk, u, R, msg, base, engine=None, async_=False):
     """NEW: n verifications.  pk (1 or n, 2, 4), u (n, 4) p252_jscalar rows, R (n, 2, 4), msg (n, 4), base (2, 4)
     -> verified (n,) uint8 (0 also for an invalid item)."""
-    eng = engine or default_engine(u.device.index if hasattr(u, "is_cuda") else 0)
+    eng = _engine_for(engine, u)
     return eng.schnorr_verify_batch(pk, u, R, msg, base, async_=async_)
