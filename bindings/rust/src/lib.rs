@@ -136,6 +136,10 @@ mod schnorr;
 // (methods on Engine).
 mod points;
 
+// JubJub multi-scalar multiplication and all-or-nothing Schnorr batch verification: their own `extern "C"` block in
+// msm.rs (methods on Engine).
+mod msm;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

@@ -401,6 +401,46 @@ int p252_points_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_f
 int p252_points_to_bytes(p252_ctx* ctx, const p252_fr* uv, size_t n, uint8_t* bytes, uint8_t* ok,
                          size_t* n_invalid, int flags);
 
+/* ---- JubJub multi-scalar multiplication and all-or-nothing Schnorr batch verification ------------------------------
+ * VARIABLE TIME: both calls read public data only, and scalar bits become bucket indexes (memory addresses) and branch
+ * conditions on the device.  Never pass a secret scalar.
+ * Layouts: scalars, weights and u are p252_jscalar; points, R and PK (u, v) pairs of p252_fr; messages p252_fr; all as in
+ * p252_schnorr_verify_batch, and challenge(R, m) is its challenge.  base_uv (G) is a HOST pointer for every memory space,
+ * checked on the host as in p252_fixed_base_batch: a coordinate >= p or a point off the curve is refused with
+ * P252_ERR_INVALID_POINT before anything runs, also for n == 0.  out_uv lives in the call's memory space; all_verified is a
+ * HOST pointer and must not be NULL.
+ * Item validity (checked on the device, for both memory spaces):
+ *   msm:        scalar < r_J, both coordinates < p, the point on the curve.  An invalid item is skipped (it adds the
+ *               identity) and counted into *n_invalid.
+ *   verify_all: as an invalid item of p252_schnorr_verify_batch (u >= r_J, msg >= p, an R coordinate >= p, PK not a curve
+ *               point with u, v < p), or weight >= r_J.  An invalid item is counted into *n_invalid and makes the answer 0.
+ *               An R with canonical coordinates off the curve is not invalid, but makes the answer 0 too.
+ * Cofactored semantics: *all_verified = 1 iff no item is invalid, every R is on the curve and
+ *   [8] ( [sum z_i u_i] G + sum [z_i c_i] PK_i - sum [z_i] R_i ) == identity,   c_i = challenge(R_i, msg_i), z_i = weight[i].
+ * Except with probability about 2^-128 over uniformly random 128-bit weights, that is exactly when every item satisfies
+ * the cofactored equation [8] ([u_i] G + [c_i] PK_i - R_i) == identity.  For PK and R in the prime-order subgroup this is
+ * per-item verification; a signature whose R is shifted by a small-order point fails p252_schnorr_verify_batch and passes
+ * here.  (Without the cofactor a random combination is not sound against torsion components.)
+ * Weights come from the caller: uniformly random, unpredictable to the signers and nonzero (128 bits are enough).  Any
+ * z < r_J is accepted; a zero weight leaves its item unchecked.  The library generates no randomness.
+ * n == 0: the MSM is the identity (0, 1) and *all_verified = 1.  n_invalid: optional HOST pointer for both memory spaces
+ * (lifetime as for p252_decrypt_batch).
+ * Batch checks, before anything runs: a NULL buffer with n > 0 (out_uv and all_verified always), n_public not 1 or n,
+ * DEVICE buffers not 16-byte aligned -> INVALID_ARGUMENT.  With P252_ASYNC, DEVICE calls defer the publication of
+ * *n_invalid and *all_verified to p252_sync (and out_uv is complete after it); HOST calls return with them published.
+ * The work is one bucket (Pippenger) multi-scalar multiplication over chunks of the batch; see DESIGN.md section 4.  Its
+ * temporaries live in the context's staging arenas, which the first call grows to about 100-145 MiB each (three per
+ * context) and which are kept until p252_destroy. */
+/* out_uv = sum over valid items of [scalars[i]] points_uv[i] (JubJubAffine; the identity is (0, 1), also for n == 0) */
+int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* points_uv, size_t n,
+                    p252_fr* out_uv, size_t* n_invalid, int flags);
+/* *all_verified = 1 iff no item is invalid, every R is on the curve, and
+ *   [8] ( [sum z_i u_i] G + sum [z_i c_i] PK_i - sum [z_i] R_i ) == identity,   c_i = challenge(R_i, msg_i),
+ * with PK_i = pk_uv[n_public == 1 ? 0 : i] and z_i = weight[i] */
+int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_jscalar* u,
+                            const p252_fr* R_uv, const p252_fr* msg, const p252_jscalar* weight, size_t n,
+                            const p252_fr* base_uv, uint8_t* all_verified, size_t* n_invalid, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

@@ -12,7 +12,7 @@
 //   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
 //   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
 //   schnorr_verify_batch, point_from_bytes / points_from_bytes_batch, point_to_bytes / points_to_bytes_batch,
-//   merkle4_build.
+//   jubjub_msm, schnorr_verify_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -477,6 +477,27 @@ inline void point_to_bytes(const Scalar (&uv)[2], uint8_t (&bytes)[32], Engine& 
     const auto r = points_to_bytes_batch(uv, 1, ok, nullptr, e);
     if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
     std::copy(r.begin(), r.end(), bytes);
+}
+
+// NEW: multi-scalar multiplication and all-or-nothing Schnorr batch verification (p252_jubjub_msm /
+// p252_schnorr_verify_all).  VARIABLE TIME: scalar bits become bucket indexes on the device, so both take public data only.
+// sum [scalars[i]] points[i] over the valid items into out_uv (the identity (0, 1) for n == 0); points holds n x 2
+// scalars; an item with a scalar >= r_J, a coordinate >= p or a point off the curve is skipped.  n_invalid may be null.
+inline void jubjub_msm(const JubJubScalar* scalars, const Scalar* points, size_t n, Scalar (&out_uv)[2],
+                       size_t* n_invalid = nullptr, Engine& e = Engine::default_engine()) {
+    check(p252_jubjub_msm(e.get(), scalars, points, n, out_uv, n_invalid, P252_MEM_HOST), e.get());
+}
+// true iff no item is invalid, every R is on the curve and [8] ([sum z u] G + sum [z c] PK - sum [z] R) is the identity
+// (c = challenge(R, m), z = weight): cofactored, so an R shifted by a small-order point passes.  pk holds 1 or n points
+// (n_public), R n x 2 scalars; weight holds n caller-chosen random nonzero scalars (128 bits are enough), unpredictable
+// to the signers.  A G off the curve throws Error(P252_ERR_INVALID_POINT).  n_invalid may be null.
+inline bool schnorr_verify_all(const Scalar* pk, size_t n_public, const JubJubScalar* u, const Scalar* R, const Scalar* msg,
+                               const JubJubScalar* weight, size_t n, const Scalar (&base_uv)[2], size_t* n_invalid = nullptr,
+                               Engine& e = Engine::default_engine()) {
+    uint8_t all = 0;
+    check(p252_schnorr_verify_all(e.get(), pk, n_public, u, R, msg, weight, n, base_uv, &all, n_invalid, P252_MEM_HOST),
+          e.get());
+    return all != 0;
 }
 
 // arity-4 tree of Domain::Merkle4 digests; returns the internal levels bottom-up (root last)

@@ -287,17 +287,22 @@ int on_slots(p252_ctx* ctx, bool wipe, Body body) {
 
 int injected_fault(p252_ctx* ctx) { return fail_cuda(ctx, cudaErrorLaunchFailure, "kernel launch (injected fault)"); }
 
-// Fixed-size HOST batches: the items stream through the slot arenas in chunks, each buffer of `ios` staged in its own
-// region, one launch per chunk.
-template <typename Launch>
-int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
-    if (n == 0) return P252_OK;
+// The largest chunk run_host_pipeline stages for `ios` and n > 0 items
+size_t pipeline_chunk(const std::vector<Io>& ios, size_t n) {
     size_t per_item = 0;
     for (auto& io : ios)
         if (!io.once && !io.device) per_item += (io.item_bytes + 15) / 16 * 16;
     size_t chunk = std::max<size_t>(1024, std::min(chunk_items_max(), kChunkBytesTarget / std::max<size_t>(per_item, 1)));
     chunk = (chunk + 127) / 128 * 128;
-    if (chunk > n) chunk = n;
+    return chunk > n ? n : chunk;
+}
+
+// Fixed-size HOST batches: the items stream through the slot arenas in chunks, each buffer of `ios` staged in its own
+// region, one launch per chunk.
+template <typename Launch>
+int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
+    if (n == 0) return P252_OK;
+    const size_t chunk = pipeline_chunk(ios, n);
     std::vector<void*> d(ios.size());
     auto carve = [&](void* arena) {
         Carve c{static_cast<uint8_t*>(arena)};
@@ -1278,6 +1283,217 @@ int p252_points_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_f
 int p252_points_to_bytes(p252_ctx* ctx, const p252_fr* uv, size_t n, uint8_t* bytes, uint8_t* ok, size_t* n_invalid,
                          int flags) {
     return points_impl(ctx, false, uv, n, bytes, ok, n_invalid, flags);
+}
+
+// ---- multi-scalar multiplication and all-or-nothing Schnorr verification -----------------------------------------------
+// Per chunk of m rows (msm_chunk): launch_msm_prep -> CUB radix sort of the digit keys -> launch_msm_fill -> launch_msm_bucket
+// until one piece is left -> launch_msm_window, whose W window sums go to the chunk's slot of a per-call array.  After the
+// pipeline, launch_msm_final on the context stream adds the chunks and writes the result.  The window width c is fixed per
+// call by the largest chunk (msm_bits), so every chunk's windows line up.  Chunks share nothing but the per-call arrays,
+// in which each writes only its own slots.  Variable time: scalars are public.
+namespace {
+
+struct MsmScratch {
+    uint4* niels;
+    uint32_t *ka, *kb, *va, *vb;
+    void* temp;
+    size_t temp_bytes;
+    uint4* buckets;
+    uint32_t* ck[2];
+    uint4* cp[2];
+};
+
+size_t ceil_div(size_t a, size_t b) { return (a + b - 1) / b; }
+
+// The temporaries of one chunk of at most M rows
+MsmScratch msm_layout(Carve& cv, size_t M, int c) {
+    const size_t W = (size_t)p252::msm_windows(c), N = M * W, nb = W << (c - 1);
+    const size_t n1 = 2 * ceil_div(N, p252::kMsmPiece), n2 = 2 * ceil_div(n1, p252::kMsmPiece);
+    MsmScratch s{};
+    s.niels = cv.take<uint4>(M * 6);
+    s.ka = cv.take<uint32_t>(N);
+    s.kb = cv.take<uint32_t>(N);
+    s.va = cv.take<uint32_t>(N);
+    s.vb = cv.take<uint32_t>(N);
+    cub::DeviceRadixSort::SortPairs(nullptr, s.temp_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                    (const uint32_t*)nullptr, (uint32_t*)nullptr, (int)N, 0, 32);
+    s.temp = cv.take<uint8_t>(s.temp_bytes);
+    s.buckets = cv.take<uint4>(nb * 8);
+    s.ck[0] = cv.take<uint32_t>(n1);
+    s.cp[0] = cv.take<uint4>(n1 * 8);
+    s.ck[1] = cv.take<uint32_t>(n2);
+    s.cp[1] = cv.take<uint4>(n2 * 8);
+    return s;
+}
+
+size_t msm_scratch_bytes(size_t M, int c) {
+    Carve cv;
+    msm_layout(cv, M, c);
+    return cv.used;
+}
+
+// One chunk: m rows (scalars sc, points pt; device) into the W window sums at wsum, with the temporaries in `scratch`
+// (msm_scratch_bytes(M, c), m <= M): a region of the arena of the chunk's slot, so that a chunk reuses the region of that
+// slot's previous chunk in stream order.  The arenas persist with the context, so the temporaries cost no allocation per
+// call; they grow each arena to about 100-145 MiB (DESIGN.md section 4).  Counts its launches beyond the first
+// (run_host_pipeline counts that one).
+cudaError_t msm_chunk(p252_ctx* ctx, const void* sc, const void* pt, size_t m, int c, void* scratch, size_t M, uint4* wsum,
+                      unsigned long long* n_invalid, cudaStream_t st) {
+    Carve cv{static_cast<uint8_t*>(scratch)};
+    MsmScratch s = msm_layout(cv, M, c);
+    const uint32_t W = (uint32_t)p252::msm_windows(c), nb = W << (c - 1), N = (uint32_t)(m * W);
+    int end_bit = 0;
+    while ((1u << end_bit) <= nb) ++end_bit;         // keys <= nb (the sentinel)
+    cudaError_t e = p252::launch_msm_prep(sc, pt, (uint32_t)m, c, s.niels, s.ka, s.va, n_invalid, st);
+    if (e == cudaSuccess)
+        e = cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ka, s.kb, s.va, s.vb, (int)N, 0, end_bit, st);
+    if (e == cudaSuccess) e = p252::launch_msm_fill(s.buckets, nb, st);
+    size_t pieces = ceil_div(N, p252::kMsmPiece);
+    int launches = 3;                                 // prep, fill, the first pass and the window sums, less one
+    if (e == cudaSuccess)
+        e = p252::launch_msm_bucket(true, s.kb, s.vb, s.niels, N, nb, s.buckets, pieces > 1 ? s.ck[0] : nullptr, s.cp[0], st);
+    for (int src = 0; e == cudaSuccess && pieces > 1; src ^= 1, ++launches) {
+        const uint32_t len = (uint32_t)(2 * pieces);
+        pieces = ceil_div(len, p252::kMsmPiece);
+        e = p252::launch_msm_bucket(false, s.ck[src], nullptr, s.cp[src], len, nb, s.buckets,
+                                    pieces > 1 ? s.ck[src ^ 1] : nullptr, s.cp[src ^ 1], st);
+    }
+    if (e == cudaSuccess) e = p252::launch_msm_window(s.buckets, c, wsum, st);
+    if (e == cudaSuccess) ctx->launches += launches;
+    return e;
+}
+
+void CUDART_CB publish_flag(void* arg) {
+    auto* pr = static_cast<std::pair<const unsigned long long*, uint8_t*>*>(arg);
+    *pr->second = *pr->first ? 1 : 0;
+    delete pr;
+}
+// counter_end for a yes / no answer: device counter `slot` (0 or 1) -> the caller's byte
+int flag_end(p252_ctx* ctx, uint8_t* out, int slot) {
+    CU(cudaMemcpyAsync(ctx->h_counter + slot, ctx->d_counter + slot, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                       ctx->stream));
+    auto* pr = new std::pair<const unsigned long long*, uint8_t*>(ctx->h_counter + slot, out);
+    cudaError_t e = cudaLaunchHostFunc(ctx->stream, publish_flag, pr);
+    if (e != cudaSuccess) {
+        delete pr;
+        return fail_cuda(ctx, e, "cudaLaunchHostFunc");
+    }
+    return P252_OK;
+}
+
+}  // namespace
+
+int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* points_uv, size_t n, p252_fr* out_uv,
+                    size_t* n_invalid, int flags) {
+    if (!ctx || !out_uv || (n && (!scalars || !points_uv))) return P252_ERR_INVALID_ARGUMENT;
+    const bool dev = (flags & P252_MEM_DEVICE) != 0;
+    if (dev && (!aligned16(scalars) || !aligned16(points_uv) || !aligned16(out_uv))) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_invalid) *n_invalid = 0;
+    // 0 scalars, 1 points; 2 the chunk's MSM temporaries (one region per slot arena)
+    std::vector<Io> ios = {{scalars, nullptr, 32, false, dev}, {points_uv, nullptr, 64, false, dev}, {nullptr, nullptr, 0, true}};
+    const size_t chunk = n ? pipeline_chunk(ios, n) : 0;
+    const int c = p252::msm_bits(std::max<size_t>(chunk, 1));
+    const size_t W = (size_t)p252::msm_windows(c), max_chunks = n ? ceil_div(n, chunk) + 3 : 0;
+    ios[2].item_bytes = msm_scratch_bytes(chunk, c);
+    int rc = P252_OK;
+    unsigned long long* counter = nullptr;
+    if (n_invalid) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    uint4* wsum = nullptr;
+    uint8_t* dout = nullptr;
+    rc = with_scratch(ctx, ctx->stream, [&](Carve& cv) {
+        wsum = cv.take<uint4>(max_chunks * W * 8);
+        dout = cv.take<uint8_t>(64);
+    }, [&]() -> int {
+        uint32_t k = 0;
+        int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+            return msm_chunk(ctx, d[0], d[1], cnt, c, d[2], chunk, wsum + (size_t)(k++) * W * 8, counter, st);
+        });
+        if (r != P252_OK) return r;
+        void* out = dev ? static_cast<void*>(out_uv) : dout;
+        if ((r = launched(ctx, p252::launch_msm_final(wsum, k, c, out, nullptr, 0, nullptr, nullptr, nullptr, nullptr,
+                                                      ctx->stream))) != P252_OK)
+            return r;
+        if (!dev) CU(cudaMemcpyAsync(out_uv, dout, 64, cudaMemcpyDeviceToHost, ctx->stream));
+        return P252_OK;
+    });
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with the sum and the count published
+}
+
+// challenge(R, m) as in p252_schnorr_verify_batch.  Per chunk: launch_schnorr_pack and the truncated launch_digest (c), then
+// launch_msmv_prep writes the chunk's MSM rows and its sums of z u (and z c) into the arena, and msm_chunk runs on those
+// rows.  launch_msm_final adds [sum z u] G from the fixed-base table (and, for one public key, [sum z c] PK), multiplies by
+// the cofactor and writes the answer into device counter 1; counter 0 counts the invalid items.
+int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_jscalar* u, const p252_fr* R_uv,
+                            const p252_fr* msg, const p252_jscalar* weight, size_t n, const p252_fr* base_uv,
+                            uint8_t* all_verified, size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv || !all_verified) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, u, n, pk_uv, n_public, {R_uv, msg, weight}, all_verified, flags);
+    if (rc != P252_OK) return rc;
+    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = schnorr_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) {
+        *all_verified = 1;
+        return P252_OK;
+    }
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    const size_t per = pb ? 1 : 2;   // MSM rows per item
+    // 0 PK, 1 u, 2 R, 3 msg, 4 weight; 5 the digest rows, 6 validity, 7 c, 8 row scalars, 9 row points and 10 the chunk's
+    // MSM temporaries live in the arena only
+    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev}, {R_uv, nullptr, 64, false, dev},
+                           {msg, nullptr, 32, false, dev}, {weight, nullptr, 32, false, dev}, {nullptr, nullptr, 96},
+                           {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 32 * per},
+                           {nullptr, nullptr, 64 * per}, {nullptr, nullptr, 0, true}};
+    const size_t chunk = pipeline_chunk(ios, n), M = chunk * per;
+    const int c = p252::msm_bits(M);
+    const size_t W = (size_t)p252::msm_windows(c), max_chunks = ceil_div(n, chunk) + 3;
+    const size_t nsum = ceil_div(n, p252::kMsmItemsPerSum);
+    ios[10].item_bytes = msm_scratch_bytes(M, c);
+    if ((rc = counter_begin(ctx, 2)) != P252_OK) return rc;
+    uint4* wsum = nullptr;
+    uint8_t *zsum = nullptr, *pkc = nullptr;
+    uint32_t* bad = nullptr;
+    rc = with_scratch(ctx, ctx->stream, [&](Carve& cv) {
+        wsum = cv.take<uint4>(max_chunks * W * 8);
+        zsum = cv.take<uint8_t>(nsum * 64);
+        bad = cv.take<uint32_t>(1);
+        pkc = cv.take<uint8_t>(64);
+    }, [&]() -> int {
+        CU(cudaMemsetAsync(bad, 0, sizeof(uint32_t), ctx->stream));
+        if (pb) CU(cudaMemcpyAsync(pkc, pk_uv, 64, cudaMemcpyDefault, ctx->stream));
+        uint32_t k = 0;
+        size_t off = 0;
+        int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+            uint8_t* valid = static_cast<uint8_t*>(d[6]);
+            cudaError_t e = p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st);
+            if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st);
+            if (e == cudaSuccess)
+                e = p252::launch_msmv_prep(d[0], pb, d[1], d[2], d[7], d[4], valid, (uint32_t)cnt, d[8], d[9], zsum,
+                                           (uint32_t)(off / p252::kMsmItemsPerSum), bad, n_invalid ? ctx->d_counter : nullptr,
+                                           st);
+            if (e == cudaSuccess) e = msm_chunk(ctx, d[8], d[9], cnt * per, c, d[10], M, wsum + (size_t)(k++) * W * 8, nullptr, st);
+            if (e == cudaSuccess) ctx->launches += 3;   // run_host_pipeline and msm_chunk count one launch each
+            off += cnt;
+            return e;
+        });
+        if (r != P252_OK) return r;
+        return launched(ctx, p252::launch_msm_final(wsum, k, c, nullptr, zsum, (uint32_t)nsum, table, pb ? pkc : nullptr, bad,
+                                                    ctx->d_counter + 1, ctx->stream));
+    });
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 0);
+    if (rc == P252_OK) rc = flag_end(ctx, all_verified, 1);
+    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with the answer and the count published
 }
 
 // ---- arity-4 Merkle tree ------------------------------------------------------------------------------

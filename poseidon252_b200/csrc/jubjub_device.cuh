@@ -699,6 +699,109 @@ __device__ __forceinline__ bool decompress(uint32_t (&u)[8], uint32_t (&v)[8], c
     return canon & square;
 }
 
+// ---- multi-scalar multiplication: sum [s_i] P_i by buckets (p252_jubjub_msm / p252_schnorr_verify_all) -----------------
+// VARIABLE TIME: every scalar is public, and its digits become bucket indexes (addresses) and branch conditions.
+// c-bit signed windows, least significant first: window w takes x = bits [c w, c w + c) of s plus the carry, x in
+// [0, 2^c]; the digit is x - 2^c carry' with carry' = (x + 2^(c-1)) >> c, in [-2^(c-1), 2^(c-1)).  With W(c) = ceil(253 / c)
+// windows the top one holds at most c - 1 bits of s < 2^252, so its x <= 2^(c-1) is the digit itself and no carry is left.
+// Digit e != 0 of window w adds sign(e) P to bucket (w, |e| - 1); bucket sums B_j (j = |e|) of a window reduce to
+// sum_j j B_j by running sums, and the windows combine as sum_w 2^(c w) S_w (Horner, c doublings per window).
+// Products: a row's on-curve check 4 and Niels form 2; a nonzero digit one mixed addition with T 7; a carried partial
+// sum (pieces of one bucket split across threads) and each running-sum step one cached addition 1 + 8.
+constexpr int kMsmMinBits = 4, kMsmMaxBits = 13;
+__host__ __device__ constexpr int msm_windows(int c) { return (253 + c - 1) / c; }
+constexpr int kProductsPerMsmRow = 4 + 2;
+constexpr int kProductsPerMsmDigit = 7;
+constexpr int kProductsPerMsmCarry = 1 + 8;
+constexpr int kProductsPerMsmBucket = 2 * (1 + 8);
+static_assert(kProductsPerMsmRow == 6 && kProductsPerMsmDigit == 7, "product counts of DESIGN.md section 4");
+static_assert(kProductsPerMsmCarry == 9 && kProductsPerMsmBucket == 18, "product counts of DESIGN.md section 4");
+static_assert(msm_windows(kMsmMaxBits) == 20 && msm_windows(kMsmMinBits) == 64, "window counts of DESIGN.md section 4");
+
+// The next digit of s (consumed c bits at a time, c in [kMsmMinBits, kMsmMaxBits]); top: the last window, no carry out
+__device__ __forceinline__ int32_t recode_window(uint32_t (&s)[8], uint32_t& carry, int c, bool top) {
+    const uint32_t x = (s[0] & ((1u << c) - 1u)) + carry;
+#pragma unroll
+    for (int k = 0; k < 7; ++k) s[k] = __funnelshift_r(s[k], s[k + 1], c);
+    s[7] >>= c;
+    if (top) {
+        carry = 0;
+        return (int32_t)x;
+    }
+    carry = (x + (1u << (c - 1))) >> c;
+    return (int32_t)x - (int32_t)(carry << c);
+}
+
+// r = a + b mod r_J for a, b < r_J (the sum < 2^253 fits 8 words; one masked subtraction)
+__device__ __forceinline__ void order_add(uint32_t (&r)[8], const uint32_t (&a)[8], const uint32_t (&b)[8]) {
+    const uint32_t n[8] = P252_JJ_ORDER;
+    uint32_t s[8], d[8], carry = 0, borrow = 0;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint64_t x = (uint64_t)a[k] + b[k] + carry;
+        s[k] = (uint32_t)x;
+        carry = (uint32_t)(x >> 32);
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        const uint64_t x = (uint64_t)s[k] - n[k] - borrow;
+        d[k] = (uint32_t)x;
+        borrow = (uint32_t)(x >> 63);
+    }
+    const uint32_t keep = 0u - borrow;                  // s < r_J
+#pragma unroll
+    for (int k = 0; k < 8; ++k) r[k] = (s[k] & keep) | (d[k] & ~keep);
+}
+
+__device__ __forceinline__ void set_identity(Ext& p) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) p.X[k] = 0, p.T[k] = 0;
+    set_one(p.Y);
+    set_one(p.Z);
+}
+
+// r = p + q for two extended points (to_cached + add): 9 products
+__device__ __forceinline__ void add_ext(Ext& r, const Ext& p, const Ext& q) {
+    Cached c;
+    to_cached(c, q);
+    add<true>(r, p, c);
+}
+
+// An extended point as 8 x 16 bytes (X, Y, Z, T)
+__device__ __forceinline__ void store_ext(uint4* d, const Ext& p) {
+    const uint32_t* src[4] = {p.X, p.Y, p.Z, p.T};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        d[2 * q] = make_uint4(src[q][0], src[q][1], src[q][2], src[q][3]);
+        d[2 * q + 1] = make_uint4(src[q][4], src[q][5], src[q][6], src[q][7]);
+    }
+}
+__device__ __forceinline__ void load_ext(Ext& p, const uint4* s) {
+    uint32_t* dst[4] = {p.X, p.Y, p.Z, p.T};
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const uint4 a = s[2 * q], b = s[2 * q + 1];
+        dst[q][0] = a.x, dst[q][1] = a.y, dst[q][2] = a.z, dst[q][3] = a.w;
+        dst[q][4] = b.x, dst[q][5] = b.y, dst[q][6] = b.z, dst[q][7] = b.w;
+    }
+}
+
+// r = [k] p for a small public k (left to right over its bits)
+__device__ __forceinline__ void mul_small(Ext& r, const Ext& p, uint32_t k) {
+    set_identity(r);
+    if (k == 0) return;
+    Cached c;
+    to_cached(c, p);
+    for (int b = 31 - __clz(k); b >= 0; --b) {
+        Ext t;
+        dbl<true>(t, r);
+        if ((k >> b) & 1u)
+            add<true>(r, t, c);
+        else
+            r = t;
+    }
+}
+
 // b = JubJubAffine::to_bytes(u, v) as 8 little-endian words, for u, v < p (Montgomery) on the curve: canonical v with the
 // low bit of canonical u in bit 255
 __device__ __forceinline__ void compress(uint32_t (&b)[8], const uint32_t (&u)[8], const uint32_t (&v)[8]) {

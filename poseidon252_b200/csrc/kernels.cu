@@ -1889,6 +1889,460 @@ cudaError_t launch_points_to_bytes(const void* uv, size_t n, void* bytes, uint8_
     return cudaGetLastError();
 }
 
+// ---- multi-scalar multiplication by buckets (jubjub_device.cuh): sum [s_i] P_i --------------------------------------
+// Variable time: scalars are public; their digits index buckets and steer branches.  One chunk of m rows at a time:
+// k_msm_prep (validity, Niels form, the (window, bucket) key of every digit) -> radix sort of the keys (capi.cu) ->
+// k_msm_fill (buckets = identity) -> k_msm_bucket over the sorted digits, then over its carries until one piece is left
+// -> k_msm_window (one window sum S_w per window).  k_msm_final adds the chunks' window sums per window and combines the
+// windows.
+constexpr int kMsmThreads = 128;
+constexpr uint32_t kMsmEmpty = 1u << 31;   // a carry slot that holds nothing (its key only keeps the list sorted)
+
+// One thread per row: row i is valid iff s < r_J, u, v < p and (u, v) on the curve (an invalid row is skipped: all its
+// keys are the sentinel W B, behind every bucket).  Digit e != 0 of window w gets key w B + |e| - 1 and value i | sign << 31;
+// keys and values are window-major (index w m + i).
+__global__ void __launch_bounds__(kMsmThreads) k_msm_prep(const uint8_t* __restrict__ sc, const uint8_t* __restrict__ pts,
+                                                          uint32_t m, int c, uint4* __restrict__ niels,
+                                                          uint32_t* __restrict__ keys, uint32_t* __restrict__ vals,
+                                                          unsigned long long* __restrict__ n_invalid) {
+    const uint32_t i = blockIdx.x * kMsmThreads + threadIdx.x;
+    if (i >= m) return;
+    uint32_t s[8], u[8], v[8], one[8];
+    load_fr(s, sc + (size_t)i * 32);
+    load_fr(u, pts + (size_t)i * 64);
+    load_fr(v, pts + (size_t)i * 64 + 32);
+    jj::set_one(one);
+    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
+    const uint32_t mc = 0u - (uint32_t)canon;            // coordinates >= p enter no product
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] = (v[k] & mc) | (one[k] & ~mc);
+    const bool valid = canon & jj::below_order(s) & jj::on_curve(u, v);
+    if (n_invalid) warp_count_every(n_invalid, !valid);
+    jj::Niels q;
+    jj::to_niels(q, u, v);
+    const uint32_t* src[3] = {q.ymx, q.ypx, q.kt};
+#pragma unroll
+    for (int q3 = 0; q3 < 3; ++q3) {
+        niels[(size_t)i * 6 + 2 * q3] = make_uint4(src[q3][0], src[q3][1], src[q3][2], src[q3][3]);
+        niels[(size_t)i * 6 + 2 * q3 + 1] = make_uint4(src[q3][4], src[q3][5], src[q3][6], src[q3][7]);
+    }
+    const int W = jj::msm_windows(c);
+    const uint32_t B = 1u << (c - 1), sentinel = (uint32_t)W * B;
+    uint32_t carry = 0;
+    for (int w = 0; w < W; ++w) {
+        const int32_t e = jj::recode_window(s, carry, c, w == W - 1);
+        const uint32_t mag = (uint32_t)(e < 0 ? -e : e);
+        keys[(size_t)w * m + i] = (valid && mag) ? (uint32_t)w * B + mag - 1 : sentinel;
+        vals[(size_t)w * m + i] = i | ((uint32_t)(e < 0) << 31);
+    }
+}
+
+__global__ void __launch_bounds__(256) k_msm_fill(uint4* __restrict__ buckets, uint32_t nb) {
+    const uint32_t i = blockIdx.x * 256 + threadIdx.x;
+    if (i >= nb) return;
+    jj::Ext p;
+    jj::set_identity(p);
+    jj::store_ext(buckets + (size_t)i * 8, p);
+}
+
+// One thread per piece of kMsmPiece consecutive entries of a key-sorted list: the sorted digits (kRows: values index the
+// Niels rows, bit 31 the sign) or the carries of the previous pass (extended points, kMsmEmpty in the key marks an empty
+// slot).  Each run of equal keys in the piece is summed; keys >= nb (the sentinel) are skipped.  A run that continues into
+// the neighbouring piece on either side goes to the next list -- slot 2 t if it starts the piece, 2 t + 1 if it ends it --
+// and every other run is a whole bucket, stored.  So no thread adds more than kMsmPiece points however the scalars fall,
+// each pass shrinks the list by kMsmPiece / 2, and a list of one piece stores everything.
+template <bool kRows>
+__global__ void __launch_bounds__(kMsmThreads) k_msm_bucket(const uint32_t* __restrict__ keys, const uint32_t* __restrict__ vals,
+                                                            const uint4* __restrict__ src, uint32_t N, uint32_t nb,
+                                                            uint4* __restrict__ buckets, uint32_t* __restrict__ okeys,
+                                                            uint4* __restrict__ opts) {
+    const uint32_t t = blockIdx.x * kMsmThreads + threadIdx.x;
+    const uint32_t lo = t * kMsmPiece;
+    if (lo >= N) return;
+    const uint32_t hi = min(N, lo + kMsmPiece);
+    auto key_at = [&](uint32_t j) { return kRows ? keys[j] : keys[j] & ~kMsmEmpty; };
+    const uint32_t none = 0xffffffffu;
+    const uint32_t prevk = lo > 0 ? key_at(lo - 1) : none, nextk = hi < N ? key_at(hi) : none;
+    bool head = false, tail = false;
+    for (uint32_t i = lo; i < hi;) {
+        const uint32_t k = key_at(i);
+        jj::Ext acc, r;
+        jj::set_identity(acc);
+        bool any = false;
+        uint32_t j = i;
+        for (; j < hi && key_at(j) == k; ++j) {
+            if (k >= nb) continue;
+            if (kRows) {
+                const uint32_t v = vals[j];
+                const uint4* e = src + (size_t)(v & 0x7fffffffu) * 6;
+                jj::Niels q;
+                uint32_t* dst[3] = {q.ymx, q.ypx, q.kt};
+#pragma unroll
+                for (int q3 = 0; q3 < 3; ++q3) {
+                    const uint4 a = __ldg(e + 2 * q3), b = __ldg(e + 2 * q3 + 1);
+                    dst[q3][0] = a.x, dst[q3][1] = a.y, dst[q3][2] = a.z, dst[q3][3] = a.w;
+                    dst[q3][4] = b.x, dst[q3][5] = b.y, dst[q3][6] = b.z, dst[q3][7] = b.w;
+                }
+                if (v >> 31) {                              // -(u, v) = (-u, v): swap v - u and v + u, negate 2d u v
+                    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll
+                    for (int k2 = 0; k2 < 8; ++k2) {
+                        const uint32_t x = q.ymx[k2];
+                        q.ymx[k2] = q.ypx[k2];
+                        q.ypx[k2] = x;
+                    }
+                    uint32_t nk[8];
+                    fr_sub_mod(nk, zero, q.kt);
+                    jj::fcopy(q.kt, nk);
+                }
+                jj::madd<true>(r, acc, q);
+            } else {
+                if (keys[j] & kMsmEmpty) continue;
+                jj::Ext p;
+                jj::load_ext(p, src + (size_t)j * 8);
+                jj::add_ext(r, acc, p);
+            }
+            acc = r;
+            any = true;
+        }
+        const bool first = i == lo;
+        if ((first && prevk == k) || (j == hi && nextk == k)) {
+            const uint32_t slot = 2 * t + (first ? 0 : 1);
+            okeys[slot] = k | (any ? 0u : kMsmEmpty);
+            if (any) jj::store_ext(opts + (size_t)slot * 8, acc);
+            (first ? head : tail) = true;
+        } else if (any) {
+            jj::store_ext(buckets + (size_t)k * 8, acc);
+        }
+        i = j;
+    }
+    if (okeys && !head) okeys[2 * t] = key_at(lo) | kMsmEmpty;
+    if (okeys && !tail) okeys[2 * t + 1] = key_at(hi - 1) | kMsmEmpty;
+}
+
+// One block per window, P = msm_window_parts(c) threads, each over L = B / P consecutive buckets (index lo + j holds
+// |digit| = lo + j + 1): running sums from the top give r = sum B and t = sum (j + 1) B, so the part's share of
+// S_w = sum |digit| B is t + [lo] r (the offset correction); the parts are added in shared memory.
+__global__ void __launch_bounds__(kMsmThreads) k_msm_window(const uint4* __restrict__ buckets, int c, uint4* __restrict__ wsum) {
+    __shared__ uint4 sh[kMsmThreads * 8];
+    const int w = blockIdx.x, p = threadIdx.x, P = blockDim.x;
+    const uint32_t B = 1u << (c - 1), L = B / P, lo = p * L;
+    jj::Ext r, t, x;
+    jj::set_identity(r);
+    jj::set_identity(t);
+    for (int j = (int)L - 1; j >= 0; --j) {
+        jj::Ext b;
+        jj::load_ext(b, buckets + ((size_t)w * B + lo + j) * 8);
+        jj::add_ext(x, r, b);
+        r = x;
+        jj::add_ext(x, t, r);
+        t = x;
+    }
+    jj::mul_small(x, r, lo);
+    jj::add_ext(r, t, x);
+    jj::store_ext(sh + p * 8, r);
+    __syncthreads();
+    for (int s = P / 2; s > 0; s >>= 1) {
+        if (p < s) {
+            jj::Ext a, b;
+            jj::load_ext(a, sh + p * 8);
+            jj::load_ext(b, sh + (p + s) * 8);
+            jj::add_ext(x, a, b);
+            jj::store_ext(sh + p * 8, x);
+        }
+        __syncthreads();
+    }
+    if (p == 0) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) wsum[(size_t)w * 8 + q] = sh[q];
+    }
+}
+
+static_assert(kMsmThreads == kMsmItemsPerSum, "one (z u, z c) sum per block of k_msmv_prep");
+static_assert(jj::kMsmMaxBits <= 13, "k_msm_window: at most 4096 buckets per window, 32 per thread of 128");
+
+int msm_windows(int c) { return jj::msm_windows(c); }
+
+// The window width for chunks of `rows` rows: the fewest products by the counts of jubjub_device.cuh, rows x W (c) digit
+// additions (a digit is 0 with probability 2^-c only) against W (c) 2^(c-1) running-sum steps.
+int msm_bits(size_t rows) {
+    int best = jj::kMsmMinBits;
+    double best_cost = 0;
+    for (int c = jj::kMsmMinBits; c <= jj::kMsmMaxBits; ++c) {
+        const double W = jj::msm_windows(c);
+        const double cost = (double)rows * W * jj::kProductsPerMsmDigit + W * (double)(1 << (c - 1)) * jj::kProductsPerMsmBucket;
+        if (c == jj::kMsmMinBits || cost < best_cost) best = c, best_cost = cost;
+    }
+    return best;
+}
+
+int msm_window_parts(int c) {
+    const int B = 1 << (c - 1);
+    return B >= 32 ? (B / 32 < kMsmThreads ? B / 32 : kMsmThreads) : 1;
+}
+
+// verify_all, one thread per item, after k_schnorr_pack (valid[i]: R and m canonical) and the truncated digest (c[i]).  The
+// item is valid iff valid[i], u < r_J, z < r_J and PK = pk[pb ? 0 : i] is a curve point with u, v < p; an R off the curve
+// is not invalid but fails the batch.  Either sets *bad.  Rows: pb: row i = (z, -R); otherwise rows 2 i = (z c mod r_J, PK)
+// and 2 i + 1 = (z, -R).  An invalid item's (and an off-curve R's) rows are (0, identity).  The block's sums of z u (and,
+// pb, of z c) modulo r_J go to zsum[blk0 + block] (64 bytes).
+__global__ void __launch_bounds__(kMsmThreads) k_msmv_prep(const uint8_t* __restrict__ pk, bool pb, const uint8_t* __restrict__ u,
+                                                           const uint8_t* __restrict__ R_uv, const uint8_t* __restrict__ c,
+                                                           const uint8_t* __restrict__ z, const uint8_t* __restrict__ valid,
+                                                           uint32_t n, uint8_t* __restrict__ rsc, uint8_t* __restrict__ rpt,
+                                                           uint8_t* __restrict__ zsum, uint32_t blk0, uint32_t* __restrict__ bad,
+                                                           unsigned long long* __restrict__ n_invalid) {
+    __shared__ uint32_t sh[kMsmThreads][16];
+    const uint32_t i = blockIdx.x * kMsmThreads + threadIdx.x;
+    uint32_t zu[8] = {0, 0, 0, 0, 0, 0, 0, 0}, zc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (i < n) {
+        uint32_t x[8], y[8], one[8], s[8], w[8], e[8];
+        jj::set_one(one);
+        load_fr(x, pk + (pb ? 0 : (size_t)i) * 64);
+        load_fr(y, pk + (pb ? 0 : (size_t)i) * 64 + 32);
+        const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
+        uint32_t mc = 0u - (uint32_t)canon;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+        load_fr(s, u + (size_t)i * 32);
+        load_fr(w, z + (size_t)i * 32);
+        load_fr(e, c + (size_t)i * 32);
+        const bool good = (valid[i] != 0) & canon & jj::on_curve(x, y) & jj::below_order(s) & jj::below_order(w);
+        uint32_t ru[8], rv[8];
+        load_fr(ru, R_uv + (size_t)i * 64);
+        load_fr(rv, R_uv + (size_t)i * 64 + 32);
+        mc = 0u - (uint32_t)good;                       // an invalid item's R may be >= p: it enters no product
+#pragma unroll
+        for (int k = 0; k < 8; ++k) ru[k] &= mc, rv[k] = (rv[k] & mc) | (one[k] & ~mc);
+        const bool r_on = jj::on_curve(ru, rv);
+        if (!good || !r_on) *bad = 1u;
+        if (n_invalid) warp_count_every(n_invalid, !good);
+        const uint32_t mg = 0u - (uint32_t)(good & r_on);
+        const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        uint32_t nu[8];
+        fr_sub_mod(nu, zero, ru);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) w[k] &= mg, s[k] &= mg, x[k] &= mg, y[k] = (y[k] & mg) | (one[k] & ~mg),
+                                    nu[k] &= mg, rv[k] = (rv[k] & mg) | (one[k] & ~mg);
+        jj::order_mul(zc, w, e);                        // c < 2^250 < r_J
+        jj::order_mul(zu, w, s);
+        const size_t rr = pb ? i : 2 * (size_t)i + 1;   // the row of (z, -R)
+        store_fr(rsc + rr * 32, w);
+        store_fr(rpt + rr * 64, nu);
+        store_fr(rpt + rr * 64 + 32, rv);
+        if (!pb) {
+            store_fr(rsc + (rr - 1) * 32, zc);
+            store_fr(rpt + (rr - 1) * 64, x);
+            store_fr(rpt + (rr - 1) * 64 + 32, y);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) zc[k] = 0;
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) sh[threadIdx.x][k] = zu[k], sh[threadIdx.x][8 + k] = zc[k];
+    __syncthreads();
+    for (int h = kMsmThreads / 2; h > 0; h >>= 1) {
+        if ((int)threadIdx.x < h) {
+            uint32_t a[8], b[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) a[k] = sh[threadIdx.x][k], b[k] = sh[threadIdx.x + h][k];
+            jj::order_add(a, a, b);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) sh[threadIdx.x][k] = a[k], a[k] = sh[threadIdx.x][8 + k], b[k] = sh[threadIdx.x + h][8 + k];
+            jj::order_add(a, a, b);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) sh[threadIdx.x][8 + k] = a[k];
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) {
+        uint32_t a[8], b[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) a[k] = sh[0][k], b[k] = sh[0][8 + k];
+        store_fr(zsum + (size_t)(blk0 + blockIdx.x) * 64, a);
+        store_fr(zsum + (size_t)(blk0 + blockIdx.x) * 64 + 32, b);
+    }
+}
+
+// One block of kMsmThreads threads.  Threads w < W add window w's sums of every chunk; with zsum (verify_all) the block
+// first adds the nsum (z u, z c) pairs modulo r_J, then thread 64 computes [sum z u] G from the fixed-base table and thread
+// 96 [sum z c] PK (pk: the one public key, or null).  Thread 0 combines the windows (c doublings each) and adds both:
+//   MSM:        out_uv = the sum, affine (the identity (0, 1) for no chunks);
+//   verify_all: *verified = [8] sum == identity (X == 0, Y == Z) and *bad == 0.
+struct MsmFinal {
+    const uint4* wsum;
+    uint32_t nchunks;
+    int c;
+    uint8_t* out_uv;
+    const uint8_t* zsum;
+    uint32_t nsum;
+    const uint4* table;
+    const uint8_t* pk;
+    const uint32_t* bad;
+    unsigned long long* verified;
+};
+
+__global__ void __launch_bounds__(kMsmThreads) k_msm_final(MsmFinal a) {
+    __shared__ uint4 sw[64 * 8], sg[8], sp[8];
+    __shared__ uint32_t ss[kMsmThreads][16];
+    const int W = jj::msm_windows(a.c), tid = threadIdx.x;
+    if (a.zsum) {
+        uint32_t x[8] = {0, 0, 0, 0, 0, 0, 0, 0}, y[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        for (uint32_t k = tid; k < a.nsum; k += kMsmThreads) {
+            uint32_t b[8];
+            load_fr_rw(b, a.zsum + (size_t)k * 64);
+            jj::order_add(x, x, b);
+            load_fr_rw(b, a.zsum + (size_t)k * 64 + 32);
+            jj::order_add(y, y, b);
+        }
+#pragma unroll
+        for (int k = 0; k < 8; ++k) ss[tid][k] = x[k], ss[tid][8 + k] = y[k];
+        __syncthreads();
+        for (int h = kMsmThreads / 2; h > 0; h >>= 1) {
+            if (tid < h) {
+                uint32_t p[8], q[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) p[k] = ss[tid][k], q[k] = ss[tid + h][k];
+                jj::order_add(p, p, q);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) ss[tid][k] = p[k], p[k] = ss[tid][8 + k], q[k] = ss[tid + h][8 + k];
+                jj::order_add(p, p, q);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) ss[tid][8 + k] = p[k];
+            }
+            __syncthreads();
+        }
+    }
+    if (tid < W) {
+        jj::Ext s, x;
+        jj::set_identity(s);
+        for (uint32_t k = 0; k < a.nchunks; ++k) {
+            jj::Ext p;
+            jj::load_ext(p, a.wsum + ((size_t)k * W + tid) * 8);
+            jj::add_ext(x, s, p);
+            s = x;
+        }
+        jj::store_ext(sw + tid * 8, s);
+    } else if (tid == 64 && a.zsum) {
+        uint32_t s[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] = ss[0][k];
+        jj::Ext t;
+        jj::fixed_base_ext<true, true>(t, s, a.table);
+        jj::store_ext(sg, t);
+    } else if (tid == 96 && a.zsum) {
+        jj::Ext t;
+        if (a.pk) {
+            uint32_t s[8], x[8], y[8], one[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s[k] = ss[0][8 + k];
+            load_fr(x, a.pk);
+            load_fr(y, a.pk + 32);
+            jj::set_one(one);
+            const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
+            uint32_t mc = 0u - (uint32_t)canon;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+            mc = 0u - (uint32_t)jj::on_curve(x, y);    // an off-curve PK made every item invalid: *bad is set
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc), s[k] &= mc;
+            jj::scalar_mul_ext<true, true>(t, s, x, y);
+        } else {
+            jj::set_identity(t);
+        }
+        jj::store_ext(sp, t);
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    jj::Ext acc, x;
+    jj::load_ext(acc, sw + (W - 1) * 8);
+    for (int w = W - 2; w >= 0; --w) {
+        for (int d = 0; d < a.c; ++d) {
+            jj::dbl<true>(x, acc);
+            acc = x;
+        }
+        jj::Ext s;
+        jj::load_ext(s, sw + w * 8);
+        jj::add_ext(x, acc, s);
+        acc = x;
+    }
+    if (!a.zsum) {
+        uint32_t zi[8], ou[8], ov[8];
+        jj::inverse(zi, acc.Z);
+        jj::fmul(ou, acc.X, zi);
+        jj::fmul(ov, acc.Y, zi);
+        store_fr(a.out_uv, ou);
+        store_fr(a.out_uv + 32, ov);
+        return;
+    }
+    jj::Ext g;
+    jj::load_ext(g, sg);
+    jj::add_ext(x, acc, g);
+    jj::load_ext(g, sp);
+    jj::add_ext(acc, x, g);
+    for (int d = 0; d < 3; ++d) {                        // the cofactor
+        jj::dbl<true>(x, acc);
+        acc = x;
+    }
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    const bool ok = jj::feq(acc.X, zero) & jj::feq(acc.Y, acc.Z) & (*a.bad == 0);
+    *a.verified = ok ? 1ull : 0ull;
+}
+
+cudaError_t launch_msm_prep(const void* scalars, const void* points, uint32_t m, int c, void* niels, uint32_t* keys,
+                            uint32_t* vals, unsigned long long* n_invalid, cudaStream_t st) {
+    if (m == 0) return cudaSuccess;
+    k_msm_prep<<<(m + kMsmThreads - 1) / kMsmThreads, kMsmThreads, 0, st>>>(
+        static_cast<const uint8_t*>(scalars), static_cast<const uint8_t*>(points), m, c, static_cast<uint4*>(niels), keys, vals,
+        n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_msm_fill(void* buckets, uint32_t nb, cudaStream_t st) {
+    k_msm_fill<<<blocks256(nb), 256, 0, st>>>(static_cast<uint4*>(buckets), nb);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_msm_bucket(bool rows, const uint32_t* keys, const uint32_t* vals, const void* src, uint32_t N, uint32_t nb,
+                              void* buckets, uint32_t* okeys, void* opts, cudaStream_t st) {
+    if (N == 0) return cudaSuccess;
+    const uint32_t pieces = (N + kMsmPiece - 1) / kMsmPiece;
+    const unsigned grid = (pieces + kMsmThreads - 1) / kMsmThreads;
+    if (rows)
+        k_msm_bucket<true><<<grid, kMsmThreads, 0, st>>>(keys, vals, static_cast<const uint4*>(src), N, nb,
+                                                         static_cast<uint4*>(buckets), okeys, static_cast<uint4*>(opts));
+    else
+        k_msm_bucket<false><<<grid, kMsmThreads, 0, st>>>(keys, vals, static_cast<const uint4*>(src), N, nb,
+                                                          static_cast<uint4*>(buckets), okeys, static_cast<uint4*>(opts));
+    return cudaGetLastError();
+}
+
+cudaError_t launch_msm_window(const void* buckets, int c, void* wsum, cudaStream_t st) {
+    k_msm_window<<<jj::msm_windows(c), msm_window_parts(c), 0, st>>>(static_cast<const uint4*>(buckets), c,
+                                                                      static_cast<uint4*>(wsum));
+    return cudaGetLastError();
+}
+
+cudaError_t launch_msm_final(const void* wsum, uint32_t nchunks, int c, void* out_uv, const void* zsum, uint32_t nsum,
+                             const void* table, const void* pk, const uint32_t* bad, unsigned long long* verified,
+                             cudaStream_t st) {
+    MsmFinal a{static_cast<const uint4*>(wsum), nchunks, c, static_cast<uint8_t*>(out_uv), static_cast<const uint8_t*>(zsum),
+               nsum, static_cast<const uint4*>(table), static_cast<const uint8_t*>(pk), bad, verified};
+    k_msm_final<<<1, kMsmThreads, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_msmv_prep(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c, const void* z,
+                             const uint8_t* valid, uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0,
+                             uint32_t* bad, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_msmv_prep<<<(n + kMsmThreads - 1) / kMsmThreads, kMsmThreads, 0, st>>>(
+        static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u), static_cast<const uint8_t*>(R_uv),
+        static_cast<const uint8_t*>(c), static_cast<const uint8_t*>(z), valid, n, static_cast<uint8_t*>(row_scalars),
+        static_cast<uint8_t*>(row_points), static_cast<uint8_t*>(zsum), blk0, bad, n_invalid);
+    return cudaGetLastError();
+}
+
 cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint64_t* leaf_idx, size_t n, int arity,
                                uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st, const uint8_t* present) {
     if (n == 0 || depth == 0) return cudaSuccess;

@@ -173,6 +173,43 @@ cudaError_t launch_points_from_bytes(const void* bytes, size_t n, void* uv, uint
                                      cudaStream_t st);
 cudaError_t launch_points_to_bytes(const void* uv, size_t n, void* bytes, uint8_t* ok, unsigned long long* n_invalid,
                                    cudaStream_t st);
+// Multi-scalar multiplication (p252_jubjub_msm / p252_schnorr_verify_all), VARIABLE TIME (scalars are public), one chunk
+// of m rows at a time with c-bit windows: W = msm_windows(c) windows of B = 2^(c-1) buckets (jubjub_device.cuh).  Rows are
+// scalars (p252_jscalar, 32 bytes) and points ((u, v) Montgomery, 64 bytes).
+// prep: niels[i] (96 bytes) = the Niels form of row i; keys / vals [w m + i] = the bucket key w B + |e| - 1 of digit e of
+// window w (the sentinel W B for e = 0 or an invalid row) and i | (e < 0) << 31.  *n_invalid (device, may be null) +=
+// invalid rows (s >= r_J, a coordinate >= p, off the curve).
+constexpr int kMsmPiece = 32;   // sorted entries per thread of launch_msm_bucket; each pass shrinks a list to 2 / kMsmPiece
+cudaError_t launch_msm_prep(const void* scalars, const void* points, uint32_t m, int c, void* niels, uint32_t* keys,
+                            uint32_t* vals, unsigned long long* n_invalid, cudaStream_t st);
+// buckets[0, nb) = the identity (128-byte extended points)
+cudaError_t launch_msm_fill(void* buckets, uint32_t nb, cudaStream_t st);
+// One pass over a key-sorted list of N entries (rows: the sorted digits, vals their values, src the Niels rows; otherwise
+// the carries of the previous pass, src their points): whole buckets are stored, runs that cross a piece boundary go to
+// (okeys, opts), 2 ceil(N / kMsmPiece) slots (null when N <= kMsmPiece).  Keys >= nb are skipped.
+cudaError_t launch_msm_bucket(bool rows, const uint32_t* keys, const uint32_t* vals, const void* src, uint32_t N, uint32_t nb,
+                              void* buckets, uint32_t* okeys, void* opts, cudaStream_t st);
+// wsum[w] (128 bytes) = sum over the buckets of window w of |digit| B_j, w < W
+cudaError_t launch_msm_window(const void* buckets, int c, void* wsum, cudaStream_t st);
+int msm_window_parts(int c);   // threads per window of launch_msm_window
+int msm_windows(int c);        // W (c)
+int msm_bits(size_t rows);     // the window width c for chunks of `rows` rows (DESIGN.md section 4)
+// Adds the chunks' window sums (wsum, nchunks x W) and combines the windows.  zsum null: out_uv (device, 64 bytes) = the
+// sum, affine.  Otherwise (verify_all) nsum (sum z u, sum z c) pairs modulo r_J are added too, and
+// *verified = [8] (sum + [sum z u] G + [sum z c] pk) == identity and *bad == 0 (table: G's fixed-base table; pk: one
+// public key (u, v), or null for none)
+cudaError_t launch_msm_final(const void* wsum, uint32_t nchunks, int c, void* out_uv, const void* zsum, uint32_t nsum,
+                             const void* table, const void* pk, const uint32_t* bad, unsigned long long* verified,
+                             cudaStream_t st);
+// verify_all rows of n items, after launch_schnorr_pack (valid) and the truncated digest (c): item i is valid iff valid[i],
+// u, z < r_J and pk[pk_bcast ? 0 : i] a curve point with u, v < p (counted into *n_invalid, device, may be null); an
+// invalid item or an R off the curve sets *bad.  Rows (scalars 32 bytes, points 64): pk_bcast: row i = (z, -R); otherwise
+// rows 2 i = (z c mod r_J, PK), 2 i + 1 = (z, -R); (0, identity) for an invalid item or an off-curve R.  zsum[blk0 + b]
+// (64 bytes) = the sums modulo r_J of z u and (pk_bcast) z c over block b of kMsmItemsPerSum items.
+constexpr int kMsmItemsPerSum = 128;
+cudaError_t launch_msmv_prep(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c, const void* z,
+                             const uint8_t* valid, uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0,
+                             uint32_t* bad, unsigned long long* n_invalid, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -17,6 +17,19 @@ def _is_torch(x):
     return hasattr(x, "data_ptr") and hasattr(x, "is_cuda")
 
 
+def _random_weights(n, like):
+    """n fresh nonzero 128-bit weights from `secrets` as (n, 4) p252_jscalar rows, in the memory space of `like`."""
+    import secrets
+    w = np.zeros((n, 4), dtype=np.uint64)
+    w[:, :2] = np.frombuffer(secrets.token_bytes(16 * n), dtype=np.uint64).reshape(n, 2)
+    for i in np.flatnonzero((w[:, 0] == 0) & (w[:, 1] == 0)):
+        w[i, 0] = 1 + secrets.randbelow((1 << 64) - 1)
+    if _is_torch(like):
+        import torch
+        return torch.from_numpy(w.view(np.int64)).to(like.device)
+    return w
+
+
 class Engine:
     def __init__(self, device=0, stream=None):
         """stream: None -> the engine creates its own non-blocking stream; an int -> an existing
@@ -626,6 +639,67 @@ class Engine:
     def last_points_invalid(self):
         """Invalid items of the last points_from_bytes or points_to_bytes (sync() first after async_)."""
         return self._last("points_invalid")
+
+    # -- multi-scalar multiplication and all-or-nothing Schnorr verification -----------------------------------------
+    def jubjub_msm(self, scalars, points, out=None, async_=False):
+        """sum [scalars[i]] points[i] by the bucket method: scalars (n, 4) p252_jscalar rows, points (n, 2, 4) BlsScalar.0
+        limbs -> the sum (2, 4), affine (the identity (0, 1) for n == 0).  VARIABLE TIME: for public scalars only.  An
+        item with a scalar >= r_J, a coordinate >= p or a point off the curve is skipped (count: last_msm_invalid())."""
+        sp, sl, flags, sk = self._in(scalars, (4,))
+        if len(sl) != 1:
+            raise EngineError(-1, "scalars must have shape (n, 4)")
+        n = int(sl[0])
+        pp, pl, fp, pk = self._in(points, (2, 4))
+        self._same_space(flags, fp)
+        self._same_lead("points", pl, n)
+        res = self._result(out, (2, 4), sk)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("msm_invalid", flags)
+        self._check(self._lib.p252_jubjub_msm(self._ctx, sp, pp, n, self._ptr(res), ctypes.byref(invalid), flags))
+        return res
+
+    def last_msm_invalid(self):
+        """Skipped items of the last jubjub_msm (sync() first after async_)."""
+        return self._last("msm_invalid")
+
+    def schnorr_verify_all(self, pk, u, R, msg, base, weights=None, async_=False):
+        """All-or-nothing verification of n signatures by one random linear combination: True iff no item is invalid,
+        every R is on the curve and [8] ([sum z u] base + sum [z c] PK - sum [z] R) is the identity, c = challenge(R, msg).
+        Except with probability ~2^-128 that is every item passing the cofactored check [8] ([u] G + [c] PK - R) == O
+        (for subgroup keys and R, per-item verification).  pk (1 or n, 2, 4), u (n, 4) p252_jscalar rows, R (n, 2, 4),
+        msg (n, 4), base (2, 4) (host-read); weights (n, 4) p252_jscalar rows in the memory space of u, or None for fresh
+        128-bit weights from `secrets`.  Invalid items (as in schnorr_verify_batch, or a weight >= r_J) are counted in
+        last_schnorr_invalid().  VARIABLE TIME (public data only).  async_: returns None; last_verify_all() after sync()."""
+        up, ul, flags, uk = self._in(u, (4,))
+        if len(ul) != 1:
+            raise EngineError(-1, "u must have shape (n, 4)")
+        n = int(ul[0])
+        if weights is None:
+            weights = _random_weights(n, uk)
+        pp, pl, fp, pkk = self._in(pk, (2, 4))
+        Rp, Rl, fR, Rk = self._in(R, (2, 4))
+        mp, ml, fm, mk = self._in(msg, (4,))
+        wp, wl, fw, wk = self._in(weights, (4,))
+        self._same_space(flags, fp, fR, fm, fw)
+        if len(pl) != 1 or int(pl[0]) not in (1, n):
+            raise EngineError(-1, "pk must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(pl)))
+        self._same_lead("R", Rl, n)
+        self._same_lead("msg", ml, n)
+        self._same_lead("weights", wl, n)
+        b = self._base(base)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("schnorr_invalid", flags)
+        answer = self._counters["verify_all"] = ctypes.c_uint8(0)
+        if flags & _native.ASYNC:
+            self._keep_until_sync(answer)
+            self._keep_until_sync(wk)
+        self._check(self._lib.p252_schnorr_verify_all(self._ctx, pp, int(pl[0]), up, Rp, mp, wp, n, b.ctypes.data,
+                                                      ctypes.byref(answer), ctypes.byref(invalid), flags))
+        return None if flags & _native.ASYNC else bool(answer.value)
+
+    def last_verify_all(self):
+        """The answer of the last schnorr_verify_all (sync() first after async_)."""
+        return bool(self._last("verify_all"))
 
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
