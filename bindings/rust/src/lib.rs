@@ -140,6 +140,9 @@ mod points;
 // msm.rs (methods on Engine).
 mod msm;
 
+// Phoenix note nullifiers (which owned notes are spent): their own `extern "C"` block in nullifier.rs (methods on Engine).
+mod nullifier;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

@@ -379,6 +379,34 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
                               const p252_fr* R_uv, const p252_fr* msg, size_t n, const p252_fr* base_uv,
                               uint8_t* verified, size_t* n_verified, size_t* n_invalid, int flags);
 
+/* ---- Note nullifiers: which owned notes are spent (Phoenix SecretKey::gen_note_sk, Note::gen_nullifier) --------------
+ *   hash(P)   = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0]                  (the stealth calls' hash, < 2^250)
+ *   note_sk   = (hash([a] R) + b) mod r_J
+ *   pk'       = [note_sk] G'                                                          (affine)
+ *   nullifier = Hash::digest(Domain::Other, [pk'.u, pk'.v, BlsScalar::from(pos)])[0]  (NOT truncated)
+ * (a, b) is the wallet's secret key, R a note's ephemeral key and pos its position in the note tree; note_sk is the
+ * discrete log of the note's stealth key: [note_sk] G = note_pk for the notes of p252_stealth_address_batch.  Scalars
+ * and points are laid out as for p252_dhke_batch; pos is one u64 per note.  base_uv (G', GENERATOR_NUMS) is a HOST pointer
+ * for every memory space, as in p252_fixed_base_batch: a coordinate >= p or a point off the curve is refused with
+ * P252_ERR_INVALID_POINT before anything runs, for every memory space and for n == 0.  There is no built-in generator.
+ * n_secret is 1 (one wallet key for every note) or n; a and b share it.
+ * Item validity (checked on the device, for both memory spaces): a < r_J, b < r_J, and R a curve point with u, v < p.  pos
+ * is any u64.  An invalid item gets ok[i] = 0 and a zeroed nullifier row, and is counted once into *n_invalid (optional
+ * HOST pointer for both memory spaces, lifetime as for p252_decrypt_batch); the call returns P252_OK.
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_secret not 1 or n -> INVALID_ARGUMENT; so are DEVICE
+ * buffers a, b, R_uv or nullifier not 16-byte aligned, and a DEVICE pos not 8-byte aligned (as the positions of the tree
+ * calls).
+ * a, b, the shared points [a] R, their hashes, note_sk and pk' live only in the context's staging arenas, for both memory
+ * spaces, and the arenas are zeroed on every exit path: the call is synchronous (P252_ASYNC only defers the publication
+ * of *n_invalid to p252_sync).  Each item is constant time (no branch and no address depends on a, b or note_sk); see
+ * DESIGN.md section 4.  The context keeps the fixed-base table of one base: alternating calls with G (the stealth calls)
+ * and G' on one context rebuild the 48 KB table on every switch; a context of its own for nullifiers avoids that. */
+/* nullifier[i] = Hash::digest(Domain::Other, [pk'.u, pk'.v, BlsScalar::from(pos[i])])[0],
+ *   pk' = [note_sk] base,  note_sk = (hash([a] R_uv[i]) + b) mod r_J,  (a, b) = (a, b)[n_secret == 1 ? 0 : i] */
+int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
+                         const p252_fr* base_uv, const p252_fr* R_uv, const uint64_t* pos, size_t n,
+                         p252_fr* nullifier, uint8_t* ok, size_t* n_invalid, int flags);
+
 /* ---- JubJub point compression (dusk-jubjub's JubJubAffine::to_bytes / from_bytes) -----------------------------------
  *   encoding:  the 32 little-endian bytes of canonical v, with bit 255 (bytes[31] >> 7) = the low bit of canonical u
  *   decoding:  sign = bit 255, cleared; the remaining 255-bit value is v (rejected if >= p); u^2 = (v^2 - 1) / (1 + d v^2)

@@ -11,8 +11,8 @@
 //   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
 //   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
 //   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
-//   schnorr_verify_batch, point_from_bytes / points_from_bytes_batch, point_to_bytes / points_to_bytes_batch,
-//   jubjub_msm, schnorr_verify_all, merkle4_build.
+//   schnorr_verify_batch, nullifier / nullifier_batch, point_from_bytes / points_from_bytes_batch, point_to_bytes /
+//   points_to_bytes_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -442,6 +442,30 @@ inline bool schnorr_verify(const Scalar (&pk_uv)[2], const JubJubScalar& u, cons
     const auto verified = schnorr_verify_batch(pk_uv, 1, &u, R_uv, &msg, 1, base_uv, nullptr, &invalid, e);
     if (invalid) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
     return verified[0] != 0;
+}
+
+// NEW: Phoenix note nullifiers (p252_nullifier_batch): nullifier = Hash::digest(Domain::Other, [pk'.u, pk'.v, pos])[0] with
+// pk' = [note_sk] G' and note_sk = (hash([a] R) + b) mod r_J, hash the stealth calls' truncated digest.  base_uv is the
+// caller's G' (no built-in generator); a G' off the curve throws Error(P252_ERR_INVALID_POINT).  a and b hold 1 or n keys
+// each (n_secret); R holds n x 2 scalars and pos n positions.  Returns the n nullifiers; ok[i] == 0 marks an invalid item
+// (a or b >= r_J, R off the curve), whose nullifier is zeroed.  n_invalid may be null.
+inline std::vector<Scalar> nullifier_batch(const JubJubScalar* a, const JubJubScalar* b, size_t n_secret,
+                                           const Scalar (&base_uv)[2], const Scalar* R, const uint64_t* pos, size_t n,
+                                           std::vector<uint8_t>& ok, size_t* n_invalid = nullptr,
+                                           Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> out(n);
+    ok.assign(n, 0);
+    check(p252_nullifier_batch(e.get(), a, b, n_secret, base_uv, R, pos, n, out.data(), ok.data(), n_invalid, P252_MEM_HOST),
+          e.get());
+    return out;
+}
+// Note::gen_nullifier for one note; throws Error(P252_ERR_INVALID_POINT) for a or b >= r_J or an R off the curve
+inline Scalar nullifier(const JubJubScalar& a, const JubJubScalar& b, const Scalar (&base_uv)[2], const Scalar (&R_uv)[2],
+                        uint64_t pos, Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok;
+    const auto r = nullifier_batch(&a, &b, 1, base_uv, R_uv, &pos, 1, ok, nullptr, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    return r[0];
 }
 
 // NEW: JubJub point compression (p252_points_from_bytes / p252_points_to_bytes), dusk-jubjub's JubJubAffine::from_bytes /

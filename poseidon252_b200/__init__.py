@@ -11,7 +11,8 @@ plus the batch entry points this engine adds:
     stealth_owns_batch (stealth addresses: the sender's note keys and a view key's ownership scan), schnorr_sign /
     schnorr_sign_batch and schnorr_verify / schnorr_verify_batch (Schnorr signatures over JubJub), point_from_bytes /
     points_from_bytes_batch and point_to_bytes / points_to_bytes_batch (JubJub point compression), jubjub_msm
-    (multi-scalar multiplication) and schnorr_verify_all (all-or-nothing batch verification), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
+    (multi-scalar multiplication) and schnorr_verify_all (all-or-nothing batch verification), nullifier /
+    nullifier_batch (Phoenix note nullifiers: which owned notes are spent), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
     with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
@@ -26,6 +27,7 @@ from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, Inv
 from .hash import Domain, Hash, pack_varlen
 from .merkle import CompactTree, SparseTree, Tree, merkle4_build, merkle4_level
 from .msm import jubjub_msm, schnorr_verify_all
+from .nullifier import nullifier, nullifier_batch
 from .points import point_from_bytes, point_to_bytes, points_from_bytes_batch, points_to_bytes_batch
 from .schnorr import schnorr_sign, schnorr_sign_batch, schnorr_verify, schnorr_verify_batch
 
@@ -37,7 +39,7 @@ __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encr
            "encrypt_batch_ephemeral", "stealth_address", "stealth_address_batch", "owns", "stealth_owns_batch",
            "schnorr_sign", "schnorr_sign_batch", "schnorr_verify", "schnorr_verify_batch",
            "point_from_bytes", "point_to_bytes", "points_from_bytes_batch", "points_to_bytes_batch",
-           "jubjub_msm", "schnorr_verify_all",
+           "jubjub_msm", "schnorr_verify_all", "nullifier", "nullifier_batch",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",

@@ -13,6 +13,7 @@
 //   Phoenix stealth addresses (consumer, not the reference) -> p252_stealth_address_batch, p252_stealth_owns_batch
 //   jubjub-schnorr sign / verify (consumer, not the reference) -> p252_schnorr_sign_batch, p252_schnorr_verify_batch
 //   JubJubAffine::from_bytes / to_bytes (dusk-jubjub, not the reference) -> p252_points_from_bytes, p252_points_to_bytes
+//   Phoenix note nullifiers (consumer, not the reference) -> p252_nullifier_batch
 //   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -1238,6 +1239,58 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
     if (rc == P252_OK) rc = counter_end(ctx, n_verified, 0);
     if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
     return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
+}
+
+// ---- note nullifiers: Hash::digest(Domain::Other, [pk'.u, pk'.v, pos])[0], pk' = [(hash([a] R) + b) mod r_J] G' --------
+// Per chunk: launch_dhke into a slot arena (the shared points and their validity), the truncated launch_digest of them
+// into the arena (h, the stealth calls' hash), launch_nullifier_key (the digest rows [pk'.u, pk'.v, pos] into the arena,
+// validity &= b < r_J), the full launch_digest of the rows into nullifier (the Schnorr challenge's tag: Domain::Other,
+// three inputs, one output), then launch_dhke_fix (invalid rows zeroed, ok, the count).  a, b, the shared points, h,
+// note_sk and pk' live only in the slot arenas for both memory spaces, so the call is synchronous and the common exit
+// join_slots(wipe) clears them on every path.
+int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret, const p252_fr* base_uv,
+                         const p252_fr* R_uv, const uint64_t* pos, size_t n, p252_fr* nullifier, uint8_t* ok,
+                         size_t* n_invalid, int flags) {
+    if (!ctx || !base_uv || (n && !pos)) return P252_ERR_INVALID_ARGUMENT;
+    int rc = dhke_args(n, a, n_secret, R_uv, n, {b, nullifier}, ok, flags);
+    if (rc != P252_OK) return rc;
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    if (dev && (reinterpret_cast<uintptr_t>(pos) & 7)) return P252_ERR_INVALID_ARGUMENT;
+    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    p252_fr tag_h, tag_n;
+    if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_tag(&tag_n)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_invalid) *n_invalid = 0;
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    unsigned long long* counter = nullptr;
+    if (dev && n_invalid) {
+        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
+        counter = ctx->d_counter;
+    }
+    // 0 a, 1 b, 2 R, 3 pos, 4 nullifier, 5 ok; 6 shared points, 7 validity, 8 h and 9 the digest rows live in the arena only
+    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev},
+                           {pos, nullptr, 8, false, dev}, {nullptr, nullifier, 32, false, dev}, {nullptr, ok, 1, false, dev},
+                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 96}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* valid = static_cast<uint8_t*>(d[7]);
+        cudaError_t e = p252::launch_dhke(d[0], sb, d[2], false, cnt, d[6], valid, nullptr, st);
+        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag_h), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st);
+        if (e == cudaSuccess)
+            e = p252::launch_nullifier_key(d[8], d[1], sb, static_cast<const uint64_t*>(d[3]), cnt, table, d[9], valid, st);
+        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag_n), d[9], cnt, 3, d[4], 1, false, ctx->coop_max, st);
+        if (e == cudaSuccess) e = p252::launch_dhke_fix(false, valid, cnt, d[4], 1, static_cast<uint8_t*>(d[5]), counter, st);
+        if (e == cudaSuccess) ctx->launches += 4;   // run_host_pipeline counts the chunk's first launch
+        return e;
+    }, /*wipe=*/true);
+    if (!dev) {
+        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
+        return rc;
+    }
+    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
+    return device_done(ctx, rc, flags);
 }
 
 // ---- JubJub point compression: JubJubAffine::from_bytes / to_bytes -----------------------------------------------------

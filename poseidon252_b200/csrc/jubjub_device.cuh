@@ -460,6 +460,13 @@ constexpr int kProductsPerSchnorrVerify =
 static_assert(kOrderProductsPerSchnorrSign == 2, "product count of DESIGN.md section 4");
 static_assert(kProductsPerSchnorrVerify == 2850, "product count of DESIGN.md section 4");
 
+// ---- note nullifiers (p252_nullifier_batch) ----------------------------------------------------------------------------
+// h = hash([a] R) < 2^250 comes from the truncated digest.  note_sk = (h + b) mod r_J is order_add (no product),
+// pk' = [note_sk] G' is fixed_base_mul, and the position's Montgomery image pos R mod p is one product by R^2 mod p
+// (fr_from_canonical).
+constexpr int kProductsPerNullifierKey = kProductsPerFixedBase + 1;
+static_assert(kProductsPerNullifierKey == 867, "product count of DESIGN.md section 4");
+
 // Arithmetic modulo r_J on 8 x 32-bit little-endian words, Montgomery form with R = 2^256.  Constants (immediates, as
 // P252_JJ_ORDER): R^2 mod r_J and kOrderInv = -r_J^-1 mod 2^32.  Constant time: no branch and no address depends on an
 // operand; each final correction is a masked subtraction or addition of r_J.

@@ -10,6 +10,7 @@
 //   dhke             src/encryption.rs:11-43  -> k_dhke (JubJub scalar multiplication, jubjub_device.cuh)
 //   stealth addresses (note_pk = [hash(shared)] G + B) -> k_stealth
 //   Schnorr signatures (u = r - c sk, [u] G + [c] PK == R) -> k_schnorr_pack, k_schnorr_sign, k_schnorr_verify
+//   note nullifiers (pk' = [(h + b) mod r_J] G', the digest rows [pk'.u, pk'.v, pos]) -> k_nullifier_key
 //   JubJubAffine::from_bytes / to_bytes (point compression) -> k_points_from_bytes, k_points_to_bytes
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
@@ -1683,6 +1684,48 @@ cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, co
                                                        static_cast<const uint8_t*>(B_uv), B_bcast, valid,
                                                        static_cast<uint8_t*>(note_pk), static_cast<uint8_t*>(R_uv), ok,
                                                        n_invalid, nullptr);
+    return cudaGetLastError();
+}
+
+// ---- note nullifiers: the digest rows [pk'.u, pk'.v, pos] of pk' = [(h + b) mod r_J] G' (jubjub_device.cuh) -------------
+// One thread per item, kProductsPerNullifierKey products, after k_dhke (valid[i]: a < r_J and R a curve point) and the
+// truncated digest (h[i] < 2^250 < r_J).  b[bb ? 0 : i] (canonical 4 x u64) must be < r_J: valid[i] &= b < r_J, and an
+// out-of-range b enters the sum as 0.  rows[i] = [pk'.u, pk'.v, Montgomery(pos[i])] (96 bytes) for every item; the caller
+// zeroes the outputs of invalid ones after the digest (launch_dhke_fix).  a, b and note_sk are secret: every item runs the
+// same schedule, the validity is a mask, and the table reads are masked selects, as in k_fixed_base.
+__global__ void __launch_bounds__(kThreads, 3) k_nullifier_key(const uint8_t* __restrict__ h, const uint8_t* __restrict__ b,
+                                                            bool bb, const uint64_t* __restrict__ pos, size_t n,
+                                                            const uint4* __restrict__ table, uint8_t* __restrict__ rows,
+                                                            uint8_t* valid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t s[8], t[8];
+    load_fr(s, h + i * 32);
+    load_fr(t, b + (bb ? 0 : i) * 32);
+    const bool in_range = jj::below_order(t);
+    const uint32_t m = 0u - (uint32_t)in_range;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) t[k] &= m;
+    uint32_t sk[8];
+    jj::order_add(sk, s, t);
+    uint32_t ou[8], ov[8];
+    jj::fixed_base_mul<true>(ou, ov, sk, table);
+    uint32_t c[8] = {0, 0, 0, 0, 0, 0, 0, 0}, pm[8];
+    const uint64_t p = pos[i];
+    c[0] = (uint32_t)p, c[1] = (uint32_t)(p >> 32);
+    fr_from_canonical(pm, c);
+    store_fr(rows + i * 96, ou);
+    store_fr(rows + i * 96 + 32, ov);
+    store_fr(rows + i * 96 + 64, pm);
+    valid[i] = (valid[i] != 0) & in_range ? 1 : 0;
+}
+
+cudaError_t launch_nullifier_key(const void* h, const void* b, bool b_bcast, const uint64_t* pos, size_t n, const void* table,
+                                 void* rows, uint8_t* valid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_nullifier_key<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), static_cast<const uint8_t*>(b), b_bcast,
+                                                      pos, n, static_cast<const uint4*>(table), static_cast<uint8_t*>(rows),
+                                                      valid);
     return cudaGetLastError();
 }
 

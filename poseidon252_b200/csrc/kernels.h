@@ -152,6 +152,12 @@ cudaError_t launch_stealth_owns(const void* h, size_t n, const void* table, cons
 cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, const void* B_uv, bool B_bcast,
                                   const uint8_t* valid, void* R_uv, void* note_pk, uint8_t* ok, unsigned long long* n_invalid,
                                   cudaStream_t st);
+// Note nullifiers (p252_nullifier_batch), one thread per item: h[i] is the truncated digest of the item's shared point
+// [a] R (4 x u64 < 2^250), valid[i] its validity from launch_dhke, table the fixed-base table of G'.  rows[i] =
+// [pk'.u, pk'.v, pos[i] as a field element] (96 bytes, Montgomery), pk' = [(h[i] + b) mod r_J] G' with b =
+// b[b_bcast ? 0 : i]; valid[i] &= b < r_J (an out-of-range b enters the sum as 0)
+cudaError_t launch_nullifier_key(const void* h, const void* b, bool b_bcast, const uint64_t* pos, size_t n, const void* table,
+                                 void* rows, uint8_t* valid, cudaStream_t st);
 // Schnorr signatures (p252_schnorr_sign_batch / p252_schnorr_verify_batch), challenge c = the truncated digest of the row
 // [R.u, R.v, m] (4 x u64 < 2^250).  Counters are device pointers and may be null.
 // pack: rows[i] = [R.u, R.v, m] (96 bytes, a value >= p written as 0); flag[i] = (and_flag ? flag[i] : 1) and all three < p

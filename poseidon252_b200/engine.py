@@ -597,6 +597,42 @@ class Engine:
         """Invalid items of the last schnorr_sign_batch or schnorr_verify_batch (sync() first after async_)."""
         return self._last("schnorr_invalid")
 
+    # -- note nullifiers --------------------------------------------------------------------------
+    def nullifier_batch(self, a, b, base, R, pos, out=None, async_=False):
+        """Phoenix note nullifiers: nullifier_i = Hash::digest(Domain::Other, [pk'.u, pk'.v, pos_i])[0] with
+        pk' = [note_sk] base and note_sk = (hash([a] R_i) + b) mod r_J, hash(P) = Hash::digest_truncated(Domain::Other,
+        [P.u, P.v])[0].  a and b (1 or n, 4) p252_jscalar rows with the same number of rows (the wallet's secret key),
+        base (2, 4) (G', host-read, as in fixed_base_batch), R (n, 2, 4), pos (n,): a numpy uint64 array or a CUDA int64
+        tensor -> (nullifier (n, 4), ok (n,) uint8).  An item with a or b >= r_J or R not a curve point has ok == 0 and a
+        zeroed nullifier row (count: last_nullifier_invalid()).  A base off the curve raises InvalidPoint."""
+        rp, rl, flags, rk = self._in(R, (2, 4))
+        if len(rl) != 1:
+            raise EngineError(-1, "R must have shape (n, 2, 4)")
+        n = int(rl[0])
+        ap, al, fa, ak = self._in(a, (4,))
+        bp, bl, fb, bk = self._in(b, (4,))
+        self._same_space(flags, fa, fb, _native.MEM_DEVICE if _is_torch(pos) else _native.MEM_HOST)
+        if len(al) != 1 or int(al[0]) not in (1, n):
+            raise EngineError(-1, "a must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(al)))
+        ns = int(al[0])
+        if tuple(bl) != (ns,):
+            raise EngineError(-1, "b must have %d rows like a, got leading shape %s" % (ns, tuple(bl)))
+        pp, npos, pk = self._idx(pos, rk, "pos")
+        if npos != n:
+            raise EngineError(-1, "pos must have %d entries, got %d" % (n, npos))
+        g = self._base(base)
+        res = self._result(out, (n, 4), rk)
+        ok = self._ok_like(rk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("nullifier_invalid", flags)
+        self._check(self._lib.p252_nullifier_batch(self._ctx, ap, bp, ns, g.ctypes.data, rp, pp, n, self._ptr(res),
+                                                   self._ptr(ok), ctypes.byref(invalid), flags))
+        return res, ok
+
+    def last_nullifier_invalid(self):
+        """Invalid items of the last nullifier_batch (sync() first after async_)."""
+        return self._last("nullifier_invalid")
+
     # -- point compression ------------------------------------------------------------------------
     def points_from_bytes(self, data, out=None, async_=False):
         """JubJubAffine::from_bytes over a batch: (n, 32) uint8 encodings (host) or (n, 4) 64-bit device tensor of the
