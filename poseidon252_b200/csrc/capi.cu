@@ -28,6 +28,7 @@
 #include <initializer_list>
 #include <mutex>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "../../include/poseidon252_b200.h"
@@ -299,7 +300,7 @@ size_t pipeline_chunk(const std::vector<Io>& ios, size_t n) {
 }
 
 // Fixed-size HOST batches: the items stream through the slot arenas in chunks, each buffer of `ios` staged in its own
-// region, one launch per chunk.
+// region.  launch(d, cnt, st) enqueues a chunk's kernels, each through launched(), and returns a P252_* status.
 template <typename Launch>
 int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
     if (n == 0) return P252_OK;
@@ -334,7 +335,7 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
                                        cudaMemcpyHostToDevice, sl.stream));
             }
             if ((long long)k == fail_at) return injected_fault(ctx);
-            if ((rc = launched(ctx, launch(d.data(), cnt, sl.stream))) != P252_OK) return rc;
+            if ((rc = launch(d.data(), cnt, sl.stream)) != P252_OK) return rc;
             for (size_t b = 0; b < ios.size(); ++b)
                 if (ios[b].h_out && !ios[b].device)
                     CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + off * ios[b].item_bytes, d[b],
@@ -374,24 +375,105 @@ int counter_begin(p252_ctx* ctx, int count = 1) {
     CU(cudaMemsetAsync(ctx->d_counter, 0, count * sizeof(unsigned long long), ctx->stream));
     return P252_OK;
 }
+template <typename T>
 void CUDART_CB publish_counter(void* arg) {
-    auto* pr = static_cast<std::pair<const unsigned long long*, size_t*>*>(arg);
-    *pr->second = (size_t)*pr->first;
+    auto* pr = static_cast<std::pair<const unsigned long long*, T*>*>(arg);
+    *pr->second = std::is_same<T, uint8_t>::value ? (T)(*pr->first != 0) : (T)*pr->first;
     delete pr;
 }
-// ... and after it copy the counter to the pinned mirror and from there to the caller's size_t (a host function on
-// the stream, so that P252_ASYNC callers see it after p252_sync).
-int counter_end(p252_ctx* ctx, size_t* n_failed, int slot = 0) {
-    if (!n_failed) return P252_OK;
+// ... and after it copy counter `slot` to the pinned mirror and from there to the caller's size_t, or as a yes / no answer
+// (0 or 1) to the caller's byte (a host function on the stream, so that P252_ASYNC callers see it after p252_sync).
+template <typename T>
+int counter_end(p252_ctx* ctx, T* out, int slot = 0) {
+    if (!out) return P252_OK;
     CU(cudaMemcpyAsync(ctx->h_counter + slot, ctx->d_counter + slot, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
                        ctx->stream));
-    auto* pr = new std::pair<const unsigned long long*, size_t*>(ctx->h_counter + slot, n_failed);
-    cudaError_t e = cudaLaunchHostFunc(ctx->stream, publish_counter, pr);
+    auto* pr = new std::pair<const unsigned long long*, T*>(ctx->h_counter + slot, out);
+    cudaError_t e = cudaLaunchHostFunc(ctx->stream, publish_counter<T>, pr);
     if (e != cudaSuccess) {
         delete pr;
         return fail_cuda(ctx, e, "cudaLaunchHostFunc");
     }
     return P252_OK;
+}
+
+bool one_or_n(size_t k, size_t n) { return k == 1 || k == n; }
+
+// The buffer checks of a fixed-length batch call of n items: with n > 0 no listed buffer may be NULL, and DEVICE buffers
+// must be 16-byte aligned (`rows`: field elements, scalars, points) or 8-byte aligned (`idx`: uint64 indices).  Result
+// bytes (`bytes`: ok / owned / verified) need no alignment.
+bool args_ok(size_t n, int flags, std::initializer_list<const void*> rows, std::initializer_list<const void*> bytes = {},
+             std::initializer_list<const void*> idx = {}) {
+    const bool dev = (flags & P252_MEM_DEVICE) != 0;
+    for (auto list : {rows, bytes, idx})
+        for (const void* b : list)
+            if (n && !b) return false;
+    for (const void* b : rows)
+        if (dev && !aligned16(b)) return false;
+    for (const void* b : idx)
+        if (dev && (reinterpret_cast<uintptr_t>(b) & 7)) return false;
+    return true;
+}
+
+// The failure counts of a fixed-length batch call, and the tail of its DEVICE calls.  The constructor zeroes the caller's
+// counts, begin() zeroes the device counters before the first launch, counter(i) is device counter i for the kernels
+// (null where nothing is counted on the device), and end(rc) publishes the counts and returns the call's status.
+//   ok-recount (the constructor): HOST calls recount the zero bytes of ok[0, n) on the host, DEVICE calls count on device
+//     counter 0.  Without a count pointer only the DEVICE tail is left (device_done).
+//   device-counted (Counts::device): both memory spaces count on device counters 0 and 1, for when ok[] alone cannot tell
+//     what is counted; counter 1 may instead be a yes / no answer published as one byte.  HOST calls return with them
+//     published.
+struct Counts {
+    p252_ctx* ctx;
+    int flags;
+    size_t* count[2];
+    uint8_t* answer = nullptr;
+    const uint8_t* ok;
+    size_t n;
+    bool device_counted = false;
+
+    Counts(p252_ctx* c, int f, size_t* failed = nullptr, const uint8_t* ok_ = nullptr, size_t n_ = 0)
+        : ctx(c), flags(f), count{failed, nullptr}, ok(ok_), n(n_) {
+        if (failed) *failed = 0;
+    }
+    static Counts device(p252_ctx* c, int f, size_t* c0, size_t* c1 = nullptr, uint8_t* answer = nullptr) {
+        Counts k(c, f, c0);
+        if ((k.count[1] = c1)) *c1 = 0;
+        k.answer = answer;
+        k.device_counted = true;
+        return k;
+    }
+    bool on_device() const { return device_counted || (flags & P252_MEM_DEVICE); }
+    unsigned long long* counter(int i) const {
+        return on_device() && (count[i] || (i == 1 && answer)) ? ctx->d_counter + i : nullptr;
+    }
+    int begin() const {
+        if (!counter(0) && !counter(1)) return P252_OK;
+        return counter_begin(ctx, counter(1) ? 2 : 1);
+    }
+    int end(int rc) const {
+        if (!on_device()) {
+            if (rc == P252_OK && count[0]) *count[0] = count_zero(ok, n);
+            return rc;
+        }
+        if (rc == P252_OK) rc = counter_end(ctx, count[0], 0);
+        if (rc == P252_OK) rc = counter_end(ctx, count[1], 1);
+        if (rc == P252_OK) rc = counter_end(ctx, answer, 1);
+        return device_done(ctx, rc, (flags & P252_MEM_DEVICE) ? flags : 0);   // HOST calls return with their counts published
+    }
+};
+
+// A single-launch batch call states its launch once, as launch(d, cnt, st) over the buffers of `ios`: DEVICE buffers run it
+// once on the context stream with the caller's pointers, HOST buffers through run_host_pipeline with the staged ones.
+template <typename Launch>
+int launch_batch(const Counts& counts, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
+    if (!(counts.flags & P252_MEM_DEVICE)) return counts.end(run_host_pipeline(counts.ctx, ios, n, launch, wipe));
+    if (n == 0) return P252_OK;
+    const int rc = counts.begin();
+    if (rc != P252_OK) return rc;
+    std::vector<void*> d;
+    for (const Io& io : ios) d.push_back(io.h_out ? io.h_out : const_cast<void*>(io.h_in));
+    return counts.end(launch(d.data(), n, counts.ctx->stream));
 }
 
 uint64_t domain_sep(int domain, bool* ok) {
@@ -701,17 +783,12 @@ int p252_encryption_tag(size_t L, p252_fr* tag) {
 
 // ---- batch entry points ---------------------------------------------------------------------------
 static int permute_impl(p252_ctx* ctx, p252_fr* states, size_t n, int flags, bool dense) {
-    if (!ctx || (!states && n)) return P252_ERR_INVALID_ARGUMENT;
+    if (!ctx || !args_ok(n, flags, {states})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(states)) return P252_ERR_INVALID_ARGUMENT;
-        if (n == 0) return P252_OK;
-        return device_done(ctx, launched(ctx, p252::launch_permute(states, n, dense, ctx->coop_max, ctx->stream)), flags);
-    }
     std::vector<Io> ios = {{states, states, 160}};
-    return run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_permute(d[0], cnt, dense, ctx->coop_max, st);
+    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_permute(d[0], cnt, dense, ctx->coop_max, st));
     });
 }
 
@@ -722,23 +799,20 @@ int p252_permute_batch_dense(p252_ctx* ctx, p252_fr* states, size_t n, int flags
     return permute_impl(ctx, states, n, flags, true);
 }
 
+// Here and in the encrypt / decrypt batches a NULL buffer is refused before the io pattern is checked, a misaligned
+// DEVICE buffer (args_ok) after it.
 static int digest_impl(p252_ctx* ctx, const p252_fr* tag, const p252_fr* in, size_t n, size_t in_len, p252_fr* out,
                        size_t out_len, int flags, bool truncate) {
     if (!ctx || !tag || ((!in || !out) && n)) return P252_ERR_INVALID_ARGUMENT;
     if (in_len == 0 || out_len == 0) return P252_ERR_INVALID_IO_PATTERN;
-    if (in_len > 0x7fffffffull / 32 || out_len > 0x7fffffffull / 32) return P252_ERR_INVALID_ARGUMENT;
+    if (in_len > 0x7fffffffull / 32 || out_len > 0x7fffffffull / 32 || !args_ok(n, flags, {in, out}))
+        return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const uint32_t il = (uint32_t)in_len, ol = (uint32_t)out_len;
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(in) || !aligned16(out)) return P252_ERR_INVALID_ARGUMENT;
-        if (n == 0) return P252_OK;
-        return device_done(
-            ctx, launched(ctx, p252::launch_digest(limbs(tag), in, n, il, out, ol, truncate, ctx->coop_max, ctx->stream)), flags);
-    }
     std::vector<Io> ios = {{in, nullptr, in_len * 32}, {nullptr, out, out_len * 32}};
-    return run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_digest(limbs(tag), d[0], cnt, il, d[1], ol, truncate, ctx->coop_max, st);
+    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_digest(limbs(tag), d[0], cnt, il, d[1], ol, truncate, ctx->coop_max, st));
     });
 }
 
@@ -764,18 +838,14 @@ int p252_hash_batch_truncated(p252_ctx* ctx, int domain, const p252_fr* in, size
 }
 
 static int convert_impl(p252_ctx* ctx, const void* in, size_t n, void* out, uint8_t* ok, int flags, bool from_bytes) {
-    if (!ctx || ((!in || !out) && n)) return P252_ERR_INVALID_ARGUMENT;
+    if (!ctx || !args_ok(n, flags, {in, out})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(in) || !aligned16(out)) return P252_ERR_INVALID_ARGUMENT;
-        if (n == 0) return P252_OK;
-        return device_done(ctx, launched(ctx, p252::launch_convert(in, n, out, ok, from_bytes, ctx->stream)), flags);
-    }
     std::vector<Io> ios = {{in, nullptr, 32}, {nullptr, out, 32}};
     if (from_bytes && ok) ios.push_back({nullptr, ok, 1});
-    return run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_convert(d[0], cnt, d[1], (from_bytes && ok) ? static_cast<uint8_t*>(d[2]) : nullptr, from_bytes, st);
+    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = (from_bytes && ok) ? static_cast<uint8_t*>(d[2]) : nullptr;
+        return launched(ctx, p252::launch_convert(d[0], cnt, d[1], okc, from_bytes, st));
     });
 }
 
@@ -793,20 +863,14 @@ int p252_encrypt_batch(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, co
     p252_fr tag;
     int rc = p252_encryption_tag(L, &tag);
     if (rc != P252_OK) return rc;
+    if (!args_ok(n, flags, {msg, secret_uv, nonce, cipher})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const uint32_t l32 = (uint32_t)L;
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(msg) || !aligned16(secret_uv) || !aligned16(nonce) || !aligned16(cipher))
-            return P252_ERR_INVALID_ARGUMENT;
-        if (n == 0) return P252_OK;
-        return device_done(
-            ctx, launched(ctx, p252::launch_encrypt(limbs(&tag), msg, n, l32, secret_uv, nonce, cipher, ctx->stream)), flags);
-    }
     std::vector<Io> ios = {{msg, nullptr, L * 32}, {secret_uv, nullptr, 64}, {nonce, nullptr, 32},
                            {nullptr, cipher, (L + 1) * 32}};
-    return run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], st);
+    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], st));
     }, /*wipe=*/true);
 }
 
@@ -816,69 +880,32 @@ int p252_decrypt_batch(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L,
     p252_fr tag;
     int rc = p252_encryption_tag(L, &tag);
     if (rc != P252_OK) return rc;
+    if (!args_ok(n, flags, {cipher, secret_uv, nonce, msg}, {ok})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const uint32_t l32 = (uint32_t)L;
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(cipher) || !aligned16(secret_uv) || !aligned16(nonce) || !aligned16(msg))
-            return P252_ERR_INVALID_ARGUMENT;
-        if (n_failed) *n_failed = 0;
-        if (n == 0) return P252_OK;
-        if (n_failed && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        rc = launched(ctx, p252::launch_decrypt(limbs(&tag), cipher, n, l32, secret_uv, nonce, msg, ok,
-                                                n_failed ? ctx->d_counter : nullptr, ctx->stream));
-        if (rc == P252_OK) rc = counter_end(ctx, n_failed);
-        return device_done(ctx, rc, flags);
-    }
+    const Counts counts(ctx, flags, n_failed, ok, n);
     std::vector<Io> ios = {{cipher, nullptr, (L + 1) * 32}, {secret_uv, nullptr, 64}, {nonce, nullptr, 32},
                            {nullptr, msg, L * 32}, {nullptr, ok, 1}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], static_cast<uint8_t*>(d[4]), nullptr, st);
+    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], static_cast<uint8_t*>(d[4]),
+                                                  counts.counter(0), st));
     }, /*wipe=*/true);
-    if (rc == P252_OK && n_failed) *n_failed = count_zero(ok, n);
-    return rc;
 }
 
 // ---- JubJub key exchange (dhke) and the encrypt / decrypt batches that derive their shared secret with it -------------
-// Batch checks shared by the three calls: the broadcast shapes (1 or n), NULL buffers with n > 0 (ok is a byte array and
-// needs no alignment), 16-byte alignment of DEVICE buffers.
-static int dhke_args(size_t n, const void* secret, size_t n_secret, const void* pub, size_t n_public,
-                     std::initializer_list<const void*> bufs, const uint8_t* ok, int flags) {
-    if ((n_secret != 1 && n_secret != n) || (n_public != 1 && n_public != n)) return P252_ERR_INVALID_ARGUMENT;
-    if (n && (!secret || !pub || !ok)) return P252_ERR_INVALID_ARGUMENT;
-    for (const void* b : bufs)
-        if (n && !b) return P252_ERR_INVALID_ARGUMENT;
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(secret) || !aligned16(pub)) return P252_ERR_INVALID_ARGUMENT;
-        for (const void* b : bufs)
-            if (!aligned16(b)) return P252_ERR_INVALID_ARGUMENT;
-    }
-    return P252_OK;
-}
-
 int p252_dhke_batch(p252_ctx* ctx, const p252_jscalar* secret, size_t n_secret, const p252_fr* public_uv, size_t n_public,
                     size_t n, p252_fr* shared_uv, uint8_t* ok, size_t* n_invalid, int flags) {
-    if (!ctx) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, secret, n_secret, public_uv, n_public, {shared_uv}, ok, flags);
-    if (rc != P252_OK) return rc;
+    if (!ctx || !one_or_n(n_secret, n) || !one_or_n(n_public, n) || !args_ok(n, flags, {secret, public_uv, shared_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool sb = n_secret == 1, pb = n_public == 1;
-    if (flags & P252_MEM_DEVICE) {
-        if (n_invalid) *n_invalid = 0;
-        if (n == 0) return P252_OK;
-        if (n_invalid && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        rc = launched(ctx, p252::launch_dhke(secret, sb, public_uv, pb, n, shared_uv, ok, n_invalid ? ctx->d_counter : nullptr,
-                                             ctx->stream));
-        if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-        return device_done(ctx, rc, flags);
-    }
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     std::vector<Io> ios = {{secret, nullptr, 32, sb}, {public_uv, nullptr, 64, pb}, {nullptr, shared_uv, 64}, {nullptr, ok, 1}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_dhke(d[0], sb, d[1], pb, cnt, d[2], static_cast<uint8_t*>(d[3]), nullptr, st);
+    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_dhke(d[0], sb, d[1], pb, cnt, d[2], static_cast<uint8_t*>(d[3]), counts.counter(0), st));
     }, /*wipe=*/true);
-    if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-    return rc;
 }
 
 // launch_dhke into a slot arena, then the unchanged launch_encrypt / launch_decrypt on those shared secrets, then
@@ -888,22 +915,19 @@ int p252_dhke_batch(p252_ctx* ctx, const p252_jscalar* secret, size_t n_secret, 
 static int crypt_dhke(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n, size_t L, const p252_jscalar* secret,
                       size_t n_secret, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce, p252_fr* out,
                       uint8_t* ok, size_t* count, int flags) {
-    if (!ctx) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, secret, n_secret, public_uv, n_public, {in, nonce, out}, ok, flags);
-    if (rc != P252_OK) return rc;
+    if (!ctx || !one_or_n(n_secret, n) || !one_or_n(n_public, n) ||
+        !args_ok(n, flags, {in, secret, public_uv, nonce, out}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
     p252_fr tag;
-    if ((rc = p252_encryption_tag(L, &tag)) != P252_OK) return rc;
+    int rc = p252_encryption_tag(L, &tag);
+    if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1, pb = n_public == 1;
     const uint32_t l32 = (uint32_t)L, out_row = decrypt ? l32 : l32 + 1;
-    if (count) *count = 0;
+    const Counts counts(ctx, flags, count, ok, n);
     if (n == 0) return P252_OK;
-    unsigned long long* counter = nullptr;
-    if (dev && count) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    if ((rc = counts.begin()) != P252_OK) return rc;
     // 0 input, 1 secret, 2 public, 3 nonce, 4 output, 5 ok; 6 shared secrets and 7 validity live in the arena only
     std::vector<Io> ios = {{in, nullptr, (decrypt ? L + 1 : L) * 32, false, dev}, {secret, nullptr, 32, sb, dev},
                            {public_uv, nullptr, 64, pb, dev}, {nonce, nullptr, 32, false, dev},
@@ -912,20 +936,15 @@ static int crypt_dhke(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n, 
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* okc = static_cast<uint8_t*>(d[5]);
         uint8_t* valid = static_cast<uint8_t*>(d[7]);
-        cudaError_t e = p252::launch_dhke(d[1], sb, d[2], pb, cnt, d[6], valid, nullptr, st);
-        if (e == cudaSuccess)
-            e = decrypt ? p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], okc, counter, st)
-                        : p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], st);
-        if (e == cudaSuccess) e = p252::launch_dhke_fix(decrypt, valid, cnt, d[4], out_row, okc, counter, st);
-        if (e == cudaSuccess) ctx->launches += 2;   // run_host_pipeline counts the chunk's first launch
+        unsigned long long* counter = counts.counter(0);
+        int e = launched(ctx, p252::launch_dhke(d[1], sb, d[2], pb, cnt, d[6], valid, nullptr, st));
+        if (e == P252_OK)
+            e = launched(ctx, decrypt ? p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], okc, counter, st)
+                                      : p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(decrypt, valid, cnt, d[4], out_row, okc, counter, st));
         return e;
     }, /*wipe=*/true);
-    if (!dev) {
-        if (rc == P252_OK && count) *count = count_zero(ok, n);
-        return rc;
-    }
-    if (rc == P252_OK) rc = counter_end(ctx, count);
-    return device_done(ctx, rc, flags);
+    return counts.end(rc);
 }
 
 int p252_encrypt_batch_dhke(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* secret, size_t n_secret,
@@ -975,30 +994,19 @@ static int base_table(p252_ctx* ctx, const p252_fr* base_uv, const void** table)
 
 int p252_fixed_base_batch(p252_ctx* ctx, const p252_fr* base_uv, const p252_jscalar* secret, size_t n, p252_fr* out_uv,
                           uint8_t* ok, size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
-    if (n && (!secret || !out_uv || !ok)) return P252_ERR_INVALID_ARGUMENT;
-    if ((flags & P252_MEM_DEVICE) && (!aligned16(secret) || !aligned16(out_uv))) return P252_ERR_INVALID_ARGUMENT;
+    if (!ctx || !base_uv || !args_ok(n, flags, {secret, out_uv}, {ok})) return P252_ERR_INVALID_ARGUMENT;
     int rc = base_check(base_uv);
     if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
     if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    if (flags & P252_MEM_DEVICE) {
-        if (n_invalid && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        rc = launched(ctx, p252::launch_fixed_base(secret, n, table, out_uv, ok, n_invalid ? ctx->d_counter : nullptr,
-                                                   ctx->stream));
-        if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-        return device_done(ctx, rc, flags);
-    }
     std::vector<Io> ios = {{secret, nullptr, 32}, {nullptr, out_uv, 64}, {nullptr, ok, 1}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_fixed_base(d[0], cnt, table, d[1], static_cast<uint8_t*>(d[2]), nullptr, st);
+    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[1], static_cast<uint8_t*>(d[2]), counts.counter(0), st));
     }, /*wipe=*/true);
-    if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-    return rc;
 }
 
 // The sender: launch_fixed_base (R), launch_dhke into a slot arena (the shared secrets), the unchanged launch_encrypt,
@@ -1008,25 +1016,19 @@ int p252_fixed_base_batch(p252_ctx* ctx, const p252_fr* base_uv, const p252_jsca
 int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* r,
                                  const p252_fr* base_uv, const p252_fr* public_uv, size_t n_public, const p252_fr* nonce,
                                  p252_fr* cipher, p252_fr* R_uv, uint8_t* ok, size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, r, n, public_uv, n_public, {msg, nonce, cipher, R_uv}, ok, flags);
-    if (rc != P252_OK) return rc;
+    if (!ctx || !base_uv || !one_or_n(n_public, n) || !args_ok(n, flags, {msg, r, public_uv, nonce, cipher, R_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
     p252_fr tag;
-    if ((rc = p252_encryption_tag(L, &tag)) != P252_OK) return rc;
-    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    int rc = p252_encryption_tag(L, &tag);
+    if (rc != P252_OK || (rc = base_check(base_uv)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
     const uint32_t l32 = (uint32_t)L;
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    unsigned long long* counter = nullptr;
-    if (dev && n_invalid) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 message, 1 r, 2 public, 3 nonce, 4 cipher, 5 R, 6 ok; 7 shared secrets and 8 validity live in the arena only
     std::vector<Io> ios = {{msg, nullptr, L * 32, false, dev}, {r, nullptr, 32, false, dev}, {public_uv, nullptr, 64, pb, dev},
                            {nonce, nullptr, 32, false, dev}, {nullptr, cipher, (size_t)(l32 + 1) * 32, false, dev},
@@ -1035,20 +1037,15 @@ int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, si
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* okc = static_cast<uint8_t*>(d[6]);
         uint8_t* valid = static_cast<uint8_t*>(d[8]);
-        cudaError_t e = p252::launch_fixed_base(d[1], cnt, table, d[5], okc, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_dhke(d[1], false, d[2], pb, cnt, d[7], valid, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[7], d[3], d[4], st);
-        if (e == cudaSuccess) e = p252::launch_dhke_fix(false, valid, cnt, d[4], l32 + 1, okc, counter, st);
-        if (e == cudaSuccess) e = p252::launch_dhke_fix(false, valid, cnt, d[5], 2, okc, nullptr, st);
-        if (e == cudaSuccess) ctx->launches += 4;   // run_host_pipeline counts the chunk's first launch
+        int e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table, d[5], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke(d[1], false, d[2], pb, cnt, d[7], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[7], d[3], d[4], st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[4], l32 + 1, okc, counts.counter(0), st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[5], 2, okc, nullptr, st));
         return e;
     }, /*wipe=*/true);
-    if (!dev) {
-        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-        return rc;
-    }
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-    return device_done(ctx, rc, flags);
+    return counts.end(rc);
 }
 
 // ---- stealth addresses: the sender's (R, note_pk) and the receiver's ownership scan ----------------------------------
@@ -1062,24 +1059,18 @@ static int stealth_tag(p252_fr* tag) { return p252_hash_tag(P252_DOMAIN_OTHER, 2
 int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, const p252_fr* base_uv, const p252_fr* A_uv,
                                const p252_fr* B_uv, size_t n_public, p252_fr* R_uv, p252_fr* note_pk_uv, uint8_t* ok,
                                size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, r, n, A_uv, n_public, {B_uv, R_uv, note_pk_uv}, ok, flags);
-    if (rc != P252_OK) return rc;
-    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    if (!ctx || !base_uv || !one_or_n(n_public, n) || !args_ok(n, flags, {r, A_uv, B_uv, R_uv, note_pk_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(base_uv);
     p252_fr tag;
-    if ((rc = stealth_tag(&tag)) != P252_OK) return rc;
+    if (rc != P252_OK || (rc = stealth_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    unsigned long long* counter = nullptr;
-    if (dev && n_invalid) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 r, 1 A, 2 B, 3 R, 4 note_pk, 5 ok; 6 shared points, 7 validity and 8 h live in the arena only
     std::vector<Io> ios = {{r, nullptr, 32, false, dev}, {A_uv, nullptr, 64, pb, dev}, {B_uv, nullptr, 64, pb, dev},
                            {nullptr, R_uv, 64, false, dev}, {nullptr, note_pk_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
@@ -1087,19 +1078,15 @@ int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, c
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* okc = static_cast<uint8_t*>(d[5]);
         uint8_t* valid = static_cast<uint8_t*>(d[7]);
-        cudaError_t e = p252::launch_fixed_base(d[0], cnt, table, d[3], okc, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_dhke(d[0], false, d[1], pb, cnt, d[6], valid, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st);
-        if (e == cudaSuccess) e = p252::launch_stealth_derive(d[8], cnt, table, d[2], pb, valid, d[3], d[4], okc, counter, st);
-        if (e == cudaSuccess) ctx->launches += 3;   // run_host_pipeline counts the chunk's first launch
+        int e = launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[3], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke(d[0], false, d[1], pb, cnt, d[6], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_stealth_derive(d[8], cnt, table, d[2], pb, valid, d[3], d[4], okc, counts.counter(0),
+                                                          st));
         return e;
     }, /*wipe=*/true);
-    if (!dev) {
-        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-        return rc;
-    }
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-    return device_done(ctx, rc, flags);
+    return counts.end(rc);
 }
 
 // The receiver's B is public and a HOST pointer, like the base: checked here, and its Niels form computed once on the host
@@ -1108,43 +1095,34 @@ int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, c
 int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p252_fr* spend_B_uv, const p252_fr* base_uv,
                             const p252_fr* R_uv, const p252_fr* note_pk_uv, size_t n, uint8_t* owned, size_t* n_owned,
                             size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv || !spend_B_uv) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, view_a, 1, R_uv, n, {note_pk_uv}, owned, flags);
-    if (rc != P252_OK) return rc;
+    if (!ctx || !base_uv || !spend_B_uv || !args_ok(n, flags, {view_a, R_uv, note_pk_uv}, {owned}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
     if ((rc = base_check(base_uv)) != P252_OK || (rc = base_check(spend_B_uv)) != P252_OK) return rc;
     p252_fr tag;
     if ((rc = stealth_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0;
-    if (n_owned) *n_owned = 0;
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts = Counts::device(ctx, flags, n_owned, n_invalid);
     if (n == 0) return P252_OK;
     uint64_t nb[12];
     p252::host::jubjub_niels(nb, spend_B_uv[0].l, spend_B_uv[1].l);
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    unsigned long long *c_owned = nullptr, *c_invalid = nullptr;
-    if (n_owned || n_invalid) {
-        if ((rc = counter_begin(ctx, 2)) != P252_OK) return rc;
-        c_owned = n_owned ? ctx->d_counter : nullptr;
-        c_invalid = n_invalid ? ctx->d_counter + 1 : nullptr;
-    }
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 view_a, 1 R, 2 note_pk, 3 owned; 4 shared points, 5 validity and 6 h live in the arena only
     std::vector<Io> ios = {{view_a, nullptr, 32, true, dev}, {R_uv, nullptr, 64, false, dev}, {note_pk_uv, nullptr, 64, false, dev},
                            {nullptr, owned, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* valid = static_cast<uint8_t*>(d[5]);
-        cudaError_t e = p252::launch_dhke(d[0], true, d[1], false, cnt, d[4], valid, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[4], cnt, 2, d[6], 1, true, ctx->coop_max, st);
-        if (e == cudaSuccess)
-            e = p252::launch_stealth_owns(d[6], cnt, table, nb, d[2], valid, static_cast<uint8_t*>(d[3]), c_owned, c_invalid, st);
-        if (e == cudaSuccess) ctx->launches += 2;   // run_host_pipeline counts the chunk's first launch
+        int e = launched(ctx, p252::launch_dhke(d[0], true, d[1], false, cnt, d[4], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[4], cnt, 2, d[6], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_stealth_owns(d[6], cnt, table, nb, d[2], valid, static_cast<uint8_t*>(d[3]),
+                                                        counts.counter(0), counts.counter(1), st));
         return e;
     }, /*wipe=*/true);
-    if (rc == P252_OK) rc = counter_end(ctx, n_owned, 0);
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
-    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
+    return counts.end(rc);
 }
 
 // ---- Schnorr signatures over JubJub: signing and verification ----------------------------------------------------------
@@ -1158,43 +1136,32 @@ static int schnorr_tag(p252_fr* tag) { return p252_hash_tag(P252_DOMAIN_OTHER, 3
 int p252_schnorr_sign_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_jscalar* r, const p252_fr* msg,
                             size_t n, const p252_fr* base_uv, p252_jscalar* u_out, p252_fr* R_uv, uint8_t* ok, size_t* n_invalid,
                             int flags) {
-    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, r, n, sk, n_secret, {msg, u_out, R_uv}, ok, flags);
-    if (rc != P252_OK) return rc;
-    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    if (!ctx || !base_uv || !one_or_n(n_secret, n) || !args_ok(n, flags, {sk, r, msg, u_out, R_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(base_uv);
     p252_fr tag;
-    if ((rc = schnorr_tag(&tag)) != P252_OK) return rc;
+    if (rc != P252_OK || (rc = schnorr_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    unsigned long long* counter = nullptr;
-    if (dev && n_invalid) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 sk, 1 r, 2 msg, 3 u, 4 R, 5 ok; 6 the digest rows and 7 c live in the arena only
     std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev},
                            {nullptr, u_out, 32, false, dev}, {nullptr, R_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
                            {nullptr, nullptr, 96}, {nullptr, nullptr, 32}};
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* okc = static_cast<uint8_t*>(d[5]);
-        cudaError_t e = p252::launch_fixed_base(d[1], cnt, table, d[4], okc, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_schnorr_pack(d[4], d[2], cnt, d[6], okc, true, st);
-        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[6], cnt, 3, d[7], 1, true, ctx->coop_max, st);
-        if (e == cudaSuccess) e = p252::launch_schnorr_sign(d[0], sb, d[1], d[7], cnt, d[3], d[4], okc, counter, st);
-        if (e == cudaSuccess) ctx->launches += 3;   // run_host_pipeline counts the chunk's first launch
+        int e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table, d[4], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_schnorr_pack(d[4], d[2], cnt, d[6], okc, true, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[6], cnt, 3, d[7], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_schnorr_sign(d[0], sb, d[1], d[7], cnt, d[3], d[4], okc, counts.counter(0), st));
         return e;
     }, /*wipe=*/true);
-    if (!dev) {
-        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-        return rc;
-    }
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-    return device_done(ctx, rc, flags);
+    return counts.end(rc);
 }
 
 // An item's verified flag does not tell an invalid item from a signature that does not verify, so both counts come from
@@ -1202,43 +1169,32 @@ int p252_schnorr_sign_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secr
 int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_jscalar* u, const p252_fr* R_uv,
                               const p252_fr* msg, size_t n, const p252_fr* base_uv, uint8_t* verified, size_t* n_verified,
                               size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, u, n, pk_uv, n_public, {R_uv, msg}, verified, flags);
-    if (rc != P252_OK) return rc;
-    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    if (!ctx || !base_uv || !one_or_n(n_public, n) || !args_ok(n, flags, {pk_uv, u, R_uv, msg}, {verified}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(base_uv);
     p252_fr tag;
-    if ((rc = schnorr_tag(&tag)) != P252_OK) return rc;
+    if (rc != P252_OK || (rc = schnorr_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
-    if (n_verified) *n_verified = 0;
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts = Counts::device(ctx, flags, n_verified, n_invalid);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    unsigned long long *c_ok = nullptr, *c_bad = nullptr;
-    if (n_verified || n_invalid) {
-        if ((rc = counter_begin(ctx, 2)) != P252_OK) return rc;
-        c_ok = n_verified ? ctx->d_counter : nullptr;
-        c_bad = n_invalid ? ctx->d_counter + 1 : nullptr;
-    }
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 PK, 1 u, 2 R, 3 msg, 4 verified; 5 the digest rows, 6 validity and 7 c live in the arena only
     std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev}, {R_uv, nullptr, 64, false, dev},
                            {msg, nullptr, 32, false, dev}, {nullptr, verified, 1, false, dev}, {nullptr, nullptr, 96},
                            {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* valid = static_cast<uint8_t*>(d[6]);
-        cudaError_t e = p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st);
-        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st);
-        if (e == cudaSuccess)
-            e = p252::launch_schnorr_verify(d[0], pb, d[1], d[2], d[7], valid, cnt, table, static_cast<uint8_t*>(d[4]), c_ok,
-                                            c_bad, st);
-        if (e == cudaSuccess) ctx->launches += 2;   // run_host_pipeline counts the chunk's first launch
+        int e = launched(ctx, p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_schnorr_verify(d[0], pb, d[1], d[2], d[7], valid, cnt, table,
+                                                          static_cast<uint8_t*>(d[4]), counts.counter(0), counts.counter(1), st));
         return e;
     });
-    if (rc == P252_OK) rc = counter_end(ctx, n_verified, 0);
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 1);
-    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with their counts published
+    return counts.end(rc);
 }
 
 // ---- note nullifiers: Hash::digest(Domain::Other, [pk'.u, pk'.v, pos])[0], pk' = [(hash([a] R) + b) mod r_J] G' --------
@@ -1251,46 +1207,36 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
 int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret, const p252_fr* base_uv,
                          const p252_fr* R_uv, const uint64_t* pos, size_t n, p252_fr* nullifier, uint8_t* ok,
                          size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv || (n && !pos)) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, a, n_secret, R_uv, n, {b, nullifier}, ok, flags);
-    if (rc != P252_OK) return rc;
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
-    if (dev && (reinterpret_cast<uintptr_t>(pos) & 7)) return P252_ERR_INVALID_ARGUMENT;
-    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    if (!ctx || !base_uv || !one_or_n(n_secret, n) || !args_ok(n, flags, {a, b, R_uv, nullifier}, {ok}, {pos}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(base_uv);
     p252_fr tag_h, tag_n;
-    if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_tag(&tag_n)) != P252_OK) return rc;
+    if (rc != P252_OK || (rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_tag(&tag_n)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (n_invalid) *n_invalid = 0;
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
-    unsigned long long* counter = nullptr;
-    if (dev && n_invalid) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 a, 1 b, 2 R, 3 pos, 4 nullifier, 5 ok; 6 shared points, 7 validity, 8 h and 9 the digest rows live in the arena only
     std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev},
                            {pos, nullptr, 8, false, dev}, {nullptr, nullifier, 32, false, dev}, {nullptr, ok, 1, false, dev},
                            {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 96}};
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* valid = static_cast<uint8_t*>(d[7]);
-        cudaError_t e = p252::launch_dhke(d[0], sb, d[2], false, cnt, d[6], valid, nullptr, st);
-        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag_h), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st);
-        if (e == cudaSuccess)
-            e = p252::launch_nullifier_key(d[8], d[1], sb, static_cast<const uint64_t*>(d[3]), cnt, table, d[9], valid, st);
-        if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag_n), d[9], cnt, 3, d[4], 1, false, ctx->coop_max, st);
-        if (e == cudaSuccess) e = p252::launch_dhke_fix(false, valid, cnt, d[4], 1, static_cast<uint8_t*>(d[5]), counter, st);
-        if (e == cudaSuccess) ctx->launches += 4;   // run_host_pipeline counts the chunk's first launch
+        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[2], false, cnt, d[6], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_nullifier_key(d[8], d[1], sb, static_cast<const uint64_t*>(d[3]), cnt, table, d[9],
+                                                         valid, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_n), d[9], cnt, 3, d[4], 1, false, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[4], 1, static_cast<uint8_t*>(d[5]), counts.counter(0),
+                                                    st));
         return e;
     }, /*wipe=*/true);
-    if (!dev) {
-        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-        return rc;
-    }
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-    return device_done(ctx, rc, flags);
+    return counts.end(rc);
 }
 
 // ---- JubJub point compression: JubJubAffine::from_bytes / to_bytes -----------------------------------------------------
@@ -1299,33 +1245,23 @@ int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscala
 // host, DEVICE calls on the device counter.
 static int points_impl(p252_ctx* ctx, bool from_bytes, const void* in, size_t n, void* out, uint8_t* ok, size_t* n_invalid,
                        int flags) {
-    if (!ctx || (n && (!in || !out || !ok))) return P252_ERR_INVALID_ARGUMENT;
+    if (!ctx || !args_ok(n, flags, {in, out}, {ok})) return P252_ERR_INVALID_ARGUMENT;
     const bool dev = (flags & P252_MEM_DEVICE) != 0;
-    if (dev && (!aligned16(in) || !aligned16(out))) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
-    int rc = P252_OK;
-    unsigned long long* counter = nullptr;
-    if (dev && n_invalid) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    int rc = counts.begin();
+    if (rc != P252_OK) return rc;
     const size_t in_bytes = from_bytes ? 32 : 64, out_bytes = from_bytes ? 64 : 32;
     // 0 input, 1 output, 2 ok
     std::vector<Io> ios = {{in, nullptr, in_bytes, false, dev}, {nullptr, out, out_bytes, false, dev}, {nullptr, ok, 1, false, dev}};
     rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         uint8_t* okc = static_cast<uint8_t*>(d[2]);
-        return from_bytes ? p252::launch_points_from_bytes(d[0], cnt, d[1], okc, counter, st)
-                          : p252::launch_points_to_bytes(d[0], cnt, d[1], okc, counter, st);
+        return launched(ctx, from_bytes ? p252::launch_points_from_bytes(d[0], cnt, d[1], okc, counts.counter(0), st)
+                                        : p252::launch_points_to_bytes(d[0], cnt, d[1], okc, counts.counter(0), st));
     });
-    if (!dev) {
-        if (rc == P252_OK && n_invalid) *n_invalid = count_zero(ok, n);
-        return rc;
-    }
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-    return device_done(ctx, rc, flags);
+    return counts.end(rc);
 }
 
 int p252_points_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out_uv, uint8_t* ok, size_t* n_invalid,
@@ -1388,74 +1324,48 @@ size_t msm_scratch_bytes(size_t M, int c) {
 // One chunk: m rows (scalars sc, points pt; device) into the W window sums at wsum, with the temporaries in `scratch`
 // (msm_scratch_bytes(M, c), m <= M): a region of the arena of the chunk's slot, so that a chunk reuses the region of that
 // slot's previous chunk in stream order.  The arenas persist with the context, so the temporaries cost no allocation per
-// call; they grow each arena to about 100-145 MiB (DESIGN.md section 4).  Counts its launches beyond the first
-// (run_host_pipeline counts that one).
-cudaError_t msm_chunk(p252_ctx* ctx, const void* sc, const void* pt, size_t m, int c, void* scratch, size_t M, uint4* wsum,
-                      unsigned long long* n_invalid, cudaStream_t st) {
+// call; they grow each arena to about 100-145 MiB (DESIGN.md section 4).
+int msm_chunk(p252_ctx* ctx, const void* sc, const void* pt, size_t m, int c, void* scratch, size_t M, uint4* wsum,
+              unsigned long long* n_invalid, cudaStream_t st) {
     Carve cv{static_cast<uint8_t*>(scratch)};
     MsmScratch s = msm_layout(cv, M, c);
     const uint32_t W = (uint32_t)p252::msm_windows(c), nb = W << (c - 1), N = (uint32_t)(m * W);
     int end_bit = 0;
     while ((1u << end_bit) <= nb) ++end_bit;         // keys <= nb (the sentinel)
-    cudaError_t e = p252::launch_msm_prep(sc, pt, (uint32_t)m, c, s.niels, s.ka, s.va, n_invalid, st);
-    if (e == cudaSuccess)
-        e = cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ka, s.kb, s.va, s.vb, (int)N, 0, end_bit, st);
-    if (e == cudaSuccess) e = p252::launch_msm_fill(s.buckets, nb, st);
+    int rc = launched(ctx, p252::launch_msm_prep(sc, pt, (uint32_t)m, c, s.niels, s.ka, s.va, n_invalid, st));
+    if (rc != P252_OK) return rc;
+    CU(cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ka, s.kb, s.va, s.vb, (int)N, 0, end_bit, st));
+    if ((rc = launched(ctx, p252::launch_msm_fill(s.buckets, nb, st))) != P252_OK) return rc;
     size_t pieces = ceil_div(N, p252::kMsmPiece);
-    int launches = 3;                                 // prep, fill, the first pass and the window sums, less one
-    if (e == cudaSuccess)
-        e = p252::launch_msm_bucket(true, s.kb, s.vb, s.niels, N, nb, s.buckets, pieces > 1 ? s.ck[0] : nullptr, s.cp[0], st);
-    for (int src = 0; e == cudaSuccess && pieces > 1; src ^= 1, ++launches) {
+    rc = launched(ctx, p252::launch_msm_bucket(true, s.kb, s.vb, s.niels, N, nb, s.buckets, pieces > 1 ? s.ck[0] : nullptr,
+                                               s.cp[0], st));
+    for (int src = 0; rc == P252_OK && pieces > 1; src ^= 1) {
         const uint32_t len = (uint32_t)(2 * pieces);
         pieces = ceil_div(len, p252::kMsmPiece);
-        e = p252::launch_msm_bucket(false, s.ck[src], nullptr, s.cp[src], len, nb, s.buckets,
-                                    pieces > 1 ? s.ck[src ^ 1] : nullptr, s.cp[src ^ 1], st);
+        rc = launched(ctx, p252::launch_msm_bucket(false, s.ck[src], nullptr, s.cp[src], len, nb, s.buckets,
+                                                   pieces > 1 ? s.ck[src ^ 1] : nullptr, s.cp[src ^ 1], st));
     }
-    if (e == cudaSuccess) e = p252::launch_msm_window(s.buckets, c, wsum, st);
-    if (e == cudaSuccess) ctx->launches += launches;
-    return e;
-}
-
-void CUDART_CB publish_flag(void* arg) {
-    auto* pr = static_cast<std::pair<const unsigned long long*, uint8_t*>*>(arg);
-    *pr->second = *pr->first ? 1 : 0;
-    delete pr;
-}
-// counter_end for a yes / no answer: device counter `slot` (0 or 1) -> the caller's byte
-int flag_end(p252_ctx* ctx, uint8_t* out, int slot) {
-    CU(cudaMemcpyAsync(ctx->h_counter + slot, ctx->d_counter + slot, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
-                       ctx->stream));
-    auto* pr = new std::pair<const unsigned long long*, uint8_t*>(ctx->h_counter + slot, out);
-    cudaError_t e = cudaLaunchHostFunc(ctx->stream, publish_flag, pr);
-    if (e != cudaSuccess) {
-        delete pr;
-        return fail_cuda(ctx, e, "cudaLaunchHostFunc");
-    }
-    return P252_OK;
+    if (rc == P252_OK) rc = launched(ctx, p252::launch_msm_window(s.buckets, c, wsum, st));
+    return rc;
 }
 
 }  // namespace
 
 int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* points_uv, size_t n, p252_fr* out_uv,
                     size_t* n_invalid, int flags) {
-    if (!ctx || !out_uv || (n && (!scalars || !points_uv))) return P252_ERR_INVALID_ARGUMENT;
+    if (!ctx || !out_uv || !args_ok(n, flags, {scalars, points_uv, out_uv})) return P252_ERR_INVALID_ARGUMENT;
     const bool dev = (flags & P252_MEM_DEVICE) != 0;
-    if (dev && (!aligned16(scalars) || !aligned16(points_uv) || !aligned16(out_uv))) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts = Counts::device(ctx, flags, n_invalid);
     // 0 scalars, 1 points; 2 the chunk's MSM temporaries (one region per slot arena)
     std::vector<Io> ios = {{scalars, nullptr, 32, false, dev}, {points_uv, nullptr, 64, false, dev}, {nullptr, nullptr, 0, true}};
     const size_t chunk = n ? pipeline_chunk(ios, n) : 0;
     const int c = p252::msm_bits(std::max<size_t>(chunk, 1));
     const size_t W = (size_t)p252::msm_windows(c), max_chunks = n ? ceil_div(n, chunk) + 3 : 0;
     ios[2].item_bytes = msm_scratch_bytes(chunk, c);
-    int rc = P252_OK;
-    unsigned long long* counter = nullptr;
-    if (n_invalid) {
-        if ((rc = counter_begin(ctx)) != P252_OK) return rc;
-        counter = ctx->d_counter;
-    }
+    int rc = counts.begin();
+    if (rc != P252_OK) return rc;
     uint4* wsum = nullptr;
     uint8_t* dout = nullptr;
     rc = with_scratch(ctx, ctx->stream, [&](Carve& cv) {
@@ -1464,7 +1374,7 @@ int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* p
     }, [&]() -> int {
         uint32_t k = 0;
         int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-            return msm_chunk(ctx, d[0], d[1], cnt, c, d[2], chunk, wsum + (size_t)(k++) * W * 8, counter, st);
+            return msm_chunk(ctx, d[0], d[1], cnt, c, d[2], chunk, wsum + (size_t)(k++) * W * 8, counts.counter(0), st);
         });
         if (r != P252_OK) return r;
         void* out = dev ? static_cast<void*>(out_uv) : dout;
@@ -1474,8 +1384,7 @@ int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* p
         if (!dev) CU(cudaMemcpyAsync(out_uv, dout, 64, cudaMemcpyDeviceToHost, ctx->stream));
         return P252_OK;
     });
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid);
-    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with the sum and the count published
+    return counts.end(rc);   // HOST calls return with the sum and the count published
 }
 
 // challenge(R, m) as in p252_schnorr_verify_batch.  Per chunk: launch_schnorr_pack and the truncated launch_digest (c), then
@@ -1485,16 +1394,15 @@ int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* p
 int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_jscalar* u, const p252_fr* R_uv,
                             const p252_fr* msg, const p252_jscalar* weight, size_t n, const p252_fr* base_uv,
                             uint8_t* all_verified, size_t* n_invalid, int flags) {
-    if (!ctx || !base_uv || !all_verified) return P252_ERR_INVALID_ARGUMENT;
-    int rc = dhke_args(n, u, n, pk_uv, n_public, {R_uv, msg, weight}, all_verified, flags);
-    if (rc != P252_OK) return rc;
-    if ((rc = base_check(base_uv)) != P252_OK) return rc;
+    if (!ctx || !base_uv || !all_verified || !one_or_n(n_public, n) || !args_ok(n, flags, {pk_uv, u, R_uv, msg, weight}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(base_uv);
     p252_fr tag;
-    if ((rc = schnorr_tag(&tag)) != P252_OK) return rc;
+    if (rc != P252_OK || (rc = schnorr_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
-    if (n_invalid) *n_invalid = 0;
+    const Counts counts = Counts::device(ctx, flags, n_invalid, nullptr, all_verified);
     if (n == 0) {
         *all_verified = 1;
         return P252_OK;
@@ -1513,7 +1421,7 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
     const size_t W = (size_t)p252::msm_windows(c), max_chunks = ceil_div(n, chunk) + 3;
     const size_t nsum = ceil_div(n, p252::kMsmItemsPerSum);
     ios[10].item_bytes = msm_scratch_bytes(M, c);
-    if ((rc = counter_begin(ctx, 2)) != P252_OK) return rc;
+    if ((rc = counts.begin()) != P252_OK) return rc;
     uint4* wsum = nullptr;
     uint8_t *zsum = nullptr, *pkc = nullptr;
     uint32_t* bad = nullptr;
@@ -1529,24 +1437,21 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
         size_t off = 0;
         int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
             uint8_t* valid = static_cast<uint8_t*>(d[6]);
-            cudaError_t e = p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st);
-            if (e == cudaSuccess) e = p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st);
-            if (e == cudaSuccess)
-                e = p252::launch_msmv_prep(d[0], pb, d[1], d[2], d[7], d[4], valid, (uint32_t)cnt, d[8], d[9], zsum,
-                                           (uint32_t)(off / p252::kMsmItemsPerSum), bad, n_invalid ? ctx->d_counter : nullptr,
-                                           st);
-            if (e == cudaSuccess) e = msm_chunk(ctx, d[8], d[9], cnt * per, c, d[10], M, wsum + (size_t)(k++) * W * 8, nullptr, st);
-            if (e == cudaSuccess) ctx->launches += 3;   // run_host_pipeline and msm_chunk count one launch each
+            const uint32_t sum0 = (uint32_t)(off / p252::kMsmItemsPerSum);
             off += cnt;
+            int e = launched(ctx, p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st));
+            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st));
+            if (e == P252_OK)
+                e = launched(ctx, p252::launch_msmv_prep(d[0], pb, d[1], d[2], d[7], d[4], valid, (uint32_t)cnt, d[8], d[9], zsum,
+                                                         sum0, bad, counts.counter(0), st));
+            if (e == P252_OK) e = msm_chunk(ctx, d[8], d[9], cnt * per, c, d[10], M, wsum + (size_t)(k++) * W * 8, nullptr, st);
             return e;
         });
         if (r != P252_OK) return r;
         return launched(ctx, p252::launch_msm_final(wsum, k, c, nullptr, zsum, (uint32_t)nsum, table, pb ? pkc : nullptr, bad,
-                                                    ctx->d_counter + 1, ctx->stream));
+                                                    counts.counter(1), ctx->stream));
     });
-    if (rc == P252_OK) rc = counter_end(ctx, n_invalid, 0);
-    if (rc == P252_OK) rc = flag_end(ctx, all_verified, 1);
-    return device_done(ctx, rc, dev ? flags : 0);   // HOST calls return with the answer and the count published
+    return counts.end(rc);   // HOST calls return with the answer and the count published
 }
 
 // ---- arity-4 Merkle tree ------------------------------------------------------------------------------
@@ -1617,12 +1522,13 @@ int p252_merkle_build(p252_ctx* ctx, int arity, const p252_fr* leaves, size_t n_
     {
         std::vector<Io> ios = {{leaves, nullptr, (size_t)arity * 32}, {nullptr, nodes_out, 32}};
         size_t done = 0;   // the pipeline hands chunks in order; mirror each chunk into d_nodes as well
-        rc = run_host_pipeline(ctx, ios, first, [&](void** d, size_t cnt, cudaStream_t st) {
-            cudaError_t e = p252::launch_digest(limbs(&tag), d[0], cnt, (uint32_t)arity, d[1], 1, false, ctx->coop_max, st);
-            if (e != cudaSuccess) return e;
-            e = cudaMemcpyAsync(d_nodes + done, d[1], cnt * sizeof(p252_fr), cudaMemcpyDeviceToDevice, st);
+        rc = run_host_pipeline(ctx, ios, first, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+            const int e = launched(ctx, p252::launch_digest(limbs(&tag), d[0], cnt, (uint32_t)arity, d[1], 1, false,
+                                                            ctx->coop_max, st));
+            if (e != P252_OK) return e;
+            CU(cudaMemcpyAsync(d_nodes + done, d[1], cnt * sizeof(p252_fr), cudaMemcpyDeviceToDevice, st));
             done += cnt;
-            return e;
+            return P252_OK;
         });
     }
     if (rc == P252_OK && first > 1) {
@@ -1683,32 +1589,21 @@ int p252_merkle_open_batch(p252_ctx* ctx, int arity, const p252_fr* leaves, size
 int p252_merkle_verify_batch(p252_ctx* ctx, int arity, int depth, const p252_fr* leaf_items, const uint64_t* leaf_idx,
                              const p252_fr* paths, const p252_fr* root, size_t n, uint8_t* ok, size_t* n_failed,
                              int flags) {
-    if (!ctx || !root || ((!leaf_items || !leaf_idx || !paths || !ok) && n)) return P252_ERR_INVALID_ARGUMENT;
+    if (!ctx || !root || !args_ok(n, flags, {leaf_items, paths}, {ok}, {leaf_idx})) return P252_ERR_INVALID_ARGUMENT;
     if (merkle_domain(arity) < 0 || depth < 1 || depth > 64) return P252_ERR_INVALID_ARGUMENT;
     p252_fr tag;
     int rc = p252_hash_tag(merkle_domain(arity), (size_t)arity, 1, &tag);
     if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    if (n_failed) *n_failed = 0;
-    if (flags & P252_MEM_DEVICE) {
-        if (!aligned16(leaf_items) || !aligned16(paths) || (reinterpret_cast<uintptr_t>(leaf_idx) & 7))
-            return P252_ERR_INVALID_ARGUMENT;
-        if (n == 0) return P252_OK;
-        if (n_failed && (rc = counter_begin(ctx)) != P252_OK) return rc;
-        rc = launched(ctx, p252::launch_merkle_verify(limbs(&tag), limbs(root), leaf_items, leaf_idx, paths, n, arity,
-                                                      (uint32_t)depth, ok, n_failed ? ctx->d_counter : nullptr, ctx->stream));
-        if (rc == P252_OK) rc = counter_end(ctx, n_failed);
-        return device_done(ctx, rc, flags);
-    }
+    const Counts counts(ctx, flags, n_failed, ok, n);
     const size_t path_bytes = (size_t)depth * (size_t)arity * 32;
     std::vector<Io> ios = {{leaf_items, nullptr, 32}, {leaf_idx, nullptr, 8}, {paths, nullptr, path_bytes}, {nullptr, ok, 1}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return p252::launch_merkle_verify(limbs(&tag), limbs(root), d[0], static_cast<const uint64_t*>(d[1]), d[2], cnt, arity,
-                                          (uint32_t)depth, static_cast<uint8_t*>(d[3]), nullptr, st);
+    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_merkle_verify(limbs(&tag), limbs(root), d[0], static_cast<const uint64_t*>(d[1]), d[2],
+                                                        cnt, arity, (uint32_t)depth, static_cast<uint8_t*>(d[3]),
+                                                        counts.counter(0), st));
     });
-    if (rc == P252_OK && n_failed) *n_failed = count_zero(ok, n);
-    return rc;
 }
 
 }  // extern "C"
