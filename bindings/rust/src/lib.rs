@@ -143,6 +143,10 @@ mod msm;
 // Phoenix note nullifiers (which owned notes are spent): their own `extern "C"` block in nullifier.rs (methods on Engine).
 mod nullifier;
 
+// Double-key Schnorr signatures over G and G' and spending a note under its note secret key: their own `extern "C"`
+// block in schnorr_double.rs (methods on Engine).
+mod schnorr_double;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

@@ -407,6 +407,53 @@ int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscala
                          const p252_fr* base_uv, const p252_fr* R_uv, const uint64_t* pos, size_t n,
                          p252_fr* nullifier, uint8_t* ok, size_t* n_invalid, int flags);
 
+/* ---- Double-key Schnorr signatures over G and G' (jubjub-schnorr's SignatureDouble) and spending a note -------------
+ *   challenge2(R, R', m) = Hash::digest_truncated(Domain::Other, [R.u, R.v, R'.u, R'.v, m])[0]      (c < 2^250 < r_J)
+ *   sign_double   (sk, r; m):            R = [r] G,  R' = [r] G',  u = (r - c sk) mod r_J,  signature = (u, R, R')
+ *   verify_double ((PK, PK'); (u, R, R'), m):  ok  <=>  [u] G + [c] PK == R  AND  [u] G' + [c] PK' == R'
+ *   note_sk(a, b, R_note) = (hash([a] R_note) + b) mod r_J     (hash: the stealth and nullifier calls' truncated digest)
+ * The key pair of a signature is (PK, PK') = ([sk] G, [sk] G'); a Phoenix note is spent under (note_pk, pk') =
+ * ([note_sk] G, [note_sk] G'), and pk' is the point p252_nullifier_batch hashes.  Both generators are caller arguments:
+ * G_uv and Gp_uv (G' = GENERATOR_NUMS) are HOST pointers for every memory space, and a coordinate >= p or a point off the
+ * curve in either is refused with P252_ERR_INVALID_POINT before anything runs, for every memory space and for n == 0.
+ * There is no built-in generator.  Scalars, points and messages are laid out as for p252_schnorr_sign_batch; both scalar
+ * multiplications multiply by the canonical integer and there is no subgroup check on PK or PK'.
+ * r is one nonce per item (no broadcast), with the same rules as for p252_schnorr_sign_batch.  n_secret (shared by a and b
+ * in the note call) and n_public (shared by PK and PK') are 1 or n.
+ * Item validity (checked on the device, for both memory spaces):
+ *   sign:      sk < r_J, r < r_J, msg < p.
+ *   note sign: a < r_J, b < r_J, R_note a curve point with u, v < p, r < r_J, msg < p.
+ *   verify:    u < r_J, msg < p, every coordinate of R and R' < p, PK and PK' curve points with u, v < p.
+ * An invalid item gets ok[i] = 0 (verified[i] = 0) and zeroed u, R, R' (and pk') rows, and is counted once into
+ * *n_invalid however many of its checks fail; verification counts it into *n_invalid, not *n_verified.  n_verified /
+ * n_invalid: optional HOST pointers for both memory spaces (lifetime as for p252_decrypt_batch).
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_secret / n_public not 1 or n, DEVICE buffers other than
+ * ok / verified not 16-byte aligned -> INVALID_ARGUMENT.
+ * Signing: sk, r, a, b, [a] R_note, its hash and note_sk live only in the context's staging arenas, for both memory
+ * spaces, and the arenas are zeroed on every exit path: both signing calls are synchronous (P252_ASYNC only defers the
+ * publication of *n_invalid to p252_sync).  Each item is constant time (no branch and no address depends on a secret); see
+ * DESIGN.md section 4.  pkp_uv, the note's pk' = [note_sk] G', is returned because a spend proof takes it as a witness: it
+ * links the spend to the note (it is the preimage of the note's nullifier) and must stay as private as the note itself.
+ * Verification reads public data only; P252_ASYNC defers the publication of the counts to p252_sync.
+ * The context caches the fixed-base tables of G and G' of these three calls in two slots of their own, apart from the
+ * one-base table of the other JubJub calls: none of these calls evicts that table, and no other call evicts theirs. */
+/* u[i], R_uv[i], Rp_uv[i] = sign_double(sk[n_secret == 1 ? 0 : i], r[i]; msg[i]) */
+int p252_schnorr_sign_double_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_jscalar* r,
+                                   const p252_fr* msg, size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv,
+                                   p252_jscalar* u, p252_fr* R_uv, p252_fr* Rp_uv, uint8_t* ok, size_t* n_invalid,
+                                   int flags);
+/* verified[i] = verify_double((pk_uv, pkp_uv)[n_public == 1 ? 0 : i]; (u[i], R_uv[i], Rp_uv[i]), msg[i]) */
+int p252_schnorr_verify_double_batch(p252_ctx* ctx, const p252_fr* pk_uv, const p252_fr* pkp_uv, size_t n_public,
+                                     const p252_jscalar* u, const p252_fr* R_uv, const p252_fr* Rp_uv, const p252_fr* msg,
+                                     size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, uint8_t* verified,
+                                     size_t* n_verified, size_t* n_invalid, int flags);
+/* u[i], R_uv[i], Rp_uv[i] = sign_double(note_sk, r[i]; msg[i]),  pkp_uv[i] = [note_sk] Gp,
+ *   note_sk = (hash([a] note_R_uv[i]) + b) mod r_J,  (a, b) = (a, b)[n_secret == 1 ? 0 : i] */
+int p252_note_sign_double_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
+                                const p252_fr* note_R_uv, const p252_jscalar* r, const p252_fr* msg, size_t n,
+                                const p252_fr* G_uv, const p252_fr* Gp_uv, p252_jscalar* u, p252_fr* R_uv, p252_fr* Rp_uv,
+                                p252_fr* pkp_uv, uint8_t* ok, size_t* n_invalid, int flags);
+
 /* ---- JubJub point compression (dusk-jubjub's JubJubAffine::to_bytes / from_bytes) -----------------------------------
  *   encoding:  the 32 little-endian bytes of canonical v, with bit 255 (bytes[31] >> 7) = the low bit of canonical u
  *   decoding:  sign = bit 255, cleared; the remaining 255-bit value is v (rejected if >= p); u^2 = (v^2 - 1) / (1 + d v^2)

@@ -11,8 +11,9 @@
 //   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
 //   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
 //   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
-//   schnorr_verify_batch, nullifier / nullifier_batch, point_from_bytes / points_from_bytes_batch, point_to_bytes /
-//   points_to_bytes_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
+//   schnorr_verify_batch, nullifier / nullifier_batch, schnorr_sign_double / schnorr_sign_double_batch,
+//   schnorr_verify_double / schnorr_verify_double_batch, note_sign_double_batch, point_from_bytes /
+//   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -466,6 +467,84 @@ inline Scalar nullifier(const JubJubScalar& a, const JubJubScalar& b, const Scal
     const auto r = nullifier_batch(&a, &b, 1, base_uv, R_uv, &pos, 1, ok, nullptr, e);
     if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
     return r[0];
+}
+
+// NEW: double-key Schnorr signatures over G and G' (p252_schnorr_sign_double_batch / p252_schnorr_verify_double_batch),
+// jubjub-schnorr's SecretKey::sign_double / SignatureDouble::verify: R = [r] G, R' = [r] G', u = (r - c sk) mod r_J with
+// c = challenge2(R, R', m) = Hash::digest_truncated(Domain::Other, [R.u, R.v, R'.u, R'.v, m])[0]; verified iff
+// [u] G + [c] PK == R and [u] G' + [c] PK' == R'.  G_uv and Gp_uv are the caller's G and G' (no built-in generator);
+// either off the curve throws Error(P252_ERR_INVALID_POINT).  r is one fresh secret nonce per message (never reused).
+// sk holds 1 or n keys (n_secret); returns the n scalars u; R and Rp receive n x 2 scalars each; ok[i] == 0 marks an
+// invalid item, whose rows are zeroed
+inline std::vector<JubJubScalar> schnorr_sign_double_batch(const JubJubScalar* sk, size_t n_secret, const JubJubScalar* r,
+                                                           const Scalar* msg, size_t n, const Scalar (&G_uv)[2],
+                                                           const Scalar (&Gp_uv)[2], std::vector<Scalar>& R,
+                                                           std::vector<Scalar>& Rp, std::vector<uint8_t>& ok,
+                                                           Engine& e = Engine::default_engine()) {
+    std::vector<JubJubScalar> u(n);
+    R.assign(2 * n, Scalar{});
+    Rp.assign(2 * n, Scalar{});
+    ok.assign(n, 0);
+    check(p252_schnorr_sign_double_batch(e.get(), sk, n_secret, r, msg, n, G_uv, Gp_uv, u.data(), R.data(), Rp.data(),
+                                         ok.data(), nullptr, P252_MEM_HOST),
+          e.get());
+    return u;
+}
+// one double-key signature (u, R, R'); throws Error(P252_ERR_INVALID_POINT) for sk or r >= r_J or msg >= p
+inline void schnorr_sign_double(const JubJubScalar& sk, const JubJubScalar& r, const Scalar& msg, const Scalar (&G_uv)[2],
+                                const Scalar (&Gp_uv)[2], JubJubScalar& u, Scalar (&R_uv)[2], Scalar (&Rp_uv)[2],
+                                Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> R, Rp;
+    std::vector<uint8_t> ok;
+    const auto us = schnorr_sign_double_batch(&sk, 1, &r, &msg, 1, G_uv, Gp_uv, R, Rp, ok, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    u = us[0];
+    R_uv[0] = R[0], R_uv[1] = R[1], Rp_uv[0] = Rp[0], Rp_uv[1] = Rp[1];
+}
+// pk and pkp hold 1 or n points each (n_public), R and Rp n x 2 scalars; returns verified[i] (0 also for an invalid
+// item); n_verified / n_invalid may be null
+inline std::vector<uint8_t> schnorr_verify_double_batch(const Scalar* pk, const Scalar* pkp, size_t n_public,
+                                                        const JubJubScalar* u, const Scalar* R, const Scalar* Rp,
+                                                        const Scalar* msg, size_t n, const Scalar (&G_uv)[2],
+                                                        const Scalar (&Gp_uv)[2], size_t* n_verified = nullptr,
+                                                        size_t* n_invalid = nullptr, Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> verified(n, 0);
+    check(p252_schnorr_verify_double_batch(e.get(), pk, pkp, n_public, u, R, Rp, msg, n, G_uv, Gp_uv, verified.data(),
+                                           n_verified, n_invalid, P252_MEM_HOST),
+          e.get());
+    return verified;
+}
+// SignatureDouble::verify for one signature; throws Error(P252_ERR_INVALID_POINT) for u >= r_J, msg >= p, a coordinate
+// of R or R' >= p or a key off the curve
+inline bool schnorr_verify_double(const Scalar (&pk_uv)[2], const Scalar (&pkp_uv)[2], const JubJubScalar& u,
+                                  const Scalar (&R_uv)[2], const Scalar (&Rp_uv)[2], const Scalar& msg,
+                                  const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2], Engine& e = Engine::default_engine()) {
+    size_t invalid = 0;
+    const auto verified = schnorr_verify_double_batch(pk_uv, pkp_uv, 1, &u, R_uv, Rp_uv, &msg, 1, G_uv, Gp_uv, nullptr,
+                                                      &invalid, e);
+    if (invalid) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    return verified[0] != 0;
+}
+// NEW: spending notes (p252_note_sign_double_batch): the double-key signature of msg[i] under the note secret key
+// note_sk = (hash([a] note_R[i]) + b) mod r_J, whose key pair is (note_pk, pk') = ([note_sk] G, [note_sk] G').  a and b
+// hold 1 or n keys each (n_secret); note_R holds n x 2 scalars.  Returns the n scalars u; R, Rp and pkp (pk', the spend
+// proof's witness: it links the spend to the note, keep it private) receive n x 2 scalars each; ok[i] == 0 marks an
+// invalid item (a, b or r >= r_J, note_R off the curve, msg >= p), whose rows are zeroed.  n_invalid may be null.
+inline std::vector<JubJubScalar> note_sign_double_batch(const JubJubScalar* a, const JubJubScalar* b, size_t n_secret,
+                                                        const Scalar* note_R, const JubJubScalar* r, const Scalar* msg,
+                                                        size_t n, const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2],
+                                                        std::vector<Scalar>& R, std::vector<Scalar>& Rp,
+                                                        std::vector<Scalar>& pkp, std::vector<uint8_t>& ok,
+                                                        size_t* n_invalid = nullptr, Engine& e = Engine::default_engine()) {
+    std::vector<JubJubScalar> u(n);
+    R.assign(2 * n, Scalar{});
+    Rp.assign(2 * n, Scalar{});
+    pkp.assign(2 * n, Scalar{});
+    ok.assign(n, 0);
+    check(p252_note_sign_double_batch(e.get(), a, b, n_secret, note_R, r, msg, n, G_uv, Gp_uv, u.data(), R.data(), Rp.data(),
+                                      pkp.data(), ok.data(), n_invalid, P252_MEM_HOST),
+          e.get());
+    return u;
 }
 
 // NEW: JubJub point compression (p252_points_from_bytes / p252_points_to_bytes), dusk-jubjub's JubJubAffine::from_bytes /

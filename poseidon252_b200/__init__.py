@@ -12,7 +12,9 @@ plus the batch entry points this engine adds:
     schnorr_sign_batch and schnorr_verify / schnorr_verify_batch (Schnorr signatures over JubJub), point_from_bytes /
     points_from_bytes_batch and point_to_bytes / points_to_bytes_batch (JubJub point compression), jubjub_msm
     (multi-scalar multiplication) and schnorr_verify_all (all-or-nothing batch verification), nullifier /
-    nullifier_batch (Phoenix note nullifiers: which owned notes are spent), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
+    nullifier_batch (Phoenix note nullifiers: which owned notes are spent), schnorr_sign_double /
+    schnorr_sign_double_batch, schnorr_verify_double / schnorr_verify_double_batch and note_sign_double_batch (double-key
+    Schnorr signatures over G and G', and spending a note under its note secret key), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
     with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
@@ -30,6 +32,8 @@ from .msm import jubjub_msm, schnorr_verify_all
 from .nullifier import nullifier, nullifier_batch
 from .points import point_from_bytes, point_to_bytes, points_from_bytes_batch, points_to_bytes_batch
 from .schnorr import schnorr_sign, schnorr_sign_batch, schnorr_verify, schnorr_verify_batch
+from .schnorr_double import (note_sign_double_batch, schnorr_sign_double, schnorr_sign_double_batch,
+                             schnorr_verify_double, schnorr_verify_double_batch)
 
 HADES_WIDTH = hades.WIDTH
 
@@ -40,6 +44,8 @@ __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encr
            "schnorr_sign", "schnorr_sign_batch", "schnorr_verify", "schnorr_verify_batch",
            "point_from_bytes", "point_to_bytes", "points_from_bytes_batch", "points_to_bytes_batch",
            "jubjub_msm", "schnorr_verify_all", "nullifier", "nullifier_batch",
+           "schnorr_sign_double", "schnorr_sign_double_batch", "schnorr_verify_double", "schnorr_verify_double_batch",
+           "note_sign_double_batch",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",

@@ -14,6 +14,8 @@
 //   jubjub-schnorr sign / verify (consumer, not the reference) -> p252_schnorr_sign_batch, p252_schnorr_verify_batch
 //   JubJubAffine::from_bytes / to_bytes (dusk-jubjub, not the reference) -> p252_points_from_bytes, p252_points_to_bytes
 //   Phoenix note nullifiers (consumer, not the reference) -> p252_nullifier_batch
+//   jubjub-schnorr SignatureDouble, Phoenix note signing (consumer, not the reference) -> p252_schnorr_sign_double_batch,
+//     p252_schnorr_verify_double_batch, p252_note_sign_double_batch
 //   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -99,6 +101,9 @@ struct p252_ctx {
     // instances, so that alternating digest and encryption calls rebuild neither
     TagTable vt, ct;
     BaseTable bt;   // fixed-base JubJub table
+    // the tables of G and G' of the double-key signature calls, only theirs: a wallet that alternates single-base calls with
+    // spend signing keeps all three
+    BaseTable bt2[2];
     // test hook: index of the staged chunk that fails in the next host-buffer call (-1 = none)
     long long fail_chunk = -1;
     // multi-GPU
@@ -626,7 +631,8 @@ void p252_destroy(p252_ctx* ctx) {
             if (ev) cudaEventDestroy(ev);
     for (TagTable* t : {&ctx->vt, &ctx->ct})
         if (t->dev) cudaFreeAsync(t->dev, ctx->stream);
-    if (ctx->bt.dev) cudaFreeAsync(ctx->bt.dev, ctx->stream);
+    for (BaseTable* t : {&ctx->bt, &ctx->bt2[0], &ctx->bt2[1]})
+        if (t->dev) cudaFreeAsync(t->dev, ctx->stream);
     if (ctx->stream) cudaStreamSynchronize(ctx->stream);   // pending host functions reference h_counter
     for (TagTable* t : {&ctx->vt, &ctx->ct}) {
         if (t->host) cudaFreeHost(t->host);
@@ -965,12 +971,11 @@ static int base_check(const p252_fr* base_uv) {
     return p252::host::jubjub_on_curve(base_uv[0].l, base_uv[1].l) ? P252_OK : P252_ERR_INVALID_POINT;
 }
 
-// The device table of base_uv: the cached one when the base is the same 64 bytes, otherwise built on the context stream
-// (k_fixed_base_table) into a new stream-ordered allocation.  The replaced table is freed in stream order, after every
-// kernel already enqueued that reads it (DEVICE calls run on the context stream, HOST and fused calls join back into it),
-// so P252_ASYNC calls with different bases may follow each other.
-static int base_table(p252_ctx* ctx, const p252_fr* base_uv, const void** table) {
-    BaseTable& t = ctx->bt;
+// The device table of base_uv in the cache slot t (ctx->bt, or one of ctx->bt2): the cached one when the base is the same
+// 64 bytes, otherwise built on the context stream (k_fixed_base_table) into a new stream-ordered allocation.  The replaced
+// table is freed in stream order, after every kernel already enqueued that reads it (DEVICE calls run on the context
+// stream, HOST and fused calls join back into it), so P252_ASYNC calls with different bases may follow each other.
+static int base_table(p252_ctx* ctx, BaseTable& t, const p252_fr* base_uv, const void** table) {
     if (t.dev && memcmp(t.key, base_uv, sizeof t.key) == 0) {
         *table = t.dev;
         return P252_OK;
@@ -1002,7 +1007,7 @@ int p252_fixed_base_batch(p252_ctx* ctx, const p252_fr* base_uv, const p252_jsca
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
     std::vector<Io> ios = {{secret, nullptr, 32}, {nullptr, out_uv, 64}, {nullptr, ok, 1}};
     return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
         return launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[1], static_cast<uint8_t*>(d[2]), counts.counter(0), st));
@@ -1028,7 +1033,7 @@ int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, si
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 message, 1 r, 2 public, 3 nonce, 4 cipher, 5 R, 6 ok; 7 shared secrets and 8 validity live in the arena only
     std::vector<Io> ios = {{msg, nullptr, L * 32, false, dev}, {r, nullptr, 32, false, dev}, {public_uv, nullptr, 64, pb, dev},
                            {nonce, nullptr, 32, false, dev}, {nullptr, cipher, (size_t)(l32 + 1) * 32, false, dev},
@@ -1070,7 +1075,7 @@ int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, c
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 r, 1 A, 2 B, 3 R, 4 note_pk, 5 ok; 6 shared points, 7 validity and 8 h live in the arena only
     std::vector<Io> ios = {{r, nullptr, 32, false, dev}, {A_uv, nullptr, 64, pb, dev}, {B_uv, nullptr, 64, pb, dev},
                            {nullptr, R_uv, 64, false, dev}, {nullptr, note_pk_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
@@ -1109,7 +1114,7 @@ int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p25
     uint64_t nb[12];
     p252::host::jubjub_niels(nb, spend_B_uv[0].l, spend_B_uv[1].l);
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 view_a, 1 R, 2 note_pk, 3 owned; 4 shared points, 5 validity and 6 h live in the arena only
     std::vector<Io> ios = {{view_a, nullptr, 32, true, dev}, {R_uv, nullptr, 64, false, dev}, {note_pk_uv, nullptr, 64, false, dev},
                            {nullptr, owned, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
@@ -1147,7 +1152,7 @@ int p252_schnorr_sign_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secr
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 sk, 1 r, 2 msg, 3 u, 4 R, 5 ok; 6 the digest rows and 7 c live in the arena only
     std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev},
                            {nullptr, u_out, 32, false, dev}, {nullptr, R_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
@@ -1180,7 +1185,7 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
     const Counts counts = Counts::device(ctx, flags, n_verified, n_invalid);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 PK, 1 u, 2 R, 3 msg, 4 verified; 5 the digest rows, 6 validity and 7 c live in the arena only
     std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev}, {R_uv, nullptr, 64, false, dev},
                            {msg, nullptr, 32, false, dev}, {nullptr, verified, 1, false, dev}, {nullptr, nullptr, 96},
@@ -1218,7 +1223,7 @@ int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscala
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
     // 0 a, 1 b, 2 R, 3 pos, 4 nullifier, 5 ok; 6 shared points, 7 validity, 8 h and 9 the digest rows live in the arena only
     std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev},
                            {pos, nullptr, 8, false, dev}, {nullptr, nullifier, 32, false, dev}, {nullptr, ok, 1, false, dev},
@@ -1234,6 +1239,138 @@ int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscala
         if (e == P252_OK)
             e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[4], 1, static_cast<uint8_t*>(d[5]), counts.counter(0),
                                                     st));
+        return e;
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+// ---- double-key Schnorr signatures over G and G' (jubjub-schnorr SignatureDouble) and note signing ----------------------
+// challenge2(R, R', m) = Hash::digest_truncated(Domain::Other, [R.u, R.v, R'.u, R'.v, m])[0].  Sign: R = [r] G, R' = [r] G',
+// u = (r - c sk) mod r_J; verify: [u] G + [c] PK == R and [u] G' + [c] PK' == R'.  The note signer's key is
+// note_sk = (hash([a] R_note) + b) mod r_J, and it also returns pk' = [note_sk] G'.  Per chunk: launch_fixed_base twice on
+// the same r (R with the table of G, R' with the table of G'; both write the same ok), launch_schnorr_pack_double writes
+// the rows [R.u, R.v, R'.u, R'.v, m] into a slot arena, the truncated launch_digest of them gives c into the arena, then
+// launch_schnorr_sign_double / launch_note_sign_double / launch_schnorr_verify_double.  The note signer first runs
+// launch_dhke and the truncated launch_digest of the shared points (h, the stealth calls' hash) into the arena, as the
+// nullifier call does.  The secrets (sk, r, a, b, [a] R_note, h, note_sk) live only in the slot arenas for both memory
+// spaces, so both signing calls are synchronous and the common exit join_slots(wipe) clears them on every path;
+// verification reads public data only.  The tables of G and G' come from the context's two-slot cache ctx->bt2.
+static int schnorr_double_tag(p252_fr* tag) { return p252_hash_tag(P252_DOMAIN_OTHER, 5, 1, tag); }
+
+static int double_tables(p252_ctx* ctx, const p252_fr* G_uv, const p252_fr* Gp_uv, const void** table, const void** table_p) {
+    const int rc = base_table(ctx, ctx->bt2[0], G_uv, table);
+    return rc != P252_OK ? rc : base_table(ctx, ctx->bt2[1], Gp_uv, table_p);
+}
+
+int p252_schnorr_sign_double_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_jscalar* r,
+                                   const p252_fr* msg, size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, p252_jscalar* u_out,
+                                   p252_fr* R_uv, p252_fr* Rp_uv, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !one_or_n(n_secret, n) || !args_ok(n, flags, {sk, r, msg, u_out, R_uv, Rp_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 sk, 1 r, 2 msg, 3 u, 4 R, 5 R', 6 ok; 7 the digest rows and 8 c live in the arena only
+    std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev},
+                           {nullptr, u_out, 32, false, dev}, {nullptr, R_uv, 64, false, dev}, {nullptr, Rp_uv, 64, false, dev},
+                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 160}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[6]);
+        int e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table, d[4], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table_p, d[5], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_schnorr_pack_double(d[4], d[5], d[2], cnt, d[7], okc, true, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[7], cnt, 5, d[8], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_schnorr_sign_double(d[0], sb, d[1], d[8], cnt, d[3], d[4], d[5], okc,
+                                                               counts.counter(0), st));
+        return e;
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+// As p252_schnorr_verify_batch, both counts come from the device counters (0: verified, 1: invalid) for both memory
+// spaces, and nothing here is secret: no wipe.
+int p252_schnorr_verify_double_batch(p252_ctx* ctx, const p252_fr* pk_uv, const p252_fr* pkp_uv, size_t n_public,
+                                     const p252_jscalar* u, const p252_fr* R_uv, const p252_fr* Rp_uv, const p252_fr* msg,
+                                     size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, uint8_t* verified, size_t* n_verified,
+                                     size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !one_or_n(n_public, n) ||
+        !args_ok(n, flags, {pk_uv, pkp_uv, u, R_uv, Rp_uv, msg}, {verified}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const Counts counts = Counts::device(ctx, flags, n_verified, n_invalid);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 PK, 1 PK', 2 u, 3 R, 4 R', 5 msg, 6 verified; 7 the digest rows, 8 validity and 9 c live in the arena only
+    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {pkp_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev},
+                           {R_uv, nullptr, 64, false, dev}, {Rp_uv, nullptr, 64, false, dev}, {msg, nullptr, 32, false, dev},
+                           {nullptr, verified, 1, false, dev}, {nullptr, nullptr, 160}, {nullptr, nullptr, 1},
+                           {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* valid = static_cast<uint8_t*>(d[8]);
+        int e = launched(ctx, p252::launch_schnorr_pack_double(d[3], d[4], d[5], cnt, d[7], valid, false, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[7], cnt, 5, d[9], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_schnorr_verify_double(d[0], d[1], pb, d[2], d[3], d[4], d[9], valid, cnt, table,
+                                                                 table_p, static_cast<uint8_t*>(d[6]), counts.counter(0),
+                                                                 counts.counter(1), st));
+        return e;
+    });
+    return counts.end(rc);
+}
+
+int p252_note_sign_double_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
+                                const p252_fr* note_R_uv, const p252_jscalar* r, const p252_fr* msg, size_t n,
+                                const p252_fr* G_uv, const p252_fr* Gp_uv, p252_jscalar* u_out, p252_fr* R_uv, p252_fr* Rp_uv,
+                                p252_fr* pkp_uv, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !one_or_n(n_secret, n) ||
+        !args_ok(n, flags, {a, b, note_R_uv, r, msg, u_out, R_uv, Rp_uv, pkp_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag_h, tag;
+    if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 a, 1 b, 2 R_note, 3 r, 4 msg, 5 u, 6 R, 7 R', 8 pk', 9 ok; 10 shared points, 11 their validity, 12 h, 13 the digest
+    // rows and 14 c live in the arena only
+    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {note_R_uv, nullptr, 64, false, dev},
+                           {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev}, {nullptr, u_out, 32, false, dev},
+                           {nullptr, R_uv, 64, false, dev}, {nullptr, Rp_uv, 64, false, dev}, {nullptr, pkp_uv, 64, false, dev},
+                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32},
+                           {nullptr, nullptr, 160}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[9]);
+        uint8_t* valid = static_cast<uint8_t*>(d[11]);
+        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[2], false, cnt, d[10], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[10], cnt, 2, d[12], 1, true, ctx->coop_max, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_fixed_base(d[3], cnt, table, d[6], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_fixed_base(d[3], cnt, table_p, d[7], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_schnorr_pack_double(d[6], d[7], d[4], cnt, d[13], okc, true, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[13], cnt, 5, d[14], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_note_sign_double(d[1], sb, d[12], valid, d[3], d[14], cnt, table_p, d[5], d[6], d[7],
+                                                            d[8], okc, counts.counter(0), st));
         return e;
     }, /*wipe=*/true);
     return counts.end(rc);
@@ -1408,7 +1545,7 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
         return P252_OK;
     }
     const void* table = nullptr;
-    if ((rc = base_table(ctx, base_uv, &table)) != P252_OK) return rc;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
     const size_t per = pb ? 1 : 2;   // MSM rows per item
     // 0 PK, 1 u, 2 R, 3 msg, 4 weight; 5 the digest rows, 6 validity, 7 c, 8 row scalars, 9 row points and 10 the chunk's
     // MSM temporaries live in the arena only

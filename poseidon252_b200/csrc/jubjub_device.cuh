@@ -467,6 +467,20 @@ static_assert(kProductsPerSchnorrVerify == 2850, "product count of DESIGN.md sec
 constexpr int kProductsPerNullifierKey = kProductsPerFixedBase + 1;
 static_assert(kProductsPerNullifierKey == 867, "product count of DESIGN.md section 4");
 
+// ---- double-key Schnorr signatures (p252_schnorr_{sign,verify}_double_batch, p252_note_sign_double_batch) ---------------
+// c = challenge2(R, R', m) < 2^250 comes from the truncated digest of [R.u, R.v, R'.u, R'.v, m].
+//   sign:      R = [r] G and R' = [r] G' are two fixed-base walks (k_fixed_base twice), u = (r - c sk) mod r_J the two
+//              order products of the single-key signer.
+//   note sign: in addition [a] R_note (k_dhke) for h, note_sk = (h + b) mod r_J (order_add, no product) and
+//              pk' = [note_sk] G' (fixed_base_mul).
+//   verify:    the single-key check twice, [c] PK + [u] G == R and [c] PK' + [u] G' == R'.
+constexpr int kProductsPerSchnorrSignDouble = 2 * kProductsPerFixedBase;   // + kOrderProductsPerSchnorrSign modulo r_J
+constexpr int kProductsPerNoteSignDouble = kProductsPerSchnorrSignDouble + kProductsPerDhke + kProductsPerFixedBase;
+constexpr int kProductsPerSchnorrVerifyDouble = 2 * kProductsPerSchnorrVerify;
+static_assert(kProductsPerSchnorrSignDouble == 1732, "product count of DESIGN.md section 4");
+static_assert(kProductsPerNoteSignDouble == 5417, "product count of DESIGN.md section 4");
+static_assert(kProductsPerSchnorrVerifyDouble == 5700, "product count of DESIGN.md section 4");
+
 // Arithmetic modulo r_J on 8 x 32-bit little-endian words, Montgomery form with R = 2^256.  Constants (immediates, as
 // P252_JJ_ORDER): R^2 mod r_J and kOrderInv = -r_J^-1 mod 2^32.  Constant time: no branch and no address depends on an
 // operand; each final correction is a masked subtraction or addition of r_J.

@@ -11,6 +11,8 @@
 //   stealth addresses (note_pk = [hash(shared)] G + B) -> k_stealth
 //   Schnorr signatures (u = r - c sk, [u] G + [c] PK == R) -> k_schnorr_pack, k_schnorr_sign, k_schnorr_verify
 //   note nullifiers (pk' = [(h + b) mod r_J] G', the digest rows [pk'.u, pk'.v, pos]) -> k_nullifier_key
+//   double-key Schnorr signatures over G and G' (SignatureDouble, note signing) -> k_schnorr_pack_double,
+//     k_schnorr_sign_double<Note>, k_schnorr_verify_double
 //   JubJubAffine::from_bytes / to_bytes (point compression) -> k_points_from_bytes, k_points_to_bytes
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
@@ -1786,22 +1788,15 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_sign(const uint8_t* __r
     if (n_invalid) warp_count_every(n_invalid, !good);
 }
 
-// Verify, one thread per item, after k_schnorr_pack (valid[i]: R and m canonical) and the truncated digest (c[i]):
-// verified[i] = valid[i], u < r_J, PK = pk[pb ? 0 : i] a curve point with u, v < p, and [c] PK + [u] G == R, compared
-// projectively (kProductsPerSchnorrVerify products).  Every operand is public, so the variable-base walk of [c] PK reads
-// one table entry per window at the digit's address (jj::scalar_mul_ext<true, ...>); k_dhke keeps the masked reads.
-// PK, then u, then R are loaded, each just before its use, so that across each walk little else is live.  An invalid
-// item runs the same code on the identity and zero.  cnt_ok += verified items, cnt_bad += invalid ones.
-__global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify(const uint8_t* __restrict__ pk, bool pb, const uint8_t* __restrict__ u,
-                                                             const uint8_t* __restrict__ R_uv, const uint8_t* __restrict__ c,
-                                                             const uint8_t* __restrict__ valid, size_t n,
-                                                             const uint4* __restrict__ table, uint8_t* __restrict__ verified,
-                                                             unsigned long long* __restrict__ cnt_ok,
-                                                             unsigned long long* __restrict__ cnt_bad) {
-    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
-    if (i >= n) return;
+// The single-key check [c] PK + [u] G == R of item i (PK = pk[pb ? 0 : i]), compared projectively
+// (kProductsPerSchnorrVerify products), with public operands only: the variable-base walk of [c] PK reads one table entry per window at the digit's address
+// (jj::scalar_mul_ext<true, ...>); k_dhke keeps the masked reads.  PK, then u, then R are loaded, each just before its
+// use, so that across each walk little else is live.  good &= PK a curve point with u, v < p and u < r_J; an invalid
+// operand is replaced by the identity or zero, so every item runs the same code.  Returns good and the equation.
+__device__ __forceinline__ bool schnorr_check(const uint8_t* __restrict__ pk, bool pb, const uint8_t* __restrict__ u,
+                                              const uint8_t* __restrict__ R_uv, const uint8_t* __restrict__ c, size_t i,
+                                              const uint4* __restrict__ table, bool& good) {
     jj::Ext acc;
-    bool good = valid[i] != 0;
     {
         uint32_t x[8], y[8], one[8], e[8];
         load_fr(x, pk + (pb ? 0 : i) * 64);
@@ -1838,7 +1833,22 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify(const uint8_t* _
     for (int k = 0; k < 8; ++k) ru[k] &= m, rv[k] &= m;
     jj::fmul(x, ru, t.Z);
     jj::fmul(y, rv, t.Z);
-    const bool ok = good & jj::feq(x, t.X) & jj::feq(y, t.Y);
+    return good & jj::feq(x, t.X) & jj::feq(y, t.Y);
+}
+
+// Verify, one thread per item, after k_schnorr_pack (valid[i]: R and m canonical) and the truncated digest (c[i]):
+// verified[i] = valid[i], u < r_J, PK = pk[pb ? 0 : i] a curve point with u, v < p, and [c] PK + [u] G == R
+// (schnorr_check).  cnt_ok += verified items, cnt_bad += invalid ones.
+__global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify(const uint8_t* __restrict__ pk, bool pb, const uint8_t* __restrict__ u,
+                                                             const uint8_t* __restrict__ R_uv, const uint8_t* __restrict__ c,
+                                                             const uint8_t* __restrict__ valid, size_t n,
+                                                             const uint4* __restrict__ table, uint8_t* __restrict__ verified,
+                                                             unsigned long long* __restrict__ cnt_ok,
+                                                             unsigned long long* __restrict__ cnt_bad) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    bool good = valid[i] != 0;
+    const bool ok = schnorr_check(pk, pb, u, R_uv, c, i, table, good);
     verified[i] = ok ? 1 : 0;
     if (cnt_ok) warp_count_every(cnt_ok, ok);
     if (cnt_bad) warp_count_every(cnt_bad, !good);
@@ -1868,6 +1878,169 @@ cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, 
     k_schnorr_verify<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u),
                                                        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(c), valid,
                                                        n, static_cast<const uint4*>(table), verified, n_verified, n_invalid);
+    return cudaGetLastError();
+}
+
+// ---- double-key Schnorr signatures over G and G': c = challenge2(R, R', m) (jubjub_device.cuh) -------------------------
+// The digest's input rows [R.u, R.v, R'.u, R'.v, m] (160 bytes): a value >= p is written as 0, and flag[i] =
+// (and_flag ? flag[i] : 1) and all five values < p.  Sign: flag is ok (r < r_J from k_fixed_base), R and R' as k_fixed_base
+// wrote them; verify: flag is the item's validity, R and R' the caller's.  Public data only.
+__global__ void __launch_bounds__(256) k_schnorr_pack_double(const uint8_t* R_uv, const uint8_t* Rp_uv,
+                                                             const uint8_t* __restrict__ msg, size_t n,
+                                                             uint8_t* __restrict__ rows, uint8_t* flag, bool and_flag) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint32_t x[5][8];
+    load_fr_rw(x[0], R_uv + i * 64);
+    load_fr_rw(x[1], R_uv + i * 64 + 32);
+    load_fr_rw(x[2], Rp_uv + i * 64);
+    load_fr_rw(x[3], Rp_uv + i * 64 + 32);
+    load_fr(x[4], msg + i * 32);
+    bool good = !and_flag || flag[i] != 0;
+#pragma unroll
+    for (int q = 0; q < 5; ++q) {
+        const bool canon = fr_is_canonical(x[q]);
+        const uint32_t m = 0u - (uint32_t)canon;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) x[q][k] &= m;
+        good &= canon;
+        store_fr(rows + i * 160 + q * 32, x[q]);
+    }
+    flag[i] = good ? 1 : 0;
+}
+
+// Sign, one thread per item, after k_fixed_base twice (R and R' rows, ok = r < r_J), k_schnorr_pack_double (ok &= m < p)
+// and the truncated digest (c[i] < 2^250).  Plain: sk = key[kb ? 0 : i], ok[i] &= sk < r_J.  Note: key is b, h[i] the
+// truncated digest of [a] R_note and valid[i] its validity from k_dhke; sk = (h + b) mod r_J with an out-of-range b entering
+// as 0, ok[i] &= valid[i] and b < r_J, and pk'[i] = [sk] G' (table: the fixed-base table of G', kProductsPerFixedBase
+// products).  u[i] = (r - c sk) mod r_J (kOrderProductsPerSchnorrSign products modulo r_J).  An item with ok = 0 runs the
+// same code on r = sk = 0 and gets zeroed u, R, R' (and pk') rows; *n_invalid += invalid items.  The keys, r and note_sk
+// are secret: every validity is a mask, the table reads are masked selects, and no branch or address depends on them.
+template <bool Note>
+__global__ void __launch_bounds__(kThreads, 3) k_schnorr_sign_double(const uint8_t* __restrict__ key, bool kb,
+                                                                  const uint8_t* __restrict__ h,
+                                                                  const uint8_t* __restrict__ valid,
+                                                                  const uint8_t* __restrict__ r, const uint8_t* __restrict__ c,
+                                                                  size_t n, const uint4* __restrict__ table,
+                                                                  uint8_t* __restrict__ u_out, uint8_t* R_uv, uint8_t* Rp_uv,
+                                                                  uint8_t* __restrict__ pkp_uv, uint8_t* ok,
+                                                                  unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t s[8];
+    load_fr(s, key + (kb ? 0 : i) * 32);
+    bool good = (ok[i] != 0) & jj::below_order(s);
+    if (Note) {
+        good &= valid[i] != 0;
+        uint32_t t[8];
+        const uint32_t mb = 0u - (uint32_t)jj::below_order(s);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) t[q] = s[q] & mb;
+        load_fr(s, h + i * 32);
+        jj::order_add(s, s, t);
+    }
+    const uint32_t m = 0u - (uint32_t)good;
+    uint32_t k[8], e[8];
+    load_fr(k, r + i * 32);
+    load_fr(e, c + i * 32);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) s[q] &= m, k[q] &= m;
+    if (Note) {
+        uint32_t pu[8], pv[8];
+        jj::fixed_base_mul<true>(pu, pv, s, table);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) pu[q] &= m, pv[q] &= m;
+        store_fr(pkp_uv + i * 64, pu);
+        store_fr(pkp_uv + i * 64 + 32, pv);
+    }
+    uint32_t x[8], u[8];
+    jj::order_mul(x, e, s);
+    jj::order_sub(u, k, x);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) u[q] &= m;
+    store_fr(u_out + i * 32, u);
+    uint8_t* const pts[2] = {R_uv + i * 64, Rp_uv + i * 64};
+#pragma unroll
+    for (int w = 0; w < 2; ++w) {
+        uint8_t* P = pts[w];
+        uint32_t pu[8], pv[8];
+        load_fr_rw(pu, P);
+        load_fr_rw(pv, P + 32);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) pu[q] &= m, pv[q] &= m;
+        store_fr(P, pu);
+        store_fr(P + 32, pv);
+    }
+    ok[i] = good ? 1 : 0;
+    if (n_invalid) warp_count_every(n_invalid, !good);
+}
+
+// Verify, one thread per item, after k_schnorr_pack_double (valid[i]: R, R' and m canonical) and the truncated digest
+// (c[i]): verified[i] = valid[i], u < r_J, PK and PK' curve points with coordinates < p, [c] PK + [u] G == R (table) and
+// [c] PK' + [u] G' == R' (table_p): schnorr_check twice, kProductsPerSchnorrVerifyDouble products.  cnt_ok += verified
+// items, cnt_bad += invalid ones (once each, whichever side made them invalid).
+__global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify_double(const uint8_t* __restrict__ pk, const uint8_t* __restrict__ pkp,
+                                                                    bool pb, const uint8_t* __restrict__ u,
+                                                                    const uint8_t* __restrict__ R_uv,
+                                                                    const uint8_t* __restrict__ Rp_uv,
+                                                                    const uint8_t* __restrict__ c,
+                                                                    const uint8_t* __restrict__ valid, size_t n,
+                                                                    const uint4* __restrict__ table,
+                                                                    const uint4* __restrict__ table_p,
+                                                                    uint8_t* __restrict__ verified,
+                                                                    unsigned long long* __restrict__ cnt_ok,
+                                                                    unsigned long long* __restrict__ cnt_bad) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    bool good = valid[i] != 0, ok = true;
+    // one copy of the check's code for both sides: the kernel's SASS stays the size of k_schnorr_verify's
+#pragma unroll 1
+    for (int side = 0; side < 2; ++side)
+        ok &= schnorr_check(side ? pkp : pk, pb, u, side ? Rp_uv : R_uv, c, i, side ? table_p : table, good);
+    verified[i] = ok ? 1 : 0;
+    if (cnt_ok) warp_count_every(cnt_ok, ok);
+    if (cnt_bad) warp_count_every(cnt_bad, !good);
+}
+
+cudaError_t launch_schnorr_pack_double(const void* R_uv, const void* Rp_uv, const void* msg, size_t n, void* rows,
+                                       uint8_t* flag, bool and_flag, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_pack_double<<<blocks256(n), 256, 0, st>>>(static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(Rp_uv),
+                                                        static_cast<const uint8_t*>(msg), n, static_cast<uint8_t*>(rows), flag,
+                                                        and_flag);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_schnorr_sign_double(const void* sk, bool sk_bcast, const void* r, const void* c, size_t n, void* u_out,
+                                       void* R_uv, void* Rp_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_sign_double<false><<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(sk), sk_bcast, nullptr, nullptr, static_cast<const uint8_t*>(r),
+        static_cast<const uint8_t*>(c), n, nullptr, static_cast<uint8_t*>(u_out), static_cast<uint8_t*>(R_uv),
+        static_cast<uint8_t*>(Rp_uv), nullptr, ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_note_sign_double(const void* b, bool b_bcast, const void* h, const uint8_t* valid, const void* r,
+                                    const void* c, size_t n, const void* table_p, void* u_out, void* R_uv, void* Rp_uv,
+                                    void* pkp_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_sign_double<true><<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(b), b_bcast, static_cast<const uint8_t*>(h), valid, static_cast<const uint8_t*>(r),
+        static_cast<const uint8_t*>(c), n, static_cast<const uint4*>(table_p), static_cast<uint8_t*>(u_out),
+        static_cast<uint8_t*>(R_uv), static_cast<uint8_t*>(Rp_uv), static_cast<uint8_t*>(pkp_uv), ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_schnorr_verify_double(const void* pk, const void* pkp, bool pk_bcast, const void* u, const void* R_uv,
+                                         const void* Rp_uv, const void* c, const uint8_t* valid, size_t n, const void* table,
+                                         const void* table_p, uint8_t* verified, unsigned long long* n_verified,
+                                         unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_schnorr_verify_double<<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(pk), static_cast<const uint8_t*>(pkp), pk_bcast, static_cast<const uint8_t*>(u),
+        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(Rp_uv), static_cast<const uint8_t*>(c), valid, n,
+        static_cast<const uint4*>(table), static_cast<const uint4*>(table_p), verified, n_verified, n_invalid);
     return cudaGetLastError();
 }
 

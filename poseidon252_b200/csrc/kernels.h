@@ -172,6 +172,30 @@ cudaError_t launch_schnorr_sign(const void* sk, bool sk_bcast, const void* r, co
 cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c,
                                   const uint8_t* valid, size_t n, const void* table, uint8_t* verified,
                                   unsigned long long* n_verified, unsigned long long* n_invalid, cudaStream_t st);
+// Double-key Schnorr signatures over G and G' (p252_schnorr_{sign,verify}_double_batch, p252_note_sign_double_batch),
+// challenge c = the truncated digest of the row [R.u, R.v, R'.u, R'.v, m] (4 x u64 < 2^250).  Counters are device pointers
+// and may be null.
+// pack: rows[i] = [R.u, R.v, R'.u, R'.v, m] (160 bytes, a value >= p written as 0); flag[i] = (and_flag ? flag[i] : 1) and
+// all five < p
+cudaError_t launch_schnorr_pack_double(const void* R_uv, const void* Rp_uv, const void* msg, size_t n, void* rows,
+                                       uint8_t* flag, bool and_flag, cudaStream_t st);
+// sign: ok[i] &= sk[sk_bcast ? 0 : i] < r_J; u_out[i] = (r[i] - c[i] sk) mod r_J.  An item with ok = 0 gets zeroed u, R_uv
+// and Rp_uv rows and is counted into *n_invalid
+cudaError_t launch_schnorr_sign_double(const void* sk, bool sk_bcast, const void* r, const void* c, size_t n, void* u_out,
+                                       void* R_uv, void* Rp_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st);
+// note sign: as sign with sk = (h[i] + b[b_bcast ? 0 : i]) mod r_J, h[i] the truncated digest of [a] R_note and valid[i]
+// its validity from launch_dhke; ok[i] &= valid[i] and b < r_J; pkp_uv[i] = [sk] G' (table_p: the fixed-base table of G'),
+// zeroed with the other rows of an invalid item
+cudaError_t launch_note_sign_double(const void* b, bool b_bcast, const void* h, const uint8_t* valid, const void* r,
+                                    const void* c, size_t n, const void* table_p, void* u_out, void* R_uv, void* Rp_uv,
+                                    void* pkp_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st);
+// verify: verified[i] = valid[i], u[i] < r_J, pk and pkp[pk_bcast ? 0 : i] curve points with u, v < p, [u[i]] G + [c[i]] pk
+// == R_uv[i] and [u[i]] G' + [c[i]] pkp == Rp_uv[i] (table, table_p: the fixed-base tables of G and G'); *n_verified +=
+// verified items, *n_invalid += invalid ones
+cudaError_t launch_schnorr_verify_double(const void* pk, const void* pkp, bool pk_bcast, const void* u, const void* R_uv,
+                                         const void* Rp_uv, const void* c, const uint8_t* valid, size_t n, const void* table,
+                                         const void* table_p, uint8_t* verified, unsigned long long* n_verified,
+                                         unsigned long long* n_invalid, cudaStream_t st);
 // Point compression (p252_points_from_bytes / p252_points_to_bytes): 32-byte encodings <-> (u, v) Montgomery pairs (64
 // bytes).  from: ok[i] = v < p and u^2 a square, an invalid item gets (0, 0); to: ok[i] = u, v < p and on the curve, an
 // invalid item gets 32 bytes of 0xff.  *n_invalid (a device counter, may be null) += invalid items.

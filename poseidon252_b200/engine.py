@@ -633,6 +633,117 @@ class Engine:
         """Invalid items of the last nullifier_batch (sync() first after async_)."""
         return self._last("nullifier_invalid")
 
+    # -- double-key Schnorr signatures (SignatureDouble) and note signing ------------------------------
+    def schnorr_sign_double_batch(self, sk, r, msg, base, base_p, async_=False):
+        """jubjub-schnorr's SecretKey::sign_double over a batch: R_i = [r_i] base, R'_i = [r_i] base_p,
+        c_i = challenge2(R_i, R'_i, msg_i) = Hash::digest_truncated(Domain::Other, [R.u, R.v, R'.u, R'.v, m])[0] and
+        u_i = (r_i - c_i sk_i) mod r_J.  sk (1 or n, 4) and r (n, 4) p252_jscalar rows (one nonce per message, never
+        reused), msg (n, 4), base (G) and base_p (G') (2, 4), host-read -> (u (n, 4), R (n, 2, 4), R' (n, 2, 4), ok (n,)
+        uint8).  An item with sk or r >= r_J or msg >= p has ok == 0 and zeroed rows (count:
+        last_schnorr_double_invalid()).  A base off the curve raises InvalidPoint."""
+        rp, rl, flags, rk = self._in(r, (4,))
+        if len(rl) != 1:
+            raise EngineError(-1, "r must have shape (n, 4)")
+        n = int(rl[0])
+        sp, sl, fs, skk = self._in(sk, (4,))
+        mp, ml, fm, mk = self._in(msg, (4,))
+        self._same_space(flags, fs, fm)
+        if len(sl) != 1 or int(sl[0]) not in (1, n):
+            raise EngineError(-1, "sk must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(sl)))
+        self._same_lead("msg", ml, n)
+        g, gp = self._base(base), self._base(base_p)
+        u = self._result(None, (n, 4), rk)
+        R = self._result(None, (n, 2, 4), rk)
+        Rp = self._result(None, (n, 2, 4), rk)
+        ok = self._ok_like(rk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("schnorr_double_invalid", flags)
+        self._check(self._lib.p252_schnorr_sign_double_batch(self._ctx, sp, int(sl[0]), rp, mp, n, g.ctypes.data,
+                                                             gp.ctypes.data, self._ptr(u), self._ptr(R), self._ptr(Rp),
+                                                             self._ptr(ok), ctypes.byref(invalid), flags))
+        return u, R, Rp, ok
+
+    def schnorr_verify_double_batch(self, pk, pk_p, u, R, R_p, msg, base, base_p, async_=False):
+        """jubjub-schnorr's SignatureDouble::verify over a batch: verified[i] = [u_i] base + [c_i] PK_i == R_i and
+        [u_i] base_p + [c_i] PK'_i == R'_i with c_i = challenge2(R_i, R'_i, msg_i).  pk and pk_p (1 or n, 2, 4) with the
+        same number of rows, u (n, 4) p252_jscalar rows, R and R_p (n, 2, 4), msg (n, 4), base and base_p (2, 4)
+        (host-read) -> verified (n,) uint8.  An item with u >= r_J, msg >= p, a coordinate of R or R' >= p, or PK or PK'
+        not a curve point is invalid: verified == 0, counted once in last_schnorr_double_invalid(), not in
+        last_schnorr_double_verified().  A base off the curve raises InvalidPoint."""
+        up, ul, flags, uk = self._in(u, (4,))
+        if len(ul) != 1:
+            raise EngineError(-1, "u must have shape (n, 4)")
+        n = int(ul[0])
+        pp, pl, fp, _ = self._in(pk, (2, 4))
+        qp, ql, fq, _ = self._in(pk_p, (2, 4))
+        Rp, Rl, fR, _ = self._in(R, (2, 4))
+        Sp, Sl, fS, _ = self._in(R_p, (2, 4))
+        mp, ml, fm, _ = self._in(msg, (4,))
+        self._same_space(flags, fp, fq, fR, fS, fm)
+        if len(pl) != 1 or int(pl[0]) not in (1, n):
+            raise EngineError(-1, "pk must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(pl)))
+        if tuple(ql) != tuple(pl):
+            raise EngineError(-1, "pk_p must have %d rows like pk, got leading shape %s" % (int(pl[0]), tuple(ql)))
+        self._same_lead("R", Rl, n)
+        self._same_lead("R_p", Sl, n)
+        self._same_lead("msg", ml, n)
+        g, gp = self._base(base), self._base(base_p)
+        verified = self._result(None, (n,), uk, itemsize=1)
+        flags = self._flags(flags, async_)
+        n_verified = self._counter("schnorr_double_verified", flags)
+        invalid = self._counter("schnorr_double_invalid", flags)
+        self._check(self._lib.p252_schnorr_verify_double_batch(self._ctx, pp, qp, int(pl[0]), up, Rp, Sp, mp, n,
+                                                               g.ctypes.data, gp.ctypes.data, self._ptr(verified),
+                                                               ctypes.byref(n_verified), ctypes.byref(invalid), flags))
+        return verified
+
+    def note_sign_double_batch(self, a, b, note_R, r, msg, base, base_p, async_=False):
+        """Spend signatures of Phoenix notes: sign_double (as schnorr_sign_double_batch) under each note's secret key
+        note_sk = (hash([a] note_R_i) + b) mod r_J, hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0].
+        a and b (1 or n, 4) p252_jscalar rows with the same number of rows (the wallet's secret key), note_R (n, 2, 4)
+        the notes' ephemeral keys, r (n, 4), msg (n, 4), base (G) and base_p (G') (2, 4), host-read -> (u (n, 4),
+        R (n, 2, 4), R' (n, 2, 4), pk' (n, 2, 4), ok (n,) uint8) with pk' = [note_sk] base_p, the spend proof's witness:
+        it links the spend to the note and must stay private.  An item with a, b or r >= r_J, note_R not a curve point
+        or msg >= p has ok == 0 and zeroed rows (count: last_schnorr_double_invalid()).  note_sk never leaves the
+        device."""
+        rp, rl, flags, rk = self._in(r, (4,))
+        if len(rl) != 1:
+            raise EngineError(-1, "r must have shape (n, 4)")
+        n = int(rl[0])
+        ap, al, fa, _ = self._in(a, (4,))
+        bp, bl, fb, _ = self._in(b, (4,))
+        np_, nl, fn, _ = self._in(note_R, (2, 4))
+        mp, ml, fm, _ = self._in(msg, (4,))
+        self._same_space(flags, fa, fb, fn, fm)
+        if len(al) != 1 or int(al[0]) not in (1, n):
+            raise EngineError(-1, "a must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(al)))
+        ns = int(al[0])
+        if tuple(bl) != (ns,):
+            raise EngineError(-1, "b must have %d rows like a, got leading shape %s" % (ns, tuple(bl)))
+        self._same_lead("note_R", nl, n)
+        self._same_lead("msg", ml, n)
+        g, gp = self._base(base), self._base(base_p)
+        u = self._result(None, (n, 4), rk)
+        R = self._result(None, (n, 2, 4), rk)
+        Rp = self._result(None, (n, 2, 4), rk)
+        pkp = self._result(None, (n, 2, 4), rk)
+        ok = self._ok_like(rk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("schnorr_double_invalid", flags)
+        self._check(self._lib.p252_note_sign_double_batch(self._ctx, ap, bp, ns, np_, rp, mp, n, g.ctypes.data,
+                                                          gp.ctypes.data, self._ptr(u), self._ptr(R), self._ptr(Rp),
+                                                          self._ptr(pkp), self._ptr(ok), ctypes.byref(invalid), flags))
+        return u, R, Rp, pkp, ok
+
+    def last_schnorr_double_verified(self):
+        """Verified signatures of the last schnorr_verify_double_batch (sync() first after async_)."""
+        return self._last("schnorr_double_verified")
+
+    def last_schnorr_double_invalid(self):
+        """Invalid items of the last schnorr_sign_double_batch, schnorr_verify_double_batch or note_sign_double_batch
+        (sync() first after async_)."""
+        return self._last("schnorr_double_invalid")
+
     # -- point compression ------------------------------------------------------------------------
     def points_from_bytes(self, data, out=None, async_=False):
         """JubJubAffine::from_bytes over a batch: (n, 32) uint8 encodings (host) or (n, 4) 64-bit device tensor of the
