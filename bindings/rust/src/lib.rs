@@ -147,6 +147,10 @@ mod nullifier;
 // block in schnorr_double.rs (methods on Engine).
 mod schnorr_double;
 
+// Phoenix note values (commitments, creating obfuscated notes and their checked opening): their own `extern "C"` block in
+// notes.rs (methods on Engine).
+mod notes;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

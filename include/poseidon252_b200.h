@@ -454,6 +454,54 @@ int p252_note_sign_double_batch(p252_ctx* ctx, const p252_jscalar* a, const p252
                                 const p252_fr* G_uv, const p252_fr* Gp_uv, p252_jscalar* u, p252_fr* R_uv, p252_fr* Rp_uv,
                                 p252_fr* pkp_uv, uint8_t* ok, size_t* n_invalid, int flags);
 
+/* ---- Phoenix note values: commitments, creating obfuscated notes and opening them ------------------------------------
+ *   commit(v, blinder)    = C = [v] G + [blinder] G'                     (v a u64, blinder < r_J; G' = GENERATOR_NUMS)
+ *   create (r, v, blinder, nonce; A, B):  R = [r] G,  S = [r] A,  note_pk = [hash(S)] G + B,  C = commit(v, blinder),
+ *                                         cipher = encrypt([Fr(v), Fr(blinder)], S, nonce)       (L = 2: 3 scalars)
+ *   open  (a; R, nonce, cipher, C):       S = [a] R,  (m0, m1) = decrypt(cipher, S, nonce); the note OPENS iff the
+ *                                         authentication passes, m0 < 2^64, m1 < r_J and [m0] G + [m1] G' == C;
+ *                                         then value = m0, blinder = m1
+ *   hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0], as in the stealth calls; (A, B) is the receiver's
+ *   public key and a its view key.  The range checks are this library's rule: an opening with m0 >= 2^64 or m1 >= r_J does
+ *   not open even when its commitment matches.  A sender may encrypt an opening that does not match C; such a note cannot
+ *   be spent, so a wallet counts only the value of notes that open.
+ * G_uv and Gp_uv are HOST pointers for every memory space, as for the double-key calls; a coordinate >= p or a point off
+ * the curve in either is refused with P252_ERR_INVALID_POINT before anything runs, for every memory space and for n == 0.
+ * value: one uint64_t per item; blinder, r, a: p252_jscalar; nonce: p252_fr; points, C: (u, v) pairs of p252_fr; cipher:
+ * 3 p252_fr per item.  n_public (shared by A and B) and n_secret (a) are 1 or n.
+ * Item validity (checked on the device, for both memory spaces):
+ *   commit: blinder < r_J.
+ *   create: r < r_J, blinder < r_J, A and B curve points with u, v < p.
+ *   open:   a < r_J, R a curve point with u, v < p.
+ * An invalid item gets ok[i] = 0 and every output row it has zeroed (commitment; R, note_pk, commitment and cipher; value
+ * and blinder), and is counted once however many of its checks fail.  In p252_note_open_batch ok[i] = 0 with zeroed value
+ * and blinder also means the note did not open, and *n_failed counts every item with ok = 0 once, whatever the reason, as
+ * p252_decrypt_batch_dhke does.  n_invalid / n_failed: optional HOST pointers for both memory spaces.
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_public / n_secret not 1 or n, DEVICE buffers not aligned
+ * (value to 8 bytes, every other buffer but ok to 16) -> INVALID_ARGUMENT.
+ * Secrets: r, v, blinder, a, the shared point S, hash(S) and the plaintext rows live only in the context's staging
+ * arenas, for both memory spaces, and the arenas are zeroed on every exit path: all three calls are synchronous
+ * (P252_ASYNC only defers the publication of the count to p252_sync).  Each item is constant time (no branch and no address
+ * depends on a secret); see DESIGN.md section 4.  p252_note_open_batch returns value and blinder to the caller on purpose:
+ * a spend proof takes them as witnesses, and they must stay as private as the note's secret key.
+ * The fixed-base tables of G and G' are the double-key signature calls' two cache slots: a wallet that alternates these
+ * calls with scans, nullifiers and spend signing rebuilds no table. */
+/* commitment_uv[i] = commit(value[i], blinder[i]) */
+int p252_value_commit_batch(p252_ctx* ctx, const uint64_t* value, const p252_jscalar* blinder, size_t n, const p252_fr* G_uv,
+                            const p252_fr* Gp_uv, p252_fr* commitment_uv, uint8_t* ok, size_t* n_invalid, int flags);
+/* R_uv[i], note_pk_uv[i], commitment_uv[i], cipher[3 i .. 3 i + 2] = create(r[i], value[i], blinder[i], nonce[i];
+ *   (A_uv, B_uv)[n_public == 1 ? 0 : i]) */
+int p252_note_create_batch(p252_ctx* ctx, const p252_jscalar* r, const uint64_t* value, const p252_jscalar* blinder,
+                           const p252_fr* nonce, size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, const p252_fr* A_uv,
+                           const p252_fr* B_uv, size_t n_public, p252_fr* R_uv, p252_fr* note_pk_uv, p252_fr* commitment_uv,
+                           p252_fr* cipher, uint8_t* ok, size_t* n_invalid, int flags);
+/* value[i], blinder[i], ok[i] = open(a[n_secret == 1 ? 0 : i]; R_uv[i], nonce[i], cipher[3 i .. 3 i + 2],
+ *   commitment_uv[i]) */
+int p252_note_open_batch(p252_ctx* ctx, const p252_jscalar* a, size_t n_secret, const p252_fr* R_uv, const p252_fr* nonce,
+                         const p252_fr* cipher, const p252_fr* commitment_uv, size_t n, const p252_fr* G_uv,
+                         const p252_fr* Gp_uv, uint64_t* value, p252_jscalar* blinder, uint8_t* ok, size_t* n_failed,
+                         int flags);
+
 /* ---- JubJub point compression (dusk-jubjub's JubJubAffine::to_bytes / from_bytes) -----------------------------------
  *   encoding:  the 32 little-endian bytes of canonical v, with bit 255 (bytes[31] >> 7) = the low bit of canonical u
  *   decoding:  sign = bit 255, cleared; the remaining 255-bit value is v (rejected if >= p); u^2 = (v^2 - 1) / (1 + d v^2)

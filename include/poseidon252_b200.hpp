@@ -13,7 +13,8 @@
 //   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
 //   schnorr_verify_batch, nullifier / nullifier_batch, schnorr_sign_double / schnorr_sign_double_batch,
 //   schnorr_verify_double / schnorr_verify_double_batch, note_sign_double_batch, point_from_bytes /
-//   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
+//   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, value_commit / value_commit_batch,
+//   note_create_batch, note_open / note_open_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -580,6 +581,88 @@ inline void point_to_bytes(const Scalar (&uv)[2], uint8_t (&bytes)[32], Engine& 
     const auto r = points_to_bytes_batch(uv, 1, ok, nullptr, e);
     if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
     std::copy(r.begin(), r.end(), bytes);
+}
+
+// NEW: Phoenix note values (p252_value_commit_batch / p252_note_create_batch / p252_note_open_batch): the value commitment
+// C = [v] G + [blinder] G' (v a u64, blinder < r_J), obfuscated notes for the receiver (A, B) -- R = [r] G, S = [r] A,
+// note_pk = [hash(S)] G + B, C, cipher = encrypt([Fr(v), Fr(blinder)], S, nonce) (3 scalars) -- and the wallet's checked
+// opening: (m0, m1) = decrypt(cipher, [a] R, nonce) opens the note iff the authentication passes, m0 < 2^64, m1 < r_J and
+// [m0] G + [m1] G' == C.  G_uv and Gp_uv are the caller's G and G' (GENERATOR_NUMS); either off the curve throws
+// Error(P252_ERR_INVALID_POINT).  ok[i] == 0 marks an invalid item (or a note that did not open), whose rows are zeroed.
+// Returns the n commitments (2 scalars each)
+inline std::vector<Scalar> value_commit_batch(const uint64_t* value, const JubJubScalar* blinder, size_t n,
+                                              const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2], std::vector<uint8_t>& ok,
+                                              size_t* n_invalid = nullptr, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> C(2 * n);
+    ok.assign(n, 0);
+    check(p252_value_commit_batch(e.get(), value, blinder, n, G_uv, Gp_uv, C.data(), ok.data(), n_invalid, P252_MEM_HOST),
+          e.get());
+    return C;
+}
+// one commitment; throws Error(P252_ERR_INVALID_POINT) for blinder >= r_J
+inline void value_commit(uint64_t value, const JubJubScalar& blinder, const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2],
+                         Scalar (&C_uv)[2], Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok;
+    const auto C = value_commit_batch(&value, &blinder, 1, G_uv, Gp_uv, ok, nullptr, e);
+    if (!ok[0]) throw Error(P252_ERR_INVALID_POINT, p252_strerror(P252_ERR_INVALID_POINT));
+    C_uv[0] = C[0], C_uv[1] = C[1];
+}
+// A and B hold 1 or n points each (n_public); R, note_pk and C receive n x 2 scalars, cipher n x 3.  Returns ok
+inline std::vector<uint8_t> note_create_batch(const JubJubScalar* r, const uint64_t* value, const JubJubScalar* blinder,
+                                              const Scalar* nonce, size_t n, const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2],
+                                              const Scalar* A, const Scalar* B, size_t n_public, std::vector<Scalar>& R,
+                                              std::vector<Scalar>& note_pk, std::vector<Scalar>& C,
+                                              std::vector<Scalar>& cipher, size_t* n_invalid = nullptr,
+                                              Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok(n, 0);
+    R.assign(2 * n, Scalar{});
+    note_pk.assign(2 * n, Scalar{});
+    C.assign(2 * n, Scalar{});
+    cipher.assign(3 * n, Scalar{});
+    check(p252_note_create_batch(e.get(), r, value, blinder, nonce, n, G_uv, Gp_uv, A, B, n_public, R.data(), note_pk.data(),
+                                 C.data(), cipher.data(), ok.data(), n_invalid, P252_MEM_HOST),
+          e.get());
+    return ok;
+}
+// a holds 1 or n view keys (n_secret); R, C n x 2 scalars, cipher n x 3.  Returns the n values; blinder receives n
+// scalars; n_failed (may be null) counts the items with ok == 0.  value and blinder are the spend proof's witnesses
+inline std::vector<uint64_t> note_open_batch(const JubJubScalar* a, size_t n_secret, const Scalar* R, const Scalar* nonce,
+                                             const Scalar* cipher, const Scalar* C, size_t n, const Scalar (&G_uv)[2],
+                                             const Scalar (&Gp_uv)[2], std::vector<JubJubScalar>& blinder,
+                                             std::vector<uint8_t>& ok, size_t* n_failed = nullptr,
+                                             Engine& e = Engine::default_engine()) {
+    std::vector<uint64_t> value(n, 0);
+    blinder.assign(n, JubJubScalar{});
+    ok.assign(n, 0);
+    check(p252_note_open_batch(e.get(), a, n_secret, R, nonce, cipher, C, n, G_uv, Gp_uv, value.data(), blinder.data(),
+                               ok.data(), n_failed, P252_MEM_HOST),
+          e.get());
+    return value;
+}
+// the opening of one note -> v; throws Error(P252_ERR_INVALID_POINT) for a >= r_J or an R off the curve, and
+// Error(P252_ERR_DECRYPTION_FAILED) for a note that does not open
+inline uint64_t note_open(const JubJubScalar& a, const Scalar (&R_uv)[2], const Scalar& nonce, const Scalar (&cipher)[3],
+                          const Scalar (&C_uv)[2], const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2], JubJubScalar& blinder,
+                          Engine& e = Engine::default_engine()) {
+    std::vector<JubJubScalar> b;
+    std::vector<uint8_t> ok;
+    const auto v = note_open_batch(&a, 1, R_uv, &nonce, cipher, C_uv, 1, G_uv, Gp_uv, b, ok, nullptr, e);
+    if (!ok[0]) {
+        static const uint64_t order[4] = {0xd0970e5ed6f72cb7ULL, 0xa6682093ccc81082ULL, 0x06673b0101343b00ULL,
+                                          0x0e7db4ea6533afa9ULL};   // r_J
+        bool below = false;
+        for (int k = 3; k >= 0; --k)
+            if (a.l[k] != order[k]) {
+                below = a.l[k] < order[k];
+                break;
+            }
+        std::vector<uint8_t> on_curve;
+        points_to_bytes_batch(R_uv, 1, on_curve, nullptr, e);
+        const int code = below && on_curve[0] ? P252_ERR_DECRYPTION_FAILED : P252_ERR_INVALID_POINT;
+        throw Error(code, p252_strerror(code));
+    }
+    blinder = b[0];
+    return v[0];
 }
 
 // NEW: multi-scalar multiplication and all-or-nothing Schnorr batch verification (p252_jubjub_msm /

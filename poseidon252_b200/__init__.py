@@ -14,7 +14,9 @@ plus the batch entry points this engine adds:
     (multi-scalar multiplication) and schnorr_verify_all (all-or-nothing batch verification), nullifier /
     nullifier_batch (Phoenix note nullifiers: which owned notes are spent), schnorr_sign_double /
     schnorr_sign_double_batch, schnorr_verify_double / schnorr_verify_double_batch and note_sign_double_batch (double-key
-    Schnorr signatures over G and G', and spending a note under its note secret key), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
+    Schnorr signatures over G and G', and spending a note under its note secret key), value_commit /
+    value_commit_batch, note_create / note_create_batch and note_open / note_open_batch (Phoenix note values: Pedersen
+    commitments, creating obfuscated notes and their checked opening), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
     with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
@@ -29,6 +31,7 @@ from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, Inv
 from .hash import Domain, Hash, pack_varlen
 from .merkle import CompactTree, SparseTree, Tree, merkle4_build, merkle4_level
 from .msm import jubjub_msm, schnorr_verify_all
+from .notes import note_create, note_create_batch, note_open, note_open_batch, value_commit, value_commit_batch
 from .nullifier import nullifier, nullifier_batch
 from .points import point_from_bytes, point_to_bytes, points_from_bytes_batch, points_to_bytes_batch
 from .schnorr import schnorr_sign, schnorr_sign_batch, schnorr_verify, schnorr_verify_batch
@@ -45,7 +48,8 @@ __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encr
            "point_from_bytes", "point_to_bytes", "points_from_bytes_batch", "points_to_bytes_batch",
            "jubjub_msm", "schnorr_verify_all", "nullifier", "nullifier_batch",
            "schnorr_sign_double", "schnorr_sign_double_batch", "schnorr_verify_double", "schnorr_verify_double_batch",
-           "note_sign_double_batch",
+           "note_sign_double_batch", "value_commit", "value_commit_batch", "note_create", "note_create_batch",
+           "note_open", "note_open_batch",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",

@@ -103,6 +103,13 @@ SIGNATURES = {
     "p252_note_sign_double_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_size_t,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                             ctypes.POINTER(c_size_t), c_int]),
+    "p252_value_commit_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p,
+                                        ctypes.POINTER(c_size_t), c_int]),
+    "p252_note_create_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       ctypes.POINTER(c_size_t), c_int]),
+    "p252_note_open_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                     c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_points_from_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_points_to_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_jubjub_msm": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_size_t), c_int]),

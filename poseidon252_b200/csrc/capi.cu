@@ -16,6 +16,8 @@
 //   Phoenix note nullifiers (consumer, not the reference) -> p252_nullifier_batch
 //   jubjub-schnorr SignatureDouble, Phoenix note signing (consumer, not the reference) -> p252_schnorr_sign_double_batch,
 //     p252_schnorr_verify_double_batch, p252_note_sign_double_batch
+//   Phoenix note values (consumer, not the reference) -> p252_value_commit_batch, p252_note_create_batch,
+//     p252_note_open_batch
 //   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -101,8 +103,8 @@ struct p252_ctx {
     // instances, so that alternating digest and encryption calls rebuild neither
     TagTable vt, ct;
     BaseTable bt;   // fixed-base JubJub table
-    // the tables of G and G' of the double-key signature calls, only theirs: a wallet that alternates single-base calls with
-    // spend signing keeps all three
+    // the tables of G and G' of the double-key signature and note value calls, only theirs: a wallet that alternates
+    // single-base calls with spend signing and note calls keeps all three
     BaseTable bt2[2];
     // test hook: index of the staged chunk that fails in the next host-buffer call (-1 = none)
     long long fail_chunk = -1;
@@ -1371,6 +1373,123 @@ int p252_note_sign_double_batch(p252_ctx* ctx, const p252_jscalar* a, const p252
         if (e == P252_OK)
             e = launched(ctx, p252::launch_note_sign_double(d[1], sb, d[12], valid, d[3], d[14], cnt, table_p, d[5], d[6], d[7],
                                                             d[8], okc, counts.counter(0), st));
+        return e;
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+// ---- note values: commitments C = [v] G + [blinder] G', creating obfuscated notes and opening them ----------------------
+// commit: one launch_value_commit per chunk.  create (the sender): launch_fixed_base (R), launch_dhke (the shared point
+// S = [r] A into a slot arena), the truncated launch_digest of S (h, the stealth calls' hash), launch_note_value (C, the
+// message rows [Fr(v), Fr(blinder)] into the arena, validity &= blinder < r_J), launch_stealth_derive (note_pk; it zeroes R
+// of an invalid item, sets ok and counts), launch_encrypt at L = 2 with S, then launch_dhke_fix on the cipher rows and again
+// on the commitment rows.  Both fixes read ok as the validity, because only ok holds every check (B's is made by
+// launch_stealth_derive); they count nothing.  open (the wallet): launch_dhke (S = [a] R), launch_decrypt at L = 2 into the
+// arena (no count), launch_note_open_value (range checks, the commitment check, outputs, ok and the count of every item
+// that did not open).  The secrets (r, v, blinder, a, S, h and the plaintext rows) live only in the slot arenas for both
+// memory spaces, so all three calls are synchronous and the common exit join_slots(wipe) clears them on every path.  The
+// tables of G and G' come from the context's two-slot cache ctx->bt2, shared with the double-key signature calls.
+int p252_value_commit_batch(p252_ctx* ctx, const uint64_t* value, const p252_jscalar* blinder, size_t n, const p252_fr* G_uv,
+                            const p252_fr* Gp_uv, p252_fr* commitment_uv, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !args_ok(n, flags, {blinder, commitment_uv}, {ok}, {value}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 value, 1 blinder, 2 commitment, 3 ok
+    std::vector<Io> ios = {{value, nullptr, 8, false, dev}, {blinder, nullptr, 32, false, dev},
+                           {nullptr, commitment_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_value_commit(static_cast<const uint64_t*>(d[0]), d[1], cnt, table, table_p, d[2],
+                                                       static_cast<uint8_t*>(d[3]), counts.counter(0), st));
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+int p252_note_create_batch(p252_ctx* ctx, const p252_jscalar* r, const uint64_t* value, const p252_jscalar* blinder,
+                           const p252_fr* nonce, size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, const p252_fr* A_uv,
+                           const p252_fr* B_uv, size_t n_public, p252_fr* R_uv, p252_fr* note_pk_uv, p252_fr* commitment_uv,
+                           p252_fr* cipher, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !one_or_n(n_public, n) ||
+        !args_ok(n, flags, {r, blinder, nonce, A_uv, B_uv, R_uv, note_pk_uv, commitment_uv, cipher}, {ok}, {value}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag_h, tag_e;
+    if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = p252_encryption_tag(2, &tag_e)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 r, 1 value, 2 blinder, 3 nonce, 4 A, 5 B, 6 R, 7 note_pk, 8 commitment, 9 cipher, 10 ok; 11 shared points,
+    // 12 validity, 13 h and 14 the message rows live in the arena only
+    std::vector<Io> ios = {{r, nullptr, 32, false, dev}, {value, nullptr, 8, false, dev}, {blinder, nullptr, 32, false, dev},
+                           {nonce, nullptr, 32, false, dev}, {A_uv, nullptr, 64, pb, dev}, {B_uv, nullptr, 64, pb, dev},
+                           {nullptr, R_uv, 64, false, dev}, {nullptr, note_pk_uv, 64, false, dev},
+                           {nullptr, commitment_uv, 64, false, dev}, {nullptr, cipher, 96, false, dev},
+                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32},
+                           {nullptr, nullptr, 64}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[10]);
+        uint8_t* valid = static_cast<uint8_t*>(d[12]);
+        int e = launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[6], okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke(d[0], false, d[4], pb, cnt, d[11], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[11], cnt, 2, d[13], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_note_value(static_cast<const uint64_t*>(d[1]), d[2], cnt, table, table_p, d[8], d[14],
+                                                      valid, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_stealth_derive(d[13], cnt, table, d[5], pb, valid, d[6], d[7], okc, counts.counter(0),
+                                                          st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_encrypt(limbs(&tag_e), d[14], cnt, 2, d[11], d[3], d[9], st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(false, okc, cnt, d[9], 3, okc, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(false, okc, cnt, d[8], 2, okc, nullptr, st));
+        return e;
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+int p252_note_open_batch(p252_ctx* ctx, const p252_jscalar* a, size_t n_secret, const p252_fr* R_uv, const p252_fr* nonce,
+                         const p252_fr* cipher, const p252_fr* commitment_uv, size_t n, const p252_fr* G_uv,
+                         const p252_fr* Gp_uv, uint64_t* value, p252_jscalar* blinder, uint8_t* ok, size_t* n_failed,
+                         int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !one_or_n(n_secret, n) ||
+        !args_ok(n, flags, {a, R_uv, nonce, cipher, commitment_uv, blinder}, {ok}, {value}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag_e;
+    if ((rc = p252_encryption_tag(2, &tag_e)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const Counts counts(ctx, flags, n_failed, ok, n);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 a, 1 R, 2 nonce, 3 cipher, 4 commitment, 5 value, 6 blinder, 7 ok; 8 shared points, 9 validity and 10 the
+    // plaintext rows live in the arena only
+    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev}, {nonce, nullptr, 32, false, dev},
+                           {cipher, nullptr, 96, false, dev}, {commitment_uv, nullptr, 64, false, dev},
+                           {nullptr, value, 8, false, dev}, {nullptr, blinder, 32, false, dev}, {nullptr, ok, 1, false, dev},
+                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 64}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* okc = static_cast<uint8_t*>(d[7]);
+        uint8_t* valid = static_cast<uint8_t*>(d[9]);
+        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[1], false, cnt, d[8], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_decrypt(limbs(&tag_e), d[3], cnt, 2, d[8], d[2], d[10], okc, nullptr, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_note_open_value(d[10], valid, d[4], cnt, table, table_p, static_cast<uint64_t*>(d[5]),
+                                                           d[6], okc, counts.counter(0), st));
         return e;
     }, /*wipe=*/true);
     return counts.end(rc);

@@ -388,19 +388,21 @@ __device__ __forceinline__ void select_niels(Niels& q, const uint4* tab, int w, 
 // adds another point to the result; without it t.T is not the result's.  t is also the windows' temporary, as it was in
 // fixed_base_mul before the split, which keeps k_fixed_base's code unchanged.
 // fixed_base_from: the same walk from acc (with T) instead of the identity, t = acc + [s] B; acc is the walk's
-// accumulator and is overwritten.
-template <bool kLdg, bool kLastT>
+// accumulator and is overwritten.  kWin: the walk covers windows 0..kWin-1 only, for s < 2^(4 (kWin - 1)) (its last
+// digit is the final carry); the default is the whole table.
+template <bool kLdg, bool kLastT, int kWin = kFbWindows>
 __device__ __forceinline__ void fixed_base_from(Ext& t, Ext& acc, const uint32_t (&s)[8], const uint4* tab) {
+    static_assert(kWin >= 1 && kWin <= kFbWindows, "a walk over the table's windows");
     uint32_t d[8], carry = 0;
     fcopy(d, s);
     Niels q;
 #pragma unroll 1
-    for (int w = 0; w < kFbWindows - 1; ++w) {
+    for (int w = 0; w < kWin - 1; ++w) {
         select_niels<kLdg>(q, tab, w, recode_digit(d, carry));
         madd<true>(t, acc, q);
         acc = t;
     }
-    select_niels<kLdg>(q, tab, kFbWindows - 1, recode_digit(d, carry));
+    select_niels<kLdg>(q, tab, kWin - 1, recode_digit(d, carry));
     madd<kLastT>(t, acc, q);
 }
 
@@ -480,6 +482,24 @@ constexpr int kProductsPerSchnorrVerifyDouble = 2 * kProductsPerSchnorrVerify;
 static_assert(kProductsPerSchnorrSignDouble == 1732, "product count of DESIGN.md section 4");
 static_assert(kProductsPerNoteSignDouble == 5417, "product count of DESIGN.md section 4");
 static_assert(kProductsPerSchnorrVerifyDouble == 5700, "product count of DESIGN.md section 4");
+
+// ---- note values: C = [v] G + [blinder] G' (p252_value_commit_batch, p252_note_create_batch, p252_note_open_batch) ----
+// [blinder] G' is the whole fixed-base walk of G' with T in every window (64 x 7); the walk of G continues from it for
+// kValueWindows windows only: a u64 v recodes to 16 signed digits in [-8, 8) and a final carry digit in {0, 1} (window 16
+// of the table).  The window count is public, so every item runs the same schedule.
+//   commit / create: the last window without T (6), the inversion and the affine conversion.  create also writes the
+//                    message rows Fr(v), Fr(blinder), one product by R^2 mod p each (fr_from_canonical).
+//   open:            the decrypted rows leave Montgomery form by two reductions (fr_to_canonical, not counted as
+//                    products), then the walk and the projective comparison with C, X == u Z and Y == v Z (2): no
+//                    inversion.
+constexpr int kValueWindows = 17;
+constexpr int kProductsPerValueCommit = kFbWindows * 7 + (kValueWindows - 1) * 7 + 6 + (kPm2Bits - 1) + (kPm2Ones - 1) + 2;
+constexpr int kProductsPerNoteCreateValue = kProductsPerValueCommit + 2;
+constexpr int kProductsPerNoteOpenValue = kFbWindows * 7 + (kValueWindows - 1) * 7 + 6 + 2;
+static_assert(kValueWindows == 64 / 4 + 1, "a u64 in signed 4-bit digits and the final carry");
+static_assert(kProductsPerValueCommit == 985, "product count of DESIGN.md section 4");
+static_assert(kProductsPerNoteCreateValue == 987, "product count of DESIGN.md section 4");
+static_assert(kProductsPerNoteOpenValue == 568, "product count of DESIGN.md section 4");
 
 // Arithmetic modulo r_J on 8 x 32-bit little-endian words, Montgomery form with R = 2^256.  Constants (immediates, as
 // P252_JJ_ORDER): R^2 mod r_J and kOrderInv = -r_J^-1 mod 2^32.  Constant time: no branch and no address depends on an

@@ -2044,6 +2044,131 @@ cudaError_t launch_schnorr_verify_double(const void* pk, const void* pkp, bool p
     return cudaGetLastError();
 }
 
+// ---- note values: C = [v] G + [blinder] G' (jubjub_device.cuh) ---------------------------------------------------------
+// One thread per item.  table / table_p: the fixed-base tables of G and G'.  [blinder] G' walks the whole table of G' with
+// T, then the walk of G continues from it over kValueWindows windows (v is a u64).  v, blinder and the plaintext rows are
+// secret: every validity is a mask, an out-of-range operand enters the walk as 0, and the table reads are masked selects.
+//   kValueCommit (kProductsPerValueCommit): value[i], blinder[i] (canonical 4 x u64) in; ok[i] = blinder < r_J; the
+//     affine C into commitment, zeroed for an invalid item; *count += invalid items.
+//   kValueCreate (kProductsPerNoteCreateValue): as commit, but C is written unmasked (the caller zeroes the rows of invalid
+//     items once every check is in), rows[i] = [Fr(v), Fr(blinder)] (64 bytes, Montgomery: the message to encrypt), and
+//     valid[i] &= blinder < r_J.
+//   kValueOpen (kProductsPerNoteOpenValue): rows[i] the decrypted [m0, m1] (Montgomery), ok[i] their authentication,
+//     valid[i] the key exchange's validity; opened = ok and valid, m0 < 2^64, m1 < r_J, C's coordinates < p and
+//     [m0] G + [m1] G' == C (projective).  value[i] = m0 and blinder[i] = m1 if opened, zeros otherwise; ok[i] = opened;
+//     *count += items not opened.
+enum ValueMode { kValueCommit, kValueCreate, kValueOpen };
+
+template <int kMode>
+__global__ void __launch_bounds__(kThreads, 3) k_value_commit(uint64_t* value, uint8_t* blinder, size_t n,
+                                                           const uint4* __restrict__ table, const uint4* __restrict__ table_p,
+                                                           uint8_t* commitment, uint8_t* rows, uint8_t* valid, uint8_t* ok,
+                                                           unsigned long long* __restrict__ count) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t v[8] = {0, 0, 0, 0, 0, 0, 0, 0}, b[8];
+    bool good;
+    if (kMode == kValueOpen) {
+        uint32_t m[8];
+        load_fr_rw(m, rows + i * 64);
+        fr_to_canonical(v, m);
+        load_fr_rw(m, rows + i * 64 + 32);
+        fr_to_canonical(b, m);
+        const bool small = (v[2] | v[3] | v[4] | v[5] | v[6] | v[7]) == 0;
+        const bool in_range = jj::below_order(b);
+        const uint32_t ms = 0u - (uint32_t)small, mb = 0u - (uint32_t)in_range;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] &= ms, b[k] &= mb;
+        good = (ok[i] != 0) & (valid[i] != 0) & small & in_range;
+    } else {
+        const uint64_t x = value[i];
+        v[0] = (uint32_t)x, v[1] = (uint32_t)(x >> 32);
+        load_fr(b, blinder + i * 32);
+        good = jj::below_order(b);
+        const uint32_t mb = 0u - (uint32_t)good;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) b[k] &= mb;
+    }
+    jj::Ext t;
+    {
+        jj::Ext acc;
+        jj::fixed_base_ext<true, true>(acc, b, table_p);
+        jj::fixed_base_from<true, false, jj::kValueWindows>(t, acc, v, table);
+    }
+    if (kMode == kValueOpen) {
+        uint32_t cu[8], cv[8], x[8], y[8];
+        load_fr(cu, commitment + i * 64);
+        load_fr(cv, commitment + i * 64 + 32);
+        const bool canon = fr_is_canonical(cu) & fr_is_canonical(cv);
+        const uint32_t mc = 0u - (uint32_t)canon;     // coordinates >= p enter no product
+#pragma unroll
+        for (int k = 0; k < 8; ++k) cu[k] &= mc, cv[k] &= mc;
+        jj::fmul(x, cu, t.Z);
+        jj::fmul(y, cv, t.Z);
+        const bool opened = good & canon & jj::feq(x, t.X) & jj::feq(y, t.Y);
+        const uint32_t mo = 0u - (uint32_t)opened;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) b[k] &= mo;
+        value[i] = ((uint64_t)v[1] << 32 | v[0]) & ((uint64_t)mo << 32 | mo);
+        store_fr(blinder + i * 32, b);
+        ok[i] = opened ? 1 : 0;
+        if (count) warp_count_every(count, !opened);
+    } else {
+        uint32_t zi[8], ou[8], ov[8];
+        jj::inverse(zi, t.Z);
+        jj::fmul(ou, t.X, zi);
+        jj::fmul(ov, t.Y, zi);
+        if (kMode == kValueCommit) {
+            const uint32_t m = 0u - (uint32_t)good;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m;
+        }
+        store_fr(commitment + i * 64, ou);
+        store_fr(commitment + i * 64 + 32, ov);
+        if (kMode == kValueCommit) {
+            ok[i] = good ? 1 : 0;
+            if (count) warp_count_every(count, !good);
+        } else {
+            uint32_t fv[8], fb[8];
+            fr_from_canonical(fv, v);
+            fr_from_canonical(fb, b);
+            store_fr(rows + i * 64, fv);
+            store_fr(rows + i * 64 + 32, fb);
+            valid[i] = (valid[i] != 0) & good ? 1 : 0;
+        }
+    }
+}
+
+cudaError_t launch_value_commit(const uint64_t* value, const void* blinder, size_t n, const void* table, const void* table_p,
+                                void* commitment, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_value_commit<kValueCommit><<<grid_for(n), kThreads, 0, st>>>(
+        const_cast<uint64_t*>(value), static_cast<uint8_t*>(const_cast<void*>(blinder)), n, static_cast<const uint4*>(table),
+        static_cast<const uint4*>(table_p), static_cast<uint8_t*>(commitment), nullptr, nullptr, ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_note_value(const uint64_t* value, const void* blinder, size_t n, const void* table, const void* table_p,
+                              void* commitment, void* rows, uint8_t* valid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_value_commit<kValueCreate><<<grid_for(n), kThreads, 0, st>>>(
+        const_cast<uint64_t*>(value), static_cast<uint8_t*>(const_cast<void*>(blinder)), n, static_cast<const uint4*>(table),
+        static_cast<const uint4*>(table_p), static_cast<uint8_t*>(commitment), static_cast<uint8_t*>(rows), valid, nullptr,
+        nullptr);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_note_open_value(const void* rows, const uint8_t* valid, const void* commitment, size_t n, const void* table,
+                                   const void* table_p, uint64_t* value, void* blinder, uint8_t* ok,
+                                   unsigned long long* n_failed, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_value_commit<kValueOpen><<<grid_for(n), kThreads, 0, st>>>(
+        value, static_cast<uint8_t*>(blinder), n, static_cast<const uint4*>(table), static_cast<const uint4*>(table_p),
+        static_cast<uint8_t*>(const_cast<void*>(commitment)), static_cast<uint8_t*>(const_cast<void*>(rows)),
+        const_cast<uint8_t*>(valid), ok, n_failed);
+    return cudaGetLastError();
+}
+
 // ---- point compression: JubJubAffine::from_bytes / to_bytes (jubjub_device.cuh) ---------------------------------------
 // One thread per point.  Public data only.
 // from_bytes (kProductsPerDecompress products): bytes[i] -> (u, v) Montgomery; ok[i] = v < p and u^2 a square.  An

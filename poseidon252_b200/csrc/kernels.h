@@ -196,6 +196,22 @@ cudaError_t launch_schnorr_verify_double(const void* pk, const void* pkp, bool p
                                          const void* Rp_uv, const void* c, const uint8_t* valid, size_t n, const void* table,
                                          const void* table_p, uint8_t* verified, unsigned long long* n_verified,
                                          unsigned long long* n_invalid, cudaStream_t st);
+// Note values (p252_value_commit_batch, p252_note_create_batch, p252_note_open_batch): C = [v] G + [blinder] G' (table,
+// table_p: the fixed-base tables of G and G'), v one u64 per item, blinder canonical 4 x u64, C as (u, v) Montgomery pairs.
+// Counters are device pointers and may be null.
+// commit: ok[i] = blinder < r_J; commitment[i] = C, zeroed for an invalid item; *n_invalid += invalid items
+cudaError_t launch_value_commit(const uint64_t* value, const void* blinder, size_t n, const void* table, const void* table_p,
+                                void* commitment, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st);
+// create: commitment[i] = C for every item (the caller zeroes invalid ones), rows[i] = [Fr(v), Fr(blinder)] (64 bytes,
+// Montgomery), valid[i] &= blinder < r_J
+cudaError_t launch_note_value(const uint64_t* value, const void* blinder, size_t n, const void* table, const void* table_p,
+                              void* commitment, void* rows, uint8_t* valid, cudaStream_t st);
+// open: rows[i] = the decrypted [m0, m1] (Montgomery), ok[i] their authentication, valid[i] the key exchange's validity.
+// ok[i] = ok and valid, m0 < 2^64, m1 < r_J, both coordinates of commitment[i] < p and [m0] G + [m1] G' == commitment[i];
+// value[i] = m0 and blinder[i] = m1 (canonical) where ok, zeros elsewhere; *n_failed += items with ok = 0
+cudaError_t launch_note_open_value(const void* rows, const uint8_t* valid, const void* commitment, size_t n, const void* table,
+                                   const void* table_p, uint64_t* value, void* blinder, uint8_t* ok,
+                                   unsigned long long* n_failed, cudaStream_t st);
 // Point compression (p252_points_from_bytes / p252_points_to_bytes): 32-byte encodings <-> (u, v) Montgomery pairs (64
 // bytes).  from: ok[i] = v < p and u^2 a square, an invalid item gets (0, 0); to: ok[i] = u, v < p and on the curve, an
 // invalid item gets 32 bytes of 0xff.  *n_invalid (a device counter, may be null) += invalid items.

@@ -744,6 +744,114 @@ class Engine:
         (sync() first after async_)."""
         return self._last("schnorr_double_invalid")
 
+    # -- note values: commitments, creating and opening notes ---------------------------------------------
+    def _values(self, value, like, n):
+        """value (n,): a numpy uint64 array, or a CUDA int64 tensor for device buffers"""
+        vp, nv, vk = self._idx(value, like, "value")
+        if nv != n:
+            raise EngineError(-1, "value must have %d entries, got %d" % (n, nv))
+        return vp, vk
+
+    def value_commit_batch(self, value, blinder, base, base_p, async_=False):
+        """Pedersen value commitments C_i = [value_i] base + [blinder_i] base_p.  value (n,) (a numpy uint64 array or a
+        CUDA int64 tensor), blinder (n, 4) p252_jscalar rows, base (G) and base_p (G' = GENERATOR_NUMS) (2, 4),
+        host-read -> (commitment (n, 2, 4), ok (n,) uint8).  An item with blinder >= r_J has ok == 0 and a zeroed row
+        (count: last_note_invalid()).  A base off the curve raises InvalidPoint."""
+        bp, bl, flags, bk = self._in(blinder, (4,))
+        if len(bl) != 1:
+            raise EngineError(-1, "blinder must have shape (n, 4)")
+        n = int(bl[0])
+        self._same_space(flags, _native.MEM_DEVICE if _is_torch(value) else _native.MEM_HOST)
+        vp, vk = self._values(value, bk, n)
+        g, gp = self._base(base), self._base(base_p)
+        C = self._result(None, (n, 2, 4), bk)
+        ok = self._ok_like(bk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("note_invalid", flags)
+        self._check(self._lib.p252_value_commit_batch(self._ctx, vp, bp, n, g.ctypes.data, gp.ctypes.data, self._ptr(C),
+                                                      self._ptr(ok), ctypes.byref(invalid), flags))
+        return C, ok
+
+    def note_create_batch(self, r, value, blinder, nonce, base, base_p, publics_A, publics_B, async_=False):
+        """The sender's obfuscated notes: R_i = [r_i] base, S_i = [r_i] A_i, note_pk_i = [hash(S_i)] base + B_i,
+        C_i = [value_i] base + [blinder_i] base_p and cipher_i = encrypt([Fr(value_i), Fr(blinder_i)], S_i, nonce_i), with
+        hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0].  r and blinder (n, 4) p252_jscalar rows, value (n,)
+        (a numpy uint64 array or a CUDA int64 tensor), nonce (n, 4), base (G) and base_p (G') (2, 4) host-read, publics_A
+        and publics_B (1 or n, 2, 4) with the same number of rows: the receiver's public key -> (R (n, 2, 4), note_pk
+        (n, 2, 4), commitment (n, 2, 4), cipher (n, 3, 4), ok (n,) uint8).  An item with r or blinder >= r_J or A or B not
+        a curve point has ok == 0 and all four rows zeroed (count: last_note_invalid()).  S and hash(S) never leave the
+        device."""
+        rp, rl, flags, rk = self._in(r, (4,))
+        if len(rl) != 1:
+            raise EngineError(-1, "r must have shape (n, 4)")
+        n = int(rl[0])
+        bp, bl, fb, bk = self._in(blinder, (4,))
+        np_, nl, fn, nk = self._in(nonce, (4,))
+        ap, al, fa, ak = self._in(publics_A, (2, 4))
+        Bp, Bl, fB, Bk = self._in(publics_B, (2, 4))
+        self._same_space(flags, fb, fn, fa, fB, _native.MEM_DEVICE if _is_torch(value) else _native.MEM_HOST)
+        self._same_lead("blinder", bl, n)
+        self._same_lead("nonce", nl, n)
+        if len(al) != 1 or int(al[0]) not in (1, n):
+            raise EngineError(-1, "publics_A must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(al)))
+        na = int(al[0])
+        if tuple(Bl) != (na,):
+            raise EngineError(-1, "publics_B must have %d rows like publics_A, got leading shape %s" % (na, tuple(Bl)))
+        vp, vk = self._values(value, rk, n)
+        g, gp = self._base(base), self._base(base_p)
+        R = self._result(None, (n, 2, 4), rk)
+        pk = self._result(None, (n, 2, 4), rk)
+        C = self._result(None, (n, 2, 4), rk)
+        cipher = self._result(None, (n, 3, 4), rk)
+        ok = self._ok_like(rk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("note_invalid", flags)
+        self._check(self._lib.p252_note_create_batch(self._ctx, rp, vp, bp, np_, n, g.ctypes.data, gp.ctypes.data, ap, Bp,
+                                                     na, self._ptr(R), self._ptr(pk), self._ptr(C), self._ptr(cipher),
+                                                     self._ptr(ok), ctypes.byref(invalid), flags))
+        return R, pk, C, cipher, ok
+
+    def note_open_batch(self, a, R, nonce, cipher, commitment, base, base_p, async_=False):
+        """The wallet's checked openings: S_i = [a] R_i, (m0, m1) = decrypt(cipher_i, S_i, nonce_i), and the note opens iff
+        the authentication passes, m0 < 2^64, m1 < r_J and [m0] base + [m1] base_p == commitment_i.  a (1 or n, 4)
+        p252_jscalar rows (the view key), R (n, 2, 4), nonce (n, 4), cipher (n, 3, 4), commitment (n, 2, 4), base (G) and
+        base_p (G') (2, 4) host-read -> (value (n,) (uint64, or int64 like the inputs' tensors), blinder (n, 4), ok (n,)
+        uint8).  ok == 0 (value and blinder zeroed) for a note that does not open and for an invalid item (a >= r_J, R not
+        a curve point); their count: last_note_failed().  value and blinder are the spend proof's witnesses: keep them as
+        private as the note's key."""
+        Rp, Rl, flags, Rk = self._in(R, (2, 4))
+        if len(Rl) != 1:
+            raise EngineError(-1, "R must have shape (n, 2, 4)")
+        n = int(Rl[0])
+        ap, al, fa, ak = self._in(a, (4,))
+        np_, nl, fn, nk = self._in(nonce, (4,))
+        cp, cl, fc, ck = self._in(cipher, (3, 4))
+        Cp, Cl, fC, Ck = self._in(commitment, (2, 4))
+        self._same_space(flags, fa, fn, fc, fC)
+        if len(al) != 1 or int(al[0]) not in (1, n):
+            raise EngineError(-1, "a must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(al)))
+        self._same_lead("nonce", nl, n)
+        self._same_lead("cipher", cl, n)
+        self._same_lead("commitment", Cl, n)
+        g, gp = self._base(base), self._base(base_p)
+        value = self._result(None, (n,), Rk)
+        blinder = self._result(None, (n, 4), Rk)
+        ok = self._ok_like(Rk, n)
+        flags = self._flags(flags, async_)
+        failed = self._counter("note_failed", flags)
+        self._check(self._lib.p252_note_open_batch(self._ctx, ap, int(al[0]), Rp, np_, cp, Cp, n, g.ctypes.data,
+                                                   gp.ctypes.data, self._ptr(value), self._ptr(blinder), self._ptr(ok),
+                                                   ctypes.byref(failed), flags))
+        return value, blinder, ok
+
+    def last_note_invalid(self):
+        """Invalid items of the last value_commit_batch or note_create_batch (sync() first after async_)."""
+        return self._last("note_invalid")
+
+    def last_note_failed(self):
+        """Items of the last note_open_batch that did not open, invalid ones included (sync() first after async_)."""
+        return self._last("note_failed")
+
     # -- point compression ------------------------------------------------------------------------
     def points_from_bytes(self, data, out=None, async_=False):
         """JubJubAffine::from_bytes over a batch: (n, 32) uint8 encodings (host) or (n, 4) 64-bit device tensor of the
