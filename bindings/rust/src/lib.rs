@@ -151,6 +151,10 @@ mod schnorr_double;
 // notes.rs (methods on Engine).
 mod notes;
 
+// Multi-key wallet scans (owner, nullifier, checked opening and per-key totals of every note): their own `extern "C"` block
+// in wallet.rs (methods on Engine).
+mod wallet;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

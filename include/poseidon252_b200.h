@@ -502,6 +502,48 @@ int p252_note_open_batch(p252_ctx* ctx, const p252_jscalar* a, size_t n_secret, 
                          const p252_fr* Gp_uv, uint64_t* value, p252_jscalar* blinder, uint8_t* ok, size_t* n_failed,
                          int flags);
 
+/* ---- Phoenix wallet scans: which of several keys owns each note, and the owned notes' nullifiers, openings and totals ---
+ * The keys are (a_j, b_j) for j < n_keys, 1 <= n_keys <= P252_WALLET_MAX_KEYS; B_j = [b_j] G is derived on the device.
+ * For note i (R, note_pk, pos, nonce, cipher, C):
+ *   owner[i]      = the smallest j whose key owns the note as p252_stealth_owns_batch decides it (note_pk ==
+ *                   [hash([a_j] R)] G + B_j), -1 if none does; with duplicate keys the smallest index wins
+ *   nullifier[i]  = the row p252_nullifier_batch(a_j, b_j, G', R, pos) returns, for j = owner[i]
+ *   value[i], blinder[i], opened[i] = what p252_note_open_batch(a_j; R, nonce, cipher, C, G, G') returns, range and
+ *                   commitment checks included.  An owned note that does not open keeps its owner and nullifier (it is
+ *                   the wallet's, but cannot be spent), with opened = 0 and value and blinder zeroed.
+ *   A note no key owns gets zeroed nullifier, value and blinder rows and opened = 0.
+ * key_totals: n_keys rows of 4 uint64_t, row j = {value_lo, value_hi, n_owned, n_opened}: the exact 128-bit sum of value
+ * over the notes key j owns that opened, how many notes it owns and how many of them opened.
+ * Validity (checked on the device, for both memory spaces):
+ *   a key is bad when a_j >= r_J or b_j >= r_J: it owns no note, and *n_bad_keys counts it;
+ *   a note is invalid when R is not a curve point with u, v < p or a coordinate of note_pk is >= p: owner -1, zeroed
+ *   rows, and *n_invalid counts it once.  A note_pk with canonical coordinates off the curve is simply not owned.  Cipher,
+ *   nonce and C are judged as p252_note_open_batch judges them.
+ * G_uv and Gp_uv are HOST pointers for every memory space, as for the note calls; a coordinate >= p or a point off the
+ * curve in either is refused with P252_ERR_INVALID_POINT before anything runs, also for n == 0.  n == 0 runs nothing: it
+ * writes nothing and counts nothing (both counts are 0, bad keys included).
+ * a, b: n_keys p252_jscalar rows; R, note_pk, C: (u, v) pairs of p252_fr; pos: uint64_t; nonce: p252_fr; cipher: 3
+ * p252_fr per note; owner: int32_t; value: uint64_t; blinder: p252_jscalar; opened: bytes.  n_invalid, n_bad_keys:
+ * optional HOST pointers for both memory spaces.
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_keys == 0 or > P252_WALLET_MAX_KEYS, DEVICE buffers
+ * not aligned (pos and value to 8 bytes, owner to 4, opened to none, every other buffer to 16) -> INVALID_ARGUMENT.
+ * Secrets and timing: a, b, every [a_j] R, its hash, note_sk, pk' and the plaintexts live only in the context's staging
+ * arenas, for both memory spaces, and the arenas are zeroed on every exit path.  The call is synchronous: P252_ASYNC only
+ * defers the publication of the counts to p252_sync.  Each (note, key) pair runs the same schedule, and so does the second
+ * phase of each owned note; the one thing that steers the schedule is ownership, which the call returns anyway: owned
+ * notes are compacted before the second phase.  The owner's rows are read by masked selects over all n_keys rows, so no
+ * address depends on which key matched (DESIGN.md section 4).
+ * The fixed-base tables of G and G' are the double-key and note calls' two cache slots: the call evicts no table, and
+ * alternating it with those calls rebuilds none. */
+#define P252_WALLET_MAX_KEYS 256
+/* owner[i], nullifier[i], value[i], blinder[i], opened[i] = scan(keys; note i);  key_totals[4 j .. 4 j + 3] = totals of
+ * key j */
+int p252_wallet_scan_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_keys, const p252_fr* R_uv,
+                           const p252_fr* note_pk_uv, const uint64_t* pos, const p252_fr* nonce, const p252_fr* cipher,
+                           const p252_fr* commitment_uv, size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, int32_t* owner,
+                           p252_fr* nullifier, uint64_t* value, p252_jscalar* blinder, uint8_t* opened, uint64_t* key_totals,
+                           size_t* n_invalid, size_t* n_bad_keys, int flags);
+
 /* ---- JubJub point compression (dusk-jubjub's JubJubAffine::to_bytes / from_bytes) -----------------------------------
  *   encoding:  the 32 little-endian bytes of canonical v, with bit 255 (bytes[31] >> 7) = the low bit of canonical u
  *   decoding:  sign = bit 255, cleared; the remaining 255-bit value is v (rejected if >= p); u^2 = (v^2 - 1) / (1 + d v^2)

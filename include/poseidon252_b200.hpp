@@ -14,7 +14,7 @@
 //   schnorr_verify_batch, nullifier / nullifier_batch, schnorr_sign_double / schnorr_sign_double_batch,
 //   schnorr_verify_double / schnorr_verify_double_batch, note_sign_double_batch, point_from_bytes /
 //   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, value_commit / value_commit_batch,
-//   note_create_batch, note_open / note_open_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
+//   note_create_batch, note_open / note_open_batch, wallet_scan_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -663,6 +663,37 @@ inline uint64_t note_open(const JubJubScalar& a, const Scalar (&R_uv)[2], const 
     }
     blinder = b[0];
     return v[0];
+}
+
+// NEW: multi-key wallet scans (p252_wallet_scan_batch): for each note the smallest key j whose (a_j, B_j = [b_j] G) owns
+// it (owner -1: none), and for owned notes the nullifier and the checked opening under that key; key_totals row j =
+// {value_lo, value_hi, n_owned, n_opened}.  a, b: n_keys keys (1..P252_WALLET_MAX_KEYS); R, note_pk, C: n x 2 scalars;
+// cipher n x 3.  G_uv / Gp_uv off the curve throw Error(P252_ERR_INVALID_POINT).  Returns every result and both counts.
+struct WalletScan {
+    std::vector<int32_t> owner;
+    std::vector<Scalar> nullifier;
+    std::vector<uint64_t> value;
+    std::vector<JubJubScalar> blinder;
+    std::vector<uint8_t> opened;
+    std::vector<uint64_t> key_totals;   // n_keys x 4
+    size_t n_invalid = 0, n_bad_keys = 0;
+};
+inline WalletScan wallet_scan_batch(const JubJubScalar* a, const JubJubScalar* b, size_t n_keys, const Scalar* R,
+                                    const Scalar* note_pk, const uint64_t* pos, const Scalar* nonce, const Scalar* cipher,
+                                    const Scalar* C, size_t n, const Scalar (&G_uv)[2], const Scalar (&Gp_uv)[2],
+                                    Engine& e = Engine::default_engine()) {
+    WalletScan w;
+    w.owner.assign(n, -1);
+    w.nullifier.assign(n, Scalar{});
+    w.value.assign(n, 0);
+    w.blinder.assign(n, JubJubScalar{});
+    w.opened.assign(n, 0);
+    w.key_totals.assign(4 * n_keys, 0);
+    check(p252_wallet_scan_batch(e.get(), a, b, n_keys, R, note_pk, pos, nonce, cipher, C, n, G_uv, Gp_uv, w.owner.data(),
+                                 w.nullifier.data(), w.value.data(), w.blinder.data(), w.opened.data(), w.key_totals.data(),
+                                 &w.n_invalid, &w.n_bad_keys, P252_MEM_HOST),
+          e.get());
+    return w;
 }
 
 // NEW: multi-scalar multiplication and all-or-nothing Schnorr batch verification (p252_jubjub_msm /

@@ -16,7 +16,8 @@ plus the batch entry points this engine adds:
     schnorr_sign_double_batch, schnorr_verify_double / schnorr_verify_double_batch and note_sign_double_batch (double-key
     Schnorr signatures over G and G', and spending a note under its note secret key), value_commit /
     value_commit_batch, note_create / note_create_batch and note_open / note_open_batch (Phoenix note values: Pedersen
-    commitments, creating obfuscated notes and their checked opening), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
+    commitments, creating obfuscated notes and their checked opening), wallet_scan_batch (which of several keys owns each
+    note, with the owned notes' nullifiers, checked openings and per-key totals), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
     with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
@@ -37,6 +38,7 @@ from .points import point_from_bytes, point_to_bytes, points_from_bytes_batch, p
 from .schnorr import schnorr_sign, schnorr_sign_batch, schnorr_verify, schnorr_verify_batch
 from .schnorr_double import (note_sign_double_batch, schnorr_sign_double, schnorr_sign_double_batch,
                              schnorr_verify_double, schnorr_verify_double_batch)
+from .wallet import wallet_scan_batch
 
 HADES_WIDTH = hades.WIDTH
 
@@ -49,7 +51,7 @@ __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encr
            "jubjub_msm", "schnorr_verify_all", "nullifier", "nullifier_batch",
            "schnorr_sign_double", "schnorr_sign_double_batch", "schnorr_verify_double", "schnorr_verify_double_batch",
            "note_sign_double_batch", "value_commit", "value_commit_batch", "note_create", "note_create_batch",
-           "note_open", "note_open_batch",
+           "note_open", "note_open_batch", "wallet_scan_batch",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",

@@ -110,6 +110,10 @@ SIGNATURES = {
                                        ctypes.POINTER(c_size_t), c_int]),
     "p252_note_open_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                                      c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_wallet_scan_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
+                                       c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t),
+                                       c_int]),
     "p252_points_from_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_points_to_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_jubjub_msm": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_size_t), c_int]),

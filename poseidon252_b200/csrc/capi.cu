@@ -352,6 +352,68 @@ int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch laun
     });
 }
 
+// Fixed-size batches whose chunks run in two phases, where the host needs something the first phase computed (a count)
+// before it can enqueue the second: the chunks are staged as in run_host_pipeline, but chunk c's second(d, cnt, st) and
+// its output copies are enqueued after chunk c + 1's first(d, cnt, st), so that while the host waits for chunk c the
+// device already has the next chunk's first phase queued on another slot, and consecutive chunks overlap.  Both callbacks
+// enqueue through launched() and return a P252_* status.
+template <typename First, typename Second>
+int run_host_pipeline2(p252_ctx* ctx, std::vector<Io>& ios, size_t n, First first, Second second, bool wipe = false) {
+    if (n == 0) return P252_OK;
+    const size_t chunk = pipeline_chunk(ios, n);
+    std::vector<void*> d[kSlots];
+    auto carve = [&](void* arena, std::vector<void*>& dd) {
+        dd.resize(ios.size());
+        Carve c{static_cast<uint8_t*>(arena)};
+        for (size_t b = 0; b < ios.size(); ++b)
+            if (!ios[b].device) dd[b] = c.take<uint8_t>((ios[b].once ? 1 : chunk) * ios[b].item_bytes);
+        return c.used;
+    };
+    const size_t need = carve(nullptr, d[0]);
+    return on_slots(ctx, wipe, [&](long long fail_at) -> int {
+        struct Pending {
+            bool on = false;
+            size_t off = 0, cnt = 0;
+            int slot = 0;
+        } prev;
+        auto finish = [&](const Pending& p) -> int {
+            cudaStream_t st = ctx->slots[p.slot].stream;
+            const int rc = second(d[p.slot].data(), p.cnt, st);
+            if (rc != P252_OK) return rc;
+            for (size_t b = 0; b < ios.size(); ++b)
+                if (ios[b].h_out && !ios[b].device)
+                    CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + p.off * ios[b].item_bytes, d[p.slot][b],
+                                       p.cnt * ios[b].item_bytes, cudaMemcpyDeviceToHost, st));
+            return P252_OK;
+        };
+        // the ramp-up of run_host_pipeline
+        size_t k = 0, cur = (n > 2 * chunk) ? std::max<size_t>(1024, chunk / 8 / 128 * 128) : chunk;
+        for (size_t off = 0, cnt = 0; off < n; off += cnt, ++k, cur = std::min(chunk, cur * 2)) {
+            cnt = std::min(cur, n - off);
+            const int s = (int)(k % kSlots);
+            Slot& sl = ctx->slots[s];
+            int rc = slot_reserve(ctx, sl, need, wipe);
+            if (rc != P252_OK) return rc;
+            carve(sl.arena, d[s]);
+            for (size_t b = 0; b < ios.size(); ++b) {
+                const Io& io = ios[b];
+                const size_t at = io.once ? 0 : off * io.item_bytes;
+                if (io.device)
+                    d[s][b] = io.h_out ? static_cast<uint8_t*>(io.h_out) + at
+                                       : const_cast<uint8_t*>(static_cast<const uint8_t*>(io.h_in) + at);
+                else if (io.h_in)
+                    CU(cudaMemcpyAsync(d[s][b], static_cast<const uint8_t*>(io.h_in) + at, (io.once ? 1 : cnt) * io.item_bytes,
+                                       cudaMemcpyHostToDevice, sl.stream));
+            }
+            if ((long long)k == fail_at) return injected_fault(ctx);
+            if ((rc = first(d[s].data(), cnt, sl.stream)) != P252_OK) return rc;
+            if (prev.on && (rc = finish(prev)) != P252_OK) return rc;
+            prev = Pending{true, off, cnt, s};
+        }
+        return finish(prev);
+    });
+}
+
 // Common exit of every HOST call that ran on the slot streams (success and failure): wipe, join, drain.
 int join_slots(p252_ctx* ctx, int rc, bool wipe) {
     const std::string first_error = ctx->last_error;
@@ -1492,6 +1554,120 @@ int p252_note_open_batch(p252_ctx* ctx, const p252_jscalar* a, size_t n_secret, 
                                                            d[6], okc, counts.counter(0), st));
         return e;
     }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+// ---- multi-key wallet scans: owner, nullifier, checked opening and per-key totals of every note -----------------------
+// Per chunk, first phase over the chunk's n k pairs (note i, key j at i k + j): launch_wallet_keys (the keys' B_j = [b_j] G
+// in Niels form and their validity, from the a and b rows staged once per chunk), launch_wallet_dhke ([a_j] R_i), the
+// truncated launch_digest of every pair's point (h, the stealth calls' hash), launch_wallet_match (the ownership check) and
+// launch_wallet_select (owner, zeroed rows, the invalid count, the owned notes compacted into dense rows).  The host then
+// reads the chunk's owned count (one synchronise per chunk, run_host_pipeline2: after the next chunk's first phase is
+// enqueued, so the chunks overlap) and the second phase runs on the owned rows only, with the nullifier call's and the opening call's unchanged kernels: launch_nullifier_key, the full launch_digest (the nullifier),
+// launch_decrypt at L = 2 and launch_note_open_value; launch_wallet_scatter writes the rows back in note order and adds to
+// the totals.  The keys, every shared point, its hash, note_sk, pk' and the plaintexts live only in the slot arenas for
+// both memory spaces (wiped by join_slots on every path).  B_j is derived per chunk, in the chunk's arena, so that it is
+// never outside a wiped arena: k fixed-base walks per chunk.  The totals accumulate in the caller's buffer (DEVICE) or in
+// one per-call device buffer (HOST), zeroed first, copied out once and wiped.  Counts: device counter 0 the invalid
+// notes, 1 the bad keys (counted in the first chunk only).
+int p252_wallet_scan_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_keys, const p252_fr* R_uv,
+                           const p252_fr* note_pk_uv, const uint64_t* pos, const p252_fr* nonce, const p252_fr* cipher,
+                           const p252_fr* commitment_uv, size_t n, const p252_fr* G_uv, const p252_fr* Gp_uv, int32_t* owner,
+                           p252_fr* nullifier, uint64_t* value, p252_jscalar* blinder, uint8_t* opened, uint64_t* key_totals,
+                           size_t* n_invalid, size_t* n_bad_keys, int flags) {
+    const bool dev = (flags & P252_MEM_DEVICE) != 0;
+    if (!ctx || !G_uv || !Gp_uv || n_keys == 0 || n_keys > P252_WALLET_MAX_KEYS ||
+        !args_ok(n, flags, {a, b, R_uv, note_pk_uv, nonce, cipher, commitment_uv, nullifier, blinder, key_totals},
+                 {owner, opened}, {pos, value}) ||
+        (dev && (reinterpret_cast<uintptr_t>(owner) & 3)))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag_h, tag_n, tag_e;
+    if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_tag(&tag_n)) != P252_OK ||
+        (rc = p252_encryption_tag(2, &tag_e)) != P252_OK)
+        return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const uint32_t k = (uint32_t)n_keys;
+    const Counts counts = Counts::device(ctx, flags, n_invalid, n_bad_keys);
+    if (n == 0) return P252_OK;
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 a, 1 b, 2 R, 3 note_pk, 4 pos, 5 nonce, 6 cipher, 7 C, 8 owner, 9 nullifier, 10 value, 11 blinder, 12 opened; in
+    // the arena only: 13 the keys' Niels rows, 14 their validity, 15 the owned count; per pair 16 shared points, 17
+    // validity, 18 h, 19 matched; the dense rows of owned notes 20 meta, 21 S, 22 h, 23 b, 24 pos, 25 nonce, 26 cipher,
+    // 27 C, 28 validity, 29 the nullifier digest rows, 30 nullifier, 31 plaintext, 32 ok, 33 value, 34 blinder
+    std::vector<Io> ios = {{a, nullptr, 32 * n_keys, true, dev}, {b, nullptr, 32 * n_keys, true, dev},
+                           {R_uv, nullptr, 64, false, dev}, {note_pk_uv, nullptr, 64, false, dev},
+                           {pos, nullptr, 8, false, dev}, {nonce, nullptr, 32, false, dev},
+                           {cipher, nullptr, 96, false, dev}, {commitment_uv, nullptr, 64, false, dev},
+                           {nullptr, owner, 4, false, dev}, {nullptr, nullifier, 32, false, dev},
+                           {nullptr, value, 8, false, dev}, {nullptr, blinder, 32, false, dev},
+                           {nullptr, opened, 1, false, dev}, {nullptr, nullptr, 96 * n_keys, true},
+                           {nullptr, nullptr, n_keys, true}, {nullptr, nullptr, 8, true},
+                           {nullptr, nullptr, 64 * n_keys}, {nullptr, nullptr, n_keys}, {nullptr, nullptr, 32 * n_keys},
+                           {nullptr, nullptr, n_keys}, {nullptr, nullptr, 8}, {nullptr, nullptr, 64}, {nullptr, nullptr, 32},
+                           {nullptr, nullptr, 32}, {nullptr, nullptr, 8}, {nullptr, nullptr, 32}, {nullptr, nullptr, 96},
+                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 96}, {nullptr, nullptr, 32},
+                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 8}, {nullptr, nullptr, 32}};
+    auto scan = [&](unsigned long long* tot) -> int {
+        const size_t tot_bytes = 4 * sizeof(uint64_t) * n_keys;
+        CU(cudaMemsetAsync(tot, 0, tot_bytes, ctx->stream));
+        bool first = true;
+        int r = run_host_pipeline2(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+            auto u8 = [&](int x) { return static_cast<uint8_t*>(d[x]); };
+            auto* n_own_d = static_cast<unsigned long long*>(d[15]);
+            const size_t np = cnt * k;
+            int e = launched(ctx, p252::launch_wallet_keys(d[0], d[1], k, table, d[13], u8(14), n_own_d,
+                                                           first ? counts.counter(1) : nullptr, st));
+            first = false;
+            if (e == P252_OK) e = launched(ctx, p252::launch_wallet_dhke(d[0], u8(14), k, d[2], np, d[16], u8(17), st));
+            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[16], np, 2, d[18], 1, true, ctx->coop_max, st));
+            if (e == P252_OK) e = launched(ctx, p252::launch_wallet_match(d[18], np, k, table, d[13], d[3], u8(17), u8(19), st));
+            const p252::WalletRows dense{d[20], d[21], d[22], d[23], static_cast<uint64_t*>(d[24]), d[25], d[26], d[27], u8(28)};
+            if (e == P252_OK)
+                e = launched(ctx, p252::launch_wallet_select(k, u8(19), d[16], d[18], d[1], d[2], d[3],
+                                                             static_cast<const uint64_t*>(d[4]), d[5], d[6], d[7], cnt,
+                                                             static_cast<int32_t*>(d[8]), d[9], static_cast<uint64_t*>(d[10]),
+                                                             d[11], u8(12), dense, n_own_d, counts.counter(0), st));
+            return e;
+        }, [&](void** d, size_t, cudaStream_t st) -> int {
+            auto u8 = [&](int x) { return static_cast<uint8_t*>(d[x]); };
+            unsigned long long n_own = 0;
+            CU(cudaMemcpyAsync(&n_own, d[15], sizeof n_own, cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+            if (n_own == 0) return P252_OK;
+            int e = launched(ctx, p252::launch_nullifier_key(d[22], d[23], false, static_cast<const uint64_t*>(d[24]), n_own, table_p,
+                                                         d[29], u8(28), st));
+            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_n), d[29], n_own, 3, d[30], 1, false, ctx->coop_max, st));
+            if (e == P252_OK)
+                e = launched(ctx, p252::launch_decrypt(limbs(&tag_e), d[26], n_own, 2, d[21], d[25], d[31], u8(32), nullptr, st));
+            if (e == P252_OK)
+                e = launched(ctx, p252::launch_note_open_value(d[31], u8(28), d[27], n_own, table, table_p,
+                                                               static_cast<uint64_t*>(d[33]), d[34], u8(32), nullptr, st));
+            if (e == P252_OK)
+                e = launched(ctx, p252::launch_wallet_scatter(d[20], d[30], static_cast<const uint64_t*>(d[33]), d[34], u8(32),
+                                                              n_own, d[9], static_cast<uint64_t*>(d[10]), d[11], u8(12), tot, st));
+            return e;
+        }, /*wipe=*/true);
+        if (!dev) {
+            if (r == P252_OK) {
+                const cudaError_t ce = cudaMemcpyAsync(key_totals, tot, tot_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+                if (ce != cudaSuccess) r = fail_cuda(ctx, ce, "cudaMemcpyAsync");
+            }
+            const cudaError_t we = cudaMemsetAsync(tot, 0, tot_bytes, ctx->stream);   // the totals are the wallet's balance
+            if (r == P252_OK && we != cudaSuccess) r = fail_cuda(ctx, we, "cudaMemsetAsync");
+        }
+        return r;
+    };
+    if (dev) {
+        rc = scan(reinterpret_cast<unsigned long long*>(key_totals));
+    } else {
+        unsigned long long* tot = nullptr;
+        rc = with_scratch(ctx, ctx->stream, [&](Carve& c) { tot = c.take<unsigned long long>(4 * n_keys); },
+                          [&] { return scan(tot); });
+    }
     return counts.end(rc);
 }
 

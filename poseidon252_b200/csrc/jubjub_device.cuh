@@ -501,6 +501,21 @@ static_assert(kProductsPerValueCommit == 985, "product count of DESIGN.md sectio
 static_assert(kProductsPerNoteCreateValue == 987, "product count of DESIGN.md section 4");
 static_assert(kProductsPerNoteOpenValue == 568, "product count of DESIGN.md section 4");
 
+// ---- multi-key wallet scans (p252_wallet_scan_batch) --------------------------------------------------------------------
+// per key:        B = [b] G (fixed_base_mul) and its Niels form (2).
+// per pair:       [a_j] R_i by k_dhke's schedule (its own inversion), then the stealth check against B_j (456); the hash
+//                 of [a_j] R_i in between is one Hades permutation (365 Montgomery products, counted with the permutation).
+// per note:       the validity of R (on-curve check, 4).
+// per owned note: k_nullifier_key (867) and the opening check (568); the nullifier digest (one permutation) and the
+//                 decryption at L = 2 (two) come on top.
+constexpr int kProductsPerWalletKey = kProductsPerFixedBase + 2;
+constexpr int kProductsPerWalletPair = kProductsPerDhke + kProductsPerStealthOwns;
+constexpr int kProductsPerWalletSelect = 4;
+constexpr int kProductsPerWalletOwned = kProductsPerNullifierKey + kProductsPerNoteOpenValue;
+static_assert(kProductsPerWalletKey == 868, "product count of DESIGN.md section 4");
+static_assert(kProductsPerWalletPair == 3275, "product count of DESIGN.md section 4");
+static_assert(kProductsPerWalletOwned == 1435, "product count of DESIGN.md section 4");
+
 // Arithmetic modulo r_J on 8 x 32-bit little-endian words, Montgomery form with R = 2^256.  Constants (immediates, as
 // P252_JJ_ORDER): R^2 mod r_J and kOrderInv = -r_J^-1 mod 2^32.  Constant time: no branch and no address depends on an
 // operand; each final correction is a masked subtraction or addition of r_J.

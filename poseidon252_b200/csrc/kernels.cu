@@ -13,6 +13,8 @@
 //   note nullifiers (pk' = [(h + b) mod r_J] G', the digest rows [pk'.u, pk'.v, pos]) -> k_nullifier_key
 //   double-key Schnorr signatures over G and G' (SignatureDouble, note signing) -> k_schnorr_pack_double,
 //     k_schnorr_sign_double<Note>, k_schnorr_verify_double
+//   multi-key wallet scans (owner, then nullifier and opening of owned notes) -> k_wallet_keys, k_wallet_dhke,
+//     k_wallet_match, k_wallet_select, k_wallet_scatter
 //   JubJubAffine::from_bytes / to_bytes (point compression) -> k_points_from_bytes, k_points_to_bytes
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
@@ -2166,6 +2168,264 @@ cudaError_t launch_note_open_value(const void* rows, const uint8_t* valid, const
         value, static_cast<uint8_t*>(blinder), n, static_cast<const uint4*>(table), static_cast<const uint4*>(table_p),
         static_cast<uint8_t*>(const_cast<void*>(commitment)), static_cast<uint8_t*>(const_cast<void*>(rows)),
         const_cast<uint8_t*>(valid), ok, n_failed);
+    return cudaGetLastError();
+}
+
+// ---- wallet scans: owner, nullifier, checked opening and per-key totals (jubjub_device.cuh) -----------------------------
+// k keys (a_j, b_j) and a chunk of n notes; a pair is (note i, key j), at index i k + j.  The key index of a pair is part of
+// the schedule (public), like the note index; what no address may depend on is which key owns a note (k_wallet_select).
+// keys (kProductsPerWalletKey per key): nb[j] = the Niels form of B_j = [b_j] G (96 bytes), kvalid[j] = a_j, b_j < r_J; a
+//   bad key derives B from b = 0.  Thread 0 zeroes the chunk's owned count; *n_bad += bad keys.
+__global__ void __launch_bounds__(kThreads, 3) k_wallet_keys(const uint8_t* __restrict__ a, const uint8_t* __restrict__ b,
+                                                          uint32_t k, const uint4* __restrict__ table, uint8_t* __restrict__ nb,
+                                                          uint8_t* __restrict__ kvalid, unsigned long long* __restrict__ n_owned,
+                                                          unsigned long long* __restrict__ n_bad) {
+    const uint32_t j = blockIdx.x * kThreads + threadIdx.x;
+    if (j == 0) *n_owned = 0;
+    if (j >= k) return;
+    uint32_t s[8], t[8];
+    load_fr(s, a + (size_t)j * 32);
+    load_fr(t, b + (size_t)j * 32);
+    const bool good = jj::below_order(s) & jj::below_order(t);
+    const uint32_t m = 0u - (uint32_t)good;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) t[q] &= m;
+    uint32_t u[8], v[8];
+    jj::fixed_base_mul<true>(u, v, t, table);
+    jj::Niels q;
+    jj::to_niels(q, u, v);
+    store_fr(nb + (size_t)j * 96, q.ymx);
+    store_fr(nb + (size_t)j * 96 + 32, q.ypx);
+    store_fr(nb + (size_t)j * 96 + 64, q.kt);
+    kvalid[j] = good ? 1 : 0;
+    if (n_bad) warp_count_every(n_bad, !good);
+}
+
+// dhke (k_dhke's schedule, kProductsPerDhke per pair): out[p] = [a_j] R_i as (u, v), ok[p] = key j good and R_i a curve
+// point with u, v < p.  An invalid pair runs the same schedule on (0, identity) and writes (0, 0).
+__global__ void __launch_bounds__(kThreads, 3) k_wallet_dhke(const uint8_t* __restrict__ a, const uint8_t* __restrict__ kvalid,
+                                                          uint32_t k, const uint8_t* __restrict__ R, size_t n_pairs,
+                                                          uint8_t* __restrict__ out, uint8_t* __restrict__ ok) {
+    const size_t p = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (p >= n_pairs) return;
+    const size_t i = p / k, j = p - i * k;
+    uint32_t s[8], u[8], v[8];
+    load_fr(s, a + j * 32);
+    load_fr(u, R + i * 64);
+    load_fr(v, R + i * 64 + 32);
+    const bool valid = (kvalid[j] != 0) & fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
+    const uint32_t m = 0u - (uint32_t)valid;
+    uint32_t one[8];
+    jj::set_one(one);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) s[q] &= m, u[q] &= m, v[q] = (v[q] & m) | (one[q] & ~m);
+    uint32_t ou[8], ov[8];
+    jj::scalar_mul(ou, ov, s, u, v);
+#pragma unroll
+    for (int q = 0; q < 8; ++q) ou[q] &= m, ov[q] &= m;
+    store_fr(out + p * 64, ou);
+    store_fr(out + p * 64 + 32, ov);
+    ok[p] = valid ? 1 : 0;
+}
+
+// match (k_stealth<true>'s check, kProductsPerStealthOwns per pair): matched[p] = valid[p], both note_pk_i coordinates < p
+// and note_pk_i == [h[p]] G + B_j, with B_j's Niels form read from nb; compared projectively.
+__global__ void __launch_bounds__(kThreads, 3) k_wallet_match(const uint8_t* __restrict__ h, size_t n_pairs, uint32_t k,
+                                                           const uint4* __restrict__ table, const uint8_t* __restrict__ nb,
+                                                           const uint8_t* __restrict__ note_pk, const uint8_t* __restrict__ valid,
+                                                           uint8_t* __restrict__ matched) {
+    const size_t p = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (p >= n_pairs) return;
+    const size_t i = p / k, j = p - i * k;
+    jj::Ext t, r;
+    {
+        uint32_t s[8];
+        load_fr(s, h + p * 32);
+        jj::fixed_base_ext<true, true>(t, s, table);
+    }
+    uint32_t u[8], v[8];
+    load_fr(u, note_pk + i * 64);
+    load_fr(v, note_pk + i * 64 + 32);
+    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
+    const uint32_t mc = 0u - (uint32_t)canon;     // coordinates >= p enter no product
+#pragma unroll
+    for (int q = 0; q < 8; ++q) u[q] &= mc, v[q] &= mc;
+    jj::Niels q;
+    load_fr(q.ymx, nb + j * 96);
+    load_fr(q.ypx, nb + j * 96 + 32);
+    load_fr(q.kt, nb + j * 96 + 64);
+    jj::madd<false>(r, t, q);
+    uint32_t x[8], y[8];
+    jj::fmul(x, u, r.Z);
+    jj::fmul(y, v, r.Z);
+    matched[p] = (valid[p] != 0) & canon & jj::feq(x, r.X) & jj::feq(y, r.Y) ? 1 : 0;
+}
+
+// select (per note, kProductsPerWalletSelect): owner[i] = the smallest j with matched[i k + j], -1 if none; the note's
+// nullifier, value, blinder and opened rows zeroed; *n_invalid += notes whose R is not a curve point with u, v < p or whose
+// note_pk has a coordinate >= p.  S, h and b of the owner's pair are read by masked selects over all k pairs and key
+// rows.  An owned note then takes the next dense row (warp-aggregated atomic on *n_owned): meta = (i, owner), S, h, b,
+// pos, nonce, cipher, C, dvalid = 1.  Ownership is the only thing that steers the schedule, and the call returns it.
+struct WalletDense {
+    uint2* meta;
+    uint8_t *S, *h, *b;
+    uint64_t* pos;
+    uint8_t *nonce, *cipher, *C, *valid;
+};
+
+__device__ __forceinline__ void copy_row(uint8_t* dst, const uint8_t* src, int words16) {
+    for (int q = 0; q < words16; ++q) reinterpret_cast<uint4*>(dst)[q] = __ldg(reinterpret_cast<const uint4*>(src) + q);
+}
+
+__global__ void __launch_bounds__(kThreads) k_wallet_select(uint32_t k, const uint8_t* __restrict__ matched,
+                                                            const uint8_t* __restrict__ S, const uint8_t* __restrict__ h,
+                                                            const uint8_t* __restrict__ b, const uint8_t* __restrict__ R,
+                                                            const uint8_t* __restrict__ note_pk, const uint64_t* __restrict__ pos,
+                                                            const uint8_t* __restrict__ nonce, const uint8_t* __restrict__ cipher,
+                                                            const uint8_t* __restrict__ C, size_t n, int32_t* __restrict__ owner,
+                                                            uint8_t* __restrict__ nullifier, uint64_t* __restrict__ value,
+                                                            uint8_t* __restrict__ blinder, uint8_t* __restrict__ opened,
+                                                            WalletDense dn, unsigned long long* __restrict__ n_owned,
+                                                            unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    int32_t own = -1;
+#pragma unroll 1
+    for (int32_t j = (int32_t)k - 1; j >= 0; --j) own = matched[i * k + j] ? j : own;
+    {
+        uint32_t u[8], v[8];
+        load_fr(u, R + i * 64);
+        load_fr(v, R + i * 64 + 32);
+        bool good = fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
+        load_fr(u, note_pk + i * 64);
+        load_fr(v, note_pk + i * 64 + 32);
+        good &= fr_is_canonical(u) & fr_is_canonical(v);
+        if (n_invalid) warp_count_every(n_invalid, !good);
+    }
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    owner[i] = own;
+    store_fr(nullifier + i * 32, zero);
+    store_fr(blinder + i * 32, zero);
+    value[i] = 0;
+    opened[i] = 0;
+    uint32_t su[8], sv[8], hs[8], bs[8];
+#pragma unroll
+    for (int q = 0; q < 8; ++q) su[q] = 0, sv[q] = 0, hs[q] = 0, bs[q] = 0;
+#pragma unroll 1
+    for (uint32_t j = 0; j < k; ++j) {            // j is the public loop counter: the same addresses for every owner
+        const uint32_t m = 0u - (uint32_t)((int32_t)j == own);
+        uint32_t x[8];
+        load_fr(x, S + (i * k + j) * 64);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) su[q] |= x[q] & m;
+        load_fr(x, S + (i * k + j) * 64 + 32);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) sv[q] |= x[q] & m;
+        load_fr(x, h + (i * k + j) * 32);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) hs[q] |= x[q] & m;
+        load_fr(x, b + (size_t)j * 32);
+#pragma unroll
+        for (int q = 0; q < 8; ++q) bs[q] |= x[q] & m;
+    }
+    const bool is_owned = own >= 0;
+    const unsigned act = __activemask();
+    const unsigned bal = __ballot_sync(act, is_owned);
+    const int lane = threadIdx.x & 31, leader = __ffs(act) - 1;
+    unsigned long long base = 0;
+    if (lane == leader && bal) base = atomicAdd(n_owned, (unsigned long long)__popc(bal));
+    base = __shfl_sync(act, base, leader);
+    if (!is_owned) return;
+    const size_t r = base + __popc(bal & ((1u << lane) - 1u));
+    dn.meta[r] = make_uint2((uint32_t)i, (uint32_t)own);
+    store_fr(dn.S + r * 64, su);
+    store_fr(dn.S + r * 64 + 32, sv);
+    store_fr(dn.h + r * 32, hs);
+    store_fr(dn.b + r * 32, bs);
+    dn.pos[r] = pos[i];
+    copy_row(dn.nonce + r * 32, nonce + i * 32, 2);
+    copy_row(dn.cipher + r * 96, cipher + i * 96, 6);
+    copy_row(dn.C + r * 64, C + i * 64, 4);
+    dn.valid[r] = 1;
+}
+
+// scatter (per owned note): dense row r back to note meta[r].x -- nullifier, value, blinder, opened -- and key meta[r].y's
+// totals: value_lo / value_hi (a 128-bit sum: the add that wraps the low word carries one into the high word), n_owned,
+// n_opened.  value is zero for a note that did not open.
+__global__ void __launch_bounds__(256) k_wallet_scatter(const uint2* __restrict__ meta, const uint8_t* __restrict__ dnul,
+                                                        const uint64_t* __restrict__ dvalue, const uint8_t* __restrict__ dblinder,
+                                                        const uint8_t* __restrict__ dok, size_t n_own, uint8_t* __restrict__ nullifier,
+                                                        uint64_t* __restrict__ value, uint8_t* __restrict__ blinder,
+                                                        uint8_t* __restrict__ opened, unsigned long long* __restrict__ totals) {
+    const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_own) return;
+    const uint2 mt = meta[r];
+    const size_t i = mt.x;
+    copy_row(nullifier + i * 32, dnul + r * 32, 2);
+    copy_row(blinder + i * 32, dblinder + r * 32, 2);
+    const uint64_t v = dvalue[r];
+    const bool op = dok[r] != 0;
+    value[i] = v;
+    opened[i] = op ? 1 : 0;
+    unsigned long long* t = totals + (size_t)mt.y * 4;
+    const unsigned long long old = atomicAdd(t, (unsigned long long)v);
+    if (old + v < old) atomicAdd(t + 1, 1ull);
+    atomicAdd(t + 2, 1ull);
+    if (op) atomicAdd(t + 3, 1ull);
+}
+
+cudaError_t launch_wallet_keys(const void* a, const void* b, uint32_t k, const void* table, void* nb, uint8_t* kvalid,
+                               unsigned long long* n_owned, unsigned long long* n_bad, cudaStream_t st) {
+    k_wallet_keys<<<(k + kThreads - 1) / kThreads, kThreads, 0, st>>>(static_cast<const uint8_t*>(a),
+                                                                     static_cast<const uint8_t*>(b), k,
+                                                                     static_cast<const uint4*>(table),
+                                                                     static_cast<uint8_t*>(nb), kvalid, n_owned, n_bad);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wallet_dhke(const void* a, const uint8_t* kvalid, uint32_t k, const void* R_uv, size_t n_pairs, void* shared_uv,
+                               uint8_t* valid, cudaStream_t st) {
+    if (n_pairs == 0) return cudaSuccess;
+    k_wallet_dhke<<<grid_for(n_pairs), kThreads, 0, st>>>(static_cast<const uint8_t*>(a), kvalid, k,
+                                                          static_cast<const uint8_t*>(R_uv), n_pairs,
+                                                          static_cast<uint8_t*>(shared_uv), valid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wallet_match(const void* h, size_t n_pairs, uint32_t k, const void* table, const void* nb, const void* note_pk,
+                                const uint8_t* valid, uint8_t* matched, cudaStream_t st) {
+    if (n_pairs == 0) return cudaSuccess;
+    k_wallet_match<<<grid_for(n_pairs), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), n_pairs, k,
+                                                           static_cast<const uint4*>(table), static_cast<const uint8_t*>(nb),
+                                                           static_cast<const uint8_t*>(note_pk), valid, matched);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wallet_select(uint32_t k, const uint8_t* matched, const void* S, const void* h, const void* b,
+                                 const void* R_uv, const void* note_pk, const uint64_t* pos, const void* nonce,
+                                 const void* cipher, const void* C, size_t n, int32_t* owner, void* nullifier, uint64_t* value,
+                                 void* blinder, uint8_t* opened, const WalletRows& dense, unsigned long long* n_owned,
+                                 unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    WalletDense dn{static_cast<uint2*>(dense.meta), static_cast<uint8_t*>(dense.S), static_cast<uint8_t*>(dense.h),
+                   static_cast<uint8_t*>(dense.b), dense.pos, static_cast<uint8_t*>(dense.nonce),
+                   static_cast<uint8_t*>(dense.cipher), static_cast<uint8_t*>(dense.C), dense.valid};
+    k_wallet_select<<<grid_for(n), kThreads, 0, st>>>(
+        k, matched, static_cast<const uint8_t*>(S), static_cast<const uint8_t*>(h), static_cast<const uint8_t*>(b),
+        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(note_pk), pos, static_cast<const uint8_t*>(nonce),
+        static_cast<const uint8_t*>(cipher), static_cast<const uint8_t*>(C), n, owner, static_cast<uint8_t*>(nullifier), value,
+        static_cast<uint8_t*>(blinder), opened, dn, n_owned, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_wallet_scatter(const void* meta, const void* nul, const uint64_t* value_rows, const void* blinder_rows,
+                                  const uint8_t* ok, size_t n_own, void* nullifier, uint64_t* value, void* blinder,
+                                  uint8_t* opened, unsigned long long* totals, cudaStream_t st) {
+    if (n_own == 0) return cudaSuccess;
+    k_wallet_scatter<<<blocks256(n_own), 256, 0, st>>>(static_cast<const uint2*>(meta), static_cast<const uint8_t*>(nul),
+                                                       value_rows, static_cast<const uint8_t*>(blinder_rows), ok, n_own,
+                                                       static_cast<uint8_t*>(nullifier), value, static_cast<uint8_t*>(blinder),
+                                                       opened, totals);
     return cudaGetLastError();
 }
 

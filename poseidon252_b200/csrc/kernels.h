@@ -212,6 +212,40 @@ cudaError_t launch_note_value(const uint64_t* value, const void* blinder, size_t
 cudaError_t launch_note_open_value(const void* rows, const uint8_t* valid, const void* commitment, size_t n, const void* table,
                                    const void* table_p, uint64_t* value, void* blinder, uint8_t* ok,
                                    unsigned long long* n_failed, cudaStream_t st);
+// Multi-key wallet scans (p252_wallet_scan_batch): k keys (a_j, b_j) (canonical 4 x u64), a chunk of n notes, pair p =
+// i k + j for note i and key j.  table / table_p: the fixed-base tables of G and G'.  Counters are device pointers; n_bad and
+// n_invalid may be null.
+// keys: nb[j] = the Niels form of [b_j] G (96 bytes, Montgomery; b = 0 for a bad key), kvalid[j] = a_j, b_j < r_J;
+// *n_owned = 0 (the chunk's owned count, for launch_wallet_select); *n_bad += bad keys
+cudaError_t launch_wallet_keys(const void* a, const void* b, uint32_t k, const void* table, void* nb, uint8_t* kvalid,
+                               unsigned long long* n_owned, unsigned long long* n_bad, cudaStream_t st);
+// dhke: shared_uv[p] = [a_j] R_i as (u, v); valid[p] = kvalid[j] and R_i a curve point with u, v < p, (0, 0) otherwise
+cudaError_t launch_wallet_dhke(const void* a, const uint8_t* kvalid, uint32_t k, const void* R_uv, size_t n_pairs, void* shared_uv,
+                               uint8_t* valid, cudaStream_t st);
+// match: matched[p] = valid[p], both note_pk[i] coordinates < p and note_pk[i] == [h[p]] G + B_j (B_j from nb)
+cudaError_t launch_wallet_match(const void* h, size_t n_pairs, uint32_t k, const void* table, const void* nb, const void* note_pk,
+                                const uint8_t* valid, uint8_t* matched, cudaStream_t st);
+// The dense rows of a chunk's owned notes (row r < *n_owned): meta (uint32 note index, uint32 owner), S (64 bytes), h (32),
+// b (32), pos (8), nonce (32), cipher (96), C (64), valid (1 byte, set to 1)
+struct WalletRows {
+    void *meta, *S, *h, *b;
+    uint64_t* pos;
+    void *nonce, *cipher, *C;
+    uint8_t* valid;
+};
+// select: owner[i] = the smallest j with matched[i k + j] (-1 if none); nullifier, value, blinder and opened rows of note i
+// zeroed; *n_invalid += notes with R not a curve point with u, v < p or a note_pk coordinate >= p; owned notes appended
+// to `dense` at *n_owned (which counts them)
+cudaError_t launch_wallet_select(uint32_t k, const uint8_t* matched, const void* S, const void* h, const void* b,
+                                 const void* R_uv, const void* note_pk, const uint64_t* pos, const void* nonce,
+                                 const void* cipher, const void* C, size_t n, int32_t* owner, void* nullifier, uint64_t* value,
+                                 void* blinder, uint8_t* opened, const WalletRows& dense, unsigned long long* n_owned,
+                                 unsigned long long* n_invalid, cudaStream_t st);
+// scatter: dense row r's nullifier, value, blinder and ok to note meta[r].x; totals[4 owner + 0..3] += value (128-bit, low
+// word first), 1, ok
+cudaError_t launch_wallet_scatter(const void* meta, const void* nul, const uint64_t* value_rows, const void* blinder_rows,
+                                  const uint8_t* ok, size_t n_own, void* nullifier, uint64_t* value, void* blinder,
+                                  uint8_t* opened, unsigned long long* totals, cudaStream_t st);
 // Point compression (p252_points_from_bytes / p252_points_to_bytes): 32-byte encodings <-> (u, v) Montgomery pairs (64
 // bytes).  from: ok[i] = v < p and u^2 a square, an invalid item gets (0, 0); to: ok[i] = u, v < p and on the curve, an
 // invalid item gets 32 bytes of 0xff.  *n_invalid (a device counter, may be null) += invalid items.

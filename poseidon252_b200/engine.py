@@ -852,6 +852,71 @@ class Engine:
         """Items of the last note_open_batch that did not open, invalid ones included (sync() first after async_)."""
         return self._last("note_failed")
 
+    # -- multi-key wallet scans ---------------------------------------------------------------------
+    WALLET_MAX_KEYS = 256
+
+    def wallet_scan_batch(self, a, b, R, note_pk, pos, nonce, cipher, commitment, base, base_p, async_=False):
+        """Which of k keys owns each of n notes, and for owned notes their nullifier, checked opening and per-key totals.
+        a and b (k, 4) p252_jscalar rows (1 <= k <= WALLET_MAX_KEYS; key j is (a_j, B_j = [b_j] base)), R and note_pk
+        (n, 2, 4), pos (n,) (a numpy uint64 array or a CUDA int64 tensor), nonce (n, 4), cipher (n, 3, 4), commitment
+        (n, 2, 4), base (G) and base_p (G') (2, 4) host-read -> (owner (n,) int32, nullifier (n, 4), value (n,), blinder
+        (n, 4), opened (n,) uint8, key_totals (k, 4)).  owner[i] is the smallest j whose key owns note i (-1: none);
+        nullifier, value, blinder and opened are nullifier_batch's and note_open_batch's rows under that key (zeroed for a
+        note no key owns; value and blinder also for an owned note that does not open).  key_totals[j] = (value_lo,
+        value_hi, n_owned, n_opened): the 128-bit sum of the opened values key j owns, and its counts.  Counts:
+        last_wallet_invalid() (notes with R not a curve point or a note_pk coordinate >= p) and last_wallet_bad_keys()
+        (a or b >= r_J).  A base off the curve raises InvalidPoint."""
+        Rp, Rl, flags, Rk = self._in(R, (2, 4))
+        if len(Rl) != 1:
+            raise EngineError(-1, "R must have shape (n, 2, 4)")
+        n = int(Rl[0])
+        ap, al, fa, ak = self._in(a, (4,))
+        bp, bl, fb, bk = self._in(b, (4,))
+        pkp, pkl, fpk, pkk = self._in(note_pk, (2, 4))
+        np_, nl, fn, nk = self._in(nonce, (4,))
+        cp, cl, fc, ck = self._in(cipher, (3, 4))
+        Cp, Cl, fC, Ck = self._in(commitment, (2, 4))
+        self._same_space(flags, fa, fb, fpk, fn, fc, fC, _native.MEM_DEVICE if _is_torch(pos) else _native.MEM_HOST)
+        if len(al) != 1 or not 1 <= int(al[0]) <= self.WALLET_MAX_KEYS:
+            raise EngineError(-1, "a must have shape (k, 4) with 1 <= k <= %d, got leading shape %s"
+                              % (self.WALLET_MAX_KEYS, tuple(al)))
+        k = int(al[0])
+        self._same_lead("b", bl, k)
+        for name, lead in (("note_pk", pkl), ("nonce", nl), ("cipher", cl), ("commitment", Cl)):
+            self._same_lead(name, lead, n)
+        pp, npos, pk = self._idx(pos, Rk, "pos")
+        if npos != n:
+            raise EngineError(-1, "pos must have %d entries, got %d" % (n, npos))
+        g, gp = self._base(base), self._base(base_p)
+        if _is_torch(Rk):
+            import torch
+            owner = torch.empty((n,), dtype=torch.int32, device=Rk.device)
+        else:
+            owner = np.empty((n,), dtype=np.int32)
+        nul = self._result(None, (n, 4), Rk)
+        value = self._result(None, (n,), Rk)
+        blinder = self._result(None, (n, 4), Rk)
+        opened = self._ok_like(Rk, n)
+        if _is_torch(Rk):
+            totals = torch.zeros((k, 4), dtype=Rk.dtype, device=Rk.device)    # n == 0 writes nothing
+        else:
+            totals = np.zeros((k, 4), dtype=np.uint64)
+        flags = self._flags(flags, async_)
+        invalid, bad = self._counter("wallet_invalid", flags), self._counter("wallet_bad_keys", flags)
+        self._check(self._lib.p252_wallet_scan_batch(self._ctx, ap, bp, k, Rp, pkp, pp, np_, cp, Cp, n, g.ctypes.data,
+                                                     gp.ctypes.data, self._ptr(owner), self._ptr(nul), self._ptr(value),
+                                                     self._ptr(blinder), self._ptr(opened), self._ptr(totals),
+                                                     ctypes.byref(invalid), ctypes.byref(bad), flags))
+        return owner, nul, value, blinder, opened, totals
+
+    def last_wallet_invalid(self):
+        """Invalid notes of the last wallet_scan_batch (sync() first after async_)."""
+        return self._last("wallet_invalid")
+
+    def last_wallet_bad_keys(self):
+        """Bad keys of the last wallet_scan_batch (sync() first after async_)."""
+        return self._last("wallet_bad_keys")
+
     # -- point compression ------------------------------------------------------------------------
     def points_from_bytes(self, data, out=None, async_=False):
         """JubJubAffine::from_bytes over a batch: (n, 32) uint8 encodings (host) or (n, 4) 64-bit device tensor of the
