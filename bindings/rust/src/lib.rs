@@ -155,6 +155,10 @@ mod notes;
 // in wallet.rs (methods on Engine).
 mod wallet;
 
+// All-or-nothing batch verification of double-key Schnorr signatures (one MSM over G and G'): its own `extern "C"` block
+// in verify_double_all.rs (a method on Engine).
+mod verify_double_all;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

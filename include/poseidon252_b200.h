@@ -606,6 +606,45 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
                             const p252_fr* R_uv, const p252_fr* msg, const p252_jscalar* weight, size_t n,
                             const p252_fr* base_uv, uint8_t* all_verified, size_t* n_invalid, int flags);
 
+/* ---- All-or-nothing batch verification of double-key Schnorr signatures (SignatureDouble) ---------------------------
+ * One answer for n double-key signatures, by one bucket multi-scalar multiplication over G and G'.  VARIABLE TIME, public
+ * data only, as p252_schnorr_verify_all.  Layouts, challenge2(R, R', m), G_uv / Gp_uv (HOST pointers, a bad one refused
+ * with P252_ERR_INVALID_POINT before anything runs, also for n == 0) and n_public (shared by PK and PK') are those of
+ * p252_schnorr_verify_double_batch; weight and weight_p are p252_jscalar rows in the call's memory space; all_verified is
+ * a HOST pointer and must not be NULL.
+ * Item validity (checked on the device, for both memory spaces): as an invalid item of p252_schnorr_verify_double_batch
+ * (u >= r_J, msg >= p, a coordinate of R or R' >= p, PK or PK' not a curve point with u, v < p), or weight >= r_J, or
+ * weight_p >= r_J.  An invalid item is counted once into *n_invalid and makes the answer 0.  An R or R' with canonical
+ * coordinates off the curve is not invalid, but makes the answer 0 too.
+ * Cofactored semantics: *all_verified = 1 iff no item is invalid, every R and R' is on the curve and
+ *   [8] ( [sum z_i u_i] G + [sum z'_i u_i] G' + sum [z_i c_i] PK_i + sum [z'_i c_i] PK'_i - sum [z_i] R_i - sum [z'_i] R'_i )
+ *   == identity,   c_i = challenge2(R_i, R'_i, msg_i),  z_i = weight[i],  z'_i = weight_p[i].
+ * Except with probability about 2^-128 over independent uniformly random 128-bit weights, that is exactly when every item
+ * satisfies both cofactored equations [8] ([u_i] G + [c_i] PK_i - R_i) == identity and
+ * [8] ([u_i] G' + [c_i] PK'_i - R'_i) == identity.  A signature whose R (or R') is shifted by a small-order point fails
+ * p252_schnorr_verify_double_batch and passes here.
+ * The two weight arrays must be drawn independently: with weight_p == weight the two equations of an item are only
+ * checked as a sum, and a signer can make them fail by opposite amounts that cancel.  (R = [r] G + D and R' = [r] G' - D
+ * for any point D, signed as usual, fail per-item verification and pass the sum with equal weights.)  Weights come from
+ * the caller: uniformly random, unpredictable to the signers and nonzero (128 bits are enough); any z < r_J is accepted,
+ * and a zero weight leaves its equation unchecked.  The library generates no randomness.
+ * n == 0: *all_verified = 1.  n_invalid: optional HOST pointer for both memory spaces (lifetime as for
+ * p252_decrypt_batch).
+ * Batch checks, before anything runs: a NULL buffer with n > 0 (all_verified always), n_public not 1 or n, DEVICE buffers
+ * not 16-byte aligned -> INVALID_ARGUMENT.  With P252_ASYNC, DEVICE calls defer the publication of *n_invalid and
+ * *all_verified to p252_sync; HOST calls return with them published.
+ * The tables of G and G' come from the two cache slots of the double-key calls: this call, schnorr_verify_double_batch and
+ * the double-key signing calls on one context build no table when they alternate, and none of them evicts the one-base
+ * table.  The MSM temporaries live in the context's staging arenas, as for p252_schnorr_verify_all; see DESIGN.md
+ * section 4. */
+/* *all_verified = 1 iff no item is invalid, every R and R' is on the curve, and the cofactored sum above is the identity,
+ * with (PK_i, PK'_i) = (pk_uv, pkp_uv)[n_public == 1 ? 0 : i] */
+int p252_schnorr_verify_double_all(p252_ctx* ctx, const p252_fr* pk_uv, const p252_fr* pkp_uv, size_t n_public,
+                                   const p252_jscalar* u, const p252_fr* R_uv, const p252_fr* Rp_uv, const p252_fr* msg,
+                                   const p252_jscalar* weight, const p252_jscalar* weight_p, size_t n,
+                                   const p252_fr* G_uv, const p252_fr* Gp_uv, uint8_t* all_verified,
+                                   size_t* n_invalid, int flags);
+
 /* One level of an arity-4 tree: parents[i] = Hash::digest(Domain::Merkle4, children[4i..4i+4])
  * (src/hash.rs:22-26). */
 int p252_merkle4_level(p252_ctx* ctx, const p252_fr* children, size_t n_parents, p252_fr* parents, int flags);

@@ -14,7 +14,8 @@
 //   schnorr_verify_batch, nullifier / nullifier_batch, schnorr_sign_double / schnorr_sign_double_batch,
 //   schnorr_verify_double / schnorr_verify_double_batch, note_sign_double_batch, point_from_bytes /
 //   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, value_commit / value_commit_batch,
-//   note_create_batch, note_open / note_open_batch, wallet_scan_batch, jubjub_msm, schnorr_verify_all, merkle4_build.
+//   note_create_batch, note_open / note_open_batch, wallet_scan_batch, jubjub_msm, schnorr_verify_all,
+//   schnorr_verify_double_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -713,6 +714,24 @@ inline bool schnorr_verify_all(const Scalar* pk, size_t n_public, const JubJubSc
                                Engine& e = Engine::default_engine()) {
     uint8_t all = 0;
     check(p252_schnorr_verify_all(e.get(), pk, n_public, u, R, msg, weight, n, base_uv, &all, n_invalid, P252_MEM_HOST),
+          e.get());
+    return all != 0;
+}
+// NEW: all-or-nothing verification of double-key signatures (p252_schnorr_verify_double_all).  VARIABLE TIME: public data
+// only.  true iff no item is invalid, every R and R' is on the curve and [8] ([sum z u] G + [sum z' u] G' + sum [z c] PK
+// + sum [z' c] PK' - sum [z] R - sum [z'] R') is the identity (c = challenge2(R, R', m), z = weight, z' = weight_p):
+// cofactored, so an R shifted by a small-order point passes.  pk and pkp hold 1 or n points each (n_public), R and Rp
+// n x 2 scalars; weight and weight_p hold n caller-chosen random nonzero scalars each (128 bits are enough), drawn
+// independently of each other and unpredictable to the signers.  A G or G' off the curve throws
+// Error(P252_ERR_INVALID_POINT).  n_invalid may be null.
+inline bool schnorr_verify_double_all(const Scalar* pk, const Scalar* pkp, size_t n_public, const JubJubScalar* u,
+                                      const Scalar* R, const Scalar* Rp, const Scalar* msg, const JubJubScalar* weight,
+                                      const JubJubScalar* weight_p, size_t n, const Scalar (&G_uv)[2],
+                                      const Scalar (&Gp_uv)[2], size_t* n_invalid = nullptr,
+                                      Engine& e = Engine::default_engine()) {
+    uint8_t all = 0;
+    check(p252_schnorr_verify_double_all(e.get(), pk, pkp, n_public, u, R, Rp, msg, weight, weight_p, n, G_uv, Gp_uv, &all,
+                                         n_invalid, P252_MEM_HOST),
           e.get());
     return all != 0;
 }

@@ -11,7 +11,8 @@ plus the batch entry points this engine adds:
     stealth_owns_batch (stealth addresses: the sender's note keys and a view key's ownership scan), schnorr_sign /
     schnorr_sign_batch and schnorr_verify / schnorr_verify_batch (Schnorr signatures over JubJub), point_from_bytes /
     points_from_bytes_batch and point_to_bytes / points_to_bytes_batch (JubJub point compression), jubjub_msm
-    (multi-scalar multiplication) and schnorr_verify_all (all-or-nothing batch verification), nullifier /
+    (multi-scalar multiplication), schnorr_verify_all and schnorr_verify_double_all (all-or-nothing batch verification
+    of single- and double-key signatures), nullifier /
     nullifier_batch (Phoenix note nullifiers: which owned notes are spent), schnorr_sign_double /
     schnorr_sign_double_batch, schnorr_verify_double / schnorr_verify_double_batch and note_sign_double_batch (double-key
     Schnorr signatures over G and G', and spending a note under its note secret key), value_commit /
@@ -31,7 +32,7 @@ from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, Inv
                      IOPatternViolation, TooFewInputElements)
 from .hash import Domain, Hash, pack_varlen
 from .merkle import CompactTree, SparseTree, Tree, merkle4_build, merkle4_level
-from .msm import jubjub_msm, schnorr_verify_all
+from .msm import jubjub_msm, schnorr_verify_all, schnorr_verify_double_all
 from .notes import note_create, note_create_batch, note_open, note_open_batch, value_commit, value_commit_batch
 from .nullifier import nullifier, nullifier_batch
 from .points import point_from_bytes, point_to_bytes, points_from_bytes_batch, points_to_bytes_batch
@@ -48,7 +49,7 @@ __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encr
            "encrypt_batch_ephemeral", "stealth_address", "stealth_address_batch", "owns", "stealth_owns_batch",
            "schnorr_sign", "schnorr_sign_batch", "schnorr_verify", "schnorr_verify_batch",
            "point_from_bytes", "point_to_bytes", "points_from_bytes_batch", "points_to_bytes_batch",
-           "jubjub_msm", "schnorr_verify_all", "nullifier", "nullifier_batch",
+           "jubjub_msm", "schnorr_verify_all", "schnorr_verify_double_all", "nullifier", "nullifier_batch",
            "schnorr_sign_double", "schnorr_sign_double_batch", "schnorr_verify_double", "schnorr_verify_double_batch",
            "note_sign_double_batch", "value_commit", "value_commit_batch", "note_create", "note_create_batch",
            "note_open", "note_open_batch", "wallet_scan_batch",

@@ -119,6 +119,9 @@ SIGNATURES = {
     "p252_jubjub_msm": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_schnorr_verify_all": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
                                         c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_schnorr_verify_double_all": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p,
+                                               c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p,
+                                               ctypes.POINTER(c_size_t), c_int]),
 }
 
 MEM_HOST, MEM_DEVICE, ASYNC, TIMING, NO_GATHER = 0, 1, 2, 4, 8

@@ -15,7 +15,7 @@
 //   JubJubAffine::from_bytes / to_bytes (dusk-jubjub, not the reference) -> p252_points_from_bytes, p252_points_to_bytes
 //   Phoenix note nullifiers (consumer, not the reference) -> p252_nullifier_batch
 //   jubjub-schnorr SignatureDouble, Phoenix note signing (consumer, not the reference) -> p252_schnorr_sign_double_batch,
-//     p252_schnorr_verify_double_batch, p252_note_sign_double_batch
+//     p252_schnorr_verify_double_batch, p252_note_sign_double_batch, p252_schnorr_verify_double_all
 //   Phoenix note values (consumer, not the reference) -> p252_value_commit_batch, p252_note_create_batch,
 //     p252_note_open_batch
 //   Error                          src/error.rs:11-44      -> p252_status
@@ -1882,6 +1882,84 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
         if (r != P252_OK) return r;
         return launched(ctx, p252::launch_msm_final(wsum, k, c, nullptr, zsum, (uint32_t)nsum, table, pb ? pkc : nullptr, bad,
                                                     counts.counter(1), ctx->stream));
+    });
+    return counts.end(rc);   // HOST calls return with the answer and the count published
+}
+
+// challenge2(R, R', m) as in p252_schnorr_verify_double_batch.  Per chunk: launch_schnorr_pack_double and the truncated
+// launch_digest (c), then launch_msmv_prep_double writes the chunk's MSM rows (4 per item, 2 for one key pair) and its
+// sums of z u, z' u (and z c, z' c) into the arena, and msm_chunk runs on those rows.  launch_msmv_final_double adds
+// [sum z u] G and [sum z' u] G' from the tables of the double-key slots (and, for one key pair, [sum z c] PK and
+// [sum z' c] PK'), multiplies by the cofactor and writes the answer into device counter 1; counter 0 counts the invalid
+// items.
+int p252_schnorr_verify_double_all(p252_ctx* ctx, const p252_fr* pk_uv, const p252_fr* pkp_uv, size_t n_public,
+                                   const p252_jscalar* u, const p252_fr* R_uv, const p252_fr* Rp_uv, const p252_fr* msg,
+                                   const p252_jscalar* weight, const p252_jscalar* weight_p, size_t n, const p252_fr* G_uv,
+                                   const p252_fr* Gp_uv, uint8_t* all_verified, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !Gp_uv || !all_verified || !one_or_n(n_public, n) ||
+        !args_ok(n, flags, {pk_uv, pkp_uv, u, R_uv, Rp_uv, msg, weight, weight_p}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc;
+    if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
+    p252_fr tag;
+    if ((rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const Counts counts = Counts::device(ctx, flags, n_invalid, nullptr, all_verified);
+    if (n == 0) {
+        *all_verified = 1;
+        return P252_OK;
+    }
+    const void *table = nullptr, *table_p = nullptr;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    const size_t per = pb ? 2 : 4;   // MSM rows per item
+    // 0 PK, 1 PK', 2 u, 3 R, 4 R', 5 msg, 6 weight, 7 weight_p; 8 the digest rows, 9 validity, 10 c, 11 row scalars,
+    // 12 row points and 13 the chunk's MSM temporaries live in the arena only
+    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {pkp_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev},
+                           {R_uv, nullptr, 64, false, dev}, {Rp_uv, nullptr, 64, false, dev}, {msg, nullptr, 32, false, dev},
+                           {weight, nullptr, 32, false, dev}, {weight_p, nullptr, 32, false, dev}, {nullptr, nullptr, 160},
+                           {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 32 * per},
+                           {nullptr, nullptr, 64 * per}, {nullptr, nullptr, 0, true}};
+    const size_t chunk = pipeline_chunk(ios, n), M = chunk * per;
+    const int c = p252::msm_bits(M);
+    const size_t W = (size_t)p252::msm_windows(c), max_chunks = ceil_div(n, chunk) + 3;
+    const size_t nsum = ceil_div(n, p252::kMsmItemsPerSum);
+    ios[13].item_bytes = msm_scratch_bytes(M, c);
+    if ((rc = counts.begin()) != P252_OK) return rc;
+    uint4* wsum = nullptr;
+    uint8_t *zsum = nullptr, *pkc = nullptr;
+    uint32_t* bad = nullptr;
+    rc = with_scratch(ctx, ctx->stream, [&](Carve& cv) {
+        wsum = cv.take<uint4>(max_chunks * W * 8);
+        zsum = cv.take<uint8_t>(nsum * 128);
+        bad = cv.take<uint32_t>(1);
+        pkc = cv.take<uint8_t>(128);
+    }, [&]() -> int {
+        CU(cudaMemsetAsync(bad, 0, sizeof(uint32_t), ctx->stream));
+        if (pb) {
+            CU(cudaMemcpyAsync(pkc, pk_uv, 64, cudaMemcpyDefault, ctx->stream));
+            CU(cudaMemcpyAsync(pkc + 64, pkp_uv, 64, cudaMemcpyDefault, ctx->stream));
+        }
+        uint32_t k = 0;
+        size_t off = 0;
+        int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+            uint8_t* valid = static_cast<uint8_t*>(d[9]);
+            const uint32_t sum0 = (uint32_t)(off / p252::kMsmItemsPerSum);
+            off += cnt;
+            int e = launched(ctx, p252::launch_schnorr_pack_double(d[3], d[4], d[5], cnt, d[8], valid, false, st));
+            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[8], cnt, 5, d[10], 1, true, ctx->coop_max, st));
+            if (e == P252_OK)
+                e = launched(ctx, p252::launch_msmv_prep_double(d[0], d[1], pb, d[2], d[3], d[4], d[10], d[6], d[7], valid,
+                                                                (uint32_t)cnt, d[11], d[12], zsum, sum0, bad,
+                                                                counts.counter(0), st));
+            if (e == P252_OK)
+                e = msm_chunk(ctx, d[11], d[12], cnt * per, c, d[13], M, wsum + (size_t)(k++) * W * 8, nullptr, st);
+            return e;
+        });
+        if (r != P252_OK) return r;
+        return launched(ctx, p252::launch_msmv_final_double(wsum, k, c, zsum, (uint32_t)nsum, table, table_p,
+                                                            pb ? pkc : nullptr, bad, counts.counter(1), ctx->stream));
     });
     return counts.end(rc);   // HOST calls return with the answer and the count published
 }

@@ -13,6 +13,7 @@
 //   note nullifiers (pk' = [(h + b) mod r_J] G', the digest rows [pk'.u, pk'.v, pos]) -> k_nullifier_key
 //   double-key Schnorr signatures over G and G' (SignatureDouble, note signing) -> k_schnorr_pack_double,
 //     k_schnorr_sign_double<Note>, k_schnorr_verify_double
+//   all-or-nothing double-key verification (one MSM over G and G') -> k_msmv_prep_double, k_msmv_final_double
 //   multi-key wallet scans (owner, then nullifier and opening of owned notes) -> k_wallet_keys, k_wallet_dhke,
 //     k_wallet_match, k_wallet_select, k_wallet_scatter
 //   JubJubAffine::from_bytes / to_bytes (point compression) -> k_points_from_bytes, k_points_to_bytes
@@ -2941,6 +2942,271 @@ cudaError_t launch_msmv_prep(const void* pk, bool pk_bcast, const void* u, const
         static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u), static_cast<const uint8_t*>(R_uv),
         static_cast<const uint8_t*>(c), static_cast<const uint8_t*>(z), valid, n, static_cast<uint8_t*>(row_scalars),
         static_cast<uint8_t*>(row_points), static_cast<uint8_t*>(zsum), blk0, bad, n_invalid);
+    return cudaGetLastError();
+}
+
+// ---- all-or-nothing verification of double-key signatures: one MSM over G and G' ---------------------------------------
+// verify_double_all, one thread per item, after k_schnorr_pack_double (valid[i]: R, R' and m canonical) and the truncated
+// digest (c[i]).  The item is valid iff valid[i], u, z, z' < r_J and PK, PK' = (pk, pkp)[pb ? 0 : i] are curve points with
+// u, v < p; an R or R' off the curve is not invalid but fails the batch.  Either sets *bad.  Rows: pb: 2 i = (z, -R) and
+// 2 i + 1 = (z', -R'); otherwise 4 i = (z c, PK), 4 i + 1 = (z' c, PK'), 4 i + 2 = (z, -R), 4 i + 3 = (z', -R').  An
+// invalid item's (and an off-curve R's or R''s) rows are (0, identity).  The block's sums modulo r_J of z u, z' u and, pb,
+// z c, z' c go to zsum[blk0 + block] (128 bytes, in that order).  The checks run first and the rows are written from a
+// second load of each side, so only one side's operands are live at a time.
+__global__ void __launch_bounds__(kMsmThreads) k_msmv_prep_double(const uint8_t* __restrict__ pk,
+                                                                  const uint8_t* __restrict__ pkp, bool pb,
+                                                                  const uint8_t* __restrict__ u,
+                                                                  const uint8_t* __restrict__ R_uv,
+                                                                  const uint8_t* __restrict__ Rp_uv,
+                                                                  const uint8_t* __restrict__ c,
+                                                                  const uint8_t* __restrict__ z,
+                                                                  const uint8_t* __restrict__ zp,
+                                                                  const uint8_t* __restrict__ valid, uint32_t n,
+                                                                  uint8_t* __restrict__ rsc, uint8_t* __restrict__ rpt,
+                                                                  uint8_t* __restrict__ zsum, uint32_t blk0,
+                                                                  uint32_t* __restrict__ bad,
+                                                                  unsigned long long* __restrict__ n_invalid) {
+    __shared__ uint32_t sh[kMsmThreads][32];
+    const uint32_t i = blockIdx.x * kMsmThreads + threadIdx.x;
+#pragma unroll
+    for (int k = 0; k < 32; ++k) sh[threadIdx.x][k] = 0;
+    if (i < n) {
+        // side 0: (z, PK, R); side 1: (z', PK', R')
+        auto key = [&](int side) { return (side ? pkp : pk) + (pb ? 0 : (size_t)i) * 64; };
+        auto wt = [&](int side) { return (side ? zp : z) + (size_t)i * 32; };
+        auto rr = [&](int side) { return (side ? Rp_uv : R_uv) + (size_t)i * 64; };
+        uint32_t one[8], s[8], x[8], y[8], w[8];
+        jj::set_one(one);
+        load_fr(s, u + (size_t)i * 32);
+        bool good = (valid[i] != 0) & jj::below_order(s);
+#pragma unroll 1
+        for (int side = 0; side < 2; ++side) {
+            load_fr(x, key(side));
+            load_fr(y, key(side) + 32);
+            const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
+            const uint32_t mc = 0u - (uint32_t)canon;   // coordinates >= p enter no product
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+            load_fr(w, wt(side));
+            good &= canon & jj::on_curve(x, y) & jj::below_order(w);
+        }
+        const uint32_t mv = 0u - (uint32_t)good;        // an invalid item's R and R' may be >= p: they enter no product
+        bool r_on = true;
+#pragma unroll 1
+        for (int side = 0; side < 2; ++side) {
+            load_fr(x, rr(side));
+            load_fr(y, rr(side) + 32);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mv, y[k] = (y[k] & mv) | (one[k] & ~mv);
+            r_on &= jj::on_curve(x, y);
+        }
+        if (!good || !r_on) *bad = 1u;
+        if (n_invalid) warp_count_every(n_invalid, !good);
+        const uint32_t mg = 0u - (uint32_t)(good & r_on);
+        const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+        uint32_t e[8], t[8];
+        load_fr(e, c + (size_t)i * 32);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] &= mg;
+        const size_t per = pb ? 2 : 4, r0 = per * i + (pb ? 0 : 2);   // the row of (z, -R); (z', -R') follows it
+#pragma unroll 1
+        for (int side = 0; side < 2; ++side) {
+            load_fr(w, wt(side));
+#pragma unroll
+            for (int k = 0; k < 8; ++k) w[k] &= mg;
+            jj::order_mul(t, w, s);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) sh[threadIdx.x][8 * side + k] = t[k];
+            jj::order_mul(t, w, e);                     // c < 2^250 < r_J
+            load_fr(x, rr(side));
+            load_fr(y, rr(side) + 32);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mg, y[k] = (y[k] & mg) | (one[k] & ~mg);
+            uint32_t nx[8];
+            fr_sub_mod(nx, zero, x);
+            store_fr(rsc + (r0 + side) * 32, w);
+            store_fr(rpt + (r0 + side) * 64, nx);
+            store_fr(rpt + (r0 + side) * 64 + 32, y);
+            if (pb) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) sh[threadIdx.x][16 + 8 * side + k] = t[k];
+            } else {
+                load_fr(x, key(side));
+                load_fr(y, key(side) + 32);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) x[k] &= mg, y[k] = (y[k] & mg) | (one[k] & ~mg);
+                store_fr(rsc + (per * i + side) * 32, t);
+                store_fr(rpt + (per * i + side) * 64, x);
+                store_fr(rpt + (per * i + side) * 64 + 32, y);
+            }
+        }
+    }
+    __syncthreads();
+    for (int h = kMsmThreads / 2; h > 0; h >>= 1) {
+        if ((int)threadIdx.x < h) {
+#pragma unroll 1
+            for (int q = 0; q < 4; ++q) {
+                uint32_t a[8], b[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) a[k] = sh[threadIdx.x][8 * q + k], b[k] = sh[threadIdx.x + h][8 * q + k];
+                jj::order_add(a, a, b);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) sh[threadIdx.x][8 * q + k] = a[k];
+            }
+        }
+        __syncthreads();
+    }
+    if (threadIdx.x < 4) {
+        uint32_t a[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) a[k] = sh[0][8 * threadIdx.x + k];
+        store_fr(zsum + (size_t)(blk0 + blockIdx.x) * 128 + threadIdx.x * 32, a);
+    }
+}
+
+// One block of kMsmFinalThreads threads, six warps.  Threads below kMsmThreads first add the nsum 4-tuples of zsum modulo
+// r_J.  Then warps 0-1 add window w's sums of every chunk (thread w < W <= 64), and four walks run on warps of their own,
+// so none waits for another: thread 64 [sum z u] G (table), thread 96 [sum z' u] G' (table_p), and, for one key pair (pk:
+// PK then PK', 128 bytes; null for none), thread 128 [sum z c] PK and thread 160 [sum z' c] PK'.  Thread 0 combines the
+// windows (c doublings each), adds the four points and writes *verified = [8] sum == identity (X == 0, Y == Z) and
+// *bad == 0.
+constexpr int kMsmFinalThreads = 192;
+struct MsmFinalDouble {
+    const uint4* wsum;
+    uint32_t nchunks;
+    int c;
+    const uint8_t* zsum;
+    uint32_t nsum;
+    const uint4* table;
+    const uint4* table_p;
+    const uint8_t* pk;
+    const uint32_t* bad;
+    unsigned long long* verified;
+};
+
+__global__ void __launch_bounds__(kMsmFinalThreads) k_msmv_final_double(MsmFinalDouble a) {
+    __shared__ uint4 sw[64 * 8], sq[4 * 8];
+    __shared__ uint32_t ss[kMsmThreads][32];
+    const int W = jj::msm_windows(a.c), tid = threadIdx.x;
+    if (tid < kMsmThreads) {
+#pragma unroll 1
+        for (int q = 0; q < 4; ++q) {
+            uint32_t x[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+            for (uint32_t k = tid; k < a.nsum; k += kMsmThreads) {
+                uint32_t b[8];
+                load_fr_rw(b, a.zsum + (size_t)k * 128 + q * 32);
+                jj::order_add(x, x, b);
+            }
+#pragma unroll
+            for (int k = 0; k < 8; ++k) ss[tid][8 * q + k] = x[k];
+        }
+    }
+    __syncthreads();
+    for (int h = kMsmThreads / 2; h > 0; h >>= 1) {
+        if (tid < h) {
+#pragma unroll 1
+            for (int q = 0; q < 4; ++q) {
+                uint32_t p[8], r[8];
+#pragma unroll
+                for (int k = 0; k < 8; ++k) p[k] = ss[tid][8 * q + k], r[k] = ss[tid + h][8 * q + k];
+                jj::order_add(p, p, r);
+#pragma unroll
+                for (int k = 0; k < 8; ++k) ss[tid][8 * q + k] = p[k];
+            }
+        }
+        __syncthreads();
+    }
+    if (tid < W) {
+        jj::Ext s, x;
+        jj::set_identity(s);
+        for (uint32_t k = 0; k < a.nchunks; ++k) {
+            jj::Ext p;
+            jj::load_ext(p, a.wsum + ((size_t)k * W + tid) * 8);
+            jj::add_ext(x, s, p);
+            s = x;
+        }
+        jj::store_ext(sw + tid * 8, s);
+    } else if (tid == 64 || tid == 96) {
+        const int side = tid == 96;
+        uint32_t s[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] = ss[0][8 * side + k];
+        jj::Ext t;
+        jj::fixed_base_ext<true, true>(t, s, side ? a.table_p : a.table);
+        jj::store_ext(sq + side * 8, t);
+    } else if (tid == 128 || tid == 160) {
+        const int side = tid == 160;
+        jj::Ext t;
+        if (a.pk) {
+            uint32_t s[8], x[8], y[8], one[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) s[k] = ss[0][16 + 8 * side + k];
+            load_fr(x, a.pk + side * 64);
+            load_fr(y, a.pk + side * 64 + 32);
+            jj::set_one(one);
+            const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
+            uint32_t mc = 0u - (uint32_t)canon;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+            mc = 0u - (uint32_t)jj::on_curve(x, y);    // an off-curve key made every item invalid: *bad is set
+#pragma unroll
+            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc), s[k] &= mc;
+            jj::scalar_mul_ext<true, true>(t, s, x, y);
+        } else {
+            jj::set_identity(t);
+        }
+        jj::store_ext(sq + (2 + side) * 8, t);
+    }
+    __syncthreads();
+    if (tid != 0) return;
+    jj::Ext acc, x;
+    jj::load_ext(acc, sw + (W - 1) * 8);
+    for (int w = W - 2; w >= 0; --w) {
+        for (int d = 0; d < a.c; ++d) {
+            jj::dbl<true>(x, acc);
+            acc = x;
+        }
+        jj::Ext s;
+        jj::load_ext(s, sw + w * 8);
+        jj::add_ext(x, acc, s);
+        acc = x;
+    }
+#pragma unroll 1
+    for (int q = 0; q < 4; ++q) {
+        jj::Ext g;
+        jj::load_ext(g, sq + q * 8);
+        jj::add_ext(x, acc, g);
+        acc = x;
+    }
+    for (int d = 0; d < 3; ++d) {                        // the cofactor
+        jj::dbl<true>(x, acc);
+        acc = x;
+    }
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    const bool ok = jj::feq(acc.X, zero) & jj::feq(acc.Y, acc.Z) & (*a.bad == 0);
+    *a.verified = ok ? 1ull : 0ull;
+}
+
+cudaError_t launch_msmv_prep_double(const void* pk, const void* pkp, bool pk_bcast, const void* u, const void* R_uv,
+                                    const void* Rp_uv, const void* c, const void* z, const void* zp, const uint8_t* valid,
+                                    uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0, uint32_t* bad,
+                                    unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_msmv_prep_double<<<(n + kMsmThreads - 1) / kMsmThreads, kMsmThreads, 0, st>>>(
+        static_cast<const uint8_t*>(pk), static_cast<const uint8_t*>(pkp), pk_bcast, static_cast<const uint8_t*>(u),
+        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(Rp_uv), static_cast<const uint8_t*>(c),
+        static_cast<const uint8_t*>(z), static_cast<const uint8_t*>(zp), valid, n, static_cast<uint8_t*>(row_scalars),
+        static_cast<uint8_t*>(row_points), static_cast<uint8_t*>(zsum), blk0, bad, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_msmv_final_double(const void* wsum, uint32_t nchunks, int c, const void* zsum, uint32_t nsum,
+                                     const void* table, const void* table_p, const void* pk, const uint32_t* bad,
+                                     unsigned long long* verified, cudaStream_t st) {
+    MsmFinalDouble a{static_cast<const uint4*>(wsum), nchunks, c, static_cast<const uint8_t*>(zsum), nsum,
+                     static_cast<const uint4*>(table), static_cast<const uint4*>(table_p), static_cast<const uint8_t*>(pk),
+                     bad, verified};
+    k_msmv_final_double<<<1, kMsmFinalThreads, 0, st>>>(a);
     return cudaGetLastError();
 }
 

@@ -290,6 +290,22 @@ constexpr int kMsmItemsPerSum = 128;
 cudaError_t launch_msmv_prep(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c, const void* z,
                              const uint8_t* valid, uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0,
                              uint32_t* bad, unsigned long long* n_invalid, cudaStream_t st);
+// verify_double_all rows of n items, after launch_schnorr_pack_double (valid) and the truncated digest (c): item i is valid
+// iff valid[i], u, z, zp < r_J and pk, pkp[pk_bcast ? 0 : i] curve points with u, v < p (counted into *n_invalid, device,
+// may be null); an invalid item or an R or R' off the curve sets *bad.  Rows: pk_bcast: 2 i = (z, -R), 2 i + 1 =
+// (zp, -R'); otherwise 4 i = (z c, PK), 4 i + 1 = (zp c, PK'), 4 i + 2 = (z, -R), 4 i + 3 = (zp, -R'); (0, identity) for
+// an invalid item or an off-curve R or R'.  zsum[blk0 + b] (128 bytes) = the sums modulo r_J of z u, zp u and
+// (pk_bcast) z c, zp c over block b of kMsmItemsPerSum items.
+cudaError_t launch_msmv_prep_double(const void* pk, const void* pkp, bool pk_bcast, const void* u, const void* R_uv,
+                                    const void* Rp_uv, const void* c, const void* z, const void* zp, const uint8_t* valid,
+                                    uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0, uint32_t* bad,
+                                    unsigned long long* n_invalid, cudaStream_t st);
+// Adds the chunks' window sums (wsum, nchunks x W) and the nsum 4-tuples of zsum modulo r_J, and writes
+// *verified = [8] (sum + [sum z u] G + [sum zp u] G' + [sum z c] PK + [sum zp c] PK') == identity and *bad == 0
+// (table, table_p: the fixed-base tables of G and G'; pk: one key pair PK, PK' (128 bytes), or null for none)
+cudaError_t launch_msmv_final_double(const void* wsum, uint32_t nchunks, int c, const void* zsum, uint32_t nsum,
+                                     const void* table, const void* table_p, const void* pk, const uint32_t* bad,
+                                     unsigned long long* verified, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

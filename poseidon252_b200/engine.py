@@ -1021,6 +1021,59 @@ class Engine:
         """The answer of the last schnorr_verify_all (sync() first after async_)."""
         return bool(self._last("verify_all"))
 
+    def schnorr_verify_double_all(self, pk, pk_p, u, R, R_p, msg, base, base_p, weights=None, weights_p=None,
+                                  async_=False):
+        """All-or-nothing verification of n double-key signatures by one random linear combination: True iff no item is
+        invalid, every R and R' is on the curve and [8] ([sum z u] base + [sum z' u] base_p + sum [z c] PK
+        + sum [z' c] PK' - sum [z] R - sum [z'] R') is the identity, c = challenge2(R, R', msg).  Except with probability
+        ~2^-128 that is every item passing both cofactored checks of schnorr_verify_double_batch.  Arguments as for
+        schnorr_verify_double_batch; weights and weights_p (n, 4) p252_jscalar rows in the memory space of u, or None for
+        fresh 128-bit weights from `secrets`, one array per equation (the two must be independent: equal weights check
+        only the sum of an item's two equations).  Invalid items (as in schnorr_verify_double_batch, or a weight >= r_J)
+        are counted once in last_schnorr_double_invalid().  VARIABLE TIME (public data only).  async_: returns None;
+        last_verify_double_all() after sync()."""
+        up, ul, flags, uk = self._in(u, (4,))
+        if len(ul) != 1:
+            raise EngineError(-1, "u must have shape (n, 4)")
+        n = int(ul[0])
+        if weights is None:
+            weights = _random_weights(n, uk)
+        if weights_p is None:
+            weights_p = _random_weights(n, uk)
+        pp, pl, fp, _ = self._in(pk, (2, 4))
+        qp, ql, fq, _ = self._in(pk_p, (2, 4))
+        Rp, Rl, fR, _ = self._in(R, (2, 4))
+        Sp, Sl, fS, _ = self._in(R_p, (2, 4))
+        mp, ml, fm, _ = self._in(msg, (4,))
+        wp, wl, fw, wk = self._in(weights, (4,))
+        vp, vl, fv, vk = self._in(weights_p, (4,))
+        self._same_space(flags, fp, fq, fR, fS, fm, fw, fv)
+        if len(pl) != 1 or int(pl[0]) not in (1, n):
+            raise EngineError(-1, "pk must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(pl)))
+        if tuple(ql) != tuple(pl):
+            raise EngineError(-1, "pk_p must have %d rows like pk, got leading shape %s" % (int(pl[0]), tuple(ql)))
+        self._same_lead("R", Rl, n)
+        self._same_lead("R_p", Sl, n)
+        self._same_lead("msg", ml, n)
+        self._same_lead("weights", wl, n)
+        self._same_lead("weights_p", vl, n)
+        g, gp = self._base(base), self._base(base_p)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("schnorr_double_invalid", flags)
+        answer = self._counters["verify_double_all"] = ctypes.c_uint8(0)
+        if flags & _native.ASYNC:
+            self._keep_until_sync(answer)
+            self._keep_until_sync(wk)
+            self._keep_until_sync(vk)
+        self._check(self._lib.p252_schnorr_verify_double_all(self._ctx, pp, qp, int(pl[0]), up, Rp, Sp, mp, wp, vp, n,
+                                                             g.ctypes.data, gp.ctypes.data, ctypes.byref(answer),
+                                                             ctypes.byref(invalid), flags))
+        return None if flags & _native.ASYNC else bool(answer.value)
+
+    def last_verify_double_all(self):
+        """The answer of the last schnorr_verify_double_all (sync() first after async_)."""
+        return bool(self._last("verify_double_all"))
+
     def _crypt_varlen_args(self, data, offsets, secrets_uv, nonces, max_len, key_extra):
         """Shared validation of encrypt_batch_varlen / decrypt_batch_varlen -> (data ptr, n_scalars, offsets ptr, n,
         max_len, secrets ptr, nonces ptr, flags, data keepalive, offsets keepalive, secrets and nonces keepalives).
