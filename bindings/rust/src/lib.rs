@@ -159,6 +159,11 @@ mod wallet;
 // in verify_double_all.rs (a method on Engine).
 mod verify_double_all;
 
+// JubJub ElGamal and the encrypted sender of a Phoenix note: their own `extern "C"` block in elgamal.rs (methods on
+// Engine).
+mod elgamal;
+pub use elgamal::SenderEncryption;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

@@ -544,6 +544,60 @@ int p252_wallet_scan_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jsca
                            p252_fr* nullifier, uint64_t* value, p252_jscalar* blinder, uint8_t* opened, uint64_t* key_totals,
                            size_t* n_invalid, size_t* n_bad_keys, int flags);
 
+/* ---- JubJub ElGamal and the encrypted sender of a Phoenix note (phoenix-core's elgamal, Sender::Encryption) ---------
+ *   elgamal_encrypt(PK, M; r)  = (c1, c2) = ([r] G, M + [r] PK)
+ *   elgamal_decrypt(sk; c1, c2) = c2 - [sk] c1
+ *   sender_encrypt(note_pk; (A, B); (r_A, r_B)) = [encrypt(note_pk, A; r_A), encrypt(note_pk, B; r_B)]
+ *   sender_decrypt(a, b; R, note_pk, enc): note_sk = (hash([a] R) + b) mod r_J (p252_nullifier_batch's note_sk); the note
+ *     is OWNED iff [note_sk] G == note_pk, and then A = c2_A - [note_sk] c1_A, B = c2_B - [note_sk] c1_B
+ * hash(P) = Hash::digest_truncated(Domain::Other, [P.u, P.v])[0], as in the stealth calls; (A, B) is the sender's public
+ * key and (a, b) the receiver's secret key.  Scalar multiplications multiply by the canonical integer; there is no
+ * subgroup check, as in p252_dhke_batch.
+ * ElGamal is NOT authenticated: p252_elgamal_decrypt_batch under a wrong key returns some other curve point with ok = 1.
+ * That is why the sender decrypt checks ownership first: a note the key does not own gets ok = 0 and zeroed A and B rows,
+ * not a plausible-looking wrong sender.
+ * Layouts: scalars p252_jscalar; points (u, v) pairs of p252_fr, outputs affine.  blinder: 2 p252_jscalar per note,
+ * [r_A, r_B]; sender_enc: 8 p252_fr per note (256 bytes), [c1_A, c2_A, c1_B, c2_B] as (u, v) pairs.  n_public (PK),
+ * n_sender (A and B together) and n_secret (sk; a and b together) are 1 or n.  r and the blinders are one per item, with
+ * no broadcast: two messages encrypted under one PK with the same r reveal M1 - M2 (c2 - c2'), so never reuse r.
+ * G_uv is a HOST pointer for every memory space, as for the note calls: a coordinate >= p or a point off the curve is
+ * refused with P252_ERR_INVALID_POINT before anything runs, for every memory space and for n == 0.
+ * p252_elgamal_decrypt_batch takes no G.
+ * Item validity (checked on the device, for both memory spaces):
+ *   encrypt:        r < r_J (each blinder), PK / note_pk and M / A / B curve points with u, v < p.
+ *   decrypt:        sk < r_J (a and b), every ciphertext point a curve point with u, v < p, R a curve point with u, v < p.
+ * r = 0, sk = 0, note_sk = 0, an identity M or PK and small-order points are valid and give what the formulas give.
+ * An invalid item gets ok[i] = 0 and zeroed output rows, and is counted once however many of its checks fail.  In
+ * p252_note_sender_decrypt_batch ok[i] = 0 also means the note is not owned (a note_pk off the curve or with a coordinate
+ * >= p is not owned), and *n_failed counts every item with ok = 0 once, whatever the reason, as p252_note_open_batch
+ * does.  n_invalid / n_failed: optional HOST pointers for both memory spaces.  n == 0 writes and counts nothing.
+ * Batch checks, before anything runs: a NULL buffer with n > 0, n_public / n_sender / n_secret not 1 or n, DEVICE buffers
+ * other than ok not 16-byte aligned -> INVALID_ARGUMENT.
+ * Secrets: r, the blinders, M, (A, B), sk, a, b, [a] R, its hash and note_sk live only in the context's staging arenas,
+ * for both memory spaces, and the arenas are zeroed on every exit path: all four calls are synchronous (P252_ASYNC only
+ * defers the publication of the count to p252_sync).  Each item is constant time (no branch and no address depends on a
+ * secret); see DESIGN.md section 4.
+ * G's fixed-base table is the first of the double-key and note calls' two cache slots: after p252_note_create_batch with
+ * the same G the encrypt calls and the sender decrypt build no table, and none of them evicts G' or the one-base table. */
+/* c1_uv[i], c2_uv[i] = elgamal_encrypt(pk_uv[n_public == 1 ? 0 : i], msg_uv[i]; r[i]) */
+int p252_elgamal_encrypt_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_fr* msg_uv,
+                               const p252_jscalar* r, size_t n, const p252_fr* G_uv, p252_fr* c1_uv, p252_fr* c2_uv,
+                               uint8_t* ok, size_t* n_invalid, int flags);
+/* msg_uv[i] = elgamal_decrypt(sk[n_secret == 1 ? 0 : i]; c1_uv[i], c2_uv[i]) */
+int p252_elgamal_decrypt_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_fr* c1_uv,
+                               const p252_fr* c2_uv, size_t n, p252_fr* msg_uv, uint8_t* ok, size_t* n_invalid, int flags);
+/* sender_enc[8 i .. 8 i + 7] = sender_encrypt(note_pk_uv[i]; (sender_A_uv, sender_B_uv)[n_sender == 1 ? 0 : i];
+ *   (blinder[2 i], blinder[2 i + 1])) */
+int p252_note_sender_encrypt_batch(p252_ctx* ctx, const p252_fr* note_pk_uv, const p252_fr* sender_A_uv,
+                                   const p252_fr* sender_B_uv, size_t n_sender, const p252_jscalar* blinder, size_t n,
+                                   const p252_fr* G_uv, p252_fr* sender_enc, uint8_t* ok, size_t* n_invalid, int flags);
+/* sender_A_uv[i], sender_B_uv[i], ok[i] = sender_decrypt((a, b)[n_secret == 1 ? 0 : i]; R_uv[i], note_pk_uv[i],
+ *   sender_enc[8 i .. 8 i + 7]) */
+int p252_note_sender_decrypt_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
+                                   const p252_fr* R_uv, const p252_fr* note_pk_uv, const p252_fr* sender_enc, size_t n,
+                                   const p252_fr* G_uv, p252_fr* sender_A_uv, p252_fr* sender_B_uv, uint8_t* ok,
+                                   size_t* n_failed, int flags);
+
 /* ---- JubJub point compression (dusk-jubjub's JubJubAffine::to_bytes / from_bytes) -----------------------------------
  *   encoding:  the 32 little-endian bytes of canonical v, with bit 255 (bytes[31] >> 7) = the low bit of canonical u
  *   decoding:  sign = bit 255, cleared; the remaining 255-bit value is v (rejected if >= p); u^2 = (v^2 - 1) / (1 + d v^2)

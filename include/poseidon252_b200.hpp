@@ -14,7 +14,8 @@
 //   schnorr_verify_batch, nullifier / nullifier_batch, schnorr_sign_double / schnorr_sign_double_batch,
 //   schnorr_verify_double / schnorr_verify_double_batch, note_sign_double_batch, point_from_bytes /
 //   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, value_commit / value_commit_batch,
-//   note_create_batch, note_open / note_open_batch, wallet_scan_batch, jubjub_msm, schnorr_verify_all,
+//   note_create_batch, note_open / note_open_batch, wallet_scan_batch, elgamal_encrypt_batch, elgamal_decrypt_batch,
+//   note_sender_encrypt_batch, note_sender_decrypt_batch, jubjub_msm, schnorr_verify_all,
 //   schnorr_verify_double_all, merkle4_build.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
@@ -695,6 +696,60 @@ inline WalletScan wallet_scan_batch(const JubJubScalar* a, const JubJubScalar* b
                                  &w.n_invalid, &w.n_bad_keys, P252_MEM_HOST),
           e.get());
     return w;
+}
+
+// NEW: JubJub ElGamal and the encrypted sender of a Phoenix note (p252_elgamal_encrypt_batch / p252_elgamal_decrypt_batch /
+// p252_note_sender_encrypt_batch / p252_note_sender_decrypt_batch): (c1, c2) = ([r] G, M + [r] PK), M = c2 - [sk] c1
+// (NOT authenticated: a wrong key gives another point); the sender field is [(c1_A, c2_A), (c1_B, c2_B)] under note_pk,
+// opened with note_sk = (hash([a] R) + b) mod r_J only where [note_sk] G == note_pk.  Points are n x 2 scalars; pk, A and
+// B hold 1 or n points (n_public / n_sender), sk, a and b 1 or n keys (n_secret); r one per message and blinder two per
+// note [r_A, r_B], never reused.  G_uv off the curve throws Error(P252_ERR_INVALID_POINT).  ok[i] == 0 marks an item
+// with zeroed rows (invalid; for the sender decrypt also not owned); the counts may be null.
+inline std::vector<uint8_t> elgamal_encrypt_batch(const Scalar* pk, size_t n_public, const Scalar* msg, const JubJubScalar* r,
+                                                  size_t n, const Scalar (&G_uv)[2], std::vector<Scalar>& c1,
+                                                  std::vector<Scalar>& c2, size_t* n_invalid = nullptr,
+                                                  Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok(n, 0);
+    c1.assign(2 * n, Scalar{});
+    c2.assign(2 * n, Scalar{});
+    check(p252_elgamal_encrypt_batch(e.get(), pk, n_public, msg, r, n, G_uv, c1.data(), c2.data(), ok.data(), n_invalid,
+                                     P252_MEM_HOST),
+          e.get());
+    return ok;
+}
+inline std::vector<Scalar> elgamal_decrypt_batch(const JubJubScalar* sk, size_t n_secret, const Scalar* c1, const Scalar* c2,
+                                                 size_t n, std::vector<uint8_t>& ok, size_t* n_invalid = nullptr,
+                                                 Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> msg(2 * n);
+    ok.assign(n, 0);
+    check(p252_elgamal_decrypt_batch(e.get(), sk, n_secret, c1, c2, n, msg.data(), ok.data(), n_invalid, P252_MEM_HOST),
+          e.get());
+    return msg;
+}
+// enc receives 8 scalars per note: [c1_A, c2_A, c1_B, c2_B]
+inline std::vector<uint8_t> note_sender_encrypt_batch(const Scalar* note_pk, const Scalar* A, const Scalar* B, size_t n_sender,
+                                                      const JubJubScalar* blinder, size_t n, const Scalar (&G_uv)[2],
+                                                      std::vector<Scalar>& enc, size_t* n_invalid = nullptr,
+                                                      Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok(n, 0);
+    enc.assign(8 * n, Scalar{});
+    check(p252_note_sender_encrypt_batch(e.get(), note_pk, A, B, n_sender, blinder, n, G_uv, enc.data(), ok.data(),
+                                         n_invalid, P252_MEM_HOST),
+          e.get());
+    return ok;
+}
+inline std::vector<uint8_t> note_sender_decrypt_batch(const JubJubScalar* a, const JubJubScalar* b, size_t n_secret,
+                                                      const Scalar* R, const Scalar* note_pk, const Scalar* enc, size_t n,
+                                                      const Scalar (&G_uv)[2], std::vector<Scalar>& A,
+                                                      std::vector<Scalar>& B, size_t* n_failed = nullptr,
+                                                      Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> ok(n, 0);
+    A.assign(2 * n, Scalar{});
+    B.assign(2 * n, Scalar{});
+    check(p252_note_sender_decrypt_batch(e.get(), a, b, n_secret, R, note_pk, enc, n, G_uv, A.data(), B.data(), ok.data(),
+                                         n_failed, P252_MEM_HOST),
+          e.get());
+    return ok;
 }
 
 // NEW: multi-scalar multiplication and all-or-nothing Schnorr batch verification (p252_jubjub_msm /

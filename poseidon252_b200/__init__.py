@@ -18,7 +18,9 @@ plus the batch entry points this engine adds:
     Schnorr signatures over G and G', and spending a note under its note secret key), value_commit /
     value_commit_batch, note_create / note_create_batch and note_open / note_open_batch (Phoenix note values: Pedersen
     commitments, creating obfuscated notes and their checked opening), wallet_scan_batch (which of several keys owns each
-    note, with the owned notes' nullifiers, checked openings and per-key totals), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
+    note, with the owned notes' nullifiers, checked openings and per-key totals), elgamal_encrypt / elgamal_encrypt_batch,
+    elgamal_decrypt / elgamal_decrypt_batch, note_sender_encrypt_batch and note_sender_decrypt /
+    note_sender_decrypt_batch (JubJub ElGamal and the encrypted sender of a Phoenix note), merkle4_build, Tree (fixed-height Merkle tree with batched appends / overwrites), SparseTree (fixed-height Merkle tree
     with batched inserts / removals at any position).
 All computation runs in hand-written sm_90a CUDA behind the C ABI in include/poseidon252_b200.h.
 """
@@ -27,6 +29,8 @@ from .encryption import (cipher_offsets, decrypt, decrypt_batch, decrypt_batch_d
                          encrypt, encrypt_batch, encrypt_batch_dhke, encrypt_batch_ephemeral, encrypt_batch_varlen,
                          fixed_base, fixed_base_batch, message_offsets, owns, stealth_address, stealth_address_batch,
                          stealth_owns_batch)
+from .elgamal import (elgamal_decrypt, elgamal_decrypt_batch, elgamal_encrypt, elgamal_encrypt_batch,
+                      note_sender_decrypt, note_sender_decrypt_batch, note_sender_encrypt_batch)
 from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
@@ -52,7 +56,9 @@ __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encr
            "jubjub_msm", "schnorr_verify_all", "schnorr_verify_double_all", "nullifier", "nullifier_batch",
            "schnorr_sign_double", "schnorr_sign_double_batch", "schnorr_verify_double", "schnorr_verify_double_batch",
            "note_sign_double_batch", "value_commit", "value_commit_batch", "note_create", "note_create_batch",
-           "note_open", "note_open_batch", "wallet_scan_batch",
+           "note_open", "note_open_batch", "wallet_scan_batch", "elgamal_encrypt", "elgamal_encrypt_batch",
+           "elgamal_decrypt", "elgamal_decrypt_batch", "note_sender_encrypt_batch", "note_sender_decrypt",
+           "note_sender_decrypt_batch",
            "hades", "merkle", "scalar", "Engine", "default_engine", "merkle4_build", "merkle4_level", "Tree", "SparseTree",
            "CompactTree",
            "IOPatternViolation", "InvalidIOPattern", "TooFewInputElements", "EncryptionFailed",

@@ -114,6 +114,15 @@ SIGNATURES = {
                                        c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p,
                                        c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), ctypes.POINTER(c_size_t),
                                        c_int]),
+    "p252_elgamal_encrypt_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_size_t, c_void_p,
+                                           c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_elgamal_decrypt_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_size_t, c_void_p,
+                                           c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_note_sender_encrypt_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t,
+                                               c_void_p, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
+    "p252_note_sender_decrypt_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_void_p,
+                                               c_size_t, c_void_p, c_void_p, c_void_p, c_void_p,
+                                               ctypes.POINTER(c_size_t), c_int]),
     "p252_points_from_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_points_to_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_jubjub_msm": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, ctypes.POINTER(c_size_t), c_int]),

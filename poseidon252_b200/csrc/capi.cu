@@ -18,6 +18,8 @@
 //     p252_schnorr_verify_double_batch, p252_note_sign_double_batch, p252_schnorr_verify_double_all
 //   Phoenix note values (consumer, not the reference) -> p252_value_commit_batch, p252_note_create_batch,
 //     p252_note_open_batch
+//   JubJub ElGamal, the encrypted sender of a Phoenix note (consumer, not the reference) -> p252_elgamal_encrypt_batch,
+//     p252_elgamal_decrypt_batch, p252_note_sender_encrypt_batch, p252_note_sender_decrypt_batch
 //   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -1668,6 +1670,121 @@ int p252_wallet_scan_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jsca
         rc = with_scratch(ctx, ctx->stream, [&](Carve& c) { tot = c.take<unsigned long long>(4 * n_keys); },
                           [&] { return scan(tot); });
     }
+    return counts.end(rc);
+}
+
+// ---- JubJub ElGamal and the encrypted sender of a Phoenix note --------------------------------------------------------
+// encrypt: (c1, c2) = ([r] G, M + [r] PK); decrypt: M = c2 - [sk] c1.  The sender field is two encryptions under note_pk,
+// [(c1_A, c2_A), (c1_B, c2_B)], opened with note_sk = (hash([a] R) + b) mod r_J after an ownership check
+// [note_sk] G == note_pk.  encrypt, sender encrypt and decrypt: one launch per chunk (launch_elgamal_encrypt,
+// launch_note_sender_encrypt, launch_elgamal_decrypt).  sender decrypt: launch_dhke ([a] R and its validity into a slot
+// arena), the truncated launch_digest of it (h, the stealth calls' hash) into the arena, then launch_note_sender_decrypt,
+// as p252_nullifier_batch does.  r, the blinders, M, (A, B), sk, a, b, [a] R, h and note_sk live only in the slot arenas
+// for both memory spaces, so all four calls are synchronous and the common exit join_slots(wipe) clears them on every
+// path.  G's fixed-base table is the double-key and note calls' first cache slot (ctx->bt2[0]): after a note call with
+// the same G these calls build no table, and they evict neither G' nor the single-base slot.
+int p252_elgamal_encrypt_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public, const p252_fr* msg_uv,
+                               const p252_jscalar* r, size_t n, const p252_fr* G_uv, p252_fr* c1_uv, p252_fr* c2_uv,
+                               uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !one_or_n(n_public, n) || !args_ok(n, flags, {pk_uv, msg_uv, r, c1_uv, c2_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(G_uv);
+    if (rc != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 PK, 1 M, 2 r, 3 c1, 4 c2, 5 ok
+    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {msg_uv, nullptr, 64, false, dev}, {r, nullptr, 32, false, dev},
+                           {nullptr, c1_uv, 64, false, dev}, {nullptr, c2_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_elgamal_encrypt(d[0], pb, d[1], false, d[2], cnt, table, d[3], d[4],
+                                                          static_cast<uint8_t*>(d[5]), counts.counter(0), st));
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+int p252_elgamal_decrypt_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_fr* c1_uv,
+                               const p252_fr* c2_uv, size_t n, p252_fr* msg_uv, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !one_or_n(n_secret, n) || !args_ok(n, flags, {sk, c1_uv, c2_uv, msg_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    int rc = counts.begin();
+    if (rc != P252_OK) return rc;
+    // 0 sk, 1 c1, 2 c2, 3 M, 4 ok
+    std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {c1_uv, nullptr, 64, false, dev}, {c2_uv, nullptr, 64, false, dev},
+                           {nullptr, msg_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_elgamal_decrypt(d[0], sb, d[1], d[2], cnt, d[3], static_cast<uint8_t*>(d[4]),
+                                                          counts.counter(0), st));
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+int p252_note_sender_encrypt_batch(p252_ctx* ctx, const p252_fr* note_pk_uv, const p252_fr* sender_A_uv,
+                                   const p252_fr* sender_B_uv, size_t n_sender, const p252_jscalar* blinder, size_t n,
+                                   const p252_fr* G_uv, p252_fr* sender_enc, uint8_t* ok, size_t* n_invalid, int flags) {
+    if (!ctx || !G_uv || !one_or_n(n_sender, n) ||
+        !args_ok(n, flags, {note_pk_uv, sender_A_uv, sender_B_uv, blinder, sender_enc}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(G_uv);
+    if (rc != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_sender == 1;
+    const Counts counts(ctx, flags, n_invalid, ok, n);
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 note_pk, 1 A, 2 B, 3 blinders, 4 sender_enc, 5 ok
+    std::vector<Io> ios = {{note_pk_uv, nullptr, 64, false, dev}, {sender_A_uv, nullptr, 64, sb, dev},
+                           {sender_B_uv, nullptr, 64, sb, dev}, {blinder, nullptr, 64, false, dev},
+                           {nullptr, sender_enc, 256, false, dev}, {nullptr, ok, 1, false, dev}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_note_sender_encrypt(d[0], d[1], d[2], sb, d[3], cnt, table, d[4],
+                                                              static_cast<uint8_t*>(d[5]), counts.counter(0), st));
+    }, /*wipe=*/true);
+    return counts.end(rc);
+}
+
+int p252_note_sender_decrypt_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
+                                   const p252_fr* R_uv, const p252_fr* note_pk_uv, const p252_fr* sender_enc, size_t n,
+                                   const p252_fr* G_uv, p252_fr* sender_A_uv, p252_fr* sender_B_uv, uint8_t* ok,
+                                   size_t* n_failed, int flags) {
+    if (!ctx || !G_uv || !one_or_n(n_secret, n) ||
+        !args_ok(n, flags, {a, b, R_uv, note_pk_uv, sender_enc, sender_A_uv, sender_B_uv}, {ok}))
+        return P252_ERR_INVALID_ARGUMENT;
+    int rc = base_check(G_uv);
+    p252_fr tag_h;
+    if (rc != P252_OK || (rc = stealth_tag(&tag_h)) != P252_OK) return rc;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const Counts counts(ctx, flags, n_failed, ok, n);
+    if (n == 0) return P252_OK;
+    const void* table = nullptr;
+    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
+    // 0 a, 1 b, 2 R, 3 note_pk, 4 sender_enc, 5 A, 6 B, 7 ok; 8 shared points, 9 validity and 10 h live in the arena only
+    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev},
+                           {note_pk_uv, nullptr, 64, false, dev}, {sender_enc, nullptr, 256, false, dev},
+                           {nullptr, sender_A_uv, 64, false, dev}, {nullptr, sender_B_uv, 64, false, dev},
+                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
+    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        uint8_t* valid = static_cast<uint8_t*>(d[9]);
+        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[2], false, cnt, d[8], valid, nullptr, st));
+        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[8], cnt, 2, d[10], 1, true, ctx->coop_max, st));
+        if (e == P252_OK)
+            e = launched(ctx, p252::launch_note_sender_decrypt(d[10], d[1], sb, valid, d[3], d[4], cnt, table, d[5], d[6],
+                                                               static_cast<uint8_t*>(d[7]), counts.counter(0), st));
+        return e;
+    }, /*wipe=*/true);
     return counts.end(rc);
 }
 

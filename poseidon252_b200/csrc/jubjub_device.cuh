@@ -243,14 +243,10 @@ __device__ __forceinline__ void window_step(Ext& acc, Cached& c, const Entry (&t
     acc = t;
 }
 
-// acc = [s] (u, v) in extended coordinates for s < 2^252 (canonical words) and an on-curve (u, v) with u, v < p
-// (Montgomery).  Fixed 4-bit window: the 16-entry table of (u, v) in thread-local memory, then 63 window_steps.
-// kPublic: s is public (signature verification), so each window reads only its entry; a secret s (the key exchange)
-// must not, and reads all 16.  kLastT: the last window also computes T, for a caller that adds another point to acc.
-template <bool kPublic, bool kLastT>
-__device__ __forceinline__ void scalar_mul_ext(Ext& acc, const uint32_t (&s)[8], const uint32_t (&u)[8], const uint32_t (&v)[8]) {
-    Entry tab[16];
-    Cached c;
+// tab[j] = [j] (u, v), j < 16, in cached form, for an on-curve (u, v) with u, v < p (Montgomery): T and 2d T of the input
+// 2, entries 2..15 14 x (8 + 1) products.  acc and c are the build's temporaries.
+__device__ __forceinline__ void var_table(Entry (&tab)[16], Ext& acc, Cached& c, const uint32_t (&u)[8],
+                                          const uint32_t (&v)[8]) {
     // tab[0] = identity (0 : 1 : 1 : 0) cached = (1, 1, 0, 2)
     set_one(c.ymx);
     set_one(c.ypx);
@@ -275,7 +271,11 @@ __device__ __forceinline__ void scalar_mul_ext(Ext& acc, const uint32_t (&s)[8],
         to_cached(c, acc);
         store_entry(tab[j], c);
     }
-    // acc = identity
+}
+
+// acc = [s] P from the identity over the table of P (var_table), 63 window_steps; c is the windows' temporary.
+template <bool kPublic, bool kLastT>
+__device__ __forceinline__ void var_walk(Ext& acc, Cached& c, const Entry (&tab)[16], const uint32_t (&s)[8]) {
 #pragma unroll
     for (int k = 0; k < 8; ++k) acc.X[k] = 0, acc.T[k] = 0;
     set_one(acc.Y);
@@ -283,6 +283,18 @@ __device__ __forceinline__ void scalar_mul_ext(Ext& acc, const uint32_t (&s)[8],
 #pragma unroll 1
     for (int w = kWindows - 1; w >= (kLastT ? 1 : 0); --w) window_step<kPublic, false>(acc, c, tab, s, w);
     if (kLastT) window_step<kPublic, true>(acc, c, tab, s, 0);
+}
+
+// acc = [s] (u, v) in extended coordinates for s < 2^252 (canonical words) and an on-curve (u, v) with u, v < p
+// (Montgomery).  Fixed 4-bit window: the 16-entry table of (u, v) in thread-local memory, then 63 window_steps.
+// kPublic: s is public (signature verification), so each window reads only its entry; a secret s (the key exchange)
+// must not, and reads all 16.  kLastT: the last window also computes T, for a caller that adds another point to acc.
+template <bool kPublic, bool kLastT>
+__device__ __forceinline__ void scalar_mul_ext(Ext& acc, const uint32_t (&s)[8], const uint32_t (&u)[8], const uint32_t (&v)[8]) {
+    Entry tab[16];
+    Cached c;
+    var_table(tab, acc, c, u, v);
+    var_walk<kPublic, kLastT>(acc, c, tab, s);
 }
 
 // (ou, ov) = [s] (u, v), affine, for a secret s: scalar_mul_ext with masked table reads, then one inversion.
@@ -515,6 +527,70 @@ constexpr int kProductsPerWalletOwned = kProductsPerNullifierKey + kProductsPerN
 static_assert(kProductsPerWalletKey == 868, "product count of DESIGN.md section 4");
 static_assert(kProductsPerWalletPair == 3275, "product count of DESIGN.md section 4");
 static_assert(kProductsPerWalletOwned == 1435, "product count of DESIGN.md section 4");
+
+// ---- JubJub ElGamal (p252_elgamal_{encrypt,decrypt}_batch, p252_note_sender_{encrypt,decrypt}_batch) --------------------
+// encrypt (kPairs pairs under one PK): (c1_j, c2_j) = ([r_j] G, M_j + [r_j] PK).  PK's on-curve check 4 and its 16-entry
+//   table 2 + 14 x 9 once; per pair M_j's on-curve check 4, [r_j] PK by the walk with T in the last window (62 x 36 + 37),
+//   M_j's Niels form 2 and one mixed addition without T 6, [r_j] G by the fixed-base walk (63 x 7 + 6); then the 2 kPairs
+//   outputs become affine with one shared inversion (batch_affine).
+// decrypt: M = c2 - [sk] c1 = c2 + [sk] (-c1).  Both points' on-curve checks 8, the table of -c1 (negating u costs no
+//   product), the walk with T in the last window, c2's Niels form and the mixed addition, one inversion, affine 2.
+// note decrypt: note_sk = (h + b) mod r_J (order_add, no product) after k_dhke and the truncated digest; the four
+//   ciphertext points' on-curve checks 16; ownership [note_sk] G (63 x 7 + 6) compared projectively with note_pk (2);
+//   per pair the decrypt's table, walk and addition; one shared inversion for both outputs.
+template <int kN>
+constexpr int batch_affine_products() { return 3 * (kN - 1) + (kPm2Bits - 1) + (kPm2Ones - 1) + 2 * kN; }
+constexpr int kProductsPerVarWalkT = 2 + 14 * 9 + (kWindows - 1) * (3 * 7 + 8 + 7) + (3 * 7 + 8 + 8);
+constexpr int kProductsPerFbWalk = (kFbWindows - 1) * 7 + 6;
+template <int kPairs>
+constexpr int elgamal_enc_products() {
+    return 4 + (2 + 14 * 9) + kPairs * (4 + (kProductsPerVarWalkT - 2 - 14 * 9) + 2 + 6 + kProductsPerFbWalk) +
+           batch_affine_products<2 * kPairs>();
+}
+constexpr int kProductsPerElGamalEnc = elgamal_enc_products<1>();
+constexpr int kProductsPerSenderEnc = elgamal_enc_products<2>();
+constexpr int kProductsPerElGamalDec = 8 + kProductsPerVarWalkT + 2 + 6 + batch_affine_products<1>();
+constexpr int kProductsPerSenderDec = 16 + kProductsPerFbWalk + 2 + 2 * (kProductsPerVarWalkT + 2 + 6) + batch_affine_products<2>();
+static_assert(kProductsPerVarWalkT == 2397, "product count of DESIGN.md section 4");
+static_assert(kProductsPerElGamalEnc == 3284, "product count of DESIGN.md section 4");
+static_assert(kProductsPerSenderEnc == 6022, "product count of DESIGN.md section 4");
+static_assert(kProductsPerElGamalDec == 2832, "product count of DESIGN.md section 4");
+static_assert(kProductsPerSenderDec == 5699, "product count of DESIGN.md section 4");
+
+struct Proj {                   // (X : Y : Z) of a result waiting for the shared inversion
+    uint32_t X[8], Y[8], Z[8];
+};
+__device__ __forceinline__ void park(Proj& p, const Ext& e) {
+    fcopy(p.X, e.X);
+    fcopy(p.Y, e.Y);
+    fcopy(p.Z, e.Z);
+}
+
+// Montgomery's trick: p[k] = (X_k / Z_k, Y_k / Z_k, -) for Z_k != 0, written back into X and Y, with one inversion:
+// prefix products kN - 1, the inversion, two products per step back kN - 1, affine 2 kN.  The loops run over public
+// counters: the same schedule for every item.
+template <int kN>
+__device__ __forceinline__ void batch_affine(Proj (&p)[kN]) {
+    uint32_t pre[kN][8], inv[8], zi[8], t[8];
+    fcopy(pre[0], p[0].Z);
+#pragma unroll
+    for (int k = 1; k < kN; ++k) fmul(pre[k], pre[k - 1], p[k].Z);
+    inverse(inv, pre[kN - 1]);
+#pragma unroll
+    for (int k = kN - 1; k >= 0; --k) {
+        if (k > 0) {
+            fmul(zi, inv, pre[k - 1]);      // 1 / Z_k
+            fmul(t, inv, p[k].Z);           // 1 / (Z_0 ... Z_{k-1})
+            fcopy(inv, t);
+        } else {
+            fcopy(zi, inv);
+        }
+        fmul(t, p[k].X, zi);
+        fcopy(p[k].X, t);
+        fmul(t, p[k].Y, zi);
+        fcopy(p[k].Y, t);
+    }
+}
 
 // Arithmetic modulo r_J on 8 x 32-bit little-endian words, Montgomery form with R = 2^256.  Constants (immediates, as
 // P252_JJ_ORDER): R^2 mod r_J and kOrderInv = -r_J^-1 mod 2^32.  Constant time: no branch and no address depends on an

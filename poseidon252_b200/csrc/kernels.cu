@@ -2430,6 +2430,230 @@ cudaError_t launch_wallet_scatter(const void* meta, const void* nul, const uint6
     return cudaGetLastError();
 }
 
+// ---- JubJub ElGamal: (c1, c2) = ([r] G, M + [r] PK), M = c2 - [sk] c1 (jubjub_device.cuh) -----------------------------
+// Whether the point row at p, loaded into (u, v), is a curve point with u, v < p
+__device__ __forceinline__ bool load_point(uint32_t (&u)[8], uint32_t (&v)[8], const uint8_t* p) {
+    load_fr(u, p);
+    load_fr(v, p + 32);
+    return fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
+}
+// (u, v) = m ? (u, v) : the identity (0, 1), for an all-ones or all-zeros mask m
+__device__ __forceinline__ void mask_point(uint32_t (&u)[8], uint32_t (&v)[8], uint32_t m) {
+    uint32_t one[8];
+    jj::set_one(one);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= m, v[k] = (v[k] & m) | (one[k] & ~m);
+}
+
+// One thread per item, jj::elgamal_enc_products<kPairs>() products.  Item i reads PK = pk[pb ? 0 : i], and for each pair
+// j < kPairs the message M_j = (j ? m1 : m0)[mb ? 0 : i] and r_j = r[kPairs i + j] (canonical 4 x u64); points are (u, v)
+// Montgomery pairs.  c1_j goes to c1 + i stride + 128 j, c2_j to c2 + i stride + 128 j: the generic call has kPairs = 1,
+// c1 and c2 two arrays of 64-byte rows; the sender call has kPairs = 2 and rows of 256 bytes [c1_A, c2_A, c1_B, c2_B]
+// with c2 = c1 + 64.  valid iff every r_j < r_J and PK and every M_j are curve points with u, v < p; an invalid item runs
+// the same schedule on r = 0 and identities, writes zeroed rows and ok = 0, and is counted once.  r and M are secret:
+// the table reads of both walks are masked selects, and the points are parked in thread-local memory (never in the
+// caller's buffers) until the shared inversion.
+template <int kPairs>
+__global__ void __launch_bounds__(kThreads, 3) k_elgamal_enc(const uint8_t* __restrict__ pk, bool pb,
+                                                          const uint8_t* __restrict__ m0, const uint8_t* __restrict__ m1,
+                                                          bool mb, const uint8_t* __restrict__ r, size_t n,
+                                                          const uint4* __restrict__ table, uint8_t* c1, uint8_t* c2,
+                                                          uint32_t stride, uint8_t* __restrict__ ok,
+                                                          unsigned long long* __restrict__ n_invalid) {
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    const uint8_t* mi0 = m0 + (mb ? 0 : i) * 64;
+    const uint8_t* mi1 = kPairs == 2 ? m1 + (mb ? 0 : i) * 64 : mi0;
+    const uint8_t* ri = r + i * kPairs * 32;
+    uint32_t u[8], v[8], s[8];
+    bool valid = load_point(u, v, pk + (pb ? 0 : i) * 64);
+#pragma unroll
+    for (int j = 0; j < kPairs; ++j) {
+        uint32_t mu[8], mv[8];
+        valid &= load_point(mu, mv, j ? mi1 : mi0);
+        load_fr(s, ri + j * 32);
+        valid &= jj::below_order(s);
+    }
+    const uint32_t m = 0u - (uint32_t)valid;
+    mask_point(u, v, m);
+    jj::Entry tab[16];
+    jj::Cached c;
+    {
+        jj::Ext acc;
+        jj::var_table(tab, acc, c, u, v);
+    }
+    jj::Proj out[2 * kPairs];   // c1_j at 2 j, c2_j at 2 j + 1
+#pragma unroll 1
+    for (int j = 0; j < kPairs; ++j) {
+        load_fr(s, ri + j * 32);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] &= m;
+        jj::Ext acc, t;
+        jj::var_walk<false, true>(acc, c, tab, s);
+        {
+            uint32_t mu[8], mv[8];
+            const uint8_t* mj = j ? mi1 : mi0;
+            load_fr(mu, mj);
+            load_fr(mv, mj + 32);
+            mask_point(mu, mv, m);
+            jj::Niels q;
+            jj::to_niels(q, mu, mv);
+            jj::madd<false>(t, acc, q);
+        }
+        jj::park(out[2 * j + 1], t);
+        jj::fixed_base_ext<true, false>(t, s, table);
+        jj::park(out[2 * j], t);
+    }
+    jj::batch_affine(out);
+#pragma unroll
+    for (int j = 0; j < 2 * kPairs; ++j) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) out[j].X[k] &= m, out[j].Y[k] &= m;
+        uint8_t* row = ((j & 1) ? c2 : c1) + i * stride + (j >> 1) * 128;
+        store_fr(row, out[j].X);
+        store_fr(row + 32, out[j].Y);
+    }
+    ok[i] = valid ? 1 : 0;
+    if (n_invalid) warp_count_every(n_invalid, !valid);
+}
+
+// One thread per item.  The ciphertext (c1_j, c2_j), j < kPairs, is read at c1 + i stride + 128 j and c2 + i stride + 128 j
+// (layouts as for k_elgamal_enc); M_j = c2_j - [s] c1_j = c2_j + [s] (-c1_j) goes to out_j + 64 i.
+//   generic (jj::kProductsPerElGamalDec): s = key[kb ? 0 : i] = sk; valid iff sk < r_J and c1, c2 curve points with
+//     u, v < p; ok[i] = valid.
+//   note (jj::kProductsPerSenderDec), after k_dhke (valid[i]: a < r_J, R a curve point) and the truncated digest (h[i]):
+//     s = note_sk = (h + b) mod r_J with b = key[kb ? 0 : i]; valid iff valid[i], b < r_J and all four ciphertext points
+//     curve points with u, v < p; ok[i] = valid and owned, owned iff both coordinates of note_pk[i] < p and
+//     [note_sk] G == note_pk[i] (table: G's fixed-base table; projective comparison, no inversion).
+// An item with ok = 0 gets zeroed rows and is counted once into *count.  Every item runs the same schedule: an invalid
+// one on s = 0 and identities, and a note that is not owned is decrypted all the same and its rows zeroed.  The keys,
+// h, note_sk and the plaintexts are secret: the table reads are masked selects.  The generic form fits in 128 registers
+// without spilling, so it keeps k_dhke's four blocks per SM; the note form needs more and runs three.
+template <bool kNote>
+__global__ void __launch_bounds__(kThreads, kNote ? 3 : 4) k_elgamal_dec(const uint8_t* __restrict__ key, bool kb,
+                                                          const uint8_t* __restrict__ h, const uint8_t* __restrict__ valid,
+                                                          const uint8_t* __restrict__ note_pk, const uint8_t* __restrict__ c1,
+                                                          const uint8_t* __restrict__ c2, uint32_t stride, size_t n,
+                                                          const uint4* __restrict__ table, uint8_t* out0, uint8_t* out1,
+                                                          uint8_t* __restrict__ ok, unsigned long long* __restrict__ count) {
+    constexpr int kPairs = kNote ? 2 : 1;
+    const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
+    if (i >= n) return;
+    uint32_t s[8], u[8], v[8];
+    load_fr(s, key + (kb ? 0 : i) * 32);
+    bool good = jj::below_order(s);
+    if (kNote) {
+        const uint32_t mb = 0u - (uint32_t)good;
+        uint32_t hh[8], t[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s[k] &= mb;
+        load_fr(hh, h + i * 32);
+        jj::order_add(t, hh, s);
+        jj::fcopy(s, t);
+        good &= valid[i] != 0;
+    }
+#pragma unroll 1
+    for (int j = 0; j < kPairs; ++j) {
+        good &= load_point(u, v, c1 + i * stride + j * 128);
+        good &= load_point(u, v, c2 + i * stride + j * 128);
+    }
+    const uint32_t m = 0u - (uint32_t)good;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) s[k] &= m;
+    jj::Proj out[kPairs];
+    const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+#pragma unroll 1
+    for (int j = 0; j < kPairs; ++j) {
+        jj::Entry tab[16];
+        jj::Cached c;
+        jj::Ext acc, t;
+        load_fr(u, c1 + i * stride + j * 128);
+        load_fr(v, c1 + i * stride + j * 128 + 32);
+        mask_point(u, v, m);
+        fr_sub_mod(u, zero, u);                     // -c1 = (-u, v)
+        jj::var_table(tab, acc, c, u, v);
+        jj::var_walk<false, true>(acc, c, tab, s);
+        load_fr(u, c2 + i * stride + j * 128);
+        load_fr(v, c2 + i * stride + j * 128 + 32);
+        mask_point(u, v, m);
+        jj::Niels q;
+        jj::to_niels(q, u, v);
+        jj::madd<false>(t, acc, q);
+        jj::park(out[j], t);
+    }
+    bool opened = good;
+    if (kNote) {
+        jj::Ext t;
+        jj::fixed_base_ext<true, false>(t, s, table);
+        load_fr(u, note_pk + i * 64);
+        load_fr(v, note_pk + i * 64 + 32);
+        const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
+        const uint32_t mc = 0u - (uint32_t)canon;   // coordinates >= p enter no product
+        uint32_t x[8], y[8];
+#pragma unroll
+        for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] &= mc;
+        jj::fmul(x, u, t.Z);
+        jj::fmul(y, v, t.Z);
+        opened = good & canon & jj::feq(x, t.X) & jj::feq(y, t.Y);
+    }
+    jj::batch_affine(out);
+    const uint32_t mo = 0u - (uint32_t)opened;
+#pragma unroll
+    for (int j = 0; j < kPairs; ++j) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) out[j].X[k] &= mo, out[j].Y[k] &= mo;
+        uint8_t* row = (j ? out1 : out0) + i * 64;
+        store_fr(row, out[j].X);
+        store_fr(row + 32, out[j].Y);
+    }
+    ok[i] = opened ? 1 : 0;
+    if (count) warp_count_every(count, !opened);
+}
+
+cudaError_t launch_elgamal_encrypt(const void* pk, bool pk_bcast, const void* msg, bool msg_bcast, const void* r, size_t n,
+                                   const void* table, void* c1_uv, void* c2_uv, uint8_t* ok, unsigned long long* n_invalid,
+                                   cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_elgamal_enc<1><<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(msg), nullptr, msg_bcast,
+        static_cast<const uint8_t*>(r), n, static_cast<const uint4*>(table), static_cast<uint8_t*>(c1_uv),
+        static_cast<uint8_t*>(c2_uv), 64, ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_note_sender_encrypt(const void* note_pk, const void* A_uv, const void* B_uv, bool sender_bcast,
+                                       const void* blinder, size_t n, const void* table, void* enc, uint8_t* ok,
+                                       unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    uint8_t* e = static_cast<uint8_t*>(enc);
+    k_elgamal_enc<2><<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(note_pk), false, static_cast<const uint8_t*>(A_uv), static_cast<const uint8_t*>(B_uv),
+        sender_bcast, static_cast<const uint8_t*>(blinder), n, static_cast<const uint4*>(table), e, e + 64, 256, ok,
+        n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_elgamal_decrypt(const void* sk, bool sk_bcast, const void* c1_uv, const void* c2_uv, size_t n,
+                                   void* msg_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_elgamal_dec<false><<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(sk), sk_bcast, nullptr, nullptr, nullptr, static_cast<const uint8_t*>(c1_uv),
+        static_cast<const uint8_t*>(c2_uv), 64, n, nullptr, static_cast<uint8_t*>(msg_uv), nullptr, ok, n_invalid);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_note_sender_decrypt(const void* h, const void* b, bool b_bcast, const uint8_t* valid, const void* note_pk,
+                                       const void* enc, size_t n, const void* table, void* A_uv, void* B_uv, uint8_t* ok,
+                                       unsigned long long* n_failed, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const uint8_t* e = static_cast<const uint8_t*>(enc);
+    k_elgamal_dec<true><<<grid_for(n), kThreads, 0, st>>>(
+        static_cast<const uint8_t*>(b), b_bcast, static_cast<const uint8_t*>(h), valid, static_cast<const uint8_t*>(note_pk),
+        e, e + 64, 256, n, static_cast<const uint4*>(table), static_cast<uint8_t*>(A_uv), static_cast<uint8_t*>(B_uv), ok,
+        n_failed);
+    return cudaGetLastError();
+}
+
 // ---- point compression: JubJubAffine::from_bytes / to_bytes (jubjub_device.cuh) ---------------------------------------
 // One thread per point.  Public data only.
 // from_bytes (kProductsPerDecompress products): bytes[i] -> (u, v) Montgomery; ok[i] = v < p and u^2 a square.  An

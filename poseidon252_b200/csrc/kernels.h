@@ -246,6 +246,29 @@ cudaError_t launch_wallet_select(uint32_t k, const uint8_t* matched, const void*
 cudaError_t launch_wallet_scatter(const void* meta, const void* nul, const uint64_t* value_rows, const void* blinder_rows,
                                   const uint8_t* ok, size_t n_own, void* nullifier, uint64_t* value, void* blinder,
                                   uint8_t* opened, unsigned long long* totals, cudaStream_t st);
+// JubJub ElGamal (p252_elgamal_{encrypt,decrypt}_batch, p252_note_sender_{encrypt,decrypt}_batch): (c1, c2) =
+// ([r] G, M + [r] PK) with table the fixed-base table of G, and M = c2 - [sk] c1.  Points are (u, v) Montgomery pairs,
+// scalars canonical 4 x u64.  Every item runs the same schedule; an item with ok = 0 gets zeroed output rows and is
+// counted once into the counter (a device pointer, may be null).
+// encrypt: c1_uv[i], c2_uv[i] = encrypt(pk[pk_bcast ? 0 : i], msg[msg_bcast ? 0 : i]; r[i]); ok[i] = r < r_J and both
+// points curve points with u, v < p
+cudaError_t launch_elgamal_encrypt(const void* pk, bool pk_bcast, const void* msg, bool msg_bcast, const void* r, size_t n,
+                                   const void* table, void* c1_uv, void* c2_uv, uint8_t* ok, unsigned long long* n_invalid,
+                                   cudaStream_t st);
+// sender encrypt: enc[i] = [c1_A, c2_A, c1_B, c2_B] (256 bytes), the encryptions of A and B (row sender_bcast ? 0 : i)
+// under note_pk[i] with blinder[2 i], blinder[2 i + 1]; ok as for encrypt, over all five operands
+cudaError_t launch_note_sender_encrypt(const void* note_pk, const void* A_uv, const void* B_uv, bool sender_bcast,
+                                       const void* blinder, size_t n, const void* table, void* enc, uint8_t* ok,
+                                       unsigned long long* n_invalid, cudaStream_t st);
+// decrypt: msg_uv[i] = c2_uv[i] - [sk[sk_bcast ? 0 : i]] c1_uv[i]; ok[i] = sk < r_J and c1, c2 curve points with u, v < p
+cudaError_t launch_elgamal_decrypt(const void* sk, bool sk_bcast, const void* c1_uv, const void* c2_uv, size_t n,
+                                   void* msg_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st);
+// sender decrypt, after launch_dhke ([a] R, valid) and the truncated digest (h): note_sk = (h[i] + b) mod r_J with
+// b = b[b_bcast ? 0 : i]; A_uv[i], B_uv[i] = c2 - [note_sk] c1 of enc[i]'s two pairs; ok[i] = valid[i], b < r_J, the four
+// ciphertext points curve points with u, v < p, and [note_sk] G == note_pk[i]; *n_failed += items with ok = 0
+cudaError_t launch_note_sender_decrypt(const void* h, const void* b, bool b_bcast, const uint8_t* valid, const void* note_pk,
+                                       const void* enc, size_t n, const void* table, void* A_uv, void* B_uv, uint8_t* ok,
+                                       unsigned long long* n_failed, cudaStream_t st);
 // Point compression (p252_points_from_bytes / p252_points_to_bytes): 32-byte encodings <-> (u, v) Montgomery pairs (64
 // bytes).  from: ok[i] = v < p and u^2 a square, an invalid item gets (0, 0); to: ok[i] = u, v < p and on the curve, an
 // invalid item gets 32 bytes of 0xff.  *n_invalid (a device counter, may be null) += invalid items.

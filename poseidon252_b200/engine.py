@@ -852,6 +852,127 @@ class Engine:
         """Items of the last note_open_batch that did not open, invalid ones included (sync() first after async_)."""
         return self._last("note_failed")
 
+    # -- JubJub ElGamal and the encrypted sender of a note ---------------------------------------------
+    def elgamal_encrypt_batch(self, pk, msg, r, base, async_=False):
+        """JubJub ElGamal: (c1_i, c2_i) = ([r_i] base, M_i + [r_i] PK_i).  pk (1 or n, 2, 4), msg (n, 2, 4), r (n, 4)
+        p252_jscalar rows (one per message, never reused under one key: c2 - c2' would reveal M - M'), base (G) (2, 4),
+        host-read -> (c1 (n, 2, 4), c2 (n, 2, 4), ok (n,) uint8).  An item with r >= r_J or PK or M not a curve point
+        has ok == 0 and zeroed rows (count: last_elgamal_invalid()).  A base off the curve raises InvalidPoint."""
+        rp, rl, flags, rk = self._in(r, (4,))
+        if len(rl) != 1:
+            raise EngineError(-1, "r must have shape (n, 4)")
+        n = int(rl[0])
+        pp, pl, fp, _ = self._in(pk, (2, 4))
+        mp, ml, fm, _ = self._in(msg, (2, 4))
+        self._same_space(flags, fp, fm)
+        if len(pl) != 1 or int(pl[0]) not in (1, n):
+            raise EngineError(-1, "pk must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(pl)))
+        self._same_lead("msg", ml, n)
+        g = self._base(base)
+        c1 = self._result(None, (n, 2, 4), rk)
+        c2 = self._result(None, (n, 2, 4), rk)
+        ok = self._ok_like(rk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("elgamal_invalid", flags)
+        self._check(self._lib.p252_elgamal_encrypt_batch(self._ctx, pp, int(pl[0]), mp, rp, n, g.ctypes.data,
+                                                         self._ptr(c1), self._ptr(c2), self._ptr(ok),
+                                                         ctypes.byref(invalid), flags))
+        return c1, c2, ok
+
+    def elgamal_decrypt_batch(self, sk, c1, c2, async_=False):
+        """JubJub ElGamal decryption: M_i = c2_i - [sk_i] c1_i.  sk (1 or n, 4) p252_jscalar rows, c1 and c2 (n, 2, 4) ->
+        (msg (n, 2, 4), ok (n,) uint8).  NOT authenticated: a wrong key gives another curve point with ok == 1.  An item
+        with sk >= r_J or c1 or c2 not a curve point has ok == 0 and a zeroed row (count: last_elgamal_invalid())."""
+        ap, al, flags, ak = self._in(c1, (2, 4))
+        if len(al) != 1:
+            raise EngineError(-1, "c1 must have shape (n, 2, 4)")
+        n = int(al[0])
+        sp, sl, fs, _ = self._in(sk, (4,))
+        bp, bl, fb, _ = self._in(c2, (2, 4))
+        self._same_space(flags, fs, fb)
+        if len(sl) != 1 or int(sl[0]) not in (1, n):
+            raise EngineError(-1, "sk must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(sl)))
+        self._same_lead("c2", bl, n)
+        msg = self._result(None, (n, 2, 4), ak)
+        ok = self._ok_like(ak, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("elgamal_invalid", flags)
+        self._check(self._lib.p252_elgamal_decrypt_batch(self._ctx, sp, int(sl[0]), ap, bp, n, self._ptr(msg),
+                                                         self._ptr(ok), ctypes.byref(invalid), flags))
+        return msg, ok
+
+    def note_sender_encrypt_batch(self, note_pk, sender_A, sender_B, blinder, base, async_=False):
+        """The encrypted sender of Phoenix notes: enc_i = [c1_A, c2_A, c1_B, c2_B], the ElGamal encryptions of the
+        sender's A and B under note_pk_i with the blinders (r_A, r_B) = blinder_i.  note_pk (n, 2, 4), sender_A and
+        sender_B (1 or n, 2, 4) with the same number of rows, blinder (n, 2, 4) p252_jscalar rows [r_A, r_B], base (G)
+        (2, 4) host-read -> (enc (n, 4, 2, 4), ok (n,) uint8).  An item with a blinder >= r_J or a point not on the curve
+        has ok == 0 and a zeroed row (count: last_elgamal_invalid())."""
+        pp, pl, flags, pk = self._in(note_pk, (2, 4))
+        if len(pl) != 1:
+            raise EngineError(-1, "note_pk must have shape (n, 2, 4)")
+        n = int(pl[0])
+        ap, al, fa, _ = self._in(sender_A, (2, 4))
+        bp, bl, fb, _ = self._in(sender_B, (2, 4))
+        rp, rl, fr, _ = self._in(blinder, (2, 4))
+        self._same_space(flags, fa, fb, fr)
+        if len(al) != 1 or int(al[0]) not in (1, n):
+            raise EngineError(-1, "sender_A must have shape (1 or %d, 2, 4), got leading shape %s" % (n, tuple(al)))
+        if tuple(bl) != tuple(al):
+            raise EngineError(-1, "sender_B must have %d rows like sender_A, got leading shape %s" % (int(al[0]), tuple(bl)))
+        self._same_lead("blinder", rl, n)
+        g = self._base(base)
+        enc = self._result(None, (n, 4, 2, 4), pk)
+        ok = self._ok_like(pk, n)
+        flags = self._flags(flags, async_)
+        invalid = self._counter("elgamal_invalid", flags)
+        self._check(self._lib.p252_note_sender_encrypt_batch(self._ctx, pp, ap, bp, int(al[0]), rp, n, g.ctypes.data,
+                                                             self._ptr(enc), self._ptr(ok), ctypes.byref(invalid), flags))
+        return enc, ok
+
+    def note_sender_decrypt_batch(self, a, b, R, note_pk, enc, base, async_=False):
+        """The owner's recovery of the sender: note_sk_i = (hash([a] R_i) + b) mod r_J, hash(P) =
+        Hash::digest_truncated(Domain::Other, [P.u, P.v])[0]; where [note_sk_i] base == note_pk_i, A_i = c2_A - [note_sk]
+        c1_A and B_i = c2_B - [note_sk] c1_B.  a and b (1 or n, 4) p252_jscalar rows with the same number of rows, R and
+        note_pk (n, 2, 4), enc (n, 4, 2, 4) as note_sender_encrypt_batch writes it, base (G) (2, 4) host-read ->
+        (A (n, 2, 4), B (n, 2, 4), ok (n,) uint8).  ok == 0 (A and B zeroed) for a note the key does not own and for an
+        invalid item (a or b >= r_J, R or a ciphertext point not on the curve); their count: last_sender_failed().
+        note_sk never leaves the device."""
+        Rp, Rl, flags, Rk = self._in(R, (2, 4))
+        if len(Rl) != 1:
+            raise EngineError(-1, "R must have shape (n, 2, 4)")
+        n = int(Rl[0])
+        ap, al, fa, _ = self._in(a, (4,))
+        bp, bl, fb, _ = self._in(b, (4,))
+        pp, pl, fp, _ = self._in(note_pk, (2, 4))
+        ep, el, fe, _ = self._in(enc, (4, 2, 4))
+        self._same_space(flags, fa, fb, fp, fe)
+        if len(al) != 1 or int(al[0]) not in (1, n):
+            raise EngineError(-1, "a must have shape (1 or %d, 4), got leading shape %s" % (n, tuple(al)))
+        ns = int(al[0])
+        if tuple(bl) != (ns,):
+            raise EngineError(-1, "b must have %d rows like a, got leading shape %s" % (ns, tuple(bl)))
+        self._same_lead("note_pk", pl, n)
+        self._same_lead("enc", el, n)
+        g = self._base(base)
+        A = self._result(None, (n, 2, 4), Rk)
+        B = self._result(None, (n, 2, 4), Rk)
+        ok = self._ok_like(Rk, n)
+        flags = self._flags(flags, async_)
+        failed = self._counter("sender_failed", flags)
+        self._check(self._lib.p252_note_sender_decrypt_batch(self._ctx, ap, bp, ns, Rp, pp, ep, n, g.ctypes.data,
+                                                             self._ptr(A), self._ptr(B), self._ptr(ok),
+                                                             ctypes.byref(failed), flags))
+        return A, B, ok
+
+    def last_elgamal_invalid(self):
+        """Invalid items of the last elgamal_encrypt_batch, elgamal_decrypt_batch or note_sender_encrypt_batch (sync()
+        first after async_)."""
+        return self._last("elgamal_invalid")
+
+    def last_sender_failed(self):
+        """Items of the last note_sender_decrypt_batch with ok == 0, not owned or invalid (sync() first after async_)."""
+        return self._last("sender_failed")
+
     # -- multi-key wallet scans ---------------------------------------------------------------------
     WALLET_MAX_KEYS = 256
 
