@@ -164,6 +164,11 @@ mod verify_double_all;
 mod elgamal;
 pub use elgamal::SenderEncryption;
 
+// BlsScalar::hash_to_scalar of many byte strings and BlsScalar::from_bytes_wide: their own `extern "C"` block in
+// hash_to_scalar.rs (methods on Engine).
+mod hash_to_scalar;
+pub use hash_to_scalar::HASH_TO_SCALAR_MAX_LEN;
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

@@ -191,6 +191,32 @@ int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t 
  * reference returns None); ok may be NULL. */
 int p252_scalars_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out, uint8_t* ok, int flags);
 int p252_scalars_to_bytes(p252_ctx* ctx, const p252_fr* in, size_t n, uint8_t* bytes, int flags);
+/* BlsScalar::from_bytes_wide on n rows of 64 bytes: out[i] = (lo + hi * 2^256) mod p in Montgomery form, lo / hi the
+ * row's first / last 32 bytes as little-endian integers.  Every input is valid.  DEVICE bytes and out must be 16-byte
+ * aligned. */
+int p252_scalars_from_bytes_wide(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out, int flags);
+
+/* Batched BlsScalar::hash_to_scalar (src/hades/permutation/scalar.rs:29-31; p252_hash_to_scalar is one call of it):
+ * out[i] = from_bytes_wide(BLAKE2b-512(bytes[offsets[i] .. offsets[i+1]))) in Montgomery form (BlsScalar.0), for i < n,
+ * one call for byte strings of any mix of lengths.  The rows can go straight in as the msg of the Schnorr calls.
+ *   bytes: n_bytes bytes, any alignment; offsets: n + 1 absolute byte offsets in the same memory space as bytes / out
+ *   (offsets[0] need not be 0, so a slice of a larger CSR array works); out: n rows, in input order.
+ *   Batch checks, before anything runs: n >= 2^31, max_len > P252_HASH_TO_SCALAR_MAX_LEN, a NULL buffer (bytes with
+ *   n_bytes > 0, offsets or out with n > 0), DEVICE offsets not 8-byte or out not 16-byte aligned -> INVALID_ARGUMENT.
+ *   Item i is valid iff offsets[i] <= offsets[i+1] <= n_bytes and its length is <= max_len.  Length 0 is valid (the
+ *   hash of the empty string), so max_len == 0 is allowed.
+ *   HOST: the whole batch is checked first; the lowest-index invalid item decides the status (INVALID_ARGUMENT) and
+ *   nothing is written.  The batch is staged in chunks of about 24 MiB of message bytes.
+ *   DEVICE: offsets are not inspected on the host; an invalid item gets a zero row and is counted into *n_rejected
+ *   (optional HOST pointer, 0 for HOST calls; lifetime as for p252_mtree_update).  No offset value makes a kernel read
+ *   a byte outside bytes[0, n_bytes) or write outside out.  With P252_ASYNC nothing is synchronised.
+ * n == 0 runs nothing.  The messages are public data, like the inputs of p252_hash_batch: they are staged in ordinary
+ * (not wiped) buffers.  One thread hashes one message: BLAKE2b is a serial chain of 128-byte blocks, so a very long item
+ * takes one thread ceil(len / 128) compressions while the rest of the batch has finished.  With max_len > 128 the items
+ * are sorted by block count on the device first, so that a warp hashes messages of nearly equal length together. */
+#define P252_HASH_TO_SCALAR_MAX_LEN (1u << 20) /* bytes per item */
+int p252_hash_to_scalar_batch(p252_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const uint64_t* offsets, size_t n,
+                              size_t max_len, p252_fr* out, size_t* n_rejected, int flags);
 
 /* encrypt_batch: n x encrypt(msg[i], (u,v)[i], nonce[i]) (src/encryption.rs:62-74).
  * msg: n x L, secret_uv: n x 2 (JubJubAffine::get_u/get_v), nonce: n, cipher: n x (L+1). */

@@ -16,7 +16,7 @@
 //   points_from_bytes_batch, point_to_bytes / points_to_bytes_batch, value_commit / value_commit_batch,
 //   note_create_batch, note_open / note_open_batch, wallet_scan_batch, elgamal_encrypt_batch, elgamal_decrypt_batch,
 //   note_sender_encrypt_batch, note_sender_decrypt_batch, jubjub_msm, schnorr_verify_all,
-//   schnorr_verify_double_all, merkle4_build.
+//   schnorr_verify_double_all, merkle4_build, hash_to_scalar_batch, scalars_from_bytes_wide.
 // Scalars are p252_fr == BlsScalar.0 (Montgomery limbs); every digest runs on the GPU (batch of 1 for the
 // single-item calls).  No CPU fallback: Engine's constructor throws without an sm_90 device.
 #pragma once
@@ -178,6 +178,32 @@ private:
     std::vector<Chunk> chunks_;
     size_t output_len_ = 1;
 };
+
+// NEW: BlsScalar::hash_to_scalar of byte strings of any lengths (empty ones included), one device call
+// (p252_hash_to_scalar_batch): BLAKE2b-512, then from_bytes_wide, as Montgomery scalars ready to be a Schnorr msg.
+// Throws Error(P252_ERR_INVALID_ARGUMENT) for a message longer than P252_HASH_TO_SCALAR_MAX_LEN (nothing computed).
+inline std::vector<Scalar> hash_to_scalar_batch(const std::vector<std::vector<uint8_t>>& messages,
+                                                Engine& e = Engine::default_engine()) {
+    std::vector<uint8_t> data;
+    std::vector<uint64_t> offsets{0};
+    size_t longest = 0;
+    for (auto& m : messages) {
+        data.insert(data.end(), m.begin(), m.end());
+        offsets.push_back(data.size());
+        longest = m.size() > longest ? m.size() : longest;
+    }
+    std::vector<Scalar> out(messages.size());
+    check(p252_hash_to_scalar_batch(e.get(), data.data(), data.size(), offsets.data(), messages.size(), longest, out.data(),
+                                    nullptr, P252_MEM_HOST),
+          e.get());
+    return out;
+}
+// NEW: BlsScalar::from_bytes_wide of n rows of 64 bytes (p252_scalars_from_bytes_wide); every row is valid
+inline std::vector<Scalar> scalars_from_bytes_wide(const uint8_t* bytes, size_t n, Engine& e = Engine::default_engine()) {
+    std::vector<Scalar> out(n);
+    check(p252_scalars_from_bytes_wide(e.get(), bytes, n, out.data(), P252_MEM_HOST), e.get());
+    return out;
+}
 
 // src/encryption.rs:62-74; shared_secret = (u, v) of the JubJubAffine point (src/encryption.rs:71)
 inline std::vector<Scalar> encrypt(const std::vector<Scalar>& message, const Scalar (&shared_secret_uv)[2],

@@ -34,6 +34,9 @@ SIGNATURES = {
     "p252_hash_batch": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_int]),
     "p252_hash_batch_truncated": (c_int, [c_void_p, c_int, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t, c_int]),
     "p252_scalars_from_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_void_p, c_int]),
+    "p252_scalars_from_bytes_wide": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
+    "p252_hash_to_scalar_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p,
+                                          ctypes.POINTER(c_size_t), c_int]),
     "p252_scalars_to_bytes": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
     "p252_encrypt_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_int]),
     "p252_decrypt_batch": (c_int, [c_void_p, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p, c_void_p, c_void_p,
@@ -135,6 +138,7 @@ SIGNATURES = {
 
 MEM_HOST, MEM_DEVICE, ASYNC, TIMING, NO_GATHER = 0, 1, 2, 4, 8
 VARLEN_MAX_LEN = 65536   # P252_VARLEN_MAX_LEN
+HASH_TO_SCALAR_MAX_LEN = 1 << 20   # P252_HASH_TO_SCALAR_MAX_LEN, bytes per item
 
 
 class KernelInfo(ctypes.Structure):

@@ -20,6 +20,8 @@
 //     p252_note_open_batch
 //   JubJub ElGamal, the encrypted sender of a Phoenix note (consumer, not the reference) -> p252_elgamal_encrypt_batch,
 //     p252_elgamal_decrypt_batch, p252_note_sender_encrypt_batch, p252_note_sender_decrypt_batch
+//   BlsScalar::hash_to_scalar / from_bytes_wide on the device   -> p252_hash_to_scalar_batch,
+//     p252_scalars_from_bytes_wide
 //   Error                          src/error.rs:11-44      -> p252_status
 // No permutation is ever computed on the host: without a CUDA device every batch call fails.
 #include <cuda_runtime.h>
@@ -927,6 +929,16 @@ int p252_scalars_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_
 
 int p252_scalars_to_bytes(p252_ctx* ctx, const p252_fr* in, size_t n, uint8_t* bytes, int flags) {
     return convert_impl(ctx, in, n, bytes, nullptr, flags, false);
+}
+
+int p252_scalars_from_bytes_wide(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out, int flags) {
+    if (!ctx || !args_ok(n, flags, {bytes, out})) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    std::vector<Io> ios = {{bytes, nullptr, 64}, {nullptr, out, 32}};
+    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_from_bytes_wide(d[0], cnt, d[1], st));
+    });
 }
 
 int p252_encrypt_batch(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_fr* secret_uv,
@@ -3165,13 +3177,14 @@ int crypt_run(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* i
         });
 }
 
-// The chunks of a variable-length HOST batch: consecutive item ranges of about kChunkBytesTarget input bytes (a longer
-// item is a chunk by itself), at most chunk_items_max() items each; chunk k = items [bounds[k], bounds[k+1]).
-std::vector<size_t> chunk_bounds(const uint64_t* offsets, size_t n) {
+// The chunks of a variable-length HOST batch whose offsets count elements of elem_bytes bytes (scalars, or bytes):
+// consecutive item ranges of about kChunkBytesTarget input bytes (a longer item is a chunk by itself), at most
+// chunk_items_max() items each; chunk k = items [bounds[k], bounds[k+1]).
+std::vector<size_t> chunk_bounds(const uint64_t* offsets, size_t n, size_t elem_bytes) {
     std::vector<size_t> bounds = {0};
     for (size_t lo = 0, hi = 0; lo < n; lo = hi) {
         hi = lo + 1;
-        while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * sizeof(p252_fr) <= kChunkBytesTarget) ++hi;
+        while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * elem_bytes <= kChunkBytesTarget) ++hi;
         bounds.push_back(hi);
     }
     return bounds;
@@ -3181,7 +3194,7 @@ std::vector<size_t> chunk_bounds(const uint64_t* offsets, size_t n) {
 // rows in one stream-ordered allocation -- hashed by varlen_run with base = the chunk's first offset, and copied back.
 int varlen_host(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n, uint32_t max_len,
                 uint32_t fixed_len, p252_fr* out, uint32_t out_len) {
-    const std::vector<size_t> bounds = chunk_bounds(offsets, n);
+    const std::vector<size_t> bounds = chunk_bounds(offsets, n, sizeof(p252_fr));
     return on_slots(ctx, false, [&](long long fail_at) -> int {
         for (size_t k = 0; k + 1 < bounds.size(); ++k) {
             const size_t lo = bounds[k], hi = bounds[k + 1], cnt = hi - lo;
@@ -3215,7 +3228,7 @@ int varlen_host(p252_ctx* ctx, const p252_fr* tags, const p252_fr* in, const uin
 // Output of chunk [lo, hi): (ns +- cnt) scalars at out + (s0 - a0 +- lo), the chunk's part of the output CSR.
 int crypt_host(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* in, const uint64_t* offsets, size_t n,
                uint32_t max_len, const p252_fr* secret_uv, const p252_fr* nonce, p252_fr* out, uint8_t* ok) {
-    const std::vector<size_t> bounds = chunk_bounds(offsets, n);
+    const std::vector<size_t> bounds = chunk_bounds(offsets, n, sizeof(p252_fr));
     p252_fr *d_in = nullptr, *d_uv = nullptr, *d_nonce = nullptr, *d_out = nullptr;
     uint64_t* d_off = nullptr;
     uint8_t* d_ok = nullptr;
@@ -3363,6 +3376,90 @@ int p252_decrypt_batch_varlen(p252_ctx* ctx, const p252_fr* cipher, size_t n_sca
                               size_t* n_failed, size_t* n_rejected, int flags) {
     return crypt_varlen(ctx, true, cipher, n_scalars, offsets, n, max_len, secret_uv, nonce, msg, ok, n_failed, n_rejected,
                         flags);
+}
+
+}  // extern "C"
+
+// ---- BlsScalar::hash_to_scalar batches (p252_hash_to_scalar_batch) ---------------------------------------------------
+namespace {
+
+// One batch on `st` (item i = bytes[offsets[i] - base ..) of n_bytes): with max_len <= 128 every item is one block and
+// k_hash_to_scalar runs in input order, counting rejected items itself; otherwise items are sorted by block count first
+// (varlen_sorted, which counts them in the keys kernel).
+int hash_to_scalar_run(p252_ctx* ctx, const uint8_t* bytes, uint64_t base, uint64_t n_bytes, const uint64_t* offsets, uint32_t n,
+                       uint32_t max_len, p252_fr* out, unsigned long long* rejected, cudaStream_t st) {
+    if (max_len <= 128)
+        return launched(ctx, p252::launch_hash_to_scalar(bytes, base, n_bytes, offsets, nullptr, n, max_len, out, rejected, st));
+    const uint32_t max_blocks = (max_len + 127) / 128;
+    return varlen_sorted(
+        ctx, n, max_blocks, st,
+        [&](uint32_t* keys, uint32_t* vals) {
+            return p252::launch_hash_to_scalar_keys(offsets, n, base, n_bytes, max_len, keys, vals, rejected, st);
+        },
+        [&](const uint32_t*, const uint32_t* perm) {
+            return p252::launch_hash_to_scalar(bytes, base, n_bytes, offsets, perm, n, max_len, out, nullptr, st);
+        });
+}
+
+// HOST batch (already validated): as varlen_host, with chunks of about kChunkBytesTarget message bytes
+int hash_to_scalar_host(p252_ctx* ctx, const uint8_t* bytes, const uint64_t* offsets, size_t n, uint32_t max_len, p252_fr* out) {
+    const std::vector<size_t> bounds = chunk_bounds(offsets, n, 1);
+    return on_slots(ctx, false, [&](long long fail_at) -> int {
+        for (size_t k = 0; k + 1 < bounds.size(); ++k) {
+            const size_t lo = bounds[k], hi = bounds[k + 1], cnt = hi - lo;
+            const uint64_t s0 = offsets[lo], nb = offsets[hi] - s0;
+            cudaStream_t st = ctx->slots[k % kSlots].stream;
+            uint8_t* d_in = nullptr;
+            uint64_t* d_off = nullptr;
+            p252_fr* d_out = nullptr;
+            auto layout = [&](Carve& c) {
+                d_in = c.take<uint8_t>(nb);
+                d_off = c.take<uint64_t>(cnt + 1);
+                d_out = c.take<p252_fr>(cnt);
+            };
+            const int rc = with_scratch(ctx, st, layout, [&]() -> int {
+                if (nb) CU(cudaMemcpyAsync(d_in, bytes + s0, nb, cudaMemcpyHostToDevice, st));
+                CU(cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
+                if ((long long)k == fail_at) return injected_fault(ctx);
+                const int r = hash_to_scalar_run(ctx, d_in, s0, nb, d_off, (uint32_t)cnt, max_len, d_out, nullptr, st);
+                if (r != P252_OK) return r;
+                CU(cudaMemcpyAsync(out + lo, d_out, cnt * sizeof(p252_fr), cudaMemcpyDeviceToHost, st));
+                return P252_OK;
+            });
+            if (rc != P252_OK) return rc;
+        }
+        return P252_OK;
+    });
+}
+
+}  // namespace
+
+extern "C" {
+
+int p252_hash_to_scalar_batch(p252_ctx* ctx, const uint8_t* bytes, size_t n_bytes, const uint64_t* offsets, size_t n,
+                              size_t max_len, p252_fr* out, size_t* n_rejected, int flags) {
+    if (!ctx || (!bytes && n_bytes) || ((!offsets || !out) && n)) return P252_ERR_INVALID_ARGUMENT;
+    if (n >= 0x80000000ull || max_len > P252_HASH_TO_SCALAR_MAX_LEN) return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_rejected) *n_rejected = 0;
+    int rc;
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(out) || (reinterpret_cast<uintptr_t>(offsets) & 7)) return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        rc = hash_to_scalar_run(ctx, bytes, 0, n_bytes, offsets, (uint32_t)n, (uint32_t)max_len, out,
+                                n_rejected ? ctx->d_counter : nullptr, ctx->stream);
+        if (rc == P252_OK) rc = counter_end(ctx, n_rejected);
+        return device_done(ctx, rc, flags);
+    }
+    // HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written
+    for (size_t i = 0; i < n; ++i) {
+        const uint64_t a = offsets[i], b = offsets[i + 1];
+        if (a > b || b > n_bytes || b - a > max_len) return P252_ERR_INVALID_ARGUMENT;
+    }
+    if (n == 0) return P252_OK;
+    return hash_to_scalar_host(ctx, bytes, offsets, n, (uint32_t)max_len, out);
 }
 
 }  // extern "C"

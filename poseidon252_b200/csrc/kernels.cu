@@ -17,6 +17,8 @@
 //   multi-key wallet scans (owner, then nullifier and opening of owned notes) -> k_wallet_keys, k_wallet_dhke,
 //     k_wallet_match, k_wallet_select, k_wallet_scatter
 //   JubJubAffine::from_bytes / to_bytes (point compression) -> k_points_from_bytes, k_points_to_bytes
+//   BlsScalar::hash_to_scalar (BLAKE2b-512 of byte strings, then from_bytes_wide) -> k_hash_to_scalar_keys,
+//     k_hash_to_scalar; BlsScalar::from_bytes_wide alone -> k_from_bytes_wide
 // capacity = state[0] = tag, rate = state[1..5]; absorb adds into state[pos+1] and permutes when
 // pos == 4; any absorb forces a permutation before the next squeeze.
 #include "kernels.h"
@@ -3672,6 +3674,228 @@ cudaError_t launch_digest_varlen(const void* tags, const void* in, uint64_t base
     } else {
         k_sponge_digest_varlen<<<grid_for(n), kThreads, 0, st>>>(t, i, base, offsets, lens, perm, n, o, out_len);
     }
+    return cudaGetLastError();
+}
+
+// ---- BlsScalar::hash_to_scalar on the device (p252_hash_to_scalar_batch, p252_scalars_from_bytes_wide) -------------
+// BLAKE2b-512 (RFC 7693; host::Blake2b in host_field.h) of a byte string, then from_bytes_wide.  Public data only.
+
+// BlsScalar::from_bytes_wide of the 64 little-endian bytes w: (lo + hi 2^256) mod p in Montgomery form, computed as
+// host::from_bytes_wide does, lo R^2 + hi R^3 with two Montgomery products.  lo and hi are raw 256-bit values (up to
+// 2^256 - 1, about 2.2 p).  montmul's contract is on the row operand alone (x + p <= 2^256, here R^2 or R^3 < p); the
+// column operand may be any y < 2^256.  So lo and hi need no pre-reduction (no fr_condsub255): each product is
+// (x y + m p) / 2^256 < (p 2^256 + 2^256 p) / 2^256 = 2p, and one conditional subtraction makes it canonical.
+__device__ __forceinline__ void fr_from_bytes_wide(uint32_t (&r)[8], const uint64_t (&w)[8]) {
+    const uint32_t r2[8] = {0xf3f29c6du, 0xc999e990u, 0x87925c23u, 0x2b6cedcbu, 0x7254398fu, 0x05d31496u, 0x9f59ff11u,
+                            0x0748d9d9u};   // R^2 mod p
+    const uint32_t r3[8] = {0x439b73afu, 0xc62c1807u, 0x8cf06990u, 0x1b3e0d18u, 0xc7b5f418u, 0x73d13c71u, 0xc8db33e9u,
+                            0x6e2a5bb9u};   // R^3 mod p
+    uint32_t lo[8], hi[8], a[8], c[8];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        lo[2 * k] = (uint32_t)w[k], lo[2 * k + 1] = (uint32_t)(w[k] >> 32);
+        hi[2 * k] = (uint32_t)w[4 + k], hi[2 * k + 1] = (uint32_t)(w[4 + k] >> 32);
+    }
+    montmul(a, r2, lo);        // lo R mod p, < 2p
+    fr_condsub(a);
+    montmul(c, r3, hi);        // hi 2^256 R mod p, < 2p
+    fr_condsub(c);
+    fr_add_mod(r, a, c);
+}
+
+// 64-bit rotations of the G function: 32 is a word swap, 24 and 16 are two funnel shifts, 63 (a rotation left by 1) two
+// left funnel shifts
+__device__ __forceinline__ uint64_t b2_rotr32(uint64_t x) { return (x << 32) | (x >> 32); }
+template <int kN>
+__device__ __forceinline__ uint64_t b2_rotr(uint64_t x) {   // 0 < kN < 32
+    const uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
+    return ((uint64_t)__funnelshift_r(hi, lo, kN) << 32) | __funnelshift_r(lo, hi, kN);
+}
+__device__ __forceinline__ uint64_t b2_rotr63(uint64_t x) {
+    const uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
+    return ((uint64_t)__funnelshift_l(lo, hi, 1) << 32) | __funnelshift_l(hi, lo, 1);
+}
+
+// The BLAKE2b compression F(h, m, t, last), fully unrolled: the SIGMA schedule is spelled out per round, so every
+// message word is a compile-time register.  t is the byte counter's low word; its high word is 0, a message being
+// shorter than 2^64 bytes.
+__device__ __forceinline__ void blake2b_compress(uint64_t (&h)[8], const uint64_t (&m)[16], uint64_t t, bool last) {
+    uint64_t v[16] = {h[0], h[1], h[2], h[3], h[4], h[5], h[6], h[7],
+                      0x6a09e667f3bcc908ull, 0xbb67ae8584caa73bull, 0x3c6ef372fe94f82bull, 0xa54ff53a5f1d36f1ull,
+                      0x510e527fade682d1ull, 0x9b05688c2b3e6c1full, 0x1f83d9abfb41bd6bull, 0x5be0cd19137e2179ull};
+    v[12] ^= t;
+    if (last) v[14] = ~v[14];
+#define P252_B2G(a, b, c, d, x, y)              \
+    v[a] = v[a] + v[b] + m[x];                  \
+    v[d] = b2_rotr32(v[d] ^ v[a]);              \
+    v[c] = v[c] + v[d];                         \
+    v[b] = b2_rotr<24>(v[b] ^ v[c]);            \
+    v[a] = v[a] + v[b] + m[y];                  \
+    v[d] = b2_rotr<16>(v[d] ^ v[a]);            \
+    v[c] = v[c] + v[d];                         \
+    v[b] = b2_rotr63(v[b] ^ v[c]);
+#define P252_B2ROUND(s0, s1, s2, s3, s4, s5, s6, s7, s8, s9, s10, s11, s12, s13, s14, s15) \
+    P252_B2G(0, 4, 8, 12, s0, s1)                                                          \
+    P252_B2G(1, 5, 9, 13, s2, s3)                                                          \
+    P252_B2G(2, 6, 10, 14, s4, s5)                                                         \
+    P252_B2G(3, 7, 11, 15, s6, s7)                                                         \
+    P252_B2G(0, 5, 10, 15, s8, s9)                                                         \
+    P252_B2G(1, 6, 11, 12, s10, s11)                                                       \
+    P252_B2G(2, 7, 8, 13, s12, s13)                                                        \
+    P252_B2G(3, 4, 9, 14, s14, s15)
+    P252_B2ROUND(0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15)
+    P252_B2ROUND(14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3)
+    P252_B2ROUND(11, 8, 12, 0, 5, 2, 15, 13, 10, 14, 3, 6, 7, 1, 9, 4)
+    P252_B2ROUND(7, 9, 3, 1, 13, 12, 11, 14, 2, 6, 5, 10, 4, 0, 15, 8)
+    P252_B2ROUND(9, 0, 5, 7, 2, 4, 10, 15, 14, 1, 11, 12, 6, 8, 3, 13)
+    P252_B2ROUND(2, 12, 6, 10, 0, 11, 8, 3, 4, 13, 7, 5, 15, 14, 1, 9)
+    P252_B2ROUND(12, 5, 1, 15, 14, 13, 4, 10, 0, 7, 6, 3, 9, 2, 8, 11)
+    P252_B2ROUND(13, 11, 7, 14, 12, 1, 3, 9, 5, 0, 15, 4, 8, 6, 2, 10)
+    P252_B2ROUND(6, 15, 14, 9, 11, 3, 0, 8, 12, 2, 13, 7, 1, 4, 10, 5)
+    P252_B2ROUND(10, 2, 8, 4, 7, 6, 1, 5, 15, 11, 9, 14, 3, 12, 13, 0)
+    P252_B2ROUND(0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13, 14, 15)
+    P252_B2ROUND(14, 10, 4, 8, 9, 15, 13, 6, 1, 12, 0, 2, 11, 7, 5, 3)
+#undef P252_B2ROUND
+#undef P252_B2G
+#pragma unroll
+    for (int i = 0; i < 8; ++i) h[i] ^= v[i] ^ v[i + 8];
+}
+
+// The 16 bytes at the 16-byte aligned address p, those outside [lo, hi) read as zero: one LDG.128 when all 16 lie
+// inside, otherwise byte loads of the inside ones only
+__device__ __forceinline__ uint4 ldg128_within(uintptr_t p, uintptr_t lo, uintptr_t hi) {
+    if (p >= lo && p + 16 <= hi) return ldg128(reinterpret_cast<const void*>(p));
+    uint32_t w[4] = {0, 0, 0, 0};
+#pragma unroll
+    for (int b = 0; b < 16; ++b)
+        if (p + b >= lo && p + b < hi) w[b >> 2] |= (uint32_t)*reinterpret_cast<const uint8_t*>(p + b) << (8 * (b & 3));
+    return make_uint4(w[0], w[1], w[2], w[3]);
+}
+
+// One message block as 16 little-endian words: the r <= 128 bytes at src (any alignment), zero past them.  The aligned
+// 16-byte loads that cover them never leave the caller's buffer [lo, hi) (ldg128_within); the block is then shifted
+// down by src mod 16 bytes -- whole words by selects, the rest by funnel shifts -- so no array is indexed at run time.
+__device__ __forceinline__ void b2_load_block(uint64_t (&m)[16], uintptr_t src, uint32_t r, uintptr_t lo, uintptr_t hi) {
+    const uintptr_t a = src & ~(uintptr_t)15;
+    const uint32_t off = (uint32_t)(src & 15);
+    uint32_t w[36];
+#pragma unroll
+    for (int c = 0; c < 9; ++c) {
+        const uint4 x = (uint32_t)(16 * c) < off + r ? ldg128_within(a + 16 * c, lo, hi) : make_uint4(0, 0, 0, 0);
+        w[4 * c] = x.x, w[4 * c + 1] = x.y, w[4 * c + 2] = x.z, w[4 * c + 3] = x.w;
+    }
+    const bool q1 = (off & 4) != 0, q2 = (off & 8) != 0;
+    const uint32_t sh = (off & 3) * 8;
+    uint32_t y[35], z[33];
+#pragma unroll
+    for (int k = 0; k < 35; ++k) y[k] = q1 ? w[k + 1] : w[k];
+#pragma unroll
+    for (int k = 0; k < 33; ++k) z[k] = q2 ? y[k + 2] : y[k];
+    uint32_t b[32];
+#pragma unroll
+    for (int k = 0; k < 32; ++k) b[k] = __funnelshift_r(z[k], z[k + 1], sh);
+    if (r < 128) {                                         // the last block of a message: zero past its end
+#pragma unroll
+        for (int k = 0; k < 32; ++k) {
+            const uint32_t keep = r > 4u * k ? r - 4u * k : 0u;   // message bytes in word k
+            b[k] = keep >= 4 ? b[k] : b[k] & ((1u << (8 * keep)) - 1u);
+        }
+    }
+#pragma unroll
+    for (int k = 0; k < 16; ++k) m[k] = ((uint64_t)b[2 * k + 1] << 32) | b[2 * k];
+}
+
+// k_hash_to_scalar: one message per thread.  Item i is bytes[offsets[i] - base .. offsets[i+1] - base) of n_bytes; it
+// is valid iff offsets[i] - base <= offsets[i+1] - base <= n_bytes and its length is <= max_len, and no byte outside
+// [bytes, bytes + n_bytes) is read.  out[i] = hash_to_scalar (Montgomery), a zero row for an invalid item, which is
+// counted into *rejected when that is given.  BLAKE2b as host::Blake2b: parameter block 0x01010040, the byte counter
+// after each block, the last block flagged final even when it is full, the empty string one zero block with counter 0.
+// kSorted: thread t hashes item perm[n - 1 - t] of the order k_hash_to_scalar_keys and the sort made (longest first,
+// so that a warp runs messages of nearly equal block counts and the longest start first); otherwise item t.
+template <bool kSorted>
+__global__ void __launch_bounds__(256) k_hash_to_scalar(const uint8_t* __restrict__ bytes, uint64_t base, uint64_t n_bytes,
+                                                        const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ perm,
+                                                        uint32_t n, uint32_t max_len, uint8_t* __restrict__ out,
+                                                        unsigned long long* __restrict__ rejected) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n) return;
+    const uint32_t i = kSorted ? perm[n - 1 - t] : t;
+    const uint64_t a = offsets[i] - base, b = offsets[i + 1] - base, len = b - a;
+    const bool ok = a <= b && b <= n_bytes && len <= max_len;
+    if (rejected) warp_count(rejected, !ok);
+    uint32_t r[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (ok) {
+        uint64_t h[8] = {0x6a09e667f3bcc908ull ^ 0x01010040ull, 0xbb67ae8584caa73bull, 0x3c6ef372fe94f82bull,
+                         0xa54ff53a5f1d36f1ull, 0x510e527fade682d1ull, 0x9b05688c2b3e6c1full, 0x1f83d9abfb41bd6bull,
+                         0x5be0cd19137e2179ull};
+        const uintptr_t lo = reinterpret_cast<uintptr_t>(bytes), hi = lo + n_bytes, src = lo + a;
+        const uint32_t L = (uint32_t)len, nblk = L ? (L + 127) / 128 : 1u;
+#pragma unroll 1
+        for (uint32_t j = 0; j < nblk; ++j) {
+            const uint32_t left = L - 128 * j, take = left < 128 ? left : 128u;
+            uint64_t m[16];
+            b2_load_block(m, src + 128 * j, take, lo, hi);
+            blake2b_compress(h, m, 128ull * j + take, j + 1 == nblk);
+        }
+        fr_from_bytes_wide(r, h);
+    }
+    store_fr(out + (size_t)i * 32, r);
+}
+
+// keys[i] = the block count max(1, ceil(len / 128)) of a valid item (as k_hash_to_scalar decides it), 0 for an invalid
+// one (counted into *rejected); vals[i] = i
+__global__ void __launch_bounds__(256) k_hash_to_scalar_keys(const uint64_t* __restrict__ offsets, uint32_t n, uint64_t base,
+                                                             uint64_t n_bytes, uint32_t max_len, uint32_t* __restrict__ keys,
+                                                             uint32_t* __restrict__ vals,
+                                                             unsigned long long* __restrict__ rejected) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t a = offsets[i] - base, b = offsets[i + 1] - base, len = b - a;
+    const bool ok = a <= b && b <= n_bytes && len <= max_len;
+    keys[i] = ok ? (len ? (uint32_t)((len + 127) / 128) : 1u) : 0u;
+    vals[i] = i;
+    if (rejected) warp_count(rejected, !ok);
+}
+
+// rows of 64 bytes -> BlsScalar::from_bytes_wide, one thread per row
+__global__ void __launch_bounds__(256) k_from_bytes_wide(const uint8_t* __restrict__ in, size_t n, uint8_t* __restrict__ out) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    uint64_t w[8];
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const uint4 x = ldg128(in + i * 64 + 16 * q);
+        w[2 * q] = ((uint64_t)x.y << 32) | x.x;
+        w[2 * q + 1] = ((uint64_t)x.w << 32) | x.z;
+    }
+    uint32_t r[8];
+    fr_from_bytes_wide(r, w);
+    store_fr(out + i * 32, r);
+}
+
+cudaError_t launch_hash_to_scalar(const void* bytes, uint64_t base, uint64_t n_bytes, const uint64_t* offsets,
+                                  const uint32_t* perm, uint32_t n, uint32_t max_len, void* out, unsigned long long* rejected,
+                                  cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    const uint8_t* b = static_cast<const uint8_t*>(bytes);
+    uint8_t* o = static_cast<uint8_t*>(out);
+    if (perm)
+        k_hash_to_scalar<true><<<blocks256(n), 256, 0, st>>>(b, base, n_bytes, offsets, perm, n, max_len, o, rejected);
+    else
+        k_hash_to_scalar<false><<<blocks256(n), 256, 0, st>>>(b, base, n_bytes, offsets, nullptr, n, max_len, o, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_hash_to_scalar_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_bytes, uint32_t max_len,
+                                       uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_hash_to_scalar_keys<<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_bytes, max_len, keys, vals, rejected);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_from_bytes_wide(const void* in, size_t n, void* out, cudaStream_t st) {
+    if (n == 0) return cudaSuccess;
+    k_from_bytes_wide<<<blocks256(n), 256, 0, st>>>(static_cast<const uint8_t*>(in), n, static_cast<uint8_t*>(out));
     return cudaGetLastError();
 }
 

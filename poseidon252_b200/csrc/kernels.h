@@ -329,6 +329,20 @@ cudaError_t launch_msmv_prep_double(const void* pk, const void* pkp, bool pk_bca
 cudaError_t launch_msmv_final_double(const void* wsum, uint32_t nchunks, int c, const void* zsum, uint32_t nsum,
                                      const void* table, const void* table_p, const void* pk, const uint32_t* bad,
                                      unsigned long long* verified, cudaStream_t st);
+// BlsScalar::hash_to_scalar (p252_hash_to_scalar_batch): item i = bytes[offsets[i] - base .. offsets[i+1] - base), valid
+// iff offsets[i] - base <= offsets[i+1] - base <= n_bytes and its length is <= max_len; no byte outside
+// bytes[0, n_bytes) is read, whatever the offsets.  out[i] = BLAKE2b-512 of the item reduced by from_bytes_wide
+// (Montgomery), a zero row for an invalid item (counted into *rejected, device, may be null).  One thread per item;
+// perm (may be null): the item order of launch_hash_to_scalar_keys and the ascending sort, hashed longest first.
+cudaError_t launch_hash_to_scalar(const void* bytes, uint64_t base, uint64_t n_bytes, const uint64_t* offsets,
+                                  const uint32_t* perm, uint32_t n, uint32_t max_len, void* out, unsigned long long* rejected,
+                                  cudaStream_t st);
+// keys[i] = the block count max(1, ceil(len / 128)) of a valid item, 0 for an invalid one (counted into *rejected);
+// vals[i] = i
+cudaError_t launch_hash_to_scalar_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_bytes, uint32_t max_len,
+                                       uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st);
+// BlsScalar::from_bytes_wide (p252_scalars_from_bytes_wide): n rows of 64 bytes -> n scalars (Montgomery)
+cudaError_t launch_from_bytes_wide(const void* in, size_t n, void* out, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -302,6 +302,55 @@ class Engine:
                                                       self._flags(flags, async_)))
         return out, ok
 
+    def scalars_from_bytes_wide(self, data, async_=False):
+        """BlsScalar::from_bytes_wide: (n, 64) uint8 rows (host) or an (n, 8) 64-bit device tensor of the same bytes
+        -> (n, 4) scalars, (lo + hi 2^256) mod p in Montgomery form.  Every row is valid."""
+        if _is_torch(data):
+            ptr, lead, flags, keep = self._in(data, (8,))
+            n = lead[0]
+        else:
+            keep = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1, 64)
+            ptr, n, flags = keep.ctypes.data, keep.shape[0], _native.MEM_HOST
+        out = self._out_like(keep, (n, 4)) if _is_torch(keep) else np.empty((n, 4), dtype=np.uint64)
+        self._check(self._lib.p252_scalars_from_bytes_wide(self._ctx, ptr, n, self._ptr(out), self._flags(flags, async_)))
+        return out
+
+    def hash_to_scalar_batch(self, data, offsets, max_len=None, out=None, async_=False):
+        """n x BlsScalar::hash_to_scalar(data[offsets[i]:offsets[i+1]]) in one call, byte strings of any lengths (0 included).
+        data: a 1-D uint8 numpy array (or bytes) with (n + 1,) uint64 offsets, or a contiguous 1-D uint8 CUDA tensor with
+        int64 / uint64 CUDA offsets; offsets[0] need not be 0.  Returns (n, 4) scalars in Montgomery form, in input order,
+        in the memory space of the inputs: the rows are ready as the msg of the Schnorr calls.  max_len bounds the item
+        lengths in bytes (at most HASH_TO_SCALAR_MAX_LEN); None takes the longest item, which for CUDA tensors costs a
+        device-to-host sync.  Host batches raise on an invalid item and write nothing; device batches give invalid items a
+        zero row and count them (last_hash_to_scalar_rejected())."""
+        if _is_torch(data):
+            if not data.is_cuda or data.device.index != self.device or str(data.dtype) != "torch.uint8" or \
+                    not data.is_contiguous() or data.dim() != 1:
+                raise EngineError(-1, "data must be a contiguous 1-D uint8 tensor on cuda:%d" % self.device)
+            self._fence_torch()
+            dp, nb, flags, dk = data.data_ptr(), int(data.shape[0]), _native.MEM_DEVICE, data
+        else:
+            if isinstance(data, (bytes, bytearray, memoryview)):
+                data = np.frombuffer(data, dtype=np.uint8)
+            dk = np.ascontiguousarray(data, dtype=np.uint8).reshape(-1)
+            dp, nb, flags = dk.ctypes.data, int(dk.shape[0]), _native.MEM_HOST
+        op, n1, ok_ = self._idx(offsets, dk, "offsets")
+        if n1 < 1:
+            raise EngineError(-1, "offsets must have n + 1 >= 1 entries")
+        n = n1 - 1
+        if max_len is None:
+            max_len = self._longest_item(ok_, n)
+        res = self._result(out, (n, 4), ok_)
+        flags = self._flags(flags, async_)
+        rejected = self._counter("hash_to_scalar_rejected", flags)
+        self._check(self._lib.p252_hash_to_scalar_batch(self._ctx, dp, nb, op, n, int(max_len), self._ptr(res),
+                                                        ctypes.byref(rejected), flags))
+        return res
+
+    def last_hash_to_scalar_rejected(self):
+        """Items of the last hash_to_scalar_batch skipped as invalid (device buffers; sync() first after async_)."""
+        return self._last("hash_to_scalar_rejected")
+
     def scalars_to_bytes(self, scalars, async_=False):
         """(n, 4) scalars -> canonical little-endian bytes: (n, 32) uint8 (host) or (n, 4) device tensor."""
         ptr, lead, flags, keep = self._in(scalars, (4,))

@@ -59,6 +59,29 @@ def hash_to_scalar(data: bytes):
     return out
 
 
+def pack_bytes(messages):
+    """A list of byte strings -> (data (sum len_i,) uint8, offsets (n + 1,) uint64, longest len_i), the layout of
+    `Engine.hash_to_scalar_batch`.  Pure host work."""
+    lens = np.fromiter((len(m) for m in messages), dtype=np.uint64, count=len(messages))
+    offsets = np.zeros(len(messages) + 1, dtype=np.uint64)
+    np.cumsum(lens, out=offsets[1:])
+    data = np.frombuffer(b"".join(bytes(m) for m in messages), dtype=np.uint8)
+    return data, offsets, int(lens.max()) if len(messages) else 0
+
+
+def hash_to_scalar_batch(messages, engine=None, max_len=None, out=None, async_=False):
+    """NEW batch entry: n x `hash_to_scalar(messages[i])` on the device, one call for byte strings of any lengths.
+    messages: a list of `bytes` (packed on the host by `pack_bytes`), or a `(data, offsets)` pair as taken by
+    `Engine.hash_to_scalar_batch` (numpy arrays, or CUDA tensors).  Returns (n, 4) Montgomery limbs in input order."""
+    if isinstance(messages, tuple):
+        data, offsets = messages
+    else:
+        data, offsets, longest = pack_bytes(messages)
+        max_len = longest if max_len is None else max_len
+    eng = _engine_for(engine, data)
+    return eng.hash_to_scalar_batch(data, offsets, max_len=max_len, out=out, async_=async_)
+
+
 def io_pattern(domain, chunk_lens, output_len):
     """src/hash.rs:62-85: one Absorb per update() chunk + Squeeze(output_len); Merkle arity check."""
     from .errors import IOPatternViolation
