@@ -211,6 +211,38 @@ struct Io {
     bool device = false; // h_in / h_out is a device buffer: the launch uses it in place at the chunk's offset, nothing staged
 };
 
+// One buffer of a Plan: in a chunk callback, b(d) is its pointer for the chunk, as a T*.
+template <typename T>
+struct Buf {
+    size_t i = 0;
+    T* operator()(void* const* d) const { return static_cast<T*>(d[i]); }
+};
+// The element type of a caller buffer's handle: bytes and integers keep theirs, rows (scalars, points) are untyped.
+template <typename T>
+using Elem = typename std::conditional<std::is_arithmetic<T>::value, T, void>::type;
+
+// The buffers of a batch call, in the order they are carved from a slot arena and staged, `bytes` per item.  in / out /
+// inout are the caller's buffers (used in place when the call's flags say DEVICE); arena buffers are temporaries that
+// live in the arena only.  once: one item read by every item of the batch (Io::once).
+struct Plan {
+    std::vector<Io> ios;
+    bool dev;
+    explicit Plan(int flags) : dev((flags & P252_MEM_DEVICE) != 0) {}
+    template <typename T>
+    Buf<Elem<T>> in(const T* p, size_t bytes, bool once = false) { return add<Elem<T>>({p, nullptr, bytes, once, dev}); }
+    template <typename T>
+    Buf<Elem<T>> out(T* p, size_t bytes) { return add<Elem<T>>({nullptr, p, bytes, false, dev}); }
+    template <typename T>
+    Buf<Elem<T>> inout(T* p, size_t bytes) { return add<Elem<T>>({p, p, bytes, false, dev}); }
+    template <typename T = void>
+    Buf<T> arena(size_t bytes, bool once = false) { return add<T>({nullptr, nullptr, bytes, once}); }
+    template <typename T>
+    Io& operator[](Buf<T> b) { return ios[b.i]; }
+  private:
+    template <typename T>
+    Buf<T> add(Io io) { ios.push_back(io); return {ios.size() - 1}; }
+};
+
 int join_slots(p252_ctx* ctx, int rc, bool wipe);
 
 // Every kernel launch of the library goes through here: a failed launch is reported, a successful one counted.
@@ -219,6 +251,11 @@ int launched(p252_ctx* ctx, cudaError_t le) {
     ctx->launches++;
     return P252_OK;
 }
+// Enqueue one kernel through launched(); a failed launch returns its status, so no later kernel is enqueued.
+#define LAUNCH(call)                                                             \
+    do {                                                                         \
+        if (const int rc__ = launched(ctx, (call)); rc__ != P252_OK) return rc__; \
+    } while (0)
 
 // Tail of every DEVICE-buffer call: the status of its work, then synchronous unless P252_ASYNC.
 int device_done(p252_ctx* ctx, int rc, int flags) {
@@ -310,59 +347,15 @@ size_t pipeline_chunk(const std::vector<Io>& ios, size_t n) {
     return chunk > n ? n : chunk;
 }
 
-// Fixed-size HOST batches: the items stream through the slot arenas in chunks, each buffer of `ios` staged in its own
-// region.  launch(d, cnt, st) enqueues a chunk's kernels, each through launched(), and returns a P252_* status.
-template <typename Launch>
-int run_host_pipeline(p252_ctx* ctx, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
-    if (n == 0) return P252_OK;
-    const size_t chunk = pipeline_chunk(ios, n);
-    std::vector<void*> d(ios.size());
-    auto carve = [&](void* arena) {
-        Carve c{static_cast<uint8_t*>(arena)};
-        for (size_t b = 0; b < ios.size(); ++b)
-            if (!ios[b].device) d[b] = c.take<uint8_t>((ios[b].once ? 1 : chunk) * ios[b].item_bytes);
-        return c.used;
-    };
-    const size_t need = carve(nullptr);
-    return on_slots(ctx, wipe, [&](long long fail_at) -> int {
-        // Ramp-up (batches of several chunks only): the first chunks are small (chunk/8, /4, /2) so that the first
-        // kernel starts after a ~1 MiB copy instead of a full chunk's; from the fourth chunk on every chunk has the
-        // full size.  A batch that fits one chunk is one launch.
-        size_t k = 0, cur = (n > 2 * chunk) ? std::max<size_t>(1024, chunk / 8 / 128 * 128) : chunk;
-        for (size_t off = 0, cnt = 0; off < n; off += cnt, ++k, cur = std::min(chunk, cur * 2)) {
-            cnt = std::min(cur, n - off);
-            Slot& sl = ctx->slots[k % kSlots];
-            int rc = slot_reserve(ctx, sl, need, wipe);
-            if (rc != P252_OK) return rc;
-            carve(sl.arena);
-            for (size_t b = 0; b < ios.size(); ++b) {
-                const Io& io = ios[b];
-                const size_t at = io.once ? 0 : off * io.item_bytes;
-                if (io.device)
-                    d[b] = io.h_out ? static_cast<uint8_t*>(io.h_out) + at
-                                    : const_cast<uint8_t*>(static_cast<const uint8_t*>(io.h_in) + at);
-                else if (io.h_in)
-                    CU(cudaMemcpyAsync(d[b], static_cast<const uint8_t*>(io.h_in) + at, (io.once ? 1 : cnt) * io.item_bytes,
-                                       cudaMemcpyHostToDevice, sl.stream));
-            }
-            if ((long long)k == fail_at) return injected_fault(ctx);
-            if ((rc = launch(d.data(), cnt, sl.stream)) != P252_OK) return rc;
-            for (size_t b = 0; b < ios.size(); ++b)
-                if (ios[b].h_out && !ios[b].device)
-                    CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + off * ios[b].item_bytes, d[b],
-                                       cnt * ios[b].item_bytes, cudaMemcpyDeviceToHost, sl.stream));
-        }
-        return P252_OK;
-    });
-}
-
-// Fixed-size batches whose chunks run in two phases, where the host needs something the first phase computed (a count)
-// before it can enqueue the second: the chunks are staged as in run_host_pipeline, but chunk c's second(d, cnt, st) and
-// its output copies are enqueued after chunk c + 1's first(d, cnt, st), so that while the host waits for chunk c the
-// device already has the next chunk's first phase queued on another slot, and consecutive chunks overlap.  Both callbacks
-// enqueue through launched() and return a P252_* status.
-template <typename First, typename Second>
-int run_host_pipeline2(p252_ctx* ctx, std::vector<Io>& ios, size_t n, First first, Second second, bool wipe = false) {
+// The chunk loop of both pipelines, on the slot streams (on_slots): chunk k goes to slot k % kSlots, whose arena is
+// grown to hold every staged buffer of `ios` and carved into one region per buffer; the chunk's inputs are copied in
+// (DEVICE buffers are used in place at the chunk's offset), and then body(d, off, cnt, st) enqueues the chunk's work
+// on the slot stream st, d being the chunk's buffers in the order of `ios` (valid until that slot's next chunk).
+// Ramp-up (batches of several chunks only): the first chunks are small (chunk/8, /4, /2) so that the first kernel
+// starts after a ~1 MiB copy instead of a full chunk's; from the fourth chunk on every chunk has the full size.  A batch
+// that fits one chunk is one launch.
+template <typename Body>
+int stage_chunks(p252_ctx* ctx, const std::vector<Io>& ios, size_t n, bool wipe, Body body) {
     if (n == 0) return P252_OK;
     const size_t chunk = pipeline_chunk(ios, n);
     std::vector<void*> d[kSlots];
@@ -373,24 +366,8 @@ int run_host_pipeline2(p252_ctx* ctx, std::vector<Io>& ios, size_t n, First firs
             if (!ios[b].device) dd[b] = c.take<uint8_t>((ios[b].once ? 1 : chunk) * ios[b].item_bytes);
         return c.used;
     };
-    const size_t need = carve(nullptr, d[0]);
+    const size_t need = carve(nullptr, d[kSlots - 1]);
     return on_slots(ctx, wipe, [&](long long fail_at) -> int {
-        struct Pending {
-            bool on = false;
-            size_t off = 0, cnt = 0;
-            int slot = 0;
-        } prev;
-        auto finish = [&](const Pending& p) -> int {
-            cudaStream_t st = ctx->slots[p.slot].stream;
-            const int rc = second(d[p.slot].data(), p.cnt, st);
-            if (rc != P252_OK) return rc;
-            for (size_t b = 0; b < ios.size(); ++b)
-                if (ios[b].h_out && !ios[b].device)
-                    CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + p.off * ios[b].item_bytes, d[p.slot][b],
-                                       p.cnt * ios[b].item_bytes, cudaMemcpyDeviceToHost, st));
-            return P252_OK;
-        };
-        // the ramp-up of run_host_pipeline
         size_t k = 0, cur = (n > 2 * chunk) ? std::max<size_t>(1024, chunk / 8 / 128 * 128) : chunk;
         for (size_t off = 0, cnt = 0; off < n; off += cnt, ++k, cur = std::min(chunk, cur * 2)) {
             cnt = std::min(cur, n - off);
@@ -406,15 +383,53 @@ int run_host_pipeline2(p252_ctx* ctx, std::vector<Io>& ios, size_t n, First firs
                     d[s][b] = io.h_out ? static_cast<uint8_t*>(io.h_out) + at
                                        : const_cast<uint8_t*>(static_cast<const uint8_t*>(io.h_in) + at);
                 else if (io.h_in)
-                    CU(cudaMemcpyAsync(d[s][b], static_cast<const uint8_t*>(io.h_in) + at, (io.once ? 1 : cnt) * io.item_bytes,
-                                       cudaMemcpyHostToDevice, sl.stream));
+                    CU(cudaMemcpyAsync(d[s][b], static_cast<const uint8_t*>(io.h_in) + at,
+                                       (io.once ? 1 : cnt) * io.item_bytes, cudaMemcpyHostToDevice, sl.stream));
             }
             if ((long long)k == fail_at) return injected_fault(ctx);
-            if ((rc = first(d[s].data(), cnt, sl.stream)) != P252_OK) return rc;
-            if (prev.on && (rc = finish(prev)) != P252_OK) return rc;
-            prev = Pending{true, off, cnt, s};
+            if ((rc = body(d[s].data(), off, cnt, sl.stream)) != P252_OK) return rc;
         }
-        return finish(prev);
+        return P252_OK;
+    });
+}
+
+// The output copies of a staged chunk (d: its buffers, at items [off, off + cnt)) back to the caller's HOST buffers.
+int copy_out(p252_ctx* ctx, const std::vector<Io>& ios, void* const* d, size_t off, size_t cnt, cudaStream_t st) {
+    for (size_t b = 0; b < ios.size(); ++b)
+        if (ios[b].h_out && !ios[b].device)
+            CU(cudaMemcpyAsync(static_cast<uint8_t*>(ios[b].h_out) + off * ios[b].item_bytes, d[b], cnt * ios[b].item_bytes,
+                               cudaMemcpyDeviceToHost, st));
+    return P252_OK;
+}
+
+// Fixed-size HOST batches: the items stream through the slot arenas in chunks, each buffer of `ios` staged in its own
+// region.  launch(d, cnt, st) enqueues a chunk's kernels, each through launched(), and returns a P252_* status; the
+// chunk's output copies follow it on the same slot stream.
+template <typename Launch>
+int run_host_pipeline(p252_ctx* ctx, const std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
+    return stage_chunks(ctx, ios, n, wipe, [&](void** d, size_t off, size_t cnt, cudaStream_t st) {
+        const int rc = launch(d, cnt, st);
+        return rc != P252_OK ? rc : copy_out(ctx, ios, d, off, cnt, st);
+    });
+}
+
+// Fixed-size batches whose chunks run in two phases, where the host needs something the first phase computed (a count)
+// before it can enqueue the second: the chunks are staged as in run_host_pipeline, but chunk c's second(d, cnt, st) and
+// its output copies are enqueued after chunk c + 1's first(d, cnt, st), so that while the host waits for chunk c the
+// device already has the next chunk's first phase queued on another slot, and consecutive chunks overlap.  Both callbacks
+// enqueue through launched() and return a P252_* status.
+template <typename First, typename Second>
+int run_host_pipeline2(p252_ctx* ctx, const std::vector<Io>& ios, size_t n, First first, Second second, bool wipe = false) {
+    struct Chunk { void** d; size_t off, cnt; cudaStream_t st; } prev{};
+    auto finish = [&](const Chunk& c) -> int {
+        const int rc = second(c.d, c.cnt, c.st);
+        return rc != P252_OK ? rc : copy_out(ctx, ios, c.d, c.off, c.cnt, c.st);
+    };
+    return stage_chunks(ctx, ios, n, wipe, [&](void** d, size_t off, size_t cnt, cudaStream_t st) -> int {
+        int rc = first(d, cnt, st);
+        if (rc != P252_OK || (prev.d && (rc = finish(prev)) != P252_OK)) return rc;
+        prev = Chunk{d, off, cnt, st};
+        return off + cnt == n ? finish(prev) : P252_OK;   // the last chunk
     });
 }
 
@@ -536,17 +551,25 @@ struct Counts {
     }
 };
 
-// A single-launch batch call states its launch once, as launch(d, cnt, st) over the buffers of `ios`: DEVICE buffers run it
-// once on the context stream with the caller's pointers, HOST buffers through run_host_pipeline with the staged ones.
+// A single-launch batch call states its launch once, as launch(d, cnt, st) over the buffers of `plan`: DEVICE buffers run
+// it once on the context stream with the caller's pointers, HOST buffers through run_host_pipeline with the staged ones.
 template <typename Launch>
-int launch_batch(const Counts& counts, std::vector<Io>& ios, size_t n, Launch launch, bool wipe = false) {
-    if (!(counts.flags & P252_MEM_DEVICE)) return counts.end(run_host_pipeline(counts.ctx, ios, n, launch, wipe));
+int launch_batch(const Counts& counts, const Plan& plan, size_t n, Launch launch, bool wipe = false) {
+    if (!(counts.flags & P252_MEM_DEVICE)) return counts.end(run_host_pipeline(counts.ctx, plan.ios, n, launch, wipe));
     if (n == 0) return P252_OK;
     const int rc = counts.begin();
     if (rc != P252_OK) return rc;
     std::vector<void*> d;
-    for (const Io& io : ios) d.push_back(io.h_out ? io.h_out : const_cast<void*>(io.h_in));
+    for (const Io& io : plan.ios) d.push_back(io.h_out ? io.h_out : const_cast<void*>(io.h_in));
     return counts.end(launch(d.data(), n, counts.ctx->stream));
+}
+
+// A batch call that runs through the slot arenas for both memory spaces (DEVICE buffers used in place, chunk by chunk):
+// the device counters are zeroed, the chunks run, and the counts are published.  Called after the n == 0 return.
+template <typename Launch>
+int staged_batch(const Counts& counts, const Plan& plan, size_t n, Launch launch, bool wipe = false) {
+    const int rc = counts.begin();
+    return counts.end(rc != P252_OK ? rc : run_host_pipeline(counts.ctx, plan.ios, n, launch, wipe));
 }
 
 uint64_t domain_sep(int domain, bool* ok) {
@@ -860,9 +883,10 @@ static int permute_impl(p252_ctx* ctx, p252_fr* states, size_t n, int flags, boo
     if (!ctx || !args_ok(n, flags, {states})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    std::vector<Io> ios = {{states, states, 160}};
-    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_permute(d[0], cnt, dense, ctx->coop_max, st));
+    Plan p(flags);
+    const auto d_states = p.inout(states, 160);
+    return launch_batch(Counts(ctx, flags), p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_permute(d_states(d), cnt, dense, ctx->coop_max, st));
     });
 }
 
@@ -884,9 +908,11 @@ static int digest_impl(p252_ctx* ctx, const p252_fr* tag, const p252_fr* in, siz
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const uint32_t il = (uint32_t)in_len, ol = (uint32_t)out_len;
-    std::vector<Io> ios = {{in, nullptr, in_len * 32}, {nullptr, out, out_len * 32}};
-    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_digest(limbs(tag), d[0], cnt, il, d[1], ol, truncate, ctx->coop_max, st));
+    Plan p(flags);
+    const auto d_in = p.in(in, in_len * 32), d_out = p.out(out, out_len * 32);
+    return launch_batch(Counts(ctx, flags), p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_digest(limbs(tag), d_in(d), cnt, il, d_out(d), ol, truncate, ctx->coop_max,
+                                                 st));
     });
 }
 
@@ -915,11 +941,12 @@ static int convert_impl(p252_ctx* ctx, const void* in, size_t n, void* out, uint
     if (!ctx || !args_ok(n, flags, {in, out})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    std::vector<Io> ios = {{in, nullptr, 32}, {nullptr, out, 32}};
-    if (from_bytes && ok) ios.push_back({nullptr, ok, 1});
-    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = (from_bytes && ok) ? static_cast<uint8_t*>(d[2]) : nullptr;
-        return launched(ctx, p252::launch_convert(d[0], cnt, d[1], okc, from_bytes, st));
+    Plan p(flags);
+    const auto d_in = p.in(in, 32), d_out = p.out(out, 32);
+    const bool with_ok = from_bytes && ok;
+    const auto d_ok = with_ok ? p.out(ok, 1) : Buf<uint8_t>{};
+    return launch_batch(Counts(ctx, flags), p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_convert(d_in(d), cnt, d_out(d), with_ok ? d_ok(d) : nullptr, from_bytes, st));
     });
 }
 
@@ -935,9 +962,11 @@ int p252_scalars_from_bytes_wide(p252_ctx* ctx, const uint8_t* bytes, size_t n, 
     if (!ctx || !args_ok(n, flags, {bytes, out})) return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    std::vector<Io> ios = {{bytes, nullptr, 64}, {nullptr, out, 32}};
-    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_from_bytes_wide(d[0], cnt, d[1], st));
+    Plan p(flags);
+    const auto d_bytes = p.in(bytes, 64);
+    const auto d_out = p.out(out, 32);
+    return launch_batch(Counts(ctx, flags), p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_from_bytes_wide(d_bytes(d), cnt, d_out(d), st));
     });
 }
 
@@ -951,10 +980,12 @@ int p252_encrypt_batch(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, co
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const uint32_t l32 = (uint32_t)L;
-    std::vector<Io> ios = {{msg, nullptr, L * 32}, {secret_uv, nullptr, 64}, {nonce, nullptr, 32},
-                           {nullptr, cipher, (L + 1) * 32}};
-    return launch_batch(Counts(ctx, flags), ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], st));
+    Plan p(flags);
+    const auto d_msg = p.in(msg, L * 32), d_secret = p.in(secret_uv, 64), d_nonce = p.in(nonce, 32),
+               d_cipher = p.out(cipher, (L + 1) * 32);
+    return launch_batch(Counts(ctx, flags), p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_encrypt(limbs(&tag), d_msg(d), cnt, l32, d_secret(d), d_nonce(d), d_cipher(d),
+                                                  st));
     }, /*wipe=*/true);
 }
 
@@ -969,11 +1000,13 @@ int p252_decrypt_batch(p252_ctx* ctx, const p252_fr* cipher, size_t n, size_t L,
     DeviceGuard g(ctx->device);
     const uint32_t l32 = (uint32_t)L;
     const Counts counts(ctx, flags, n_failed, ok, n);
-    std::vector<Io> ios = {{cipher, nullptr, (L + 1) * 32}, {secret_uv, nullptr, 64}, {nonce, nullptr, 32},
-                           {nullptr, msg, L * 32}, {nullptr, ok, 1}};
-    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[1], d[2], d[3], static_cast<uint8_t*>(d[4]),
-                                                  counts.counter(0), st));
+    Plan p(flags);
+    const auto d_cipher = p.in(cipher, (L + 1) * 32), d_secret = p.in(secret_uv, 64), d_nonce = p.in(nonce, 32),
+               d_msg = p.out(msg, L * 32);
+    const auto d_ok = p.out(ok, 1);
+    return launch_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_decrypt(limbs(&tag), d_cipher(d), cnt, l32, d_secret(d), d_nonce(d), d_msg(d),
+                                                  d_ok(d), counts.counter(0), st));
     }, /*wipe=*/true);
 }
 
@@ -986,9 +1019,12 @@ int p252_dhke_batch(p252_ctx* ctx, const p252_jscalar* secret, size_t n_secret, 
     DeviceGuard g(ctx->device);
     const bool sb = n_secret == 1, pb = n_public == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
-    std::vector<Io> ios = {{secret, nullptr, 32, sb}, {public_uv, nullptr, 64, pb}, {nullptr, shared_uv, 64}, {nullptr, ok, 1}};
-    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_dhke(d[0], sb, d[1], pb, cnt, d[2], static_cast<uint8_t*>(d[3]), counts.counter(0), st));
+    Plan p(flags);
+    const auto d_secret = p.in(secret, 32, sb), d_public = p.in(public_uv, 64, pb), d_shared = p.out(shared_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    return launch_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_dhke(d_secret(d), sb, d_public(d), pb, cnt, d_shared(d), d_ok(d),
+                                               counts.counter(0), st));
     }, /*wipe=*/true);
 }
 
@@ -1007,28 +1043,24 @@ static int crypt_dhke(p252_ctx* ctx, bool decrypt, const p252_fr* in, size_t n, 
     if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1, pb = n_public == 1;
+    const bool sb = n_secret == 1, pb = n_public == 1;
     const uint32_t l32 = (uint32_t)L, out_row = decrypt ? l32 : l32 + 1;
     const Counts counts(ctx, flags, count, ok, n);
     if (n == 0) return P252_OK;
-    if ((rc = counts.begin()) != P252_OK) return rc;
-    // 0 input, 1 secret, 2 public, 3 nonce, 4 output, 5 ok; 6 shared secrets and 7 validity live in the arena only
-    std::vector<Io> ios = {{in, nullptr, (decrypt ? L + 1 : L) * 32, false, dev}, {secret, nullptr, 32, sb, dev},
-                           {public_uv, nullptr, 64, pb, dev}, {nonce, nullptr, 32, false, dev},
-                           {nullptr, out, (size_t)out_row * 32, false, dev}, {nullptr, ok, 1, false, dev},
-                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[5]);
-        uint8_t* valid = static_cast<uint8_t*>(d[7]);
+    Plan p(flags);
+    const auto d_in = p.in(in, (decrypt ? L + 1 : L) * 32), d_secret = p.in(secret, 32, sb),
+               d_public = p.in(public_uv, 64, pb), d_nonce = p.in(nonce, 32), d_out = p.out(out, (size_t)out_row * 32);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
         unsigned long long* counter = counts.counter(0);
-        int e = launched(ctx, p252::launch_dhke(d[1], sb, d[2], pb, cnt, d[6], valid, nullptr, st));
-        if (e == P252_OK)
-            e = launched(ctx, decrypt ? p252::launch_decrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], okc, counter, st)
-                                      : p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[6], d[3], d[4], st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(decrypt, valid, cnt, d[4], out_row, okc, counter, st));
-        return e;
+        LAUNCH(p252::launch_dhke(d_secret(d), sb, d_public(d), pb, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(decrypt ? p252::launch_decrypt(limbs(&tag), d_in(d), cnt, l32, d_shared(d), d_nonce(d), d_out(d), d_ok(d),
+                                              counter, st)
+                       : p252::launch_encrypt(limbs(&tag), d_in(d), cnt, l32, d_shared(d), d_nonce(d), d_out(d), st));
+        return launched(ctx, p252::launch_dhke_fix(decrypt, d_valid(d), cnt, d_out(d), out_row, d_ok(d), counter, st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 int p252_encrypt_batch_dhke(p252_ctx* ctx, const p252_fr* msg, size_t n, size_t L, const p252_jscalar* secret, size_t n_secret,
@@ -1086,9 +1118,12 @@ int p252_fixed_base_batch(p252_ctx* ctx, const p252_fr* base_uv, const p252_jsca
     if (n == 0) return P252_OK;
     const void* table = nullptr;
     if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
-    std::vector<Io> ios = {{secret, nullptr, 32}, {nullptr, out_uv, 64}, {nullptr, ok, 1}};
-    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[1], static_cast<uint8_t*>(d[2]), counts.counter(0), st));
+    Plan p(flags);
+    const auto d_secret = p.in(secret, 32), d_out = p.out(out_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    return launch_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_fixed_base(d_secret(d), cnt, table, d_out(d), d_ok(d), counts.counter(0),
+                                                     st));
     }, /*wipe=*/true);
 }
 
@@ -1106,29 +1141,25 @@ int p252_encrypt_batch_ephemeral(p252_ctx* ctx, const p252_fr* msg, size_t n, si
     if (rc != P252_OK || (rc = base_check(base_uv)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const uint32_t l32 = (uint32_t)L;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 message, 1 r, 2 public, 3 nonce, 4 cipher, 5 R, 6 ok; 7 shared secrets and 8 validity live in the arena only
-    std::vector<Io> ios = {{msg, nullptr, L * 32, false, dev}, {r, nullptr, 32, false, dev}, {public_uv, nullptr, 64, pb, dev},
-                           {nonce, nullptr, 32, false, dev}, {nullptr, cipher, (size_t)(l32 + 1) * 32, false, dev},
-                           {nullptr, R_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64},
-                           {nullptr, nullptr, 1}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[6]);
-        uint8_t* valid = static_cast<uint8_t*>(d[8]);
-        int e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table, d[5], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke(d[1], false, d[2], pb, cnt, d[7], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_encrypt(limbs(&tag), d[0], cnt, l32, d[7], d[3], d[4], st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[4], l32 + 1, okc, counts.counter(0), st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[5], 2, okc, nullptr, st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_msg = p.in(msg, L * 32), d_r = p.in(r, 32), d_public = p.in(public_uv, 64, pb),
+               d_nonce = p.in(nonce, 32), d_cipher = p.out(cipher, (size_t)(l32 + 1) * 32), d_R = p.out(R_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table, d_R(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_dhke(d_r(d), false, d_public(d), pb, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_encrypt(limbs(&tag), d_msg(d), cnt, l32, d_shared(d), d_nonce(d), d_cipher(d), st));
+        LAUNCH(p252::launch_dhke_fix(false, d_valid(d), cnt, d_cipher(d), l32 + 1, d_ok(d), counts.counter(0), st));
+        return launched(ctx, p252::launch_dhke_fix(false, d_valid(d), cnt, d_R(d), 2, d_ok(d), nullptr, st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // ---- stealth addresses: the sender's (R, note_pk) and the receiver's ownership scan ----------------------------------
@@ -1149,27 +1180,25 @@ int p252_stealth_address_batch(p252_ctx* ctx, const p252_jscalar* r, size_t n, c
     if (rc != P252_OK || (rc = stealth_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 r, 1 A, 2 B, 3 R, 4 note_pk, 5 ok; 6 shared points, 7 validity and 8 h live in the arena only
-    std::vector<Io> ios = {{r, nullptr, 32, false, dev}, {A_uv, nullptr, 64, pb, dev}, {B_uv, nullptr, 64, pb, dev},
-                           {nullptr, R_uv, 64, false, dev}, {nullptr, note_pk_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
-                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[5]);
-        uint8_t* valid = static_cast<uint8_t*>(d[7]);
-        int e = launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[3], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke(d[0], false, d[1], pb, cnt, d[6], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_stealth_derive(d[8], cnt, table, d[2], pb, valid, d[3], d[4], okc, counts.counter(0),
-                                                          st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_r = p.in(r, 32), d_A = p.in(A_uv, 64, pb), d_B = p.in(B_uv, 64, pb), d_R = p.out(R_uv, 64),
+               d_note_pk = p.out(note_pk_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_h = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table, d_R(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_dhke(d_r(d), false, d_A(d), pb, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_shared(d), cnt, 2, d_h(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_stealth_derive(d_h(d), cnt, table, d_B(d), pb, d_valid(d), d_R(d),
+                                                         d_note_pk(d), d_ok(d), counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // The receiver's B is public and a HOST pointer, like the base: checked here, and its Niels form computed once on the host
@@ -1186,26 +1215,24 @@ int p252_stealth_owns_batch(p252_ctx* ctx, const p252_jscalar* view_a, const p25
     if ((rc = stealth_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0;
     const Counts counts = Counts::device(ctx, flags, n_owned, n_invalid);
     if (n == 0) return P252_OK;
     uint64_t nb[12];
     p252::host::jubjub_niels(nb, spend_B_uv[0].l, spend_B_uv[1].l);
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 view_a, 1 R, 2 note_pk, 3 owned; 4 shared points, 5 validity and 6 h live in the arena only
-    std::vector<Io> ios = {{view_a, nullptr, 32, true, dev}, {R_uv, nullptr, 64, false, dev}, {note_pk_uv, nullptr, 64, false, dev},
-                           {nullptr, owned, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* valid = static_cast<uint8_t*>(d[5]);
-        int e = launched(ctx, p252::launch_dhke(d[0], true, d[1], false, cnt, d[4], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[4], cnt, 2, d[6], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_stealth_owns(d[6], cnt, table, nb, d[2], valid, static_cast<uint8_t*>(d[3]),
-                                                        counts.counter(0), counts.counter(1), st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_a = p.in(view_a, 32, true), d_R = p.in(R_uv, 64), d_note_pk = p.in(note_pk_uv, 64);
+    const auto d_owned = p.out(owned, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_h = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_dhke(d_a(d), true, d_R(d), false, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_shared(d), cnt, 2, d_h(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_stealth_owns(d_h(d), cnt, table, nb, d_note_pk(d), d_valid(d), d_owned(d),
+                                                       counts.counter(0), counts.counter(1), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // ---- Schnorr signatures over JubJub: signing and verification ----------------------------------------------------------
@@ -1226,25 +1253,23 @@ int p252_schnorr_sign_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secr
     if (rc != P252_OK || (rc = schnorr_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 sk, 1 r, 2 msg, 3 u, 4 R, 5 ok; 6 the digest rows and 7 c live in the arena only
-    std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev},
-                           {nullptr, u_out, 32, false, dev}, {nullptr, R_uv, 64, false, dev}, {nullptr, ok, 1, false, dev},
-                           {nullptr, nullptr, 96}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[5]);
-        int e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table, d[4], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_schnorr_pack(d[4], d[2], cnt, d[6], okc, true, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[6], cnt, 3, d[7], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_schnorr_sign(d[0], sb, d[1], d[7], cnt, d[3], d[4], okc, counts.counter(0), st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_sk = p.in(sk, 32, sb), d_r = p.in(r, 32), d_msg = p.in(msg, 32), d_u = p.out(u_out, 32),
+               d_R = p.out(R_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_rows = p.arena(96), d_c = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table, d_R(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_schnorr_pack(d_R(d), d_msg(d), cnt, d_rows(d), d_ok(d), true, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 3, d_c(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_schnorr_sign(d_sk(d), sb, d_r(d), d_c(d), cnt, d_u(d), d_R(d), d_ok(d),
+                                                       counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // An item's verified flag does not tell an invalid item from a signature that does not verify, so both counts come from
@@ -1259,25 +1284,23 @@ int p252_schnorr_verify_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_publ
     if (rc != P252_OK || (rc = schnorr_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts = Counts::device(ctx, flags, n_verified, n_invalid);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 PK, 1 u, 2 R, 3 msg, 4 verified; 5 the digest rows, 6 validity and 7 c live in the arena only
-    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev}, {R_uv, nullptr, 64, false, dev},
-                           {msg, nullptr, 32, false, dev}, {nullptr, verified, 1, false, dev}, {nullptr, nullptr, 96},
-                           {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* valid = static_cast<uint8_t*>(d[6]);
-        int e = launched(ctx, p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_schnorr_verify(d[0], pb, d[1], d[2], d[7], valid, cnt, table,
-                                                          static_cast<uint8_t*>(d[4]), counts.counter(0), counts.counter(1), st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_pk = p.in(pk_uv, 64, pb), d_u = p.in(u, 32), d_R = p.in(R_uv, 64), d_msg = p.in(msg, 32);
+    const auto d_verified = p.out(verified, 1);
+    const auto d_rows = p.arena(96);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_c = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_schnorr_pack(d_R(d), d_msg(d), cnt, d_rows(d), d_valid(d), false, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 3, d_c(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_schnorr_verify(d_pk(d), pb, d_u(d), d_R(d), d_c(d), d_valid(d), cnt, table,
+                                                         d_verified(d), counts.counter(0), counts.counter(1), st));
     });
-    return counts.end(rc);
 }
 
 // ---- note nullifiers: Hash::digest(Domain::Other, [pk'.u, pk'.v, pos])[0], pk' = [(hash([a] R) + b) mod r_J] G' --------
@@ -1297,29 +1320,27 @@ int p252_nullifier_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscala
     if (rc != P252_OK || (rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_tag(&tag_n)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 a, 1 b, 2 R, 3 pos, 4 nullifier, 5 ok; 6 shared points, 7 validity, 8 h and 9 the digest rows live in the arena only
-    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev},
-                           {pos, nullptr, 8, false, dev}, {nullptr, nullifier, 32, false, dev}, {nullptr, ok, 1, false, dev},
-                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 96}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* valid = static_cast<uint8_t*>(d[7]);
-        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[2], false, cnt, d[6], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[6], cnt, 2, d[8], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_nullifier_key(d[8], d[1], sb, static_cast<const uint64_t*>(d[3]), cnt, table, d[9],
-                                                         valid, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_n), d[9], cnt, 3, d[4], 1, false, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_dhke_fix(false, valid, cnt, d[4], 1, static_cast<uint8_t*>(d[5]), counts.counter(0),
-                                                    st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_a = p.in(a, 32, sb), d_b = p.in(b, 32, sb), d_R = p.in(R_uv, 64);
+    const auto d_pos = p.in(pos, 8);
+    const auto d_nullifier = p.out(nullifier, 32);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_h = p.arena(32), d_rows = p.arena(96);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_dhke(d_a(d), sb, d_R(d), false, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_digest(limbs(&tag_h), d_shared(d), cnt, 2, d_h(d), 1, true, ctx->coop_max, st));
+        LAUNCH(p252::launch_nullifier_key(d_h(d), d_b(d), sb, d_pos(d), cnt, table, d_rows(d), d_valid(d), st));
+        LAUNCH(p252::launch_digest(limbs(&tag_n), d_rows(d), cnt, 3, d_nullifier(d), 1, false, ctx->coop_max, st));
+        return launched(ctx, p252::launch_dhke_fix(false, d_valid(d), cnt, d_nullifier(d), 1, d_ok(d),
+                                                   counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // ---- double-key Schnorr signatures over G and G' (jubjub-schnorr SignatureDouble) and note signing ----------------------
@@ -1351,27 +1372,24 @@ int p252_schnorr_sign_double_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t
     if ((rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
-    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 sk, 1 r, 2 msg, 3 u, 4 R, 5 R', 6 ok; 7 the digest rows and 8 c live in the arena only
-    std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev},
-                           {nullptr, u_out, 32, false, dev}, {nullptr, R_uv, 64, false, dev}, {nullptr, Rp_uv, 64, false, dev},
-                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 160}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[6]);
-        int e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table, d[4], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_fixed_base(d[1], cnt, table_p, d[5], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_schnorr_pack_double(d[4], d[5], d[2], cnt, d[7], okc, true, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[7], cnt, 5, d[8], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_schnorr_sign_double(d[0], sb, d[1], d[8], cnt, d[3], d[4], d[5], okc,
-                                                               counts.counter(0), st));
-        return e;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_sk = p.in(sk, 32, sb), d_r = p.in(r, 32), d_msg = p.in(msg, 32), d_u = p.out(u_out, 32),
+               d_R = p.out(R_uv, 64), d_Rp = p.out(Rp_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_rows = p.arena(160), d_c = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table, d_R(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table_p, d_Rp(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_schnorr_pack_double(d_R(d), d_Rp(d), d_msg(d), cnt, d_rows(d), d_ok(d), true, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 5, d_c(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_schnorr_sign_double(d_sk(d), sb, d_r(d), d_c(d), cnt, d_u(d), d_R(d), d_Rp(d),
+                                                              d_ok(d), counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // As p252_schnorr_verify_batch, both counts come from the device counters (0: verified, 1: invalid) for both memory
@@ -1389,27 +1407,25 @@ int p252_schnorr_verify_double_batch(p252_ctx* ctx, const p252_fr* pk_uv, const 
     if ((rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts = Counts::device(ctx, flags, n_verified, n_invalid);
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
-    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 PK, 1 PK', 2 u, 3 R, 4 R', 5 msg, 6 verified; 7 the digest rows, 8 validity and 9 c live in the arena only
-    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {pkp_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev},
-                           {R_uv, nullptr, 64, false, dev}, {Rp_uv, nullptr, 64, false, dev}, {msg, nullptr, 32, false, dev},
-                           {nullptr, verified, 1, false, dev}, {nullptr, nullptr, 160}, {nullptr, nullptr, 1},
-                           {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* valid = static_cast<uint8_t*>(d[8]);
-        int e = launched(ctx, p252::launch_schnorr_pack_double(d[3], d[4], d[5], cnt, d[7], valid, false, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[7], cnt, 5, d[9], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_schnorr_verify_double(d[0], d[1], pb, d[2], d[3], d[4], d[9], valid, cnt, table,
-                                                                 table_p, static_cast<uint8_t*>(d[6]), counts.counter(0),
-                                                                 counts.counter(1), st));
-        return e;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_pk = p.in(pk_uv, 64, pb), d_pkp = p.in(pkp_uv, 64, pb), d_u = p.in(u, 32), d_R = p.in(R_uv, 64),
+               d_Rp = p.in(Rp_uv, 64), d_msg = p.in(msg, 32);
+    const auto d_verified = p.out(verified, 1);
+    const auto d_rows = p.arena(160);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_c = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_schnorr_pack_double(d_R(d), d_Rp(d), d_msg(d), cnt, d_rows(d), d_valid(d), false, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 5, d_c(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_schnorr_verify_double(d_pk(d), d_pkp(d), pb, d_u(d), d_R(d), d_Rp(d), d_c(d),
+                                                                d_valid(d), cnt, table, table_p, d_verified(d),
+                                                                counts.counter(0), counts.counter(1), st));
     });
-    return counts.end(rc);
 }
 
 int p252_note_sign_double_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
@@ -1425,33 +1441,30 @@ int p252_note_sign_double_batch(p252_ctx* ctx, const p252_jscalar* a, const p252
     if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
-    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 a, 1 b, 2 R_note, 3 r, 4 msg, 5 u, 6 R, 7 R', 8 pk', 9 ok; 10 shared points, 11 their validity, 12 h, 13 the digest
-    // rows and 14 c live in the arena only
-    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {note_R_uv, nullptr, 64, false, dev},
-                           {r, nullptr, 32, false, dev}, {msg, nullptr, 32, false, dev}, {nullptr, u_out, 32, false, dev},
-                           {nullptr, R_uv, 64, false, dev}, {nullptr, Rp_uv, 64, false, dev}, {nullptr, pkp_uv, 64, false, dev},
-                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32},
-                           {nullptr, nullptr, 160}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[9]);
-        uint8_t* valid = static_cast<uint8_t*>(d[11]);
-        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[2], false, cnt, d[10], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[10], cnt, 2, d[12], 1, true, ctx->coop_max, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_fixed_base(d[3], cnt, table, d[6], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_fixed_base(d[3], cnt, table_p, d[7], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_schnorr_pack_double(d[6], d[7], d[4], cnt, d[13], okc, true, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[13], cnt, 5, d[14], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_note_sign_double(d[1], sb, d[12], valid, d[3], d[14], cnt, table_p, d[5], d[6], d[7],
-                                                            d[8], okc, counts.counter(0), st));
-        return e;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_a = p.in(a, 32, sb), d_b = p.in(b, 32, sb), d_note_R = p.in(note_R_uv, 64), d_r = p.in(r, 32),
+               d_msg = p.in(msg, 32), d_u = p.out(u_out, 32), d_R = p.out(R_uv, 64), d_Rp = p.out(Rp_uv, 64),
+               d_pkp = p.out(pkp_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_h = p.arena(32), d_rows = p.arena(160), d_c = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_dhke(d_a(d), sb, d_note_R(d), false, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_digest(limbs(&tag_h), d_shared(d), cnt, 2, d_h(d), 1, true, ctx->coop_max, st));
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table, d_R(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table_p, d_Rp(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_schnorr_pack_double(d_R(d), d_Rp(d), d_msg(d), cnt, d_rows(d), d_ok(d), true, st));
+        LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 5, d_c(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_note_sign_double(d_b(d), sb, d_h(d), d_valid(d), d_r(d), d_c(d), cnt, table_p,
+                                                           d_u(d), d_R(d), d_Rp(d), d_pkp(d), d_ok(d),
+                                                           counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // ---- note values: commitments C = [v] G + [blinder] G', creating obfuscated notes and opening them ----------------------
@@ -1473,19 +1486,18 @@ int p252_value_commit_batch(p252_ctx* ctx, const uint64_t* value, const p252_jsc
     if ((rc = base_check(G_uv)) != P252_OK || (rc = base_check(Gp_uv)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
-    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 value, 1 blinder, 2 commitment, 3 ok
-    std::vector<Io> ios = {{value, nullptr, 8, false, dev}, {blinder, nullptr, 32, false, dev},
-                           {nullptr, commitment_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_value_commit(static_cast<const uint64_t*>(d[0]), d[1], cnt, table, table_p, d[2],
-                                                       static_cast<uint8_t*>(d[3]), counts.counter(0), st));
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_value = p.in(value, 8);
+    const auto d_blinder = p.in(blinder, 32), d_C = p.out(commitment_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_value_commit(d_value(d), d_blinder(d), cnt, table, table_p, d_C(d), d_ok(d),
+                                                       counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 int p252_note_create_batch(p252_ctx* ctx, const p252_jscalar* r, const uint64_t* value, const p252_jscalar* blinder,
@@ -1501,37 +1513,33 @@ int p252_note_create_batch(p252_ctx* ctx, const p252_jscalar* r, const uint64_t*
     if ((rc = stealth_tag(&tag_h)) != P252_OK || (rc = p252_encryption_tag(2, &tag_e)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
-    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 r, 1 value, 2 blinder, 3 nonce, 4 A, 5 B, 6 R, 7 note_pk, 8 commitment, 9 cipher, 10 ok; 11 shared points,
-    // 12 validity, 13 h and 14 the message rows live in the arena only
-    std::vector<Io> ios = {{r, nullptr, 32, false, dev}, {value, nullptr, 8, false, dev}, {blinder, nullptr, 32, false, dev},
-                           {nonce, nullptr, 32, false, dev}, {A_uv, nullptr, 64, pb, dev}, {B_uv, nullptr, 64, pb, dev},
-                           {nullptr, R_uv, 64, false, dev}, {nullptr, note_pk_uv, 64, false, dev},
-                           {nullptr, commitment_uv, 64, false, dev}, {nullptr, cipher, 96, false, dev},
-                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32},
-                           {nullptr, nullptr, 64}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[10]);
-        uint8_t* valid = static_cast<uint8_t*>(d[12]);
-        int e = launched(ctx, p252::launch_fixed_base(d[0], cnt, table, d[6], okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke(d[0], false, d[4], pb, cnt, d[11], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[11], cnt, 2, d[13], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_note_value(static_cast<const uint64_t*>(d[1]), d[2], cnt, table, table_p, d[8], d[14],
-                                                      valid, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_stealth_derive(d[13], cnt, table, d[5], pb, valid, d[6], d[7], okc, counts.counter(0),
-                                                          st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_encrypt(limbs(&tag_e), d[14], cnt, 2, d[11], d[3], d[9], st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(false, okc, cnt, d[9], 3, okc, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_dhke_fix(false, okc, cnt, d[8], 2, okc, nullptr, st));
-        return e;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_r = p.in(r, 32);
+    const auto d_value = p.in(value, 8);
+    const auto d_blinder = p.in(blinder, 32), d_nonce = p.in(nonce, 32), d_A = p.in(A_uv, 64, pb),
+               d_B = p.in(B_uv, 64, pb), d_R = p.out(R_uv, 64), d_note_pk = p.out(note_pk_uv, 64),
+               d_C = p.out(commitment_uv, 64), d_cipher = p.out(cipher, 96);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_h = p.arena(32), d_rows = p.arena(64);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_fixed_base(d_r(d), cnt, table, d_R(d), d_ok(d), nullptr, st));
+        LAUNCH(p252::launch_dhke(d_r(d), false, d_A(d), pb, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_digest(limbs(&tag_h), d_shared(d), cnt, 2, d_h(d), 1, true, ctx->coop_max, st));
+        LAUNCH(p252::launch_note_value(d_value(d), d_blinder(d), cnt, table, table_p, d_C(d), d_rows(d), d_valid(d),
+                                       st));
+        LAUNCH(p252::launch_stealth_derive(d_h(d), cnt, table, d_B(d), pb, d_valid(d), d_R(d), d_note_pk(d), d_ok(d),
+                                           counts.counter(0), st));
+        LAUNCH(p252::launch_encrypt(limbs(&tag_e), d_rows(d), cnt, 2, d_shared(d), d_nonce(d), d_cipher(d), st));
+        LAUNCH(p252::launch_dhke_fix(false, d_ok(d), cnt, d_cipher(d), 3, d_ok(d), nullptr, st));
+        return launched(ctx, p252::launch_dhke_fix(false, d_ok(d), cnt, d_C(d), 2, d_ok(d), nullptr, st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 int p252_note_open_batch(p252_ctx* ctx, const p252_jscalar* a, size_t n_secret, const p252_fr* R_uv, const p252_fr* nonce,
@@ -1547,28 +1555,27 @@ int p252_note_open_batch(p252_ctx* ctx, const p252_jscalar* a, size_t n_secret, 
     if ((rc = p252_encryption_tag(2, &tag_e)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_failed, ok, n);
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
-    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 a, 1 R, 2 nonce, 3 cipher, 4 commitment, 5 value, 6 blinder, 7 ok; 8 shared points, 9 validity and 10 the
-    // plaintext rows live in the arena only
-    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev}, {nonce, nullptr, 32, false, dev},
-                           {cipher, nullptr, 96, false, dev}, {commitment_uv, nullptr, 64, false, dev},
-                           {nullptr, value, 8, false, dev}, {nullptr, blinder, 32, false, dev}, {nullptr, ok, 1, false, dev},
-                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 64}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[7]);
-        uint8_t* valid = static_cast<uint8_t*>(d[9]);
-        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[1], false, cnt, d[8], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_decrypt(limbs(&tag_e), d[3], cnt, 2, d[8], d[2], d[10], okc, nullptr, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_note_open_value(d[10], valid, d[4], cnt, table, table_p, static_cast<uint64_t*>(d[5]),
-                                                           d[6], okc, counts.counter(0), st));
-        return e;
+    if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_a = p.in(a, 32, sb), d_R = p.in(R_uv, 64), d_nonce = p.in(nonce, 32), d_cipher = p.in(cipher, 96),
+               d_C = p.in(commitment_uv, 64);
+    const auto d_value = p.out(value, 8);
+    const auto d_blinder = p.out(blinder, 32);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_rows = p.arena(64);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_dhke(d_a(d), sb, d_R(d), false, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_decrypt(limbs(&tag_e), d_cipher(d), cnt, 2, d_shared(d), d_nonce(d), d_rows(d), d_ok(d),
+                                    nullptr, st));
+        return launched(ctx, p252::launch_note_open_value(d_rows(d), d_valid(d), d_C(d), cnt, table, table_p,
+                                                          d_value(d), d_blinder(d), d_ok(d), counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // ---- multi-key wallet scans: owner, nullifier, checked opening and per-key totals of every note -----------------------
@@ -1608,62 +1615,67 @@ int p252_wallet_scan_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jsca
     if (n == 0) return P252_OK;
     const void *table = nullptr, *table_p = nullptr;
     if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 a, 1 b, 2 R, 3 note_pk, 4 pos, 5 nonce, 6 cipher, 7 C, 8 owner, 9 nullifier, 10 value, 11 blinder, 12 opened; in
-    // the arena only: 13 the keys' Niels rows, 14 their validity, 15 the owned count; per pair 16 shared points, 17
-    // validity, 18 h, 19 matched; the dense rows of owned notes 20 meta, 21 S, 22 h, 23 b, 24 pos, 25 nonce, 26 cipher,
-    // 27 C, 28 validity, 29 the nullifier digest rows, 30 nullifier, 31 plaintext, 32 ok, 33 value, 34 blinder
-    std::vector<Io> ios = {{a, nullptr, 32 * n_keys, true, dev}, {b, nullptr, 32 * n_keys, true, dev},
-                           {R_uv, nullptr, 64, false, dev}, {note_pk_uv, nullptr, 64, false, dev},
-                           {pos, nullptr, 8, false, dev}, {nonce, nullptr, 32, false, dev},
-                           {cipher, nullptr, 96, false, dev}, {commitment_uv, nullptr, 64, false, dev},
-                           {nullptr, owner, 4, false, dev}, {nullptr, nullifier, 32, false, dev},
-                           {nullptr, value, 8, false, dev}, {nullptr, blinder, 32, false, dev},
-                           {nullptr, opened, 1, false, dev}, {nullptr, nullptr, 96 * n_keys, true},
-                           {nullptr, nullptr, n_keys, true}, {nullptr, nullptr, 8, true},
-                           {nullptr, nullptr, 64 * n_keys}, {nullptr, nullptr, n_keys}, {nullptr, nullptr, 32 * n_keys},
-                           {nullptr, nullptr, n_keys}, {nullptr, nullptr, 8}, {nullptr, nullptr, 64}, {nullptr, nullptr, 32},
-                           {nullptr, nullptr, 32}, {nullptr, nullptr, 8}, {nullptr, nullptr, 32}, {nullptr, nullptr, 96},
-                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 96}, {nullptr, nullptr, 32},
-                           {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 8}, {nullptr, nullptr, 32}};
+    Plan p(flags);
+    const auto d_a = p.in(a, 32 * n_keys, true), d_b = p.in(b, 32 * n_keys, true), d_R = p.in(R_uv, 64),
+               d_note_pk = p.in(note_pk_uv, 64);
+    const auto d_pos = p.in(pos, 8);
+    const auto d_nonce = p.in(nonce, 32), d_cipher = p.in(cipher, 96), d_C = p.in(commitment_uv, 64);
+    const auto d_owner = p.out(owner, 4);
+    const auto d_nullifier = p.out(nullifier, 32);
+    const auto d_value = p.out(value, 8);
+    const auto d_blinder = p.out(blinder, 32);
+    const auto d_opened = p.out(opened, 1);
+    const auto d_nb = p.arena(96 * n_keys, true);
+    const auto d_kvalid = p.arena<uint8_t>(n_keys, true);
+    const auto d_n_own = p.arena<unsigned long long>(8, true);
+    const auto d_shared = p.arena(64 * n_keys);
+    const auto d_pvalid = p.arena<uint8_t>(n_keys);
+    const auto d_h = p.arena(32 * n_keys);
+    const auto d_matched = p.arena<uint8_t>(n_keys);
+    // dn_: the dense rows of owned notes
+    const auto dn_meta = p.arena(8), dn_S = p.arena(64), dn_h = p.arena(32), dn_b = p.arena(32);
+    const auto dn_pos = p.arena<uint64_t>(8);
+    const auto dn_nonce = p.arena(32), dn_cipher = p.arena(96), dn_C = p.arena(64);
+    const auto dn_valid = p.arena<uint8_t>(1);
+    const auto dn_rows = p.arena(96), dn_nullifier = p.arena(32), dn_plain = p.arena(64);
+    const auto dn_ok = p.arena<uint8_t>(1);
+    const auto dn_value = p.arena<uint64_t>(8);
+    const auto dn_blinder = p.arena(32);
     auto scan = [&](unsigned long long* tot) -> int {
         const size_t tot_bytes = 4 * sizeof(uint64_t) * n_keys;
         CU(cudaMemsetAsync(tot, 0, tot_bytes, ctx->stream));
         bool first = true;
-        int r = run_host_pipeline2(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
-            auto u8 = [&](int x) { return static_cast<uint8_t*>(d[x]); };
-            auto* n_own_d = static_cast<unsigned long long*>(d[15]);
+        int r = run_host_pipeline2(ctx, p.ios, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
             const size_t np = cnt * k;
-            int e = launched(ctx, p252::launch_wallet_keys(d[0], d[1], k, table, d[13], u8(14), n_own_d,
-                                                           first ? counts.counter(1) : nullptr, st));
+            LAUNCH(p252::launch_wallet_keys(d_a(d), d_b(d), k, table, d_nb(d), d_kvalid(d), d_n_own(d),
+                                            first ? counts.counter(1) : nullptr, st));
             first = false;
-            if (e == P252_OK) e = launched(ctx, p252::launch_wallet_dhke(d[0], u8(14), k, d[2], np, d[16], u8(17), st));
-            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[16], np, 2, d[18], 1, true, ctx->coop_max, st));
-            if (e == P252_OK) e = launched(ctx, p252::launch_wallet_match(d[18], np, k, table, d[13], d[3], u8(17), u8(19), st));
-            const p252::WalletRows dense{d[20], d[21], d[22], d[23], static_cast<uint64_t*>(d[24]), d[25], d[26], d[27], u8(28)};
-            if (e == P252_OK)
-                e = launched(ctx, p252::launch_wallet_select(k, u8(19), d[16], d[18], d[1], d[2], d[3],
-                                                             static_cast<const uint64_t*>(d[4]), d[5], d[6], d[7], cnt,
-                                                             static_cast<int32_t*>(d[8]), d[9], static_cast<uint64_t*>(d[10]),
-                                                             d[11], u8(12), dense, n_own_d, counts.counter(0), st));
-            return e;
+            LAUNCH(p252::launch_wallet_dhke(d_a(d), d_kvalid(d), k, d_R(d), np, d_shared(d), d_pvalid(d), st));
+            LAUNCH(p252::launch_digest(limbs(&tag_h), d_shared(d), np, 2, d_h(d), 1, true, ctx->coop_max, st));
+            LAUNCH(p252::launch_wallet_match(d_h(d), np, k, table, d_nb(d), d_note_pk(d), d_pvalid(d), d_matched(d),
+                                             st));
+            const p252::WalletRows dense{dn_meta(d),  dn_S(d),      dn_h(d), dn_b(d),    dn_pos(d),
+                                         dn_nonce(d), dn_cipher(d), dn_C(d), dn_valid(d)};
+            return launched(ctx, p252::launch_wallet_select(k, d_matched(d), d_shared(d), d_h(d), d_b(d), d_R(d),
+                                                            d_note_pk(d), d_pos(d), d_nonce(d), d_cipher(d), d_C(d),
+                                                            cnt, d_owner(d), d_nullifier(d), d_value(d), d_blinder(d),
+                                                            d_opened(d), dense, d_n_own(d), counts.counter(0), st));
         }, [&](void** d, size_t, cudaStream_t st) -> int {
-            auto u8 = [&](int x) { return static_cast<uint8_t*>(d[x]); };
             unsigned long long n_own = 0;
-            CU(cudaMemcpyAsync(&n_own, d[15], sizeof n_own, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(&n_own, d_n_own(d), sizeof n_own, cudaMemcpyDeviceToHost, st));
             CU(cudaStreamSynchronize(st));
             if (n_own == 0) return P252_OK;
-            int e = launched(ctx, p252::launch_nullifier_key(d[22], d[23], false, static_cast<const uint64_t*>(d[24]), n_own, table_p,
-                                                         d[29], u8(28), st));
-            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_n), d[29], n_own, 3, d[30], 1, false, ctx->coop_max, st));
-            if (e == P252_OK)
-                e = launched(ctx, p252::launch_decrypt(limbs(&tag_e), d[26], n_own, 2, d[21], d[25], d[31], u8(32), nullptr, st));
-            if (e == P252_OK)
-                e = launched(ctx, p252::launch_note_open_value(d[31], u8(28), d[27], n_own, table, table_p,
-                                                               static_cast<uint64_t*>(d[33]), d[34], u8(32), nullptr, st));
-            if (e == P252_OK)
-                e = launched(ctx, p252::launch_wallet_scatter(d[20], d[30], static_cast<const uint64_t*>(d[33]), d[34], u8(32),
-                                                              n_own, d[9], static_cast<uint64_t*>(d[10]), d[11], u8(12), tot, st));
-            return e;
+            LAUNCH(p252::launch_nullifier_key(dn_h(d), dn_b(d), false, dn_pos(d), n_own, table_p, dn_rows(d),
+                                              dn_valid(d), st));
+            LAUNCH(p252::launch_digest(limbs(&tag_n), dn_rows(d), n_own, 3, dn_nullifier(d), 1, false, ctx->coop_max,
+                                       st));
+            LAUNCH(p252::launch_decrypt(limbs(&tag_e), dn_cipher(d), n_own, 2, dn_S(d), dn_nonce(d), dn_plain(d),
+                                        dn_ok(d), nullptr, st));
+            LAUNCH(p252::launch_note_open_value(dn_plain(d), dn_valid(d), dn_C(d), n_own, table, table_p, dn_value(d),
+                                                dn_blinder(d), dn_ok(d), nullptr, st));
+            return launched(ctx, p252::launch_wallet_scatter(dn_meta(d), dn_nullifier(d), dn_value(d), dn_blinder(d),
+                                                             dn_ok(d), n_own, d_nullifier(d), d_value(d), d_blinder(d),
+                                                             d_opened(d), tot, st));
         }, /*wipe=*/true);
         if (!dev) {
             if (r == P252_OK) {
@@ -1704,19 +1716,19 @@ int p252_elgamal_encrypt_batch(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_pub
     if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 PK, 1 M, 2 r, 3 c1, 4 c2, 5 ok
-    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {msg_uv, nullptr, 64, false, dev}, {r, nullptr, 32, false, dev},
-                           {nullptr, c1_uv, 64, false, dev}, {nullptr, c2_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_elgamal_encrypt(d[0], pb, d[1], false, d[2], cnt, table, d[3], d[4],
-                                                          static_cast<uint8_t*>(d[5]), counts.counter(0), st));
+    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_pk = p.in(pk_uv, 64, pb), d_M = p.in(msg_uv, 64), d_r = p.in(r, 32), d_c1 = p.out(c1_uv, 64),
+               d_c2 = p.out(c2_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_elgamal_encrypt(d_pk(d), pb, d_M(d), false, d_r(d), cnt, table, d_c1(d),
+                                                          d_c2(d), d_ok(d), counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 int p252_elgamal_decrypt_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_secret, const p252_fr* c1_uv,
@@ -1725,19 +1737,16 @@ int p252_elgamal_decrypt_batch(p252_ctx* ctx, const p252_jscalar* sk, size_t n_s
         return P252_ERR_INVALID_ARGUMENT;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
-    int rc = counts.begin();
-    if (rc != P252_OK) return rc;
-    // 0 sk, 1 c1, 2 c2, 3 M, 4 ok
-    std::vector<Io> ios = {{sk, nullptr, 32, sb, dev}, {c1_uv, nullptr, 64, false, dev}, {c2_uv, nullptr, 64, false, dev},
-                           {nullptr, msg_uv, 64, false, dev}, {nullptr, ok, 1, false, dev}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_elgamal_decrypt(d[0], sb, d[1], d[2], cnt, d[3], static_cast<uint8_t*>(d[4]),
+    Plan p(flags);
+    const auto d_sk = p.in(sk, 32, sb), d_c1 = p.in(c1_uv, 64), d_c2 = p.in(c2_uv, 64), d_M = p.out(msg_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_elgamal_decrypt(d_sk(d), sb, d_c1(d), d_c2(d), cnt, d_M(d), d_ok(d),
                                                           counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 int p252_note_sender_encrypt_batch(p252_ctx* ctx, const p252_fr* note_pk_uv, const p252_fr* sender_A_uv,
@@ -1750,20 +1759,19 @@ int p252_note_sender_encrypt_batch(p252_ctx* ctx, const p252_fr* note_pk_uv, con
     if (rc != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_sender == 1;
+    const bool sb = n_sender == 1;
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 note_pk, 1 A, 2 B, 3 blinders, 4 sender_enc, 5 ok
-    std::vector<Io> ios = {{note_pk_uv, nullptr, 64, false, dev}, {sender_A_uv, nullptr, 64, sb, dev},
-                           {sender_B_uv, nullptr, 64, sb, dev}, {blinder, nullptr, 64, false, dev},
-                           {nullptr, sender_enc, 256, false, dev}, {nullptr, ok, 1, false, dev}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_note_sender_encrypt(d[0], d[1], d[2], sb, d[3], cnt, table, d[4],
-                                                              static_cast<uint8_t*>(d[5]), counts.counter(0), st));
+    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_note_pk = p.in(note_pk_uv, 64), d_A = p.in(sender_A_uv, 64, sb), d_B = p.in(sender_B_uv, 64, sb),
+               d_blinder = p.in(blinder, 64), d_enc = p.out(sender_enc, 256);
+    const auto d_ok = p.out(ok, 1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_note_sender_encrypt(d_note_pk(d), d_A(d), d_B(d), sb, d_blinder(d), cnt,
+                                                              table, d_enc(d), d_ok(d), counts.counter(0), st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 int p252_note_sender_decrypt_batch(p252_ctx* ctx, const p252_jscalar* a, const p252_jscalar* b, size_t n_secret,
@@ -1778,26 +1786,25 @@ int p252_note_sender_decrypt_batch(p252_ctx* ctx, const p252_jscalar* a, const p
     if (rc != P252_OK || (rc = stealth_tag(&tag_h)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, sb = n_secret == 1;
+    const bool sb = n_secret == 1;
     const Counts counts(ctx, flags, n_failed, ok, n);
     if (n == 0) return P252_OK;
     const void* table = nullptr;
-    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK || (rc = counts.begin()) != P252_OK) return rc;
-    // 0 a, 1 b, 2 R, 3 note_pk, 4 sender_enc, 5 A, 6 B, 7 ok; 8 shared points, 9 validity and 10 h live in the arena only
-    std::vector<Io> ios = {{a, nullptr, 32, sb, dev}, {b, nullptr, 32, sb, dev}, {R_uv, nullptr, 64, false, dev},
-                           {note_pk_uv, nullptr, 64, false, dev}, {sender_enc, nullptr, 256, false, dev},
-                           {nullptr, sender_A_uv, 64, false, dev}, {nullptr, sender_B_uv, 64, false, dev},
-                           {nullptr, ok, 1, false, dev}, {nullptr, nullptr, 64}, {nullptr, nullptr, 1}, {nullptr, nullptr, 32}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* valid = static_cast<uint8_t*>(d[9]);
-        int e = launched(ctx, p252::launch_dhke(d[0], sb, d[2], false, cnt, d[8], valid, nullptr, st));
-        if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag_h), d[8], cnt, 2, d[10], 1, true, ctx->coop_max, st));
-        if (e == P252_OK)
-            e = launched(ctx, p252::launch_note_sender_decrypt(d[10], d[1], sb, valid, d[3], d[4], cnt, table, d[5], d[6],
-                                                               static_cast<uint8_t*>(d[7]), counts.counter(0), st));
-        return e;
+    if ((rc = base_table(ctx, ctx->bt2[0], G_uv, &table)) != P252_OK) return rc;
+    Plan p(flags);
+    const auto d_a = p.in(a, 32, sb), d_b = p.in(b, 32, sb), d_R = p.in(R_uv, 64), d_note_pk = p.in(note_pk_uv, 64),
+               d_enc = p.in(sender_enc, 256), d_A = p.out(sender_A_uv, 64), d_B = p.out(sender_B_uv, 64);
+    const auto d_ok = p.out(ok, 1);
+    const auto d_shared = p.arena(64);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_h = p.arena(32);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+        LAUNCH(p252::launch_dhke(d_a(d), sb, d_R(d), false, cnt, d_shared(d), d_valid(d), nullptr, st));
+        LAUNCH(p252::launch_digest(limbs(&tag_h), d_shared(d), cnt, 2, d_h(d), 1, true, ctx->coop_max, st));
+        return launched(ctx, p252::launch_note_sender_decrypt(d_h(d), d_b(d), sb, d_valid(d), d_note_pk(d), d_enc(d),
+                                                              cnt, table, d_A(d), d_B(d), d_ok(d), counts.counter(0),
+                                                              st));
     }, /*wipe=*/true);
-    return counts.end(rc);
 }
 
 // ---- JubJub point compression: JubJubAffine::from_bytes / to_bytes -----------------------------------------------------
@@ -1807,22 +1814,18 @@ int p252_note_sender_decrypt_batch(p252_ctx* ctx, const p252_jscalar* a, const p
 static int points_impl(p252_ctx* ctx, bool from_bytes, const void* in, size_t n, void* out, uint8_t* ok, size_t* n_invalid,
                        int flags) {
     if (!ctx || !args_ok(n, flags, {in, out}, {ok})) return P252_ERR_INVALID_ARGUMENT;
-    const bool dev = (flags & P252_MEM_DEVICE) != 0;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const Counts counts(ctx, flags, n_invalid, ok, n);
     if (n == 0) return P252_OK;
-    int rc = counts.begin();
-    if (rc != P252_OK) return rc;
-    const size_t in_bytes = from_bytes ? 32 : 64, out_bytes = from_bytes ? 64 : 32;
-    // 0 input, 1 output, 2 ok
-    std::vector<Io> ios = {{in, nullptr, in_bytes, false, dev}, {nullptr, out, out_bytes, false, dev}, {nullptr, ok, 1, false, dev}};
-    rc = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        uint8_t* okc = static_cast<uint8_t*>(d[2]);
-        return launched(ctx, from_bytes ? p252::launch_points_from_bytes(d[0], cnt, d[1], okc, counts.counter(0), st)
-                                        : p252::launch_points_to_bytes(d[0], cnt, d[1], okc, counts.counter(0), st));
+    Plan p(flags);
+    const auto d_in = p.in(in, from_bytes ? 32 : 64), d_out = p.out(out, from_bytes ? 64 : 32);
+    const auto d_ok = p.out(ok, 1);
+    return staged_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        unsigned long long* counter = counts.counter(0);
+        return launched(ctx, from_bytes ? p252::launch_points_from_bytes(d_in(d), cnt, d_out(d), d_ok(d), counter, st)
+                                        : p252::launch_points_to_bytes(d_in(d), cnt, d_out(d), d_ok(d), counter, st));
     });
-    return counts.end(rc);
 }
 
 int p252_points_from_bytes(p252_ctx* ctx, const uint8_t* bytes, size_t n, p252_fr* out_uv, uint8_t* ok, size_t* n_invalid,
@@ -1893,21 +1896,19 @@ int msm_chunk(p252_ctx* ctx, const void* sc, const void* pt, size_t m, int c, vo
     const uint32_t W = (uint32_t)p252::msm_windows(c), nb = W << (c - 1), N = (uint32_t)(m * W);
     int end_bit = 0;
     while ((1u << end_bit) <= nb) ++end_bit;         // keys <= nb (the sentinel)
-    int rc = launched(ctx, p252::launch_msm_prep(sc, pt, (uint32_t)m, c, s.niels, s.ka, s.va, n_invalid, st));
-    if (rc != P252_OK) return rc;
+    LAUNCH(p252::launch_msm_prep(sc, pt, (uint32_t)m, c, s.niels, s.ka, s.va, n_invalid, st));
     CU(cub::DeviceRadixSort::SortPairs(s.temp, s.temp_bytes, s.ka, s.kb, s.va, s.vb, (int)N, 0, end_bit, st));
-    if ((rc = launched(ctx, p252::launch_msm_fill(s.buckets, nb, st))) != P252_OK) return rc;
+    LAUNCH(p252::launch_msm_fill(s.buckets, nb, st));
     size_t pieces = ceil_div(N, p252::kMsmPiece);
-    rc = launched(ctx, p252::launch_msm_bucket(true, s.kb, s.vb, s.niels, N, nb, s.buckets, pieces > 1 ? s.ck[0] : nullptr,
-                                               s.cp[0], st));
-    for (int src = 0; rc == P252_OK && pieces > 1; src ^= 1) {
+    LAUNCH(p252::launch_msm_bucket(true, s.kb, s.vb, s.niels, N, nb, s.buckets, pieces > 1 ? s.ck[0] : nullptr, s.cp[0],
+                                   st));
+    for (int src = 0; pieces > 1; src ^= 1) {
         const uint32_t len = (uint32_t)(2 * pieces);
         pieces = ceil_div(len, p252::kMsmPiece);
-        rc = launched(ctx, p252::launch_msm_bucket(false, s.ck[src], nullptr, s.cp[src], len, nb, s.buckets,
-                                                   pieces > 1 ? s.ck[src ^ 1] : nullptr, s.cp[src ^ 1], st));
+        LAUNCH(p252::launch_msm_bucket(false, s.ck[src], nullptr, s.cp[src], len, nb, s.buckets,
+                                       pieces > 1 ? s.ck[src ^ 1] : nullptr, s.cp[src ^ 1], st));
     }
-    if (rc == P252_OK) rc = launched(ctx, p252::launch_msm_window(s.buckets, c, wsum, st));
-    return rc;
+    return launched(ctx, p252::launch_msm_window(s.buckets, c, wsum, st));
 }
 
 }  // namespace
@@ -1919,12 +1920,13 @@ int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* p
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
     const Counts counts = Counts::device(ctx, flags, n_invalid);
-    // 0 scalars, 1 points; 2 the chunk's MSM temporaries (one region per slot arena)
-    std::vector<Io> ios = {{scalars, nullptr, 32, false, dev}, {points_uv, nullptr, 64, false, dev}, {nullptr, nullptr, 0, true}};
-    const size_t chunk = n ? pipeline_chunk(ios, n) : 0;
+    Plan p(flags);
+    // d_scratch: the chunk's MSM temporaries (one region per slot arena), sized below
+    const auto d_sc = p.in(scalars, 32), d_pt = p.in(points_uv, 64), d_scratch = p.arena(0, true);
+    const size_t chunk = n ? pipeline_chunk(p.ios, n) : 0;
     const int c = p252::msm_bits(std::max<size_t>(chunk, 1));
     const size_t W = (size_t)p252::msm_windows(c), max_chunks = n ? ceil_div(n, chunk) + 3 : 0;
-    ios[2].item_bytes = msm_scratch_bytes(chunk, c);
+    p[d_scratch].item_bytes = msm_scratch_bytes(chunk, c);
     int rc = counts.begin();
     if (rc != P252_OK) return rc;
     uint4* wsum = nullptr;
@@ -1934,14 +1936,13 @@ int p252_jubjub_msm(p252_ctx* ctx, const p252_jscalar* scalars, const p252_fr* p
         dout = cv.take<uint8_t>(64);
     }, [&]() -> int {
         uint32_t k = 0;
-        int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-            return msm_chunk(ctx, d[0], d[1], cnt, c, d[2], chunk, wsum + (size_t)(k++) * W * 8, counts.counter(0), st);
+        const int r = run_host_pipeline(ctx, p.ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
+            return msm_chunk(ctx, d_sc(d), d_pt(d), cnt, c, d_scratch(d), chunk, wsum + (size_t)(k++) * W * 8,
+                             counts.counter(0), st);
         });
         if (r != P252_OK) return r;
         void* out = dev ? static_cast<void*>(out_uv) : dout;
-        if ((r = launched(ctx, p252::launch_msm_final(wsum, k, c, out, nullptr, 0, nullptr, nullptr, nullptr, nullptr,
-                                                      ctx->stream))) != P252_OK)
-            return r;
+        LAUNCH(p252::launch_msm_final(wsum, k, c, out, nullptr, 0, nullptr, nullptr, nullptr, nullptr, ctx->stream));
         if (!dev) CU(cudaMemcpyAsync(out_uv, dout, 64, cudaMemcpyDeviceToHost, ctx->stream));
         return P252_OK;
     });
@@ -1962,7 +1963,7 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
     if (rc != P252_OK || (rc = schnorr_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts = Counts::device(ctx, flags, n_invalid, nullptr, all_verified);
     if (n == 0) {
         *all_verified = 1;
@@ -1971,17 +1972,16 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
     const void* table = nullptr;
     if ((rc = base_table(ctx, ctx->bt, base_uv, &table)) != P252_OK) return rc;
     const size_t per = pb ? 1 : 2;   // MSM rows per item
-    // 0 PK, 1 u, 2 R, 3 msg, 4 weight; 5 the digest rows, 6 validity, 7 c, 8 row scalars, 9 row points and 10 the chunk's
-    // MSM temporaries live in the arena only
-    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev}, {R_uv, nullptr, 64, false, dev},
-                           {msg, nullptr, 32, false, dev}, {weight, nullptr, 32, false, dev}, {nullptr, nullptr, 96},
-                           {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 32 * per},
-                           {nullptr, nullptr, 64 * per}, {nullptr, nullptr, 0, true}};
-    const size_t chunk = pipeline_chunk(ios, n), M = chunk * per;
+    Plan p(flags);
+    const auto d_pk = p.in(pk_uv, 64, pb), d_u = p.in(u, 32), d_R = p.in(R_uv, 64), d_msg = p.in(msg, 32),
+               d_weight = p.in(weight, 32), d_rows = p.arena(96);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_c = p.arena(32), d_sc = p.arena(32 * per), d_pt = p.arena(64 * per), d_scratch = p.arena(0, true);
+    const size_t chunk = pipeline_chunk(p.ios, n), M = chunk * per;
     const int c = p252::msm_bits(M);
     const size_t W = (size_t)p252::msm_windows(c), max_chunks = ceil_div(n, chunk) + 3;
     const size_t nsum = ceil_div(n, p252::kMsmItemsPerSum);
-    ios[10].item_bytes = msm_scratch_bytes(M, c);
+    p[d_scratch].item_bytes = msm_scratch_bytes(M, c);   // the chunk's MSM temporaries (one region per slot arena)
     if ((rc = counts.begin()) != P252_OK) return rc;
     uint4* wsum = nullptr;
     uint8_t *zsum = nullptr, *pkc = nullptr;
@@ -1996,17 +1996,15 @@ int p252_schnorr_verify_all(p252_ctx* ctx, const p252_fr* pk_uv, size_t n_public
         if (pb) CU(cudaMemcpyAsync(pkc, pk_uv, 64, cudaMemcpyDefault, ctx->stream));
         uint32_t k = 0;
         size_t off = 0;
-        int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-            uint8_t* valid = static_cast<uint8_t*>(d[6]);
+        const int r = run_host_pipeline(ctx, p.ios, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
             const uint32_t sum0 = (uint32_t)(off / p252::kMsmItemsPerSum);
             off += cnt;
-            int e = launched(ctx, p252::launch_schnorr_pack(d[2], d[3], cnt, d[5], valid, false, st));
-            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[5], cnt, 3, d[7], 1, true, ctx->coop_max, st));
-            if (e == P252_OK)
-                e = launched(ctx, p252::launch_msmv_prep(d[0], pb, d[1], d[2], d[7], d[4], valid, (uint32_t)cnt, d[8], d[9], zsum,
-                                                         sum0, bad, counts.counter(0), st));
-            if (e == P252_OK) e = msm_chunk(ctx, d[8], d[9], cnt * per, c, d[10], M, wsum + (size_t)(k++) * W * 8, nullptr, st);
-            return e;
+            LAUNCH(p252::launch_schnorr_pack(d_R(d), d_msg(d), cnt, d_rows(d), d_valid(d), false, st));
+            LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 3, d_c(d), 1, true, ctx->coop_max, st));
+            LAUNCH(p252::launch_msmv_prep(d_pk(d), pb, d_u(d), d_R(d), d_c(d), d_weight(d), d_valid(d), (uint32_t)cnt,
+                                          d_sc(d), d_pt(d), zsum, sum0, bad, counts.counter(0), st));
+            return msm_chunk(ctx, d_sc(d), d_pt(d), cnt * per, c, d_scratch(d), M, wsum + (size_t)(k++) * W * 8, nullptr,
+                             st);
         });
         if (r != P252_OK) return r;
         return launched(ctx, p252::launch_msm_final(wsum, k, c, nullptr, zsum, (uint32_t)nsum, table, pb ? pkc : nullptr, bad,
@@ -2034,7 +2032,7 @@ int p252_schnorr_verify_double_all(p252_ctx* ctx, const p252_fr* pk_uv, const p2
     if ((rc = schnorr_double_tag(&tag)) != P252_OK) return rc;
     P252_LOCK(ctx);
     DeviceGuard g(ctx->device);
-    const bool dev = (flags & P252_MEM_DEVICE) != 0, pb = n_public == 1;
+    const bool pb = n_public == 1;
     const Counts counts = Counts::device(ctx, flags, n_invalid, nullptr, all_verified);
     if (n == 0) {
         *all_verified = 1;
@@ -2043,18 +2041,17 @@ int p252_schnorr_verify_double_all(p252_ctx* ctx, const p252_fr* pk_uv, const p2
     const void *table = nullptr, *table_p = nullptr;
     if ((rc = double_tables(ctx, G_uv, Gp_uv, &table, &table_p)) != P252_OK) return rc;
     const size_t per = pb ? 2 : 4;   // MSM rows per item
-    // 0 PK, 1 PK', 2 u, 3 R, 4 R', 5 msg, 6 weight, 7 weight_p; 8 the digest rows, 9 validity, 10 c, 11 row scalars,
-    // 12 row points and 13 the chunk's MSM temporaries live in the arena only
-    std::vector<Io> ios = {{pk_uv, nullptr, 64, pb, dev}, {pkp_uv, nullptr, 64, pb, dev}, {u, nullptr, 32, false, dev},
-                           {R_uv, nullptr, 64, false, dev}, {Rp_uv, nullptr, 64, false, dev}, {msg, nullptr, 32, false, dev},
-                           {weight, nullptr, 32, false, dev}, {weight_p, nullptr, 32, false, dev}, {nullptr, nullptr, 160},
-                           {nullptr, nullptr, 1}, {nullptr, nullptr, 32}, {nullptr, nullptr, 32 * per},
-                           {nullptr, nullptr, 64 * per}, {nullptr, nullptr, 0, true}};
-    const size_t chunk = pipeline_chunk(ios, n), M = chunk * per;
+    Plan p(flags);
+    const auto d_pk = p.in(pk_uv, 64, pb), d_pkp = p.in(pkp_uv, 64, pb), d_u = p.in(u, 32), d_R = p.in(R_uv, 64),
+               d_Rp = p.in(Rp_uv, 64), d_msg = p.in(msg, 32), d_weight = p.in(weight, 32),
+               d_weight_p = p.in(weight_p, 32), d_rows = p.arena(160);
+    const auto d_valid = p.arena<uint8_t>(1);
+    const auto d_c = p.arena(32), d_sc = p.arena(32 * per), d_pt = p.arena(64 * per), d_scratch = p.arena(0, true);
+    const size_t chunk = pipeline_chunk(p.ios, n), M = chunk * per;
     const int c = p252::msm_bits(M);
     const size_t W = (size_t)p252::msm_windows(c), max_chunks = ceil_div(n, chunk) + 3;
     const size_t nsum = ceil_div(n, p252::kMsmItemsPerSum);
-    ios[13].item_bytes = msm_scratch_bytes(M, c);
+    p[d_scratch].item_bytes = msm_scratch_bytes(M, c);   // the chunk's MSM temporaries (one region per slot arena)
     if ((rc = counts.begin()) != P252_OK) return rc;
     uint4* wsum = nullptr;
     uint8_t *zsum = nullptr, *pkc = nullptr;
@@ -2072,19 +2069,16 @@ int p252_schnorr_verify_double_all(p252_ctx* ctx, const p252_fr* pk_uv, const p2
         }
         uint32_t k = 0;
         size_t off = 0;
-        int r = run_host_pipeline(ctx, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-            uint8_t* valid = static_cast<uint8_t*>(d[9]);
+        const int r = run_host_pipeline(ctx, p.ios, n, [&](void** d, size_t cnt, cudaStream_t st) -> int {
             const uint32_t sum0 = (uint32_t)(off / p252::kMsmItemsPerSum);
             off += cnt;
-            int e = launched(ctx, p252::launch_schnorr_pack_double(d[3], d[4], d[5], cnt, d[8], valid, false, st));
-            if (e == P252_OK) e = launched(ctx, p252::launch_digest(limbs(&tag), d[8], cnt, 5, d[10], 1, true, ctx->coop_max, st));
-            if (e == P252_OK)
-                e = launched(ctx, p252::launch_msmv_prep_double(d[0], d[1], pb, d[2], d[3], d[4], d[10], d[6], d[7], valid,
-                                                                (uint32_t)cnt, d[11], d[12], zsum, sum0, bad,
-                                                                counts.counter(0), st));
-            if (e == P252_OK)
-                e = msm_chunk(ctx, d[11], d[12], cnt * per, c, d[13], M, wsum + (size_t)(k++) * W * 8, nullptr, st);
-            return e;
+            LAUNCH(p252::launch_schnorr_pack_double(d_R(d), d_Rp(d), d_msg(d), cnt, d_rows(d), d_valid(d), false, st));
+            LAUNCH(p252::launch_digest(limbs(&tag), d_rows(d), cnt, 5, d_c(d), 1, true, ctx->coop_max, st));
+            LAUNCH(p252::launch_msmv_prep_double(d_pk(d), d_pkp(d), pb, d_u(d), d_R(d), d_Rp(d), d_c(d), d_weight(d),
+                                                 d_weight_p(d), d_valid(d), (uint32_t)cnt, d_sc(d), d_pt(d), zsum, sum0,
+                                                 bad, counts.counter(0), st));
+            return msm_chunk(ctx, d_sc(d), d_pt(d), cnt * per, c, d_scratch(d), M, wsum + (size_t)(k++) * W * 8, nullptr,
+                             st);
         });
         if (r != P252_OK) return r;
         return launched(ctx, p252::launch_msmv_final_double(wsum, k, c, zsum, (uint32_t)nsum, table, table_p,
@@ -2159,13 +2153,13 @@ int p252_merkle_build(p252_ctx* ctx, int arity, const p252_fr* leaves, size_t n_
     p252_fr tag;
     p252_hash_tag(merkle_domain(arity), (size_t)arity, 1, &tag);
     {
-        std::vector<Io> ios = {{leaves, nullptr, (size_t)arity * 32}, {nullptr, nodes_out, 32}};
+        Plan p(flags);
+        const auto d_leaves = p.in(leaves, (size_t)arity * 32), d_parents = p.out(nodes_out, 32);
         size_t done = 0;   // the pipeline hands chunks in order; mirror each chunk into d_nodes as well
-        rc = run_host_pipeline(ctx, ios, first, [&](void** d, size_t cnt, cudaStream_t st) -> int {
-            const int e = launched(ctx, p252::launch_digest(limbs(&tag), d[0], cnt, (uint32_t)arity, d[1], 1, false,
-                                                            ctx->coop_max, st));
-            if (e != P252_OK) return e;
-            CU(cudaMemcpyAsync(d_nodes + done, d[1], cnt * sizeof(p252_fr), cudaMemcpyDeviceToDevice, st));
+        rc = run_host_pipeline(ctx, p.ios, first, [&](void** d, size_t cnt, cudaStream_t st) -> int {
+            LAUNCH(p252::launch_digest(limbs(&tag), d_leaves(d), cnt, (uint32_t)arity, d_parents(d), 1, false,
+                                       ctx->coop_max, st));
+            CU(cudaMemcpyAsync(d_nodes + done, d_parents(d), cnt * sizeof(p252_fr), cudaMemcpyDeviceToDevice, st));
             done += cnt;
             return P252_OK;
         });
@@ -2237,11 +2231,14 @@ int p252_merkle_verify_batch(p252_ctx* ctx, int arity, int depth, const p252_fr*
     DeviceGuard g(ctx->device);
     const Counts counts(ctx, flags, n_failed, ok, n);
     const size_t path_bytes = (size_t)depth * (size_t)arity * 32;
-    std::vector<Io> ios = {{leaf_items, nullptr, 32}, {leaf_idx, nullptr, 8}, {paths, nullptr, path_bytes}, {nullptr, ok, 1}};
-    return launch_batch(counts, ios, n, [&](void** d, size_t cnt, cudaStream_t st) {
-        return launched(ctx, p252::launch_merkle_verify(limbs(&tag), limbs(root), d[0], static_cast<const uint64_t*>(d[1]), d[2],
-                                                        cnt, arity, (uint32_t)depth, static_cast<uint8_t*>(d[3]),
-                                                        counts.counter(0), st));
+    Plan p(flags);
+    const auto d_leaf = p.in(leaf_items, 32);
+    const auto d_idx = p.in(leaf_idx, 8);
+    const auto d_paths = p.in(paths, path_bytes);
+    const auto d_ok = p.out(ok, 1);
+    return launch_batch(counts, p, n, [&](void** d, size_t cnt, cudaStream_t st) {
+        return launched(ctx, p252::launch_merkle_verify(limbs(&tag), limbs(root), d_leaf(d), d_idx(d), d_paths(d), cnt,
+                                                        arity, (uint32_t)depth, d_ok(d), counts.counter(0), st));
     });
 }
 
@@ -3389,7 +3386,8 @@ namespace {
 int hash_to_scalar_run(p252_ctx* ctx, const uint8_t* bytes, uint64_t base, uint64_t n_bytes, const uint64_t* offsets, uint32_t n,
                        uint32_t max_len, p252_fr* out, unsigned long long* rejected, cudaStream_t st) {
     if (max_len <= 128)
-        return launched(ctx, p252::launch_hash_to_scalar(bytes, base, n_bytes, offsets, nullptr, n, max_len, out, rejected, st));
+        return launched(ctx, p252::launch_hash_to_scalar(bytes, base, n_bytes, offsets, nullptr, n, max_len, out,
+                                                         rejected, st));
     const uint32_t max_blocks = (max_len + 127) / 128;
     return varlen_sorted(
         ctx, n, max_blocks, st,
