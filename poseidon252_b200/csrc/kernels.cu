@@ -1346,8 +1346,30 @@ static inline FrArg to_arg(const uint64_t tag[4]) {
     return a;
 }
 
-static inline unsigned grid_for(size_t n) { return (unsigned)((n + kThreads - 1) / kThreads); }
-static inline unsigned blocks256(uint64_t n) { return (unsigned)((n + 255) / 256); }
+// A launcher's untyped buffer (void* or const void*) becomes the kernel's typed pointer parameter; every other argument
+// is passed as it is, so a const buffer still needs a visible const_cast to reach a non-const parameter.
+template <class P, class A>
+static inline P kernel_arg(A a) { return a; }
+template <class P>
+static inline P kernel_arg(void* a) { return static_cast<P>(a); }
+template <class P>
+static inline P kernel_arg(const void* a) { return static_cast<P>(a); }
+
+// Launches kernel k with `grid` blocks of `threads` threads on stream st and returns the launch's status.  An empty
+// grid (an empty batch) launches nothing and returns cudaSuccess.
+template <class... P, class... A>
+static cudaError_t launch_grid(void (*k)(P...), unsigned grid, unsigned threads, cudaStream_t st, A... a) {
+    if (grid == 0) return cudaSuccess;
+    k<<<grid, threads, 0, st>>>(kernel_arg<P>(a)...);
+    return cudaGetLastError();
+}
+
+// The same for n items, one per thread: ceil(n / threads) blocks
+template <class... P, class... A>
+static cudaError_t launch(void (*k)(P...), size_t n, unsigned threads, cudaStream_t st, A... a) {
+    return launch_grid(k, (unsigned)((n + threads - 1) / threads), threads, st, a...);
+}
+
 // lane-split kernels: kCoopItemsPerWarp items per warp
 static inline unsigned coop_grid(size_t n) {
     return (unsigned)(((n + kCoopItemsPerWarp - 1) / kCoopItemsPerWarp + kWarps - 1) / kWarps);
@@ -1368,38 +1390,20 @@ size_t coop_max_items(int sm_count) {
 }
 
 cudaError_t launch_permute(void* states, size_t n, bool dense, size_t coop_max, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    if (!dense && n <= coop_max) {
-        k_permute_coop<<<coop_grid(n), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
-        return cudaGetLastError();
-    }
-    if (dense)
-        k_permute<true><<<grid_for(n), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
-    else if (n >= kWideShapeMinItems)
-        k_permute<false, 256, 2><<<blocks256(n), 256, 0, st>>>(static_cast<uint8_t*>(states), n);
-    else
-        k_permute<false><<<grid_for(n), kThreads, 0, st>>>(static_cast<uint8_t*>(states), n);
-    return cudaGetLastError();
+    if (!dense && n <= coop_max) return launch_grid(k_permute_coop, coop_grid(n), kThreads, st, states, n);
+    if (dense) return launch(k_permute<true>, n, kThreads, st, states, n);
+    if (n >= kWideShapeMinItems) return launch(k_permute<false, 256, 2>, n, 256, st, states, n);
+    return launch(k_permute<false>, n, kThreads, st, states, n);
 }
 
 cudaError_t launch_digest(const uint64_t tag[4], const void* in, size_t n, uint32_t in_len, void* out,
                           uint32_t out_len, bool truncate, size_t coop_max, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    if (!truncate && n <= coop_max) {
-        k_sponge_digest_coop<<<coop_grid(n), kThreads, 0, st>>>(
-            to_arg(tag), static_cast<const uint8_t*>(in), n, in_len, static_cast<uint8_t*>(out), out_len);
-        return cudaGetLastError();
-    }
-    if (truncate)
-        k_sponge_digest<true><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), static_cast<const uint8_t*>(in), n, in_len,
-                                                                static_cast<uint8_t*>(out), out_len);
-    else if (n >= kWideShapeMinItems)
-        k_sponge_digest<false, 256, 2><<<blocks256(n), 256, 0, st>>>(
-            to_arg(tag), static_cast<const uint8_t*>(in), n, in_len, static_cast<uint8_t*>(out), out_len);
-    else
-        k_sponge_digest<false><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), static_cast<const uint8_t*>(in), n, in_len,
-                                                                 static_cast<uint8_t*>(out), out_len);
-    return cudaGetLastError();
+    const FrArg t = to_arg(tag);
+    if (!truncate && n <= coop_max)
+        return launch_grid(k_sponge_digest_coop, coop_grid(n), kThreads, st, t, in, n, in_len, out, out_len);
+    if (truncate) return launch(k_sponge_digest<true>, n, kThreads, st, t, in, n, in_len, out, out_len);
+    if (n >= kWideShapeMinItems) return launch(k_sponge_digest<false, 256, 2>, n, 256, st, t, in, n, in_len, out, out_len);
+    return launch(k_sponge_digest<false>, n, kThreads, st, t, in, n, in_len, out, out_len);
 }
 
 // ---- wire format: canonical 32-byte little-endian <-> BlsScalar.0 (Montgomery limbs) ---------------------
@@ -1427,33 +1431,69 @@ __global__ void __launch_bounds__(256) k_convert(const uint8_t* __restrict__ in,
 }
 
 cudaError_t launch_convert(const void* in, size_t n, void* out, uint8_t* ok, bool from_bytes, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    const unsigned grid = blocks256(n);
-    if (from_bytes)
-        k_convert<true><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(in), n, static_cast<uint8_t*>(out), ok);
-    else
-        k_convert<false><<<grid, 256, 0, st>>>(static_cast<const uint8_t*>(in), n, static_cast<uint8_t*>(out), nullptr);
-    return cudaGetLastError();
+    if (from_bytes) return launch(k_convert<true>, n, 256, st, in, n, out, ok);
+    return launch(k_convert<false>, n, 256, st, in, n, out, nullptr);
 }
 
 cudaError_t launch_encrypt(const uint64_t tag[4], const void* msg, size_t n, uint32_t L, const void* secret_uv,
                            const void* nonce, void* cipher, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_crypt<false><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), static_cast<const uint8_t*>(msg), n, L,
-                                                     static_cast<const uint8_t*>(secret_uv),
-                                                     static_cast<const uint8_t*>(nonce),
-                                                     static_cast<uint8_t*>(cipher), nullptr, nullptr);
-    return cudaGetLastError();
+    return launch(k_crypt<false>, n, kThreads, st, to_arg(tag), msg, n, L, secret_uv, nonce, cipher, nullptr, nullptr);
 }
 
 cudaError_t launch_decrypt(const uint64_t tag[4], const void* cipher, size_t n, uint32_t L, const void* secret_uv,
                            const void* nonce, void* msg, uint8_t* ok, unsigned long long* n_failed, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_crypt<true><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), static_cast<const uint8_t*>(cipher), n, L,
-                                                    static_cast<const uint8_t*>(secret_uv),
-                                                    static_cast<const uint8_t*>(nonce), static_cast<uint8_t*>(msg),
-                                                    ok, n_failed);
-    return cudaGetLastError();
+    return launch(k_crypt<true>, n, kThreads, st, to_arg(tag), cipher, n, L, secret_uv, nonce, msg, ok, n_failed);
+}
+
+// ---- JubJub operands: point rows, masks and the projective comparison -----------------------------------------------
+// Every JubJub kernel runs the same instructions for every item (DESIGN.md §4): an invalid operand is replaced by the
+// identity or by zero, never skipped.  None of these helpers branches on or indexes by an operand's value; a mask m is
+// all ones or all zeros.
+
+// Loads the point row at p into (u, v) and returns whether it is a curve point with u, v < p.  Substitutes nothing.
+__device__ __forceinline__ bool load_curve_point(uint32_t (&u)[8], uint32_t (&v)[8], const uint8_t* p) {
+    load_fr(u, p);
+    load_fr(v, p + 32);
+    return fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
+}
+
+// Loads the point row at p into (u, v) and returns whether u, v < p (no curve check).  A pair with a coordinate >= p is
+// replaced so that it enters no product: by the identity (0, 1) if kIdentity, by (0, 0) otherwise.
+template <bool kIdentity>
+__device__ __forceinline__ bool load_canonical_point(uint32_t (&u)[8], uint32_t (&v)[8], const uint8_t* p) {
+    load_fr(u, p);
+    load_fr(v, p + 32);
+    uint32_t one[8];
+    jj::set_one(one);
+    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
+    const uint32_t mc = 0u - (uint32_t)canon;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] = (v[k] & mc) | (kIdentity ? one[k] & ~mc : 0u);
+    return canon;
+}
+
+// (u, v) = m ? (u, v) : the identity (0, 1)
+__device__ __forceinline__ void mask_point(uint32_t (&u)[8], uint32_t (&v)[8], uint32_t m) {
+    uint32_t one[8];
+    jj::set_one(one);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= m, v[k] = (v[k] & m) | (one[k] & ~m);
+}
+
+// (u, v) &= m, then stores (u, v) as the 64-byte point row at p: a zeroed row where m is zero
+__device__ __forceinline__ void store_masked_point(uint8_t* p, uint32_t (&u)[8], uint32_t (&v)[8], uint32_t m) {
+#pragma unroll
+    for (int k = 0; k < 8; ++k) u[k] &= m, v[k] &= m;
+    store_fr(p, u);
+    store_fr(p + 32, v);
+}
+
+// Whether the affine (u, v) is the point t, compared projectively (u Z == X and v Z == Y): no inversion
+__device__ __forceinline__ bool equals_affine(const uint32_t (&u)[8], const uint32_t (&v)[8], const jj::Ext& t) {
+    uint32_t x[8], y[8];
+    jj::fmul(x, u, t.Z);
+    jj::fmul(y, v, t.Z);
+    return jj::feq(x, t.X) & jj::feq(y, t.Y);
 }
 
 // ---- JubJub key exchange (dhke(secret, public) = [s] public, JubJubAffine out) -------------------------------------
@@ -1471,16 +1511,12 @@ __global__ void __launch_bounds__(kThreads, 3) k_dhke(const uint8_t* __restrict_
     load_fr(v, pub + (pb ? 0 : i) * 64 + 32);
     const bool valid = jj::below_order(s) & fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
     const uint32_t m = 0u - (uint32_t)valid;
-    uint32_t one[8];
-    jj::set_one(one);
 #pragma unroll
-    for (int k = 0; k < 8; ++k) s[k] &= m, u[k] &= m, v[k] = (v[k] & m) | (one[k] & ~m);
+    for (int k = 0; k < 8; ++k) s[k] &= m;
+    mask_point(u, v, m);
     uint32_t ou[8], ov[8];
     jj::scalar_mul(ou, ov, s, u, v);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m;
-    store_fr(out + i * 64, ou);
-    store_fr(out + i * 64 + 32, ov);
+    store_masked_point(out + i * 64, ou, ov, m);
     ok[i] = valid ? 1 : 0;
     if (n_invalid) warp_count(n_invalid, !valid);
 }
@@ -1507,17 +1543,12 @@ __global__ void __launch_bounds__(256) k_dhke_fix(bool decrypt, const uint8_t* _
 
 cudaError_t launch_dhke(const void* secret, bool secret_bcast, const void* pub, bool pub_bcast, size_t n, void* shared_uv,
                         uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_dhke<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(secret), secret_bcast, static_cast<const uint8_t*>(pub),
-                                             pub_bcast, n, static_cast<uint8_t*>(shared_uv), ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_dhke, n, kThreads, st, secret, secret_bcast, pub, pub_bcast, n, shared_uv, ok, n_invalid);
 }
 
 cudaError_t launch_dhke_fix(bool decrypt, const uint8_t* valid, size_t n, void* out, uint32_t row, uint8_t* ok,
                             unsigned long long* count, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_dhke_fix<<<blocks256(n), 256, 0, st>>>(decrypt, valid, n, static_cast<uint8_t*>(out), row, ok, count);
-    return cudaGetLastError();
+    return launch(k_dhke_fix, n, 256, st, decrypt, valid, n, out, row, ok, count);
 }
 
 // ---- fixed-base JubJub scalar multiplication (out = [s] B for one base B of the whole batch) -------------------------
@@ -1552,10 +1583,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_fixed_base(const uint8_t* __res
     for (int k = 0; k < 8; ++k) s[k] &= m;
     uint32_t ou[8], ov[8];
     jj::fixed_base_mul<true>(ou, ov, s, table);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m;
-    store_fr(out + i * 64, ou);
-    store_fr(out + i * 64 + 32, ov);
+    store_masked_point(out + i * 64, ou, ov, m);
     ok[i] = valid ? 1 : 0;
     if (n_invalid) warp_count(n_invalid, !valid);
 }
@@ -1563,16 +1591,12 @@ __global__ void __launch_bounds__(kThreads, 3) k_fixed_base(const uint8_t* __res
 cudaError_t launch_fixed_base_table(const uint64_t base_uv[8], void* table, cudaStream_t st) {
     FixedBase b;
     for (int k = 0; k < 8; ++k) b.uv[2 * k] = (uint32_t)base_uv[k], b.uv[2 * k + 1] = (uint32_t)(base_uv[k] >> 32);
-    k_fixed_base_table<<<jj::kFbWindows * jj::kFbEntries / 128, 128, 0, st>>>(b, static_cast<uint4*>(table));
-    return cudaGetLastError();
+    return launch(k_fixed_base_table, jj::kFbWindows * jj::kFbEntries, 128, st, b, table);
 }
 
 cudaError_t launch_fixed_base(const void* secret, size_t n, const void* table, void* out_uv, uint8_t* ok,
                               unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_fixed_base<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(secret), n, static_cast<const uint4*>(table),
-                                                   static_cast<uint8_t*>(out_uv), ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_fixed_base, n, kThreads, st, secret, n, table, out_uv, ok, n_invalid);
 }
 
 // ---- stealth addresses: note_pk = [h] G + B, h = hash([r] A) = hash([a] R) (jubjub_device.cuh) ------------------------
@@ -1606,20 +1630,11 @@ __global__ void __launch_bounds__(kThreads, 3) k_stealth(const uint8_t* __restri
     // The point operand is loaded twice (derive: its check runs before [h] G, its Niels form after) so that during the
     // 64 windows of [h] G nothing but the scalar and a flag is live.  Coordinates >= p enter no product: they are
     // replaced first (derive: by the identity (0, 1)).
-    uint32_t u[8], v[8], one[8];
-    jj::set_one(one);
+    uint32_t u[8], v[8];
     const uint8_t* pt = kOwns ? pk + i * 64 : B_uv + (bb ? 0 : i) * 64;
-    auto load_point = [&](bool& canon) {
-        load_fr(u, pt);
-        load_fr(v, pt + 32);
-        canon = fr_is_canonical(u) & fr_is_canonical(v);
-        const uint32_t mc = 0u - (uint32_t)canon;
-#pragma unroll
-        for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] = (v[k] & mc) | (kOwns ? 0u : one[k] & ~mc);
-    };
-    bool good = valid[i] != 0, canon;
+    bool good = valid[i] != 0;
     if (!kOwns) {
-        load_point(canon);
+        const bool canon = load_canonical_point<true>(u, v, pt);
         good &= canon & jj::on_curve(u, v);
     }
     jj::Ext t, r;
@@ -1628,24 +1643,19 @@ __global__ void __launch_bounds__(kThreads, 3) k_stealth(const uint8_t* __restri
         load_fr(s, h + i * 32);
         jj::fixed_base_ext<true, true>(t, s, table);
     }
-    load_point(canon);
+    const bool canon = load_canonical_point<!kOwns>(u, v, pt);
     jj::Niels q;
     if (kOwns) {
 #pragma unroll
         for (int k = 0; k < 8; ++k) q.ymx[k] = nb.w[k], q.ypx[k] = nb.w[8 + k], q.kt[k] = nb.w[16 + k];
         good &= canon;
     } else {
-        const uint32_t mo = 0u - (uint32_t)good;   // an item that is not valid adds the identity: B is on the curve
-#pragma unroll
-        for (int k = 0; k < 8; ++k) u[k] &= mo, v[k] = (v[k] & mo) | (one[k] & ~mo);
+        mask_point(u, v, 0u - (uint32_t)good);   // an item that is not valid adds the identity: B is on the curve
         jj::to_niels(q, u, v);
     }
     jj::madd<false>(r, t, q);
     if (kOwns) {
-        uint32_t x[8], y[8];
-        jj::fmul(x, u, r.Z);
-        jj::fmul(y, v, r.Z);
-        const bool owned = good & jj::feq(x, r.X) & jj::feq(y, r.Y);
+        const bool owned = good & equals_affine(u, v, r);
         flag[i] = owned ? 1 : 0;
         if (cnt_a) warp_count_every(cnt_a, owned);
         if (cnt_b) warp_count_every(cnt_b, !good);
@@ -1658,12 +1668,8 @@ __global__ void __launch_bounds__(kThreads, 3) k_stealth(const uint8_t* __restri
         uint32_t ru[8], rv[8];
         load_fr_rw(ru, R_uv + i * 64);
         load_fr_rw(rv, R_uv + i * 64 + 32);
-#pragma unroll
-        for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m, ru[k] &= m, rv[k] &= m;
-        store_fr(pk + i * 64, ou);
-        store_fr(pk + i * 64 + 32, ov);
-        store_fr(R_uv + i * 64, ru);
-        store_fr(R_uv + i * 64 + 32, rv);
+        store_masked_point(pk + i * 64, ou, ov, m);
+        store_masked_point(R_uv + i * 64, ru, rv, m);
         flag[i] = good ? 1 : 0;
         if (cnt_a) warp_count_every(cnt_a, !good);
     }
@@ -1672,26 +1678,17 @@ __global__ void __launch_bounds__(kThreads, 3) k_stealth(const uint8_t* __restri
 cudaError_t launch_stealth_owns(const void* h, size_t n, const void* table, const uint64_t b_niels[12], const void* note_pk,
                                 const uint8_t* valid, uint8_t* owned, unsigned long long* n_owned,
                                 unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
     NielsArg nb;
     for (int k = 0; k < 12; ++k) nb.w[2 * k] = (uint32_t)b_niels[k], nb.w[2 * k + 1] = (uint32_t)(b_niels[k] >> 32);
-    k_stealth<true><<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), n, static_cast<const uint4*>(table), nb,
-                                                      nullptr, false, valid,
-                                                      const_cast<uint8_t*>(static_cast<const uint8_t*>(note_pk)), nullptr,
-                                                      owned, n_owned, n_invalid);
-    return cudaGetLastError();
+    return launch(k_stealth<true>, n, kThreads, st, h, n, table, nb, nullptr, false, valid, const_cast<void*>(note_pk), nullptr,
+                  owned, n_owned, n_invalid);
 }
 
 cudaError_t launch_stealth_derive(const void* h, size_t n, const void* table, const void* B_uv, bool B_bcast,
                                   const uint8_t* valid, void* R_uv, void* note_pk, uint8_t* ok, unsigned long long* n_invalid,
                                   cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    NielsArg nb = {};
-    k_stealth<false><<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), n, static_cast<const uint4*>(table), nb,
-                                                       static_cast<const uint8_t*>(B_uv), B_bcast, valid,
-                                                       static_cast<uint8_t*>(note_pk), static_cast<uint8_t*>(R_uv), ok,
-                                                       n_invalid, nullptr);
-    return cudaGetLastError();
+    return launch(k_stealth<false>, n, kThreads, st, h, n, table, NielsArg{}, B_uv, B_bcast, valid, note_pk, R_uv, ok, n_invalid,
+                  nullptr);
 }
 
 // ---- note nullifiers: the digest rows [pk'.u, pk'.v, pos] of pk' = [(h + b) mod r_J] G' (jubjub_device.cuh) -------------
@@ -1729,11 +1726,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_nullifier_key(const uint8_t* __
 
 cudaError_t launch_nullifier_key(const void* h, const void* b, bool b_bcast, const uint64_t* pos, size_t n, const void* table,
                                  void* rows, uint8_t* valid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_nullifier_key<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), static_cast<const uint8_t*>(b), b_bcast,
-                                                      pos, n, static_cast<const uint4*>(table), static_cast<uint8_t*>(rows),
-                                                      valid);
-    return cudaGetLastError();
+    return launch(k_nullifier_key, n, kThreads, st, h, b, b_bcast, pos, n, table, rows, valid);
 }
 
 // ---- Schnorr signatures: u = r - c sk mod r_J; [u] G + [c] PK == R, c = challenge(R, m) (jubjub_device.cuh) -----------
@@ -1785,10 +1778,9 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_sign(const uint8_t* __r
     load_fr_rw(ru, R_uv + i * 64);
     load_fr_rw(rv, R_uv + i * 64 + 32);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) u[q] &= m, ru[q] &= m, rv[q] &= m;
+    for (int q = 0; q < 8; ++q) u[q] &= m;
     store_fr(u_out + i * 32, u);
-    store_fr(R_uv + i * 64, ru);
-    store_fr(R_uv + i * 64 + 32, rv);
+    store_masked_point(R_uv + i * 64, ru, rv, m);
     ok[i] = good ? 1 : 0;
     if (n_invalid) warp_count_every(n_invalid, !good);
 }
@@ -1808,14 +1800,12 @@ __device__ __forceinline__ bool schnorr_check(const uint8_t* __restrict__ pk, bo
         load_fr(y, pk + (pb ? 0 : i) * 64 + 32);
         const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
         jj::set_one(one);
-        uint32_t mc = 0u - (uint32_t)canon;            // coordinates >= p enter no product
+        const uint32_t mc = 0u - (uint32_t)canon;      // coordinates >= p enter no product
 #pragma unroll
         for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
         const bool on = canon & jj::on_curve(x, y);
         good &= on;
-        mc = 0u - (uint32_t)on;                         // an off-curve PK is replaced by the identity
-#pragma unroll
-        for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+        mask_point(x, y, 0u - (uint32_t)on);           // an off-curve PK is replaced by the identity
         load_fr(e, c + i * 32);
         jj::scalar_mul_ext<true, true>(acc, e, x, y);
     }
@@ -1830,15 +1820,13 @@ __device__ __forceinline__ bool schnorr_check(const uint8_t* __restrict__ pk, bo
         for (int k = 0; k < 8; ++k) s[k] &= m;
         jj::fixed_base_from<true, false>(t, acc, s, table);
     }
-    uint32_t ru[8], rv[8], x[8], y[8];
+    uint32_t ru[8], rv[8];
     load_fr(ru, R_uv + i * 64);
     load_fr(rv, R_uv + i * 64 + 32);
     const uint32_t m = 0u - (uint32_t)good;             // an invalid item's R may be >= p: it enters no product
 #pragma unroll
     for (int k = 0; k < 8; ++k) ru[k] &= m, rv[k] &= m;
-    jj::fmul(x, ru, t.Z);
-    jj::fmul(y, rv, t.Z);
-    return good & jj::feq(x, t.X) & jj::feq(y, t.Y);
+    return good & equals_affine(ru, rv, t);
 }
 
 // Verify, one thread per item, after k_schnorr_pack (valid[i]: R and m canonical) and the truncated digest (c[i]):
@@ -1861,29 +1849,18 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify(const uint8_t* _
 
 cudaError_t launch_schnorr_pack(const void* R_uv, const void* msg, size_t n, void* rows, uint8_t* flag, bool and_flag,
                                 cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_pack<<<blocks256(n), 256, 0, st>>>(static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(msg), n,
-                                                 static_cast<uint8_t*>(rows), flag, and_flag);
-    return cudaGetLastError();
+    return launch(k_schnorr_pack, n, 256, st, R_uv, msg, n, rows, flag, and_flag);
 }
 
 cudaError_t launch_schnorr_sign(const void* sk, bool sk_bcast, const void* r, const void* c, size_t n, void* u_out, void* R_uv,
                                 uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_sign<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(sk), sk_bcast, static_cast<const uint8_t*>(r),
-                                                     static_cast<const uint8_t*>(c), n, static_cast<uint8_t*>(u_out),
-                                                     static_cast<uint8_t*>(R_uv), ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_schnorr_sign, n, kThreads, st, sk, sk_bcast, r, c, n, u_out, R_uv, ok, n_invalid);
 }
 
 cudaError_t launch_schnorr_verify(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c,
                                   const uint8_t* valid, size_t n, const void* table, uint8_t* verified,
                                   unsigned long long* n_verified, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_verify<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u),
-                                                       static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(c), valid,
-                                                       n, static_cast<const uint4*>(table), verified, n_verified, n_invalid);
-    return cudaGetLastError();
+    return launch(k_schnorr_verify, n, kThreads, st, pk, pk_bcast, u, R_uv, c, valid, n, table, verified, n_verified, n_invalid);
 }
 
 // ---- double-key Schnorr signatures over G and G': c = challenge2(R, R', m) (jubjub_device.cuh) -------------------------
@@ -1953,10 +1930,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_sign_double(const uint8
     if (Note) {
         uint32_t pu[8], pv[8];
         jj::fixed_base_mul<true>(pu, pv, s, table);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) pu[q] &= m, pv[q] &= m;
-        store_fr(pkp_uv + i * 64, pu);
-        store_fr(pkp_uv + i * 64 + 32, pv);
+        store_masked_point(pkp_uv + i * 64, pu, pv, m);
     }
     uint32_t x[8], u[8];
     jj::order_mul(x, e, s);
@@ -1971,10 +1945,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_sign_double(const uint8
         uint32_t pu[8], pv[8];
         load_fr_rw(pu, P);
         load_fr_rw(pv, P + 32);
-#pragma unroll
-        for (int q = 0; q < 8; ++q) pu[q] &= m, pv[q] &= m;
-        store_fr(P, pu);
-        store_fr(P + 32, pv);
+        store_masked_point(P, pu, pv, m);
     }
     ok[i] = good ? 1 : 0;
     if (n_invalid) warp_count_every(n_invalid, !good);
@@ -2009,44 +1980,28 @@ __global__ void __launch_bounds__(kThreads, 3) k_schnorr_verify_double(const uin
 
 cudaError_t launch_schnorr_pack_double(const void* R_uv, const void* Rp_uv, const void* msg, size_t n, void* rows,
                                        uint8_t* flag, bool and_flag, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_pack_double<<<blocks256(n), 256, 0, st>>>(static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(Rp_uv),
-                                                        static_cast<const uint8_t*>(msg), n, static_cast<uint8_t*>(rows), flag,
-                                                        and_flag);
-    return cudaGetLastError();
+    return launch(k_schnorr_pack_double, n, 256, st, R_uv, Rp_uv, msg, n, rows, flag, and_flag);
 }
 
 cudaError_t launch_schnorr_sign_double(const void* sk, bool sk_bcast, const void* r, const void* c, size_t n, void* u_out,
                                        void* R_uv, void* Rp_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_sign_double<false><<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(sk), sk_bcast, nullptr, nullptr, static_cast<const uint8_t*>(r),
-        static_cast<const uint8_t*>(c), n, nullptr, static_cast<uint8_t*>(u_out), static_cast<uint8_t*>(R_uv),
-        static_cast<uint8_t*>(Rp_uv), nullptr, ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_schnorr_sign_double<false>, n, kThreads, st, sk, sk_bcast, nullptr, nullptr, r, c, n, nullptr, u_out, R_uv,
+                  Rp_uv, nullptr, ok, n_invalid);
 }
 
 cudaError_t launch_note_sign_double(const void* b, bool b_bcast, const void* h, const uint8_t* valid, const void* r,
                                     const void* c, size_t n, const void* table_p, void* u_out, void* R_uv, void* Rp_uv,
                                     void* pkp_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_sign_double<true><<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(b), b_bcast, static_cast<const uint8_t*>(h), valid, static_cast<const uint8_t*>(r),
-        static_cast<const uint8_t*>(c), n, static_cast<const uint4*>(table_p), static_cast<uint8_t*>(u_out),
-        static_cast<uint8_t*>(R_uv), static_cast<uint8_t*>(Rp_uv), static_cast<uint8_t*>(pkp_uv), ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_schnorr_sign_double<true>, n, kThreads, st, b, b_bcast, h, valid, r, c, n, table_p, u_out, R_uv, Rp_uv,
+                  pkp_uv, ok, n_invalid);
 }
 
 cudaError_t launch_schnorr_verify_double(const void* pk, const void* pkp, bool pk_bcast, const void* u, const void* R_uv,
                                          const void* Rp_uv, const void* c, const uint8_t* valid, size_t n, const void* table,
                                          const void* table_p, uint8_t* verified, unsigned long long* n_verified,
                                          unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_schnorr_verify_double<<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(pk), static_cast<const uint8_t*>(pkp), pk_bcast, static_cast<const uint8_t*>(u),
-        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(Rp_uv), static_cast<const uint8_t*>(c), valid, n,
-        static_cast<const uint4*>(table), static_cast<const uint4*>(table_p), verified, n_verified, n_invalid);
-    return cudaGetLastError();
+    return launch(k_schnorr_verify_double, n, kThreads, st, pk, pkp, pk_bcast, u, R_uv, Rp_uv, c, valid, n, table, table_p,
+                  verified, n_verified, n_invalid);
 }
 
 // ---- note values: C = [v] G + [blinder] G' (jubjub_device.cuh) ---------------------------------------------------------
@@ -2101,16 +2056,9 @@ __global__ void __launch_bounds__(kThreads, 3) k_value_commit(uint64_t* value, u
         jj::fixed_base_from<true, false, jj::kValueWindows>(t, acc, v, table);
     }
     if (kMode == kValueOpen) {
-        uint32_t cu[8], cv[8], x[8], y[8];
-        load_fr(cu, commitment + i * 64);
-        load_fr(cv, commitment + i * 64 + 32);
-        const bool canon = fr_is_canonical(cu) & fr_is_canonical(cv);
-        const uint32_t mc = 0u - (uint32_t)canon;     // coordinates >= p enter no product
-#pragma unroll
-        for (int k = 0; k < 8; ++k) cu[k] &= mc, cv[k] &= mc;
-        jj::fmul(x, cu, t.Z);
-        jj::fmul(y, cv, t.Z);
-        const bool opened = good & canon & jj::feq(x, t.X) & jj::feq(y, t.Y);
+        uint32_t cu[8], cv[8];
+        const bool canon = load_canonical_point<false>(cu, cv, commitment + i * 64);
+        const bool opened = good & canon & equals_affine(cu, cv, t);
         const uint32_t mo = 0u - (uint32_t)opened;
 #pragma unroll
         for (int k = 0; k < 8; ++k) b[k] &= mo;
@@ -2123,13 +2071,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_value_commit(uint64_t* value, u
         jj::inverse(zi, t.Z);
         jj::fmul(ou, t.X, zi);
         jj::fmul(ov, t.Y, zi);
-        if (kMode == kValueCommit) {
-            const uint32_t m = 0u - (uint32_t)good;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) ou[k] &= m, ov[k] &= m;
-        }
-        store_fr(commitment + i * 64, ou);
-        store_fr(commitment + i * 64 + 32, ov);
+        store_masked_point(commitment + i * 64, ou, ov, kMode == kValueCommit ? 0u - (uint32_t)good : ~0u);
         if (kMode == kValueCommit) {
             ok[i] = good ? 1 : 0;
             if (count) warp_count_every(count, !good);
@@ -2146,32 +2088,21 @@ __global__ void __launch_bounds__(kThreads, 3) k_value_commit(uint64_t* value, u
 
 cudaError_t launch_value_commit(const uint64_t* value, const void* blinder, size_t n, const void* table, const void* table_p,
                                 void* commitment, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_value_commit<kValueCommit><<<grid_for(n), kThreads, 0, st>>>(
-        const_cast<uint64_t*>(value), static_cast<uint8_t*>(const_cast<void*>(blinder)), n, static_cast<const uint4*>(table),
-        static_cast<const uint4*>(table_p), static_cast<uint8_t*>(commitment), nullptr, nullptr, ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_value_commit<kValueCommit>, n, kThreads, st, const_cast<uint64_t*>(value), const_cast<void*>(blinder), n,
+                  table, table_p, commitment, nullptr, nullptr, ok, n_invalid);
 }
 
 cudaError_t launch_note_value(const uint64_t* value, const void* blinder, size_t n, const void* table, const void* table_p,
                               void* commitment, void* rows, uint8_t* valid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_value_commit<kValueCreate><<<grid_for(n), kThreads, 0, st>>>(
-        const_cast<uint64_t*>(value), static_cast<uint8_t*>(const_cast<void*>(blinder)), n, static_cast<const uint4*>(table),
-        static_cast<const uint4*>(table_p), static_cast<uint8_t*>(commitment), static_cast<uint8_t*>(rows), valid, nullptr,
-        nullptr);
-    return cudaGetLastError();
+    return launch(k_value_commit<kValueCreate>, n, kThreads, st, const_cast<uint64_t*>(value), const_cast<void*>(blinder), n,
+                  table, table_p, commitment, rows, valid, nullptr, nullptr);
 }
 
 cudaError_t launch_note_open_value(const void* rows, const uint8_t* valid, const void* commitment, size_t n, const void* table,
                                    const void* table_p, uint64_t* value, void* blinder, uint8_t* ok,
                                    unsigned long long* n_failed, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_value_commit<kValueOpen><<<grid_for(n), kThreads, 0, st>>>(
-        value, static_cast<uint8_t*>(blinder), n, static_cast<const uint4*>(table), static_cast<const uint4*>(table_p),
-        static_cast<uint8_t*>(const_cast<void*>(commitment)), static_cast<uint8_t*>(const_cast<void*>(rows)),
-        const_cast<uint8_t*>(valid), ok, n_failed);
-    return cudaGetLastError();
+    return launch(k_value_commit<kValueOpen>, n, kThreads, st, value, blinder, n, table, table_p, const_cast<void*>(commitment),
+                  const_cast<void*>(rows), const_cast<uint8_t*>(valid), ok, n_failed);
 }
 
 // ---- wallet scans: owner, nullifier, checked opening and per-key totals (jubjub_device.cuh) -----------------------------
@@ -2218,16 +2149,12 @@ __global__ void __launch_bounds__(kThreads, 3) k_wallet_dhke(const uint8_t* __re
     load_fr(v, R + i * 64 + 32);
     const bool valid = (kvalid[j] != 0) & fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
     const uint32_t m = 0u - (uint32_t)valid;
-    uint32_t one[8];
-    jj::set_one(one);
 #pragma unroll
-    for (int q = 0; q < 8; ++q) s[q] &= m, u[q] &= m, v[q] = (v[q] & m) | (one[q] & ~m);
+    for (int q = 0; q < 8; ++q) s[q] &= m;
+    mask_point(u, v, m);
     uint32_t ou[8], ov[8];
     jj::scalar_mul(ou, ov, s, u, v);
-#pragma unroll
-    for (int q = 0; q < 8; ++q) ou[q] &= m, ov[q] &= m;
-    store_fr(out + p * 64, ou);
-    store_fr(out + p * 64 + 32, ov);
+    store_masked_point(out + p * 64, ou, ov, m);
     ok[p] = valid ? 1 : 0;
 }
 
@@ -2247,21 +2174,13 @@ __global__ void __launch_bounds__(kThreads, 3) k_wallet_match(const uint8_t* __r
         jj::fixed_base_ext<true, true>(t, s, table);
     }
     uint32_t u[8], v[8];
-    load_fr(u, note_pk + i * 64);
-    load_fr(v, note_pk + i * 64 + 32);
-    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
-    const uint32_t mc = 0u - (uint32_t)canon;     // coordinates >= p enter no product
-#pragma unroll
-    for (int q = 0; q < 8; ++q) u[q] &= mc, v[q] &= mc;
+    const bool canon = load_canonical_point<false>(u, v, note_pk + i * 64);
     jj::Niels q;
     load_fr(q.ymx, nb + j * 96);
     load_fr(q.ypx, nb + j * 96 + 32);
     load_fr(q.kt, nb + j * 96 + 64);
     jj::madd<false>(r, t, q);
-    uint32_t x[8], y[8];
-    jj::fmul(x, u, r.Z);
-    jj::fmul(y, v, r.Z);
-    matched[p] = (valid[p] != 0) & canon & jj::feq(x, r.X) & jj::feq(y, r.Y) ? 1 : 0;
+    matched[p] = (valid[p] != 0) & canon & equals_affine(u, v, r) ? 1 : 0;
 }
 
 // select (per note, kProductsPerWalletSelect): owner[i] = the smallest j with matched[i k + j], -1 if none; the note's
@@ -2297,12 +2216,8 @@ __global__ void __launch_bounds__(kThreads) k_wallet_select(uint32_t k, const ui
     for (int32_t j = (int32_t)k - 1; j >= 0; --j) own = matched[i * k + j] ? j : own;
     {
         uint32_t u[8], v[8];
-        load_fr(u, R + i * 64);
-        load_fr(v, R + i * 64 + 32);
-        bool good = fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
-        load_fr(u, note_pk + i * 64);
-        load_fr(v, note_pk + i * 64 + 32);
-        good &= fr_is_canonical(u) & fr_is_canonical(v);
+        bool good = load_curve_point(u, v, R + i * 64);
+        good &= load_canonical_point<false>(u, v, note_pk + i * 64);
         if (n_invalid) warp_count_every(n_invalid, !good);
     }
     const uint32_t zero[8] = {0, 0, 0, 0, 0, 0, 0, 0};
@@ -2379,29 +2294,17 @@ __global__ void __launch_bounds__(256) k_wallet_scatter(const uint2* __restrict_
 
 cudaError_t launch_wallet_keys(const void* a, const void* b, uint32_t k, const void* table, void* nb, uint8_t* kvalid,
                                unsigned long long* n_owned, unsigned long long* n_bad, cudaStream_t st) {
-    k_wallet_keys<<<(k + kThreads - 1) / kThreads, kThreads, 0, st>>>(static_cast<const uint8_t*>(a),
-                                                                     static_cast<const uint8_t*>(b), k,
-                                                                     static_cast<const uint4*>(table),
-                                                                     static_cast<uint8_t*>(nb), kvalid, n_owned, n_bad);
-    return cudaGetLastError();
+    return launch(k_wallet_keys, k, kThreads, st, a, b, k, table, nb, kvalid, n_owned, n_bad);
 }
 
 cudaError_t launch_wallet_dhke(const void* a, const uint8_t* kvalid, uint32_t k, const void* R_uv, size_t n_pairs, void* shared_uv,
                                uint8_t* valid, cudaStream_t st) {
-    if (n_pairs == 0) return cudaSuccess;
-    k_wallet_dhke<<<grid_for(n_pairs), kThreads, 0, st>>>(static_cast<const uint8_t*>(a), kvalid, k,
-                                                          static_cast<const uint8_t*>(R_uv), n_pairs,
-                                                          static_cast<uint8_t*>(shared_uv), valid);
-    return cudaGetLastError();
+    return launch(k_wallet_dhke, n_pairs, kThreads, st, a, kvalid, k, R_uv, n_pairs, shared_uv, valid);
 }
 
 cudaError_t launch_wallet_match(const void* h, size_t n_pairs, uint32_t k, const void* table, const void* nb, const void* note_pk,
                                 const uint8_t* valid, uint8_t* matched, cudaStream_t st) {
-    if (n_pairs == 0) return cudaSuccess;
-    k_wallet_match<<<grid_for(n_pairs), kThreads, 0, st>>>(static_cast<const uint8_t*>(h), n_pairs, k,
-                                                           static_cast<const uint4*>(table), static_cast<const uint8_t*>(nb),
-                                                           static_cast<const uint8_t*>(note_pk), valid, matched);
-    return cudaGetLastError();
+    return launch(k_wallet_match, n_pairs, kThreads, st, h, n_pairs, k, table, nb, note_pk, valid, matched);
 }
 
 cudaError_t launch_wallet_select(uint32_t k, const uint8_t* matched, const void* S, const void* h, const void* b,
@@ -2409,44 +2312,21 @@ cudaError_t launch_wallet_select(uint32_t k, const uint8_t* matched, const void*
                                  const void* cipher, const void* C, size_t n, int32_t* owner, void* nullifier, uint64_t* value,
                                  void* blinder, uint8_t* opened, const WalletRows& dense, unsigned long long* n_owned,
                                  unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
     WalletDense dn{static_cast<uint2*>(dense.meta), static_cast<uint8_t*>(dense.S), static_cast<uint8_t*>(dense.h),
                    static_cast<uint8_t*>(dense.b), dense.pos, static_cast<uint8_t*>(dense.nonce),
                    static_cast<uint8_t*>(dense.cipher), static_cast<uint8_t*>(dense.C), dense.valid};
-    k_wallet_select<<<grid_for(n), kThreads, 0, st>>>(
-        k, matched, static_cast<const uint8_t*>(S), static_cast<const uint8_t*>(h), static_cast<const uint8_t*>(b),
-        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(note_pk), pos, static_cast<const uint8_t*>(nonce),
-        static_cast<const uint8_t*>(cipher), static_cast<const uint8_t*>(C), n, owner, static_cast<uint8_t*>(nullifier), value,
-        static_cast<uint8_t*>(blinder), opened, dn, n_owned, n_invalid);
-    return cudaGetLastError();
+    return launch(k_wallet_select, n, kThreads, st, k, matched, S, h, b, R_uv, note_pk, pos, nonce, cipher, C, n, owner, nullifier,
+                  value, blinder, opened, dn, n_owned, n_invalid);
 }
 
 cudaError_t launch_wallet_scatter(const void* meta, const void* nul, const uint64_t* value_rows, const void* blinder_rows,
                                   const uint8_t* ok, size_t n_own, void* nullifier, uint64_t* value, void* blinder,
                                   uint8_t* opened, unsigned long long* totals, cudaStream_t st) {
-    if (n_own == 0) return cudaSuccess;
-    k_wallet_scatter<<<blocks256(n_own), 256, 0, st>>>(static_cast<const uint2*>(meta), static_cast<const uint8_t*>(nul),
-                                                       value_rows, static_cast<const uint8_t*>(blinder_rows), ok, n_own,
-                                                       static_cast<uint8_t*>(nullifier), value, static_cast<uint8_t*>(blinder),
-                                                       opened, totals);
-    return cudaGetLastError();
+    return launch(k_wallet_scatter, n_own, 256, st, meta, nul, value_rows, blinder_rows, ok, n_own, nullifier, value, blinder,
+                  opened, totals);
 }
 
 // ---- JubJub ElGamal: (c1, c2) = ([r] G, M + [r] PK), M = c2 - [sk] c1 (jubjub_device.cuh) -----------------------------
-// Whether the point row at p, loaded into (u, v), is a curve point with u, v < p
-__device__ __forceinline__ bool load_point(uint32_t (&u)[8], uint32_t (&v)[8], const uint8_t* p) {
-    load_fr(u, p);
-    load_fr(v, p + 32);
-    return fr_is_canonical(u) & fr_is_canonical(v) & jj::on_curve(u, v);
-}
-// (u, v) = m ? (u, v) : the identity (0, 1), for an all-ones or all-zeros mask m
-__device__ __forceinline__ void mask_point(uint32_t (&u)[8], uint32_t (&v)[8], uint32_t m) {
-    uint32_t one[8];
-    jj::set_one(one);
-#pragma unroll
-    for (int k = 0; k < 8; ++k) u[k] &= m, v[k] = (v[k] & m) | (one[k] & ~m);
-}
-
 // One thread per item, jj::elgamal_enc_products<kPairs>() products.  Item i reads PK = pk[pb ? 0 : i], and for each pair
 // j < kPairs the message M_j = (j ? m1 : m0)[mb ? 0 : i] and r_j = r[kPairs i + j] (canonical 4 x u64); points are (u, v)
 // Montgomery pairs.  c1_j goes to c1 + i stride + 128 j, c2_j to c2 + i stride + 128 j: the generic call has kPairs = 1,
@@ -2468,11 +2348,11 @@ __global__ void __launch_bounds__(kThreads, 3) k_elgamal_enc(const uint8_t* __re
     const uint8_t* mi1 = kPairs == 2 ? m1 + (mb ? 0 : i) * 64 : mi0;
     const uint8_t* ri = r + i * kPairs * 32;
     uint32_t u[8], v[8], s[8];
-    bool valid = load_point(u, v, pk + (pb ? 0 : i) * 64);
+    bool valid = load_curve_point(u, v, pk + (pb ? 0 : i) * 64);
 #pragma unroll
     for (int j = 0; j < kPairs; ++j) {
         uint32_t mu[8], mv[8];
-        valid &= load_point(mu, mv, j ? mi1 : mi0);
+        valid &= load_curve_point(mu, mv, j ? mi1 : mi0);
         load_fr(s, ri + j * 32);
         valid &= jj::below_order(s);
     }
@@ -2508,13 +2388,8 @@ __global__ void __launch_bounds__(kThreads, 3) k_elgamal_enc(const uint8_t* __re
     }
     jj::batch_affine(out);
 #pragma unroll
-    for (int j = 0; j < 2 * kPairs; ++j) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) out[j].X[k] &= m, out[j].Y[k] &= m;
-        uint8_t* row = ((j & 1) ? c2 : c1) + i * stride + (j >> 1) * 128;
-        store_fr(row, out[j].X);
-        store_fr(row + 32, out[j].Y);
-    }
+    for (int j = 0; j < 2 * kPairs; ++j)
+        store_masked_point(((j & 1) ? c2 : c1) + i * stride + (j >> 1) * 128, out[j].X, out[j].Y, m);
     ok[i] = valid ? 1 : 0;
     if (n_invalid) warp_count_every(n_invalid, !valid);
 }
@@ -2556,8 +2431,8 @@ __global__ void __launch_bounds__(kThreads, kNote ? 3 : 4) k_elgamal_dec(const u
     }
 #pragma unroll 1
     for (int j = 0; j < kPairs; ++j) {
-        good &= load_point(u, v, c1 + i * stride + j * 128);
-        good &= load_point(u, v, c2 + i * stride + j * 128);
+        good &= load_curve_point(u, v, c1 + i * stride + j * 128);
+        good &= load_curve_point(u, v, c2 + i * stride + j * 128);
     }
     const uint32_t m = 0u - (uint32_t)good;
 #pragma unroll
@@ -2587,13 +2462,8 @@ __global__ void __launch_bounds__(kThreads, kNote ? 3 : 4) k_elgamal_dec(const u
     if (kNote) {
         jj::Ext t;
         jj::fixed_base_ext<true, false>(t, s, table);
-        load_fr(u, note_pk + i * 64);
-        load_fr(v, note_pk + i * 64 + 32);
-        const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
-        const uint32_t mc = 0u - (uint32_t)canon;   // coordinates >= p enter no product
+        const bool canon = load_canonical_point<false>(u, v, note_pk + i * 64);
         uint32_t x[8], y[8];
-#pragma unroll
-        for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] &= mc;
         jj::fmul(x, u, t.Z);
         jj::fmul(y, v, t.Z);
         opened = good & canon & jj::feq(x, t.X) & jj::feq(y, t.Y);
@@ -2601,13 +2471,7 @@ __global__ void __launch_bounds__(kThreads, kNote ? 3 : 4) k_elgamal_dec(const u
     jj::batch_affine(out);
     const uint32_t mo = 0u - (uint32_t)opened;
 #pragma unroll
-    for (int j = 0; j < kPairs; ++j) {
-#pragma unroll
-        for (int k = 0; k < 8; ++k) out[j].X[k] &= mo, out[j].Y[k] &= mo;
-        uint8_t* row = (j ? out1 : out0) + i * 64;
-        store_fr(row, out[j].X);
-        store_fr(row + 32, out[j].Y);
-    }
+    for (int j = 0; j < kPairs; ++j) store_masked_point((j ? out1 : out0) + i * 64, out[j].X, out[j].Y, mo);
     ok[i] = opened ? 1 : 0;
     if (count) warp_count_every(count, !opened);
 }
@@ -2615,45 +2479,30 @@ __global__ void __launch_bounds__(kThreads, kNote ? 3 : 4) k_elgamal_dec(const u
 cudaError_t launch_elgamal_encrypt(const void* pk, bool pk_bcast, const void* msg, bool msg_bcast, const void* r, size_t n,
                                    const void* table, void* c1_uv, void* c2_uv, uint8_t* ok, unsigned long long* n_invalid,
                                    cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_elgamal_enc<1><<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(msg), nullptr, msg_bcast,
-        static_cast<const uint8_t*>(r), n, static_cast<const uint4*>(table), static_cast<uint8_t*>(c1_uv),
-        static_cast<uint8_t*>(c2_uv), 64, ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_elgamal_enc<1>, n, kThreads, st, pk, pk_bcast, msg, nullptr, msg_bcast, r, n, table, c1_uv, c2_uv, 64, ok,
+                  n_invalid);
 }
 
 cudaError_t launch_note_sender_encrypt(const void* note_pk, const void* A_uv, const void* B_uv, bool sender_bcast,
                                        const void* blinder, size_t n, const void* table, void* enc, uint8_t* ok,
                                        unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
     uint8_t* e = static_cast<uint8_t*>(enc);
-    k_elgamal_enc<2><<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(note_pk), false, static_cast<const uint8_t*>(A_uv), static_cast<const uint8_t*>(B_uv),
-        sender_bcast, static_cast<const uint8_t*>(blinder), n, static_cast<const uint4*>(table), e, e + 64, 256, ok,
-        n_invalid);
-    return cudaGetLastError();
+    return launch(k_elgamal_enc<2>, n, kThreads, st, note_pk, false, A_uv, B_uv, sender_bcast, blinder, n, table, e, e + 64, 256,
+                  ok, n_invalid);
 }
 
 cudaError_t launch_elgamal_decrypt(const void* sk, bool sk_bcast, const void* c1_uv, const void* c2_uv, size_t n,
                                    void* msg_uv, uint8_t* ok, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_elgamal_dec<false><<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(sk), sk_bcast, nullptr, nullptr, nullptr, static_cast<const uint8_t*>(c1_uv),
-        static_cast<const uint8_t*>(c2_uv), 64, n, nullptr, static_cast<uint8_t*>(msg_uv), nullptr, ok, n_invalid);
-    return cudaGetLastError();
+    return launch(k_elgamal_dec<false>, n, kThreads, st, sk, sk_bcast, nullptr, nullptr, nullptr, c1_uv, c2_uv, 64, n, nullptr,
+                  msg_uv, nullptr, ok, n_invalid);
 }
 
 cudaError_t launch_note_sender_decrypt(const void* h, const void* b, bool b_bcast, const uint8_t* valid, const void* note_pk,
                                        const void* enc, size_t n, const void* table, void* A_uv, void* B_uv, uint8_t* ok,
                                        unsigned long long* n_failed, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
     const uint8_t* e = static_cast<const uint8_t*>(enc);
-    k_elgamal_dec<true><<<grid_for(n), kThreads, 0, st>>>(
-        static_cast<const uint8_t*>(b), b_bcast, static_cast<const uint8_t*>(h), valid, static_cast<const uint8_t*>(note_pk),
-        e, e + 64, 256, n, static_cast<const uint4*>(table), static_cast<uint8_t*>(A_uv), static_cast<uint8_t*>(B_uv), ok,
-        n_failed);
-    return cudaGetLastError();
+    return launch(k_elgamal_dec<true>, n, kThreads, st, b, b_bcast, h, valid, note_pk, e, e + 64, 256, n, table, A_uv, B_uv, ok,
+                  n_failed);
 }
 
 // ---- point compression: JubJubAffine::from_bytes / to_bytes (jubjub_device.cuh) ---------------------------------------
@@ -2668,11 +2517,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_points_from_bytes(const uint8_t
     uint32_t b[8], u[8], v[8];
     load_fr(b, bytes + i * 32);
     const bool good = jj::decompress(u, v, b);
-    const uint32_t m = 0u - (uint32_t)good;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) u[k] &= m, v[k] &= m;
-    store_fr(uv + i * 64, u);
-    store_fr(uv + i * 64 + 32, v);
+    store_masked_point(uv + i * 64, u, v, 0u - (uint32_t)good);
     ok[i] = good ? 1 : 0;
     if (n_invalid) warp_count_every(n_invalid, !good);
 }
@@ -2685,12 +2530,7 @@ __global__ void __launch_bounds__(kThreads, 3) k_points_to_bytes(const uint8_t* 
     const size_t i = (size_t)blockIdx.x * kThreads + threadIdx.x;
     if (i >= n) return;
     uint32_t u[8], v[8], b[8];
-    load_fr(u, uv + i * 64);
-    load_fr(v, uv + i * 64 + 32);
-    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
-    const uint32_t mc = 0u - (uint32_t)canon;           // coordinates >= p enter no product
-#pragma unroll
-    for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] &= mc;
+    const bool canon = load_canonical_point<false>(u, v, uv + i * 64);
     const bool good = canon & jj::on_curve(u, v);
     jj::compress(b, u, v);
     const uint32_t m = 0u - (uint32_t)good;
@@ -2703,18 +2543,12 @@ __global__ void __launch_bounds__(kThreads, 3) k_points_to_bytes(const uint8_t* 
 
 cudaError_t launch_points_from_bytes(const void* bytes, size_t n, void* uv, uint8_t* ok, unsigned long long* n_invalid,
                                      cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_points_from_bytes<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(bytes), n, static_cast<uint8_t*>(uv), ok,
-                                                          n_invalid);
-    return cudaGetLastError();
+    return launch(k_points_from_bytes, n, kThreads, st, bytes, n, uv, ok, n_invalid);
 }
 
 cudaError_t launch_points_to_bytes(const void* uv, size_t n, void* bytes, uint8_t* ok, unsigned long long* n_invalid,
                                    cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_points_to_bytes<<<grid_for(n), kThreads, 0, st>>>(static_cast<const uint8_t*>(uv), n, static_cast<uint8_t*>(bytes), ok,
-                                                        n_invalid);
-    return cudaGetLastError();
+    return launch(k_points_to_bytes, n, kThreads, st, uv, n, bytes, ok, n_invalid);
 }
 
 // ---- multi-scalar multiplication by buckets (jubjub_device.cuh): sum [s_i] P_i --------------------------------------
@@ -2735,15 +2569,9 @@ __global__ void __launch_bounds__(kMsmThreads) k_msm_prep(const uint8_t* __restr
                                                           unsigned long long* __restrict__ n_invalid) {
     const uint32_t i = blockIdx.x * kMsmThreads + threadIdx.x;
     if (i >= m) return;
-    uint32_t s[8], u[8], v[8], one[8];
+    uint32_t s[8], u[8], v[8];
     load_fr(s, sc + (size_t)i * 32);
-    load_fr(u, pts + (size_t)i * 64);
-    load_fr(v, pts + (size_t)i * 64 + 32);
-    jj::set_one(one);
-    const bool canon = fr_is_canonical(u) & fr_is_canonical(v);
-    const uint32_t mc = 0u - (uint32_t)canon;            // coordinates >= p enter no product
-#pragma unroll
-    for (int k = 0; k < 8; ++k) u[k] &= mc, v[k] = (v[k] & mc) | (one[k] & ~mc);
+    const bool canon = load_canonical_point<true>(u, v, pts + (size_t)i * 64);
     const bool valid = canon & jj::below_order(s) & jj::on_curve(u, v);
     if (n_invalid) warp_count_every(n_invalid, !valid);
     jj::Niels q;
@@ -2929,7 +2757,7 @@ __global__ void __launch_bounds__(kMsmThreads) k_msmv_prep(const uint8_t* __rest
         load_fr(x, pk + (pb ? 0 : (size_t)i) * 64);
         load_fr(y, pk + (pb ? 0 : (size_t)i) * 64 + 32);
         const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
-        uint32_t mc = 0u - (uint32_t)canon;
+        const uint32_t mc = 0u - (uint32_t)canon;
 #pragma unroll
         for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
         load_fr(s, u + (size_t)i * 32);
@@ -2939,9 +2767,7 @@ __global__ void __launch_bounds__(kMsmThreads) k_msmv_prep(const uint8_t* __rest
         uint32_t ru[8], rv[8];
         load_fr(ru, R_uv + (size_t)i * 64);
         load_fr(rv, R_uv + (size_t)i * 64 + 32);
-        mc = 0u - (uint32_t)good;                       // an invalid item's R may be >= p: it enters no product
-#pragma unroll
-        for (int k = 0; k < 8; ++k) ru[k] &= mc, rv[k] = (rv[k] & mc) | (one[k] & ~mc);
+        mask_point(ru, rv, 0u - (uint32_t)good);        // an invalid item's R may be >= p: it enters no product
         const bool r_on = jj::on_curve(ru, rv);
         if (!good || !r_on) *bad = 1u;
         if (n_invalid) warp_count_every(n_invalid, !good);
@@ -3064,14 +2890,9 @@ __global__ void __launch_bounds__(kMsmThreads) k_msm_final(MsmFinal a) {
             uint32_t s[8], x[8], y[8], one[8];
 #pragma unroll
             for (int k = 0; k < 8; ++k) s[k] = ss[0][8 + k];
-            load_fr(x, a.pk);
-            load_fr(y, a.pk + 32);
+            load_canonical_point<true>(x, y, a.pk);
             jj::set_one(one);
-            const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
-            uint32_t mc = 0u - (uint32_t)canon;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
-            mc = 0u - (uint32_t)jj::on_curve(x, y);    // an off-curve PK made every item invalid: *bad is set
+            const uint32_t mc = 0u - (uint32_t)jj::on_curve(x, y);    // an off-curve PK made every item invalid: *bad is set
 #pragma unroll
             for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc), s[k] &= mc;
             jj::scalar_mul_ext<true, true>(t, s, x, y);
@@ -3119,36 +2940,22 @@ __global__ void __launch_bounds__(kMsmThreads) k_msm_final(MsmFinal a) {
 
 cudaError_t launch_msm_prep(const void* scalars, const void* points, uint32_t m, int c, void* niels, uint32_t* keys,
                             uint32_t* vals, unsigned long long* n_invalid, cudaStream_t st) {
-    if (m == 0) return cudaSuccess;
-    k_msm_prep<<<(m + kMsmThreads - 1) / kMsmThreads, kMsmThreads, 0, st>>>(
-        static_cast<const uint8_t*>(scalars), static_cast<const uint8_t*>(points), m, c, static_cast<uint4*>(niels), keys, vals,
-        n_invalid);
-    return cudaGetLastError();
+    return launch(k_msm_prep, m, kMsmThreads, st, scalars, points, m, c, niels, keys, vals, n_invalid);
 }
 
 cudaError_t launch_msm_fill(void* buckets, uint32_t nb, cudaStream_t st) {
-    k_msm_fill<<<blocks256(nb), 256, 0, st>>>(static_cast<uint4*>(buckets), nb);
-    return cudaGetLastError();
+    return launch(k_msm_fill, nb, 256, st, buckets, nb);
 }
 
 cudaError_t launch_msm_bucket(bool rows, const uint32_t* keys, const uint32_t* vals, const void* src, uint32_t N, uint32_t nb,
                               void* buckets, uint32_t* okeys, void* opts, cudaStream_t st) {
-    if (N == 0) return cudaSuccess;
-    const uint32_t pieces = (N + kMsmPiece - 1) / kMsmPiece;
-    const unsigned grid = (pieces + kMsmThreads - 1) / kMsmThreads;
-    if (rows)
-        k_msm_bucket<true><<<grid, kMsmThreads, 0, st>>>(keys, vals, static_cast<const uint4*>(src), N, nb,
-                                                         static_cast<uint4*>(buckets), okeys, static_cast<uint4*>(opts));
-    else
-        k_msm_bucket<false><<<grid, kMsmThreads, 0, st>>>(keys, vals, static_cast<const uint4*>(src), N, nb,
-                                                          static_cast<uint4*>(buckets), okeys, static_cast<uint4*>(opts));
-    return cudaGetLastError();
+    const uint32_t pieces = (N + kMsmPiece - 1) / kMsmPiece;   // one thread per piece
+    if (rows) return launch(k_msm_bucket<true>, pieces, kMsmThreads, st, keys, vals, src, N, nb, buckets, okeys, opts);
+    return launch(k_msm_bucket<false>, pieces, kMsmThreads, st, keys, vals, src, N, nb, buckets, okeys, opts);
 }
 
 cudaError_t launch_msm_window(const void* buckets, int c, void* wsum, cudaStream_t st) {
-    k_msm_window<<<jj::msm_windows(c), msm_window_parts(c), 0, st>>>(static_cast<const uint4*>(buckets), c,
-                                                                      static_cast<uint4*>(wsum));
-    return cudaGetLastError();
+    return launch_grid(k_msm_window, jj::msm_windows(c), msm_window_parts(c), st, buckets, c, wsum);
 }
 
 cudaError_t launch_msm_final(const void* wsum, uint32_t nchunks, int c, void* out_uv, const void* zsum, uint32_t nsum,
@@ -3156,19 +2963,14 @@ cudaError_t launch_msm_final(const void* wsum, uint32_t nchunks, int c, void* ou
                              cudaStream_t st) {
     MsmFinal a{static_cast<const uint4*>(wsum), nchunks, c, static_cast<uint8_t*>(out_uv), static_cast<const uint8_t*>(zsum),
                nsum, static_cast<const uint4*>(table), static_cast<const uint8_t*>(pk), bad, verified};
-    k_msm_final<<<1, kMsmThreads, 0, st>>>(a);
-    return cudaGetLastError();
+    return launch_grid(k_msm_final, 1, kMsmThreads, st, a);
 }
 
 cudaError_t launch_msmv_prep(const void* pk, bool pk_bcast, const void* u, const void* R_uv, const void* c, const void* z,
                              const uint8_t* valid, uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0,
                              uint32_t* bad, unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_msmv_prep<<<(n + kMsmThreads - 1) / kMsmThreads, kMsmThreads, 0, st>>>(
-        static_cast<const uint8_t*>(pk), pk_bcast, static_cast<const uint8_t*>(u), static_cast<const uint8_t*>(R_uv),
-        static_cast<const uint8_t*>(c), static_cast<const uint8_t*>(z), valid, n, static_cast<uint8_t*>(row_scalars),
-        static_cast<uint8_t*>(row_points), static_cast<uint8_t*>(zsum), blk0, bad, n_invalid);
-    return cudaGetLastError();
+    return launch(k_msmv_prep, n, kMsmThreads, st, pk, pk_bcast, u, R_uv, c, z, valid, n, row_scalars, row_points, zsum, blk0,
+                  bad, n_invalid);
 }
 
 // ---- all-or-nothing verification of double-key signatures: one MSM over G and G' ---------------------------------------
@@ -3207,12 +3009,7 @@ __global__ void __launch_bounds__(kMsmThreads) k_msmv_prep_double(const uint8_t*
         bool good = (valid[i] != 0) & jj::below_order(s);
 #pragma unroll 1
         for (int side = 0; side < 2; ++side) {
-            load_fr(x, key(side));
-            load_fr(y, key(side) + 32);
-            const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
-            const uint32_t mc = 0u - (uint32_t)canon;   // coordinates >= p enter no product
-#pragma unroll
-            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
+            const bool canon = load_canonical_point<true>(x, y, key(side));
             load_fr(w, wt(side));
             good &= canon & jj::on_curve(x, y) & jj::below_order(w);
         }
@@ -3246,8 +3043,7 @@ __global__ void __launch_bounds__(kMsmThreads) k_msmv_prep_double(const uint8_t*
             jj::order_mul(t, w, e);                     // c < 2^250 < r_J
             load_fr(x, rr(side));
             load_fr(y, rr(side) + 32);
-#pragma unroll
-            for (int k = 0; k < 8; ++k) x[k] &= mg, y[k] = (y[k] & mg) | (one[k] & ~mg);
+            mask_point(x, y, mg);
             uint32_t nx[8];
             fr_sub_mod(nx, zero, x);
             store_fr(rsc + (r0 + side) * 32, w);
@@ -3259,8 +3055,7 @@ __global__ void __launch_bounds__(kMsmThreads) k_msmv_prep_double(const uint8_t*
             } else {
                 load_fr(x, key(side));
                 load_fr(y, key(side) + 32);
-#pragma unroll
-                for (int k = 0; k < 8; ++k) x[k] &= mg, y[k] = (y[k] & mg) | (one[k] & ~mg);
+                mask_point(x, y, mg);
                 store_fr(rsc + (per * i + side) * 32, t);
                 store_fr(rpt + (per * i + side) * 64, x);
                 store_fr(rpt + (per * i + side) * 64 + 32, y);
@@ -3367,14 +3162,9 @@ __global__ void __launch_bounds__(kMsmFinalThreads) k_msmv_final_double(MsmFinal
             uint32_t s[8], x[8], y[8], one[8];
 #pragma unroll
             for (int k = 0; k < 8; ++k) s[k] = ss[0][16 + 8 * side + k];
-            load_fr(x, a.pk + side * 64);
-            load_fr(y, a.pk + side * 64 + 32);
+            load_canonical_point<true>(x, y, a.pk + side * 64);
             jj::set_one(one);
-            const bool canon = fr_is_canonical(x) & fr_is_canonical(y);
-            uint32_t mc = 0u - (uint32_t)canon;
-#pragma unroll
-            for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc);
-            mc = 0u - (uint32_t)jj::on_curve(x, y);    // an off-curve key made every item invalid: *bad is set
+            const uint32_t mc = 0u - (uint32_t)jj::on_curve(x, y);    // an off-curve key made every item invalid: *bad is set
 #pragma unroll
             for (int k = 0; k < 8; ++k) x[k] &= mc, y[k] = (y[k] & mc) | (one[k] & ~mc), s[k] &= mc;
             jj::scalar_mul_ext<true, true>(t, s, x, y);
@@ -3417,13 +3207,8 @@ cudaError_t launch_msmv_prep_double(const void* pk, const void* pkp, bool pk_bca
                                     const void* Rp_uv, const void* c, const void* z, const void* zp, const uint8_t* valid,
                                     uint32_t n, void* row_scalars, void* row_points, void* zsum, uint32_t blk0, uint32_t* bad,
                                     unsigned long long* n_invalid, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_msmv_prep_double<<<(n + kMsmThreads - 1) / kMsmThreads, kMsmThreads, 0, st>>>(
-        static_cast<const uint8_t*>(pk), static_cast<const uint8_t*>(pkp), pk_bcast, static_cast<const uint8_t*>(u),
-        static_cast<const uint8_t*>(R_uv), static_cast<const uint8_t*>(Rp_uv), static_cast<const uint8_t*>(c),
-        static_cast<const uint8_t*>(z), static_cast<const uint8_t*>(zp), valid, n, static_cast<uint8_t*>(row_scalars),
-        static_cast<uint8_t*>(row_points), static_cast<uint8_t*>(zsum), blk0, bad, n_invalid);
-    return cudaGetLastError();
+    return launch(k_msmv_prep_double, n, kMsmThreads, st, pk, pkp, pk_bcast, u, R_uv, Rp_uv, c, z, zp, valid, n, row_scalars,
+                  row_points, zsum, blk0, bad, n_invalid);
 }
 
 cudaError_t launch_msmv_final_double(const void* wsum, uint32_t nchunks, int c, const void* zsum, uint32_t nsum,
@@ -3432,249 +3217,174 @@ cudaError_t launch_msmv_final_double(const void* wsum, uint32_t nchunks, int c, 
     MsmFinalDouble a{static_cast<const uint4*>(wsum), nchunks, c, static_cast<const uint8_t*>(zsum), nsum,
                      static_cast<const uint4*>(table), static_cast<const uint4*>(table_p), static_cast<const uint8_t*>(pk),
                      bad, verified};
-    k_msmv_final_double<<<1, kMsmFinalThreads, 0, st>>>(a);
-    return cudaGetLastError();
+    return launch_grid(k_msmv_final_double, 1, kMsmFinalThreads, st, a);
 }
 
 cudaError_t launch_merkle_open(const void* leaves, const void* nodes, const uint64_t* leaf_idx, size_t n, int arity,
                                uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st, const uint8_t* present) {
-    if (n == 0 || depth == 0) return cudaSuccess;
-    const unsigned grid = blocks256(n * depth);
-    const uint8_t* l = static_cast<const uint8_t*>(leaves);
-    const uint8_t* o = static_cast<const uint8_t*>(nodes);
     const uint32_t la = log2_arity(arity);
     if (present)
-        k_merkle_open<true><<<grid, 256, 0, st>>>(l, o, leaf_idx, n, la, depth, lv, static_cast<uint8_t*>(paths), present);
-    else
-        k_merkle_open<false><<<grid, 256, 0, st>>>(l, o, leaf_idx, n, la, depth, lv, static_cast<uint8_t*>(paths), nullptr);
-    return cudaGetLastError();
+        return launch(k_merkle_open<true>, n * depth, 256, st, leaves, nodes, leaf_idx, n, la, depth, lv, paths, present);
+    return launch(k_merkle_open<false>, n * depth, 256, st, leaves, nodes, leaf_idx, n, la, depth, lv, paths, nullptr);
 }
 
 cudaError_t launch_mtree_keys(const uint64_t* idx, uint32_t n_upd, uint64_t n_old, uint32_t total, uint64_t* keys,
                               uint32_t* pos, unsigned long long* rejected, cudaStream_t st) {
-    if (total == 0) return cudaSuccess;
-    k_mtree_keys<<<blocks256(total), 256, 0, st>>>(idx, n_upd, n_old, total, keys, pos, rejected);
-    return cudaGetLastError();
+    return launch(k_mtree_keys, total, 256, st, idx, n_upd, n_old, total, keys, pos, rejected);
 }
 
 cudaError_t launch_mtree_leaf_write(const uint64_t* keys, const uint32_t* pos, uint32_t total, uint64_t sentinel, int arity,
                                     const void* values, uint32_t n_upd, const void* append, void* leaves, uint8_t* flag,
                                     uint64_t* parent, cudaStream_t st) {
-    if (total == 0) return cudaSuccess;
-    k_mtree_leaf_write<<<blocks256(total), 256, 0, st>>>(keys, pos, total, sentinel, log2_arity(arity),
-                                                            static_cast<const uint8_t*>(values), n_upd,
-                                                            static_cast<const uint8_t*>(append), static_cast<uint8_t*>(leaves),
-                                                            flag, parent);
-    return cudaGetLastError();
+    return launch(k_mtree_leaf_write, total, 256, st, keys, pos, total, sentinel, log2_arity(arity), values, n_upd, append, leaves,
+                  flag, parent);
 }
 
 cudaError_t launch_mtree_parents(const uint64_t* d, const int* cnt, uint32_t bound, int arity, uint8_t* flag, uint64_t* parent,
                                  cudaStream_t st) {
-    if (bound == 0) return cudaSuccess;
-    k_mtree_parents<<<blocks256(bound), 256, 0, st>>>(d, cnt, bound, log2_arity(arity), flag, parent);
-    return cudaGetLastError();
+    return launch(k_mtree_parents, bound, 256, st, d, cnt, bound, log2_arity(arity), flag, parent);
 }
 
 template <bool kSparse>
-static void mtree_digest(FrArg tag, const uint8_t* b, int arity, uint8_t* o, const uint64_t* d, const int* cnt, size_t bound,
-                         size_t coop_max, cudaStream_t st, const uint8_t* bp, uint8_t* lp) {
-    if (bound <= coop_max) {
-        k_mtree_digest_coop<kSparse><<<coop_grid(bound), kThreads, 0, st>>>(tag, b, (uint32_t)arity, o, d, cnt, bp, lp);
-    } else if (arity == 4) {
-        k_mtree_digest<2, kSparse><<<grid_for(bound), kThreads, 0, st>>>(tag, b, o, d, cnt, bp, lp);
-    } else {
-        k_mtree_digest<1, kSparse><<<grid_for(bound), kThreads, 0, st>>>(tag, b, o, d, cnt, bp, lp);
-    }
+static cudaError_t mtree_digest(FrArg tag, const void* b, int arity, void* o, const uint64_t* d, const int* cnt, size_t bound,
+                                size_t coop_max, cudaStream_t st, const uint8_t* bp, uint8_t* lp) {
+    if (bound <= coop_max)
+        return launch_grid(k_mtree_digest_coop<kSparse>, coop_grid(bound), kThreads, st, tag, b, (uint32_t)arity, o, d, cnt, bp, lp);
+    if (arity == 4) return launch(k_mtree_digest<2, kSparse>, bound, kThreads, st, tag, b, o, d, cnt, bp, lp);
+    return launch(k_mtree_digest<1, kSparse>, bound, kThreads, st, tag, b, o, d, cnt, bp, lp);
 }
 
 cudaError_t launch_mtree_digest(const uint64_t tag[4], const void* below, int arity, void* level, const uint64_t* d,
                                 const int* cnt, size_t bound, size_t coop_max, cudaStream_t st, const uint8_t* below_present,
                                 uint8_t* level_present) {
-    if (bound == 0) return cudaSuccess;
-    const uint8_t* b = static_cast<const uint8_t*>(below);
-    uint8_t* o = static_cast<uint8_t*>(level);
     if (below_present)
-        mtree_digest<true>(to_arg(tag), b, arity, o, d, cnt, bound, coop_max, st, below_present, level_present);
-    else
-        mtree_digest<false>(to_arg(tag), b, arity, o, d, cnt, bound, coop_max, st, nullptr, nullptr);
-    return cudaGetLastError();
+        return mtree_digest<true>(to_arg(tag), below, arity, level, d, cnt, bound, coop_max, st, below_present, level_present);
+    return mtree_digest<false>(to_arg(tag), below, arity, level, d, cnt, bound, coop_max, st, nullptr, nullptr);
 }
 
 cudaError_t launch_smtree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t capacity, uint64_t* keys,
                                uint32_t* bpos, unsigned long long* rejected, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_smtree_keys<<<blocks256(n), 256, 0, st>>>(pos, op, n, capacity, keys, bpos, rejected);
-    return cudaGetLastError();
+    return launch(k_smtree_keys, n, 256, st, pos, op, n, capacity, keys, bpos, rejected);
 }
 
 cudaError_t launch_smtree_leaf_write(const uint64_t* keys, const uint32_t* bpos, uint32_t n, uint64_t sentinel, int arity,
                                      const uint8_t* op, const void* values, void* leaves, uint8_t* present, uint8_t* flag,
                                      uint64_t* parent, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_smtree_leaf_write<<<blocks256(n), 256, 0, st>>>(keys, bpos, n, sentinel, log2_arity(arity), op,
-                                                         static_cast<const uint8_t*>(values), static_cast<uint8_t*>(leaves),
-                                                         present, flag, parent);
-    return cudaGetLastError();
+    return launch(k_smtree_leaf_write, n, 256, st, keys, bpos, n, sentinel, log2_arity(arity), op, values, leaves, present, flag,
+                  parent);
 }
 
 cudaError_t launch_smtree_seed(uint8_t* present, void* leaves, uint64_t groups, uint64_t capacity, int arity, uint8_t* flag,
                                uint64_t* parent, cudaStream_t st) {
-    if (groups == 0) return cudaSuccess;
-    k_smtree_seed<<<blocks256(groups), 256, 0, st>>>(present, static_cast<uint8_t*>(leaves), groups, capacity, log2_arity(arity),
-                                                     flag, parent);
-    return cudaGetLastError();
+    return launch(k_smtree_seed, groups, 256, st, present, leaves, groups, capacity, log2_arity(arity), flag, parent);
 }
 
 cudaError_t launch_smtree_count(const uint8_t* present, uint64_t n, unsigned long long* out, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_smtree_count<<<n < 4096 * 256 ? blocks256(n) : 4096u, 256, 0, st>>>(present, n, out);
-    return cudaGetLastError();
+    const unsigned grid = n < 4096 * 256 ? (unsigned)((n + 255) / 256) : 4096u;   // at most 4096 blocks: grid-stride
+    return launch_grid(k_smtree_count, grid, 256, st, present, n, out);
 }
 
 cudaError_t launch_ctree_keys(const uint64_t* pos, const uint8_t* op, uint32_t n, uint64_t max_pos, uint64_t* keys, uint32_t* bpos,
                               unsigned long long* rejected, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_ctree_keys<<<blocks256(n), 256, 0, st>>>(pos, op, n, max_pos, keys, bpos, rejected);
-    return cudaGetLastError();
+    return launch(k_ctree_keys, n, 256, st, pos, op, n, max_pos, keys, bpos, rejected);
 }
 
 cudaError_t launch_ctree_valid(const uint32_t* bpos, uint32_t n, uint8_t* flag, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_ctree_valid<<<blocks256(n), 256, 0, st>>>(bpos, n, flag);
-    return cudaGetLastError();
+    return launch(k_ctree_valid, n, 256, st, bpos, n, flag);
 }
 
 cudaError_t launch_ctree_last(const uint64_t* keys, const int* cnt, uint32_t n, uint8_t* flag, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_ctree_last<<<blocks256(n), 256, 0, st>>>(keys, cnt, n, flag);
-    return cudaGetLastError();
+    return launch(k_ctree_last, n, 256, st, keys, cnt, n, flag);
 }
 
 cudaError_t launch_ctree_leaf_changes(const uint32_t* bpos, const int* cnt, uint32_t n, const uint8_t* op, const void* values,
                                       void* cval, uint8_t* cpres, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_ctree_leaf_changes<<<blocks256(n), 256, 0, st>>>(bpos, cnt, n, op, static_cast<const uint8_t*>(values),
-                                                      static_cast<uint8_t*>(cval), cpres);
-    return cudaGetLastError();
+    return launch(k_ctree_leaf_changes, n, 256, st, bpos, cnt, n, op, values, cval, cpres);
 }
 
 cudaError_t launch_ctree_mark(const uint64_t* lkeys, const uint64_t* lcount, uint64_t s, const uint64_t* ckeys, const int* ccnt,
                               uint32_t nb, const uint8_t* cpres, uint32_t* kept, uint32_t* ins, cudaStream_t st) {
-    k_ctree_mark<<<blocks256(s > nb ? s : nb), 256, 0, st>>>(lkeys, lcount, s, ckeys, ccnt, nb, cpres, kept, ins);
-    return cudaGetLastError();
+    return launch(k_ctree_mark, s > nb ? s : nb, 256, st, lkeys, lcount, s, ckeys, ccnt, nb, cpres, kept, ins);
 }
 
 cudaError_t launch_ctree_scatter(const uint64_t* lkeys, const void* lvals, const uint64_t* lcount, uint64_t s,
                                  const uint64_t* ckeys, const void* cvals, const int* ccnt, uint32_t nb, const uint32_t* kept,
                                  const uint32_t* K, const uint32_t* ins, const uint32_t* I, uint64_t* okeys, void* ovals,
                                  cudaStream_t st) {
-    k_ctree_scatter<<<blocks256(s > nb ? s : nb), 256, 0, st>>>(lkeys, static_cast<const uint8_t*>(lvals), lcount, s, ckeys,
-                                                               static_cast<const uint8_t*>(cvals), ccnt, nb, kept, K, ins, I,
-                                                               okeys, static_cast<uint8_t*>(ovals));
-    return cudaGetLastError();
+    return launch(k_ctree_scatter, s > nb ? s : nb, 256, st, lkeys, lvals, lcount, s, ckeys, cvals, ccnt, nb, kept, K, ins, I,
+                  okeys, ovals);
 }
 
 cudaError_t launch_ctree_count(const uint64_t* lcount, uint64_t s, uint32_t nb, const uint32_t* kept, const uint32_t* K,
                                const uint32_t* ins, const uint32_t* I, bool level0, uint32_t n, uint64_t* stats, uint32_t* ok,
                                unsigned long long* rejected, cudaStream_t st) {
-    k_ctree_count<<<1, 1, 0, st>>>(lcount, s, nb, kept, K, ins, I, level0, n, stats, ok, rejected);
-    return cudaGetLastError();
+    return launch_grid(k_ctree_count, 1, 1, st, lcount, s, nb, kept, K, ins, I, level0, n, stats, ok, rejected);
 }
 
 cudaError_t launch_ctree_commit(const uint64_t* okeys, const void* ovals, uint64_t s, const uint64_t* stats, const uint32_t* ok,
                                 uint64_t* lkeys, void* lvals, uint64_t* lcount, cudaStream_t st) {
-    k_ctree_commit<<<blocks256(s), 256, 0, st>>>(okeys, static_cast<const uint8_t*>(ovals), s, stats, ok, lkeys,
-                                                 static_cast<uint8_t*>(lvals), lcount);
-    return cudaGetLastError();
+    return launch(k_ctree_commit, s, 256, st, okeys, ovals, s, stats, ok, lkeys, lvals, lcount);
 }
 
 cudaError_t launch_ctree_gather(const uint64_t* okeys, const void* ovals, const uint64_t* stats, uint64_t s, const uint64_t* pkeys,
                                 const int* pcnt, uint32_t nb, int arity, void* groups, uint8_t* gpres, cudaStream_t st) {
-    k_ctree_gather<<<blocks256(nb), 256, 0, st>>>(okeys, static_cast<const uint8_t*>(ovals), stats, s, pkeys, pcnt, nb,
-                                                  log2_arity(arity), static_cast<uint8_t*>(groups), gpres);
-    return cudaGetLastError();
+    return launch(k_ctree_gather, nb, 256, st, okeys, ovals, stats, s, pkeys, pcnt, nb, log2_arity(arity), groups, gpres);
 }
 
 cudaError_t launch_ctree_iota(uint64_t* d, uint32_t n, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_ctree_iota<<<blocks256(n), 256, 0, st>>>(d, n);
-    return cudaGetLastError();
+    return launch(k_ctree_iota, n, 256, st, d, n);
 }
 
 cudaError_t launch_ctree_open(const uint64_t* keys, const void* values, const uint64_t* count, const uint64_t* pos, size_t n,
                               int arity, uint32_t depth, const OpenLevels& lv, void* paths, cudaStream_t st) {
-    if (n == 0 || depth == 0) return cudaSuccess;
-    k_ctree_open<<<blocks256(n * depth), 256, 0, st>>>(keys, static_cast<const uint8_t*>(values), count, pos, n, log2_arity(arity),
-                                                       depth, lv, static_cast<uint8_t*>(paths));
-    return cudaGetLastError();
+    return launch(k_ctree_open, n * depth, 256, st, keys, values, count, pos, n, log2_arity(arity), depth, lv, paths);
 }
 
 cudaError_t launch_merkle_verify(const uint64_t tag[4], const uint64_t root[4], const void* leaf_items,
                                  const uint64_t* leaf_idx, const void* paths, size_t n, int arity, uint32_t depth,
                                  uint8_t* ok, unsigned long long* n_failed, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
     if (arity == 4)
-        k_merkle_verify<2><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), to_arg(root), static_cast<const uint8_t*>(leaf_items),
-                                                             leaf_idx, static_cast<const uint8_t*>(paths), n, depth, ok, n_failed);
-    else
-        k_merkle_verify<1><<<grid_for(n), kThreads, 0, st>>>(to_arg(tag), to_arg(root), static_cast<const uint8_t*>(leaf_items),
-                                                             leaf_idx, static_cast<const uint8_t*>(paths), n, depth, ok, n_failed);
-    return cudaGetLastError();
+        return launch(k_merkle_verify<2>, n, kThreads, st, to_arg(tag), to_arg(root), leaf_items, leaf_idx, paths, n, depth, ok,
+                      n_failed);
+    return launch(k_merkle_verify<1>, n, kThreads, st, to_arg(tag), to_arg(root), leaf_items, leaf_idx, paths, n, depth, ok,
+                  n_failed);
 }
 
 cudaError_t launch_varlen_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars, uint32_t max_len,
                                uint32_t fixed_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_varlen_keys<0><<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
-    return cudaGetLastError();
+    return launch(k_varlen_keys<0>, n, 256, st, offsets, n, base, n_scalars, max_len, fixed_len, keys, vals, rejected);
 }
 
 cudaError_t launch_crypt_varlen_keys(bool decrypt, const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_scalars,
                                      uint32_t max_len, uint32_t* keys, uint32_t* vals, unsigned long long* rejected,
                                      cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    if (decrypt)
-        k_varlen_keys<2><<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
-    else
-        k_varlen_keys<1><<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
-    return cudaGetLastError();
+    if (decrypt) return launch(k_varlen_keys<2>, n, 256, st, offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
+    return launch(k_varlen_keys<1>, n, 256, st, offsets, n, base, n_scalars, max_len, 0, keys, vals, rejected);
 }
 
 cudaError_t launch_crypt_varlen(bool decrypt, const void* tags, const void* src, uint64_t base, const uint64_t* offsets,
                                 const uint32_t* lens, const uint32_t* perm, uint32_t n, const void* secret_uv, const void* nonce,
                                 void* dst, uint8_t* ok, unsigned long long* n_failed, size_t coop_max, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    const uint8_t* t = static_cast<const uint8_t*>(tags);
-    const uint8_t* s = static_cast<const uint8_t*>(src);
-    const uint8_t* uv = static_cast<const uint8_t*>(secret_uv);
-    const uint8_t* no = static_cast<const uint8_t*>(nonce);
-    uint8_t* d = static_cast<uint8_t*>(dst);
     if (n <= coop_max) {
-        const unsigned grid = coop_grid(n);
         if (decrypt)
-            k_crypt_varlen_coop<true><<<grid, kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, ok, n_failed);
-        else
-            k_crypt_varlen_coop<false><<<grid, kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, nullptr, nullptr);
-    } else if (decrypt) {
-        k_crypt_varlen<true><<<grid_for(n), kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, ok, n_failed);
-    } else {
-        k_crypt_varlen<false><<<grid_for(n), kThreads, 0, st>>>(t, s, base, offsets, lens, perm, n, uv, no, d, nullptr, nullptr);
+            return launch_grid(k_crypt_varlen_coop<true>, coop_grid(n), kThreads, st, tags, src, base, offsets, lens, perm, n,
+                               secret_uv, nonce, dst, ok, n_failed);
+        return launch_grid(k_crypt_varlen_coop<false>, coop_grid(n), kThreads, st, tags, src, base, offsets, lens, perm, n,
+                           secret_uv, nonce, dst, nullptr, nullptr);
     }
-    return cudaGetLastError();
+    if (decrypt)
+        return launch(k_crypt_varlen<true>, n, kThreads, st, tags, src, base, offsets, lens, perm, n, secret_uv, nonce, dst, ok,
+                      n_failed);
+    return launch(k_crypt_varlen<false>, n, kThreads, st, tags, src, base, offsets, lens, perm, n, secret_uv, nonce, dst, nullptr,
+                  nullptr);
 }
 
 cudaError_t launch_digest_varlen(const void* tags, const void* in, uint64_t base, const uint64_t* offsets, const uint32_t* lens,
                                  const uint32_t* perm, uint32_t n, void* out, uint32_t out_len, size_t coop_max, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    const uint8_t* t = static_cast<const uint8_t*>(tags);
-    const uint8_t* i = static_cast<const uint8_t*>(in);
-    uint8_t* o = static_cast<uint8_t*>(out);
-    if (n <= coop_max) {
-        k_sponge_digest_varlen_coop<<<coop_grid(n), kThreads, 0, st>>>(t, i, base, offsets, lens, perm, n, o, out_len);
-    } else {
-        k_sponge_digest_varlen<<<grid_for(n), kThreads, 0, st>>>(t, i, base, offsets, lens, perm, n, o, out_len);
-    }
-    return cudaGetLastError();
+    if (n <= coop_max)
+        return launch_grid(k_sponge_digest_varlen_coop, coop_grid(n), kThreads, st, tags, in, base, offsets, lens, perm, n, out,
+                           out_len);
+    return launch(k_sponge_digest_varlen, n, kThreads, st, tags, in, base, offsets, lens, perm, n, out, out_len);
 }
 
 // ---- BlsScalar::hash_to_scalar on the device (p252_hash_to_scalar_batch, p252_scalars_from_bytes_wide) -------------
@@ -3876,27 +3586,17 @@ __global__ void __launch_bounds__(256) k_from_bytes_wide(const uint8_t* __restri
 cudaError_t launch_hash_to_scalar(const void* bytes, uint64_t base, uint64_t n_bytes, const uint64_t* offsets,
                                   const uint32_t* perm, uint32_t n, uint32_t max_len, void* out, unsigned long long* rejected,
                                   cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    const uint8_t* b = static_cast<const uint8_t*>(bytes);
-    uint8_t* o = static_cast<uint8_t*>(out);
-    if (perm)
-        k_hash_to_scalar<true><<<blocks256(n), 256, 0, st>>>(b, base, n_bytes, offsets, perm, n, max_len, o, rejected);
-    else
-        k_hash_to_scalar<false><<<blocks256(n), 256, 0, st>>>(b, base, n_bytes, offsets, nullptr, n, max_len, o, rejected);
-    return cudaGetLastError();
+    if (perm) return launch(k_hash_to_scalar<true>, n, 256, st, bytes, base, n_bytes, offsets, perm, n, max_len, out, rejected);
+    return launch(k_hash_to_scalar<false>, n, 256, st, bytes, base, n_bytes, offsets, nullptr, n, max_len, out, rejected);
 }
 
 cudaError_t launch_hash_to_scalar_keys(const uint64_t* offsets, uint32_t n, uint64_t base, uint64_t n_bytes, uint32_t max_len,
                                        uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_hash_to_scalar_keys<<<blocks256(n), 256, 0, st>>>(offsets, n, base, n_bytes, max_len, keys, vals, rejected);
-    return cudaGetLastError();
+    return launch(k_hash_to_scalar_keys, n, 256, st, offsets, n, base, n_bytes, max_len, keys, vals, rejected);
 }
 
 cudaError_t launch_from_bytes_wide(const void* in, size_t n, void* out, cudaStream_t st) {
-    if (n == 0) return cudaSuccess;
-    k_from_bytes_wide<<<blocks256(n), 256, 0, st>>>(static_cast<const uint8_t*>(in), n, static_cast<uint8_t*>(out));
-    return cudaGetLastError();
+    return launch(k_from_bytes_wide, n, 256, st, in, n, out);
 }
 
 uint32_t wide_mul_per_permutation() { return (uint32_t)kWideMulPerPerm; }
