@@ -169,6 +169,11 @@ pub use elgamal::SenderEncryption;
 mod hash_to_scalar;
 pub use hash_to_scalar::HASH_TO_SCALAR_MAX_LEN;
 
+// Mixed digest batches (items of any domains, input and output lengths, finalized or truncated): their own `extern "C"`
+// block in hash_mixed.rs (a method on Engine).
+mod hash_mixed;
+pub use hash_mixed::{MixedItem, MIXED_TRUNCATED};
+
 /// Engine failures that have no dusk_poseidon::Error counterpart.
 #[derive(Debug)]
 pub enum BatchError {

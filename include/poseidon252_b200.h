@@ -186,6 +186,38 @@ int p252_hash_batch_truncated(p252_ctx* ctx, int domain, const p252_fr* in, size
 int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t n_scalars, const uint64_t* offsets, size_t n,
                            size_t max_len, p252_fr* out, size_t out_len, size_t* n_rejected, int flags);
 
+/* Mixed digest batch: every Hash the reference can build, one call for items of different domains, input and output
+ * lengths, finalized or truncated.  Item i is Hash::new(mode[i] & 3), update(in[offsets[i] .. offsets[i+1])),
+ * output_len(out_len_i), then finalize() -- or, with mode[i] & P252_MIXED_TRUNCATED, finalize_truncated(), whose
+ * rows are the raw limbs masked to 250 bits as in p252_hash_batch_truncated (src/hash.rs:128-183).  The chunk layout
+ * of update() never changes a digest (consecutive absorbs aggregate into one tag word), so the concatenated input
+ * describes the item.
+ *   mode: n bytes, mode[i] & 3 the item's p252_domain; in: n_scalars scalars; offsets, out_offsets: n + 1 entries each;
+ *   out: n_out rows, item i writes the rows out[out_offsets[i] .. out_offsets[i+1]), so out_len_i = out_offsets[i+1] -
+ *   out_offsets[i].  mode, offsets and out_offsets live in the same memory space as in / out; offsets[0] and
+ *   out_offsets[0] need not be 0.
+ *   Batch checks, before anything runs, all INVALID_ARGUMENT: a NULL buffer the call needs, n >= 2^31, max_len or
+ *   max_out_len == 0 or > P252_VARLEN_MAX_LEN, DEVICE in / out not 16-byte or offsets / out_offsets not 8-byte aligned.
+ *   Item checks, in this order: a mode bit outside 0x83 -> INVALID_ARGUMENT; an input range that decreases or lies
+ *   outside [0, n_scalars] -> INVALID_ARGUMENT; an output range that decreases or lies outside [0, n_out] ->
+ *   INVALID_ARGUMENT; a Merkle domain with len_i != arity or out_len_i != 1 -> IO_PATTERN_VIOLATION; len_i == 0 or
+ *   out_len_i == 0 -> INVALID_IO_PATTERN; len_i > max_len or out_len_i > max_out_len -> INVALID_ARGUMENT.  Apart from
+ *   the mode bits these are the rules of p252_hash_tag; a non-Merkle domain with out_len_i > 1 is accepted (the
+ *   reference's output_len() rule is applied by the front ends).
+ *   HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written.
+ *   DEVICE: descriptors are not inspected on the host; an invalid item is counted into *n_rejected (optional HOST
+ *   pointer, 0 for HOST calls; lifetime as for p252_mtree_update) and gets zero rows where its output range is valid,
+ *   nothing otherwise.  No descriptor value makes a kernel read outside in or write outside out; where the valid
+ *   output ranges of a non-monotone out_offsets overlap, the rows are unspecified.  With P252_ASYNC nothing is
+ *   synchronised.  n == 0 runs nothing.
+ * Each item's tag (hash_to_scalar of its 16-byte tag input, one BLAKE2b block) is derived on the device; items are
+ * sorted on the device by step count ceil(len / 4) + ceil(out_len / 4), so that a warp hashes items of (nearly) equal
+ * work. */
+#define P252_MIXED_TRUNCATED 0x80
+int p252_hash_batch_mixed(p252_ctx* ctx, const uint8_t* mode, const p252_fr* in, size_t n_scalars,
+                          const uint64_t* offsets, size_t n, size_t max_len, p252_fr* out, size_t n_out,
+                          const uint64_t* out_offsets, size_t max_out_len, size_t* n_rejected, int flags);
+
 /* Wire format (BlsScalar::from_bytes / to_bytes as used at src/hades.rs:94-105,131): n canonical 32-byte
  * little-endian integers <-> BlsScalar.0.  from_bytes: ok[i] = 0 and out[i] = 0 when the value is >= p (the
  * reference returns None); ok may be NULL. */

@@ -7,8 +7,8 @@
 //   dusk_poseidon::Hash{new,output_len,update,finalize,digest}   (src/hash.rs:92-195)  -> p252::Hash
 //   dusk_poseidon::{encrypt, decrypt}        (src/encryption.rs:62-95) -> p252::encrypt / p252::decrypt
 //   dusk_poseidon::Error                     (src/error.rs:11-32)      -> p252::Error (exception)
-//   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, hades::permute_batch, encrypt_batch,
-//   decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
+//   NEW batch entries: Hash::digest_batch, Hash::digest_batch_varlen, Hash::finalize_batch, hades::permute_batch,
+//   encrypt_batch, decrypt_batch, encrypt_batch_varlen, decrypt_batch_varlen, dhke / dhke_batch, encrypt_batch_dhke,
 //   decrypt_batch_dhke, fixed_base / fixed_base_batch, encrypt_batch_ephemeral, stealth_address /
 //   stealth_address_batch, owns / stealth_owns_batch, schnorr_sign / schnorr_sign_batch, schnorr_verify /
 //   schnorr_verify_batch, nullifier / nullifier_batch, schnorr_sign_double / schnorr_sign_double_batch,
@@ -165,6 +165,50 @@ public:
               e.get());
         std::vector<std::vector<Scalar>> res(inputs.size());
         for (size_t i = 0; i < res.size(); ++i) res[i].assign(out.begin() + i * ol, out.begin() + (i + 1) * ol);
+        return res;
+    }
+
+    // NEW: hashes[i].finalize(), or hashes[i].finalize_truncated() where truncated[i] (empty: none truncated), for
+    // hashes of any domains, update() chunks and output lengths, one device call (p252_hash_batch_mixed).  A truncated
+    // item's rows are the raw limbs masked to 250 bits (JubJubScalar::from_raw's input).  Throws the Error
+    // Hash::finalize throws for the lowest-index invalid hash before anything runs.
+    static std::vector<std::vector<Scalar>> finalize_batch(const std::vector<Hash>& hashes,
+                                                           const std::vector<bool>& truncated = {}, Engine* e = nullptr) {
+        if (!truncated.empty() && truncated.size() != hashes.size())
+            throw Error(P252_ERR_INVALID_ARGUMENT, "truncated must be empty or hold one flag per hash");
+        std::vector<uint8_t> mode;
+        std::vector<Scalar> data;
+        std::vector<uint64_t> offsets{0}, out_offsets{0};
+        size_t longest = 1, longest_out = 1;
+        for (size_t i = 0; i < hashes.size(); ++i) {
+            const Hash& h = hashes[i];
+            size_t total = 0;
+            bool empty_chunk = h.chunks_.empty();
+            for (auto& c : h.chunks_) {
+                data.insert(data.end(), c.ptr, c.ptr + c.len);
+                total += c.len;
+                empty_chunk = empty_chunk || c.len == 0;
+            }
+            if ((h.domain_ == Domain::Merkle2 && (total != 2 || h.output_len_ != 1)) ||
+                (h.domain_ == Domain::Merkle4 && (total != 4 || h.output_len_ != 1)))
+                throw Error(P252_ERR_IO_PATTERN_VIOLATION, p252_strerror(P252_ERR_IO_PATTERN_VIOLATION));
+            if (empty_chunk) throw Error(P252_ERR_INVALID_IO_PATTERN, p252_strerror(P252_ERR_INVALID_IO_PATTERN));
+            const bool trunc = !truncated.empty() && truncated[i];
+            mode.push_back(static_cast<uint8_t>(static_cast<int>(h.domain_) | (trunc ? P252_MIXED_TRUNCATED : 0)));
+            offsets.push_back(data.size());
+            out_offsets.push_back(out_offsets.back() + h.output_len_);
+            longest = std::max(longest, total);
+            longest_out = std::max(longest_out, h.output_len_);
+        }
+        std::vector<Scalar> out(out_offsets.back());
+        Engine& eng = e ? *e : Engine::default_engine();
+        check(p252_hash_batch_mixed(eng.get(), mode.data(), data.data(), data.size(), offsets.data(), hashes.size(),
+                                    longest, out.data(), out.size(), out_offsets.data(), longest_out, nullptr,
+                                    P252_MEM_HOST),
+              eng.get());
+        std::vector<std::vector<Scalar>> res(hashes.size());
+        for (size_t i = 0; i < res.size(); ++i)
+            res[i].assign(out.begin() + out_offsets[i], out.begin() + out_offsets[i + 1]);
         return res;
     }
 

@@ -3,7 +3,9 @@
 Public surface mirrors src/lib.rs:13-31:
     Hash, Domain, Error, HADES_WIDTH, encrypt, decrypt
 plus the batch entry points this engine adds:
-    Hash.digest_batch, Hash.digest_batch_varlen (inputs of different lengths in one call), hash_to_scalar_batch
+    Hash.digest_batch, Hash.digest_batch_varlen (inputs of different lengths in one call), finalize_batch /
+    digest_batch_mixed (Hash.finalize_batch / Hash.digest_batch_mixed: items of different domains, input and output lengths,
+    finalized or truncated, in one call), hash_to_scalar_batch
     (BlsScalar::hash_to_scalar of byte strings of different lengths in one call), hades.permute_batch,
     encrypt_batch, decrypt_batch, encrypt_batch_varlen / decrypt_batch_varlen (messages of different lengths in one call),
     dhke / dhke_batch (JubJub key exchange), encrypt_batch_dhke / decrypt_batch_dhke (shared secret derived on the device),
@@ -35,7 +37,7 @@ from .elgamal import (elgamal_decrypt, elgamal_decrypt_batch, elgamal_encrypt, e
 from .engine import Engine, default_engine
 from .errors import (DecryptionFailed, EncryptionFailed, EngineError, Error, InvalidIOPattern, InvalidPoint,
                      IOPatternViolation, TooFewInputElements)
-from .hash import Domain, Hash, hash_to_scalar_batch, pack_bytes, pack_varlen
+from .hash import Domain, Hash, digest_batch_mixed, finalize_batch, hash_to_scalar_batch, pack_bytes, pack_varlen
 from .merkle import CompactTree, SparseTree, Tree, merkle4_build, merkle4_level
 from .msm import jubjub_msm, schnorr_verify_all, schnorr_verify_double_all
 from .notes import note_create, note_create_batch, note_open, note_open_batch, value_commit, value_commit_batch
@@ -49,7 +51,7 @@ from .wallet import wallet_scan_batch
 HADES_WIDTH = hades.WIDTH
 
 __all__ = ["Hash", "Domain", "Error", "HADES_WIDTH", "encrypt", "decrypt", "encrypt_batch", "decrypt_batch", "pack_varlen",
-           "hash_to_scalar_batch", "pack_bytes",
+           "hash_to_scalar_batch", "pack_bytes", "finalize_batch", "digest_batch_mixed",
            "encrypt_batch_varlen", "decrypt_batch_varlen", "cipher_offsets", "message_offsets",
            "dhke", "dhke_batch", "encrypt_batch_dhke", "decrypt_batch_dhke", "fixed_base", "fixed_base_batch",
            "encrypt_batch_ephemeral", "stealth_address", "stealth_address_batch", "owns", "stealth_owns_batch",

@@ -73,6 +73,8 @@ SIGNATURES = {
     "p252_ctree_open_batch": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_int]),
     "p252_hash_batch_varlen":(c_int, [c_void_p, c_int, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t,
                                        ctypes.POINTER(c_size_t), c_int]),
+    "p252_hash_batch_mixed": (c_int, [c_void_p, c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_size_t,
+                                      c_void_p, c_size_t, ctypes.POINTER(c_size_t), c_int]),
     "p252_encrypt_batch_varlen": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p,
                                           c_void_p, ctypes.POINTER(c_size_t), c_int]),
     "p252_decrypt_batch_varlen": (c_int, [c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_size_t, c_void_p, c_void_p,
@@ -138,6 +140,7 @@ SIGNATURES = {
 
 MEM_HOST, MEM_DEVICE, ASYNC, TIMING, NO_GATHER = 0, 1, 2, 4, 8
 VARLEN_MAX_LEN = 65536   # P252_VARLEN_MAX_LEN
+MIXED_TRUNCATED = 0x80   # P252_MIXED_TRUNCATED, the mode bit of a finalize_truncated() item of p252_hash_batch_mixed
 HASH_TO_SCALAR_MAX_LEN = 1 << 20   # P252_HASH_TO_SCALAR_MAX_LEN, bytes per item
 
 

@@ -2,7 +2,8 @@
 // (io-pattern checks, tag derivation), staging for HOST buffers, kernel launches, fixed-height trees with batched
 // updates (p252_mtree_*), sparse fixed-height trees with inserts and removals at any position (p252_smtree_*),
 // compact sparse trees stored as sorted present nodes per level (p252_ctree_*),
-// variable-length digest batches (p252_hash_batch_varlen), and the multi-GPU arity-4 tree build
+// variable-length digest batches (p252_hash_batch_varlen), mixed digest batches with a domain, input and output length
+// and truncation per item (p252_hash_batch_mixed), and the multi-GPU arity-4 tree build
 // (one process per GPU, NCCL all-gather per level).
 //
 // Mirrors, for the batch path, the reference's public surface (src/lib.rs:13-31):
@@ -3176,12 +3177,17 @@ int crypt_run(p252_ctx* ctx, bool decrypt, const p252_fr* tags, const p252_fr* i
 
 // The chunks of a variable-length HOST batch whose offsets count elements of elem_bytes bytes (scalars, or bytes):
 // consecutive item ranges of about kChunkBytesTarget input bytes (a longer item is a chunk by itself), at most
-// chunk_items_max() items each; chunk k = items [bounds[k], bounds[k+1]).
-std::vector<size_t> chunk_bounds(const uint64_t* offsets, size_t n, size_t elem_bytes) {
+// chunk_items_max() items each; chunk k = items [bounds[k], bounds[k+1]).  out_offsets (optional, output rows of 32
+// bytes): a chunk also stays within about kChunkBytesTarget output bytes.
+std::vector<size_t> chunk_bounds(const uint64_t* offsets, size_t n, size_t elem_bytes,
+                                 const uint64_t* out_offsets = nullptr) {
     std::vector<size_t> bounds = {0};
     for (size_t lo = 0, hi = 0; lo < n; lo = hi) {
         hi = lo + 1;
-        while (hi < n && hi - lo < chunk_items_max() && (offsets[hi + 1] - offsets[lo]) * elem_bytes <= kChunkBytesTarget) ++hi;
+        while (hi < n && hi - lo < chunk_items_max() &&
+               (offsets[hi + 1] - offsets[lo]) * elem_bytes <= kChunkBytesTarget &&
+               (!out_offsets || (out_offsets[hi + 1] - out_offsets[lo]) * sizeof(p252_fr) <= kChunkBytesTarget))
+            ++hi;
         bounds.push_back(hi);
     }
     return bounds;
@@ -3308,6 +3314,125 @@ int p252_hash_batch_varlen(p252_ctx* ctx, int domain, const p252_fr* in, size_t 
     if (n == 0) return P252_OK;
     if ((rc = varlen_tags(ctx, domain, max_len, out_len, &tags)) != P252_OK) return rc;
     return varlen_host(ctx, tags, in, offsets, n, (uint32_t)max_len, fixed_len, out, (uint32_t)out_len);
+}
+
+}  // extern "C"
+
+// ---- mixed digest batches (p252_hash_batch_mixed) --------------------------------------------------------------------
+namespace {
+
+// One mixed batch on `st`: keys (step count or 0 = rejected) with the tags derived on the device -> radix sort by step
+// count -> the mixed digest kernel.  in / out hold n_scalars / n_out rows, addressed by offsets - base and
+// out_offsets - obase.
+int mixed_run(p252_ctx* ctx, const uint8_t* mode, const p252_fr* in, uint64_t base, uint64_t n_scalars, const uint64_t* offsets,
+              const uint64_t* out_offsets, uint64_t obase, uint64_t n_out, uint32_t n, uint32_t max_len, uint32_t max_out_len,
+              p252_fr* out, unsigned long long* rejected, cudaStream_t st) {
+    const uint32_t max_steps = (max_len + 3) / 4 + (max_out_len + 3) / 4;
+    p252_fr* tags = nullptr;
+    uint2* desc = nullptr;
+    auto layout = [&](Carve& c) {
+        tags = c.take<p252_fr>(n);
+        desc = c.take<uint2>(n);
+    };
+    return with_scratch(ctx, st, layout, [&]() -> int {
+        return varlen_sorted(
+            ctx, n, max_steps, st,
+            [&](uint32_t* keys, uint32_t* vals) {
+                return p252::launch_mixed_keys(mode, offsets, base, n_scalars, out_offsets, obase, n_out, n, max_len, max_out_len,
+                                               out, keys, vals, tags, desc, rejected, st);
+            },
+            [&](const uint32_t*, const uint32_t* perm) {
+                return p252::launch_digest_mixed(tags, desc, in, base, offsets, obase, out_offsets, perm, n, out, ctx->coop_max,
+                                                 st);
+            });
+    });
+}
+
+// HOST batch (already validated, so both offset arrays are non-decreasing): as varlen_host, with chunks bounded by input
+// and output bytes; each chunk stages its modes, both offset slices and its input rows, and copies back its output rows.
+int mixed_host(p252_ctx* ctx, const uint8_t* mode, const p252_fr* in, const uint64_t* offsets, const uint64_t* out_offsets,
+               size_t n, uint32_t max_len, uint32_t max_out_len, p252_fr* out) {
+    const std::vector<size_t> bounds = chunk_bounds(offsets, n, sizeof(p252_fr), out_offsets);
+    return on_slots(ctx, false, [&](long long fail_at) -> int {
+        for (size_t k = 0; k + 1 < bounds.size(); ++k) {
+            const size_t lo = bounds[k], hi = bounds[k + 1], cnt = hi - lo;
+            const uint64_t s0 = offsets[lo], ns = offsets[hi] - s0, o0 = out_offsets[lo], no = out_offsets[hi] - o0;
+            cudaStream_t st = ctx->slots[k % kSlots].stream;
+            p252_fr *d_in = nullptr, *d_out = nullptr;
+            uint64_t *d_off = nullptr, *d_ooff = nullptr;
+            uint8_t* d_mode = nullptr;
+            auto layout = [&](Carve& c) {
+                d_in = c.take<p252_fr>(ns);
+                d_off = c.take<uint64_t>(cnt + 1);
+                d_ooff = c.take<uint64_t>(cnt + 1);
+                d_mode = c.take<uint8_t>(cnt);
+                d_out = c.take<p252_fr>(no);
+            };
+            const int rc = with_scratch(ctx, st, layout, [&]() -> int {
+                CU(cudaMemcpyAsync(d_in, in + s0, ns * sizeof(p252_fr), cudaMemcpyHostToDevice, st));
+                CU(cudaMemcpyAsync(d_off, offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
+                CU(cudaMemcpyAsync(d_ooff, out_offsets + lo, (cnt + 1) * 8, cudaMemcpyHostToDevice, st));
+                CU(cudaMemcpyAsync(d_mode, mode + lo, cnt, cudaMemcpyHostToDevice, st));
+                if ((long long)k == fail_at) return injected_fault(ctx);
+                const int r = mixed_run(ctx, d_mode, d_in, s0, ns, d_off, d_ooff, o0, no, (uint32_t)cnt, max_len, max_out_len,
+                                        d_out, nullptr, st);
+                if (r != P252_OK) return r;
+                CU(cudaMemcpyAsync(out + o0, d_out, no * sizeof(p252_fr), cudaMemcpyDeviceToHost, st));
+                return P252_OK;
+            });
+            if (rc != P252_OK) return rc;
+        }
+        return P252_OK;
+    });
+}
+
+// The status of item i of a HOST mixed batch, in the order of the header's item checks
+int mixed_item_status(const uint8_t* mode, const uint64_t* offsets, const uint64_t* out_offsets, size_t i, size_t n_scalars,
+                      size_t n_out, size_t max_len, size_t max_out_len) {
+    const uint64_t a = offsets[i], b = offsets[i + 1], oa = out_offsets[i], ob = out_offsets[i + 1];
+    if (mode[i] & ~(P252_MIXED_TRUNCATED | 3)) return P252_ERR_INVALID_ARGUMENT;   // domain bits and truncation only
+    if (a > b || b > n_scalars) return P252_ERR_INVALID_ARGUMENT;
+    if (oa > ob || ob > n_out) return P252_ERR_INVALID_ARGUMENT;
+    const int domain = mode[i] & 3;
+    const uint64_t arity = domain == P252_DOMAIN_MERKLE4 ? 4 : (domain == P252_DOMAIN_MERKLE2 ? 2 : 0);
+    if (arity && (b - a != arity || ob - oa != 1)) return P252_ERR_IO_PATTERN_VIOLATION;
+    if (b == a || ob == oa) return P252_ERR_INVALID_IO_PATTERN;
+    if (b - a > max_len || ob - oa > max_out_len) return P252_ERR_INVALID_ARGUMENT;
+    return P252_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int p252_hash_batch_mixed(p252_ctx* ctx, const uint8_t* mode, const p252_fr* in, size_t n_scalars, const uint64_t* offsets,
+                          size_t n, size_t max_len, p252_fr* out, size_t n_out, const uint64_t* out_offsets, size_t max_out_len,
+                          size_t* n_rejected, int flags) {
+    if (!ctx || (!in && n_scalars) || (!out && n_out) || ((!mode || !offsets || !out_offsets || !out) && n))
+        return P252_ERR_INVALID_ARGUMENT;
+    if (n >= 0x80000000ull || max_len == 0 || max_len > P252_VARLEN_MAX_LEN || max_out_len == 0 ||
+        max_out_len > P252_VARLEN_MAX_LEN)
+        return P252_ERR_INVALID_ARGUMENT;
+    P252_LOCK(ctx);
+    DeviceGuard g(ctx->device);
+    if (n_rejected) *n_rejected = 0;
+    int rc;
+    if (flags & P252_MEM_DEVICE) {
+        if (!aligned16(in) || !aligned16(out) || (reinterpret_cast<uintptr_t>(offsets) & 7) ||
+            (reinterpret_cast<uintptr_t>(out_offsets) & 7))
+            return P252_ERR_INVALID_ARGUMENT;
+        if (n == 0) return P252_OK;
+        if (n_rejected && (rc = counter_begin(ctx)) != P252_OK) return rc;
+        rc = mixed_run(ctx, mode, in, 0, n_scalars, offsets, out_offsets, 0, n_out, (uint32_t)n, (uint32_t)max_len,
+                       (uint32_t)max_out_len, out, n_rejected ? ctx->d_counter : nullptr, ctx->stream);
+        if (rc == P252_OK) rc = counter_end(ctx, n_rejected);
+        return device_done(ctx, rc, flags);
+    }
+    // HOST: the whole batch is checked first; the lowest-index invalid item decides the status and nothing is written
+    for (size_t i = 0; i < n; ++i)
+        if ((rc = mixed_item_status(mode, offsets, out_offsets, i, n_scalars, n_out, max_len, max_out_len)) != P252_OK) return rc;
+    if (n == 0) return P252_OK;
+    return mixed_host(ctx, mode, in, offsets, out_offsets, n, (uint32_t)max_len, (uint32_t)max_out_len, out);
 }
 
 }  // extern "C"

@@ -4,7 +4,8 @@
 // covers whole 128-byte item chunks), per-thread 2 x 128-bit per scalar for encrypt/decrypt.
 //
 // Sponge schedule = dusk-safe 0.3 `Sponge` as driven by the reference:
-//   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest (k_sponge_digest_varlen: inputs of any lengths)
+//   Hash::finalize   src/hash.rs:128-155      -> k_sponge_digest (k_sponge_digest_varlen: inputs of any lengths;
+//     k_mixed_keys, k_sponge_digest_mixed: items of any domains, lengths and truncation, tags derived on the device)
 //   encrypt/decrypt  src/encryption.rs:62-95  -> k_crypt (k_crypt_varlen: messages of any lengths)
 //   Safe::permute    src/hades/permutation/scalar.rs:25-27 -> k_permute
 //   dhke             src/encryption.rs:11-43  -> k_dhke (JubJub scalar multiplication, jubjub_device.cuh)
@@ -1009,39 +1010,22 @@ __global__ void __launch_bounds__(256) k_varlen_keys(const uint64_t* __restrict_
     if (rejected) warp_count(rejected, !ok);
 }
 
-// k_sponge_digest_varlen: k_sponge_digest over the items sorted by length.  Warp item k is item i = perm[k] with
-// len = lens[k]; every lane carries its own tag, step count and last-chunk width, input chunks go through the warp tile
-// with a per-item base address (shuffled, as in k_mtree_digest), outputs are stored per item.  The loop runs to the
-// warp's largest step count; a lane past its own last step neither absorbs nor permutes.  Rejected items (len 0, sorted
-// to the front) write zero rows.  Warps take the sorted segments from the end, so the longest items start first.
-// 4 resident blocks per SM (128 registers): the per-lane sponge bookkeeping does not fit kMinBlocks' 96 without spills.
-__global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint8_t* __restrict__ tags,
-                                                                      const uint8_t* __restrict__ in, uint64_t base,
-                                                                      const uint64_t* __restrict__ offsets,
-                                                                      const uint32_t* __restrict__ lens,
-                                                                      const uint32_t* __restrict__ perm, uint32_t n,
-                                                                      uint8_t* __restrict__ out, uint32_t out_len) {
-    __shared__ uint4 stage[kWarps][32][8];
-    P252_STAGE_TABLES
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const uint32_t nseg = (n + 31) / 32;
-    const uint32_t wg = blockIdx.x * kWarps + warp;
-    if (wg >= nseg) return;
-    const uint32_t item0 = (nseg - 1 - wg) * 32;
-    const int nitems = (n - item0 < 32) ? (int)(n - item0) : 32;
-    uint4(*st)[8] = stage[warp];
-    const bool live = lane < nitems;
-    const uint32_t k = item0 + (live ? lane : 0);
-    const uint32_t len = live ? lens[k] : 0u;
-    const uint32_t i = perm[k];
-    const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
-    uint8_t* dst = out + (size_t)i * out_len * 32;
+// The loop of the variable-length digest kernels, one lane per item, shared by k_sponge_digest_varlen (one out_len and a
+// tag table indexed by length) and k_sponge_digest_mixed (kMixed: a tag, out_len, output base and truncation per lane).
+// tag: the lane's tag row; src / dst: its input and output rows; len == 0: a rejected item (out_len zero rows).  The loop
+// runs to the warp's largest step count; a lane past its own last step neither absorbs nor permutes.  kMixed && trunc:
+// every squeezed scalar is stored as k_sponge_digest<true> stores it.  kMixed keeps out_len and trunc in one word, the
+// last squeeze chunk's padding 4 nout - out_len | trunc << 2: a per-lane out_len takes a register the kernel parameter
+// of k_sponge_digest_varlen does not, and a second one for trunc spills under the 128-register bound.
+template <bool kMixed>
+__device__ __forceinline__ void sponge_varlen_lane(uint4 (*st)[8], int lane, bool live, const uint8_t* tag, const uint8_t* src,
+                                                   uint8_t* dst, uint32_t len, uint32_t out_len, bool trunc) {
     const uint32_t nin = (len + 3) / 4, nout = (out_len + 3) / 4;
     const uint32_t steps = len ? nin + nout : 0u;
     const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
+    const uint32_t tail = kMixed ? (4 * nout - out_len) | (trunc ? 4u : 0u) : 0u;
     uint32_t s[5][8];
-    load_fr(s[0], tags + (size_t)len * 32);
+    load_fr(s[0], tag);
 #pragma unroll
     for (int q = 1; q < 5; ++q)
 #pragma unroll
@@ -1053,7 +1037,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint
     for (uint32_t step = 0; step < wsteps; ++step) {
         if (step > 0 && step < steps) {
             uint32_t need = 0x1fu;
-            if (step + 1 == steps) need = last_squeeze_lanes(out_len);
+            if (step + 1 == steps) need = kMixed ? ((1u << (4 - (tail & 3))) - 1u) << 1 : last_squeeze_lanes(out_len);
             hades_permute(s, need P252_TAB_PASS);
         }
         const uint32_t left = step < nin ? len - 4 * step : 0u;
@@ -1086,37 +1070,94 @@ __global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint
         }
         if (step >= nin && step < steps) {
             const uint32_t c = step - nin;
-            const uint32_t oleft = out_len - 4 * c;
+            const uint32_t oleft = kMixed ? 4 * (steps - step) - (tail & 3) : out_len - 4 * c;
 #pragma unroll
-            for (int q = 0; q < 4; ++q)
-                if ((uint32_t)q < oleft) store_fr(dst + (size_t)(4 * c + q) * 32, s[1 + q]);
+            for (int q = 0; q < 4; ++q) {
+                if ((uint32_t)q < oleft) {
+                    if (kMixed && (tail & 4)) {
+                        uint32_t v[8];
+                        fr_to_canonical(v, s[1 + q]);
+                        v[7] &= 0x03ffffffu;               // TRUNCATION_MASK, src/hash.rs:167-172
+                        store_fr(dst + (size_t)(4 * c + q) * 32, v);
+                    } else {
+                        store_fr(dst + (size_t)(4 * c + q) * 32, s[1 + q]);
+                    }
+                }
+            }
         }
     }
 }
 
-// the same for small batches: five threads per item (hades_permute_coop), as k_sponge_digest_coop.  Every thread runs
-// the warp's largest step count (the permutation's shuffles span the warp); a group past its own last step only idles.
-__global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const uint8_t* __restrict__ tags,
-                                                                        const uint8_t* __restrict__ in, uint64_t base,
-                                                                        const uint64_t* __restrict__ offsets,
-                                                                        const uint32_t* __restrict__ lens,
-                                                                        const uint32_t* __restrict__ perm, uint32_t n,
-                                                                        uint8_t* __restrict__ out, uint32_t out_len) {
-    const LaneSplit ls;
-    if (ls.idle(n)) return;
-    const bool live = ls.live(n);
-    double crow[5];
-    ls.mds_row(crow);
-    const uint32_t len = live ? lens[ls.item] : 0u;
-    const uint32_t i = live ? perm[ls.item] : 0u;
+// k_sponge_digest_varlen: k_sponge_digest over the items sorted by length.  Warp item k is item i = perm[k] with
+// len = lens[k]; every lane carries its own tag, step count and last-chunk width, input chunks go through the warp tile
+// with a per-item base address (shuffled, as in k_mtree_digest), outputs are stored per item.  Rejected items (len 0,
+// sorted to the front) write zero rows.  Warps take the sorted segments from the end, so the longest items start first.
+// 4 resident blocks per SM (128 registers): the per-lane sponge bookkeeping does not fit kMinBlocks' 96 without spills.
+__global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_varlen(const uint8_t* __restrict__ tags,
+                                                                      const uint8_t* __restrict__ in, uint64_t base,
+                                                                      const uint64_t* __restrict__ offsets,
+                                                                      const uint32_t* __restrict__ lens,
+                                                                      const uint32_t* __restrict__ perm, uint32_t n,
+                                                                      uint8_t* __restrict__ out, uint32_t out_len) {
+    __shared__ uint4 stage[kWarps][32][8];
+    P252_STAGE_TABLES
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const uint32_t nseg = (n + 31) / 32;
+    const uint32_t wg = blockIdx.x * kWarps + warp;
+    if (wg >= nseg) return;
+    const uint32_t item0 = (nseg - 1 - wg) * 32;
+    const int nitems = (n - item0 < 32) ? (int)(n - item0) : 32;
+    const bool live = lane < nitems;
+    const uint32_t k = item0 + (live ? lane : 0);
+    const uint32_t len = live ? lens[k] : 0u;
+    const uint32_t i = perm[k];
     const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
     uint8_t* dst = out + (size_t)i * out_len * 32;
+    sponge_varlen_lane<false>(stage[warp], lane, live, tags + (size_t)len * 32, src, dst, len, out_len, false);
+}
+
+// k_sponge_digest_mixed (p252_hash_batch_mixed): the same over the order of k_mixed_keys and the sort (by step count).
+// Warp item k is item i = perm[k]; desc[i] = (len, out_len | truncated << 31), (0, 0) for a rejected item (its zero rows
+// were written by k_mixed_keys), so a lane of a rejected item only idles; tags + 32 i is its tag, row out_offsets[i] -
+// obase of `out` its first output row.
+__global__ void __launch_bounds__(kThreads, 4) k_sponge_digest_mixed(const uint8_t* __restrict__ tags,
+                                                                     const uint2* __restrict__ desc,
+                                                                     const uint8_t* __restrict__ in, uint64_t base,
+                                                                     const uint64_t* __restrict__ offsets, uint64_t obase,
+                                                                     const uint64_t* __restrict__ out_offsets,
+                                                                     const uint32_t* __restrict__ perm, uint32_t n,
+                                                                     uint8_t* __restrict__ out) {
+    __shared__ uint4 stage[kWarps][32][8];
+    P252_STAGE_TABLES
+    const int lane = threadIdx.x & 31;
+    const int warp = threadIdx.x >> 5;
+    const uint32_t nseg = (n + 31) / 32;
+    const uint32_t wg = blockIdx.x * kWarps + warp;
+    if (wg >= nseg) return;
+    const uint32_t item0 = (nseg - 1 - wg) * 32;
+    const int nitems = (n - item0 < 32) ? (int)(n - item0) : 32;
+    const bool live = lane < nitems;
+    const uint32_t i = perm[item0 + (live ? lane : 0)];
+    const uint2 d = live ? desc[i] : make_uint2(0, 0);
+    const uint32_t len = d.x, out_len = d.y & 0x7fffffffu;
+    const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
+    uint8_t* dst = out + (len ? (out_offsets[i] - obase) * 32 : 0);
+    sponge_varlen_lane<true>(stage[warp], lane, false, tags + (size_t)i * 32, src, dst, len, out_len, (d.y >> 31) != 0);
+}
+
+// The lane-split loop of the variable-length digest kernels (five threads per item, hades_permute_coop), shared as
+// sponge_varlen_lane is.  Every thread runs the warp's largest step count (the permutation's shuffles span the warp); a
+// group past its own last step only idles.
+template <bool kMixed>
+__device__ __forceinline__ void sponge_varlen_coop(const LaneSplit& ls, bool live, const double (&crow)[5], const uint8_t* tag,
+                                                   const uint8_t* src, uint8_t* dst, uint32_t len, uint32_t out_len, bool trunc) {
     const uint32_t nin = (len + 3) / 4, nout = (out_len + 3) / 4;
     const uint32_t steps = len ? nin + nout : 0u;
     const uint32_t wsteps = __reduce_max_sync(0xffffffffu, steps);
     uint32_t s[8];
     if (ls.li == 0) {
-        load_fr(s, tags + (size_t)len * 32);
+        load_fr(s, tag);
     } else {
 #pragma unroll
         for (int w = 0; w < 8; ++w) s[w] = 0u;
@@ -1137,9 +1178,58 @@ __global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const ui
             }
         } else if (step < steps) {
             const uint32_t q = 4 * (step - nin) + (uint32_t)ls.li - 1;
-            if (ls.li >= 1 && q < out_len) store_fr(dst + (size_t)q * 32, s);
+            if (ls.li >= 1 && q < out_len) {
+                if (kMixed && trunc) {
+                    uint32_t v[8];
+                    fr_to_canonical(v, s);
+                    v[7] &= 0x03ffffffu;                         // TRUNCATION_MASK, src/hash.rs:167-172
+                    store_fr(dst + (size_t)q * 32, v);
+                } else {
+                    store_fr(dst + (size_t)q * 32, s);
+                }
+            }
         }
     }
+}
+
+// the same for small batches: five threads per item (hades_permute_coop), as k_sponge_digest_coop
+__global__ void __launch_bounds__(kThreads) k_sponge_digest_varlen_coop(const uint8_t* __restrict__ tags,
+                                                                        const uint8_t* __restrict__ in, uint64_t base,
+                                                                        const uint64_t* __restrict__ offsets,
+                                                                        const uint32_t* __restrict__ lens,
+                                                                        const uint32_t* __restrict__ perm, uint32_t n,
+                                                                        uint8_t* __restrict__ out, uint32_t out_len) {
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
+    double crow[5];
+    ls.mds_row(crow);
+    const uint32_t len = live ? lens[ls.item] : 0u;
+    const uint32_t i = live ? perm[ls.item] : 0u;
+    const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
+    uint8_t* dst = out + (size_t)i * out_len * 32;
+    sponge_varlen_coop<false>(ls, live, crow, tags + (size_t)len * 32, src, dst, len, out_len, false);
+}
+
+// k_sponge_digest_mixed for small batches: five threads per item, as k_sponge_digest_varlen_coop
+__global__ void __launch_bounds__(kThreads) k_sponge_digest_mixed_coop(const uint8_t* __restrict__ tags,
+                                                                       const uint2* __restrict__ desc,
+                                                                       const uint8_t* __restrict__ in, uint64_t base,
+                                                                       const uint64_t* __restrict__ offsets, uint64_t obase,
+                                                                       const uint64_t* __restrict__ out_offsets,
+                                                                       const uint32_t* __restrict__ perm, uint32_t n,
+                                                                       uint8_t* __restrict__ out) {
+    const LaneSplit ls;
+    if (ls.idle(n)) return;
+    const bool live = ls.live(n);
+    double crow[5];
+    ls.mds_row(crow);
+    const uint32_t i = live ? perm[ls.item] : 0u;
+    const uint2 d = live ? desc[i] : make_uint2(0, 0);
+    const uint32_t len = d.x, out_len = d.y & 0x7fffffffu;
+    const uint8_t* src = in + (len ? (offsets[i] - base) * 32 : 0);
+    uint8_t* dst = out + (len ? (out_offsets[i] - obase) * 32 : 0);
+    sponge_varlen_coop<true>(ls, false, crow, tags + (size_t)i * 32, src, dst, len, out_len, (d.y >> 31) != 0);
 }
 
 // ---- variable-length encrypt / decrypt batches (p252_encrypt_batch_varlen / p252_decrypt_batch_varlen) ---------------
@@ -3581,6 +3671,71 @@ __global__ void __launch_bounds__(256) k_from_bytes_wide(const uint8_t* __restri
     uint32_t r[8];
     fr_from_bytes_wide(r, w);
     store_fr(out + i * 32, r);
+}
+
+// ---- mixed digest batches (p252_hash_batch_mixed): per-item domain, input and output lengths, truncation --------------
+// k_mixed_keys: one thread per item.  Item i is Hash::new(mode[i] & 3), update(in[offsets[i] - base .. offsets[i+1] - base))
+// (n_scalars scalars), output_len(out_len), finalize() or (mode[i] & 0x80) finalize_truncated(), written to the rows
+// [out_offsets[i] - obase, out_offsets[i+1] - obase) of `out` (n_out rows).  Valid: no mode bit outside 0x83, both ranges
+// non-decreasing and inside their buffers, a Merkle domain with len == arity and out_len == 1, 1 <= len <= max_len and
+// 1 <= out_len <= max_out_len -- the rules of p252_hash_tag.  Every later access of `in` and `out` is bounded by this.
+// A valid item gets key = its step count ceil(len / 4) + ceil(out_len / 4), desc = (len, out_len | truncated << 31) and
+// its tag: hash_to_scalar(BE32(0x80000000 | len) || BE32(out_len) || BE64(domain_sep)), one BLAKE2b block, derived here
+// so that the sponge kernels keep their register budget.  An invalid item gets key 0, desc (0, 0), a zero tag and, when
+// its output range is valid, zero rows; it is counted into *rejected.  vals[i] = i.
+__global__ void __launch_bounds__(256) k_mixed_keys(const uint8_t* __restrict__ mode, const uint64_t* __restrict__ offsets,
+                                                    uint64_t base, uint64_t n_scalars, const uint64_t* __restrict__ out_offsets,
+                                                    uint64_t obase, uint64_t n_out, uint32_t n, uint32_t max_len,
+                                                    uint32_t max_out_len, uint8_t* __restrict__ out, uint32_t* __restrict__ keys,
+                                                    uint32_t* __restrict__ vals, uint8_t* __restrict__ tags,
+                                                    uint2* __restrict__ desc, unsigned long long* __restrict__ rejected) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t m = mode[i], dom = m & 3u;
+    const uint64_t a = offsets[i] - base, b = offsets[i + 1] - base, len = b - a;
+    const uint64_t oa = out_offsets[i] - obase, ob = out_offsets[i + 1] - obase, olen = ob - oa;
+    const bool out_ok = oa <= ob && ob <= n_out;
+    const uint64_t arity = dom == 0 ? 4u : (dom == 1 ? 2u : 0u);   // P252_DOMAIN_MERKLE4, P252_DOMAIN_MERKLE2
+    const bool ok = (m & ~0x83u) == 0 && a <= b && b <= n_scalars && out_ok && (arity == 0 || (len == arity && olen == 1)) &&
+                    len >= 1 && olen >= 1 && len <= max_len && olen <= max_out_len;
+    if (rejected) warp_count(rejected, !ok);
+    uint32_t r[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    if (ok) {
+        // u64::from(Domain), src/hash.rs:43-55
+        const uint64_t dsep = dom == 0 ? 0xfull : (dom == 1 ? 0x3ull : (dom == 2 ? 0x100000000ull : 0ull));
+        const uint32_t w0 = 0x80000000u | (uint32_t)len, w1 = (uint32_t)olen;
+        uint64_t msg[16] = {};
+        msg[0] = ((uint64_t)__byte_perm(w1, 0, 0x0123) << 32) | __byte_perm(w0, 0, 0x0123);   // big-endian words
+        msg[1] = ((uint64_t)__byte_perm((uint32_t)dsep, 0, 0x0123) << 32) | __byte_perm((uint32_t)(dsep >> 32), 0, 0x0123);
+        uint64_t h[8] = {0x6a09e667f3bcc908ull ^ 0x01010040ull, 0xbb67ae8584caa73bull, 0x3c6ef372fe94f82bull,
+                         0xa54ff53a5f1d36f1ull, 0x510e527fade682d1ull, 0x9b05688c2b3e6c1full, 0x1f83d9abfb41bd6bull,
+                         0x5be0cd19137e2179ull};
+        blake2b_compress(h, msg, 16, true);
+        fr_from_bytes_wide(r, h);
+    }
+    store_fr(tags + (size_t)i * 32, r);
+    keys[i] = ok ? (uint32_t)((len + 3) / 4 + (olen + 3) / 4) : 0u;
+    vals[i] = i;
+    desc[i] = ok ? make_uint2((uint32_t)len, (uint32_t)olen | (m & 0x80u) << 24) : make_uint2(0, 0);
+    if (!ok && out_ok)                                     // rejected: zero rows
+        for (uint64_t q = oa; q < ob; ++q) store_fr(out + q * 32, r);
+}
+
+cudaError_t launch_mixed_keys(const uint8_t* mode, const uint64_t* offsets, uint64_t base, uint64_t n_scalars,
+                              const uint64_t* out_offsets, uint64_t obase, uint64_t n_out, uint32_t n, uint32_t max_len,
+                              uint32_t max_out_len, void* out, uint32_t* keys, uint32_t* vals, void* tags, uint2* desc,
+                              unsigned long long* rejected, cudaStream_t st) {
+    return launch(k_mixed_keys, n, 256, st, mode, offsets, base, n_scalars, out_offsets, obase, n_out, n, max_len, max_out_len,
+                  out, keys, vals, tags, desc, rejected);
+}
+
+cudaError_t launch_digest_mixed(const void* tags, const uint2* desc, const void* in, uint64_t base, const uint64_t* offsets,
+                                uint64_t obase, const uint64_t* out_offsets, const uint32_t* perm, uint32_t n, void* out,
+                                size_t coop_max, cudaStream_t st) {
+    if (n <= coop_max)
+        return launch_grid(k_sponge_digest_mixed_coop, coop_grid(n), kThreads, st, tags, desc, in, base, offsets, obase,
+                           out_offsets, perm, n, out);
+    return launch(k_sponge_digest_mixed, n, kThreads, st, tags, desc, in, base, offsets, obase, out_offsets, perm, n, out);
 }
 
 cudaError_t launch_hash_to_scalar(const void* bytes, uint64_t base, uint64_t n_bytes, const uint64_t* offsets,

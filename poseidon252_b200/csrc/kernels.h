@@ -343,6 +343,21 @@ cudaError_t launch_hash_to_scalar_keys(const uint64_t* offsets, uint32_t n, uint
                                        uint32_t* keys, uint32_t* vals, unsigned long long* rejected, cudaStream_t st);
 // BlsScalar::from_bytes_wide (p252_scalars_from_bytes_wide): n rows of 64 bytes -> n scalars (Montgomery)
 cudaError_t launch_from_bytes_wide(const void* in, size_t n, void* out, cudaStream_t st);
+// Mixed digest batches (p252_hash_batch_mixed): item i = Hash::new(mode[i] & 3), in[offsets[i] - base .. offsets[i+1] -
+// base) of n_scalars, finalize() or (mode[i] & 0x80) finalize_truncated() into the rows [out_offsets[i] - obase,
+// out_offsets[i+1] - obase) of out (n_out rows).  keys: the step count ceil(len / 4) + ceil(out_len / 4) of a valid item
+// (the rules of p252_hash_tag plus len <= max_len, out_len <= max_out_len and no mode bit outside 0x83), 0 for an invalid
+// one (counted into *rejected; zero rows where its output range is valid); vals[i] = i; tags (n rows) and desc (n) the
+// item's tag, derived on the device, and (len, out_len | truncated << 31), (0, 0) for an invalid item
+cudaError_t launch_mixed_keys(const uint8_t* mode, const uint64_t* offsets, uint64_t base, uint64_t n_scalars,
+                              const uint64_t* out_offsets, uint64_t obase, uint64_t n_out, uint32_t n, uint32_t max_len,
+                              uint32_t max_out_len, void* out, uint32_t* keys, uint32_t* vals, void* tags, uint2* desc,
+                              unsigned long long* rejected, cudaStream_t st);
+// over the keys sorted ascending with their values (perm): the digests of the valid items; lane-split kernel when
+// n <= coop_max
+cudaError_t launch_digest_mixed(const void* tags, const uint2* desc, const void* in, uint64_t base, const uint64_t* offsets,
+                                uint64_t obase, const uint64_t* out_offsets, const uint32_t* perm, uint32_t n, void* out,
+                                size_t coop_max, cudaStream_t st);
 void kernel_launch_shape(int* threads_per_block, int* min_blocks_per_sm);
 size_t coop_max_items(int sm_count);   // default small-batch threshold (P252_COOP_MAX or derived from the SM count)
 // 32x32->64-bit multiply instructions (IMAD.WIDE / IMAD.HI class) and DFMA per Hades permutation, counted from

@@ -287,6 +287,48 @@ class Engine:
         """Items of the last hash_batch_varlen skipped as invalid (device buffers; sync() first after async_)."""
         return self._last("varlen_rejected")
 
+    def hash_batch_mixed(self, mode, data, offsets, out_offsets, max_len=None, max_out_len=None, out=None, async_=False):
+        """Every Hash the reference can build, in one call: item i is Hash::new(mode[i] & 3), update(data[offsets[i]:
+        offsets[i+1]]), output_len(out_offsets[i+1] - out_offsets[i]), then finalize(), or finalize_truncated() where
+        mode[i] & MIXED_TRUNCATED (raw limbs masked to 250 bits).  mode (n,) uint8, data (n_scalars, 4), offsets and
+        out_offsets (n + 1,) live in one memory space (numpy, or CUDA tensors on one device); offsets[0] and out_offsets[0]
+        need not be 0.  Returns (n_out, 4) with n_out = out_offsets[-1]: item i's rows are out[out_offsets[i]:
+        out_offsets[i+1]]; a caller's `out` of (n_out, 4) may hold more rows.  max_len / max_out_len bound the input /
+        output lengths (at most VARLEN_MAX_LEN); None takes the longest item, which for CUDA tensors costs a
+        device-to-host sync.  Host batches raise for the lowest-index
+        invalid item and write nothing; device batches give invalid items zero rows and count them
+        (last_mixed_rejected())."""
+        dp, dlead, flags, dk = self._in(data, (4,))
+        op, n1, ok_ = self._idx(offsets, dk, "offsets")
+        oop, no1, ook = self._idx(out_offsets, dk, "out_offsets")
+        if n1 < 1 or no1 != n1:
+            raise EngineError(-1, "offsets and out_offsets must both have n + 1 >= 1 entries")
+        n = n1 - 1
+        mp, mk = self._bytes(mode, dk, "mode", n)
+        if max_len is None:
+            max_len = self._longest_item(ok_, n)
+        if max_out_len is None:
+            max_out_len = self._longest_item(ook, n)
+        if out is None:
+            if _is_torch(ook):
+                import torch
+                n_out = int(ook.view(torch.int64)[-1].item())
+            else:
+                n_out = int(ook[-1])
+            res = self._rows_like(dk, n_out)
+        else:
+            n_out = int(out.shape[0]) if getattr(out, "ndim", 0) == 2 else -1
+            res = self._check_out(out, (n_out, 4), dk)
+        flags = self._flags(flags, async_)
+        rejected = self._counter("mixed_rejected", flags)
+        self._check(self._lib.p252_hash_batch_mixed(self._ctx, mp, dp, int(dlead[0]), op, n, int(max_len), self._ptr(res),
+                                                    n_out, oop, int(max_out_len), ctypes.byref(rejected), flags))
+        return res
+
+    def last_mixed_rejected(self):
+        """Items of the last hash_batch_mixed skipped as invalid (device buffers; sync() first after async_)."""
+        return self._last("mixed_rejected")
+
     def scalars_from_bytes(self, data, async_=False):
         """(n, 32) uint8 canonical little-endian (host) or (n, 4) 64-bit device tensor of the same bytes
         -> (scalars (n, 4), ok (n,) uint8); ok == 0 where the value is >= p."""

@@ -1,7 +1,8 @@
 """`Hash` / `Domain` -- host-side mirror of src/hash.rs over the GPU engine.
 
 Same names, argument meaning and error behaviour as the reference; every digest is computed by the
-CUDA sponge kernel (a single `Hash::digest` is a batch of one).  New: `Hash.digest_batch`."""
+CUDA sponge kernel (a single `Hash::digest` is a batch of one).  New: `Hash.digest_batch` and the other batch entries
+below; `Hash.finalize_batch` / `Hash.digest_batch_mixed` take items of any domains, lengths and truncation in one call."""
 import ctypes
 import enum
 
@@ -147,6 +148,50 @@ class Hash:
         return eng.hash_batch_truncated(self.domain, self.input[0].reshape(1, -1, 4), self._output_len)[0]
 
     @staticmethod
+    def finalize_batch(hashes, truncated=False, engine=None):
+        """NEW batch entry: [h.finalize() or h.finalize_truncated() for h in hashes] in one device call
+        (Engine.hash_batch_mixed), whatever their domains, update() chunks and output lengths (inputs and outputs of up to
+        VARLEN_MAX_LEN scalars each).  truncated: one bool for all, or one per hash.  Raises what Hash.finalize would raise for the lowest-index invalid hash (a Merkle arity
+        violation, no input or a zero-length update() chunk) before any engine is touched.  engine: None takes the first
+        hash's engine, then the default one."""
+        from .errors import InvalidIOPattern
+        hashes = list(hashes)
+        if isinstance(truncated, (bool, np.bool_)):
+            truncated = [truncated] * len(hashes)
+        trunc = [bool(t) for t in truncated]
+        if len(trunc) != len(hashes):
+            raise ValueError("truncated must be one bool or one per hash")
+        for h in hashes:
+            lens = [int(c.shape[0]) for c in h.input]
+            io_pattern(h.domain, lens, h._output_len)
+            if not lens or 0 in lens:
+                raise InvalidIOPattern()
+        if not hashes:
+            return []
+        mode = np.array([int(h.domain) | (_native.MIXED_TRUNCATED if t else 0) for h, t in zip(hashes, trunc)],
+                        dtype=np.uint8)
+        lens = np.array([sum(int(c.shape[0]) for c in h.input) for h in hashes], dtype=np.uint64)
+        out_lens = np.array([h._output_len for h in hashes], dtype=np.uint64)
+        offsets = np.zeros(len(hashes) + 1, dtype=np.uint64)
+        out_offsets = np.zeros(len(hashes) + 1, dtype=np.uint64)
+        np.cumsum(lens, out=offsets[1:])
+        np.cumsum(out_lens, out=out_offsets[1:])
+        data = np.concatenate([c for h in hashes for c in h.input], axis=0)
+        eng = _engine_for(engine if engine is not None else hashes[0]._engine)
+        out = eng.hash_batch_mixed(mode, data, offsets, out_offsets, int(lens.max()), int(out_lens.max()))
+        return [out[out_offsets[i]:out_offsets[i + 1]] for i in range(len(hashes))]
+
+    @staticmethod
+    def digest_batch_mixed(mode, data, offsets, out_offsets, engine=None, max_len=None, max_out_len=None, out=None,
+                           async_=False):
+        """NEW batch entry: Engine.hash_batch_mixed over CSR arrays (numpy, or CUDA tensors): item i is
+        Hash::new(mode[i] & 3) over data[offsets[i]:offsets[i+1]] with out_offsets[i+1] - out_offsets[i] outputs, truncated where mode[i] &
+        MIXED_TRUNCATED.  Output lengths are taken as given, for every domain.  Returns the (n_out, 4) output rows."""
+        eng = _engine_for(engine, data)
+        return eng.hash_batch_mixed(mode, data, offsets, out_offsets, max_len=max_len, max_out_len=max_out_len, out=out,
+                                    async_=async_)
+
+    @staticmethod
     def digest(domain, data, engine=None):
         """src/hash.rs:191-195"""
         h = Hash(domain, engine)
@@ -192,3 +237,7 @@ class Hash:
         ol = int(output_len) if (domain == Domain.Other and output_len > 0) else 1
         eng = _engine_for(engine, inputs)
         return eng.hash_batch(domain, inputs, ol, out=out, async_=async_)
+
+
+finalize_batch = Hash.finalize_batch
+digest_batch_mixed = Hash.digest_batch_mixed
